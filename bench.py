@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Benchmark of the NPHM hot path on B200 (contract: see the task statement / DESIGN.md section "Measurement").
+"""Benchmark of the NPHM hot path on H100 (see DESIGN.md section "Measurement").
 
 N = 1 (BASELINE.json configs[1]): a step = SDF of the 40-member ensemble on the 256^3 grid + marching cubes of one head.
   value   SDF query points/s, inputs (latent, weights) resident in HBM, grid generated in-kernel
   e2e     the same through the reference-facing drop-in API with HOST buffers: pinned latent -> H2D,
           get_logits(...) -> numpy volume (D2H), mesh_from_logits(numpy) -> mesh (H2D volume, D2H mesh)
-  stock_gpu   the UNMODIFIED reference modules (.cuda(), its own get_logits, 672 chunks) on the same B200, full volume;
+  stock_gpu   the UNMODIFIED reference modules (.cuda(), its own get_logits, 672 chunks) on the same GPU, full volume;
           the volume it returns is also compared with ours (parity on all 16.7 M points)
   cpu_baseline  the UNMODIFIED reference modules on the host cores, bounded sample (+ C marching cubes on the step's volume)
 N > 1 (BASELINE.json configs[4]): a step = ONE head on the 512^3 grid, x-slabs sharded over the N ranks
@@ -17,6 +17,7 @@ N > 1 (BASELINE.json configs[4]): a step = ONE head on the 512^3 grid, x-slabs s
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference        # CPU arm: the reference's own modules (oracle/_ref) on the host cores
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR     # + what the last timed step computed, as .npy
 """
 import argparse
 import json
@@ -49,7 +50,33 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-stock-gpu', action='store_true')
     ap.add_argument('--cpu-sample-chunks', type=int, default=2)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last one computed to DIR/<name>.npy (N = 1 only)')
     return ap.parse_args()
+
+
+DUMP_SEED = 1234
+DUMP_VOLUME_SAMPLES = 1 << 20            # 4 MB of the 64 MB volume
+DUMP_MESH_ROWS = 1 << 19                 # per mesh array (vertices, triangles), 12 MB each as float64
+
+
+def dump_outputs(out_dir, volume, verts, tris):
+    """The arrays a caller of the timed path receives - the SDF volume of query_grid and the mesh of marching_cubes_device -
+    as float32 / float64 .npy files (< 64 MB together): a fixed, seeded sample of the volume and of larger meshes, the
+    full arrays where they are small.  Triangle ids are integers below 2^53, exact in float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.RandomState(DUMP_SEED)
+    vol = volume.detach().cpu().numpy().astype(np.float32).reshape(-1)
+    idx = np.sort(rng.choice(vol.size, size=min(DUMP_VOLUME_SAMPLES, vol.size), replace=False))
+    np.save(os.path.join(out_dir, 'sdf_volume_sample.npy'), vol[idx])
+    np.save(os.path.join(out_dir, 'sdf_volume_sample_index.npy'), idx.astype(np.float64))
+    v = verts.detach().cpu().numpy().astype(np.float64)
+    t = tris.detach().cpu().numpy().astype(np.float64)
+    np.save(os.path.join(out_dir, 'mesh_counts.npy'), np.array([len(v), len(t)], dtype=np.float64))
+    for name, a in (('mesh_vertices', v), ('mesh_triangles', t)):
+        if len(a) > DUMP_MESH_ROWS:
+            a = a[np.sort(rng.choice(len(a), size=DUMP_MESH_ROWS, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
 
 
 def workload_name(res, world):
@@ -272,7 +299,7 @@ def roofline_block(res_key, flops, sdf_ms, note_extra=''):
     peak_tf = peaks.get('bf16_tflops_sustained', None)
     peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)'
     if peak_tf is None:
-        peak_tf, peak_src = 1590.0, 'fallback (B200_PROFILING.md)'
+        peak_tf, peak_src = 989.0, 'H100 SXM data sheet, dense BF16/FP16 (not a measured rate)'
     achieved_tf = flops / (sdf_ms * 1e-3) / 1e12
     traffic, traffic_src = None, 'no ncu capture recorded for this resolution'
     try:
@@ -303,7 +330,7 @@ def run_single(args, torch, dev):
     eng = dec.engine()
     lat = sample_latent(1).to(dev)
     volume = torch.empty(total, device=dev, dtype=torch.float32)
-    flush = torch.empty(64 * 1024 * 1024, device=dev, dtype=torch.float32)      # 256 MB > 126 MB L2
+    flush = torch.empty(64 * 1024 * 1024, device=dev, dtype=torch.float32)      # 256 MB > 50 MB L2
     launches = {'n': 0}
     per_step_launches = _native.launches_per_grid_query(args.impl) + _native.MC_LAUNCHES
 
@@ -331,6 +358,7 @@ def run_single(args, torch, dev):
     kev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(args.steps)]
     ev[0].record()
     n_tris = 0
+    last = None
     for i in range(args.steps):
         kev[i][0].record()
         eng.query_grid(lat, MINI, MAXI, res, 0, total, quirk_period=CHUNK, out=volume)
@@ -339,6 +367,8 @@ def run_single(args, torch, dev):
         kev[i][2].record()
         launches['n'] += per_step_launches
         n_tris = t.shape[0]
+        if i == args.steps - 1 and args.dump_outputs:
+            last = (v, t)
         del v, t                        # the mesh buffers go back to torch's caching allocator (no cudaMalloc in the loop)
         flush.zero_()                   # L2 flush between timed iterations (inside the timed region)
         kev[i][3].record()
@@ -351,6 +381,9 @@ def run_single(args, torch, dev):
     flush_ms = float(np.mean([k[2].elapsed_time(k[3]) for k in kev]))
     ms_per_step = ms_total / args.steps
     value = total / (ms_per_step * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, volume, *last)
+        del last
 
     # ---- opt-in pruned kernel (reported separately; NOT the dense reference computation) ---------------------
     pruned = None
@@ -417,7 +450,7 @@ def run_single(args, torch, dev):
     if pruned is not None:
         line['pruned_opt_in'] = pruned
 
-    # ---- the reference itself: stock GPU path on this B200 (+ parity on the whole volume), CPU sample -----------
+    # ---- the reference itself: stock GPU path on the same GPU (+ parity on the whole volume), CPU sample -----------
     ours = volume.cpu().numpy()
     if not args.no_stock_gpu:
         try:
@@ -610,6 +643,10 @@ def main():
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
     os.environ['NPHM_B200_IMPL'] = args.impl
+    if args.dump_outputs and world > 1:
+        raise SystemExit('--dump-outputs is implemented for --gpus 1')
+    if args.steps < 1:
+        raise SystemExit('--steps must be at least 1 (the timed steps are what is measured and dumped)')
     if world > 1:
         dist.init_process_group('nccl', device_id=dev)
         try:

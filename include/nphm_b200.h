@@ -1,4 +1,4 @@
-/* nphm_b200.h - C ABI of libnphm_b200.so, the B200-native engine behind NPHM's hot path.
+/* nphm_b200.h - C ABI of libnphm_b200.so, the H100 (sm_90a) engine behind NPHM's hot path.
  *
  * The reference (SimonGiebenhain/NPHM) has no FFI layer: its hot path sits behind Python call signatures
  * (SURVEY.md 8b).  This header is the boundary a binding would target; the Python mirror of the reference
@@ -27,10 +27,10 @@ extern "C" {
 #define NPHM_ERR_CAPACITY    -4   /* caller-provided buffer too small */
 
 /* kernel selection for the network queries */
-#define NPHM_IMPL_AUTO   0   /* tcgen05 kernel when the configuration allows it, else SIMT */
+#define NPHM_IMPL_AUTO   0   /* tensor-core kernel when the configuration allows it, else SIMT */
 #define NPHM_IMPL_SIMT   1   /* fp32 FFMA kernel (any configuration) */
-#define NPHM_IMPL_TC     2   /* tcgen05 / TMEM kernel, 3-pass fp16 split (fp32-equivalent accuracy) */
-#define NPHM_IMPL_TC_PRUNED 3 /* OPT-IN: tcgen05 kernel that skips, per compact tile of 128 points, the ensemble members whose
+#define NPHM_IMPL_TC     2   /* tensor-core (wgmma) kernel, 3-pass fp16 split (fp32-equivalent accuracy) */
+#define NPHM_IMPL_TC_PRUNED 3 /* OPT-IN: tensor-core kernel that skips, per compact tile of 128 points, the ensemble members whose
                                 normalised Gaussian blend weight is < tau for every point of the tile.  Not the dense
                                 reference computation: |error| <= n_members * tau * max_k |s_k| (tau default 1e-8). */
 
@@ -114,7 +114,7 @@ void nphm_mlp_destroy(nphm_mlp *h);
 /* w_dev[l]: (out_l, in_l) row-major, b_dev[l]: (out_l), l = 0..n_layers (keys lin{l}.weight/bias). */
 int nphm_mlp_load_weights(nphm_mlp *h, const float *const *w_dev, const float *const *b_dev, void *stream);
 /* xyz_dev n_queries*n_points*3, cond_dev n_queries*lat_dim -> out_dev n_queries*n_points*out_dim.
- * impl: NPHM_IMPL_AUTO picks the tcgen05 kernel for the deformation-backbone configuration (hidden 512, 6 hidden layers,
+ * impl: NPHM_IMPL_AUTO picks the tensor-core path for the deformation-backbone configuration (hidden 512, 6 hidden layers,
  * condition 232, 3 outputs) and the fp32 FFMA kernel otherwise; NPHM_IMPL_SIMT / NPHM_IMPL_TC force one. */
 int nphm_mlp_query(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries,
                    long long n_points, float *out_dev, int impl, void *stream);
@@ -207,7 +207,7 @@ int nphm_fit_surface_grad(nphm_ensemble *h, const float *points_dev, long long n
                           float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
- * DeepSDF-style stacks layer by layer on the generic fp32-accurate tcgen05 linear layer (csrc/tc_linear.cu, mlp_chain.cu).
+ * DeepSDF-style stacks layer by layer on the generic fp32-accurate wgmma linear layer (csrc/tc_linear.cu, mlp_chain.cu).
  * ---------------------------------------------------------------------------------------------- */
 /* == nphm_mlp_query for ANY width (DeepSDF.forward, reference src/NPHM/models/deepSDF.py:64-89; e.g. the NPM baseline
  * 515 -> 1024 x 8 of scripts/configs/npm.yaml:2-4, which no fused kernel takes). */

@@ -1,4 +1,4 @@
-"""nphm_b200 - B200-native engine for the hot path of NPHM (Neural Parametric Head Models).
+"""nphm_b200 - H100 (sm_90a) engine for the hot path of NPHM (Neural Parametric Head Models).
 
 The sub-packages mirror the reference's module layout (``NPHM.models.*``, ``NPHM.utils.*``) so that the
 reference's ``scripts/fitting`` and ``scripts/training`` run unchanged on top of this engine after

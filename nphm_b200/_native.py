@@ -18,7 +18,7 @@ import torch
 IMPL_AUTO, IMPL_SIMT, IMPL_TC, IMPL_TC_PRUNED = 0, 1, 2, 3
 _IMPL_BY_NAME = {'auto': IMPL_AUTO, 'simt': IMPL_SIMT, 'tc': IMPL_TC, 'tc_pruned': IMPL_TC_PRUNED}
 
-# NPHM_B200_LIB: developer override used for A/B runs of kernel variants (tools/ab_bench.sh); default = the in-tree build
+# NPHM_B200_LIB: developer override to load another build of the library (A/B runs of kernel variants); default = the in-tree build
 _LIB_PATH = os.environ.get('NPHM_B200_LIB') or os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libnphm_b200.so')
 _lib = None
 
@@ -348,8 +348,8 @@ class MlpEngine(_Versioned):
         cfg = MlpConfig(module.lat_dim, hidden, self.n_lin - 1, module.out_dim_net)
         check(lib().nphm_mlp_create(byref(cfg), byref(self._h)), 'nphm_mlp_create')
         self.out_dim = module.out_dim_net
-        # which kernel family AUTO picks (mirrors tc_mlp_supported in csrc/tc_mlp.cu): the fully fused tcgen05 kernel takes the
-        # forward-deformation backbone only; every other shape runs layer by layer on the generic tcgen05 linear layer
+        # which kernel family AUTO picks (mirrors tc_mlp_supported in csrc/mlp_chain.cu): nphm_mlp_query sends the
+        # forward-deformation backbone to the tensor cores; every other shape runs layer by layer on the generic wgmma linear layer
         # (csrc/tc_linear.cu, any width - e.g. the NPM baseline 515 -> 1024 x 8); the fp32 FFMA kernel is kept for impl='simt'
         self.fused_shape = (hidden == 512 and self.n_lin == 7 and module.lat_dim == 232 and module.out_dim_net == 3)
         self.simt_ok = hidden <= 880
@@ -396,7 +396,7 @@ class MlpEngine(_Versioned):
         return out
 
     def query_layers(self, xyz: torch.Tensor, cond: torch.Tensor) -> torch.Tensor:
-        """Forward, layer by layer on the generic tcgen05 linear layer (any width): xyz B x N x 3, cond B x lat_dim."""
+        """Forward, layer by layer on the generic wgmma linear layer (any width): xyz B x N x 3, cond B x lat_dim."""
         B, N, _ = xyz.shape
         dev = xyz.device
         xyz = _f32c(xyz)

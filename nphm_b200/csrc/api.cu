@@ -20,9 +20,9 @@ int sm_count()
 {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev < 64 && cached[dev]) return cached[dev];
-    int n = 148;
+    int n = 132;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     if (dev < 64) cached[dev] = n;
     return n;
@@ -222,7 +222,7 @@ static int pick_impl(nphm_ensemble *h, int impl, bool *use_tc)
     h->tc_prune = impl == NPHM_IMPL_TC_PRUNED;
     if (impl == NPHM_IMPL_TC_PRUNED) impl = NPHM_IMPL_TC;
     if (impl == NPHM_IMPL_TC && !tc_ok) {
-        set_error("tcgen05 ensemble kernel does not support this configuration");
+        set_error("tensor-core ensemble kernel does not support this configuration");
         return NPHM_ERR_UNSUPPORTED;
     }
     *use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && tc_ok);
@@ -329,8 +329,6 @@ extern "C" int nphm_mlp_load_weights(nphm_mlp *h, const float *const *w_dev, con
     int rc = h->weights.load(h->dims, 1, w_dev, b_dev, static_cast<cudaStream_t>(stream_));
     if (rc) return rc;
     fill_descriptors(h->dims, h->weights, 1, 0, h->cfg.lat_dim, 0, 0, h->net, h->spec);
-    rc = tc_mlp_pack(h, static_cast<cudaStream_t>(stream_));
-    if (rc) return rc;
     if (h->dims.skip >= 1 && h->dims.skip < h->dims.n_lin - 1) {       // stacks the layer chain can run (mlp_chain.cu)
         rc = chain_pack(h, static_cast<cudaStream_t>(stream_));
         if (rc) return rc;
@@ -352,8 +350,8 @@ int mlp_prepare(nphm_mlp *h, const float *cond_dev, int n_queries, cudaStream_t 
 int mlp_run(nphm_mlp *h, const float *xyz_dev, int n_queries, long long n_points, float *out_dev, int impl, cudaStream_t stream)
 {
     if (n_points == 0) return NPHM_OK;
-    const bool use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && tc_mlp_supported(h) && h->tc_ready);
-    if (use_tc) return tc_mlp_launch(h, xyz_dev, h->cvec.as<float>(), n_queries, n_points, out_dev, stream);
+    const bool use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && tc_mlp_supported(h));
+    if (use_tc) return chain_forward(h, xyz_dev, n_queries, n_points, out_dev, stream);
     SimtQuery q{};
     q.xyz = xyz_dev; q.total = n_points; q.n_points = n_points; q.n_queries = n_queries; q.quirk_period = 0;
     q.cvec = h->cvec.as<float>(); q.anchors = nullptr; q.blend = 0; q.out = out_dev;
@@ -369,9 +367,9 @@ extern "C" int nphm_mlp_query(nphm_mlp *h, const float *xyz_dev, const float *co
     NPHM_REQUIRE(n_queries >= 1 && n_points >= 0, "nphm_mlp_query: bad sizes");
     NPHM_REQUIRE(cond_dev && (n_points == 0 || (xyz_dev && out_dev)), "nphm_mlp_query: NULL pointer");
     NPHM_REQUIRE(impl == NPHM_IMPL_AUTO || impl == NPHM_IMPL_SIMT || impl == NPHM_IMPL_TC, "nphm_mlp_query: unknown impl %d", impl);
-    const bool tc_ok = tc_mlp_supported(h) && h->tc_ready;
+    const bool tc_ok = tc_mlp_supported(h);
     if (impl == NPHM_IMPL_TC && !tc_ok) {
-        set_error("tcgen05 MLP kernel supports only the deformation backbone (hidden 512, 6 layers, condition 232, 3 outputs)");
+        set_error("tensor-core MLP path supports only the deformation backbone (hidden 512, 6 layers, condition 232, 3 outputs)");
         return NPHM_ERR_UNSUPPORTED;
     }
     const bool use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && tc_ok);

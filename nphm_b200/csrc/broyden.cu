@@ -159,7 +159,6 @@ extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n
     if ((rc = mlp_prepare(h, cond_dev, n_queries, stream))) return rc;
     const unsigned blocks = (unsigned)ceil_div(n, 256);
     if ((rc = mlp_run(h, s.x, n_queries, n_points, s.f, NPHM_IMPL_AUTO, stream))) return rc;
-    h->tc_records_fresh = true;          // same condition for every evaluation of the loop
     broyden::init_kernel<<<blocks, 256, 0, stream>>>(s, obs_dev, n);
     NPHM_CUDA_CHECK(cudaGetLastError());
     int done = 0;
@@ -168,10 +167,12 @@ extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n
         NPHM_CUDA_CHECK(cudaGetLastError());
         // once nobody is active (counter of the previous step == 0) the network evaluation returns at once: a device-side
         // early exit that needs no host synchronisation (the reference leaves its loop at that point)
-        h->tc_live = step > 0 ? counters + (step - 1) : nullptr;
+        // once nobody is active (counter of the previous step == 0) the network evaluation returns at once: a device-side
+        // early exit that needs no host synchronisation (the reference leaves its loop at that point)
+        h->live = step > 0 ? counters + (step - 1) : nullptr;
         rc = mlp_run(h, s.x, n_queries, n_points, s.f, NPHM_IMPL_AUTO, stream);
-        h->tc_live = nullptr;
-        if (rc) { h->tc_records_fresh = false; return rc; }
+        h->live = nullptr;
+        if (rc) return rc;
         s.n_active = counters + step;
         broyden::update_kernel<<<blocks, 256, 0, stream>>>(s, obs_dev, n, cvg_thresh, dvg_thresh, eps);
         NPHM_CUDA_CHECK(cudaGetLastError());
@@ -186,7 +187,6 @@ extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n
             if (alive == 0) break;
         }
     }
-    h->tc_records_fresh = false;
     broyden::finish_kernel<<<blocks, 256, 0, stream>>>(s, n, cvg_thresh, diff_dev, valid_dev);
     NPHM_CUDA_CHECK(cudaGetLastError());
     if (steps_done) *steps_done = done;

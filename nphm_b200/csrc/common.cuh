@@ -1,4 +1,4 @@
-// Shared host/device helpers for libnphm_b200.so (sm_100a only).
+// Shared host/device helpers for libnphm_b200.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

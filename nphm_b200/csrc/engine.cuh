@@ -68,12 +68,7 @@ struct nphm_mlp {
     nphm::FoldedNet net;
     nphm::PackSpec spec;
     nphm::DeviceBuffer cvec;
-    // tensor-core path (tc_mlp.cu)
-    nphm::DeviceBuffer tc_weights, tc_consts, tc_coff;
-    bool tc_ready = false;
-    const int *tc_live = nullptr;   // set around a launch by the Broyden loop: device counter, 0 = skip the evaluation
-    bool tc_records_fresh = false;  // set by the Broyden loop after its first evaluation: the per-query records of the tensor-core
-                                    // kernel are still those of this condition, do not rebuild them
+    const int *live = nullptr;      // set around an evaluation by the Broyden loop: device counter, 0 = skip the evaluation
     // layer-by-layer tensor-core passes: any width, Jacobian, adjoint (mlp_chain.cu)
     nphm::MlpChain *chain = nullptr;
 };
@@ -84,11 +79,9 @@ int ensemble_prepare(nphm_ensemble *h, const float *latents_dev, int n_queries, 
 bool tc_ensemble_supported(const nphm_ensemble *h);
 int tc_ensemble_pack(nphm_ensemble *h, cudaStream_t stream);
 int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream);
-// tensor-core MLP kernel (tc_mlp.cu): deformation backbone configuration only
+// tensor-core MLP forward (mlp_chain.cu, layer by layer): the deformation backbone is the configuration AUTO sends there
 bool tc_mlp_supported(const nphm_mlp *h);
-int tc_mlp_pack(nphm_mlp *h, cudaStream_t stream);
-int tc_mlp_launch(nphm_mlp *h, const float *xyz, const float *cvec, int n_queries, long long n_points, float *out,
-                  cudaStream_t stream);
+int chain_forward(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, cudaStream_t stream);
 // fitting (fit.cu)
 void fit_packs_destroy(nphm_ensemble *h);
 // layer chain (mlp_chain.cu)

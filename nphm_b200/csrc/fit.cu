@@ -15,8 +15,8 @@
 //   fit_member_kernel<bwd>  (configurations without the tensor-core path) forward again with all activations resident in
 //                           shared memory (199 KB), backward in place, per-member delta sums and blend-path anchor
 //                           gradients -> atomics
-//   tensor-core path        forward = tc::ensemble_tc_kernel_v8<.., ACTS> (member outputs + activation derivatives to global
-//                           memory), backward = three batched tcgen05 GEMMs (tc_linear.cu) between fit_upstream_kernel and
+//   tensor-core path        forward = tc::wg::ensemble_wgmma_kernel<.., ACTS> (member outputs + activation derivatives to global
+//                           memory), backward = three batched wgmma GEMMs (tc_linear.cu) between fit_upstream_kernel and
 //                           fit_reduce_kernel
 //   fit_member_grad_kernel  per member: delta sums -> g_u, g_c -> latent / anchor gradients
 //   fit_finalize_kernel     mlp_pos forward/backward, regularisers, loss terms, Adam
@@ -215,8 +215,8 @@ __global__ void __launch_bounds__(kThreads, 1) fit_member_kernel(const Dims d, c
 
 // ---------------------------------------------------------------------------------------------------------------
 // ---------------------------------------------------------------------------------------------------------------------
-// Backward pass of the tensor-core path, layer by layer on tcgen05 (tc_linear.cu, batched over the members):
-//   the forward (tc::ensemble_tc_kernel_v8<.., ACTS>) leaves sigma'_l = d softplus / d pre-activation of every hidden unit, a block
+// Backward pass of the tensor-core path, layer by layer on wgmma (tc_linear.cu, batched over the members):
+//   the forward (tc::wg::ensemble_wgmma_kernel<.., ACTS>) leaves sigma'_l = d softplus / d pre-activation of every hidden unit, a block
 //   of tc::kActLd features x 128 points per (member, 128-point tile);
 //   fit_upstream_kernel   g_s[m][p] = dL/d s_m(p) (blend + loss), blend-weight gradients w.r.t. anchors and points
 //   3 batched GEMMs       delta2 = sigma'2 * (sigma'3 (diag(w4) W3));  delta1 = sigma'1 * (delta2 W2[:, :N1]) / sqrt2;

@@ -1,4 +1,4 @@
-// Marching cubes over an SDF slab on sm_100a, bit-exact (triangle ids, vertex order, double-precision vertex
+// Marching cubes over an SDF slab on sm_90a, bit-exact (triangle ids, vertex order, double-precision vertex
 // positions) with the sequential PyMCubes algorithm restated in oracle/mc_oracle.c.
 //
 // Reference call site: src/NPHM/utils/reconstruction.py:30  mcubes.marching_cubes(logits, 0.0)

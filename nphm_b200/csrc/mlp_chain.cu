@@ -1,4 +1,4 @@
-// Layer-by-layer passes of a DeepSDF-style stack on the generic tcgen05 linear layer (tc_linear.cu):
+// Layer-by-layer passes of a DeepSDF-style stack on the generic wgmma linear layer (tc_linear.cu):
 //
 //   value pass     h_l = softplus(W_l in_l + c_l), s_l = softplus'(.)          (any width: the NPM baseline 515 -> 1024 x 8 ...)
 //   tangent pass   forward-mode derivative w.r.t. xyz:  t_l = s_l * (W_l t_{l-1}),  3 rows per point  ->  Jacobian d out / d xyz
@@ -144,6 +144,7 @@ struct MlpChain {
     // activations between the layers live in the packed operand format (Hp: values, Tp: tangents, Dp: adjoints), the
     // activation derivatives S in the blocked fp32 layout ([128-row tile][feature][128]) - every access of the passes is coalesced
     DeviceBuffer Hp[kMaxLayers], S[kMaxLayers], Tp[2], Dp[2], Tlast, sums0, sumss, out_tmp, xtmp;
+    DeviceBuffer Fp[2];                       // ping-pong activations of the forward-only pass (forward_pass)
     int ld[kMaxLayers];
     long long value_rows = 0;                 // rows of the last value pass that kept the activation derivatives
     bool have_deriv = false;
@@ -227,6 +228,54 @@ static int value_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_
     return NPHM_OK;
 }
 
+// Forward only (no derivatives kept), in chunks of at most kForwardChunkRows rows through two ping-pong operand buffers: the
+// memory it needs is bounded by the chunk (2 x 128 MB for the deformation backbone), not by the number of points, so a whole
+// 256^3 grid can be queried in one call.  Chunks hold whole queries, or a run of rows of one query.  `live` (optional device
+// counter): every launch returns at once when it reads 0.
+constexpr long long kForwardChunkRows = 1 << 16;
+static int forward_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, const int *live,
+                        cudaStream_t stream)
+{
+    if (n_points == 0) return NPHM_OK;
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    int ks_max = 1, rc;
+    for (int l = 0; l + 1 < s.n_lin; ++l) ks_max = std::max(ks_max, c.fwd[l].packed_ksteps_out());
+    const long long qpc = n_points <= kForwardChunkRows ? std::max(1LL, kForwardChunkRows / n_points) : 1;   // queries per chunk
+    const long long ppc = std::min(n_points, kForwardChunkRows);                                             // points per chunk
+    const long long max_rows = std::min((long long)n_queries, qpc) * ppc;
+    for (int b = 0; b < 2; ++b)
+        if ((rc = c.Fp[b].reserve(packed_bytes(max_rows, ks_max)))) return rc;
+    const int out_dim = s.N[s.n_lin - 1];
+    for (long long q0 = 0; q0 < n_queries; q0 += qpc) {
+        const long long nq = std::min(qpc, (long long)n_queries - q0);
+        for (long long p0 = 0; p0 < n_points; p0 += ppc) {
+            const long long np = std::min(ppc, n_points - p0);       // nq > 1 only with whole queries (np == n_points)
+            const size_t row0 = (size_t)q0 * n_points + p0;
+            const float *x = xyz + row0 * 3;
+            for (int l = 0; l < s.n_lin; ++l) {
+                tcl::LinearParams p;
+                p.M = nq * np;
+                p.live = live;
+                if (l == 0) { p.A1 = x; p.lda1 = 3; p.K1 = 3; }
+                else { p.Ap = c.Fp[(l - 1) & 1].as<uint8_t>(); p.a_ksteps = c.fwd[l].ksteps; }
+                p.bias = h->cvec.as<float>() + (size_t)q0 * s.cvec_stride + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = np;
+                if (l == s.n_lin - 1) {
+                    p.mode = tcl::kModeLinear;
+                    p.C = out + row0 * out_dim; p.ldc = out_dim;
+                } else {
+                    p.mode = tcl::kModeSoftplus;
+                    p.Cp = c.Fp[l & 1].as<uint8_t>(); p.c_ksteps = c.fwd[l].packed_ksteps_out();
+                    if (l + 1 == s.skip) { p.app = x; p.app_ld = 3; p.app_w = 3; }
+                }
+                if ((rc = tcl::launch_linear(c.fwd[l], p, stream))) return rc;
+            }
+        }
+    }
+    c.have_deriv = false;
+    return NPHM_OK;
+}
+
 }  // namespace nphm
 
 using namespace nphm;
@@ -239,6 +288,24 @@ static int chain_ready(nphm_mlp *h, const char *who)
     return NPHM_OK;
 }
 
+namespace nphm {
+// the forward-deformation backbone (DeepSDF MLP, hidden 512, 6 hidden layers, condition 232, 3 outputs: the `compress`
+// DeformationNetwork of scripts/configs/nphm_def.yaml) - the shape NPHM_IMPL_AUTO sends to the tensor cores
+bool tc_mlp_supported(const nphm_mlp *h)
+{
+    return h->cfg.hidden_dim == 512 && h->cfg.n_layers == 6 && h->cfg.lat_dim == 232 && h->cfg.out_dim == 3 && h->chain &&
+           h->chain->packed;
+}
+
+// forward with the constants of the last mlp_prepare
+int chain_forward(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, cudaStream_t stream)
+{
+    int rc = chain_ready(h, "chain_forward");
+    if (rc) return rc;
+    return forward_pass(h, xyz, n_queries, n_points, out, h->live, stream);
+}
+}  // namespace nphm
+
 // forward of an arbitrary-width stack, layer by layer (used when no fused kernel takes the shape)
 extern "C" int nphm_mlp_query_layers(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
                                      float *out_dev, void *stream_)
@@ -250,7 +317,7 @@ extern "C" int nphm_mlp_query_layers(nphm_mlp *h, const float *xyz_dev, const fl
     if (n_points == 0) return NPHM_OK;
     NPHM_REQUIRE(xyz_dev && out_dev, "nphm_mlp_query_layers: NULL pointer");
     if ((rc = mlp_prepare(h, cond_dev, n_queries, stream))) return rc;
-    return value_pass(h, xyz_dev, n_queries, n_points, false, out_dev, stream);
+    return forward_pass(h, xyz_dev, n_queries, n_points, out_dev, nullptr, stream);
 }
 
 // value + forward-mode tangents: out [q][n][out_dim] (optional), jac [q][n][out_dim][3] = d out / d xyz

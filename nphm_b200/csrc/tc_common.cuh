@@ -1,16 +1,13 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy PTX helpers and the log2-unit softplus shared by the tensor-core kernels.
+// wgmma / mbarrier / bulk-copy PTX helpers and the log2-unit softplus shared by the tensor-core kernels (sm_90a).
 #pragma once
 #include "common.cuh"
 #include <cuda_fp16.h>
+#include "wgmma.cuh"
 
 namespace nphm {
 namespace tc {
 
 constexpr float kS = 144.26950408889634f;            // 100 * log2(e)
-constexpr int kTmemCols = 512;
-#ifndef NPHM_POLY_MASK
-#define NPHM_POLY_MASK 0x88          // which of 8 consecutive elements evaluate lg2(1+e) on the FMA pipe (bit set) vs MUFU
-#endif
 
 // ------------------------------------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -43,51 +40,34 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar)
+// warpgroup MMA ordering: fence before the first wgmma that reads registers written by ordinary instructions, commit the
+// issued wgmmas as one group, wait until at most N groups are in flight (their accumulators / operands are then usable)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator / operand register across the asynchronous MMAs
+template <int N> __device__ __forceinline__ void wg_reg_fence(float (&d)[N])
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                 ::"r"(smem_u32(bar)) : "memory");
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t acc)
+template <int N> __device__ __forceinline__ void wg_reg_fence(uint32_t (&a)[N])
 {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, uint32_t (&r)[8])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_st8(uint32_t taddr, const uint32_t (&r)[8])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tc_st4(uint32_t taddr, const uint32_t (&r)[4])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};"
-                 ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
-// UMMA shared-memory descriptor, K-major, no swizzle: 8x(16 B) core matrices of 128 contiguous bytes;
-// LBO = byte distance between the two core matrices along K, SBO = between 8-row groups along N.
+// wgmma shared-memory descriptor, K-major, no swizzle: 8x(16 B) core matrices of 128 contiguous bytes;
+// LBO = byte distance between the two core matrices along K, SBO = between 8-row groups along M / N.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo)
 {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
-           (1ull << 46);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-// kind::f16 instruction descriptor: D fp32, A/B fp16, K-major both, M = 128
-__host__ __device__ constexpr uint32_t make_idesc(int n)
-{
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
+
+// Accumulator layout of a 64 x N warpgroup MMA (fp32): warp w (of the warpgroup) and lane l hold rows 16 w + l / 4 and
+// 16 w + l / 4 + 8; d[4 i + 0, 1] = (row, 8 i + 2 (l % 4) + 0, 1), d[4 i + 2, 3] = (row + 8, same columns).  The register A
+// operand of a k-step has the same layout: a[0] = row, k 2 (l % 4) + 0, 1 | a[1] = row + 8 | a[2], a[3]: k + 8 - so the
+// accumulator columns [16 j, 16 j + 16) of one layer, split to fp16, ARE the A registers of k-step j of the next one.
 
 // softplus in log2 units: sp'(t) = lg2(1 + 2^t) = max(t, 0) + lg2(1 + 2^-|t|)
 __device__ __forceinline__ float sp_t(float t)
@@ -98,31 +78,21 @@ __device__ __forceinline__ float sp_t(float t)
     return fmaxf(t, 0.0f) + l;
 }
 
-// same, with lg2(1 + e) evaluated on the FMA pipe: e * P6(e), |error| < 4.4e-7 (log2 units) on e in [0, 1].
-// Used for every other element so that the MUFU pipe (16 lanes/clk/SM) and the issue slots are balanced.
-__device__ __forceinline__ float sp_t_poly(float t)
+// softplus in log2 units with lg2(1 + e) on the FMA pipe: e * P5(e), |error| < 2.2e-6 log2 units = 1.5e-8 in SDF units
+// (fp32 evaluation included), i.e. at the round-off level of the activations it produces.  One MUFU (ex2) instead of two.
+__device__ __forceinline__ float sp_t_poly5(float t)
 {
     float e;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-fabsf(t)));
-    float pl = fmaf(e, 0.015529831517364317f, -0.0795574350973204f);
-    pl = fmaf(pl, e, 0.1942939234405454f);
-    pl = fmaf(pl, e, -0.3259017087892866f);
-    pl = fmaf(pl, e, 0.4735533221244069f);
-    pl = fmaf(pl, e, -0.720585455006072f);
-    pl = fmaf(pl, e, 1.4426678284772665f);
+    float pl = fmaf(e, -0.02645743577f, 0.1234514468f);
+    pl = fmaf(pl, e, -0.2795380944f);
+    pl = fmaf(pl, e, 0.4582707841f);
+    pl = fmaf(pl, e, -0.7182819141f);
+    pl = fmaf(pl, e, 1.442553145f);
     return fmaf(pl, e, fmaxf(t, 0.0f));
 }
-// softplus of 8 (4) accumulator values: even elements through MUFU lg2, odd ones through the polynomial
-__device__ __forceinline__ void sp8(const uint32_t (&r)[8], float (&v)[8])
-{
-#pragma unroll
-    for (int e = 0; e < 8; ++e) v[e] = (NPHM_POLY_MASK >> e) & 1 ? sp_t_poly(__uint_as_float(r[e])) : sp_t(__uint_as_float(r[e]));
-}
-__device__ __forceinline__ void sp4(const uint32_t (&r)[4], float (&v)[4])
-{
-#pragma unroll
-    for (int e = 0; e < 4; e += 2) { v[e] = sp_t(__uint_as_float(r[e])); v[e + 1] = sp_t_poly(__uint_as_float(r[e + 1])); }
-}
+// every other element through the polynomial: balances the MUFU pipe (16 lanes/clk/SM) against the FMA issue slots
+__device__ __forceinline__ float sp_sel(float t, int e) { return (e & 1) ? sp_t_poly5(t) : sp_t(t); }
 
 // split two fp32 values into packed fp16 (hi, lo) pairs; element 0 in the low half (lower K index)
 __device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t &lo)
@@ -134,27 +104,6 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t 
     lo = *reinterpret_cast<const uint32_t *>(&l);
 }
 
-
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc)
-{
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void tc_ld4(uint32_t taddr, uint32_t (&r)[4])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_st2(uint32_t taddr, uint32_t a, uint32_t b)
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(taddr), "r"(a), "r"(b) : "memory");
-}
-// kind::f16 instruction descriptor for an M x n tile: D fp32, A/B fp16, both K-major
-__host__ __device__ constexpr uint32_t make_idesc_m(int m, int n)
-{
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
 
 }  // namespace tc
 }  // namespace nphm

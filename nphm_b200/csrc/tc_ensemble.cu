@@ -1,54 +1,27 @@
-// tcgen05 / TMEM kernel for the identity-SDF ensemble (NPHM configuration: 40 members, hidden 200, 4 hidden
-// layers, condition 64+32) - the dominant kernel of the hot path.
+// Tensor-core path of the identity-SDF ensemble (NPHM configuration: 40 members, hidden 200, 4 hidden layers, condition
+// 64+32) - the dominant kernel of the hot path: weight packing, per-(query, member) records, launch (kernel: tc_ensemble_wgmma.cu).
 //
 // Reference semantics: FastEnsembleDeepSDFMirrored.forward  src/NPHM/models/EnsembledDeepSDF.py:203-267
 //
 // Math (SURVEY.md 8a'): per member, per point
 //   h0 = sp(W0x c + v0)            K=3   -> CUDA cores (v0 = latent part + bias, per query/member)
-//   h1 = sp(W1 h0 + b1)            128x112x208 UMMA   (N 101 -> 112, K 200 -> 208)
-//   h2 = sp(W2a h1/r2 + W2x c/r2 + v2)   128x208x112 UMMA   (K = 101 + 3 -> 112)
-//   h3 = sp(W3 h2 + b3)            128x208x208 UMMA
-//   s  = w4 . h3 + b4              CUDA cores, fused into the h3 epilogue; Gaussian anchor blend in registers.
-// Precision: tensor cores run kind::f16 with fp32 accumulation; every operand is split in two fp16 terms
+//   h1 = sp(W1 h0 + b1)            64x112x208 wgmma per warpgroup   (N 101 -> 112, K 200 -> 208)
+//   h2 = sp(W2a h1/r2 + W2x c/r2 + v2)   64x208x112 wgmma   (K = 101 + 3 -> 112)
+//   h3 = sp(W3 h2 + b3)            64x208x208 wgmma
+//   s  = w4 . h3 + b4              CUDA cores, on the layer-3 accumulators; Gaussian anchor blend in registers.
+// Precision: tensor cores run fp16 MMAs with fp32 accumulation; every operand is split in two fp16 terms
 // (x = hi + lo, 22 significant bits) and each product is evaluated as hi*hi + hi*lo + lo*hi (3 MMAs), which
-// keeps the result at fp32 round-off level (measured ~1e-7 abs against the fp32 reference, tolerance 1e-5).
+// keeps the result at fp32 round-off level (tolerance 1e-5 against the fp32 reference).
 // Activations are kept in "log2 units": t = a * 100*log2(e), sp'(t) = max(t,0) + lg2(1 + 2^-|t|) = 100*log2(e) *
 // softplus_100(a), so the softplus costs 2 MUFU + 3 ALU and the unit change is folded into biases / w4.
-//
-// Data flow per CTA (persistent, one CTA per SM, 18 warps):
-//   warp 16 : bulk-async-copy (TMA engine, cp.async.bulk) producer: streams pre-split fp16 weight slabs
-//             (N x 16 K-columns, hi|lo, UMMA no-swizzle K-major core-matrix order) from L2 into a 14-slot ring,
-//             and the per-(query,member) constant record (layer-0 weights, biases, w4, anchor) into a 2-slot ring.
-//   warp 17 : allocates TMEM, single-thread tcgen05.mma issuer: A (activations) from TMEM, B (weights) from smem,
-//             D (fp32) in TMEM; tcgen05.commit releases ring slots and signals the epilogue.
-//   warps 0-15: thread = point (TMEM lane) x column group: read D with tcgen05.ld, softplus, split to fp16 hi/lo,
-//             write the next layer's A operand back to TMEM with tcgen05.st, pre-load D with the next bias.
-// TMEM map (columns): D [0,208)  A_hi [208,312)  A_lo [312,416)   (fp16 pairs, 2 K-values per column).
 #include "tc_ensemble.cuh"
 #include <cstdlib>
 
 namespace nphm {
 namespace tc {
 
-// store 8 consecutive activations as fp16 hi/lo pairs: col_hi / col_lo = TMEM column of the first pair (2 K values per column)
-__device__ __forceinline__ void store_a8(uint32_t col_hi, uint32_t col_lo, const float (&v)[8])
-{
-    uint32_t hi[4], lo[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) split2(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
-    tc_st4(col_hi, hi);
-    tc_st4(col_lo, lo);
-}
-__device__ __forceinline__ void store_a4(uint32_t col_hi, uint32_t col_lo, const float (&v)[4])
-{
-    uint32_t h0, l0, h1, l1;
-    split2(v[0], v[1], h0, l0); split2(v[2], v[3], h1, l1);
-    tc_st2(col_hi, h0, h1);
-    tc_st2(col_lo, l0, l1);
-}
-
 // ------------------------------------------------------------------------------------------------ packing
-// Weight slabs: for weight set s, tensor layer L (1..3), k-step j: N x 16 fp16 hi then N x 16 fp16 lo, each in UMMA
+// Weight slabs: for weight set s, tensor layer L (1..3), k-step j: N x 16 fp16 hi then N x 16 fp16 lo, each in
 // no-swizzle K-major core-matrix order: byte offset of (n, kk) = (n/8)*256 + (kk/8)*128 + (n%8)*16 + (kk%8)*2.
 // Bias rows: the K padding of layers 1 and 3 (k = 200) carries S * b_l (per weight set, no latent part); the A operand has
 // the constant 1.0 at that k, so the MMAs add the bias and the epilogues do not (layer 2's constant depends on the latent:
@@ -157,75 +130,46 @@ __global__ void l2_slab_kernel(const uint8_t *__restrict__ weights, const float 
 }
 
 // ------------------------------------------------------------------------------------------------ MMA self test
-// One CTA: D[128 x n] = A[128 x 16*ks] * B[n x 16*ks]^T with the exact operand plumbing of the main kernel
-// (fp16 hi/lo split, A in TMEM, B slabs in smem).  `variant` bit0: swap LBO/SBO, bit1: swap the fp16 pair order.
-__global__ void __launch_bounds__(160, 1) mma_selftest_kernel(const float *__restrict__ A, const uint8_t *__restrict__ slabs,
+// One warpgroup: D[64 x n] = A[64 x 16*ks] * B[n x 16*ks]^T with the operand plumbing of the ensemble kernel (fp16 hi/lo split,
+// A in registers, B slabs in shared memory, 16-column wgmmas).  Rows 64 .. 127 of a 128-row test run in a second CTA.
+// `variant` bit0: swap LBO/SBO, bit1: swap the fp16 pair order (layout probes: only variant 0 is right).
+__global__ void __launch_bounds__(128, 1) mma_selftest_kernel(const float *__restrict__ A, const uint8_t *__restrict__ slabs,
                                                               int n, int ks, int variant, float *__restrict__ D)
 {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q4 = lane & 3;
     const int slab_bytes = n * 64;
-    if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32(&tmem_base)), "r"((uint32_t)kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     for (int i = threadIdx.x; i < ks * slab_bytes / 16; i += blockDim.x)
-        reinterpret_cast<uint4 *>(base)[i] = reinterpret_cast<const uint4 *>(slabs)[i];
+        reinterpret_cast<uint4 *>(smem_raw)[i] = reinterpret_cast<const uint4 *>(slabs)[i];
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base;
-    if (warp < 4) {
-        const int row = warp * 32 + lane;
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        for (int k0 = 0; k0 < ks * 16; k0 += 8) {
-            float v[8];
-            for (int e = 0; e < 8; ++e) v[e] = A[(size_t)row * ks * 16 + k0 + e];
-            if (variant & 2) for (int e = 0; e < 8; e += 2) { const float t = v[e]; v[e] = v[e + 1]; v[e + 1] = t; }
-            store_a8(tl + kColAhi + (k0 >> 1), tl + kColAlo + (k0 >> 1), v);
-        }
-        const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        for (int c = 0; c < n; c += 8) tc_st8(tl + kColD + c, zero);
-        tc_wait_st();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (threadIdx.x == 128) {
-        const uint32_t idesc = make_idesc(n);
-        const uint32_t lbo = (variant & 1) ? 256 : 128, sbo = (variant & 1) ? 128 : 256;
+    const int r0 = 64 * blockIdx.x + 16 * warp + (lane >> 2);
+    const uint32_t lbo = (variant & 1) ? 256 : 128, sbo = (variant & 1) ? 128 : 256;
+    for (int c = 0; c < n; c += 16) {
+        float d[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         for (int j = 0; j < ks; ++j) {
-            const uint32_t b = smem_u32(base + (size_t)j * slab_bytes);
-            const uint64_t b_hi = make_desc(b, lbo, sbo), b_lo = make_desc(b + n * 32, lbo, sbo);
-            tc_mma_ts(tmem + kColD, tmem + kColAhi + j * 8, b_hi, idesc, 1);
-            tc_mma_ts(tmem + kColD, tmem + kColAhi + j * 8, b_lo, idesc, 1);
-            tc_mma_ts(tmem + kColD, tmem + kColAlo + j * 8, b_hi, idesc, 1);
+            uint32_t ah[4], al[4];
+            for (int f = 0; f < 4; ++f) {                    // register A: (row r0 | r0 + 8, k 2 q4 | 8 + 2 q4)
+                const int r = r0 + 8 * (f & 1), k = 16 * j + 8 * (f >> 1) + 2 * q4;
+                float v0 = A[(size_t)r * ks * 16 + k], v1 = A[(size_t)r * ks * 16 + k + 1];
+                if (variant & 2) { const float t = v0; v0 = v1; v1 = t; }
+                split2(v0, v1, ah[f], al[f]);
+            }
+            const uint32_t b = smem_u32(smem_raw + (size_t)j * slab_bytes) + 2 * c * 16;
+            const uint64_t bh = make_desc(b, lbo, sbo), bl = make_desc(b + n * 32, lbo, sbo);
+            wg_fence();
+            wgmma_rs_n16(d, ah, bh, 1);
+            wgmma_rs_n16(d, ah, bl, 1);
+            wgmma_rs_n16(d, al, bh, 1);
+            wg_commit();
+            wg_wait<0>();
+            wg_reg_fence(d);
         }
-        tc_commit(&bar);
-    }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
-    if (warp < 4) {
-        const int row = warp * 32 + lane;
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        for (int c = 0; c < n; c += 8) {
-            uint32_t r[8];
-            tc_ld8(tl + kColD + c, r);
-            tc_wait_ld();
-            for (int e = 0; e < 8; ++e) D[(size_t)row * n + c + e] = __uint_as_float(r[e]);
+        for (int i = 0; i < 8; ++i) {
+            const int r = r0 + 8 * ((i >> 1) & 1), col = c + 8 * (i >> 2) + 2 * q4 + (i & 1);
+            D[(size_t)r * n + col] = d[i];
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == 4)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)kTmemCols) : "memory");
 }
 
 __global__ void pack_test_slabs_kernel(const float *__restrict__ B, int n, int ks, uint8_t *__restrict__ out)
@@ -271,7 +215,7 @@ int tc_ensemble_pack(nphm_ensemble *h, cudaStream_t stream)
 
 int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream)
 {
-    NPHM_REQUIRE(h->tc_ready, "tcgen05 ensemble kernel: weights not packed");
+    NPHM_REQUIRE(h->tc_ready, "tensor-core ensemble kernel: weights not packed");
     int rc;
     if ((rc = h->tc_consts.reserve((size_t)q.n_queries * h->n_members * tc::kRecFloats * sizeof(float)))) return rc;
     dim3 grid(h->n_members, q.n_queries);
@@ -319,7 +263,7 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     }
     const long long n_items = n_tiles * p.member_groups;
     const int grid_x = (int)(n_items < sm_count() ? n_items : sm_count());
-    if ((rc = tc::launch_ensemble_v8(p, prune, q.acts_out != nullptr, grid_x, stream))) return rc;
+    if ((rc = tc::launch_ensemble_wgmma(p, prune, q.acts_out != nullptr, grid_x, stream))) return rc;
     return NPHM_OK;
 }
 
@@ -335,167 +279,12 @@ extern "C" int nphm_debug_tc_mma(const float *a_dev, const float *b_dev, int n, 
     uint8_t *slabs = nullptr;
     NPHM_CUDA_CHECK(cudaMalloc(&slabs, (size_t)ks * n * 64));
     tc::pack_test_slabs_kernel<<<64, 256, 0, stream>>>(b_dev, n, ks, slabs);
-    const int smem = ks * n * 64 + 1024;
+    const int smem = ks * n * 64;
     NPHM_CUDA_CHECK(cudaFuncSetAttribute(tc::mma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tc::mma_selftest_kernel<<<1, 160, smem, stream>>>(a_dev, slabs, n, ks, variant, d_dev);
+    tc::mma_selftest_kernel<<<2, 128, smem, stream>>>(a_dev, slabs, n, ks, variant, d_dev);
     cudaError_t e = cudaStreamSynchronize(stream);
     cudaFree(slabs);
     if (e != cudaSuccess) { set_error("nphm_debug_tc_mma: %s", cudaGetErrorString(e)); return NPHM_ERR_CUDA; }
     return NPHM_OK;
 }
 
-// Micro-benchmark: `iters` MMAs (M=128, K=16, A from TMEM, B from smem) accumulating into one D (alternate=0) or
-// round-robin into `alternate` disjoint D ranges; returns SM cycles from first issue to commit completion.
-namespace nphm { namespace tc {
-__global__ void __launch_bounds__(160, 1) mma_bench_kernel(int n, int iters, int alternate, long long *cycles)
-{
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base;
-    const int warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32(&tmem_base)), "r"((uint32_t)kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    for (int i = threadIdx.x; i < 208 * 64 / 16; i += blockDim.x) reinterpret_cast<uint4 *>(smem_raw)[i] = make_uint4(0, 0, 0, 0);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base;
-    if (threadIdx.x == 128) {
-        const uint32_t idesc = make_idesc(n);
-        const uint64_t b = make_desc(smem_u32(smem_raw), 128, 256);
-        const long long t0 = clock64();
-        for (int i = 0; i < iters; ++i) {
-            const int d = alternate > 1 ? (i % alternate) * n : 0;
-            tc_mma_ts(tmem + d, tmem + 448, b, idesc, 1);
-        }
-        tc_commit(&bar);
-        mbar_wait(&bar, 0);
-        cycles[0] = clock64() - t0;
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == 4)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)kTmemCols) : "memory");
-}
-}}
-extern "C" int nphm_debug_tc_mma_bench(int n, int iters, int alternate, long long *cycles_host)
-{
-    using namespace nphm;
-    long long *d = nullptr;
-    NPHM_CUDA_CHECK(cudaMalloc(&d, 8));
-    const int smem = 208 * 64 + 1024;
-    NPHM_CUDA_CHECK(cudaFuncSetAttribute(tc::mma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tc::mma_bench_kernel<<<1, 160, smem>>>(n, iters, alternate, d);
-    cudaError_t e = cudaMemcpy(cycles_host, d, 8, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    if (e != cudaSuccess) { set_error("nphm_debug_tc_mma_bench: %s", cudaGetErrorString(e)); return NPHM_ERR_CUDA; }
-    return NPHM_OK;
-}
-
-// Layout probe for M = 64, A and B both from shared memory (SS form): D[64 x n] = A[64 x 16*ks] * B[n x 16*ks]^T.
-// A is stored K-chunk-major (for each 8-column K chunk: 64 rows x 16 B contiguous; LBO = 1024 B, SBO = 128 B), hi plane
-// then lo plane.  The whole TMEM accumulator region (128 lanes x n columns) is dumped so the host can recover the
-// row -> lane mapping.
-namespace nphm { namespace tc {
-__global__ void __launch_bounds__(160, 1) mma_m64_probe_kernel(const float *__restrict__ A, const uint8_t *__restrict__ slabs,
-                                                               int n, int ks, int variant, float *__restrict__ dump)
-{
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int slab_bytes = n * 64;
-    uint8_t *a_hi = smem_raw, *a_lo = smem_raw + ks * 4096, *b_base = smem_raw + ks * 8192;
-    if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32(&tmem_base)), "r"((uint32_t)kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    for (int i = threadIdx.x; i < ks * slab_bytes / 16; i += blockDim.x)
-        reinterpret_cast<uint4 *>(b_base)[i] = reinterpret_cast<const uint4 *>(slabs)[i];
-    const int m_rows = (variant & 8) ? 128 : 64;
-    const int vlay = variant & 3;
-    if (threadIdx.x < m_rows) {
-        const int row = threadIdx.x;
-        for (int kc = 0; kc < ks * 2; ++kc) {            // 8-column K chunks
-            uint32_t hi[4], lo[4];
-            for (int i = 0; i < 4; ++i) split2(A[(size_t)row * ks * 16 + kc * 8 + 2 * i], A[(size_t)row * ks * 16 + kc * 8 + 2 * i + 1], hi[i], lo[i]);
-            // variant 0/1: K-chunk-major (chunk kc: 64 rows x 16 B); variant 2: like the B slabs (row-group-major per k-step)
-            const size_t off = vlay == 2 ? (size_t)(kc >> 1) * (m_rows * 32) + (size_t)(row >> 3) * 256 + (size_t)(kc & 1) * 128 + (size_t)(row & 7) * 16
-                                         : (size_t)kc * (m_rows * 16) + (size_t)row * 16;
-            *reinterpret_cast<uint4 *>(a_hi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4 *>(a_lo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base;
-    if (warp < 4) {
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        uint32_t fill[8];
-        for (int e = 0; e < 8; ++e) fill[e] = __float_as_uint(0.f);
-        for (int c = 0; c < n; c += 8) tc_st8(tl + c, fill);
-        tc_wait_st();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (threadIdx.x == 128) {
-        const int m_rows2 = (variant & 8) ? 128 : 64;
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m_rows2 >> 4) << 24);
-        for (int j = 0; j < ks; ++j) {
-            const uint32_t albo = (variant & 3) == 2 ? 128 : m_rows2 * 16, asbo = (variant & 3) == 2 ? 256 : 128;
-            const uint32_t astep = m_rows2 * 32;
-            uint64_t ah = make_desc(smem_u32(a_hi + j * astep), albo, asbo), al = make_desc(smem_u32(a_lo + j * astep), albo, asbo);
-            const uint32_t b = smem_u32(b_base + (size_t)j * slab_bytes);
-            uint64_t bh = make_desc(b, 128, 256), bl = make_desc(b + n * 32, 128, 256);
-            if (variant & 4) { uint64_t t = ah; ah = bh; bh = t; t = al; al = bl; bl = t; }      // swap operand order
-            tc_mma_ss(tmem, ah, bh, idesc, 1);
-            tc_mma_ss(tmem, ah, bl, idesc, 1);
-            tc_mma_ss(tmem, al, bh, idesc, 1);
-        }
-        tc_commit(&bar);
-    }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
-    if (warp < 4) {
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        for (int c = 0; c < n; c += 8) {
-            uint32_t r[8];
-            tc_ld8(tl + c, r);
-            tc_wait_ld();
-            for (int e = 0; e < 8; ++e) dump[(size_t)(warp * 32 + lane) * n + c + e] = __uint_as_float(r[e]);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == 4)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)kTmemCols) : "memory");
-}
-}}
-extern "C" int nphm_debug_tc_mma_m64(const float *a_dev, const float *b_dev, int n, int ks, int variant, float *dump_dev, void *stream_)
-{
-    using namespace nphm;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    NPHM_REQUIRE(n % 16 == 0 && n >= 16 && n <= 256 && ks >= 1 && ks <= 8, "nphm_debug_tc_mma_m64: bad shape");
-    uint8_t *slabs = nullptr;
-    NPHM_CUDA_CHECK(cudaMalloc(&slabs, (size_t)ks * n * 64));
-    tc::pack_test_slabs_kernel<<<64, 256, 0, stream>>>(b_dev, n, ks, slabs);
-    const int smem = ks * 8192 + ks * n * 64 + 1024;
-    NPHM_CUDA_CHECK(cudaFuncSetAttribute(tc::mma_m64_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tc::mma_m64_probe_kernel<<<1, 160, smem, stream>>>(a_dev, slabs, n, ks, variant, dump_dev);
-    cudaError_t e = cudaStreamSynchronize(stream);
-    cudaFree(slabs);
-    if (e != cudaSuccess) { set_error("nphm_debug_tc_mma_m64: %s", cudaGetErrorString(e)); return NPHM_ERR_CUDA; }
-    return NPHM_OK;
-}

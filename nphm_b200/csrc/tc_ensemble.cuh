@@ -1,5 +1,5 @@
-// Shared definitions of the tensor-core ensemble kernels (tc_ensemble.cu = v6 column-rotation kernel,
-// tc_ensemble_v8.cu = in-place operand conversion kernel): shapes, weight-slab / record layout, kernel parameters.
+// Shared definitions of the tensor-core ensemble kernel (tc_ensemble.cu: packing and launch, tc_ensemble_wgmma.cu: the
+// kernel): shapes, weight-slab / record layout, kernel parameters.
 #pragma once
 #include "engine.cuh"
 #include "tc_common.cuh"
@@ -17,20 +17,6 @@ constexpr int kSlabBytes = kNP2 * 64;
 constexpr int kGroupBytes = 7 * kSlabBytes;             // weight groups: L1 | L2 | L3 k-steps 0-6 | L3 k-steps 7-12
 constexpr int kL1Bytes = kKS1 * kSlab1Bytes, kL2Bytes = kKS2 * kSlabBytes, kL3Bytes = kKS3 * kSlabBytes;
 constexpr int kSetBytes = kL1Bytes + kL2Bytes + kL3Bytes;     // 359424 per weight set
-constexpr int kColD = 0, kColAhi = 208, kColAlo = 312;      // map of the MMA self-test / micro-benchmark kernels only
-// TMEM column map of the ensemble kernel.  Operands rotate through the 512 columns so that (a) the layer-2 MMAs can run
-// WHILE the layer-1 epilogue is still producing their A operand (D2 is disjoint from D1 and A1) and (b) the first six
-// k-steps of the next member's layer 1 can be issued while its remaining layer-0 outputs are still being computed:
-//   A0a (layer-1 A, K 0..95, written one member ahead)   hi [416,464) lo [464,512)
-//   A0b (layer-1 A, K 96..207)                            hi [0,56)    lo [56,112)
-//   D1 [112,224)   A1 (layer-2 A, K 0..111) hi [0,56) lo [56,112)   D2 [304,512)
-//   A2 (layer-3 A, K 0..207) hi [0,104) lo [104,208)      D3 [208,416)
-// Every overlap is between objects whose lifetimes are separated by an mbarrier (see the hazard notes in the kernel).
-constexpr int kColSpareHi = 416, kColSpareLo = 464, kNA = 96;
-constexpr int kColA0bHi = 0, kColA0bLo = 56;
-constexpr int kColD1 = 112, kColA1Hi = 0, kColA1Lo = 56;
-constexpr int kColD2 = 304, kColA2Hi = 0, kColA2Lo = 104;
-constexpr int kColD3 = 208;
 constexpr int kRecSlots = 3;
 // activation derivatives saved per (member, point) for the fitting backward: sigma'0 [208] | sigma'1 [112] | sigma'2 [208] | sigma'3 [208]
 constexpr int kActOff0 = 0, kActOff1 = 208, kActOff2 = 320, kActLd = 528;
@@ -43,9 +29,6 @@ constexpr int kRecB3 = 1152;       // 208
 constexpr int kRecW4 = 1360;       // 208
 constexpr int kRecMisc = 1568;     // b4, ax, ay, az, has_anchor, mirror, -, -
 constexpr int kRecFloats = 1576;
-constexpr int kEpiWarps = 16;      // 4 lane quarters x 4 column groups (8-column chunks dealt round-robin)
-constexpr int kParts = kEpiWarps / 4;
-constexpr int kThreads = 32 * (kEpiWarps + 2);
 
 struct Params {
     const uint8_t *weights;     // [n_sets][kSetBytes]
@@ -71,8 +54,7 @@ struct Params {
     int blocked, px0, px1, by, bz;
 };
 
-// v8 kernel (tc_ensemble_v8.cu): same parameters, same weight slabs and records
-int launch_ensemble_v8(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream);
+int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream);
 
 }  // namespace tc
 }  // namespace nphm

@@ -1,0 +1,457 @@
+// Warpgroup-MMA (wgmma, sm_90a) kernel for the identity-SDF ensemble.
+//
+// Reference semantics: FastEnsembleDeepSDFMirrored.forward  src/NPHM/models/EnsembledDeepSDF.py:203-267
+// Math, weight slabs and per-(query, member) records are those of tc_ensemble.cu (see the header there).
+//
+// A CTA is persistent over 128-point tiles: two consumer warpgroups of 64 points each and one producer warpgroup, which
+// hands most of its registers to the consumers (setmaxnreg: 24 / 240 per thread).
+//   producer (warp 8, one lane): bulk async copies of the record of every member and of its weight groups
+//       L1 | L2 | L3 k-steps 0-6 | L3 k-steps 7-12 into two shared-memory buffers (one mbarrier pair each).
+//   consumers (warps 0-7): per member, layer 0 on CUDA cores straight into registers; layers 1-3 as 64 x N x 16 wgmmas with
+//       A in REGISTERS and B (weights) in shared memory.  The accumulator layout of a 64 x N wgmma is the register layout of
+//       its A operand (tc_common.cuh), so the epilogue of a layer (softplus, fp16 hi/lo split) produces the next layer's A
+//       operand in place, without a round trip through memory.  The output layer (dot with w4) and the anchor blend run on
+//       the accumulator registers of layer 3.
+// Wide layers are issued in two column halves (112 + 96) so that the accumulators and the A operand of a layer fit the
+// register file together: the first half of layer 2 is converted while the MMAs of the second half run.
+#include "tc_ensemble.cuh"
+
+namespace nphm {
+namespace tc {
+namespace wg {
+
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 32 * (kConsumerWarps + 4);
+constexpr int kUnits208 = 13, kUnits112 = 7;
+constexpr uint32_t kHalfRows = 14 * 256;       // byte offset of slab row 112 (the second column half of a 208-wide layer)
+
+struct __align__(128) Smem {
+    uint8_t wbuf[2][kGroupBytes];            // weight groups (one bulk copy + one barrier each)
+    float rec[kRecSlots][kRecFloats];
+    uint64_t w_full[2], w_empty[2];
+    uint64_t rec_full[kRecSlots], rec_empty[kRecSlots];
+    uint64_t mask_ready;
+    unsigned long long maskq[2][kConsumerWarps];
+};
+
+// 3 MMAs of one k-step (hi*hi + hi*lo + lo*hi): `b` = shared address of the slab's hi half, its lo half lies lo_off further
+template <int N, typename F>
+__device__ __forceinline__ void kstep(F &&mma, float (&d)[N / 2], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint32_t b,
+                                      uint32_t lo_off)
+{
+    const uint64_t bh = make_desc(b, 128, 256), bl = make_desc(b + lo_off, 128, 256);
+    mma(d, ah, bh, 1);
+    mma(d, ah, bl, 1);
+    mma(d, al, bh, 1);
+}
+
+// k-step j of an accumulator -> A registers of the next layer.  f(value, column, row 0/1, element) returns the activation.
+template <int N, typename F>
+__device__ __forceinline__ void to_operand(const float (&d)[N], int j, int col0, int q4, uint32_t (&ah)[4], uint32_t (&al)[4], F &&f)
+{
+    float v[2][4];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int col = col0 + 16 * j + 8 * hh + 2 * q4 + e;
+                v[r][2 * hh + e] = f(d[4 * (2 * j + hh) + 2 * r + e], col, r, 2 * hh + e);
+            }
+    split2(v[0][0], v[0][1], ah[0], al[0]);
+    split2(v[1][0], v[1][1], ah[1], al[1]);
+    split2(v[0][2], v[0][3], ah[2], al[2]);
+    split2(v[1][2], v[1][3], ah[3], al[3]);
+}
+
+template <bool PRUNE, bool ACTS>
+__global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Params p)
+{
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long tiles_per_query = p.blocked ? p.n_tiles : (p.n_points + 127) / 128;
+    const long long n_tiles = p.n_tiles;
+    // ACTS (fitting: few points, so few tiles): the members of a tile are split over `member_groups` CTAs - a work item is
+    // (tile, group of consecutive members), the in-kernel blend is meaningless then and `out` is not written
+    const int n_groups = ACTS ? p.member_groups : 1;
+    const long long n_items = n_tiles * n_groups;
+    auto group_mask = [&](long long item) -> unsigned long long {
+        const unsigned long long all = p.n_members >= 64 ? ~0ull : (1ull << p.n_members) - 1;
+        if (!ACTS || n_groups == 1) return all;
+        const int per = (p.n_members + n_groups - 1) / n_groups, lo = (int)(item % n_groups) * per;
+        const int hi = min(p.n_members, lo + per);
+        return ((1ull << hi) - 1) & ~((1ull << lo) - 1);
+    };
+
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < 2; ++i) { mbar_init(&sm.w_full[i], 1); mbar_init(&sm.w_empty[i], kConsumerWarps); }
+        for (int i = 0; i < kRecSlots; ++i) { mbar_init(&sm.rec_full[i], 1); mbar_init(&sm.rec_empty[i], kConsumerWarps); }
+        mbar_init(&sm.mask_ready, kConsumerWarps);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp >= kConsumerWarps) {
+        // =========================================================================== producer (bulk async copies)
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
+        if (warp == kConsumerWarps && lane == 0) {
+            int wb = 0;
+            uint32_t wph = 0, tcount = 0, rcount = 0;
+            for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
+                const long long tile = ACTS ? item / n_groups : item;
+                const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
+                unsigned long long mask = group_mask(item);
+                if (PRUNE) {
+                    mbar_wait(&sm.mask_ready, tcount & 1);
+                    mask = 0;
+                    for (int w = 0; w < kConsumerWarps; ++w) mask |= sm.maskq[tcount & 1][w];
+                }
+                for (int m = 0; m < p.n_members; ++m) {
+                    if (!((mask >> m) & 1)) continue;
+                    const int rslot = rcount % kRecSlots;
+                    mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
+                    mbar_expect_tx(&sm.rec_full[rslot], kRecFloats * 4);
+                    bulk_g2s(sm.rec[rslot], p.recs + ((size_t)qi * p.n_members + m) * kRecFloats, kRecFloats * 4, &sm.rec_full[rslot]);
+                    ++rcount;
+                    const int set = m < 2 * p.n_symm ? (m >> 1) : m - p.n_symm;
+                    const uint8_t *w = p.weights + (size_t)set * kSetBytes;
+#pragma unroll 1
+                    for (int g = 0; g < 4; ++g) {
+                        const uint32_t bytes = g == 0 ? kL1Bytes : (g == 1 ? kL2Bytes : (g == 2 ? 7 * kSlabBytes : 6 * kSlabBytes));
+                        mbar_wait(&sm.w_empty[wb], wph ^ 1);
+                        mbar_expect_tx(&sm.w_full[wb], bytes);
+                        if (g == 1) {
+                            // layer 2: the last k-step slab carries this (query, member)'s bias row (l2_slab_kernel)
+                            bulk_g2s(sm.wbuf[wb], w, bytes - kSlabBytes, &sm.w_full[wb]);
+                            bulk_g2s(sm.wbuf[wb] + (bytes - kSlabBytes), p.l2_slabs + ((size_t)qi * p.n_members + m) * kSlabBytes,
+                                     kSlabBytes, &sm.w_full[wb]);
+                        } else {
+                            bulk_g2s(sm.wbuf[wb], w, bytes, &sm.w_full[wb]);
+                        }
+                        w += bytes;
+                        if (++wb == 2) { wb = 0; wph ^= 1; }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // =========================================================================== consumer warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 240;" ::: "memory");
+    const int q4 = lane & 3;
+    int rl[2];                                   // tile rows (points) of this thread's accumulator rows
+    rl[0] = 64 * (warp >> 2) + 16 * (warp & 3) + (lane >> 2);
+    rl[1] = rl[0] + 8;
+    int wb = 0;
+    uint32_t wph = 0, tcount = 0, rcount = 0;
+    auto release = [&](uint64_t *bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+    auto next_buf = [&]() { if (++wb == 2) { wb = 0; wph ^= 1; } };
+
+    for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
+        const long long tile = ACTS ? item / n_groups : item;
+        const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
+        long long idx[2], g[2];
+        bool valid[2], quirk[2];
+        float x[2], y[2], z[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int row = rl[i];
+            if (p.blocked) {
+                // compact 8 x 4 x 4 block of grid points (z fastest inside the block)
+                const long long tz = tile % p.bz, txy = tile / p.bz;
+                const int ty = (int)(txy % p.by), tx = (int)(txy / p.by);
+                const int ix = p.px0 + tx * 8 + (row >> 4), iy = ty * 4 + ((row >> 2) & 3), iz = (int)tz * 4 + (row & 3);
+                g[i] = ((long long)ix * p.res + iy) * p.res + iz;
+                valid[i] = ix <= p.px1 && iy < p.res && iz < p.res && g[i] >= p.first && g[i] < p.first + p.n_points;
+                idx[i] = g[i] - p.first;
+                const int cx_ = min(ix, p.res - 1), cy_ = min(iy, p.res - 1), cz_ = min(iz, p.res - 1);
+                x[i] = __ldg(p.axes + cx_); y[i] = __ldg(p.axes + p.res + cy_); z[i] = __ldg(p.axes + 2 * p.res + cz_);
+                if (!valid[i]) g[i] = p.first;
+            } else {
+                idx[i] = (tile - (long long)qi * tiles_per_query) * 128 + row;
+                valid[i] = idx[i] < p.n_points;
+                g[i] = p.first + (valid[i] ? idx[i] : 0);
+                if (p.xyz) {
+                    const float *pp = p.xyz + ((size_t)qi * p.n_points + (valid[i] ? idx[i] : 0)) * 3;
+                    x[i] = pp[0]; y[i] = pp[1]; z[i] = pp[2];
+                } else {
+                    const long long rr = (long long)p.res * p.res;
+                    const int ix = (int)(g[i] / rr), iy = (int)((g[i] - ix * rr) / p.res), iz = (int)(g[i] % p.res);
+                    x[i] = __ldg(p.axes + ix); y[i] = __ldg(p.axes + p.res + iy); z[i] = __ldg(p.axes + 2 * p.res + iz);
+                }
+            }
+            quirk[i] = p.quirk_period > 0 && ((g[i] % p.quirk_period) == p.quirk_period - 1 || g[i] == p.total - 1);
+        }
+        float num[2] = {0.f, 0.f}, den[2] = {0.f, 0.f};
+        unsigned long long mask = group_mask(item);
+        if (PRUNE) {
+            // blend weights of all members for this thread's points: S = sum_k w_k; a member is needed by the tile if
+            // w_k >= tau * (S + 1e-6) for at least one of its points (dropped mass per point < n_members * tau).
+            const float *anc = p.anchors + (size_t)qi * (p.n_members - 1) * 3;
+            auto weight = [&](int k, int i) {
+                float d = -0.2f;
+                if (k < p.n_members - 1) {
+                    const float dx = __ldg(anc + 3 * k) - x[i], dy = __ldg(anc + 3 * k + 1) - y[i], dz = __ldg(anc + 3 * k + 2) - z[i];
+                    const float nrm = sqrtf(dx * dx + dy * dy + dz * dz) + 10e-6f;
+                    d = -(nrm * nrm);
+                }
+                return expf(__fdiv_rn(d, 0.01f));
+            };
+            float thr[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                float S = 0.f;
+                for (int k = 0; k < p.n_members; ++k) S += weight(k, i);
+                den[i] = S;
+                thr[i] = p.prune_tau * (S + 1e-6f);
+            }
+            unsigned long long wm = 0;
+            for (int k = 0; k < p.n_members; ++k) {
+                const bool need = (valid[0] && weight(k, 0) >= thr[0]) || (valid[1] && weight(k, 1) >= thr[1]);
+                if (__any_sync(0xffffffffu, need)) wm |= 1ull << k;
+            }
+            wm |= 1ull << (p.n_members - 1);      // every tile evaluates >= 1 member
+            if (lane == 0) {
+                sm.maskq[tcount & 1][warp] = wm;
+                mbar_arrive(&sm.mask_ready);
+            }
+            mbar_wait(&sm.mask_ready, tcount & 1);
+            mask = 0;
+            for (int w = 0; w < kConsumerWarps; ++w) mask |= sm.maskq[tcount & 1][w];
+        }
+
+        for (int m = 0; m < p.n_members; ++m) {
+            if (!((mask >> m) & 1)) continue;
+            const uint32_t rslot = rcount % kRecSlots;
+            mbar_wait(&sm.rec_full[rslot], (rcount / kRecSlots) & 1);
+            const float *rec = sm.rec[rslot];
+            float cx[2], cy[2], cz[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                cx[i] = x[i] - rec[kRecMisc + 1]; cy[i] = y[i] - rec[kRecMisc + 2]; cz[i] = z[i] - rec[kRecMisc + 3];
+                if (rec[kRecMisc + 5] != 0.f) cx[i] = -cx[i];          // mirrored member
+                cx[i] *= kS; cy[i] *= kS; cz[i] *= kS;                 // coordinates in log2 units
+            }
+            // activation derivatives for the fitting backward, sigma'(pre) = 1 - 2^(-softplus) (log2 units): per (member, tile) a
+            // block of kActLd features x 128 points, feature-major.  Columns beyond a layer's width receive don't-care values.
+            float *const ab = ACTS ? p.acts_out + ((size_t)m * tiles_per_query + (tile % tiles_per_query)) * kActLd * 128 : nullptr;
+            auto save_act = [&](int off, int col, int r, float v) {
+                if (ACTS) {
+                    float ex;
+                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(-v));
+                    ab[(size_t)(off + col) * 128 + rl[r]] = 1.0f - ex;
+                }
+            };
+
+            // ---------------- layer 0 on CUDA cores -> A operand of layer 1 (K 208: h0 (200) | 1.0 (bias row) | zeros)
+            uint32_t a0h[kUnits208][4], a0l[kUnits208][4];
+#pragma unroll
+            for (int j = 0; j < kUnits208; ++j) {
+                float v[2][4];
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const int col = 16 * j + 8 * (c >> 1) + 2 * q4 + (c & 1);
+                    const float4 w = reinterpret_cast<const float4 *>(rec + kRecL0)[col];
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        float a;
+                        if (col < kH) a = sp_sel(fmaf(w.x, cx[r], fmaf(w.y, cy[r], fmaf(w.z, cz[r], w.w))), c);
+                        else a = col == kH ? 1.0f : 0.0f;
+                        save_act(kActOff0, col, r, a);
+                        v[r][c] = a;
+                    }
+                }
+                split2(v[0][0], v[0][1], a0h[j][0], a0l[j][0]);
+                split2(v[1][0], v[1][1], a0h[j][1], a0l[j][1]);
+                split2(v[0][2], v[0][3], a0h[j][2], a0l[j][2]);
+                split2(v[1][2], v[1][3], a0h[j][3], a0l[j][3]);
+            }
+
+            // ---------------- layer 1 (N 112, K 208)
+            float acc1[56];
+#pragma unroll
+            for (int i = 0; i < 56; ++i) acc1[i] = 0.f;
+            mbar_wait(&sm.w_full[wb], wph);
+            {
+                const uint32_t b0 = smem_u32(sm.wbuf[wb]);
+                wg_fence();
+#pragma unroll
+                for (int j = 0; j < kUnits208; ++j)
+                    kstep<112>(wgmma_rs_n112, acc1, a0h[j], a0l[j], b0 + j * kSlab1Bytes, kNP1 * 32);
+                wg_commit();
+                wg_wait<0>();
+                wg_reg_fence(acc1);
+            }
+            release(&sm.w_empty[wb]);
+            next_buf();
+
+            // ---------------- epilogue of layer 1 -> A operand of layer 2 (K 112: h1 (101) | c (3) | 1.0 (bias row) | zeros)
+            uint32_t a1h[kUnits112][4], a1l[kUnits112][4];
+#pragma unroll
+            for (int j = 0; j < kUnits112; ++j)
+                to_operand(acc1, j, 0, q4, a1h[j], a1l[j], [&](float t, int col, int r, int e) {
+                    float a;
+                    if (col < kN1) a = sp_sel(t, e);
+                    else if (col < kN1 + 3) a = col == kN1 ? cx[r] : (col == kN1 + 1 ? cy[r] : cz[r]);
+                    else a = col == kN1 + 3 ? 1.0f : 0.0f;
+                    save_act(kActOff1, col, r, a);
+                    return a;
+                });
+
+            // ---------------- layer 2 (N 208 = 112 + 96, K 112): the first half is converted while the second one runs
+            float acc2a[56], acc2b[48];
+#pragma unroll
+            for (int i = 0; i < 56; ++i) acc2a[i] = 0.f;
+#pragma unroll
+            for (int i = 0; i < 48; ++i) acc2b[i] = 0.f;
+            mbar_wait(&sm.w_full[wb], wph);
+            uint32_t a2h[kUnits208][4], a2l[kUnits208][4];
+            auto e2 = [&](float t, int col, int r, int e) {
+                const float a = col < kH ? sp_sel(t, e) : (col == kH ? 1.0f : 0.0f);     // k = 200: bias row of layer 3
+                save_act(kActOff2, col, r, a);
+                return a;
+            };
+            {
+                const uint32_t b0 = smem_u32(sm.wbuf[wb]);
+                wg_fence();
+#pragma unroll
+                for (int j = 0; j < kUnits112; ++j)
+                    kstep<112>(wgmma_rs_n112, acc2a, a1h[j], a1l[j], b0 + j * kSlabBytes, kNP2 * 32);
+                wg_commit();
+#pragma unroll
+                for (int j = 0; j < kUnits112; ++j)
+                    kstep<96>(wgmma_rs_n96, acc2b, a1h[j], a1l[j], b0 + j * kSlabBytes + kHalfRows, kNP2 * 32);
+                wg_commit();
+                wg_wait<1>();
+                wg_reg_fence(acc2a);
+#pragma unroll
+                for (int j = 0; j < 7; ++j) to_operand(acc2a, j, 0, q4, a2h[j], a2l[j], e2);
+                wg_wait<0>();
+                wg_reg_fence(acc2b);
+            }
+            release(&sm.w_empty[wb]);
+            next_buf();
+#pragma unroll
+            for (int j = 0; j < 6; ++j) to_operand(acc2b, j, 112, q4, a2h[7 + j], a2l[7 + j], e2);
+
+            // ---------------- layer 3 (N 208 = 112 + 96, K 208 in two weight groups) and the output layer w4 . h3 + b4
+            const int wbA = wb;
+            const uint32_t phA = wph;
+            next_buf();
+            const int wbB = wb;
+            const uint32_t phB = wph;
+            next_buf();
+            mbar_wait(&sm.w_full[wbA], phA);
+            mbar_wait(&sm.w_full[wbB], phB);
+            const uint32_t bA = smem_u32(sm.wbuf[wbA]), bB = smem_u32(sm.wbuf[wbB]);
+            float part[2] = {0.f, 0.f};
+            // sigma'3 is the A operand of the first backward GEMM: saved operand-ready (tc_linear.cuh "packed": per k-step = unit
+            // of 16 features [128 x 16 fp16 hi | 128 x 16 fp16 lo], core-matrix order), zeros in the K padding
+            uint8_t *const pk = ACTS ? p.acts_packed_out + ((size_t)m * tiles_per_query + (tile % tiles_per_query)) * p.acts_packed_tile_steps * 8192
+                                     : nullptr;
+            auto out_layer = [&](const auto &acc, int col0, int units) {
+#pragma unroll
+                for (int j = 0; j < units; ++j)
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            float v[2];
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int col = col0 + 16 * j + 8 * hh + 2 * q4 + e;
+                                v[e] = sp_sel(acc[4 * (2 * j + hh) + 2 * r + e], e);
+                                part[r] = fmaf(v[e], rec[kRecW4 + col], part[r]);          // w4 is zero in the padding
+                                if (ACTS) {
+                                    float ex;
+                                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(-v[e]));
+                                    v[e] = col < kH ? 1.0f - ex : 0.f;
+                                }
+                            }
+                            if (ACTS) {
+                                uint32_t hi, lo;
+                                split2(v[0], v[1], hi, lo);
+                                const int row = rl[r], u = (col0 >> 4) + j;
+                                uint8_t *dst = pk + (size_t)u * 8192 + (size_t)(row >> 3) * 256 + (size_t)hh * 128 + (size_t)(row & 7) * 16 + 4 * q4;
+                                *reinterpret_cast<uint32_t *>(dst) = hi;
+                                *reinterpret_cast<uint32_t *>(dst + 4096) = lo;
+                            }
+                        }
+            };
+            {
+                float acc3[56];
+#pragma unroll
+                for (int i = 0; i < 56; ++i) acc3[i] = 0.f;
+                wg_fence();
+#pragma unroll
+                for (int j = 0; j < kUnits208; ++j)
+                    kstep<112>(wgmma_rs_n112, acc3, a2h[j], a2l[j], (j < 7 ? bA + j * kSlabBytes : bB + (j - 7) * kSlabBytes), kNP3 * 32);
+                wg_commit();
+                wg_wait<0>();
+                wg_reg_fence(acc3);
+                out_layer(acc3, 0, 7);
+            }
+            {
+                float acc3[48];
+#pragma unroll
+                for (int i = 0; i < 48; ++i) acc3[i] = 0.f;
+                wg_fence();
+#pragma unroll
+                for (int j = 0; j < kUnits208; ++j)
+                    kstep<96>(wgmma_rs_n96, acc3, a2h[j], a2l[j], (j < 7 ? bA + j * kSlabBytes : bB + (j - 7) * kSlabBytes) + kHalfRows,
+                              kNP3 * 32);
+                wg_commit();
+                wg_wait<0>();
+                wg_reg_fence(acc3);
+                release(&sm.w_empty[wbA]);
+                release(&sm.w_empty[wbB]);
+                out_layer(acc3, 112, 6);
+            }
+
+            // ---------------- member output (reduced over the 4 lanes of a row) and the anchor blend
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                float s = part[r];
+                s += __shfl_xor_sync(0xffffffffu, s, 1);
+                s += __shfl_xor_sync(0xffffffffu, s, 2);
+                s += rec[kRecMisc + 0];
+                if (q4 == 0 && p.members_out && valid[r]) p.members_out[((size_t)qi * p.n_points + idx[r]) * p.n_members + m] = s;
+                float d;
+                if (rec[kRecMisc + 4] != 0.f) {
+                    const float dx = rec[kRecMisc + 1] - x[r], dy = rec[kRecMisc + 2] - y[r], dz = rec[kRecMisc + 3] - z[r];
+                    const float nrm = sqrtf(dx * dx + dy * dy + dz * dz) + 10e-6f;
+                    d = -(nrm * nrm);
+                } else {
+                    d = -0.2f;
+                }
+                const float w = expf(__fdiv_rn(d, 0.01f));
+                num[r] = fmaf(w, quirk[r] ? 1.0f : s, num[r]);
+                if (!PRUNE) den[r] += w;
+            }
+            release(&sm.rec_empty[rslot]);
+            ++rcount;
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+            if (q4 == 0 && valid[r] && n_groups == 1) p.out[(size_t)qi * p.n_points + idx[r]] = __fdiv_rn(num[r], den[r] + 1e-6f);
+    }
+}
+
+}  // namespace wg
+
+int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream)
+{
+    const int smem = (int)sizeof(wg::Smem);
+    auto kern = acts ? wg::ensemble_wgmma_kernel<false, true>
+                     : (prune ? wg::ensemble_wgmma_kernel<true, false> : wg::ensemble_wgmma_kernel<false, false>);
+    NPHM_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    kern<<<grid_x, wg::kThreads, smem, stream>>>(p);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+}  // namespace tc
+}  // namespace nphm

@@ -1,17 +1,18 @@
-// Generic fp32-accurate linear layer on tcgen05:  C = epilogue( [A1 | A2] * W^T )
+// Generic fp32-accurate linear layer on Hopper warpgroup MMAs (wgmma):  C = epilogue( [A1 | A2] * W^T )
 //
-// One building block for everything on the hot path that is a chain of dense layers but does not fit the two fully fused
-// kernels (tc_ensemble_v8.cu: hidden 200 ensemble, tc_mlp.cu: hidden 512 forward): the forward-mode Jacobian and the
+// One building block for everything on the hot path that is a chain of dense layers but does not fit the fully fused
+// ensemble kernel (tc_ensemble_wgmma.cu, hidden 200): the forward pass, the forward-mode Jacobian and the
 // backward pass of the forward-deformation network (reference src/NPHM/models/diff_operators.py:26-54 `jac`,
 // src/NPHM/models/fitting.py:99-106,167 - implicit differentiation of the Broyden root and loss.backward()), and DeepSDF
 // stacks of any width (NPM baseline 515 -> 1024 x 8, scripts/configs/npm.yaml:2-4).
 //
-// Arithmetic: kind::f16 MMAs with fp32 accumulation in TMEM, both operands split x = hi + lo in two fp16 terms, products
-// hi*hi + hi*lo + lo*hi (3 MMAs per k-step) - the same fp32-level scheme as the fused kernels.  A is read as fp32 from
-// global memory and split on the fly by eight "row" warps (thread = row of the 128-row tile x half of the k-step) into a 3- or
-// 4-stage shared-memory ring in UMMA K-major core-matrix order; W comes pre-split and pre-packed (pack_linear_kernel) through
-// bulk async copies; SS-form MMAs by one elected lane; the same eight warps run the epilogue (thread = accumulator row, every
-// other 16-column unit).  Operands are row-major or `blocked` ([128-row tile][feature][128]: what the fused ensemble forward
+// Arithmetic: fp16 MMAs with fp32 accumulation in registers, both operands split x = hi + lo in two fp16 terms, products
+// hi*hi + hi*lo + lo*hi (3 MMAs per k-step) - the same fp32-level scheme as the fused kernel.  A is read as fp32 from
+// global memory and split on the fly by eight "row" warps (thread = row of the 128-row tile x half of the k-step) into a
+// 4-stage shared-memory ring in K-major core-matrix order; W comes pre-split and pre-packed (pack_linear_kernel) through
+// bulk async copies.  The same eight warps are two warpgroups: each issues the SS-form wgmmas of its 64-row half of the tile
+// (16 output columns per instruction), parks its accumulators in a shared-memory tile after the last k-step, and all eight
+// run the epilogue from there (thread = row, every other 16-column unit).  Operands are row-major or `blocked` ([128-row tile][feature][128]: what the fused ensemble forward
 // writes for the fitting backward); launches can be batched over gridDim.z with per-entry operands and weight sets.
 //
 //   A1 [M x K1] fp32 row-major, optional A2 [M x K2] appended along K (skip connection `cat([h, x])`, the 1/sqrt(2) is folded
@@ -28,33 +29,39 @@ namespace nphm {
 namespace tcl {
 using namespace tc;
 
-constexpr int kMaxStages = 4;                   // operand ring: 4 stages, 3 when two CTAs are to share an SM (batched launches)
+constexpr int kMaxStages = 4;                   // operand ring: as many stages (2..4) as fit next to the accumulator tile
+constexpr int kMaxSmem = 227 * 1024;
 constexpr int kARing = 4;                       // fp32 staging ring of A (independent of the operand ring)
 constexpr int kRowWarps = 8;                      // two per 32-row quarter of the tile
-constexpr int kThreads = 32 * (kRowWarps + 2);
-constexpr int kMaxNt = 256;
+constexpr int kThreads = 32 * (kRowWarps + 1);
+constexpr int kMaxNt = 256;                     // accumulator columns held in registers: kMaxNt / 2 per thread
+constexpr int kChunks = kMaxNt / 16;            // 64 x 16 MMAs per k-step and warpgroup
 constexpr int kPackedStep = 2 * 128 * 32;       // bytes of one k-step of a packed A tile: 128 x 16 fp16 hi | 128 x 16 fp16 lo
 
 constexpr int kAPitch = 20;                      // floats per staged fp32 row (16 + 4: 80-byte pitch spreads the banks)
 constexpr int kADepth = 3;                       // k-steps of A kept in flight per thread (cp.async groups)
-// dynamic shared memory: [Ctl | stages x (a_hi 4 KB | a_lo 4 KB | b Nt*64) | a32 ring]
+// dynamic shared memory: [Ctl | stages x (a_hi 4 KB | a_lo 4 KB | b Nt*64) | a32 ring | accumulator tile 128 x (Nt + 4) fp32]
 #ifndef NPHM_TCL_MULSLOTS
 #define NPHM_TCL_MULSLOTS 3
 #endif
 constexpr int kMulSlots = NPHM_TCL_MULSLOTS;                     // ring of multiplier units (16 features x 128 rows fp32 = 8 KB) in the a32 space
 struct __align__(128) Ctl {
-    uint64_t a_full[kMaxStages], b_full[kMaxStages], empty[kMaxStages], d_ready;
+    uint64_t a_full[kMaxStages], b_full[kMaxStages], empty[kMaxStages];
     uint64_t mul_full[kMaxNt / 16], mul_empty[kMaxNt / 16];       // one single-use pair per 16-column unit (no phase bookkeeping)
-    uint32_t tmem_base;
 };
 constexpr int kCtlBytes = 512;
 static_assert(kMulSlots * 16 * 128 * 4 <= kARing * 128 * kAPitch * 4, "multiplier ring must fit the fp32 staging area of A");
 static_assert(sizeof(Ctl) <= kCtlBytes, "control block");
+static_assert(kCtlBytes + 2 * (2 * 128 * 32 + kMaxNt * 64) + kARing * 128 * kAPitch * 4 + 128 * (kMaxNt + 4) * 4 <= kMaxSmem, "smem");
 constexpr int kA32Bytes = kARing * 128 * kAPitch * 4;
 __host__ __device__ inline int stage_bytes(int Nt) { return 2 * 128 * 32 + Nt * 64; }
 constexpr int kMulRingBytes = kMulSlots * 16 * 128 * 4;
-// behind the operand stages: the fp32 staging ring of A, or (packed A: no staging) just the multiplier ring
-inline int smem_bytes(int Nt, int stages, bool packed_a) { return kCtlBytes + stages * stage_bytes(Nt) + (packed_a ? kMulRingBytes : kA32Bytes); }
+__host__ __device__ inline int dtile_pitch(int Nt) { return Nt + 4; }
+// behind the operand stages: the fp32 staging ring of A, or (packed A: no staging) just the multiplier ring; then the accumulators
+inline int smem_bytes(int Nt, int stages, bool packed_a)
+{
+    return kCtlBytes + stages * stage_bytes(Nt) + (packed_a ? kMulRingBytes : kA32Bytes) + 128 * dtile_pitch(Nt) * 4;
+}
 
 #ifdef NPHM_TCL_TRACE
 #ifndef NPHM_TCL_TRACE_NT
@@ -68,25 +75,13 @@ __device__ long long g_tcl_trace[16 * 64];
 #define TCL_EVT(cond, field, j) do { } while (0)
 #endif
 
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
-}
 
 // MODE and PACKED_C (packed output present) are compile-time: the epilogue is the longest part of a latency-bound layer and
 // loses ~a fifth of its instructions when the per-unit mode / layout tests disappear
 template <int MODE, bool PACKED_C>
-__global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearParams p)
+__global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearParams p)
 {
+    if (p.live && *p.live == 0) return;                 // uniform over the grid (Broyden: every sample of the search is frozen)
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     Ctl &sm = *reinterpret_cast<Ctl *>(smem_raw);
     const int kStages = p.stages;
@@ -96,30 +91,23 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
     auto st_a_lo = [&](int s) { return st0 + (size_t)s * st_bytes + 128 * 32; };
     auto st_b = [&](int s) { return st0 + (size_t)s * st_bytes + 2 * 128 * 32; };
     float (*a32)[128][kAPitch] = reinterpret_cast<float (*)[128][kAPitch]>(st0 + (size_t)kStages * st_bytes);
+    const bool packed_a = p.Ap != nullptr;
+    float *const dtile = reinterpret_cast<float *>(st0 + (size_t)kStages * st_bytes + (packed_a ? kMulRingBytes : kA32Bytes));
+    const int dp = dtile_pitch(p.Nt);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long row0 = (long long)blockIdx.x * 128;
     const int nt_idx = blockIdx.y;
     const int z = blockIdx.z;                             // batch entry: own A / C / Mul / row scale, weights of set(z)
     const int wset = z < 2 * p.w_pairs ? (z >> 1) : z - p.w_pairs;
     const int n0 = nt_idx * p.Nt;
-    const uint32_t tmem_cols = p.Nt <= 32 ? 32 : (p.Nt <= 64 ? 64 : (p.Nt <= 128 ? 128 : 256));
 
     TCL_EVT(threadIdx.x == 0, 10, 0);
     if (threadIdx.x == 0) {
-        for (int i = 0; i < kStages; ++i) { mbar_init(&sm.a_full[i], kRowWarps); mbar_init(&sm.b_full[i], 1); mbar_init(&sm.empty[i], 1); }
-        mbar_init(&sm.d_ready, 1);
+        for (int i = 0; i < kStages; ++i) { mbar_init(&sm.a_full[i], kRowWarps); mbar_init(&sm.b_full[i], 1); mbar_init(&sm.empty[i], 2); }
         for (int i = 0; i < kMaxNt / 16; ++i) { mbar_init(&sm.mul_full[i], 1); mbar_init(&sm.mul_empty[i], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kRowWarps + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32(&sm.tmem_base)), "r"(tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm.tmem_base;
     const int slab_bytes = p.Nt * 64;
     TCL_EVT(threadIdx.x == 0, 10, 1);
 
@@ -160,38 +148,13 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
             }
             fetch_mul(n_units);                            // the rest as the epilogue frees the slots
         }
-    } else if (warp == kRowWarps + 1) {
-        // ================================================================ MMA issuer (whole warp runs the loop, one lane issues)
-        const bool leader = elect_one();
-        const uint32_t idesc = make_idesc_m(128, p.Nt);
-        uint32_t ph = 0;
-        for (int j = 0, s = 0; j < p.ksteps; ++j) {
-            TCL_EVT(leader, 1, j);
-            if (!p.Ap) mbar_wait(&sm.a_full[s], ph);
-            TCL_EVT(leader, 2, j);
-            mbar_wait(&sm.b_full[s], ph);
-            TCL_EVT(leader, 3, j);
-            tc_fence_after();
-            if (leader) {
-                const uint64_t a_hi = make_desc(smem_u32(st_a_hi(s)), 128, 256), a_lo = make_desc(smem_u32(st_a_lo(s)), 128, 256);
-                const uint64_t b_hi = make_desc(smem_u32(st_b(s)), 128, 256);
-                const uint64_t b_lo = b_hi + (uint64_t)(p.Nt * 2);          // lo half: Nt * 32 bytes further
-                tc_mma_ss(tmem, a_hi, b_hi, idesc, j == 0 ? 0 : 1);
-                tc_mma_ss(tmem, a_hi, b_lo, idesc, 1);
-                tc_mma_ss(tmem, a_lo, b_hi, idesc, 1);
-                tc_commit(&sm.empty[s]);
-                if (j == p.ksteps - 1) tc_commit(&sm.d_ready);
-            }
-            __syncwarp();
-            if (++s == kStages) { s = 0; ph ^= 1; }
-        }
     } else {
-        // ================================================================ row warps: split A into the ring, then the epilogue
-        // Two warps per 32-row quarter of the tile (TMEM lanes 32 (warp % 4) ..): `half` = warp / 4 converts inputs
-        // [8 half, 8 half + 8) of every k-step and finishes the accumulator units u with u % 2 == half.  (With one warp per
-        // quarter the kernel was bound by the dependent-instruction latency of 2 resident warps per scheduler.)
-        const int t = threadIdx.x & 127;                  // row of the tile = TMEM lane
-        const int half = warp >> 2, q = warp & 3;
+        // ================================================================ row warps: split A into the ring, MMAs, epilogue
+        // Thread t of each warpgroup converts row t of the tile: `half` = warp / 4 converts inputs [8 half, 8 half + 8) of every
+        // k-step and finishes the accumulator units u with u % 2 == half.  As MMA issuers, warpgroup `half` owns rows
+        // [64 half, 64 half + 64) of the tile.
+        const int t = threadIdx.x & 127;                  // row of the tile (conversion and epilogue)
+        const int half = warp >> 2;
         const long long row = row0 + t;
         const bool row_ok = row < p.M;
         // row-major: element (row, k) at row * lda + k.  blocked: tiles of 128 rows, feature-major inside a tile,
@@ -239,7 +202,15 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
             asm volatile("cp.async.commit_group;" ::: "memory");
         };
         if (!p.Ap) for (int d = 0; d < kADepth; ++d) prefetch(d);
-        for (int j = 0, s = 0, ph = 0; j < (p.Ap ? 0 : p.ksteps); ++j) {
+        float acc[kChunks][8];
+#pragma unroll
+        for (int c = 0; c < kChunks; ++c)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[c][e] = 0.f;
+        const uint32_t a_rows = (uint32_t)half * 2048;    // this warpgroup's 64 rows: 8 row groups of 256 B further
+        int prev_s = 0;
+        for (int j = 0, s = 0, ph = 0; j < p.ksteps; ++j) {
+          if (!p.Ap) {
             const int sa = j % kARing;
             float cur[8];
             TCL_EVT(threadIdx.x == 0, 4, j);
@@ -265,15 +236,52 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
             __syncwarp();
             if (lane == 0) mbar_arrive(&sm.a_full[s]);
             TCL_EVT(threadIdx.x == 0, 8, j);
+            mbar_wait(&sm.a_full[s], ph);
+          }
+            mbar_wait(&sm.b_full[s], ph);
+            {
+                const uint64_t a_hi = make_desc(smem_u32(st_a_hi(s)) + a_rows, 128, 256);
+                const uint64_t a_lo = make_desc(smem_u32(st_a_lo(s)) + a_rows, 128, 256);
+                const uint32_t b = smem_u32(st_b(s));
+                wg_fence();
+#pragma unroll
+                for (int c = 0; c < kChunks; ++c) {
+                    if (16 * c < p.Nt) {
+                        const uint64_t b_hi = make_desc(b + 512 * c, 128, 256), b_lo = make_desc(b + 512 * c + p.Nt * 32, 128, 256);
+                        wgmma_ss_n16(acc[c], a_hi, b_hi, 1);
+                        wgmma_ss_n16(acc[c], a_hi, b_lo, 1);
+                        wgmma_ss_n16(acc[c], a_lo, b_hi, 1);
+                    }
+                }
+                wg_commit();
+                wg_wait<1>();                              // k-step j - 1 is complete: its stage may be refilled
+            }
+            if (j > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&sm.empty[prev_s]);
+            prev_s = s;
             if (++s == kStages) { s = 0; ph ^= 1; }
         }
+        wg_wait<0>();
+#pragma unroll
+        for (int c = 0; c < kChunks; ++c) wg_reg_fence(acc[c]);
         asm volatile("cp.async.wait_group 0;" ::: "memory");
+        {
+            // accumulators -> shared tile [row][column] (fragment rows 16 (warp % 4) + lane / 4 (+ 8) of this warpgroup's half)
+            const int fr = 64 * half + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+            for (int c = 0; c < kChunks; ++c) {
+                if (16 * c < p.Nt) {
+                    float *d0 = dtile + (size_t)fr * dp + 16 * c + fc, *d1 = d0 + 8 * dp;
+                    *reinterpret_cast<float2 *>(d0) = make_float2(acc[c][0], acc[c][1]);
+                    *reinterpret_cast<float2 *>(d1) = make_float2(acc[c][2], acc[c][3]);
+                    *reinterpret_cast<float2 *>(d0 + 8) = make_float2(acc[c][4], acc[c][5]);
+                    *reinterpret_cast<float2 *>(d1 + 8) = make_float2(acc[c][6], acc[c][7]);
+                }
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(32 * kRowWarps) : "memory");   // the row warps only
+        }
         // ---------------- epilogue: thread = row, 16 accumulator columns at a time (units of this warp's parity)
-        TCL_EVT(threadIdx.x == 0, 9, 0);
-        mbar_wait(&sm.d_ready, 0);
-        tc_fence_after();
         TCL_EVT(threadIdx.x == 0, 9, 1);
-        const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16);
+        const float *drow = dtile + (size_t)t * dp;
         const float *bias = p.bias ? p.bias + (size_t)(row_ok ? row / p.rows_per_bias : 0) * p.ldb : nullptr;
         const bool mul_blk = p.blocked || p.mul_blocked;
         const long long mrow = row_ok ? row / p.mul_div : 0;                     // multiplier row (tangent passes: 3 rows per point)
@@ -295,8 +303,6 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
         // FULL: all 16 columns of the unit exist (no per-column guards, constant address offsets)
         auto finish_unit = [&](int c0, auto full_c) {
             constexpr bool FULL = decltype(full_c)::value;
-            uint32_t r[16];
-            tc_ld16(tl + c0, r);
             float aux[16];
             const int unit = c0 >> 4;
             if (unit_in_ring(unit)) {
@@ -323,13 +329,11 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
                 }
             }
             TCL_EVT(threadIdx.x == 0, 11, c0 >> 4);
-            tc_wait_ld();
-            TCL_EVT(threadIdx.x == 0, 12, c0 >> 4);
             if (!row_ok) return;
             float o[16], dv[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) {
-                float x = __uint_as_float(r[e]);
+                float x = drow[c0 + e];
                 dv[e] = 0.f;
                 if (!FULL && n0 + c0 + e >= p.N) {
                     // beyond the layer's width: zero, or the columns appended for the next layer (`cat([h, xyz])`, tangent seeds)
@@ -404,15 +408,15 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
                     if (FULL || n0 + c0 + e < p.N) crow[e] = o[e];
             }
             if (p.Dv && !p.dv_blocked) {
-                float *drow = p.Dv + (size_t)row * p.lddv + n0 + c0;
+                float *dvrow = p.Dv + (size_t)row * p.lddv + n0 + c0;
                 if (FULL && d_vec) {
 #pragma unroll
                     for (int i = 0; i < 4; ++i)
-                        reinterpret_cast<float4 *>(drow)[i] = make_float4(dv[4 * i], dv[4 * i + 1], dv[4 * i + 2], dv[4 * i + 3]);
+                        reinterpret_cast<float4 *>(dvrow)[i] = make_float4(dv[4 * i], dv[4 * i + 1], dv[4 * i + 2], dv[4 * i + 3]);
                 } else {
 #pragma unroll
                     for (int e = 0; e < 16; ++e)
-                        if (FULL || n0 + c0 + e < p.N) drow[e] = dv[e];
+                        if (FULL || n0 + c0 + e < p.N) dvrow[e] = dv[e];
                 }
             }
         };
@@ -423,11 +427,6 @@ __global__ void __launch_bounds__(kThreads, 2) linear_tc_kernel(const LinearPara
         TCL_EVT(threadIdx.x == 0, 9, 2);
     }
 
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == kRowWarps + 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
 }
 
 // W [rows x ldw] fp32 (reference layout [out][in]) -> slabs.  B[n][k] = scale * (transpose ? W[k0 + k][n0w + n] : W[n0w + n][k0 + k])
@@ -514,21 +513,16 @@ int launch_linear(const PackedLinear &w, LinearParams p, cudaStream_t stream)
     p.N = w.N; p.Nt = w.Nt; p.ksteps = w.ksteps;
     if (p.rows_per_bias <= 0) p.rows_per_bias = p.M;
     if (p.mul_div <= 0) p.mul_div = 1;
-    // three operand stages leave room for two CTAs per SM (the epilogue of one overlaps the main loop of the other); wide tiles
-    // and single launches of few tiles keep four
-    // two CTAs per SM when there are enough tiles (the epilogue of one overlaps the main loop of the other): as many operand
-    // stages as fit in half of the shared memory, at least three; otherwise four stages, one CTA per SM
     const bool packed_a = p.Ap != nullptr;
-    const bool many = ceil_div(p.M, 128) * w.n_tiles * p.batch > 148;
     p.stages = kMaxStages;
-    if (many && smem_bytes(p.Nt, kMaxStages, packed_a) > 112 * 1024 && smem_bytes(p.Nt, 3, packed_a) <= 112 * 1024) p.stages = 3;
+    while (p.stages > 2 && smem_bytes(p.Nt, p.stages, packed_a) > kMaxSmem) --p.stages;
     const int smem = smem_bytes(p.Nt, p.stages, packed_a);
     using Kernel = void (*)(const LinearParams);
     const bool pc = p.Cp != nullptr;
     Kernel kern = p.mode == kModeMult       ? (pc ? (Kernel)linear_tc_kernel<kModeMult, true> : (Kernel)linear_tc_kernel<kModeMult, false>)
                   : p.mode == kModeSoftplus ? (pc ? (Kernel)linear_tc_kernel<kModeSoftplus, true> : (Kernel)linear_tc_kernel<kModeSoftplus, false>)
                                             : (pc ? (Kernel)linear_tc_kernel<kModeLinear, true> : (Kernel)linear_tc_kernel<kModeLinear, false>);
-    NPHM_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(kMaxNt, kMaxStages, false)));
+    NPHM_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
     dim3 grid((unsigned)ceil_div(p.M, 128), (unsigned)w.n_tiles, (unsigned)p.batch);
     kern<<<grid, kThreads, smem, stream>>>(p);
     NPHM_CUDA_CHECK(cudaGetLastError());

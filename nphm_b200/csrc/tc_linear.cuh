@@ -1,4 +1,4 @@
-// Generic fp32-accurate tcgen05 linear layer (tc_linear.cu): parameters, packed weights, launch.
+// Generic fp32-accurate wgmma linear layer (tc_linear.cu): parameters, packed weights, launch.
 #pragma once
 #include "engine.cuh"
 #include "tc_common.cuh"
@@ -20,7 +20,7 @@ struct LinearParams {
     const float *Mul = nullptr; int ldmul = 0; long long mul_div = 1;        // MULT: C = t * Mul[row / mul_div][n]
     const float *row_scale = nullptr;                        // MULT: additional factor row_scale[row]
     int mul_blocked = 0, dv_blocked = 0;                     // Mul / Dv alone in the blocked layout (see `blocked`)
-    // operand-ready ("packed") activations: per 128-row tile and k-step 8 KB = [128 x 16 fp16 hi | 128 x 16 fp16 lo] in UMMA core-
+    // operand-ready ("packed") activations: per 128-row tile and k-step 8 KB = [128 x 16 fp16 hi | 128 x 16 fp16 lo] in K-major core-
     // matrix order.  Cp: the epilogue writes its output split like that (unit u of 16 columns = k-step u of the next layer), so
     // the next launch takes it as Ap with one bulk copy per k-step and no conversion work in its main loop.
     const uint8_t *Ap = nullptr; int a_ksteps = 0; long long sAp = 0;        // replaces A1 / A2; 16 a_ksteps = packed K
@@ -34,6 +34,7 @@ struct LinearParams {
     // batched launch (gridDim.z): entry z reads A1 + z sA1, Mul + z sMul, row_scale + z sRow, writes C + z sC (strides in floats)
     // and uses weight set z/2 for z < 2 w_pairs, z - w_pairs beyond (the mirrored pairs of the ensemble share weights)
     int batch = 1; long long sA1 = 0, sC = 0, sMul = 0, sRow = 0; int w_pairs = 0;
+    const int *live = nullptr;                               // optional device counter: the launch does nothing when *live == 0
     // filled by launch_linear from the packed weights
     const uint8_t *W = nullptr; long long w_stride = 0; int N = 0, Nt = 0, ksteps = 0, stages = 0;
 };

@@ -10,7 +10,7 @@ Same class names, constructor signatures, parameter names/shapes (``state_dict``
 ``strict=True``), attributes and return values.  Two execution paths:
 
   * **fused**  - CUDA tensors, autograd not recording: one call into ``libnphm_b200.so``
-    (hand-written sm_100a kernels, see ``nphm_b200/csrc``).  This is the product path; it raises
+    (hand-written sm_90a kernels, see ``nphm_b200/csrc``).  This is the product path; it raises
     if the native library is missing, it never falls back.
   * **composite** - anything that needs autograd (training, double backward for the eikonal /
     normal losses of ``scripts/training``) or runs on CPU tensors (host-logic tests): stock

@@ -8,7 +8,7 @@ Reference interface (file:line):
 Parameter names (``lin{i}.weight/bias``, ``compressor.0.*``, ``defDeepSDF.lin{i}.*``) and
 constructor signatures are those of the reference so checkpoints load with ``strict=True``.
 As in :mod:`.EnsembledDeepSDF`, CUDA no-grad calls with a per-query-constant condition run in
-the native sm_100a MLP kernel; everything else uses a PyTorch composite that keeps autograd.
+the native sm_90a MLP path; everything else uses a PyTorch composite that keeps autograd.
 """
 from __future__ import annotations
 

@@ -255,7 +255,7 @@ class JointFitter:
         self.t = 0
         self.anchors = None
         # Broyden early exit (the reference leaves its loop when nobody is active) costs a host sync every third step; without it
-        # an iteration is a pure launch sequence.  Default: on for small batches is not worth a sync on a B200 - off.
+        # an iteration is a pure launch sequence.  Default: on for small batches is not worth a sync - off.
         self.early_exit = bool(int(os.environ.get('NPHM_BROYDEN_EARLY_EXIT', '0')))
 
     def step(self, obs, obs_idx, lambdas, clamp, lr, apply_update: bool = True):

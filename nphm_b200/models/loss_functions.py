@@ -9,7 +9,7 @@ ensemble - ``anchors``, ``symm_dist``, ``middle_dist``).  Two ways to get the SD
 
   * **native** (no autograd graph: validation, monitoring, loss curves of a frozen model): one call per batch element and
     point set into ``nphm_ensemble_backward_inputs`` with an upstream gradient of ones - a point's SDF depends on its own
-    coordinates only, so that vector-Jacobian product IS the per-point spatial gradient (tcgen05 forward and backward,
+    coordinates only, so that vector-Jacobian product IS the per-point spatial gradient (tensor-core forward and backward,
     ``csrc/fit.cu``).  Used when autograd is not recording (the reference cannot evaluate these losses at all under
     ``torch.no_grad()``: its ``gradient`` needs a graph) or with ``native=True``; training-mode forward only.
   * **composite** (training): the decoder's autograd path and ``diff_operators.gradient`` with ``create_graph=True`` -

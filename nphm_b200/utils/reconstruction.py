@@ -2,7 +2,7 @@
 
   * ``create_grid_points_from_bounds``  src/NPHM/utils/reconstruction.py:5-20
   * ``mesh_from_logits``                src/NPHM/utils/reconstruction.py:22-37  (mcubes.marching_cubes -> the
-    sm_100a marching-cubes kernels of ``nphm_b200/csrc/marching_cubes.cu``)
+    sm_90a marching-cubes kernels of ``nphm_b200/csrc/marching_cubes.cu``)
 """
 from __future__ import annotations
 

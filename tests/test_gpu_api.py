@@ -53,7 +53,7 @@ def test_empty_and_tiny_queries(cuda_device):
 
 
 def test_unsupported_configuration_uses_ffma_and_tc_request_fails(cuda_device):
-    """A non-NPHM ensemble shape (hidden 160, 10 anchors) runs on the general FFMA kernel; forcing the tcgen05 kernel
+    """A non-NPHM ensemble shape (hidden 160, 10 anchors) runs on the general FFMA kernel; forcing the tensor-core kernel
     reports NPHM_ERR_UNSUPPORTED instead of silently doing something else."""
     from nphm_b200 import _native
     from nphm_b200.models.EnsembledDeepSDF import FastEnsembleDeepSDFMirrored

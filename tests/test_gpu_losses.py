@@ -1,51 +1,30 @@
 """SURVEY.md 8f-3: the identity-space training losses (reference loss_functions.py:20-110) evaluated natively - SDF values and
 spatial gradients from nphm_ensemble_backward_inputs, no autograd graph - against the UNMODIFIED reference function running on
-its own modules with autograd, same weights, same batch, on the GPU."""
-import numpy as np
+its own modules with autograd, same weights, same batch (its values: tests/golden/losses.npz, make_golden_losses.py)."""
 import pytest
 import torch
 
-from conftest import make_ensemble
-from oracle import ref_loader
+from conftest import load_golden, make_ensemble
 
 pytestmark = pytest.mark.gpu
-
-
-def _batch(rng, B, n, dev):
-    def pts(scale):
-        return torch.from_numpy((rng.randn(B, n, 3) * scale + np.array([0.0, 0.05, -0.1])).astype(np.float32)).to(dev)
-
-    def unit():
-        v = rng.randn(B, n, 3).astype(np.float32)
-        return torch.from_numpy(v / np.linalg.norm(v, axis=-1, keepdims=True)).to(dev)
-    return {'points_face': pts(0.12), 'points_non_face': pts(0.2), 'sup_grad_near': pts(0.15), 'sup_grad_far': pts(0.4),
-            'normals_face': unit(), 'normals_non_face': unit(),
-            'gt_anchors': torch.from_numpy((rng.randn(B, 39, 3) * 0.1).astype(np.float32)).to(dev)}
+KEYS = ('points_face', 'points_non_face', 'sup_grad_near', 'sup_grad_far', 'normals_face', 'normals_non_face', 'gt_anchors')
 
 
 def test_native_training_losses_match_the_reference_function(cuda_device):
-    if not ref_loader.available():
-        pytest.skip('reference modules (oracle/_ref) not available')
-    ns = ref_loader.load()
-    if ns.loss_functions is None:
-        pytest.skip('oracle/_ref was built without loss_functions.py')
     from nphm_b200.models import loss_functions as L
-    ref = ref_loader.make_ensemble(ns, 0, cuda_device).train()
+    g = load_golden('losses.npz')
     ours = make_ensemble(0, device=cuda_device).train()
-    ours.load_state_dict(ref.state_dict(), strict=True)
-    rng = np.random.RandomState(5)
-    B, n = 3, 700
-    batch = _batch(rng, B, n, cuda_device)
-    cond = torch.from_numpy((rng.randn(B, 1, 1344) * 0.3).astype(np.float32)).to(cuda_device)
-    want = ns.loss_functions.actual_compute_loss(batch, ref, cond)
+    batch = {k: torch.from_numpy(g['gpu_' + k]).to(cuda_device) for k in KEYS}
+    cond = torch.from_numpy(g['gpu_cond']).to(cuda_device)
+    want = dict(zip(g['gpu_loss_names'], g['gpu_loss_values']))
     with torch.no_grad():
         got = L.actual_compute_loss(batch, ours, cond)                      # native: no graph
     got_graph = L.actual_compute_loss(batch, ours, cond)                    # composite: autograd, what training uses
     assert set(got) == set(want) == set(got_graph)
     for k, w in want.items():
-        w = float(w.detach())
-        for name, g in (('native', got[k]), ('composite', got_graph[k])):
-            g = float(g.detach())
-            assert abs(g - w) <= 2e-5 * max(1.0, abs(w)), (k, name, g, w)
+        w = float(w)
+        for name, gv in (('native', got[k]), ('composite', got_graph[k])):
+            gv = float(gv.detach())
+            assert abs(gv - w) <= 2e-5 * max(1.0, abs(w)), (k, name, gv, w)
         print('%-12s reference %.7f  native %.7f  composite %.7f' % (k, w, float(got[k].detach()), float(got_graph[k].detach())))
     assert not got['grad'].requires_grad and got_graph['grad'].requires_grad

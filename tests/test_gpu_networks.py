@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA kernels, called through the C ABI
+"""GPU parity tests (run with -m gpu on an H100): the CUDA kernels, called through the C ABI
 (nphm_b200._native -> libnphm_b200.so), against the oracle and the golden vectors of the reference.
 Tolerance 1e-5 abs fp32 (north_star) - the kernels are expected to be ~1e-7."""
 import numpy as np
@@ -163,7 +163,7 @@ def test_deform_mesh_dropin(cuda_device):
 
 
 def test_tensor_core_operand_plumbing(cuda_device):
-    """D = A * B^T through the tcgen05 operand path (fp16 hi/lo split, A in TMEM, B slabs in shared memory)."""
+    """D = A * B^T through the wgmma operand path (fp16 hi/lo split, A in registers, B slabs in shared memory)."""
     import ctypes
     from nphm_b200 import _native
     lib = _native.lib()
@@ -207,7 +207,7 @@ def test_pruned_kernel_is_opt_in_and_within_its_error_bound(cuda_device):
 
 
 def test_deformation_tensor_core_kernel(cuda_device):
-    """tcgen05 MLP kernel (M=64 tiles, A in shared memory) against the reference golden, the oracle and the FFMA kernel."""
+    """Tensor-core MLP path (layer chain on the wgmma linear layer) against the reference golden, the oracle and the FFMA kernel."""
     d = load_golden('deform.npz')
     dfn = make_deformation(cuda_device)
     eng = dfn.defDeepSDF.engine()
@@ -233,6 +233,22 @@ def test_deformation_tensor_core_kernel(cuda_device):
             assert np.abs(got[b] - O.mlp_forward(mp, x[b], c[b])).max() < TOL, n
 
 
+def test_deformation_forward_streams_rows_in_chunks(cuda_device):
+    """The tensor-core forward runs in bounded chunks of 65 536 rows: queries longer than a chunk (ragged last chunk) and
+    several short queries per chunk give what the FFMA kernel gives on the whole call."""
+    dfn = make_deformation(cuda_device)
+    eng = dfn.defDeepSDF.engine()
+    rng = np.random.RandomState(4)
+    for B, n in ((2, 70001), (3, 30000)):
+        x = torch.from_numpy((rng.rand(B, n, 3) - 0.5).astype(np.float32)).to(cuda_device)
+        c = torch.from_numpy((rng.randn(B, 232) * 0.3).astype(np.float32)).to(cuda_device)
+        tc = eng.query(x, c, impl='tc')
+        simt = eng.query(x, c, impl='simt')
+        err = (tc - simt).abs().max().item()
+        print('chunked deformation forward B=%d n=%d: max abs diff vs FFMA kernel %.3g' % (B, n, err))
+        assert err < 2e-6
+
+
 # ---------------------------------------------------------------------------------------------- layer chain (tc_linear)
 def _chain_case(kind, device):
     from nphm_b200.models.deepSDF import DeepSDF
@@ -247,7 +263,7 @@ def _chain_case(kind, device):
 
 @pytest.mark.parametrize('kind', ['deform', 'npm', 'small'])
 def test_layer_chain_forward_jacobian_adjoint_match_autograd(cuda_device, kind):
-    """nphm_mlp_query_layers / nphm_mlp_jacobian / nphm_mlp_backward_inputs (generic tcgen05 linear layer) against the
+    """nphm_mlp_query_layers / nphm_mlp_jacobian / nphm_mlp_backward_inputs (generic wgmma linear layer) against the
     reference-pinned composite module under torch autograd: values <= 1e-5, Jacobian and gradients <= 2e-4 relative (5e-4 for
     the 8 x 1024 NPM stack, whose fp32 autograd reference itself carries that much round-off)."""
     net, lat_dim, out_dim = _chain_case(kind, cuda_device)

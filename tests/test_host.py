@@ -221,8 +221,12 @@ def test_mc_tables_identical_in_oracle_and_product():
 
 
 def test_bench_reference_arm_contract(tmp_path):
-    """`bench.py --impl reference`: rank 0 prints one JSON line with the contract's keys, other ranks exit 0 silently."""
+    """`bench.py --impl reference`: rank 0 prints one JSON line with the contract's keys, other ranks exit 0 silently.
+    The arm runs the reference's own modules, so it needs oracle/_ref (oracle/make_ref.py) or a reference checkout."""
     import json, os, subprocess, sys
+    from oracle import ref_loader
+    if not ref_loader.available():
+        pytest.skip('reference modules (oracle/_ref) not available')
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     cmd = [sys.executable, os.path.join(root, 'bench.py'), '--impl', 'reference', '--steps', '1', '--warmup', '0', '--res', '32',
            '--cpu-sample-chunks', '1']

@@ -1,40 +1,26 @@
 """CPU check of the composite (autograd) path of nphm_b200.models.loss_functions against the reference's
-actual_compute_loss (loss_functions.py:20-110) - same weights, same batch.  The native path needs a GPU (test_gpu_losses.py)."""
+actual_compute_loss (loss_functions.py:20-110) - same weights, same batch; the reference's values are stored in
+tests/golden/losses.npz (make_golden_losses.py).  The native path needs a GPU (test_gpu_losses.py)."""
 import numpy as np
-import pytest
 import torch
 
-from conftest import make_ensemble
-from oracle import ref_loader
+from conftest import load_golden, make_ensemble
+
+KEYS = ('points_face', 'points_non_face', 'sup_grad_near', 'sup_grad_far', 'normals_face', 'normals_non_face', 'gt_anchors')
 
 
 def test_composite_training_losses_match_the_reference_function_on_cpu():
-    if not ref_loader.available():
-        pytest.skip('reference modules (oracle/_ref) not available')
-    ns = ref_loader.load()
-    if ns.loss_functions is None:
-        pytest.skip('oracle/_ref was built without loss_functions.py')
     from nphm_b200.models import loss_functions as L
-    ref = ref_loader.make_ensemble(ns, 0, 'cpu').train()
+    g = load_golden('losses.npz')
     ours = make_ensemble(0).train()
-    ours.load_state_dict(ref.state_dict(), strict=True)
-    rng = np.random.RandomState(11)
-    B, n = 2, 40
-
-    def pts(scale):
-        return torch.from_numpy((rng.randn(B, n, 3) * scale).astype(np.float32))
-    batch = {'points_face': pts(0.12), 'points_non_face': pts(0.2), 'sup_grad_near': pts(0.15), 'sup_grad_far': pts(0.4),
-             'normals_face': pts(1.0), 'normals_non_face': pts(1.0), 'gt_anchors': pts(0.1)[:, :39]}
-    batch['gt_anchors'] = torch.from_numpy((rng.randn(B, 39, 3) * 0.1).astype(np.float32))
-    cond = torch.from_numpy((rng.randn(B, 1, 1344) * 0.3).astype(np.float32)).requires_grad_()
-    want = ns.loss_functions.actual_compute_loss(batch, ref, cond)
+    batch = {k: torch.from_numpy(g['cpu_' + k]) for k in KEYS}
+    cond = torch.from_numpy(g['cpu_cond']).requires_grad_()
+    want = dict(zip(g['cpu_loss_names'], g['cpu_loss_values']))
     got = L.actual_compute_loss(batch, ours, cond)
     assert set(got) == set(want)
     for k in want:
-        assert abs(float(got[k].detach()) - float(want[k].detach())) <= 1e-5 * max(1.0, abs(float(want[k].detach()))), (k, float(got[k].detach()), float(want[k].detach()))
+        assert abs(float(got[k].detach()) - want[k]) <= 1e-5 * max(1.0, abs(want[k])), (k, float(got[k].detach()), want[k])
     # the graph reaches the weights through the spatial gradient (double backward), like the reference's
-    total_w = sum(want[k] for k in ('surf_sdf', 'normals', 'grad'))
     total_g = sum(got[k] for k in ('surf_sdf', 'normals', 'grad'))
-    gw = torch.autograd.grad(total_w, ref.ensembled_deep_sdf.lin1.weight)[0]
-    gg = torch.autograd.grad(total_g, ours.ensembled_deep_sdf.lin1.weight)[0]
-    assert float((gw - gg).abs().max()) <= 1e-4 * max(1e-6, float(gw.abs().max()))
+    gg = torch.autograd.grad(total_g, ours.ensembled_deep_sdf.lin1.weight)[0].reshape(-1).numpy()
+    assert float(np.abs(gg[g['cpu_lin1_grad_idx']] - g['cpu_lin1_grad']).max()) <= 1e-4 * max(1e-6, float(g['cpu_lin1_grad_absmax']))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Secondary paths of the hot path on one B200: deformation-field query (config 3 ingredient), identity fitting
+"""Secondary paths of the hot path on one GPU: deformation-field query (config 3 ingredient), identity fitting
 iterations/s (config 4 ingredient).  Prints one JSON line.   python tools/bench_aux.py [--res 128]"""
 import argparse, json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,5 +1,6 @@
-import sys, time, ctypes
-sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests')
+import os, sys, time, ctypes
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import torch, numpy as np
 from nphm_b200 import _native
 from conftest import sphere_volume
