@@ -231,6 +231,29 @@ int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const float *con
 int nphm_mlp_inverse_jacobian(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
                               float *out_dev, float *jinv_dev, void *stream);
 
+/* ---- training (first order): the stage-2 loss of the reference (src/NPHM/models/loss_functions.py:282-322, stepped by
+ * training_corresp.py:154-176) differentiated to the weights on the tensor cores.  A forward keeps everything its backward
+ * needs in a caller-owned device workspace, so several forwards may be alive at once; the backward reads nothing from the
+ * handle except the packed weights.
+ * Per-row condition noise: cond_noise_dev [q][n][noise_dim] is added to the leading noise_dim condition columns of every
+ * point (the train-mode `compressed += randn(...) / 200` of deepSDF.py:220-221); noise_dim = 0: none. */
+/* bytes of the workspace of one nphm_mlp_train_forward call (-1: bad arguments) */
+long long nphm_mlp_train_workspace_bytes(const nphm_mlp *h, int n_queries, long long n_points, int noise_dim);
+/* value pass of DeepSDF.forward (deepSDF.py:64-89): out_dev [q][n][out_dim]; activations, their derivatives, the staged
+ * [xyz | noise] rows and a copy of cond_dev [q][lat_dim] go to workspace_dev (nphm_mlp_train_workspace_bytes bytes). */
+int nphm_mlp_train_forward(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, const float *cond_noise_dev, int noise_dim,
+                           int n_queries, long long n_points, float *out_dev, void *workspace_dev, void *stream);
+/* what autograd's backward of that forward gives for the upstream gradient grad_out_dev [q][n][out_dim]:
+ * grad_w_dev[l] / grad_b_dev[l] in the state_dict layout of lin{l}.weight / bias (overwritten; the arrays or entries may be
+ * NULL = not needed), grad_cond_dev [q][lat_dim] (summed over the points of a query), grad_xyz_dev [q][n][3] (may be NULL).
+ * Deterministic: the same inputs give bitwise-identical gradients.  workspace_bytes / noise_dim / n_queries / n_points: the
+ * size of the workspace and the shape of the forward that filled it; rejected (NPHM_ERR_INVALID) when the size does not match
+ * that shape on this network.  Nothing is read back from the device: the call does not wait for the stream. */
+int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, const void *workspace_dev, long long workspace_bytes,
+                            int noise_dim, int n_queries, long long n_points,
+                            float *const *grad_w_dev, float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev,
+                            void *stream);
+
 /* anchors_dev [n_queries][n_loc][3] = mlp_pos(z_glob) + mean anchors (reference src/NPHM/models/EnsembledDeepSDF.py:228-229)
  * without evaluating the ensemble - what the fitters read from `decoder(zeros(1,1,3), lat)[1]` (fitting.py:59, :211). */
 int nphm_ensemble_anchors(nphm_ensemble *h, const float *latents_dev, int n_queries, float *anchors_dev, void *stream);

@@ -33,6 +33,7 @@ EXPORTED_SYMBOLS = (
     'nphm_fit_workspace_bytes', 'nphm_fit_identity_step', 'nphm_fit_surface_grad', 'nphm_fit_apply_gradient',
     'nphm_ensemble_backward_inputs', 'nphm_ensemble_anchors',
     'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
+    'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
 )
 
 
@@ -149,6 +150,12 @@ def lib() -> ctypes.CDLL:
                                           c_float, c_float, c_float, c_void_p, c_void_p, POINTER(c_int), c_void_p,
                                           c_void_p]
     L.nphm_nearest_neighbors.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p]
+    L.nphm_mlp_train_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong, c_int]
+    L.nphm_mlp_train_workspace_bytes.restype = c_longlong
+    L.nphm_mlp_train_forward.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_longlong, c_void_p, c_void_p,
+                                         c_void_p]
+    L.nphm_mlp_train_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_longlong, POINTER(c_void_p),
+                                          POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -353,6 +360,8 @@ class MlpEngine(_Versioned):
         # (csrc/tc_linear.cu, any width - e.g. the NPM baseline 515 -> 1024 x 8); the fp32 FFMA kernel is kept for impl='simt'
         self.fused_shape = (hidden == 512 and self.n_lin == 7 and module.lat_dim == 232 and module.out_dim_net == 3)
         self.simt_ok = hidden <= 880
+        self.lat_dim = module.lat_dim
+        self.layer_shapes = [tuple(getattr(module, 'lin%d' % i).weight.shape) for i in range(self.n_lin)]
         self._sig = None
 
     def __del__(self):
@@ -449,6 +458,47 @@ class MlpEngine(_Versioned):
                                                  g.data_ptr(), g_cond.data_ptr(), _ptr(g_xyz), _stream_ptr(dev)),
                   'nphm_mlp_backward_inputs')
         return g_cond, g_xyz
+
+    # ------------------------------------------------------------ training (first order)
+    def train_forward(self, xyz: torch.Tensor, cond: torch.Tensor, noise: Optional[torch.Tensor] = None):
+        """Value pass that keeps what the backward needs (nphm_mlp_train_forward): xyz B x N x 3, cond B x lat_dim, noise
+        B x N x noise_dim (added to the leading condition columns of every point) or None.  Returns ``(out B x N x out_dim,
+        workspace)``; the workspace (a uint8 CUDA tensor) belongs to the caller and goes to :meth:`train_backward` with the
+        same ``noise_dim``."""
+        B, N, _ = xyz.shape
+        dev = xyz.device
+        xyz = _f32c(xyz)
+        cond = _f32c(cond).to(dev)
+        nd = 0 if noise is None else int(noise.shape[-1])
+        noise = None if noise is None else _f32c(noise).reshape(B, N, nd)
+        out = torch.empty(B, N, self.out_dim, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            nbytes = int(lib().nphm_mlp_train_workspace_bytes(self._h, B, N, nd))
+            if nbytes < 0:
+                check(-1, 'nphm_mlp_train_workspace_bytes')
+            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            check(lib().nphm_mlp_train_forward(self._h, xyz.data_ptr(), cond.data_ptr(), _ptr(noise), nd, B, N, out.data_ptr(),
+                                               ws.data_ptr(), _stream_ptr(dev)), 'nphm_mlp_train_forward')
+        return out, ws
+
+    def train_backward(self, ws: torch.Tensor, grad_out: torch.Tensor, noise_dim: int = 0, weights: bool = True,
+                       biases: bool = True, want_cond: bool = True, want_xyz: bool = False):
+        """Backward of :meth:`train_forward` (nphm_mlp_train_backward) for grad_out B x N x out_dim; ``noise_dim``: the width of
+        the noise that forward took (0: none).  Returns
+        ``(weight grads [lin{l}.weight shape] | None, bias grads | None, d/d cond B x lat_dim | None, d/d xyz B x N x 3 | None)``."""
+        B, N, _ = grad_out.shape
+        dev = grad_out.device
+        g = _f32c(grad_out)
+        shapes = self.layer_shapes
+        gw = [torch.empty(s, device=dev, dtype=torch.float32) for s in shapes] if weights else None
+        gb = [torch.empty(s[0], device=dev, dtype=torch.float32) for s in shapes] if biases else None
+        g_cond = torch.empty(B, self.lat_dim, device=dev, dtype=torch.float32) if want_cond else None
+        g_xyz = torch.empty(B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None
+        with torch.cuda.device(dev):
+            check(lib().nphm_mlp_train_backward(self._h, g.data_ptr(), ws.data_ptr(), ws.numel(), int(noise_dim), B, N,
+                                                _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
+                                                _ptr(g_cond), _ptr(g_xyz), _stream_ptr(dev)), 'nphm_mlp_train_backward')
+        return gw, gb, g_cond, g_xyz
 
     def broyden_search(self, obs: torch.Tensor, cond: torch.Tensor, x_init: torch.Tensor, J_inv_init: torch.Tensor,
                        max_steps: int = 15, cvg_thresh: float = 1e-6, dvg_thresh: float = 0.2, eps: float = 1e-6,

@@ -10,6 +10,7 @@
 // network in the joint fitter.  The condition is constant over the points of a query, so its part of layers 0 and `skip` is
 // folded into per-query constants (simt.cu: cvec) and its gradient only needs the per-query column sums of d_0 and d_skip.
 #include "tc_linear.cuh"
+#include "tc_wgrad.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cuda_fp16.h>
@@ -148,6 +149,12 @@ struct MlpChain {
     int ld[kMaxLayers];
     long long value_rows = 0;                 // rows of the last value pass that kept the activation derivatives
     bool have_deriv = false;
+    // training (nphm_mlp_train_forward / _backward): layers 0, skip - 1 and skip take `train_nd` per-row condition columns
+    // more (layer 0: [xyz | noise], the skip layer: [h | xyz | noise] / sqrt2, the layer before it appends them); packed on
+    // first use after every weight load.  Scratch of the backward: adjoints, GEMM partials, per-query column sums.
+    tcl::PackedLinear tfwd[kMaxLayers];
+    int train_nd = -1;
+    DeviceBuffer Dl, wg_partials, gscale, qsums, qsums0, qsumss, xs_tmp;
 };
 
 static int pad4(int n) { return (n + 3) / 4 * 4; }
@@ -180,6 +187,7 @@ int chain_pack(nphm_mlp *h, cudaStream_t stream)
         (rc = c.adj_xs.pack(h->weights.W[s.skip].as<float>(), s.in_total[s.skip], 3, s.N[s.skip], s.N[s.skip - 1], 0, true,
                             chain::kInvSqrt2, stream))) return rc;
     c.packed = true;
+    c.train_nd = -1;
     return NPHM_OK;
 }
 
@@ -470,5 +478,366 @@ extern "C" int nphm_mlp_inverse_jacobian(nphm_mlp *h, const float *xyz_dev, cons
     const long long M = (long long)n_queries * n_points;
     chain::inverse_plus_identity_kernel<<<(unsigned)ceil_div(M, 256), 256, 0, static_cast<cudaStream_t>(stream_)>>>(jinv_dev, M);
     NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+// ================================================================================================ training
+// One step of the stage-2 loss (reference scripts/training/train_corresp.py -> TrainerAutoDecoder.train_step,
+// src/NPHM/models/training_corresp.py:154-176) needs, per decoder call, a value pass that keeps its activations, and later an
+// adjoint pass with the weight gradient of every layer.  Everything the backward needs lives in the caller's workspace, so
+// several forwards can be alive at once (the loss calls the decoder twice and autograd runs the backwards in reverse order).
+//
+// Per-row condition columns: in train mode the reference adds randn(B, N, 32) / 200 to the compressed columns of every point
+// (deepSDF.py:220-221).  The noise enters layer 0 and the skip layer; both take it as extra point-dependent input columns:
+// [xyz | noise] is staged once as a row array X0, read as A1 by layer 0 and appended (app) to the output of the layer in
+// front of the skip.  Weight gradients of those columns fall out of the same GEMM; the per-query part of the condition is
+// the outer product of the per-query column sums of d_0 / d_skip with the condition.
+//
+// fp16 range: the upstream gradient of the loss is of order 1e-5, where the hi part of the fp16 split is subnormal and the lo
+// part is lost.  The backward scales it on the device by a power of two (its largest magnitude to 2^10) and undoes the scale in
+// the fp32 epilogues of the gradients (grad_scale_kernel).
+namespace nphm {
+namespace train {
+
+// workspace of one forward: 256-byte aligned pieces
+struct Layout {
+    size_t cond = 0, x0 = 0, x0p = 0, hp[kMaxLayers] = {}, s[kMaxLayers] = {}, total = 0;
+    int ldx = 0, ks_x0 = 0, ks_h[kMaxLayers] = {};
+};
+
+static Layout layout(const StackDims &s, int n_queries, long long n_points, int nd)
+{
+    Layout L;
+    const long long M = (long long)n_queries * n_points, tiles = ceil_div(M, 128);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
+    L.cond = take((size_t)n_queries * s.cond_dim * sizeof(float));
+    L.ldx = pad4(3 + nd);
+    L.ks_x0 = (3 + nd + 15) / 16;
+    L.x0 = take((size_t)M * L.ldx * sizeof(float));
+    L.x0p = take((size_t)tiles * L.ks_x0 * 8192);
+    for (int l = 0; l + 1 < s.n_lin; ++l) {
+        L.ks_h[l] = (s.N[l] + (l + 1 == s.skip ? 3 + nd : 0) + 15) / 16;
+        L.hp[l] = take((size_t)tiles * L.ks_h[l] * 8192);
+        L.s[l] = take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
+    }
+    L.total = off;
+    return L;
+}
+
+// X0[row] = [xyz | noise | 0 ...]  (ldx columns)
+__global__ void stage_x0_kernel(const float *__restrict__ xyz, const float *__restrict__ noise, int nd, long long M, int ldx,
+                                float *__restrict__ X0)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= M * ldx) return;
+    const long long r = idx / ldx;
+    const int c = (int)(idx % ldx);
+    X0[idx] = c < 3 ? xyz[r * 3 + c] : (c < 3 + nd ? noise[r * nd + c - 3] : 0.f);
+}
+
+// fp32 rows [M][ld] (the first `width` columns, times scale[0] if given) -> packed operand tiles of `ks` k-steps
+// (tc_linear.cuh); the rows of the last tile beyond M are zero.  Thread = (row, 8 columns).
+__global__ void pack_rows_kernel(const float *__restrict__ src, int ld, int width, long long M, int ks, const float *__restrict__ scale,
+                                 uint8_t *__restrict__ dst)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (M + 127) / 128 * 128 * 2 * ks) return;
+    const long long row = idx / (2 * ks);
+    const int g = (int)(idx % (2 * ks));
+    const float sc = scale ? scale[0] : 1.0f;
+    float v[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int c = 8 * g + i;
+        v[i] = (row < M && c < width) ? src[(size_t)row * ld + c] * sc : 0.f;
+    }
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) tc::split2(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
+    uint8_t *d = dst + ((size_t)(row >> 7) * ks + (g >> 1)) * 8192 + (size_t)((row & 127) >> 3) * 256 + (g & 1) * 128 + (row & 7) * 16;
+    *reinterpret_cast<uint4 *>(d) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
+
+// scale[0] = 2^(kGradExp - e) with 2^e <= max |g| < 2^(e+1) (1 for an all-zero or non-finite g), scale[1] = 1 / scale[0].
+// kGradExp: the adjoint shrinks layer by layer (~0.3x per 512-wide layer at initialisation), and an fp16 hi | lo pair only
+// keeps its 22 bits while |x| >= 2^-3 (below that lo is subnormal): the top of the chain starts at 2^10 so that d_0 is still
+// in that range, which leaves 2^5 of headroom below the fp16 maximum for an adjoint that grows instead.  One block.
+constexpr int kGradExp = 10;
+__global__ void grad_scale_kernel(const float *__restrict__ g, long long n, float *__restrict__ scale)
+{
+    __shared__ float red[32];
+    float m = 0.f;
+    for (long long i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(g[i]));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, red[w]);
+        const int e = (m > 0.f && isfinite(m)) ? max(-100, min(100, ilogbf(m))) - kGradExp : 0;
+        scale[0] = ldexpf(1.0f, -e);
+        scale[1] = ldexpf(1.0f, e);
+    }
+}
+
+// out[q][c] = scale[1] * (sum over the rows of query q of the packed X[row][c]), in a fixed order.  grid (k-steps, queries),
+// 256 threads = 16 columns x 16 row lanes.
+__global__ void __launch_bounds__(256) query_sums_kernel(const uint8_t *__restrict__ X, int ks, long long n_points, int n_cols,
+                                                         const float *__restrict__ scale, float *__restrict__ out)
+{
+    __shared__ float part[16][17];
+    const int c = threadIdx.x & 15, rl = threadIdx.x >> 4, j = blockIdx.x, q = blockIdx.y;
+    const long long r1 = (long long)(q + 1) * n_points;
+    float s = 0.f;
+    for (long long r = (long long)q * n_points + rl; r < r1; r += 16) {
+        const uint8_t *p = X + ((size_t)(r >> 7) * ks + j) * 8192 + (size_t)((r & 127) >> 3) * 256 + (c >> 3) * 128 + (r & 7) * 16 + (c & 7) * 2;
+        s += __half2float(*reinterpret_cast<const __half *>(p)) + __half2float(*reinterpret_cast<const __half *>(p + 4096));
+    }
+    part[rl][c] = s;
+    __syncthreads();
+    if (rl == 0 && j * 16 + c < n_cols) {
+        float t = 0.f;
+        for (int i = 0; i < 16; ++i) t += part[i][c];
+        out[(size_t)q * n_cols + j * 16 + c] = t * scale[1];
+    }
+}
+
+// out[c] = sum_q sums[q][c]  (bias gradient)
+__global__ void sum_queries_kernel(const float *__restrict__ sums, int n_queries, int n, float *__restrict__ out)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    float t = 0.f;
+    for (int q = 0; q < n_queries; ++q) t += sums[(size_t)q * n + c];
+    out[c] = t;
+}
+
+// per-query condition columns of layer 0 / skip:  dW[n][c0 + j] = (j < nd ? dW[n][c0 + j] : 0) + scale * sum_q sums[q][n] cond[q][j]
+// (the first nd columns already hold the noise part from the GEMM)
+__global__ void cond_outer_kernel(const float *__restrict__ sums, const float *__restrict__ cond, int n_queries, int N, int cond_dim,
+                                  int nd, float scale, float *__restrict__ dW, int ldw, int c0)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)N * cond_dim) return;
+    const int n = (int)(idx / cond_dim), j = (int)(idx % cond_dim);
+    float t = 0.f;
+    for (int q = 0; q < n_queries; ++q) t = fmaf(sums[(size_t)q * N + n], cond[(size_t)q * cond_dim + j], t);
+    float *w = dW + (size_t)n * ldw + c0 + j;
+    *w = (j < nd ? *w : 0.f) + scale * t;
+}
+
+// grad_xyz[r][i] = (a[r][i] + b[r][i]) * scale[1]   (a, b: ld 4)
+__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, const float *__restrict__ scale,
+                                float *__restrict__ out)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= M * 3) return;
+    const long long r = idx / 3;
+    const int i = (int)(idx % 3);
+    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * scale[1];
+}
+
+static bool noise_layer(const StackDims &s, int l) { return l == 0 || l + 1 == s.skip || l == s.skip; }
+
+static const tcl::PackedLinear &layer(const MlpChain &c, const StackDims &s, int l)
+{
+    return noise_layer(s, l) ? c.tfwd[l] : c.fwd[l];
+}
+
+// the training variants of layers 0, skip - 1 and skip for nd noise columns
+static int pack(nphm_mlp *h, int nd, cudaStream_t stream)
+{
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    if (c.train_nd == nd) return NPHM_OK;
+    for (int l = 0; l < s.n_lin; ++l) {
+        if (!noise_layer(s, l)) continue;
+        const int K = l == 0 ? 3 + nd : l == s.skip ? s.N[l - 1] + 3 + nd : s.K[l];
+        int rc = c.tfwd[l].pack(h->weights.W[l].as<float>(), s.in_total[l], s.N[l], K, 0, 0, false,
+                                l == s.skip ? chain::kInvSqrt2 : 1.0f, stream, 1, 0, nullptr, 0, l + 1 == s.skip ? 3 + nd : 0, kChainNt);
+        if (rc) return rc;
+    }
+    c.train_nd = nd;
+    return NPHM_OK;
+}
+
+}  // namespace train
+}  // namespace nphm
+
+extern "C" long long nphm_mlp_train_workspace_bytes(const nphm_mlp *h, int n_queries, long long n_points, int noise_dim)
+{
+    if (!h || !h->loaded || n_queries < 1 || n_points < 1 || noise_dim < 0 || noise_dim > h->dims.cond_dim) {
+        set_error("nphm_mlp_train_workspace_bytes: bad arguments");
+        return -1;
+    }
+    return (long long)train::layout(h->dims, n_queries, n_points, noise_dim).total;
+}
+
+extern "C" int nphm_mlp_train_forward(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, const float *cond_noise_dev,
+                                      int noise_dim, int n_queries, long long n_points, float *out_dev, void *workspace_dev,
+                                      void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = chain_ready(h, "nphm_mlp_train_forward");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && out_dev && workspace_dev,
+                 "nphm_mlp_train_forward: bad arguments");
+    NPHM_REQUIRE(noise_dim >= 0 && noise_dim <= h->dims.cond_dim && (noise_dim == 0 || cond_noise_dev),
+                 "nphm_mlp_train_forward: noise_dim %d out of range [0, %d] or no noise given", noise_dim, h->dims.cond_dim);
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    const train::Layout L = train::layout(s, n_queries, n_points, noise_dim);
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const long long M = (long long)n_queries * n_points;
+    if ((rc = train::pack(h, noise_dim, stream))) return rc;
+    if ((rc = mlp_prepare(h, cond_dev, n_queries, stream))) return rc;
+    float *X0 = reinterpret_cast<float *>(ws + L.x0);
+    train::stage_x0_kernel<<<(unsigned)ceil_div(M * L.ldx, 256), 256, 0, stream>>>(xyz_dev, cond_noise_dev, noise_dim, M, L.ldx, X0);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    train::pack_rows_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128 * 2 * L.ks_x0, 256), 256, 0, stream>>>(
+        X0, L.ldx, 3 + noise_dim, M, L.ks_x0, nullptr, ws + L.x0p);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(ws + L.cond, cond_dev, (size_t)n_queries * s.cond_dim * sizeof(float), cudaMemcpyDeviceToDevice,
+                                    stream));
+    for (int l = 0; l < s.n_lin; ++l) {
+        const tcl::PackedLinear &W = train::layer(c, s, l);
+        tcl::LinearParams p;
+        p.M = M;
+        if (l == 0) { p.A1 = X0; p.lda1 = L.ldx; p.K1 = 3 + noise_dim; }
+        else { p.Ap = ws + L.hp[l - 1]; p.a_ksteps = W.ksteps; }
+        p.bias = h->cvec.as<float>() + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = n_points;
+        if (l == s.n_lin - 1) {
+            p.mode = tcl::kModeLinear;
+            p.C = out_dev; p.ldc = s.N[l];
+        } else {
+            p.mode = tcl::kModeSoftplus;
+            p.Cp = ws + L.hp[l]; p.c_ksteps = L.ks_h[l];
+            if (l + 1 == s.skip) { p.app = X0; p.app_ld = L.ldx; p.app_w = 3 + noise_dim; }
+            p.Dv = reinterpret_cast<float *>(ws + L.s[l]); p.lddv = c.ld[l]; p.dv_blocked = 1;
+        }
+        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
+    }
+    return NPHM_OK;
+}
+
+extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, const void *workspace_dev,
+                                       long long workspace_bytes, int nd, int n_queries, long long n_points, float *const *grad_w_dev, float *const *grad_b_dev, float *grad_cond_dev,
+                                       float *grad_xyz_dev, void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = chain_ready(h, "nphm_mlp_train_backward");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && grad_out_dev && workspace_dev, "nphm_mlp_train_backward: bad arguments");
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    const uint8_t *ws = static_cast<const uint8_t *>(workspace_dev);
+    // the workspace must hold a forward of this stack at these sizes (a few bytes read back: the shapes decide the launches)
+    // the caller states the shape the workspace was made for; checked against its size, without reading it back
+    NPHM_REQUIRE(nd >= 0 && nd <= s.cond_dim && workspace_bytes == (long long)train::layout(s, n_queries, n_points, nd).total,
+                 "nphm_mlp_train_backward: a workspace of %lld bytes does not hold a training forward of this network at %d x %lld "
+                 "points with %d noise columns", workspace_bytes, n_queries, n_points, nd);
+    const train::Layout L = train::layout(s, n_queries, n_points, nd);
+    const long long M = (long long)n_queries * n_points;
+    const int last = s.n_lin - 1, out_dim = s.N[last];
+    const float *cond = reinterpret_cast<const float *>(ws + L.cond);
+
+    // upstream gradient scaled by 2^-e into the packed d_L
+    if ((rc = c.gscale.reserve(2 * sizeof(float)))) return rc;
+    const float *gs = c.gscale.as<float>();
+    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_out_dev, M * out_dim, c.gscale.as<float>());
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    const int ks_out = (out_dim + 15) / 16;
+    if ((rc = c.Dl.reserve(packed_bytes(M, ks_out)))) return rc;
+    train::pack_rows_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128 * 2 * ks_out, 256), 256, 0, stream>>>(
+        grad_out_dev, out_dim, out_dim, M, ks_out, gs, c.Dl.as<uint8_t>());
+    NPHM_CUDA_CHECK(cudaGetLastError());
+
+    int max_ks = 1, max_n = 1;
+    for (int l = 1; l <= last; ++l) max_ks = std::max(max_ks, (s.N[l - 1] + 15) / 16);
+    for (int l = 0; l <= last; ++l) max_n = std::max(max_n, s.N[l]);
+    for (int i = 0; i < 2; ++i)
+        if ((rc = c.Dp[i].reserve(packed_bytes(M, max_ks)))) return rc;
+    if ((rc = c.qsums.reserve((size_t)n_queries * max_n * sizeof(float))) ||
+        (rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
+        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
+        return rc;
+    if (grad_xyz_dev && ((rc = c.xtmp.reserve((size_t)M * 4 * sizeof(float))) || (rc = c.xs_tmp.reserve((size_t)M * 4 * sizeof(float)))))
+        return rc;
+
+    // gradients of layer l from its pre-activation adjoint d (packed, ks k-steps, scaled by 2^-e)
+    auto layer_grads = [&](int l, const uint8_t *d, int ks) -> int {
+        float *gw = grad_w_dev ? grad_w_dev[l] : nullptr, *gb = grad_b_dev ? grad_b_dev[l] : nullptr;
+        const bool cond_layer = l == 0 || l == s.skip;
+        const float sc = l == s.skip ? chain::kInvSqrt2 : 1.0f;
+        if (gw) {
+            const uint8_t *H = l == 0 ? ws + L.x0p : ws + L.hp[l - 1];
+            const int hks = l == 0 ? L.ks_x0 : L.ks_h[l - 1];
+            const int K = l == 0 ? 3 + nd : l == s.skip ? s.N[l - 1] + 3 + nd : s.N[l - 1];
+            int r = wgrad::launch(d, ks, H, hks, M, s.N[l], K, sc, gs + 1, gw, s.in_total[l], c.wg_partials, stream);
+            if (r) return r;
+        }
+        float *sums = l == 0 ? c.qsums0.as<float>() : l == s.skip ? c.qsumss.as<float>() : c.qsums.as<float>();
+        if (gb || (cond_layer && (gw || grad_cond_dev))) {
+            train::query_sums_kernel<<<dim3((unsigned)ks, (unsigned)n_queries), 256, 0, stream>>>(d, ks, n_points, s.N[l], gs, sums);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+        if (gb) {
+            train::sum_queries_kernel<<<(unsigned)ceil_div(s.N[l], 128), 128, 0, stream>>>(sums, n_queries, s.N[l], gb);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+        if (cond_layer && gw) {
+            const long long total = (long long)s.N[l] * s.cond_dim;
+            train::cond_outer_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(
+                sums, cond, n_queries, s.N[l], s.cond_dim, nd, sc, gw, s.in_total[l], l == 0 ? 3 : s.N[l - 1] + 3);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+        return NPHM_OK;
+    };
+
+    // d_{l-1} = s_{l-1} * (d_l W_l), from the output layer down to d_0; d_l lives in Dp[l & 1] (d_L in Dl)
+    const uint8_t *d = c.Dl.as<uint8_t>();
+    int ks = ks_out;
+    for (int l = last; l >= 1; --l) {
+        if ((rc = layer_grads(l, d, ks))) return rc;
+        if (l == s.skip && grad_xyz_dev) {
+            tcl::LinearParams px;
+            px.M = M;
+            px.Ap = d; px.a_ksteps = ks;
+            px.mode = tcl::kModeLinear; px.C = c.xs_tmp.as<float>(); px.ldc = 4;
+            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+        }
+        tcl::LinearParams p;
+        p.M = M;
+        p.Ap = d; p.a_ksteps = ks;
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + L.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
+        const int ks_next = (s.N[l - 1] + 15) / 16;
+        p.Cp = c.Dp[(l - 1) & 1].as<uint8_t>(); p.c_ksteps = ks_next;
+        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
+        d = c.Dp[(l - 1) & 1].as<uint8_t>();
+        ks = ks_next;
+    }
+    if ((rc = layer_grads(0, d, ks))) return rc;
+    if (grad_cond_dev) {
+        // the noise does not change the gradient with respect to the condition
+        NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
+        dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 1);          // one chunk: a fixed summation order
+        chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
+                                                          h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
+                                                          s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    if (grad_xyz_dev) {
+        tcl::LinearParams px;
+        px.M = M;
+        px.Ap = d; px.a_ksteps = ks;
+        px.mode = tcl::kModeLinear; px.C = c.xtmp.as<float>(); px.ldc = 4;
+        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
+        train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(c.xtmp.as<float>(), c.xs_tmp.as<float>(), M, gs,
+                                                                                  grad_xyz_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
     return NPHM_OK;
 }

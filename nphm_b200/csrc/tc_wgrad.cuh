@@ -1,0 +1,16 @@
+// Weight gradient of a linear layer from packed operands (tc_wgrad.cu):  dW[n][k] = scale * sum_rows D[row][n] H[row][k]
+#pragma once
+#include "engine.cuh"
+
+namespace nphm {
+namespace wgrad {
+
+// D: packed pre-activation adjoints (d_ksteps k-steps), H: packed layer inputs (h_ksteps k-steps), both over M rows in the
+// operand format of tc_linear.cuh.  Writes dW[n * ldw + k] for n < N, k < K:  scale * inv_scale_dev[0] * (D^T H)[n][k].
+// The rows are split over the CTAs; the partial sums go to `partials` and are added in a fixed order (no atomics), so equal
+// inputs give bitwise-equal gradients.  `partials`: scratch, grown on demand.
+int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
+           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream);
+
+}  // namespace wgrad
+}  // namespace nphm

@@ -9,6 +9,8 @@ Parameter names (``lin{i}.weight/bias``, ``compressor.0.*``, ``defDeepSDF.lin{i}
 constructor signatures are those of the reference so checkpoints load with ``strict=True``.
 As in :mod:`.EnsembledDeepSDF`, CUDA no-grad calls with a per-query-constant condition run in
 the native sm_90a MLP path; everything else uses a PyTorch composite that keeps autograd.
+``forward_native_grad`` is the explicit first-order training path: native forward and native
+backward (weight, bias, condition and point gradients), for a condition that is constant per query.
 """
 from __future__ import annotations
 
@@ -19,11 +21,49 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from torch.autograd.function import once_differentiable
+
 from .. import _native
 from . import _composite
 from .EnsembledDeepSDF import sample_point_feature  # same function in the reference (:92-115)
 
 _SQRT2 = math.sqrt(2.0)
+
+
+def _native_backward(ctx, grad_out):
+    ws, *params = ctx.saved_tensors                   # raises if a parameter was changed in place since the forward
+    need = ctx.needs_input_grad                       # (engine, xyz, cond, noise, lin0.weight, lin0.bias, ...)
+    gw, gb, g_cond, g_xyz = ctx.engine.train_backward(ws, grad_out, ctx.noise_dim, weights=any(need[4::2]), biases=any(need[5::2]),
+                                                      want_cond=need[2], want_xyz=need[1])
+    grads = [None, g_xyz, g_cond, None]
+    for i in range(len(params) // 2):
+        grads.append(gw[i] if need[4 + 2 * i] else None)
+        grads.append(gb[i] if need[5 + 2 * i] else None)
+    return tuple(grads)
+
+
+class _NativeTrainFn(torch.autograd.Function):
+    """``DeepSDF`` stack with a per-query condition on the native training kernels (``nphm_mlp_train_forward`` /
+    ``_backward``): xyz B x N x 3, cond B x lat_dim, noise B x N x d (added to the leading ``d`` condition columns of each
+    point, no gradient) or None, then the ``lin{l}.weight / bias`` parameters.  First order only."""
+
+    @staticmethod
+    def forward(ctx, engine, xyz, cond, noise, *params):
+        out, ws = engine.train_forward(xyz, cond, noise)
+        ctx.engine = engine
+        ctx.noise_dim = 0 if noise is None else noise.shape[-1]
+        ctx.save_for_backward(ws, *params)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        if torch.is_grad_enabled():
+            raise RuntimeError('forward_native_grad is differentiable to first order only: a double backward '
+                               '(create_graph=True) through it is not supported; use the composite forward() instead')
+        return _native_backward_once(ctx, grad_out)
+
+
+_native_backward_once = once_differentiable(_native_backward)
 
 
 class DeepSDF(nn.Module):
@@ -85,6 +125,36 @@ class DeepSDF(nn.Module):
                                         or any(p.requires_grad for p in self.parameters())):
             return False
         return xyz.dtype == torch.float32 and xyz.dim() == 3
+
+    def native_grad_supported(self, xyz, lat_rep=None) -> bool:
+        """Whether :meth:`forward_native_grad` takes these points: CUDA fp32 B x N x 3, no positional encoding, Softplus(100),
+        a depth / width the native stack builder accepts (and, if given, a condition that is B x D or B x 1 x D)."""
+        n_lin = self.num_layers - 1
+        if lat_rep is not None and not (lat_rep.dim() == 2 or lat_rep.shape[1] == 1 or lat_rep.stride(1) == 0):
+            return False
+        return (xyz.is_cuda and xyz.dtype == torch.float32 and xyz.dim() == 3 and self.num_freq_bands is None
+                and self.beta == 100 and self.out_dim_net <= 8 and next(self.parameters()).dtype == torch.float32
+                and _native.stack_supported(n_lin - 1, _native.hidden_width(self, n_lin), self.lat_dim))
+
+    def _native_train(self, xyz, cond, noise=None):
+        """xyz B x N x 3, cond B x lat_dim (differentiable), noise B x N x d or None -> B x N x out_dim."""
+        if not self.native_grad_supported(xyz):
+            raise _native.NativeError('forward_native_grad: unsupported input or network (needs CUDA fp32 B x N x 3 points, '
+                                      'no positional encoding, Softplus(beta=100), a stack the native builder accepts)')
+        params = []
+        for i in range(self.num_layers - 1):
+            lin = getattr(self, 'lin%d' % i)
+            params += [lin.weight, lin.bias]
+        return _NativeTrainFn.apply(self.engine(), xyz, cond, None if noise is None else noise.detach(), *params)
+
+    def forward_native_grad(self, xyz, lat_rep, anchors=None):
+        """:meth:`forward` on the native training kernels, differentiable to first order (weights, biases, ``lat_rep``,
+        ``xyz``).  ``lat_rep``: B x D, B x 1 x D, or B x N x D equal for all points of a query; of a B x N x D tensor the
+        gradient reaches the first row (an ``expand`` / ``repeat`` of a B x 1 x D code passes the reference's gradient on)."""
+        cond = _native.constant_latent_rows(lat_rep)
+        if cond is None:
+            raise ValueError('forward_native_grad: the condition must be constant over the points of a query')
+        return self._native_train(xyz, cond), None
 
     def forward(self, xyz, lat_rep, anchors=None):
         if self._fused_ok(xyz, lat_rep):
@@ -245,6 +315,41 @@ class DeformationNetwork(nn.Module):
         cond = self._condition(xyz, lat_rep, anchors, per_point=lat_rep.shape[1] != 1)
         _, J = _input_jacobian(backbone, xyz, cond)
         return J[..., :3, :]
+
+    def native_grad_supported(self, xyz, lat_rep) -> bool:
+        """Whether :meth:`forward_native_grad` takes this call (mode, backbone, points, a condition constant per query)."""
+        if xyz.dim() < 3:
+            xyz = xyz.unsqueeze(0)
+        return (self.mode in ('compress', 'expr_only', 'glob_only') and self.defDeepSDF.native_grad_supported(xyz)
+                and (lat_rep.dim() == 2 or lat_rep.shape[1] == 1 or lat_rep.stride(1) == 0))
+
+    def forward_native_grad(self, xyz, lat_rep, anchors):
+        """:meth:`forward` on the native training kernels, differentiable to first order.  ``lat_rep``: B x 1 x D (or B x D,
+        or B x N x D equal over the points; see :meth:`DeepSDF.forward_native_grad` for its gradient).  In ``compress`` mode
+        ``compressor([z_id | anchors])`` stays in autograd, and in train mode the noise is drawn by the reference's own call
+        (``torch.randn(B, N, 32) / 200``, deepSDF.py:220-221), so a seeded run sees the same noise as :meth:`forward`."""
+        if xyz.dim() < 3:
+            xyz = xyz.unsqueeze(0)
+        if self.mode not in ('compress', 'expr_only', 'glob_only'):
+            raise ValueError('forward_native_grad: mode %r keeps the composite path' % self.mode)
+        lat = _native.constant_latent_rows(lat_rep)
+        if lat is None:
+            raise ValueError('forward_native_grad: the condition must be constant over the points of a query')
+        B, N, _ = xyz.shape
+        E = self.lat_dim_expr
+        noise = None
+        if self.mode == 'compress':
+            a0 = anchors[:, 0] if anchors.dim() == 4 else anchors
+            compressed = self.compressor(torch.cat([lat[:, :-E], a0.reshape(B, -1)], dim=-1))          # B x 32
+            if self.training:
+                noise = torch.randn((B, N, compressed.shape[-1]), device=compressed.device) / 200
+            cond = torch.cat([compressed, lat[:, -E:]], dim=-1)
+        elif self.mode == 'glob_only':
+            cond = torch.cat([lat[:, :self.lat_dim_glob_shape], lat[:, -E:]], dim=-1)
+        else:
+            cond = lat[:, -E:]
+        pred = self.defDeepSDF._native_train(xyz, cond, noise)
+        return pred[..., :3], pred[..., -1:]
 
     def forward(self,
                 xyz: torch.Tensor,

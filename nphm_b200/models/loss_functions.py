@@ -1,7 +1,8 @@
-"""Identity-space training / validation losses of the reference, ``NPHM.models.loss_functions``:
+"""Training / validation losses of the reference, ``NPHM.models.loss_functions``:
 
-  * ``compute_loss``         src/NPHM/models/loss_functions.py:7-17
-  * ``actual_compute_loss``  src/NPHM/models/loss_functions.py:20-110   (SURVEY.md 8f-3)
+  * ``compute_loss``                  src/NPHM/models/loss_functions.py:7-17
+  * ``actual_compute_loss``           src/NPHM/models/loss_functions.py:20-110   (SURVEY.md 8f-3)
+  * ``compute_loss_corresp_forward``  src/NPHM/models/loss_functions.py:282-322  (stage 2: the expression space)
 
 Same inputs (a batch dict with ``points_face``, ``points_non_face``, ``sup_grad_far``, ``sup_grad_near``, the normals and
 ``gt_anchors``), same returned dict (``surf_sdf``, ``normals``, ``space_sdf``, ``grad``, ``lat_reg`` and - for the
@@ -14,6 +15,11 @@ ensemble - ``anchors``, ``symm_dist``, ``middle_dist``).  Two ways to get the SD
     ``torch.no_grad()``: its ``gradient`` needs a graph) or with ``native=True``; training-mode forward only.
   * **composite** (training): the decoder's autograd path and ``diff_operators.gradient`` with ``create_graph=True`` -
     weight gradients of the normal / eikonal terms need the double backward, which stays in PyTorch.
+
+``compute_loss_corresp_forward`` is first order (no gradient with respect to the points is used), so its decoder calls run
+natively to the weights: ``DeformationNetwork.forward_native_grad`` (forward and backward on the tensor cores, the compressor
+and the embeddings in autograd).  ``native=None`` picks that path for a CUDA fp32 decoder the native chain supports,
+``native=False`` keeps the composite one.
 
 This module is NOT installed over ``NPHM.models.loss_functions`` by ``install_as_nphm`` (the reference's own file keeps
 working on top of the drop-in decoder); import it explicitly.
@@ -110,3 +116,58 @@ def actual_compute_loss(batch_cuda, decoder, glob_cond, native=None):
     losses['symm_dist'] = symm_dist
     losses['middle_dist'] = middle_dist
     return losses
+
+
+def _corresp_native_ok(decoder, points, glob_cond) -> bool:
+    return (hasattr(decoder, 'native_grad_supported') and points.is_cuda and points.dtype == torch.float32
+            and glob_cond.dim() == 3 and glob_cond.shape[1] == 1 and decoder.native_grad_supported(points, glob_cond))
+
+
+def compute_loss_corresp_forward(batch, decoder, decoder_shape, latent_codes, latent_codes_shape, device, epoch=-1,
+                                 exp_path=None, native=None):
+    """Stage-2 loss of the reference (same arguments, same random draws in the same order, same returned dict:
+    ``corresp``, ``lat_reg``, ``loss_reg_zero``).  ``native``: None = the native first-order decoder path when it supports
+    the call, False = the composite path, True = the native path (raises if unsupported)."""
+    if 'path' in batch:
+        del batch['path']
+    batch_cuda = {k: v.to(device).float() for (k, v) in zip(batch.keys(), batch.values())}
+    glob_cond_shape = latent_codes_shape(batch['subj_ind'].to(device))
+    glob_cond_pose = latent_codes(batch['idx'].to(device))
+
+    if 'gt_anchors' in batch_cuda and decoder_shape is not None and decoder_shape.mlp_pos is None:
+        gt_anchors = batch_cuda['gt_anchors']
+    elif decoder_shape is not None and decoder_shape.mlp_pos is not None:
+        gt_anchors = decoder_shape.mlp_pos(glob_cond_shape[..., :decoder_shape.lat_dim_glob]).view(glob_cond_pose.shape[0], -1, 3)
+        gt_anchors += decoder.anchors.squeeze(0)
+    else:
+        gt_anchors = batch_cuda['gt_anchors']
+
+    glob_cond = torch.cat([glob_cond_shape, glob_cond_pose], dim=-1)
+    points_neutral = batch_cuda['points_neutral'].clone().detach().requires_grad_()
+    if native is None:
+        native = _corresp_native_ok(decoder, points_neutral, glob_cond)
+    elif native and not _corresp_native_ok(decoder, points_neutral, glob_cond):
+        raise ValueError('compute_loss_corresp_forward(native=True): the decoder / batch is not supported natively')
+
+    if native:
+        # B x 1 x D condition: its gradient is the sum over the points, which is what the reference's repeat() passes on
+        decoder_call = lambda x, n: decoder.forward_native_grad(x, glob_cond, gt_anchors)     # noqa: E731
+    else:
+        cond = glob_cond.repeat(1, points_neutral.shape[1], 1)
+        decoder_call = lambda x, n: decoder(x, cond[:, :n, :], gt_anchors)                    # noqa: E731
+
+    delta, _ = decoder_call(points_neutral, points_neutral.shape[1])
+    pred_posed = points_neutral + delta.squeeze()
+    points_posed = batch_cuda['points_posed']
+    loss_corresp = (pred_posed - points_posed[:, :, :3]) ** 2
+
+    lat_mag = torch.norm(glob_cond_pose, dim=-1) ** 2
+
+    # enforce deformation field to be zero elsewhere
+    samps = (torch.rand(glob_cond.shape[0], 100, 3, device=glob_cond.device, dtype=glob_cond.dtype) - 0.5) * 2.5
+    delta, _ = decoder_call(samps, 100)
+    loss_reg_zero = (delta ** 2).mean()
+
+    return {'corresp': loss_corresp.mean(),
+            'lat_reg': lat_mag.mean(),
+            'loss_reg_zero': loss_reg_zero}

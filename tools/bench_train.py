@@ -1,0 +1,161 @@
+#!/usr/bin/env python
+"""Stage-2 training step (reference TrainerAutoDecoder.train_step, src/NPHM/models/training_corresp.py:154-176, loss
+compute_loss_corresp_forward) at scripts/configs/nphm_def.yaml settings: 32 samples x 1000 points plus 32 x 100 `samps`,
+lambdas corresp 100 / loss_reg_zero 5e-5 / lat_reg 5e-5, AdamW (lr 1e-4, weight decay 5e-4) on the decoder, SparseAdam
+(lr_lat 5e-4) on the expression codes, clip_grad_norm_ 0.025 on the decoder and on the codes (grad_clip, grad_clip_lat),
+codes as the reference makes them (sparse Embedding, max_norm 1.0; the codes' clip is done on the coalesced sparse
+gradient, which torch's clip_grad_norm_ cannot take), and the per-step `.item()` of every loss term and of
+the total.  Random weights and codes (no dataset): the step's work does not depend on the values.
+
+    python tools/bench_train.py --steps 20 --warmup 3
+
+Native (forward_native_grad: tensor-core forward and weight gradients) and composite (PyTorch autograd) steps alternate
+in one process on one GPU, for the `compress` DeformationNetwork (235 -> 512 x 6 -> 3) and the `-mode npm` expression
+decoder (715 -> 1024 x 8 -> 3).  CUDA events split a step into loss forward, backward and optimizer.  Prints one JSON line."""
+import argparse, json, os, subprocess, sys
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
+import torch
+
+LAMBDAS = {'corresp': 100.0, 'loss_reg_zero': 5.0e-05, 'lat_reg': 5.0e-05}          # nphm_def.yaml
+
+def gpu_info():
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i',
+                              str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power = [x.strip() for x in out.split(',')]
+        return name, power
+    except Exception:
+        return torch.cuda.get_device_name(), 'not measured'
+
+
+def setup(mode, dev):
+    from conftest import make_deformation
+    from nphm_b200.models.deepSDF import DeepSDF
+    torch.manual_seed(0)
+    if mode == 'compress':
+        dec = make_deformation(dev).train()
+        lat_shape_dim = 32 * 39 + 32 + 64
+    else:
+        dec = DeepSDF(lat_dim=712, hidden_dim=1024, nlayers=8, geometric_init=False, out_dim=3).to(dev).train()
+        lat_shape_dim = 512
+    lat_expr = torch.nn.Embedding(64, 200, max_norm=1.0, sparse=True).to(dev)
+    lat_shape = torch.nn.Embedding(16, lat_shape_dim, max_norm=1.0, sparse=True).to(dev)
+    with torch.no_grad():
+        lat_expr.weight.mul_(0.1)
+        lat_shape.weight.mul_(0.1)
+    opt = torch.optim.AdamW(dec.parameters(), lr=1e-4, weight_decay=5e-4)
+    opt_lat = torch.optim.SparseAdam(lat_expr.parameters(), lr=5e-4)
+    return dec, lat_expr, lat_shape, opt, opt_lat
+
+
+def batch(B, N, dev, step):
+    g = torch.Generator().manual_seed(step)
+    pts = (torch.rand(B, N, 3, generator=g) - 0.5) * 1.2
+    return {'points_neutral': pts, 'points_posed': pts + 0.02 * torch.randn(B, N, 3, generator=g),
+            'gt_anchors': torch.rand(B, 39, 3, generator=g) - 0.5,
+            'idx': torch.randint(0, 64, (B, 1), generator=g), 'subj_ind': torch.randint(0, 16, (B, 1), generator=g)}
+
+
+def clip_sparse_grad_norm_(p, max_norm):
+    """clip_grad_norm_ of the reference's grad_clip_lat for the sparse gradient of an Embedding(sparse=True): this torch's
+    clip_grad_norm_ has no sparse norm kernel, the coalesced values carry the same norm."""
+    g = p.grad.coalesce()
+    coef = torch.clamp(max_norm / (g.values().norm() + 1e-6), max=1.0)
+    p.grad = g * coef
+
+
+def train_step(state, b, native, ev):
+    from nphm_b200.models.loss_functions import compute_loss_corresp_forward
+    dec, lat_expr, lat_shape, opt, opt_lat = state
+    ev[0].record()
+    opt.zero_grad()
+    opt_lat.zero_grad()
+    losses = compute_loss_corresp_forward(dict(b), dec, None, lat_expr, lat_shape, 'cuda', native=native)
+    tot = 0
+    for k, lam in LAMBDAS.items():
+        tot = tot + lam * losses[k]
+    ev[1].record()
+    tot.backward()
+    ev[2].record()
+    torch.nn.utils.clip_grad_norm_(dec.parameters(), max_norm=0.025)
+    clip_sparse_grad_norm_(lat_expr.weight, max_norm=0.025)
+    opt.step()
+    opt_lat.step()
+    ev[3].record()
+    values = {k: v.item() for k, v in losses.items()}                # the reference's per-step read-backs
+    values['loss'] = tot.item()
+    return values['loss']
+
+
+def run_mode(mode, args, dev):
+    B, N = 32, 1000
+    res = {}
+    states = {nat: setup(mode, dev) for nat in (True, False)}
+    times = {nat: [] for nat in (True, False)}
+    for step in range(args.warmup + args.steps):
+        b = batch(B, N, dev, step)
+        for nat in (True, False):                       # alternate native / composite
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            tot = train_step(states[nat], b, nat, ev)
+            torch.cuda.synchronize()
+            if step >= args.warmup:
+                times[nat].append([ev[0].elapsed_time(ev[3]), ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2]),
+                                   ev[2].elapsed_time(ev[3])])
+            res.setdefault('finite', True)
+            res['finite'] &= bool(tot == tot and abs(tot) != float('inf'))
+    for nat in (True, False):
+        t = torch.tensor(times[nat]).median(dim=0).values.tolist()
+        res['native' if nat else 'composite'] = {'steps_per_s': 1000.0 / t[0], 'ms_step': t[0], 'ms_forward': t[1],
+                                                 'ms_backward': t[2], 'ms_optimizer': t[3]}
+    res['speedup'] = res['native']['steps_per_s'] / res['composite']['steps_per_s']
+    return res
+
+
+def profile_native(dev, steps=5):
+    """CUDA time per kernel (ms per step, largest first) of native `compress` steps, from torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+    state = setup('compress', dev)
+    for step in range(3):
+        train_step(state, batch(32, 1000, dev, step), True, [torch.cuda.Event(enable_timing=True) for _ in range(4)])
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for step in range(steps):
+            train_step(state, batch(32, 1000, dev, 100 + step), True, [torch.cuda.Event(enable_timing=True) for _ in range(4)])
+        torch.cuda.synchronize()
+    rows = {}
+    for e in prof.key_averages():
+        t = getattr(e, 'device_time_total', None)
+        if t is None:
+            t = e.cuda_time_total
+        if t > 0 and e.count > 0:
+            rows[e.key[:90]] = (t / 1000.0 / steps, e.count // steps)
+    top = sorted(rows.items(), key=lambda kv: -kv[1][0])
+    total = sum(v[0] for _, v in top)
+    return {'ms_per_step_kernels': total, 'kernels': [{'name': k, 'ms_per_step': round(v[0], 4), 'launches_per_step': v[1]}
+                                                      for k, v in top[:25]]}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--steps', type=int, default=20)
+    ap.add_argument('--warmup', type=int, default=3)
+    ap.add_argument('--profile', action='store_true',
+                    help='instead: torch.profiler over 5 native `compress` steps, CUDA time per kernel of the step (JSON)')
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
+    dev = torch.device('cuda', torch.cuda.current_device())
+    name, power = gpu_info()
+    if args.profile:
+        print(json.dumps({'metric': 'stage2_native_kernels', 'gpu': name, 'power_limit': power, **profile_native(dev)}))
+        return
+    out = {'metric': 'stage2_train_step', 'gpu': name, 'power_limit': power, 'batch': '32 x (1000 + 100) points',
+           'steps': args.steps, 'timing': 'median of CUDA-event times per step, native and composite alternated'}
+    for mode in ('compress', 'npm'):
+        out[mode] = run_mode(mode, args, dev)
+    print(json.dumps(out))
+
+
+if __name__ == '__main__':
+    main()
