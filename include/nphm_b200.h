@@ -254,6 +254,28 @@ int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, const void *
                             float *const *grad_w_dev, float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev,
                             void *stream);
 
+/* ---- training through the spatial gradient: the stage-1 loss of the reference (src/NPHM/models/loss_functions.py:20-110,
+ * scripts/training/train.py) reaches a one-output DeepSDF stack through s = f(x) and g = grad_x s, so its normal and eikonal
+ * terms need second derivatives.  Stacks with out_dim != 1 are rejected with NPHM_ERR_UNSUPPORTED.  As for the first-order
+ * calls, a forward keeps what its backward needs in a caller-owned device workspace. */
+/* bytes of the workspace of one nphm_mlp_sdfgrad_forward call (-1: bad arguments) */
+long long nphm_mlp_sdfgrad_workspace_bytes(const nphm_mlp *h, int n_queries, long long n_points);
+/* sdf_out_dev [q][n] = f(xyz, cond), grad_out_dev [q][n][3] = d sdf / d xyz (value pass and one adjoint pass with unit
+ * upstream); xyz_dev [q][n][3], cond_dev [q][lat_dim]. */
+int nphm_mlp_sdfgrad_forward(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
+                             float *sdf_out_dev, float *grad_out_dev, void *workspace_dev, void *stream);
+/* what autograd's backward of that forward gives for upstream gradients grad_sdf_dev [q][n] and grad_grad_dev [q][n][3]:
+ * grad_w_dev[l] / grad_b_dev[l] in the state_dict layout of lin{l}.weight / bias (overwritten; the arrays or entries may be
+ * NULL), grad_cond_dev [q][lat_dim] (summed over the points of a query, may be NULL), grad_xyz_dev [q][n][3] (may be NULL).
+ * The tail of the workspace is the call's scratch (its whole per-point memory; the handle only keeps buffers of the layer
+ * widths), so the call writes to it; what the forward stored is left as it was.
+ * Deterministic; workspace_bytes / n_queries / n_points state the forward that filled the workspace and are checked against
+ * its size (NPHM_ERR_INVALID on a mismatch; a shape with the same workspace size is not detected).  Nothing is read back
+ * from the device. */
+int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
+                              long long workspace_bytes, int n_queries, long long n_points, float *const *grad_w_dev,
+                              float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream);
+
 /* anchors_dev [n_queries][n_loc][3] = mlp_pos(z_glob) + mean anchors (reference src/NPHM/models/EnsembledDeepSDF.py:228-229)
  * without evaluating the ensemble - what the fitters read from `decoder(zeros(1,1,3), lat)[1]` (fitting.py:59, :211). */
 int nphm_ensemble_anchors(nphm_ensemble *h, const float *latents_dev, int n_queries, float *anchors_dev, void *stream);

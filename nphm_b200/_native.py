@@ -34,6 +34,7 @@ EXPORTED_SYMBOLS = (
     'nphm_ensemble_backward_inputs', 'nphm_ensemble_anchors',
     'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
+    'nphm_mlp_sdfgrad_workspace_bytes', 'nphm_mlp_sdfgrad_forward', 'nphm_mlp_sdfgrad_backward',
 )
 
 
@@ -156,6 +157,11 @@ def lib() -> ctypes.CDLL:
                                          c_void_p]
     L.nphm_mlp_train_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_longlong, POINTER(c_void_p),
                                           POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
+    L.nphm_mlp_sdfgrad_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong]
+    L.nphm_mlp_sdfgrad_workspace_bytes.restype = c_longlong
+    L.nphm_mlp_sdfgrad_forward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.nphm_mlp_sdfgrad_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_longlong, POINTER(c_void_p),
+                                            POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -498,6 +504,44 @@ class MlpEngine(_Versioned):
             check(lib().nphm_mlp_train_backward(self._h, g.data_ptr(), ws.data_ptr(), ws.numel(), int(noise_dim), B, N,
                                                 _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
                                                 _ptr(g_cond), _ptr(g_xyz), _stream_ptr(dev)), 'nphm_mlp_train_backward')
+        return gw, gb, g_cond, g_xyz
+
+    # ------------------------------------------------------------ training through grad_x sdf (second order)
+    def sdfgrad_forward(self, xyz: torch.Tensor, cond: torch.Tensor):
+        """SDF and its spatial gradient, keeping what the backward needs (nphm_mlp_sdfgrad_forward): xyz B x N x 3, cond
+        B x lat_dim -> ``(sdf B x N x 1, d sdf / d xyz B x N x 3, workspace)``; one-output stacks only."""
+        B, N, _ = xyz.shape
+        dev = xyz.device
+        xyz = _f32c(xyz)
+        cond = _f32c(cond).to(dev)
+        sdf = torch.empty(B, N, 1, device=dev, dtype=torch.float32)
+        grad = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            nbytes = int(lib().nphm_mlp_sdfgrad_workspace_bytes(self._h, B, N))
+            if nbytes < 0:
+                check(-1, 'nphm_mlp_sdfgrad_workspace_bytes')
+            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            check(lib().nphm_mlp_sdfgrad_forward(self._h, xyz.data_ptr(), cond.data_ptr(), B, N, sdf.data_ptr(), grad.data_ptr(),
+                                                 ws.data_ptr(), _stream_ptr(dev)), 'nphm_mlp_sdfgrad_forward')
+        return sdf, grad, ws
+
+    def sdfgrad_backward(self, ws: torch.Tensor, grad_sdf: torch.Tensor, grad_grad: torch.Tensor, weights: bool = True,
+                         biases: bool = True, want_cond: bool = True, want_xyz: bool = False):
+        """Backward of :meth:`sdfgrad_forward` (nphm_mlp_sdfgrad_backward) for grad_sdf B x N x 1 and grad_grad B x N x 3; the
+        workspace's tail is its scratch (all of its per-point memory), the part the forward filled stays as it was.
+        Returns ``(weight grads | None, bias grads | None, d/d cond B x lat_dim | None, d/d xyz B x N x 3 | None)``."""
+        B, N, _ = grad_grad.shape
+        dev = grad_grad.device
+        gs, gg = _f32c(grad_sdf), _f32c(grad_grad)
+        shapes = self.layer_shapes
+        gw = [torch.empty(s, device=dev, dtype=torch.float32) for s in shapes] if weights else None
+        gb = [torch.empty(s[0], device=dev, dtype=torch.float32) for s in shapes] if biases else None
+        g_cond = torch.empty(B, self.lat_dim, device=dev, dtype=torch.float32) if want_cond else None
+        g_xyz = torch.empty(B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None
+        with torch.cuda.device(dev):
+            check(lib().nphm_mlp_sdfgrad_backward(self._h, gs.data_ptr(), gg.data_ptr(), ws.data_ptr(), ws.numel(), B, N,
+                                                  _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
+                                                  _ptr(g_cond), _ptr(g_xyz), _stream_ptr(dev)), 'nphm_mlp_sdfgrad_backward')
         return gw, gb, g_cond, g_xyz
 
     def broyden_search(self, obs: torch.Tensor, cond: torch.Tensor, x_init: torch.Tensor, J_inv_init: torch.Tensor,

@@ -564,12 +564,15 @@ __global__ void pack_rows_kernel(const float *__restrict__ src, int ld, int widt
 // kGradExp: the adjoint shrinks layer by layer (~0.3x per 512-wide layer at initialisation), and an fp16 hi | lo pair only
 // keeps its 22 bits while |x| >= 2^-3 (below that lo is subnormal): the top of the chain starts at 2^10 so that d_0 is still
 // in that range, which leaves 2^5 of headroom below the fp16 maximum for an adjoint that grows instead.  One block.
+// g2 (optional, n2 values): the maximum is taken over both arrays.
 constexpr int kGradExp = 10;
-__global__ void grad_scale_kernel(const float *__restrict__ g, long long n, float *__restrict__ scale)
+__global__ void grad_scale_kernel(const float *__restrict__ g, long long n, const float *__restrict__ g2, long long n2,
+                                  float *__restrict__ scale)
 {
     __shared__ float red[32];
     float m = 0.f;
     for (long long i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(g[i]));
+    for (long long i = threadIdx.x; i < n2; i += blockDim.x) m = fmaxf(m, fabsf(g2[i]));
 #pragma unroll
     for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
@@ -644,6 +647,56 @@ static bool noise_layer(const StackDims &s, int l) { return l == 0 || l + 1 == s
 static const tcl::PackedLinear &layer(const MlpChain &c, const StackDims &s, int l)
 {
     return noise_layer(s, l) ? c.tfwd[l] : c.fwd[l];
+}
+
+// what the gradients of one layer need: the forward's workspace and the caller's outputs
+struct GradTargets {
+    nphm_mlp *h;
+    const Layout *L;
+    const uint8_t *ws;
+    int n_queries, nd;
+    long long n_points;
+    const float *gs;                          // device [scale, 1 / scale] of the adjoints
+    float *const *grad_w, *const *grad_b;
+    bool want_cond;
+};
+
+// weight, bias and condition-column gradients of layer l from its pre-activation adjoint d (packed, ks k-steps, scaled by
+// gs[0]); with (d2, h2): + d2^T h2 in the weight gradient (a second operand pair over the same rows and k-steps)
+static int layer_grads(const GradTargets &g, int l, const uint8_t *d, int ks, const uint8_t *d2, const uint8_t *h2,
+                       cudaStream_t stream)
+{
+    MlpChain &c = *g.h->chain;
+    const StackDims &s = g.h->dims;
+    const long long M = (long long)g.n_queries * g.n_points;
+    const int nd = g.nd;
+    float *gw = g.grad_w ? g.grad_w[l] : nullptr, *gb = g.grad_b ? g.grad_b[l] : nullptr;
+    const bool cond_layer = l == 0 || l == s.skip;
+    const float sc = l == s.skip ? chain::kInvSqrt2 : 1.0f;
+    const float *cond = reinterpret_cast<const float *>(g.ws + g.L->cond);
+    if (gw) {
+        const uint8_t *H = l == 0 ? g.ws + g.L->x0p : g.ws + g.L->hp[l - 1];
+        const int hks = l == 0 ? g.L->ks_x0 : g.L->ks_h[l - 1];
+        const int K = l == 0 ? 3 + nd : l == s.skip ? s.N[l - 1] + 3 + nd : s.N[l - 1];
+        int r = wgrad::launch(d, ks, H, hks, M, s.N[l], K, sc, g.gs + 1, gw, s.in_total[l], c.wg_partials, stream, d2, h2);
+        if (r) return r;
+    }
+    float *sums = l == 0 ? c.qsums0.as<float>() : l == s.skip ? c.qsumss.as<float>() : c.qsums.as<float>();
+    if (gb || (cond_layer && (gw || g.want_cond))) {
+        query_sums_kernel<<<dim3((unsigned)ks, (unsigned)g.n_queries), 256, 0, stream>>>(d, ks, g.n_points, s.N[l], g.gs, sums);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    if (gb) {
+        sum_queries_kernel<<<(unsigned)ceil_div(s.N[l], 128), 128, 0, stream>>>(sums, g.n_queries, s.N[l], gb);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    if (cond_layer && gw) {
+        const long long total = (long long)s.N[l] * s.cond_dim;
+        cond_outer_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(
+            sums, cond, g.n_queries, s.N[l], s.cond_dim, nd, sc, gw, s.in_total[l], l == 0 ? 3 : s.N[l - 1] + 3);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    return NPHM_OK;
 }
 
 // the training variants of layers 0, skip - 1 and skip for nd noise columns
@@ -741,12 +794,11 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
     const train::Layout L = train::layout(s, n_queries, n_points, nd);
     const long long M = (long long)n_queries * n_points;
     const int last = s.n_lin - 1, out_dim = s.N[last];
-    const float *cond = reinterpret_cast<const float *>(ws + L.cond);
 
     // upstream gradient scaled by 2^-e into the packed d_L
     if ((rc = c.gscale.reserve(2 * sizeof(float)))) return rc;
     const float *gs = c.gscale.as<float>();
-    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_out_dev, M * out_dim, c.gscale.as<float>());
+    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_out_dev, M * out_dim, nullptr, 0, c.gscale.as<float>());
     NPHM_CUDA_CHECK(cudaGetLastError());
     const int ks_out = (out_dim + 15) / 16;
     if ((rc = c.Dl.reserve(packed_bytes(M, ks_out)))) return rc;
@@ -766,35 +818,8 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
     if (grad_xyz_dev && ((rc = c.xtmp.reserve((size_t)M * 4 * sizeof(float))) || (rc = c.xs_tmp.reserve((size_t)M * 4 * sizeof(float)))))
         return rc;
 
-    // gradients of layer l from its pre-activation adjoint d (packed, ks k-steps, scaled by 2^-e)
-    auto layer_grads = [&](int l, const uint8_t *d, int ks) -> int {
-        float *gw = grad_w_dev ? grad_w_dev[l] : nullptr, *gb = grad_b_dev ? grad_b_dev[l] : nullptr;
-        const bool cond_layer = l == 0 || l == s.skip;
-        const float sc = l == s.skip ? chain::kInvSqrt2 : 1.0f;
-        if (gw) {
-            const uint8_t *H = l == 0 ? ws + L.x0p : ws + L.hp[l - 1];
-            const int hks = l == 0 ? L.ks_x0 : L.ks_h[l - 1];
-            const int K = l == 0 ? 3 + nd : l == s.skip ? s.N[l - 1] + 3 + nd : s.N[l - 1];
-            int r = wgrad::launch(d, ks, H, hks, M, s.N[l], K, sc, gs + 1, gw, s.in_total[l], c.wg_partials, stream);
-            if (r) return r;
-        }
-        float *sums = l == 0 ? c.qsums0.as<float>() : l == s.skip ? c.qsumss.as<float>() : c.qsums.as<float>();
-        if (gb || (cond_layer && (gw || grad_cond_dev))) {
-            train::query_sums_kernel<<<dim3((unsigned)ks, (unsigned)n_queries), 256, 0, stream>>>(d, ks, n_points, s.N[l], gs, sums);
-            NPHM_CUDA_CHECK(cudaGetLastError());
-        }
-        if (gb) {
-            train::sum_queries_kernel<<<(unsigned)ceil_div(s.N[l], 128), 128, 0, stream>>>(sums, n_queries, s.N[l], gb);
-            NPHM_CUDA_CHECK(cudaGetLastError());
-        }
-        if (cond_layer && gw) {
-            const long long total = (long long)s.N[l] * s.cond_dim;
-            train::cond_outer_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(
-                sums, cond, n_queries, s.N[l], s.cond_dim, nd, sc, gw, s.in_total[l], l == 0 ? 3 : s.N[l - 1] + 3);
-            NPHM_CUDA_CHECK(cudaGetLastError());
-        }
-        return NPHM_OK;
-    };
+    const train::GradTargets tg{h, &L, ws, n_queries, nd, n_points, gs, grad_w_dev, grad_b_dev, grad_cond_dev != nullptr};
+    auto layer_grads = [&](int l, const uint8_t *d, int ks) { return train::layer_grads(tg, l, d, ks, nullptr, nullptr, stream); };
 
     // d_{l-1} = s_{l-1} * (d_l W_l), from the output layer down to d_0; d_l lives in Dp[l & 1] (d_L in Dl)
     const uint8_t *d = c.Dl.as<uint8_t>();
@@ -837,6 +862,279 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
         if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
         train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(c.xtmp.as<float>(), c.xs_tmp.as<float>(), M, gs,
                                                                                   grad_xyz_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    return NPHM_OK;
+}
+
+// ================================================================================================ training through grad_x sdf
+// Stage 1 of the reference (scripts/training/train.py -> actual_compute_loss, src/NPHM/models/loss_functions.py:20-110)
+// reaches a DeepSDF decoder through s = f(x) and g = grad_x s.  With upstream gradients s_bar, g_bar per row,
+//   dL/dtheta = s_bar ds/dtheta + d/dtheta (g_bar . grad_x s),
+// and the second term is the gradient of a forward-mode tangent in the direction v = g_bar.  With z_l = W_l h_{l-1} + b_l,
+// h_l = softplus_100(z_l), S_l = sigmoid(100 z_l) (kept by the value pass) and softplus'' = 100 S (1 - S):
+//   forward   value pass (keeps h_l packed, S_l blocked), then the adjoint with unit upstream  a_L = 1,
+//             a_l = S_l * (W_{l+1}^T a_{l+1}) (kept packed): its bottom gives g through W_0[:, 0:3] and the skip's xyz columns
+//   backward  tangent pass  zt_l = W_l ht_{l-1}, ht_l = S_l * zt_l  (ht_{-1} = v; v appended at the skip)
+//             value adjoint zb_L = s_bar,  zb_l = S_l * (W_{l+1}^T zb_{l+1}) + 100 (1 - S_l) * zt_l * a_l
+//             dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1} (one GEMM over both pairs), db_l = sum zb_l, condition and xyz as the
+//             first-order backward does from zb
+// fp16 range: a starts at 2^kGradExp (the unit column), so it spends the chain where an fp16 hi | lo pair keeps its bits;
+// s_bar and g_bar (~1e-5 at the NPM batch) share one device-side power of two sigma that brings their largest magnitude to
+// 2^kGradExp (grad_scale_kernel over both).  The direction is v' = sigma 2^-kGradExp g_bar, so zt' a' and a' ht' carry the same
+// scale sigma as zb': the coupling keeps its plain coefficient 100 and the GEMM adds the two pairs as they are; the fp32
+// epilogues multiply by 1 / sigma.
+// Memory: everything per row lives in the caller's workspace, the backward's scratch included (its tail: the tangents, the
+// adjoint ping-pong, the direction), so it is counted and released by the caller's allocator; the handle keeps only
+// buffers of the layer widths (GEMM partials, per-query sums).
+namespace nphm {
+namespace sdfgrad {
+
+constexpr float kBeta = 100.0f;
+
+// workspace of one forward: the first-order training layout without noise, then the unit column, its scale pair and a_l;
+// then the scratch of the calls: ht_l packed (tg) and zt_l blocked fp32 (zg), the ping-pong of zb (dp), zb_L (dl), the
+// direction as rows of 4 (v4) and packed (vp), and two [M][4] point-gradient temporaries (xa, xb)
+struct Layout {
+    train::Layout base;
+    size_t unit = 0, consts = 0, a[kMaxLayers] = {}, total = 0;
+    int ks_a[kMaxLayers] = {}, ks_dp = 1;
+    size_t tg[kMaxLayers] = {}, zg[kMaxLayers] = {}, dp[2] = {}, dl = 0, v4 = 0, vp = 0, xa = 0, xb = 0;
+};
+
+static Layout layout(const StackDims &s, int n_queries, long long n_points)
+{
+    Layout G;
+    G.base = train::layout(s, n_queries, n_points, 0);
+    const long long tiles = ceil_div((long long)n_queries * n_points, 128);
+    size_t off = G.base.total;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
+    G.unit = take((size_t)tiles * 8192);
+    G.consts = take(2 * sizeof(float));
+    for (int l = 0; l + 1 < s.n_lin; ++l) {
+        G.ks_a[l] = (s.N[l] + 15) / 16;
+        G.a[l] = take((size_t)tiles * G.ks_a[l] * 8192);
+    }
+    const size_t M = (size_t)n_queries * n_points;
+    for (int l = 0; l + 1 < s.n_lin; ++l) {
+        G.tg[l] = take((size_t)tiles * G.base.ks_h[l] * 8192);
+        G.zg[l] = take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
+        G.ks_dp = std::max(G.ks_dp, G.ks_a[l]);                 // zb_l, l < L, in the operand format
+    }
+    for (int i = 0; i < 2; ++i) G.dp[i] = take((size_t)tiles * G.ks_dp * 8192);
+    G.dl = take((size_t)tiles * 8192);
+    G.vp = take((size_t)tiles * 8192);
+    G.v4 = take(M * 4 * sizeof(float));
+    G.xa = take(M * 4 * sizeof(float));
+    G.xb = take(M * 4 * sizeof(float));
+    G.total = off;
+    return G;
+}
+
+// packed one-column operand (1 k-step): column 0 = 2^kGradExp on the rows < M, everything else 0; consts = {2^E, 2^-E}.
+// Thread = row of the padded tiles.
+__global__ void unit_column_kernel(long long M, uint8_t *__restrict__ dst, float *__restrict__ consts)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0) { consts[0] = ldexpf(1.0f, train::kGradExp); consts[1] = ldexpf(1.0f, -train::kGradExp); }
+    if (r >= (M + 127) / 128 * 128) return;
+    const __half v = __float2half_rn(r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
+    const uint32_t w0 = (uint32_t)__half_as_ushort(v);
+    uint8_t *d = dst + (size_t)(r >> 7) * 8192 + (size_t)((r & 127) >> 3) * 256 + (r & 7) * 16;
+    *reinterpret_cast<uint4 *>(d) = make_uint4(w0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(d + 128) = make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(d + 4096 + 128) = make_uint4(0, 0, 0, 0);
+}
+
+// V[r] = (g_bar[r] * scale[0] * 2^-kGradExp, 0): the tangent direction, ld 4
+__global__ void direction_kernel(const float *__restrict__ gg, long long M, const float *__restrict__ scale, float *__restrict__ V)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= M * 4) return;
+    const long long r = idx >> 2;
+    const int c = (int)(idx & 3);
+    V[idx] = c < 3 ? gg[r * 3 + c] * (scale[0] * ldexpf(1.0f, -train::kGradExp)) : 0.f;
+}
+
+static int ready(nphm_mlp *h, const char *who)
+{
+    int rc = chain_ready(h, who);
+    if (rc) return rc;
+    if (h->dims.N[h->dims.n_lin - 1] != 1) {
+        set_error("%s: needs a stack with one output (an SDF), this one has %d", who, h->dims.N[h->dims.n_lin - 1]);
+        return NPHM_ERR_UNSUPPORTED;
+    }
+    return NPHM_OK;
+}
+
+}  // namespace sdfgrad
+}  // namespace nphm
+
+extern "C" long long nphm_mlp_sdfgrad_workspace_bytes(const nphm_mlp *h, int n_queries, long long n_points)
+{
+    if (!h || !h->loaded || n_queries < 1 || n_points < 1) {
+        set_error("nphm_mlp_sdfgrad_workspace_bytes: bad arguments");
+        return -1;
+    }
+    return (long long)sdfgrad::layout(h->dims, n_queries, n_points).total;
+}
+
+extern "C" int nphm_mlp_sdfgrad_forward(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
+                                        float *sdf_out_dev, float *grad_out_dev, void *workspace_dev, void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = sdfgrad::ready(h, "nphm_mlp_sdfgrad_forward");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && sdf_out_dev && grad_out_dev && workspace_dev,
+                 "nphm_mlp_sdfgrad_forward: bad arguments");
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    const sdfgrad::Layout G = sdfgrad::layout(s, n_queries, n_points);
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const long long M = (long long)n_queries * n_points;
+    // value pass: the first-order training forward fills the leading part of the workspace
+    if ((rc = nphm_mlp_train_forward(h, xyz_dev, cond_dev, nullptr, 0, n_queries, n_points, sdf_out_dev, ws, stream_))) return rc;
+    float *consts = reinterpret_cast<float *>(ws + G.consts);
+    sdfgrad::unit_column_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128, 256), 256, 0, stream>>>(M, ws + G.unit, consts);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    float *xa = reinterpret_cast<float *>(ws + G.xa), *xb = reinterpret_cast<float *>(ws + G.xb);
+    // a_{l-1} = S_{l-1} * (a_l W_l) from the unit column down to a_0, kept in the workspace
+    const uint8_t *d = ws + G.unit;
+    int ks = 1;
+    for (int l = s.n_lin - 1; l >= 1; --l) {
+        if (l == s.skip) {
+            tcl::LinearParams px;
+            px.M = M;
+            px.Ap = d; px.a_ksteps = ks;
+            px.mode = tcl::kModeLinear; px.C = xb; px.ldc = 4;
+            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+        }
+        tcl::LinearParams p;
+        p.M = M;
+        p.Ap = d; p.a_ksteps = ks;
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + G.base.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
+        p.Cp = ws + G.a[l - 1]; p.c_ksteps = G.ks_a[l - 1];
+        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
+        d = ws + G.a[l - 1];
+        ks = G.ks_a[l - 1];
+    }
+    tcl::LinearParams px;
+    px.M = M;
+    px.Ap = d; px.a_ksteps = ks;
+    px.mode = tcl::kModeLinear; px.C = xa; px.ldc = 4;
+    if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
+    train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(xa, xb, M, consts, grad_out_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
+                                         long long workspace_bytes, int n_queries, long long n_points, float *const *grad_w_dev,
+                                         float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = sdfgrad::ready(h, "nphm_mlp_sdfgrad_backward");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && grad_sdf_dev && grad_grad_dev && workspace_dev,
+                 "nphm_mlp_sdfgrad_backward: bad arguments");
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    // the caller states the shape the workspace was made for; checked against its size, without reading it back
+    NPHM_REQUIRE(workspace_bytes == (long long)sdfgrad::layout(s, n_queries, n_points).total,
+                 "nphm_mlp_sdfgrad_backward: a workspace of %lld bytes does not hold an SDF-gradient forward of this network at "
+                 "%d x %lld points", workspace_bytes, n_queries, n_points);
+    const sdfgrad::Layout G = sdfgrad::layout(s, n_queries, n_points);
+    const train::Layout &L = G.base;
+    const long long M = (long long)n_queries * n_points, tiles = ceil_div(M, 128);
+    const int last = s.n_lin - 1;
+    if ((rc = train::pack(h, 0, stream))) return rc;
+
+    // one power of two for both upstream gradients; zb_L = s_bar packed, the direction as rows and packed
+    if ((rc = c.gscale.reserve(2 * sizeof(float)))) return rc;
+    const float *gs = c.gscale.as<float>();
+    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_sdf_dev, M, grad_grad_dev, M * 3, c.gscale.as<float>());
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    uint8_t *const dl = ws + G.dl, *const vp = ws + G.vp;
+    float *const v4 = reinterpret_cast<float *>(ws + G.v4);
+    float *const xa = reinterpret_cast<float *>(ws + G.xa), *const xb = reinterpret_cast<float *>(ws + G.xb);
+    auto tg = [&](int l) { return ws + G.tg[l]; };
+    auto zg = [&](int l) { return reinterpret_cast<float *>(ws + G.zg[l]); };
+    const unsigned pack_blocks = (unsigned)ceil_div(tiles * 128 * 2, 256);
+    train::pack_rows_kernel<<<pack_blocks, 256, 0, stream>>>(grad_sdf_dev, 1, 1, M, 1, gs, dl);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    sdfgrad::direction_kernel<<<(unsigned)ceil_div(M * 4, 256), 256, 0, stream>>>(grad_grad_dev, M, gs, v4);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    train::pack_rows_kernel<<<pack_blocks, 256, 0, stream>>>(v4, 4, 3, M, 1, nullptr, vp);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+
+    // tangent pass: ht_l packed (tg, the next layer's input and the GEMM's second H), zt_l blocked fp32 (zg)
+    for (int l = 0; l < last; ++l) {
+        const tcl::PackedLinear &W = train::layer(c, s, l);
+        tcl::LinearParams p;
+        p.M = M;
+        if (l == 0) { p.A1 = v4; p.lda1 = 4; p.K1 = 3; }
+        else { p.Ap = tg(l - 1); p.a_ksteps = W.ksteps; }
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + L.s[l]); p.ldmul = c.ld[l]; p.mul_div = 1; p.mul_blocked = 1;
+        p.Cp = tg(l); p.c_ksteps = L.ks_h[l];
+        if (l + 1 == s.skip) { p.app = v4; p.app_ld = 4; p.app_w = 3; }
+        p.Dv = zg(l); p.lddv = c.ld[l]; p.dv_blocked = 1;
+        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
+    }
+
+    int max_n = 1;
+    for (int l = 0; l <= last; ++l) max_n = std::max(max_n, s.N[l]);
+    if ((rc = c.qsums.reserve((size_t)n_queries * max_n * sizeof(float))) ||
+        (rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
+        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
+        return rc;
+    const train::GradTargets targets{h, &L, ws, n_queries, 0, n_points, gs, grad_w_dev, grad_b_dev, grad_cond_dev != nullptr};
+
+    // value adjoint with the coupling, from zb_L = s_bar down to zb_0; zb_l lives in dp[l & 1] (zb_L in dl)
+    const uint8_t *d = dl;
+    int ks = 1;
+    for (int l = last; l >= 1; --l) {
+        const uint8_t *a = l == last ? ws + G.unit : ws + G.a[l];
+        if ((rc = train::layer_grads(targets, l, d, ks, a, tg(l - 1), stream))) return rc;
+        if (l == s.skip && grad_xyz_dev) {
+            tcl::LinearParams px;
+            px.M = M;
+            px.Ap = d; px.a_ksteps = ks;
+            px.mode = tcl::kModeLinear; px.C = xb; px.ldc = 4;
+            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+        }
+        tcl::LinearParams p;
+        p.M = M;
+        p.Ap = d; p.a_ksteps = ks;
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + L.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
+        p.cpl_z = zg(l - 1); p.cpl_a = ws + G.a[l - 1]; p.cpl_a_steps = G.ks_a[l - 1]; p.cpl_coef = sdfgrad::kBeta;
+        const int ks_next = (s.N[l - 1] + 15) / 16;
+        p.Cp = ws + G.dp[(l - 1) & 1]; p.c_ksteps = ks_next;
+        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
+        d = ws + G.dp[(l - 1) & 1];
+        ks = ks_next;
+    }
+    if ((rc = train::layer_grads(targets, 0, d, ks, ws + G.a[0], vp, stream))) return rc;
+    if (grad_cond_dev) {
+        NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
+        dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 1);          // one chunk: a fixed summation order
+        chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
+                                                          h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
+                                                          s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    if (grad_xyz_dev) {
+        // s_bar g + H v: the point gradient of zb, as in the first-order backward
+        tcl::LinearParams px;
+        px.M = M;
+        px.Ap = d; px.a_ksteps = ks;
+        px.mode = tcl::kModeLinear; px.C = xa; px.ldc = 4;
+        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
+        train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(xa, xb, M, gs, grad_xyz_dev);
         NPHM_CUDA_CHECK(cudaGetLastError());
     }
     return NPHM_OK;

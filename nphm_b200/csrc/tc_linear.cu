@@ -21,6 +21,7 @@
 //   epilogue modes:  LINEAR   C = t + bias[row / rows_per_bias][n]
 //                    SOFTPLUS C = softplus_100(t + bias), optionally D = sigmoid(100 (t + bias))   (the activation's derivative)
 //                    MULT     C = t * Mul[row / mul_div][n]                                         (tangent / adjoint passes)
+//                             (+ coef (1 - Mul) z a: the second-order coupling of the SDF-gradient training backward)
 #include "tc_linear.cuh"
 #include <cuda_fp16.h>
 #include <type_traits>
@@ -330,6 +331,26 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
             }
             TCL_EVT(threadIdx.x == 0, 11, c0 >> 4);
             if (!row_ok) return;
+            // second-order coupling: cpl = coef * z * a of this row's 16 features (a: hi + lo of the packed operand)
+            float cpl[16];
+            const bool coupled = MODE == kModeMult && p.cpl_z && ((n0 + c0) >> 4) < p.cpl_a_steps;
+            if (coupled) {
+                const float *zb = p.cpl_z + (size_t)blockIdx.x * p.ldmul * 128 + (size_t)(n0 + c0) * 128 + t;
+                const uint8_t *ab = p.cpl_a + ((size_t)blockIdx.x * p.cpl_a_steps + ((n0 + c0) >> 4)) * kPackedStep +
+                                    (size_t)(t >> 3) * 256 + (size_t)(t & 7) * 16;
+                const uint4 h0 = *reinterpret_cast<const uint4 *>(ab), h1 = *reinterpret_cast<const uint4 *>(ab + 128);
+                const uint4 l0 = *reinterpret_cast<const uint4 *>(ab + 4096), l1 = *reinterpret_cast<const uint4 *>(ab + 4096 + 128);
+                const uint32_t hw[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+                const uint32_t lw[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&hw[i]));
+                    const float2 b = __half22float2(*reinterpret_cast<const __half2 *>(&lw[i]));
+                    const bool ok0 = FULL || n0 + c0 + 2 * i < p.N, ok1 = FULL || n0 + c0 + 2 * i + 1 < p.N;
+                    cpl[2 * i] = ok0 ? p.cpl_coef * zb[(size_t)(2 * i) * 128] * (a.x + b.x) : 0.f;
+                    cpl[2 * i + 1] = ok1 ? p.cpl_coef * zb[(size_t)(2 * i + 1) * 128] * (a.y + b.y) : 0.f;
+                }
+            }
             float o[16], dv[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) {
@@ -342,8 +363,11 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
                     if (a < p.app_w) x = p.app_onehot ? (a == app_hot ? 1.f : 0.f) : (app ? app[a] : 0.f);
                 }
                 if (FULL || n0 + c0 + e < p.N) {
-                    if (MODE == kModeMult) x *= aux[e] * rscale;
-                    else {
+                    if (MODE == kModeMult) {
+                        dv[e] = x;
+                        x *= aux[e] * rscale;
+                        if (coupled) x = fmaf(1.0f - aux[e], cpl[e], x);
+                    } else {
                         x += aux[e];
                         if (MODE == kModeSoftplus) {
                             // softplus(beta = 100) and its derivative in log2 units: u = 100 log2(e) x
@@ -498,6 +522,9 @@ int launch_linear(const PackedLinear &w, LinearParams p, cudaStream_t stream)
                  "tc_linear: packed output misconfigured");
     NPHM_REQUIRE(p.app_w == 0 || p.Cp, "tc_linear: appended columns need a packed output");
     NPHM_REQUIRE(p.mode != kModeMult || (p.Mul && p.mul_div > 0), "tc_linear: multiplier missing");
+    NPHM_REQUIRE(!p.cpl_z || (p.mode == kModeMult && p.cpl_a && p.cpl_a_steps > 0 && (p.blocked || p.mul_blocked) && p.mul_div <= 1 &&
+                              p.batch == 1),
+                 "tc_linear: the coupling term needs the multiplier epilogue with a blocked multiplier, one row per multiplier row");
     NPHM_REQUIRE(!p.blocked || (!p.bias && !p.A2 && !p.a2_onehot && p.mul_div <= 1),
                  "tc_linear: the blocked layout supports the plain and the multiplier epilogue only");
     NPHM_REQUIRE(p.batch >= 1 && (p.batch == 1 || (!p.Dv && !p.bias && !p.A2 && !p.a2_onehot && !p.app)),

@@ -16,10 +16,14 @@ struct LinearParams {
     const float *bias = nullptr; int ldb = 0; long long rows_per_bias = 0;   // bias row = row / rows_per_bias (0: one row for all)
     int mode = kModeLinear;
     float *C = nullptr; int ldc = 0;
-    float *Dv = nullptr; int lddv = 0;                       // SOFTPLUS: derivative of the activation (optional)
+    float *Dv = nullptr; int lddv = 0;                       // SOFTPLUS: derivative of the activation (optional); MULT: below
     const float *Mul = nullptr; int ldmul = 0; long long mul_div = 1;        // MULT: C = t * Mul[row / mul_div][n]
     const float *row_scale = nullptr;                        // MULT: additional factor row_scale[row]
     int mul_blocked = 0, dv_blocked = 0;                     // Mul / Dv alone in the blocked layout (see `blocked`)
+    // MULT, second-order coupling (native SDF-gradient training):  C = t * Mul + cpl_coef * (1 - Mul) * cpl_z * cpl_a, with
+    // cpl_z blocked fp32 (ld = ldmul) and cpl_a packed (cpl_a_steps k-steps per tile), both over the rows and features of C.
+    // MULT with Dv: Dv = t, the product before the multiplier (a tangent pass keeps its pre-activation tangents).
+    const float *cpl_z = nullptr; const uint8_t *cpl_a = nullptr; int cpl_a_steps = 0; float cpl_coef = 0.f;
     // operand-ready ("packed") activations: per 128-row tile and k-step 8 KB = [128 x 16 fp16 hi | 128 x 16 fp16 lo] in K-major core-
     // matrix order.  Cp: the epilogue writes its output split like that (unit u of 16 columns = k-step u of the next layer), so
     // the next launch takes it as Ap with one bulk copy per k-step and no conversion work in its main loop.

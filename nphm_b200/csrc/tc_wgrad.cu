@@ -10,6 +10,9 @@
 // (M = 3 200 .. 35 200 per call) are split over gridDim.y so that the few output tiles of a layer still fill the GPU.  Each
 // CTA streams its 128-row tiles through a two-stage cp.async ring (32 KB of D | 32 KB of H per stage; rows beyond M are
 // zero-filled) and writes its partial sums; a second kernel adds the partials in split order.
+//
+// Two operand pairs (dW = D^T H + D2^T H2, the SDF-gradient training backward): the row tiles of the second pair follow
+// those of the first in one sequence of 2 x row_tiles tiles, so the sum is taken in one fixed order.
 #include "tc_wgrad.cuh"
 #include "tc_common.cuh"
 
@@ -43,23 +46,26 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
 }
 
 // partial[split][n][k] (ld kb_count * 64) of output tile (blockIdx.x / kb_count, blockIdx.x % kb_count) over row tiles
-// [split * tiles_per_split, ...)
+// [split * tiles_per_split, ...) of the row_tiles tiles of (D, H) followed, with D2 given, by the row_tiles tiles of (D2, H2)
 __global__ void __launch_bounds__(kThreads) wgrad_kernel(const uint8_t *__restrict__ D, int ks_d, const uint8_t *__restrict__ H,
-                                                         int ks_h, long long M, int row_tiles, int tiles_per_split, int nb_count,
+                                                         int ks_h, const uint8_t *__restrict__ D2, const uint8_t *__restrict__ H2,
+                                                         long long M, int row_tiles, int tiles_per_split, int nb_count,
                                                          int kb_count, float *__restrict__ partial)
 {
     extern __shared__ __align__(128) uint8_t smem[];
     const int nb = blockIdx.x / kb_count, kb = blockIdx.x % kb_count, split = blockIdx.y;
-    const int t0 = split * tiles_per_split, t1 = min(row_tiles, t0 + tiles_per_split);
+    const int t0 = split * tiles_per_split, t1 = min(D2 ? 2 * row_tiles : row_tiles, t0 + tiles_per_split);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wn = warp >> 1, wk = warp & 1;
 
     // one stage: 2 operands x 4 k-steps x 512 lines of 16 bytes; line -> row of the tile: ((line & 255) >> 4) * 8 + (line & 7)
     auto load = [&](int t, int s) {
         const uint32_t dst0 = smem_u32(smem + (size_t)s * kStageBytes);
+        const bool second = t >= row_tiles;
+        if (second) t -= row_tiles;
         for (int i = threadIdx.x; i < 2 * 4 * 512; i += kThreads) {
             const int op = i >> 11, u = (i >> 9) & 3, line = i & 511;
-            const uint8_t *base = op ? H : D;
+            const uint8_t *base = op ? (second ? H2 : H) : (second ? D2 : D);
             const int ks = op ? ks_h : ks_d, j = (op ? kb : nb) * 4 + u;
             const int r = ((line & 255) >> 4) * 8 + (line & 7);
             const bool ok = j < ks && (long long)t * 128 + r < M;
@@ -143,15 +149,16 @@ __global__ void wgrad_finish_kernel(const float *__restrict__ partial, int split
 }
 
 int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
-           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream)
+           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream, const uint8_t *D2,
+           const uint8_t *H2)
 {
-    NPHM_REQUIRE(M > 0 && N <= d_ksteps * 16 && K <= h_ksteps * 16, "wgrad: bad operand shapes");
+    NPHM_REQUIRE(M > 0 && N <= d_ksteps * 16 && K <= h_ksteps * 16 && !D2 == !H2, "wgrad: bad operand shapes");
     const int nb_count = (d_ksteps + 3) / 4, kb_count = (h_ksteps + 3) / 4;
-    const int row_tiles = (int)ceil_div(M, 128);
+    const int row_tiles = (int)ceil_div(M, 128), all_tiles = D2 ? 2 * row_tiles : row_tiles;
     const int tiles = nb_count * kb_count;
-    int splits = std::max(1, std::min(row_tiles, (int)ceil_div(2LL * sm_count(), tiles)));
-    const int tiles_per_split = (int)ceil_div(row_tiles, splits);
-    splits = (int)ceil_div(row_tiles, tiles_per_split);
+    int splits = std::max(1, std::min(all_tiles, (int)ceil_div(2LL * sm_count(), tiles)));
+    const int tiles_per_split = (int)ceil_div(all_tiles, splits);
+    splits = (int)ceil_div(all_tiles, tiles_per_split);
     const int ldn = nb_count * kTile, ldk = kb_count * kTile;
     int rc;
     if ((rc = partials.reserve((size_t)splits * ldn * ldk * sizeof(float)))) return rc;
@@ -162,7 +169,7 @@ int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long 
         NPHM_CUDA_CHECK(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
         if (dev < 64) smem_set[dev] = true;
     }
-    wgrad_kernel<<<dim3(tiles, splits), kThreads, kSmem, stream>>>(D, d_ksteps, H, h_ksteps, M, row_tiles, tiles_per_split,
+    wgrad_kernel<<<dim3(tiles, splits), kThreads, kSmem, stream>>>(D, d_ksteps, H, h_ksteps, D2, H2, M, row_tiles, tiles_per_split,
                                                                    nb_count, kb_count, partials.as<float>());
     NPHM_CUDA_CHECK(cudaGetLastError());
     const long long total = (long long)N * K;

@@ -9,8 +9,11 @@ namespace wgrad {
 // operand format of tc_linear.cuh.  Writes dW[n * ldw + k] for n < N, k < K:  scale * inv_scale_dev[0] * (D^T H)[n][k].
 // The rows are split over the CTAs; the partial sums go to `partials` and are added in a fixed order (no atomics), so equal
 // inputs give bitwise-equal gradients.  `partials`: scratch, grown on demand.
+// D2, H2 (optional, both or neither; same k-steps and rows as D, H): a second pair, dW = scale * inv_scale (D^T H + D2^T H2),
+// accumulated in the same fixed order (all row tiles of the first pair, then those of the second).
 int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
-           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream);
+           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream,
+           const uint8_t *D2 = nullptr, const uint8_t *H2 = nullptr);
 
 }  // namespace wgrad
 }  // namespace nphm

@@ -11,6 +11,8 @@ As in :mod:`.EnsembledDeepSDF`, CUDA no-grad calls with a per-query-constant con
 the native sm_90a MLP path; everything else uses a PyTorch composite that keeps autograd.
 ``forward_native_grad`` is the explicit first-order training path: native forward and native
 backward (weight, bias, condition and point gradients), for a condition that is constant per query.
+``DeepSDF.forward_with_gradient_native`` returns the SDF and its spatial gradient; its backward differentiates both
+(the second-order terms of the stage-1 loss) natively.
 """
 from __future__ import annotations
 
@@ -64,6 +66,42 @@ class _NativeTrainFn(torch.autograd.Function):
 
 
 _native_backward_once = once_differentiable(_native_backward)
+
+
+def _sdfgrad_backward(ctx, grad_sdf, grad_grad):
+    ws, *params = ctx.saved_tensors                   # raises if a parameter was changed in place since the forward
+    need = ctx.needs_input_grad                       # (engine, xyz, cond, lin0.weight, lin0.bias, ...)
+    gw, gb, g_cond, g_xyz = ctx.engine.sdfgrad_backward(ws, grad_sdf, grad_grad, weights=any(need[3::2]), biases=any(need[4::2]),
+                                                        want_cond=need[2], want_xyz=need[1])
+    grads = [None, g_xyz, g_cond]
+    for i in range(len(params) // 2):
+        grads.append(gw[i] if need[3 + 2 * i] else None)
+        grads.append(gb[i] if need[4 + 2 * i] else None)
+    return tuple(grads)
+
+
+_sdfgrad_backward_once = once_differentiable(_sdfgrad_backward)
+
+
+class _NativeSdfGradFn(torch.autograd.Function):
+    """One-output ``DeepSDF`` stack on the native kernels (``nphm_mlp_sdfgrad_forward`` / ``_backward``): xyz B x N x 3,
+    cond B x lat_dim, then the ``lin{l}.weight / bias`` parameters -> (sdf B x N x 1, d sdf / d xyz B x N x 3).  The backward
+    takes upstream gradients of both outputs (the weight gradient of the gradient output is the second-order part);
+    differentiable to first order only."""
+
+    @staticmethod
+    def forward(ctx, engine, xyz, cond, *params):
+        sdf, grad, ws = engine.sdfgrad_forward(xyz, cond)
+        ctx.engine = engine
+        ctx.save_for_backward(ws, *params)
+        return sdf, grad
+
+    @staticmethod
+    def backward(ctx, grad_sdf, grad_grad):
+        if torch.is_grad_enabled():
+            raise RuntimeError('forward_with_gradient_native is differentiable to first order only: a double backward '
+                               '(create_graph=True) through it is not supported; use the composite forward() instead')
+        return _sdfgrad_backward_once(ctx, grad_sdf, grad_grad)
 
 
 class DeepSDF(nn.Module):
@@ -155,6 +193,29 @@ class DeepSDF(nn.Module):
         if cond is None:
             raise ValueError('forward_native_grad: the condition must be constant over the points of a query')
         return self._native_train(xyz, cond), None
+
+    def sdfgrad_supported(self, xyz, lat_rep=None) -> bool:
+        """Whether :meth:`forward_with_gradient_native` takes these points: what :meth:`native_grad_supported` asks, and
+        one output."""
+        return self.out_dim_net == 1 and self.native_grad_supported(xyz, lat_rep)
+
+    def forward_with_gradient_native(self, xyz, lat_rep):
+        """``(sdf B x N x 1, d sdf / d xyz B x N x 3)`` on the native kernels: the reference's ``forward`` followed by
+        ``gradient(sdf, xyz)`` (diff_operators.py), differentiable to first order in the parameters, ``lat_rep`` and ``xyz``,
+        so a loss on the gradient (normals, eikonal) trains the weights without a double backward in PyTorch.  ``lat_rep``
+        as in :meth:`forward_native_grad`.  Raises ``ValueError`` for a stack or input it does not support (more than one
+        output, ReLU, positional encoding, not CUDA fp32)."""
+        if not self.sdfgrad_supported(xyz, lat_rep):
+            raise ValueError('forward_with_gradient_native: unsupported input or network (needs CUDA fp32 B x N x 3 points, '
+                             'one output, no positional encoding, Softplus(beta=100), a stack the native builder accepts)')
+        cond = _native.constant_latent_rows(lat_rep)
+        if cond is None:
+            raise ValueError('forward_with_gradient_native: the condition must be constant over the points of a query')
+        params = []
+        for i in range(self.num_layers - 1):
+            lin = getattr(self, 'lin%d' % i)
+            params += [lin.weight, lin.bias]
+        return _NativeSdfGradFn.apply(self.engine(), xyz, cond, *params)
 
     def forward(self, xyz, lat_rep, anchors=None):
         if self._fused_ok(xyz, lat_rep):

@@ -16,6 +16,11 @@ ensemble - ``anchors``, ``symm_dist``, ``middle_dist``).  Two ways to get the SD
   * **composite** (training): the decoder's autograd path and ``diff_operators.gradient`` with ``create_graph=True`` -
     weight gradients of the normal / eikonal terms need the double backward, which stays in PyTorch.
 
+With ``native=True`` and a ``DeepSDF`` decoder (the NPM baseline) the loss takes a third way, with or without autograd:
+``DeepSDF.forward_with_gradient_native`` evaluates the four point sets in one call (concatenated along the points of each
+query) and differentiates the SDF and its spatial gradient natively, second-order terms included.  ``native=None`` keeps the
+composite path for it.
+
 ``compute_loss_corresp_forward`` is first order (no gradient with respect to the points is used), so its decoder calls run
 natively to the weights: ``DeformationNetwork.forward_native_grad`` (forward and backward on the tensor cores, the compressor
 and the embeddings in autograd).  ``native=None`` picks that path for a CUDA fp32 decoder the native chain supports,
@@ -29,6 +34,7 @@ from __future__ import annotations
 import torch
 
 from .EnsembledDeepSDF import FastEnsembleDeepSDFMirrored
+from .deepSDF import DeepSDF
 from .diff_operators import gradient
 
 _POINT_SETS = ('points_face', 'points_non_face', 'sup_grad_near', 'sup_grad_far')
@@ -67,15 +73,30 @@ def _pair_distance(latents):
     return torch.norm(latents[:, 0:n:2, :] - latents[:, 1:n:2, :], dim=-1).mean()
 
 
+def _sdfgrad_native(decoder, batch_cuda, glob_cond):
+    """All four point sets in one ``forward_with_gradient_native`` call -> ({name: sdf}, {name: d sdf / d x})."""
+    sets = [batch_cuda[name] for name in _POINT_SETS]
+    pts = torch.cat(sets, dim=1)
+    if not (glob_cond.dim() == 3 and glob_cond.shape[1] == 1 and decoder.sdfgrad_supported(pts, glob_cond)):
+        raise ValueError('actual_compute_loss(native=True): this DeepSDF decoder / batch is not supported natively (needs '
+                         'CUDA fp32 points, one output, Softplus(beta=100), no positional encoding, B x 1 x D codes)')
+    sdf, g = decoder.forward_with_gradient_native(pts, glob_cond)
+    sizes = [p.shape[1] for p in sets]
+    return dict(zip(_POINT_SETS, sdf.split(sizes, dim=1))), dict(zip(_POINT_SETS, g.split(sizes, dim=1)))
+
+
 def actual_compute_loss(batch_cuda, decoder, glob_cond, native=None):
     is_ensemble = isinstance(decoder, FastEnsembleDeepSDFMirrored)
     anchor_preds = batch_cuda['gt_anchors'] if hasattr(decoder, 'anchors') else None
+    sdfgrad = native is not None and bool(native) and isinstance(decoder, DeepSDF)
     if native is None:
         native = not torch.is_grad_enabled()
     native = bool(native) and is_ensemble and decoder.training and batch_cuda['points_face'].is_cuda
 
     pred, grad, anchors = {}, {}, None
-    if native:
+    if sdfgrad:
+        pred, grad = _sdfgrad_native(decoder, batch_cuda, glob_cond)
+    elif native:
         with torch.no_grad():
             for name in _POINT_SETS:
                 pred[name], grad[name] = _native_values_and_gradients(decoder, batch_cuda[name], glob_cond)
