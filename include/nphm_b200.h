@@ -276,6 +276,21 @@ int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev, const floa
                               long long workspace_bytes, int n_queries, long long n_points, float *const *grad_w_dev,
                               float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream);
 
+/* ---- fitting with a one-output DeepSDF stack (the NPM baseline's identity decoder): the surface term of
+ * inference_identity_space and inference_iterative_root_finding_joint (reference src/NPHM/models/fitting.py:114-125, :229-247)
+ *   loss = mean over { p : mask[p] != 0 and |s_p| < clamp } of |s_p|,   s = f(xyz, cond)
+ * Stacks with out_dim != 1 are rejected with NPHM_ERR_UNSUPPORTED. */
+/* bytes of the workspace of one nphm_mlp_fit_surface_grad call (-1: bad arguments) */
+long long nphm_mlp_fit_workspace_bytes(const nphm_mlp *h, int n_queries, long long n_points);
+/* xyz_dev [q][n][3], cond_dev [q][lat_dim], mask_dev [q*n] bytes (may be NULL = all valid).  loss_terms_dev[0] = loss (NaN if
+ * nothing is kept, like torch), [5] = number of kept points, [1..4] = 0 (the layout of nphm_fit_surface_grad).
+ * grad_cond_dev [q][lat_dim] = d loss / d cond_q (summed over the points of the query), grad_xyz_dev [q][n][3] (may be NULL);
+ * both exactly zero when nothing is kept.  All per-point memory is the caller's workspace; workspace_bytes is checked against
+ * the shape (NPHM_ERR_INVALID on a mismatch).  Bitwise deterministic; nothing is read back from the device. */
+int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
+                              const unsigned char *mask_dev, float clamp, float *loss_terms_dev, float *grad_cond_dev,
+                              float *grad_xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream);
+
 /* anchors_dev [n_queries][n_loc][3] = mlp_pos(z_glob) + mean anchors (reference src/NPHM/models/EnsembledDeepSDF.py:228-229)
  * without evaluating the ensemble - what the fitters read from `decoder(zeros(1,1,3), lat)[1]` (fitting.py:59, :211). */
 int nphm_ensemble_anchors(nphm_ensemble *h, const float *latents_dev, int n_queries, float *anchors_dev, void *stream);

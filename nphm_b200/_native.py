@@ -35,6 +35,7 @@ EXPORTED_SYMBOLS = (
     'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
     'nphm_mlp_sdfgrad_workspace_bytes', 'nphm_mlp_sdfgrad_forward', 'nphm_mlp_sdfgrad_backward',
+    'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad',
 )
 
 
@@ -162,6 +163,10 @@ def lib() -> ctypes.CDLL:
     L.nphm_mlp_sdfgrad_forward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p]
     L.nphm_mlp_sdfgrad_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_longlong, POINTER(c_void_p),
                                             POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
+    L.nphm_mlp_fit_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong]
+    L.nphm_mlp_fit_workspace_bytes.restype = c_longlong
+    L.nphm_mlp_fit_surface_grad.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_float, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_longlong, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -543,6 +548,36 @@ class MlpEngine(_Versioned):
                                                   _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
                                                   _ptr(g_cond), _ptr(g_xyz), _stream_ptr(dev)), 'nphm_mlp_sdfgrad_backward')
         return gw, gb, g_cond, g_xyz
+
+    # ------------------------------------------------------------ fitting (surface term of a one-output stack)
+    def fit_workspace(self, n_queries: int, n_points: int, device) -> torch.Tensor:
+        """A workspace for :meth:`fit_surface_grad` at ``n_queries x n_points`` (a uint8 CUDA tensor the caller may keep)."""
+        nbytes = int(lib().nphm_mlp_fit_workspace_bytes(self._h, int(n_queries), int(n_points)))
+        if nbytes < 0:
+            check(-1, 'nphm_mlp_fit_workspace_bytes')
+        return torch.empty(nbytes, device=device, dtype=torch.uint8)
+
+    def fit_surface_grad(self, xyz: torch.Tensor, cond: torch.Tensor, mask: Optional[torch.Tensor], clamp: float,
+                         want_xyz: bool = True, workspace: Optional[torch.Tensor] = None, out=None):
+        """Surface term of the fitters (nphm_mlp_fit_surface_grad): ``mean |s|`` over the points with ``mask != 0`` and
+        ``|s| < clamp``, xyz B x N x 3, cond B x lat_dim, mask B x N (or None: all valid).  Returns
+        ``(loss_terms (8,): [0] loss (NaN if nothing is kept), [5] kept count;  d loss / d cond  B x lat_dim;
+        d loss / d xyz  B x N x 3 | None)``.  ``workspace`` / ``out`` (a tuple like the result) let a loop reuse its buffers."""
+        B, N, _ = xyz.shape
+        dev = xyz.device
+        xyz = _f32c(xyz)
+        cond = _f32c(cond).to(dev)
+        m = None if mask is None else mask.reshape(-1).to(torch.uint8).contiguous()
+        if out is None:
+            out = (torch.zeros(8, device=dev, dtype=torch.float32), torch.empty(B, self.lat_dim, device=dev, dtype=torch.float32),
+                   torch.empty(B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None)
+        terms, g_cond, g_xyz = out
+        with torch.cuda.device(dev):
+            ws = self.fit_workspace(B, N, dev) if workspace is None else workspace
+            check(lib().nphm_mlp_fit_surface_grad(self._h, xyz.data_ptr(), cond.data_ptr(), B, N, _ptr(m), float(clamp),
+                                                  terms.data_ptr(), g_cond.data_ptr(), _ptr(g_xyz), ws.data_ptr(), ws.numel(),
+                                                  _stream_ptr(dev)), 'nphm_mlp_fit_surface_grad')
+        return terms, g_cond, g_xyz
 
     def broyden_search(self, obs: torch.Tensor, cond: torch.Tensor, x_init: torch.Tensor, J_inv_init: torch.Tensor,
                        max_steps: int = 15, cvg_thresh: float = 1e-6, dvg_thresh: float = 0.2, eps: float = 1e-6,

@@ -346,11 +346,13 @@ int mlp_prepare(nphm_mlp *h, const float *cond_dev, int n_queries, cudaStream_t 
     return launch_cvec(h->spec, cond_dev, n_queries, h->cvec.as<float>(), stream);
 }
 
-// point pass with the constants of the last mlp_prepare; impl AUTO = tensor-core kernel when the shape allows it
+// point pass with the constants of the last mlp_prepare; impl AUTO = tensor-core kernel when the shape allows it, and the
+// layer chain for stacks too wide for the FFMA kernel (the NPM expression decoder, 715 -> 1024 x 8 -> 3: the Broyden search)
 int mlp_run(nphm_mlp *h, const float *xyz_dev, int n_queries, long long n_points, float *out_dev, int impl, cudaStream_t stream)
 {
     if (n_points == 0) return NPHM_OK;
-    const bool use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && tc_mlp_supported(h));
+    const bool too_wide = !folded_net_fits(h->net) && chain_packed(h);
+    const bool use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && (tc_mlp_supported(h) || too_wide));
     if (use_tc) return chain_forward(h, xyz_dev, n_queries, n_points, out_dev, stream);
     SimtQuery q{};
     q.xyz = xyz_dev; q.total = n_points; q.n_points = n_points; q.n_queries = n_queries; q.quirk_period = 0;

@@ -81,6 +81,7 @@ int tc_ensemble_pack(nphm_ensemble *h, cudaStream_t stream);
 int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream);
 // tensor-core MLP forward (mlp_chain.cu, layer by layer): the deformation backbone is the configuration AUTO sends there
 bool tc_mlp_supported(const nphm_mlp *h);
+bool chain_packed(const nphm_mlp *h);
 int chain_forward(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, cudaStream_t stream);
 // fitting (fit.cu)
 void fit_packs_destroy(nphm_ensemble *h);

@@ -305,6 +305,8 @@ bool tc_mlp_supported(const nphm_mlp *h)
            h->chain->packed;
 }
 
+bool chain_packed(const nphm_mlp *h) { return h->chain && h->chain->packed; }
+
 // forward with the constants of the last mlp_prepare
 int chain_forward(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, cudaStream_t stream)
 {
@@ -1129,6 +1131,177 @@ extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev,
     }
     if (grad_xyz_dev) {
         // s_bar g + H v: the point gradient of zb, as in the first-order backward
+        tcl::LinearParams px;
+        px.M = M;
+        px.Ap = d; px.a_ksteps = ks;
+        px.mode = tcl::kModeLinear; px.C = xa; px.ldc = 4;
+        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
+        train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(xa, xb, M, gs, grad_xyz_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    return NPHM_OK;
+}
+
+// ================================================================================================ fitting a one-output stack
+// The surface term of both fitters with a DeepSDF decoder (reference src/NPHM/models/fitting.py:114-125 and :229-247):
+//   loss = mean over the kept points of |s|,  kept = mask != 0 and |s| < clamp
+// with its gradients w.r.t. the per-query condition (the identity code) and the points.  One value pass (the first-order
+// training forward, no noise), one kernel that forms the kept set, counts it, sums |s| in a fixed order and writes the upstream
+// sign(s) * kept as the packed output-layer adjoint, then the adjoint chain with the per-query condition sums.
+// fp16 range: the true upstream is 1 / n_kept (~2e-4 at 5 x 1000 points) and the adjoint shrinks through eight 1024-wide
+// layers; the adjoint starts at +-2^kGradExp like the unit column of the SDF-gradient forward, and the fp32 epilogues multiply
+// by 2^-kGradExp / n_kept (0 when nothing is kept, so both gradients are exactly zero then).
+// Memory: everything per point lives in the caller's workspace (the training layout, s, the adjoint ping-pong, the point-
+// gradient temporaries); the handle keeps only the per-query sums of the layer widths.
+namespace nphm {
+namespace fitsurf {
+
+constexpr int kThreads = 1024;
+
+struct Layout {
+    train::Layout base;
+    size_t sdf = 0, dl = 0, consts = 0, dp[2] = {}, xa = 0, xb = 0, total = 0;
+    int ks_dp = 1;
+};
+
+static Layout layout(const StackDims &s, int n_queries, long long n_points)
+{
+    Layout F;
+    F.base = train::layout(s, n_queries, n_points, 0);
+    const size_t M = (size_t)n_queries * n_points, tiles = (size_t)ceil_div((long long)M, 128);
+    size_t off = F.base.total;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
+    F.sdf = take(M * sizeof(float));
+    F.dl = take(tiles * 8192);
+    F.consts = take(2 * sizeof(float));
+    for (int l = 0; l + 1 < s.n_lin; ++l) F.ks_dp = std::max(F.ks_dp, (s.N[l] + 15) / 16);
+    for (int i = 0; i < 2; ++i) F.dp[i] = take(tiles * F.ks_dp * 8192);
+    F.xa = take(M * 4 * sizeof(float));
+    F.xb = take(M * 4 * sizeof(float));
+    F.total = off;
+    return F;
+}
+
+// One block.  Row r of the padded tiles: column 0 of the packed adjoint = 2^kGradExp sign(s_r) if r is kept, else 0 (sign(0) = 0,
+// as torch's abs backward).  n_kept and sum |s| are reduced in a fixed order (strided per thread, then a fixed tree), so the
+// call is bitwise deterministic.  gs = {2^kGradExp, 2^-kGradExp / n_kept}; loss_terms = [loss, 0, 0, 0, 0, n_kept].
+__global__ void __launch_bounds__(kThreads) surface_upstream_kernel(const float *__restrict__ sdf, const unsigned char *__restrict__ mask,
+                                                                     long long M, float clamp, uint8_t *__restrict__ dst,
+                                                                     float *__restrict__ gs, float *__restrict__ loss_terms)
+{
+    __shared__ float w_sum[kThreads / 32];
+    __shared__ int w_cnt[kThreads / 32];
+    const float top = ldexpf(1.0f, train::kGradExp);
+    float sum = 0.f;
+    int cnt = 0;
+    const long long rows = (M + 127) / 128 * 128;
+    for (long long r = threadIdx.x; r < rows; r += kThreads) {
+        float v = 0.f;
+        if (r < M) {
+            const float s = sdf[r], a = fabsf(s);
+            if ((!mask || mask[r]) && a < clamp) {
+                sum += a;
+                ++cnt;
+                v = s > 0.f ? top : (s < 0.f ? -top : 0.f);
+            }
+        }
+        const uint32_t w0 = (uint32_t)__half_as_ushort(__float2half_rn(v));
+        uint8_t *d = dst + (size_t)(r >> 7) * 8192 + (size_t)((r & 127) >> 3) * 256 + (r & 7) * 16;
+        *reinterpret_cast<uint4 *>(d) = make_uint4(w0, 0, 0, 0);
+        *reinterpret_cast<uint4 *>(d + 128) = make_uint4(0, 0, 0, 0);
+        *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(0, 0, 0, 0);
+        *reinterpret_cast<uint4 *>(d + 4096 + 128) = make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    }
+    if ((threadIdx.x & 31) == 0) { w_sum[threadIdx.x >> 5] = sum; w_cnt[threadIdx.x >> 5] = cnt; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.f;
+        int n = 0;
+        for (int w = 0; w < kThreads / 32; ++w) { t += w_sum[w]; n += w_cnt[w]; }
+        gs[0] = top;
+        gs[1] = n > 0 ? ldexpf(1.0f, -train::kGradExp) / (float)n : 0.f;
+        loss_terms[0] = t / (float)n;                   // NaN when nothing is kept, like torch's mean of an empty tensor
+        loss_terms[1] = loss_terms[2] = loss_terms[3] = loss_terms[4] = 0.f;
+        loss_terms[5] = (float)n;
+    }
+}
+
+}  // namespace fitsurf
+}  // namespace nphm
+
+extern "C" long long nphm_mlp_fit_workspace_bytes(const nphm_mlp *h, int n_queries, long long n_points)
+{
+    if (!h || !h->loaded || n_queries < 1 || n_points < 1) {
+        set_error("nphm_mlp_fit_workspace_bytes: bad arguments");
+        return -1;
+    }
+    return (long long)fitsurf::layout(h->dims, n_queries, n_points).total;
+}
+
+extern "C" int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
+                                         const unsigned char *mask_dev, float clamp, float *loss_terms_dev, float *grad_cond_dev,
+                                         float *grad_xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = sdfgrad::ready(h, "nphm_mlp_fit_surface_grad");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && loss_terms_dev && grad_cond_dev && workspace_dev,
+                 "nphm_mlp_fit_surface_grad: bad arguments");
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    const fitsurf::Layout F = fitsurf::layout(s, n_queries, n_points);
+    NPHM_REQUIRE(workspace_bytes == (long long)F.total,
+                 "nphm_mlp_fit_surface_grad: a workspace of %lld bytes does not fit this network at %d x %lld points (needs %lld)",
+                 workspace_bytes, n_queries, n_points, (long long)F.total);
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const long long M = (long long)n_queries * n_points;
+    const int last = s.n_lin - 1;
+    float *const sdf = reinterpret_cast<float *>(ws + F.sdf), *const gs = reinterpret_cast<float *>(ws + F.consts);
+    float *const xa = reinterpret_cast<float *>(ws + F.xa), *const xb = reinterpret_cast<float *>(ws + F.xb);
+    if ((rc = nphm_mlp_train_forward(h, xyz_dev, cond_dev, nullptr, 0, n_queries, n_points, sdf, ws, stream_))) return rc;
+    fitsurf::surface_upstream_kernel<<<1, fitsurf::kThreads, 0, stream>>>(sdf, mask_dev, M, clamp, ws + F.dl, gs, loss_terms_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    if ((rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
+        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
+        return rc;
+    const train::GradTargets targets{h, &F.base, ws, n_queries, 0, n_points, gs, nullptr, nullptr, true};
+
+    // d_{l-1} = s_{l-1} * (d_l W_l) from the packed upstream down to d_0; d_l lives in dp[l & 1]
+    const uint8_t *d = ws + F.dl;
+    int ks = 1;
+    for (int l = last; l >= 1; --l) {
+        if ((rc = train::layer_grads(targets, l, d, ks, nullptr, nullptr, stream))) return rc;     // condition sums at the skip
+        if (l == s.skip && grad_xyz_dev) {
+            tcl::LinearParams px;
+            px.M = M;
+            px.Ap = d; px.a_ksteps = ks;
+            px.mode = tcl::kModeLinear; px.C = xb; px.ldc = 4;
+            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+        }
+        tcl::LinearParams p;
+        p.M = M;
+        p.Ap = d; p.a_ksteps = ks;
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + F.base.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
+        const int ks_next = (s.N[l - 1] + 15) / 16;
+        p.Cp = ws + F.dp[(l - 1) & 1]; p.c_ksteps = ks_next;
+        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
+        d = ws + F.dp[(l - 1) & 1];
+        ks = ks_next;
+    }
+    if ((rc = train::layer_grads(targets, 0, d, ks, nullptr, nullptr, stream))) return rc;
+    NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
+    dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 1);              // one chunk: a fixed summation order
+    chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
+                                                      h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
+                                                      s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    if (grad_xyz_dev) {
         tcl::LinearParams px;
         px.M = M;
         px.Ap = d; px.a_ksteps = ks;

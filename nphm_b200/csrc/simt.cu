@@ -137,6 +137,8 @@ __global__ void __launch_bounds__(256) folded_net_kernel(const FoldedNet net, co
 
 int simt_smem_bytes(const FoldedNet &net, int tm) { return 2 * net.max_rows * 32 * tm * (int)sizeof(float); }
 
+bool folded_net_fits(const FoldedNet &net) { return simt_smem_bytes(net, 1) <= 227 * 1024; }
+
 int launch_folded_net(const FoldedNet &net, const SimtQuery &q, cudaStream_t stream)
 {
     // largest point tile whose two activation buffers fit in shared memory

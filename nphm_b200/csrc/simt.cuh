@@ -43,6 +43,8 @@ struct PackSpec {
 };
 
 int launch_folded_net(const FoldedNet &net, const SimtQuery &q, cudaStream_t stream);
+// whether launch_folded_net can hold the network's activations in shared memory (hidden widths up to ~880)
+bool folded_net_fits(const FoldedNet &net);
 int launch_cvec(const PackSpec &spec, const float *latents, int n_queries, float *cvec, cudaStream_t stream);
 int launch_anchors(const float *latents, int n_queries, int lat_dim, int lat_glob, int hid, int n_out,
                    const float *const *w, const float *const *b, const float *mean, float *anchors,

@@ -6,7 +6,9 @@
 ``inference_identity_space`` runs on the fused fitting kernels (``nphm_fit_identity_step``: forward, clamped |sdf|
 loss, analytic latent gradient and Adam in five launches, no autograd graph) when the decoder is a
 ``FastEnsembleDeepSDFMirrored`` on a CUDA device; otherwise it falls back to autograd through the composite modules,
-written here independently but following the same loop.  Host-side behaviour kept from the reference: the
+written here independently but following the same loop.  With a ``DeepSDF`` decoder (the NPM baseline of
+scripts/configs/fitting_npm.yaml) on CUDA both fitters run natively as well (:class:`NpmIdentityFitter`,
+:class:`NpmJointFitter`).  Host-side behaviour kept from the reference: the
 point sampling draws from torch's global CPU generator in the same order (``torch.randint`` at :214,:219), the
 ``lambdas`` dict is mutated by the schedule (:199-206), Adam runs with lr 0.01*lr_scale halved by the schedule, and the
 returned anchors are those of the LAST iteration's pre-update latent (:211).
@@ -148,9 +150,17 @@ def inference_identity_space(decoder,
                              schedule_cfg: Dict,
                              step_scale=1,
                              lr_scale=1):
-    """Fit the identity code to point-cloud observations.  Returns ``(lat_rep_shape (1,1,D), anchors (1,K,3))``."""
+    """Fit the identity code to point-cloud observations.  Returns ``(lat_rep_shape (1,1,D), anchors (1,K,3))``; a
+    ``DeepSDF`` decoder has no anchors (``None``), as in the reference."""
     device = all_obs[0].device
     lr = 0.01 * lr_scale
+    if device.type == 'cuda' and _native_npm_decoder(decoder, 1):
+        fitter = NpmIdentityFitter(decoder, device)
+        for j in range(int(n_steps * step_scale)):
+            lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
+            obs, _ = _sample_observations(all_obs)
+            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+        return fitter.latent.reshape(1, 1, -1).clone().requires_grad_(True), None
     if _fused_identity(decoder) and device.type == 'cuda':
         fitter = IdentityFitter(decoder, device)
         z_prev = fitter.latent.clone()
@@ -163,8 +173,13 @@ def inference_identity_space(decoder,
             _, anchors = fitter.engine.query(torch.zeros(1, 1, 3, device=device), z_prev.reshape(1, -1), eval_quirk=False)
         lat_rep_shape = fitter.latent.reshape(1, 1, -1).clone().requires_grad_(True)
         return lat_rep_shape, anchors
+    return _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
 
-    # ---- autograd path (any decoder, CPU or GPU)
+
+def _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1):
+    """The composite path of :func:`inference_identity_space`: autograd through the modules (any decoder, CPU or GPU)."""
+    device = all_obs[0].device
+    lr = 0.01 * lr_scale
     lat_dim = decoder.lat_dim
     lat_rep_shape = torch.zeros([1, 1, lat_dim], device=device, requires_grad=True)
     opt = optim.Adam(params=[lat_rep_shape], lr=lr)
@@ -317,6 +332,139 @@ class JointFitter:
             return None
 
 
+# ------------------------------------------------------------------------------------------ NPM baseline (DeepSDF decoders)
+NPM_EXPR_DIM = 200          # the reference's expression code width when decoder_expr has no lat_dim_expr (fitting.py:26-29)
+
+
+def _native_npm_decoder(decoder, out_dim: int) -> bool:
+    """A ``DeepSDF`` the native fitters take: CUDA fp32, Softplus(100), no positional encoding, ``out_dim`` outputs and a
+    stack the native builder accepts (the condition of ``DeepSDF.native_grad_supported``)."""
+    from .deepSDF import DeepSDF
+    if not isinstance(decoder, DeepSDF) or decoder.out_dim_net != out_dim:
+        return False
+    p = next(decoder.parameters())
+    n_lin = decoder.num_layers - 1
+    return (p.is_cuda and p.dtype == torch.float32 and decoder.num_freq_bands is None and decoder.beta == 100
+            and _native.stack_supported(n_lin - 1, _native.hidden_width(decoder, n_lin), decoder.lat_dim))
+
+
+def _native_npm_joint(decoder, decoder_expr, device) -> bool:
+    """The NPM baseline of fitting_npm.yaml: a one-output ``DeepSDF`` identity decoder and a 3-output ``DeepSDF`` expression
+    decoder conditioned on ``[z_id | z_ex]``, both on ``device``."""
+    if device.type != 'cuda' or not (_native_npm_decoder(decoder, 1) and _native_npm_decoder(decoder_expr, 3)):
+        return False
+    if hasattr(decoder_expr, 'lat_dim_expr') or decoder_expr.lat_dim != decoder.lat_dim + NPM_EXPR_DIM:
+        return False
+    return next(decoder.parameters()).device == device and next(decoder_expr.parameters()).device == device
+
+
+def _pow2_scale(x: torch.Tensor) -> torch.Tensor:
+    """A power of two (0-dim tensor, computed on the device) that brings the largest magnitude of ``x`` to [2^9, 2^10)."""
+    _, e = torch.frexp(x.abs().amax())
+    return torch.ldexp(torch.ones((), device=x.device), 10 - e)
+
+
+class NpmIdentityFitter:
+    """``inference_identity_space`` for a one-output ``DeepSDF`` (reference fitting.py:180-285) without an autograd graph.
+    Per iteration: the surface term with its code gradient (``nphm_mlp_fit_surface_grad``, all sampled points as one query
+    with condition ``z``), ``reg_global = ||z||^2`` (gradient ``2 z``; the reference sets reg_loc, reg_unobserved and
+    symm_dist to 0 for a DeepSDF), and Adam (``nphm_adam_step``)."""
+
+    def __init__(self, decoder, device):
+        self.device = device
+        self.engine = decoder.engine()
+        self.latent = torch.zeros(decoder.lat_dim, device=device, dtype=torch.float32)
+        self.m = torch.zeros_like(self.latent)
+        self.v = torch.zeros_like(self.latent)
+        self.loss_terms = torch.zeros(8, device=device, dtype=torch.float32)
+        self.grad = torch.zeros_like(self.latent)
+        self.t = 0
+        self._ws = None
+
+    def step(self, points: torch.Tensor, lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
+        """One iteration on ``points`` (B x N x 3); with ``apply_update=False`` only ``grad`` and ``loss_terms`` are set."""
+        pts = points.reshape(1, -1, 3).to(dtype=torch.float32).contiguous()
+        if apply_update:
+            self.t += 1
+        lam_s, lam_g = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0))
+        with torch.no_grad(), torch.cuda.device(self.device):
+            if self._ws is None or self._ws[0] != pts.shape[1]:
+                self._ws = (pts.shape[1], self.engine.fit_workspace(1, pts.shape[1], self.device))
+            terms, g_cond, _ = self.engine.fit_surface_grad(pts, self.latent[None], None, clamp, want_xyz=False,
+                                                            workspace=self._ws[1])
+            self.loss_terms.copy_(terms)
+            torch.add(lam_s * g_cond[0], self.latent, alpha=2.0 * lam_g, out=self.grad)
+            if apply_update:
+                _native.check(_native.lib().nphm_adam_step(self.latent.data_ptr(), self.grad.data_ptr(), self.m.data_ptr(),
+                                                           self.v.data_ptr(), self.latent.numel(), float(lr), self.t,
+                                                           torch.cuda.current_stream(self.device).cuda_stream), 'nphm_adam_step')
+
+
+class NpmJointFitter:
+    """One iteration of ``inference_iterative_root_finding_joint`` (reference fitting.py:38-175) for the NPM baseline
+    (``DeepSDF`` identity and expression decoders) without an autograd graph.  The chain of :class:`JointFitter` without the
+    compressor, anchors or mlp_pos:
+        cond_b = [z_id | z_ex[idx_b]]
+        J0^-1 at the observations, Broyden on the device (sync-free), J^-1 at the roots     nphm_mlp_inverse_jacobian / _broyden_search
+        d surface / d z_id, g_x = d surface / d xc  (mask = valid)                          nphm_mlp_fit_surface_grad
+        u = -J^-T g_x,  g_cond = sum_n (dF/d cond)^T u_n                                      nphm_mlp_backward_inputs (value pass reused)
+        z_id += g_cond[:, :D] summed over the scans,  z_ex[idx_b] += g_cond[b, D:] + reg_expr,  two Adam steps.
+    u is of order 1e-4 and the adjoint pass works on fp16 hi | lo operands, so u is scaled by a power of two (largest magnitude
+    to 2^10, chosen on the device) before the call and g_cond is divided by it afterwards; the adjoint is linear in u."""
+
+    def __init__(self, decoder, decoder_expr, num_observations: int, device):
+        self.device = device
+        self.eng = decoder.engine()
+        self.mlp = decoder_expr.engine()
+        D = decoder.lat_dim
+        self.z_id = torch.zeros(D, device=device)
+        self.m_id, self.v_id = torch.zeros_like(self.z_id), torch.zeros_like(self.z_id)
+        self.z_ex = torch.zeros(num_observations, decoder_expr.lat_dim - D, device=device)
+        self.m_ex, self.v_ex = torch.zeros_like(self.z_ex), torch.zeros_like(self.z_ex)
+        self.loss_terms = torch.zeros(8, device=device)
+        self.t = 0
+        self.anchors = None                     # a DeepSDF has no anchors
+        self.early_exit = bool(int(os.environ.get('NPHM_BROYDEN_EARLY_EXIT', '0')))
+        self._ws = None
+
+    def step(self, obs, obs_idx, lambdas, clamp, lr, apply_update: bool = True):
+        """One iteration; with ``apply_update=False`` nothing is modified and ``(d loss / d z_id, d loss / d z_ex)`` - the
+        tensors the reference hands to its two ``Adam.step()`` calls - are returned."""
+        nat, dev = _native, self.device
+        nb, n_point, _ = obs.shape
+        D = self.z_id.shape[0]
+        if apply_update:
+            self.t += 1
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
+        lam_g = float(lambdas.get('reg_global', 0.0))
+        with torch.no_grad(), torch.cuda.device(dev):
+            cond = torch.cat([self.z_id[None].expand(nb, D), self.z_ex[obs_idx]], dim=1).contiguous()
+            obs = obs.to(torch.float32).contiguous()
+            _, j0_inv = self.mlp.inverse_jacobian(obs, cond)
+            p, _, valid, _ = self.mlp.broyden_search(obs, cond, obs, j0_inv, max_steps=15, cvg_thresh=1e-6, dvg_thresh=0.2,
+                                                     early_exit=self.early_exit)
+            _, j_inv = self.mlp.inverse_jacobian(p, cond)
+            if self._ws is None or self._ws[0] != nb * n_point:
+                self._ws = (nb * n_point, self.eng.fit_workspace(1, nb * n_point, dev))
+            terms, g_lat, g_pts = self.eng.fit_surface_grad(p.reshape(1, -1, 3), self.z_id[None], valid, clamp,
+                                                            workspace=self._ws[1])
+            self.loss_terms.copy_(terms)
+            u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                     # -J^-T g_x
+            sc = _pow2_scale(u)
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u * sc, reuse_value_pass=True)
+            g_cond = g_cond / sc
+            g_zid = lam_s * (g_lat[0] + g_cond[:, :D].sum(0)) + (2.0 * lam_g) * self.z_id
+            g_zex = torch.zeros_like(self.z_ex)
+            g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
+            if not apply_update:
+                return g_zid, g_zex
+            for z, g, m, v in ((self.z_id, g_zid, self.m_id, self.v_id), (self.z_ex, g_zex, self.m_ex, self.v_ex)):
+                nat.check(nat.lib().nphm_adam_step(z.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), z.numel(), float(lr),
+                                                   self.t, stream), 'nphm_adam_step')
+            return None
+
+
 def inference_iterative_root_finding_joint(decoder,
                                            decoder_expr,
                                            all_obs: List[torch.Tensor],
@@ -328,21 +476,35 @@ def inference_iterative_root_finding_joint(decoder,
     """Joint identity + expression fitting with Broyden correspondences (reference :14-177).
 
     Shipped configuration (fused ensemble + 'compress' DeformationNetwork on CUDA): no autograd graph at all, see
-    :class:`JointFitter`.  Anything else: the correspondence search runs on the device (`nphm_mlp_broyden_search`), the
+    :class:`JointFitter`; the same for the NPM baseline (``DeepSDF`` decoders on CUDA), see :class:`NpmJointFitter`.
+    ``NPHM_JOINT_AUTOGRAD=1`` keeps both on the composite path.  Anything else: the correspondence search runs on the device (`nphm_mlp_broyden_search`), the
     surface term comes from `nphm_fit_surface_grad`, the deformation network's part of the chain stays on autograd.  Returns
     ``(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)``."""
     device = all_obs[0].device
     num_observations = len(all_obs)
-    if _native_joint(decoder, decoder_expr, device) and not os.environ.get('NPHM_JOINT_AUTOGRAD'):
-        fitter = JointFitter(decoder, decoder_expr, num_observations, device)
-        lr = 0.01 * lr_scale
-        for j in range(int(n_steps * step_scale)):
-            lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
-            obs, obs_idx = _sample_observations(all_obs)
-            fitter.step(obs, obs_idx.long().to(device), lambdas, _clamp_for_iteration(j, step_scale), lr)
-        lat_rep = fitter.z_ex.reshape(num_observations, 1, -1).clone().requires_grad_(True)
-        lat_rep_shape = fitter.z_id.reshape(1, 1, -1).clone().requires_grad_(True)
-        return lat_rep, lat_rep_shape, fitter.anchors
+    if not os.environ.get('NPHM_JOINT_AUTOGRAD'):
+        fitter = None
+        if _native_joint(decoder, decoder_expr, device):
+            fitter = JointFitter(decoder, decoder_expr, num_observations, device)
+        elif _native_npm_joint(decoder, decoder_expr, device):
+            fitter = NpmJointFitter(decoder, decoder_expr, num_observations, device)
+        if fitter is not None:
+            lr = 0.01 * lr_scale
+            for j in range(int(n_steps * step_scale)):
+                lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
+                obs, obs_idx = _sample_observations(all_obs)
+                fitter.step(obs, obs_idx.long().to(device), lambdas, _clamp_for_iteration(j, step_scale), lr)
+            lat_rep = fitter.z_ex.reshape(num_observations, 1, -1).clone().requires_grad_(True)
+            lat_rep_shape = fitter.z_id.reshape(1, 1, -1).clone().requires_grad_(True)
+            return lat_rep, lat_rep_shape, fitter.anchors
+    return _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
+
+
+def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1):
+    """The composite path of :func:`inference_iterative_root_finding_joint`: the correspondence search on the device where
+    the search supports the decoder, everything else on autograd through the modules."""
+    device = all_obs[0].device
+    num_observations = len(all_obs)
     lat_expr_dim = decoder_expr.lat_dim_expr if hasattr(decoder_expr, 'lat_dim_expr') else 200
     lat_rep = torch.zeros([num_observations, 1, lat_expr_dim], device=device, requires_grad=True)
     lat_rep_shape = torch.zeros([1, 1, decoder.lat_dim], device=device, requires_grad=True)

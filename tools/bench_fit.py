@@ -6,7 +6,13 @@
 
 Every rank fits its own synthetic scan (3 observations x 2500 points, seed 100 + rank) with the reference's loop
 (`inference_identity_space`, 5 x 1000 sampled points per iteration, reference schedule) on the fused fitting kernels.
-Prints one JSON line on rank 0: iterations/s and scans/hour over all ranks (time = max over ranks)."""
+Prints one JSON line on rank 0: iterations/s and scans/hour over all ranks (time = max over ranks).
+
+    python tools/bench_fit.py --decoder npm --steps 10 [--iters 20]
+
+The NPM baseline of fitting_npm.yaml (DeepSDF 515 -> 1024 x 8 -> 1, seeded as in tests/npm_fit_common.py) on one GPU: native
+(NpmIdentityFitter) and composite (autograd) runs of `--iters` iterations alternate `--steps` times; median ms per iteration
+of each, with the card and its power limit."""
 import argparse, json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
@@ -21,7 +27,11 @@ def main():
     ap.add_argument('--sharded', action='store_true',
                     help='ONE head, the sampled points of every iteration sharded over the ranks, one all-reduce per iteration '
                          '(nphm_b200.distributed.inference_identity_space_sharded) instead of one scan per GPU')
+    ap.add_argument('--decoder', choices=('nphm', 'npm'), default='nphm')
+    ap.add_argument('--iters', type=int, default=20, help='--decoder npm: iterations per timed run')
     args = ap.parse_args()
+    if args.decoder == 'npm':
+        return bench_npm(args)
     from conftest import make_ensemble
     from nphm_b200.models.fitting import inference_identity_space
     world = int(os.environ.get('WORLD_SIZE', '1')); rank = int(os.environ.get('RANK', '0'))
@@ -68,6 +78,33 @@ def main():
                           else 'replicas (one scan per GPU, no collective)'}))
     if dist.is_initialized():
         dist.destroy_process_group()
+
+
+def bench_npm(args):
+    from bench_joint import alternate
+    from bench_train import gpu_info
+    from npm_fit_common import LAMBDAS_IDENTITY, SCHEDULE, make_decoders
+    from nphm_b200.models import fitting as F
+    from nphm_b200.models.deepSDF import DeepSDF
+    dev = torch.device('cuda', torch.cuda.current_device())
+    dec, _ = make_decoders(DeepSDF, dev)
+    assert F._native_npm_decoder(dec, 1)
+    rng = np.random.RandomState(100)
+    obs = [torch.from_numpy((rng.randn(2500, 3) * 0.1 + np.array([0.0, 0.05, -0.1])).astype(np.float32)).to(dev) for _ in range(3)]
+
+    def run(fn):
+        def go(n):
+            np.random.seed(0); torch.manual_seed(0)
+            return fn(dec, obs, dict(LAMBDAS_IDENTITY), n, SCHEDULE)
+        return go
+
+    name, power = gpu_info()
+    ms = alternate({'native': run(F.inference_identity_space), 'composite': run(F._inference_identity_space_autograd)},
+                   args.steps, args.iters)
+    print(json.dumps({'metric': 'identity_fit_npm', 'gpu': name, 'power_limit': power, 'points': '5 x 1000 per iteration',
+                      'runs': args.steps, 'iterations_per_run': args.iters, 'native_ms_per_iter': ms['native'],
+                      'composite_ms_per_iter': ms['composite'], 'speedup': ms['composite'] / ms['native'],
+                      'timing': 'median over runs of CUDA-event time per iteration, native and composite alternated'}))
 
 
 if __name__ == '__main__':
