@@ -195,6 +195,13 @@ def _ptr_array(tensors):
     return arr
 
 
+def _workspace(nbytes: int, what: str, device) -> torch.Tensor:
+    """A uint8 workspace of the size a ``*_workspace_bytes`` entry point returned (-1: raise its error)."""
+    if nbytes < 0:
+        check(-1, what)
+    return torch.empty(nbytes, device=device, dtype=torch.uint8)
+
+
 def constant_latent_rows(lat_rep: torch.Tensor) -> Optional[torch.Tensor]:
     """``B x N x D`` (or ``B x 1 x D``) latent -> ``B x D`` if it is the same for all points of a batch
     entry, else ``None``.  Broadcast views (stride 0) are recognised without reading the data; a
@@ -471,6 +478,15 @@ class MlpEngine(_Versioned):
         return g_cond, g_xyz
 
     # ------------------------------------------------------------ training (first order)
+    def _grad_buffers(self, B, N, dev, weights, biases, want_cond, want_xyz):
+        """Outputs of a training backward: (weight grads | None, bias grads | None, d/d cond | None, d/d xyz | None)."""
+        shapes = self.layer_shapes
+        gw = [torch.empty(s, device=dev, dtype=torch.float32) for s in shapes] if weights else None
+        gb = [torch.empty(s[0], device=dev, dtype=torch.float32) for s in shapes] if biases else None
+        g_cond = torch.empty(B, self.lat_dim, device=dev, dtype=torch.float32) if want_cond else None
+        g_xyz = torch.empty(B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None
+        return gw, gb, g_cond, g_xyz
+
     def train_forward(self, xyz: torch.Tensor, cond: torch.Tensor, noise: Optional[torch.Tensor] = None):
         """Value pass that keeps what the backward needs (nphm_mlp_train_forward): xyz B x N x 3, cond B x lat_dim, noise
         B x N x noise_dim (added to the leading condition columns of every point) or None.  Returns ``(out B x N x out_dim,
@@ -484,10 +500,7 @@ class MlpEngine(_Versioned):
         noise = None if noise is None else _f32c(noise).reshape(B, N, nd)
         out = torch.empty(B, N, self.out_dim, device=dev, dtype=torch.float32)
         with torch.cuda.device(dev):
-            nbytes = int(lib().nphm_mlp_train_workspace_bytes(self._h, B, N, nd))
-            if nbytes < 0:
-                check(-1, 'nphm_mlp_train_workspace_bytes')
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            ws = _workspace(lib().nphm_mlp_train_workspace_bytes(self._h, B, N, nd), 'nphm_mlp_train_workspace_bytes', dev)
             check(lib().nphm_mlp_train_forward(self._h, xyz.data_ptr(), cond.data_ptr(), _ptr(noise), nd, B, N, out.data_ptr(),
                                                ws.data_ptr(), _stream_ptr(dev)), 'nphm_mlp_train_forward')
         return out, ws
@@ -500,11 +513,7 @@ class MlpEngine(_Versioned):
         B, N, _ = grad_out.shape
         dev = grad_out.device
         g = _f32c(grad_out)
-        shapes = self.layer_shapes
-        gw = [torch.empty(s, device=dev, dtype=torch.float32) for s in shapes] if weights else None
-        gb = [torch.empty(s[0], device=dev, dtype=torch.float32) for s in shapes] if biases else None
-        g_cond = torch.empty(B, self.lat_dim, device=dev, dtype=torch.float32) if want_cond else None
-        g_xyz = torch.empty(B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None
+        gw, gb, g_cond, g_xyz = self._grad_buffers(B, N, dev, weights, biases, want_cond, want_xyz)
         with torch.cuda.device(dev):
             check(lib().nphm_mlp_train_backward(self._h, g.data_ptr(), ws.data_ptr(), ws.numel(), int(noise_dim), B, N,
                                                 _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
@@ -522,10 +531,7 @@ class MlpEngine(_Versioned):
         sdf = torch.empty(B, N, 1, device=dev, dtype=torch.float32)
         grad = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
         with torch.cuda.device(dev):
-            nbytes = int(lib().nphm_mlp_sdfgrad_workspace_bytes(self._h, B, N))
-            if nbytes < 0:
-                check(-1, 'nphm_mlp_sdfgrad_workspace_bytes')
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            ws = _workspace(lib().nphm_mlp_sdfgrad_workspace_bytes(self._h, B, N), 'nphm_mlp_sdfgrad_workspace_bytes', dev)
             check(lib().nphm_mlp_sdfgrad_forward(self._h, xyz.data_ptr(), cond.data_ptr(), B, N, sdf.data_ptr(), grad.data_ptr(),
                                                  ws.data_ptr(), _stream_ptr(dev)), 'nphm_mlp_sdfgrad_forward')
         return sdf, grad, ws
@@ -538,11 +544,7 @@ class MlpEngine(_Versioned):
         B, N, _ = grad_grad.shape
         dev = grad_grad.device
         gs, gg = _f32c(grad_sdf), _f32c(grad_grad)
-        shapes = self.layer_shapes
-        gw = [torch.empty(s, device=dev, dtype=torch.float32) for s in shapes] if weights else None
-        gb = [torch.empty(s[0], device=dev, dtype=torch.float32) for s in shapes] if biases else None
-        g_cond = torch.empty(B, self.lat_dim, device=dev, dtype=torch.float32) if want_cond else None
-        g_xyz = torch.empty(B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None
+        gw, gb, g_cond, g_xyz = self._grad_buffers(B, N, dev, weights, biases, want_cond, want_xyz)
         with torch.cuda.device(dev):
             check(lib().nphm_mlp_sdfgrad_backward(self._h, gs.data_ptr(), gg.data_ptr(), ws.data_ptr(), ws.numel(), B, N,
                                                   _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
@@ -552,10 +554,8 @@ class MlpEngine(_Versioned):
     # ------------------------------------------------------------ fitting (surface term of a one-output stack)
     def fit_workspace(self, n_queries: int, n_points: int, device) -> torch.Tensor:
         """A workspace for :meth:`fit_surface_grad` at ``n_queries x n_points`` (a uint8 CUDA tensor the caller may keep)."""
-        nbytes = int(lib().nphm_mlp_fit_workspace_bytes(self._h, int(n_queries), int(n_points)))
-        if nbytes < 0:
-            check(-1, 'nphm_mlp_fit_workspace_bytes')
-        return torch.empty(nbytes, device=device, dtype=torch.uint8)
+        return _workspace(lib().nphm_mlp_fit_workspace_bytes(self._h, int(n_queries), int(n_points)), 'nphm_mlp_fit_workspace_bytes',
+                          device)
 
     def fit_surface_grad(self, xyz: torch.Tensor, cond: torch.Tensor, mask: Optional[torch.Tensor], clamp: float,
                          want_xyz: bool = True, workspace: Optional[torch.Tensor] = None, out=None):

@@ -19,22 +19,11 @@ namespace nphm {
 namespace chain {
 
 constexpr float kInvSqrt2 = 0.70710678118654752440f;
+constexpr float kBeta = 100.0f;                       // Softplus(beta = 100): softplus'' = kBeta S (1 - S)
 
-__global__ void column_sums_kernel(const float *__restrict__ X, int ld, long long rows_per_query, int n_cols, float *__restrict__ out)
-{
-    // out[q][c] = sum over the rows of query q of X[row][c]; grid = (col blocks, queries, row chunks), atomics across chunks
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    const int q = blockIdx.y;
-    if (c >= n_cols) return;
-    const long long chunk = (rows_per_query + gridDim.z - 1) / gridDim.z;
-    const long long r0 = (long long)blockIdx.z * chunk, r1 = min(rows_per_query, r0 + chunk);
-    float s = 0.f;
-    for (long long r = r0; r < r1; ++r) s += X[((size_t)q * rows_per_query + r) * ld + c];
-    if (r1 > r0) atomicAdd(out + (size_t)q * n_cols + c, s);
-}
-
-// The same sums over a PACKED activation buffer (tc_linear.cuh: per 128-row tile and k-step [128 x 16 fp16 hi | 128 x 16 fp16 lo],
-// core-matrix order; value = hi + lo).  grid (tiles, k-steps), 256 threads: thread = (row of the tile, 8 of the 16 columns).
+// out[q][c] += sum over the rows of query q of X[row][c], X a PACKED activation buffer (tc_linear.cuh: per 128-row tile and
+// k-step [128 x 16 fp16 hi | 128 x 16 fp16 lo], core-matrix order; value = hi + lo), with float atomics.  grid (tiles, k-steps),
+// 256 threads: thread = (row of the tile, 8 of the 16 columns).
 __global__ void __launch_bounds__(256) column_sums_packed_kernel(const uint8_t *__restrict__ X, int ksteps, long long M,
                                                                  long long rows_per_query, int n_cols, float *__restrict__ out)
 {
@@ -127,10 +116,15 @@ __global__ void inverse_plus_identity_kernel(float *__restrict__ J, long long n)
     m[6] = C * inv; m[7] = -(a * h - b * g) * inv; m[8] = (a * e - b * d) * inv;
 }
 
-__global__ void add3_kernel(const float *__restrict__ src, int ld, long long rows, float *__restrict__ dst)
+// grad_xyz[r][i] = (a[r][i] + b[r][i]) * scale[1]   (a, b: ld 4; scale == nullptr: 1)
+__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, const float *__restrict__ scale,
+                                float *__restrict__ out)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx < rows * 3) dst[idx] += src[(idx / 3) * ld + idx % 3];
+    if (idx >= M * 3) return;
+    const long long r = idx / 3;
+    const int i = (int)(idx % 3);
+    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * (scale ? scale[1] : 1.0f);
 }
 
 }  // namespace chain
@@ -144,17 +138,19 @@ struct MlpChain {
     tcl::PackedLinear adj_x0, adj_xs;         // W_0[:, 0:3]^T and W_skip[:, Nh:Nh+3]^T / sqrt2  (gradient w.r.t. xyz)
     // activations between the layers live in the packed operand format (Hp: values, Tp: tangents, Dp: adjoints), the
     // activation derivatives S in the blocked fp32 layout ([128-row tile][feature][128]) - every access of the passes is coalesced
-    DeviceBuffer Hp[kMaxLayers], S[kMaxLayers], Tp[2], Dp[2], Tlast, sums0, sumss, out_tmp, xtmp;
+    DeviceBuffer Hp[kMaxLayers], S[kMaxLayers], Tp[2], Dp[2], Tlast, out_tmp;
     DeviceBuffer Fp[2];                       // ping-pong activations of the forward-only pass (forward_pass)
     int ld[kMaxLayers];
     long long value_rows = 0;                 // rows of the last value pass that kept the activation derivatives
     bool have_deriv = false;
-    // training (nphm_mlp_train_forward / _backward): layers 0, skip - 1 and skip take `train_nd` per-row condition columns
-    // more (layer 0: [xyz | noise], the skip layer: [h | xyz | noise] / sqrt2, the layer before it appends them); packed on
-    // first use after every weight load.  Scratch of the backward: adjoints, GEMM partials, per-query column sums.
+    // training (nphm_mlp_train_forward / _backward) with condition noise: layers 0, skip - 1 and skip take `train_nd` > 0
+    // per-row condition columns more (layer 0: [xyz | noise], the skip layer: [h | xyz | noise] / sqrt2, the layer before it
+    // appends them); packed on first use after every weight load.
     tcl::PackedLinear tfwd[kMaxLayers];
     int train_nd = -1;
-    DeviceBuffer Dl, wg_partials, gscale, qsums, qsums0, qsumss, xs_tmp;
+    // scratch of the backwards: the packed top adjoint, GEMM partials, per-query column sums (of d_0, d_skip and the other
+    // layers), the two [M][4] point-gradient parts (d_0 and d_skip times their layer's xyz columns)
+    DeviceBuffer Dl, wg_partials, gscale, qsums, qsums0, qsumss, xtmp, xs_tmp;
 };
 
 static int pad4(int n) { return (n + 3) / 4 * 4; }
@@ -199,6 +195,53 @@ void chain_destroy(nphm_mlp *h)
 
 static size_t packed_bytes(long long rows, int ksteps) { return (size_t)ceil_div(rows, 128) * ksteps * 8192; }
 
+// 256-byte aligned pieces of a workspace, from `off` on
+struct Carver {
+    size_t off = 0;
+    size_t take(size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; }
+};
+
+// the layers that take the per-row condition noise as extra input columns (training, MlpChain::tfwd)
+static bool noise_layer(const StackDims &s, int l) { return l == 0 || l + 1 == s.skip || l == s.skip; }
+
+// packed forward weights of layer l with nd noise columns
+static const tcl::PackedLinear &fwd_layer(const MlpChain &c, const StackDims &s, int l, int nd)
+{
+    return nd > 0 && noise_layer(s, l) ? c.tfwd[l] : c.fwd[l];
+}
+
+// value pass over M rows, softplus layers 0 .. n_lin - 2 and the linear output layer.  X: rows [xyz | nd noise columns]
+// (ld ldx), the input of layer 0 and the columns appended behind layer skip - 1.  Layer l < n_lin - 1 writes h_l packed to
+// Hp[l] and, if S is given, s_l blocked to S[l]; the output layer writes `out` row-major.  bias: the per-query constants of
+// the first query, rows_per_bias rows per query.  live: see forward_pass.
+static int value_layers(nphm_mlp *h, long long M, const float *X, int ldx, int nd, const float *bias, long long rows_per_bias,
+                        uint8_t *const *Hp, float *const *S, float *out, const int *live, cudaStream_t stream)
+{
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    for (int l = 0; l < s.n_lin; ++l) {
+        const tcl::PackedLinear &W = fwd_layer(c, s, l, nd);
+        tcl::LinearParams p;
+        p.M = M;
+        p.live = live;
+        if (l == 0) { p.A1 = X; p.lda1 = ldx; p.K1 = 3 + nd; }
+        else { p.Ap = Hp[l - 1]; p.a_ksteps = W.ksteps; }        // at the skip layer: [h | xyz | noise], appended below
+        p.bias = bias + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = rows_per_bias;
+        if (l == s.n_lin - 1) {
+            p.mode = tcl::kModeLinear;
+            p.C = out; p.ldc = s.N[l];
+        } else {
+            p.mode = tcl::kModeSoftplus;
+            p.Cp = Hp[l]; p.c_ksteps = W.packed_ksteps_out();
+            if (l + 1 == s.skip) { p.app = X; p.app_ld = ldx; p.app_w = 3 + nd; }
+            if (S) { p.Dv = S[l]; p.lddv = c.ld[l]; p.dv_blocked = 1; }
+        }
+        int rc = tcl::launch_linear(W, p, stream);
+        if (rc) return rc;
+    }
+    return NPHM_OK;
+}
+
 // value pass over M = n_queries * n_points rows; keeps h_l (packed) and (want_deriv) s_l (blocked) of every hidden layer;
 // `out` = last layer, row-major
 static int value_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, bool want_deriv, float *out,
@@ -207,30 +250,17 @@ static int value_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_
     MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
     const long long M = (long long)n_queries * n_points;
+    uint8_t *Hp[kMaxLayers];
+    float *S[kMaxLayers];
     int rc;
-    for (int l = 0; l < s.n_lin; ++l) {
-        const bool last = l == s.n_lin - 1;
-        tcl::LinearParams p;
-        p.M = M;
-        if (l == 0) { p.A1 = xyz; p.lda1 = 3; p.K1 = 3; }
-        else { p.Ap = c.Hp[l - 1].as<uint8_t>(); p.a_ksteps = c.fwd[l].ksteps; }     // at the skip layer: [h | xyz], appended below
-        p.bias = h->cvec.as<float>() + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = n_points;
-        if (last) {
-            p.mode = tcl::kModeLinear;
-            p.C = out; p.ldc = s.N[l];
-        } else {
-            const int ks = c.fwd[l].packed_ksteps_out();
-            if ((rc = c.Hp[l].reserve(packed_bytes(M, ks)))) return rc;
-            p.mode = tcl::kModeSoftplus;
-            p.Cp = c.Hp[l].as<uint8_t>(); p.c_ksteps = ks;
-            if (l + 1 == s.skip) { p.app = xyz; p.app_ld = 3; p.app_w = 3; }
-            if (want_deriv) {
-                if ((rc = c.S[l].reserve((size_t)ceil_div(M, 128) * 128 * c.ld[l] * sizeof(float)))) return rc;
-                p.Dv = c.S[l].as<float>(); p.lddv = c.ld[l]; p.dv_blocked = 1;
-            }
-        }
-        if ((rc = tcl::launch_linear(c.fwd[l], p, stream))) return rc;
+    for (int l = 0; l + 1 < s.n_lin; ++l) {
+        if ((rc = c.Hp[l].reserve(packed_bytes(M, c.fwd[l].packed_ksteps_out())))) return rc;
+        if (want_deriv && (rc = c.S[l].reserve((size_t)ceil_div(M, 128) * 128 * c.ld[l] * sizeof(float)))) return rc;
+        Hp[l] = c.Hp[l].as<uint8_t>();
+        S[l] = c.S[l].as<float>();
     }
+    if ((rc = value_layers(h, M, xyz, 3, 0, h->cvec.as<float>(), n_points, Hp, want_deriv ? S : nullptr, out, nullptr, stream)))
+        return rc;
     c.value_rows = M;
     c.have_deriv = want_deriv;
     return NPHM_OK;
@@ -254,33 +284,100 @@ static int forward_pass(nphm_mlp *h, const float *xyz, int n_queries, long long 
     const long long max_rows = std::min((long long)n_queries, qpc) * ppc;
     for (int b = 0; b < 2; ++b)
         if ((rc = c.Fp[b].reserve(packed_bytes(max_rows, ks_max)))) return rc;
+    uint8_t *Hp[kMaxLayers];
+    for (int l = 0; l + 1 < s.n_lin; ++l) Hp[l] = c.Fp[l & 1].as<uint8_t>();
     const int out_dim = s.N[s.n_lin - 1];
     for (long long q0 = 0; q0 < n_queries; q0 += qpc) {
         const long long nq = std::min(qpc, (long long)n_queries - q0);
         for (long long p0 = 0; p0 < n_points; p0 += ppc) {
             const long long np = std::min(ppc, n_points - p0);       // nq > 1 only with whole queries (np == n_points)
             const size_t row0 = (size_t)q0 * n_points + p0;
-            const float *x = xyz + row0 * 3;
-            for (int l = 0; l < s.n_lin; ++l) {
-                tcl::LinearParams p;
-                p.M = nq * np;
-                p.live = live;
-                if (l == 0) { p.A1 = x; p.lda1 = 3; p.K1 = 3; }
-                else { p.Ap = c.Fp[(l - 1) & 1].as<uint8_t>(); p.a_ksteps = c.fwd[l].ksteps; }
-                p.bias = h->cvec.as<float>() + (size_t)q0 * s.cvec_stride + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = np;
-                if (l == s.n_lin - 1) {
-                    p.mode = tcl::kModeLinear;
-                    p.C = out + row0 * out_dim; p.ldc = out_dim;
-                } else {
-                    p.mode = tcl::kModeSoftplus;
-                    p.Cp = c.Fp[l & 1].as<uint8_t>(); p.c_ksteps = c.fwd[l].packed_ksteps_out();
-                    if (l + 1 == s.skip) { p.app = x; p.app_ld = 3; p.app_w = 3; }
-                }
-                if ((rc = tcl::launch_linear(c.fwd[l], p, stream))) return rc;
-            }
+            if ((rc = value_layers(h, nq * np, xyz + row0 * 3, 3, 0, h->cvec.as<float>() + (size_t)q0 * s.cvec_stride, np, Hp,
+                                   nullptr, out + row0 * out_dim, live, stream)))
+                return rc;
         }
     }
     c.have_deriv = false;
+    return NPHM_OK;
+}
+
+// the adjoint of a layer's pre-activations: row-major fp32 rows (the caller's output gradient) or packed (ks k-steps)
+struct Adjoint {
+    const float *rows = nullptr; int ld = 0;
+    const uint8_t *packed = nullptr; int ks = 0;
+};
+
+// what one adjoint walk reads and writes; per-layer entries for l < L = n_lin - 1
+struct AdjointWalk {
+    Adjoint top;                                   // d_L
+    const float *S[kMaxLayers] = {};               // s_l, blocked fp32
+    uint8_t *D[kMaxLayers] = {};                   // where d_l goes, packed
+    const float *cpl_z[kMaxLayers] = {};           // optional coupling of the SDF-gradient backward:
+    const uint8_t *cpl_a[kMaxLayers] = {};         //   d_l += kBeta (1 - s_l) * cpl_z[l] * cpl_a[l]
+    float *xs = nullptr;                           // optional [M][4]: d_skip W_skip[:, Nh:Nh+3]^T / sqrt2
+};
+
+// d_{l-1} = s_{l-1} * (d_l W_l) from d_L down to d_0 (left in w.D[0]).  hook(l, d_l, ks) runs for l = L .. 1 before the
+// descent below layer l (d_L given as rows: d_l == nullptr) and for l = 0 at the bottom.
+template <class Hook>
+static int adjoint_walk(nphm_mlp *h, long long M, const AdjointWalk &w, Hook &&hook, cudaStream_t stream)
+{
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    Adjoint d = w.top;
+    int rc;
+    for (int l = s.n_lin - 1; l >= 1; --l) {
+        if ((rc = hook(l, d.packed, d.ks))) return rc;
+        if (l == s.skip && w.xs) {                 // d_skip is packed: chain_ready keeps the skip layer below the output layer
+            tcl::LinearParams px;
+            px.M = M;
+            px.Ap = d.packed; px.a_ksteps = d.ks;
+            px.mode = tcl::kModeLinear; px.C = w.xs; px.ldc = 4;
+            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+        }
+        const int ks = (s.N[l - 1] + 15) / 16;
+        tcl::LinearParams p;
+        p.M = M;
+        if (d.packed) { p.Ap = d.packed; p.a_ksteps = d.ks; }
+        else { p.A1 = d.rows; p.lda1 = d.ld; p.K1 = s.N[l]; }
+        p.mode = tcl::kModeMult;
+        p.Mul = w.S[l - 1]; p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
+        if (w.cpl_a[l - 1]) { p.cpl_z = w.cpl_z[l - 1]; p.cpl_a = w.cpl_a[l - 1]; p.cpl_a_steps = ks; p.cpl_coef = chain::kBeta; }
+        p.Cp = w.D[l - 1]; p.c_ksteps = ks;
+        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
+        d = Adjoint{nullptr, 0, w.D[l - 1], ks};
+    }
+    return hook(0, d.packed, d.ks);
+}
+
+// grad_cond [q][cond_dim] from the per-query column sums of d_0 (qsums0) and d_skip (qsumss).  chunks: CTAs per output over
+// the n range, added with float atomics; 1 keeps a fixed summation order.
+static int cond_grad(nphm_mlp *h, int n_queries, int chunks, float *grad_cond, cudaStream_t stream)
+{
+    MlpChain &c = *h->chain;
+    const StackDims &s = h->dims;
+    NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
+    dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, (unsigned)chunks);
+    chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
+                                                      h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
+                                                      s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+// grad_xyz = (d_0 W_0[:, 0:3]^T + xs) * scale[1] (scale == nullptr: 1): d_0 packed (w.D[0] of the walk), x0 an [M][4]
+// temporary, xs the walk's skip-layer part
+static int xyz_grad(nphm_mlp *h, long long M, const uint8_t *d0, float *x0, const float *xs, const float *scale, float *grad_xyz,
+                    cudaStream_t stream)
+{
+    tcl::LinearParams p;
+    p.M = M;
+    p.Ap = d0; p.a_ksteps = (h->dims.N[0] + 15) / 16;
+    p.mode = tcl::kModeLinear; p.C = x0; p.ldc = 4;
+    int rc = tcl::launch_linear(h->chain->adj_x0, p, stream);
+    if (rc) return rc;
+    chain::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(x0, xs, M, scale, grad_xyz);
+    NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
 
@@ -407,67 +504,29 @@ extern "C" int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const
     for (int l = 1; l <= L; ++l) max_ks = std::max(max_ks, (s.N[l - 1] + 15) / 16);
     for (int i = 0; i < 2; ++i)
         if ((rc = c.Dp[i].reserve(packed_bytes(M, max_ks)))) return rc;
-    if ((rc = c.sums0.reserve((size_t)n_queries * s.N[0] * sizeof(float)))) return rc;
-    if ((rc = c.sumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float)))) return rc;
-    NPHM_CUDA_CHECK(cudaMemsetAsync(c.sums0.ptr, 0, (size_t)n_queries * s.N[0] * sizeof(float), stream));
-    NPHM_CUDA_CHECK(cudaMemsetAsync(c.sumss.ptr, 0, (size_t)n_queries * s.N[s.skip] * sizeof(float), stream));
-    // the adjoint of a layer's pre-activations: row-major fp32 for the output layer (the caller's grad_out), packed below it
-    struct Adjoint { const float *rows; int ld; const uint8_t *packed; int ksteps; int width; };
-    auto as_input = [&](tcl::LinearParams &p, const Adjoint &d) {
-        if (d.packed) { p.Ap = d.packed; p.a_ksteps = d.ksteps; }
-        else { p.A1 = d.rows; p.lda1 = d.ld; p.K1 = d.width; }
-    };
-    auto col_sums = [&](const Adjoint &d, float *out) {
-        dim3 grid((unsigned)ceil_div(M, 128), (unsigned)d.ksteps);
-        chain::column_sums_packed_kernel<<<grid, 256, 0, stream>>>(d.packed, d.ksteps, M, n_points, d.width, out);
-    };
-    // d_{l-1} = s_{l-1} * (d_l W_l), from the output layer down to d_0;  d_l lives in Dp[l & 1]
-    Adjoint d_cur{grad_out_dev, out_dim, nullptr, 0, out_dim};
-    for (int l = L; l >= 1; --l) {
-        tcl::LinearParams p;
-        p.M = M;
-        as_input(p, d_cur);
-        p.mode = tcl::kModeMult; p.Mul = c.S[l - 1].as<float>(); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
-        const int ks = (s.N[l - 1] + 15) / 16;
-        p.Cp = c.Dp[(l - 1) & 1].as<uint8_t>(); p.c_ksteps = ks;
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        if (l == s.skip) {
-            // d_skip (the layer's pre-activation gradient) is d_cur here: its column sums feed the condition gradient
-            NPHM_REQUIRE(d_cur.packed, "nphm_mlp_backward_inputs: skip layer directly below the output is not supported");
-            col_sums(d_cur, c.sumss.as<float>());
-            NPHM_CUDA_CHECK(cudaGetLastError());
-            if (grad_xyz_dev) {
-                tcl::LinearParams px;
-                px.M = M;
-                as_input(px, d_cur);
-                px.mode = tcl::kModeLinear; px.C = grad_xyz_dev; px.ldc = 3;
-                if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
-            }
-        }
-        d_cur = Adjoint{nullptr, 0, c.Dp[(l - 1) & 1].as<uint8_t>(), ks, s.N[l - 1]};
-    }
-    col_sums(d_cur, c.sums0.as<float>());
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    if (grad_cond_dev) {
-        NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
-        dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 16);
-        chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.sums0.as<float>(),
-                                                          h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
-                                                          s.N[s.skip - 1] + 3, c.sumss.as<float>(), s.cond_dim, grad_cond_dev);
+    if ((rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
+        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
+        return rc;
+    if (grad_xyz_dev && ((rc = c.xtmp.reserve((size_t)M * 4 * sizeof(float))) || (rc = c.xs_tmp.reserve((size_t)M * 4 * sizeof(float)))))
+        return rc;
+    NPHM_CUDA_CHECK(cudaMemsetAsync(c.qsums0.ptr, 0, (size_t)n_queries * s.N[0] * sizeof(float), stream));
+    NPHM_CUDA_CHECK(cudaMemsetAsync(c.qsumss.ptr, 0, (size_t)n_queries * s.N[s.skip] * sizeof(float), stream));
+    // the output layer's adjoint is the caller's grad_out as it is; d_l lives in Dp[l & 1]
+    AdjointWalk w;
+    w.top = Adjoint{grad_out_dev, out_dim, nullptr, 0};
+    for (int l = 0; l < L; ++l) { w.S[l] = c.S[l].as<float>(); w.D[l] = c.Dp[l & 1].as<uint8_t>(); }
+    w.xs = grad_xyz_dev ? c.xs_tmp.as<float>() : nullptr;
+    // the column sums of d_0 and d_skip feed the condition gradient
+    auto col_sums = [&](int l, const uint8_t *d, int ks) {
+        if (l != 0 && l != s.skip) return NPHM_OK;
+        chain::column_sums_packed_kernel<<<dim3((unsigned)ceil_div(M, 128), (unsigned)ks), 256, 0, stream>>>(
+            d, ks, M, n_points, s.N[l], l == 0 ? c.qsums0.as<float>() : c.qsumss.as<float>());
         NPHM_CUDA_CHECK(cudaGetLastError());
-    }
-    if (grad_xyz_dev) {
-        // + d_0 W_0[:, 0:3]  (the skip-layer part was written above): through a temporary, then accumulate
-        tcl::LinearParams px;
-        px.M = M;
-        as_input(px, d_cur);
-        px.mode = tcl::kModeLinear;
-        if ((rc = c.xtmp.reserve((size_t)M * 4 * sizeof(float)))) return rc;
-        px.C = c.xtmp.as<float>(); px.ldc = 4;
-        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
-        chain::add3_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(c.xtmp.as<float>(), 4, M, grad_xyz_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
+        return NPHM_OK;
+    };
+    if ((rc = adjoint_walk(h, M, w, col_sums, stream))) return rc;
+    if (grad_cond_dev && (rc = cond_grad(h, n_queries, 16, grad_cond_dev, stream))) return rc;
+    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], c.xtmp.as<float>(), w.xs, nullptr, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
 
@@ -511,19 +570,18 @@ static Layout layout(const StackDims &s, int n_queries, long long n_points, int 
 {
     Layout L;
     const long long M = (long long)n_queries * n_points, tiles = ceil_div(M, 128);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    L.cond = take((size_t)n_queries * s.cond_dim * sizeof(float));
+    Carver w;
+    L.cond = w.take((size_t)n_queries * s.cond_dim * sizeof(float));
     L.ldx = pad4(3 + nd);
     L.ks_x0 = (3 + nd + 15) / 16;
-    L.x0 = take((size_t)M * L.ldx * sizeof(float));
-    L.x0p = take((size_t)tiles * L.ks_x0 * 8192);
+    L.x0 = w.take((size_t)M * L.ldx * sizeof(float));
+    L.x0p = w.take((size_t)tiles * L.ks_x0 * 8192);
     for (int l = 0; l + 1 < s.n_lin; ++l) {
         L.ks_h[l] = (s.N[l] + (l + 1 == s.skip ? 3 + nd : 0) + 15) / 16;
-        L.hp[l] = take((size_t)tiles * L.ks_h[l] * 8192);
-        L.s[l] = take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
+        L.hp[l] = w.take((size_t)tiles * L.ks_h[l] * 8192);
+        L.s[l] = w.take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
     }
-    L.total = off;
+    L.total = w.off;
     return L;
 }
 
@@ -633,24 +691,6 @@ __global__ void cond_outer_kernel(const float *__restrict__ sums, const float *_
     *w = (j < nd ? *w : 0.f) + scale * t;
 }
 
-// grad_xyz[r][i] = (a[r][i] + b[r][i]) * scale[1]   (a, b: ld 4)
-__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, const float *__restrict__ scale,
-                                float *__restrict__ out)
-{
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= M * 3) return;
-    const long long r = idx / 3;
-    const int i = (int)(idx % 3);
-    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * scale[1];
-}
-
-static bool noise_layer(const StackDims &s, int l) { return l == 0 || l + 1 == s.skip || l == s.skip; }
-
-static const tcl::PackedLinear &layer(const MlpChain &c, const StackDims &s, int l)
-{
-    return noise_layer(s, l) ? c.tfwd[l] : c.fwd[l];
-}
-
 // what the gradients of one layer need: the forward's workspace and the caller's outputs
 struct GradTargets {
     nphm_mlp *h;
@@ -701,12 +741,12 @@ static int layer_grads(const GradTargets &g, int l, const uint8_t *d, int ks, co
     return NPHM_OK;
 }
 
-// the training variants of layers 0, skip - 1 and skip for nd noise columns
+// the training variants of layers 0, skip - 1 and skip for nd > 0 noise columns (without noise, fwd is used as it is)
 static int pack(nphm_mlp *h, int nd, cudaStream_t stream)
 {
     MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
-    if (c.train_nd == nd) return NPHM_OK;
+    if (nd == 0 || c.train_nd == nd) return NPHM_OK;
     for (int l = 0; l < s.n_lin; ++l) {
         if (!noise_layer(s, l)) continue;
         const int K = l == 0 ? 3 + nd : l == s.skip ? s.N[l - 1] + 3 + nd : s.K[l];
@@ -741,7 +781,6 @@ extern "C" int nphm_mlp_train_forward(nphm_mlp *h, const float *xyz_dev, const f
                  "nphm_mlp_train_forward: bad arguments");
     NPHM_REQUIRE(noise_dim >= 0 && noise_dim <= h->dims.cond_dim && (noise_dim == 0 || cond_noise_dev),
                  "nphm_mlp_train_forward: noise_dim %d out of range [0, %d] or no noise given", noise_dim, h->dims.cond_dim);
-    MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
     const train::Layout L = train::layout(s, n_queries, n_points, noise_dim);
     uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
@@ -756,25 +795,10 @@ extern "C" int nphm_mlp_train_forward(nphm_mlp *h, const float *xyz_dev, const f
     NPHM_CUDA_CHECK(cudaGetLastError());
     NPHM_CUDA_CHECK(cudaMemcpyAsync(ws + L.cond, cond_dev, (size_t)n_queries * s.cond_dim * sizeof(float), cudaMemcpyDeviceToDevice,
                                     stream));
-    for (int l = 0; l < s.n_lin; ++l) {
-        const tcl::PackedLinear &W = train::layer(c, s, l);
-        tcl::LinearParams p;
-        p.M = M;
-        if (l == 0) { p.A1 = X0; p.lda1 = L.ldx; p.K1 = 3 + noise_dim; }
-        else { p.Ap = ws + L.hp[l - 1]; p.a_ksteps = W.ksteps; }
-        p.bias = h->cvec.as<float>() + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = n_points;
-        if (l == s.n_lin - 1) {
-            p.mode = tcl::kModeLinear;
-            p.C = out_dev; p.ldc = s.N[l];
-        } else {
-            p.mode = tcl::kModeSoftplus;
-            p.Cp = ws + L.hp[l]; p.c_ksteps = L.ks_h[l];
-            if (l + 1 == s.skip) { p.app = X0; p.app_ld = L.ldx; p.app_w = 3 + noise_dim; }
-            p.Dv = reinterpret_cast<float *>(ws + L.s[l]); p.lddv = c.ld[l]; p.dv_blocked = 1;
-        }
-        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
-    }
-    return NPHM_OK;
+    uint8_t *Hp[kMaxLayers];
+    float *S[kMaxLayers];
+    for (int l = 0; l + 1 < s.n_lin; ++l) { Hp[l] = ws + L.hp[l]; S[l] = reinterpret_cast<float *>(ws + L.s[l]); }
+    return value_layers(h, M, X0, L.ldx, noise_dim, h->cvec.as<float>(), n_points, Hp, S, out_dev, nullptr, stream);
 }
 
 extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, const void *workspace_dev,
@@ -788,7 +812,6 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
     MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
     const uint8_t *ws = static_cast<const uint8_t *>(workspace_dev);
-    // the workspace must hold a forward of this stack at these sizes (a few bytes read back: the shapes decide the launches)
     // the caller states the shape the workspace was made for; checked against its size, without reading it back
     NPHM_REQUIRE(nd >= 0 && nd <= s.cond_dim && workspace_bytes == (long long)train::layout(s, n_queries, n_points, nd).total,
                  "nphm_mlp_train_backward: a workspace of %lld bytes does not hold a training forward of this network at %d x %lld "
@@ -823,49 +846,15 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
     const train::GradTargets tg{h, &L, ws, n_queries, nd, n_points, gs, grad_w_dev, grad_b_dev, grad_cond_dev != nullptr};
     auto layer_grads = [&](int l, const uint8_t *d, int ks) { return train::layer_grads(tg, l, d, ks, nullptr, nullptr, stream); };
 
-    // d_{l-1} = s_{l-1} * (d_l W_l), from the output layer down to d_0; d_l lives in Dp[l & 1] (d_L in Dl)
-    const uint8_t *d = c.Dl.as<uint8_t>();
-    int ks = ks_out;
-    for (int l = last; l >= 1; --l) {
-        if ((rc = layer_grads(l, d, ks))) return rc;
-        if (l == s.skip && grad_xyz_dev) {
-            tcl::LinearParams px;
-            px.M = M;
-            px.Ap = d; px.a_ksteps = ks;
-            px.mode = tcl::kModeLinear; px.C = c.xs_tmp.as<float>(); px.ldc = 4;
-            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
-        }
-        tcl::LinearParams p;
-        p.M = M;
-        p.Ap = d; p.a_ksteps = ks;
-        p.mode = tcl::kModeMult;
-        p.Mul = reinterpret_cast<const float *>(ws + L.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
-        const int ks_next = (s.N[l - 1] + 15) / 16;
-        p.Cp = c.Dp[(l - 1) & 1].as<uint8_t>(); p.c_ksteps = ks_next;
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        d = c.Dp[(l - 1) & 1].as<uint8_t>();
-        ks = ks_next;
-    }
-    if ((rc = layer_grads(0, d, ks))) return rc;
-    if (grad_cond_dev) {
-        // the noise does not change the gradient with respect to the condition
-        NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
-        dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 1);          // one chunk: a fixed summation order
-        chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
-                                                          h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
-                                                          s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
-    if (grad_xyz_dev) {
-        tcl::LinearParams px;
-        px.M = M;
-        px.Ap = d; px.a_ksteps = ks;
-        px.mode = tcl::kModeLinear; px.C = c.xtmp.as<float>(); px.ldc = 4;
-        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
-        train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(c.xtmp.as<float>(), c.xs_tmp.as<float>(), M, gs,
-                                                                                  grad_xyz_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
+    // d_L in Dl, d_l in Dp[l & 1]
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, c.Dl.as<uint8_t>(), ks_out};
+    for (int l = 0; l < last; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + L.s[l]); w.D[l] = c.Dp[l & 1].as<uint8_t>(); }
+    w.xs = grad_xyz_dev ? c.xs_tmp.as<float>() : nullptr;
+    if ((rc = adjoint_walk(h, M, w, layer_grads, stream))) return rc;
+    // the noise does not change the gradient with respect to the condition; one chunk: a fixed summation order
+    if (grad_cond_dev && (rc = cond_grad(h, n_queries, 1, grad_cond_dev, stream))) return rc;
+    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], c.xtmp.as<float>(), w.xs, gs, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
 
@@ -892,8 +881,6 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
 namespace nphm {
 namespace sdfgrad {
 
-constexpr float kBeta = 100.0f;
-
 // workspace of one forward: the first-order training layout without noise, then the unit column, its scale pair and a_l;
 // then the scratch of the calls: ht_l packed (tg) and zt_l blocked fp32 (zg), the ping-pong of zb (dp), zb_L (dl), the
 // direction as rows of 4 (v4) and packed (vp), and two [M][4] point-gradient temporaries (xa, xb)
@@ -909,44 +896,48 @@ static Layout layout(const StackDims &s, int n_queries, long long n_points)
     Layout G;
     G.base = train::layout(s, n_queries, n_points, 0);
     const long long tiles = ceil_div((long long)n_queries * n_points, 128);
-    size_t off = G.base.total;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    G.unit = take((size_t)tiles * 8192);
-    G.consts = take(2 * sizeof(float));
+    Carver w{G.base.total};
+    G.unit = w.take((size_t)tiles * 8192);
+    G.consts = w.take(2 * sizeof(float));
     for (int l = 0; l + 1 < s.n_lin; ++l) {
         G.ks_a[l] = (s.N[l] + 15) / 16;
-        G.a[l] = take((size_t)tiles * G.ks_a[l] * 8192);
+        G.a[l] = w.take((size_t)tiles * G.ks_a[l] * 8192);
     }
     const size_t M = (size_t)n_queries * n_points;
     for (int l = 0; l + 1 < s.n_lin; ++l) {
-        G.tg[l] = take((size_t)tiles * G.base.ks_h[l] * 8192);
-        G.zg[l] = take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
+        G.tg[l] = w.take((size_t)tiles * G.base.ks_h[l] * 8192);
+        G.zg[l] = w.take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
         G.ks_dp = std::max(G.ks_dp, G.ks_a[l]);                 // zb_l, l < L, in the operand format
     }
-    for (int i = 0; i < 2; ++i) G.dp[i] = take((size_t)tiles * G.ks_dp * 8192);
-    G.dl = take((size_t)tiles * 8192);
-    G.vp = take((size_t)tiles * 8192);
-    G.v4 = take(M * 4 * sizeof(float));
-    G.xa = take(M * 4 * sizeof(float));
-    G.xb = take(M * 4 * sizeof(float));
-    G.total = off;
+    for (int i = 0; i < 2; ++i) G.dp[i] = w.take((size_t)tiles * G.ks_dp * 8192);
+    G.dl = w.take((size_t)tiles * 8192);
+    G.vp = w.take((size_t)tiles * 8192);
+    G.v4 = w.take(M * 4 * sizeof(float));
+    G.xa = w.take(M * 4 * sizeof(float));
+    G.xb = w.take(M * 4 * sizeof(float));
+    G.total = w.off;
     return G;
 }
 
-// packed one-column operand (1 k-step): column 0 = 2^kGradExp on the rows < M, everything else 0; consts = {2^E, 2^-E}.
+// row r of a packed one-column operand (1 k-step): column 0 = v (the fp16 hi part; lo 0), columns 1 .. 15 = 0
+__device__ __forceinline__ void store_column0(uint8_t *__restrict__ dst, long long r, float v)
+{
+    const uint32_t w0 = (uint32_t)__half_as_ushort(__float2half_rn(v));
+    uint8_t *d = dst + (size_t)(r >> 7) * 8192 + (size_t)((r & 127) >> 3) * 256 + (r & 7) * 16;
+    *reinterpret_cast<uint4 *>(d) = make_uint4(w0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(d + 128) = make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(d + 4096 + 128) = make_uint4(0, 0, 0, 0);
+}
+
+// packed one-column operand: column 0 = 2^kGradExp on the rows < M, everything else 0; consts = {2^E, 2^-E}.
 // Thread = row of the padded tiles.
 __global__ void unit_column_kernel(long long M, uint8_t *__restrict__ dst, float *__restrict__ consts)
 {
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (r == 0) { consts[0] = ldexpf(1.0f, train::kGradExp); consts[1] = ldexpf(1.0f, -train::kGradExp); }
     if (r >= (M + 127) / 128 * 128) return;
-    const __half v = __float2half_rn(r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
-    const uint32_t w0 = (uint32_t)__half_as_ushort(v);
-    uint8_t *d = dst + (size_t)(r >> 7) * 8192 + (size_t)((r & 127) >> 3) * 256 + (r & 7) * 16;
-    *reinterpret_cast<uint4 *>(d) = make_uint4(w0, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(d + 128) = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(d + 4096 + 128) = make_uint4(0, 0, 0, 0);
+    store_column0(dst, r, r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
 }
 
 // V[r] = (g_bar[r] * scale[0] * 2^-kGradExp, 0): the tangent direction, ld 4
@@ -990,7 +981,6 @@ extern "C" int nphm_mlp_sdfgrad_forward(nphm_mlp *h, const float *xyz_dev, const
     if (rc) return rc;
     NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && sdf_out_dev && grad_out_dev && workspace_dev,
                  "nphm_mlp_sdfgrad_forward: bad arguments");
-    MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
     const sdfgrad::Layout G = sdfgrad::layout(s, n_queries, n_points);
     uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
@@ -1000,36 +990,13 @@ extern "C" int nphm_mlp_sdfgrad_forward(nphm_mlp *h, const float *xyz_dev, const
     float *consts = reinterpret_cast<float *>(ws + G.consts);
     sdfgrad::unit_column_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128, 256), 256, 0, stream>>>(M, ws + G.unit, consts);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    float *xa = reinterpret_cast<float *>(ws + G.xa), *xb = reinterpret_cast<float *>(ws + G.xb);
     // a_{l-1} = S_{l-1} * (a_l W_l) from the unit column down to a_0, kept in the workspace
-    const uint8_t *d = ws + G.unit;
-    int ks = 1;
-    for (int l = s.n_lin - 1; l >= 1; --l) {
-        if (l == s.skip) {
-            tcl::LinearParams px;
-            px.M = M;
-            px.Ap = d; px.a_ksteps = ks;
-            px.mode = tcl::kModeLinear; px.C = xb; px.ldc = 4;
-            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
-        }
-        tcl::LinearParams p;
-        p.M = M;
-        p.Ap = d; p.a_ksteps = ks;
-        p.mode = tcl::kModeMult;
-        p.Mul = reinterpret_cast<const float *>(ws + G.base.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
-        p.Cp = ws + G.a[l - 1]; p.c_ksteps = G.ks_a[l - 1];
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        d = ws + G.a[l - 1];
-        ks = G.ks_a[l - 1];
-    }
-    tcl::LinearParams px;
-    px.M = M;
-    px.Ap = d; px.a_ksteps = ks;
-    px.mode = tcl::kModeLinear; px.C = xa; px.ldc = 4;
-    if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
-    train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(xa, xb, M, consts, grad_out_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return NPHM_OK;
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, ws + G.unit, 1};
+    for (int l = 0; l + 1 < s.n_lin; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + G.base.s[l]); w.D[l] = ws + G.a[l]; }
+    w.xs = reinterpret_cast<float *>(ws + G.xb);
+    if ((rc = adjoint_walk(h, M, w, [](int, const uint8_t *, int) { return NPHM_OK; }, stream))) return rc;
+    return xyz_grad(h, M, w.D[0], reinterpret_cast<float *>(ws + G.xa), w.xs, consts, grad_out_dev, stream);
 }
 
 extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
@@ -1052,7 +1019,6 @@ extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev,
     const train::Layout &L = G.base;
     const long long M = (long long)n_queries * n_points, tiles = ceil_div(M, 128);
     const int last = s.n_lin - 1;
-    if ((rc = train::pack(h, 0, stream))) return rc;
 
     // one power of two for both upstream gradients; zb_L = s_bar packed, the direction as rows and packed
     if ((rc = c.gscale.reserve(2 * sizeof(float)))) return rc;
@@ -1074,7 +1040,7 @@ extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev,
 
     // tangent pass: ht_l packed (tg, the next layer's input and the GEMM's second H), zt_l blocked fp32 (zg)
     for (int l = 0; l < last; ++l) {
-        const tcl::PackedLinear &W = train::layer(c, s, l);
+        const tcl::PackedLinear &W = c.fwd[l];
         tcl::LinearParams p;
         p.M = M;
         if (l == 0) { p.A1 = v4; p.lda1 = 4; p.K1 = 3; }
@@ -1094,51 +1060,25 @@ extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev,
         (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
         return rc;
     const train::GradTargets targets{h, &L, ws, n_queries, 0, n_points, gs, grad_w_dev, grad_b_dev, grad_cond_dev != nullptr};
+    // dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1}  (a_L: the unit column, ht_{-1}: the direction)
+    auto layer_grads = [&](int l, const uint8_t *d, int ks) {
+        return train::layer_grads(targets, l, d, ks, l == last ? ws + G.unit : ws + G.a[l], l ? tg(l - 1) : vp, stream);
+    };
 
-    // value adjoint with the coupling, from zb_L = s_bar down to zb_0; zb_l lives in dp[l & 1] (zb_L in dl)
-    const uint8_t *d = dl;
-    int ks = 1;
-    for (int l = last; l >= 1; --l) {
-        const uint8_t *a = l == last ? ws + G.unit : ws + G.a[l];
-        if ((rc = train::layer_grads(targets, l, d, ks, a, tg(l - 1), stream))) return rc;
-        if (l == s.skip && grad_xyz_dev) {
-            tcl::LinearParams px;
-            px.M = M;
-            px.Ap = d; px.a_ksteps = ks;
-            px.mode = tcl::kModeLinear; px.C = xb; px.ldc = 4;
-            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
-        }
-        tcl::LinearParams p;
-        p.M = M;
-        p.Ap = d; p.a_ksteps = ks;
-        p.mode = tcl::kModeMult;
-        p.Mul = reinterpret_cast<const float *>(ws + L.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
-        p.cpl_z = zg(l - 1); p.cpl_a = ws + G.a[l - 1]; p.cpl_a_steps = G.ks_a[l - 1]; p.cpl_coef = sdfgrad::kBeta;
-        const int ks_next = (s.N[l - 1] + 15) / 16;
-        p.Cp = ws + G.dp[(l - 1) & 1]; p.c_ksteps = ks_next;
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        d = ws + G.dp[(l - 1) & 1];
-        ks = ks_next;
+    // value adjoint with the coupling, from zb_L = s_bar (in dl) down to zb_0; zb_l lives in dp[l & 1]
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, dl, 1};
+    for (int l = 0; l < last; ++l) {
+        w.S[l] = reinterpret_cast<const float *>(ws + L.s[l]);
+        w.D[l] = ws + G.dp[l & 1];
+        w.cpl_z[l] = zg(l);
+        w.cpl_a[l] = ws + G.a[l];
     }
-    if ((rc = train::layer_grads(targets, 0, d, ks, ws + G.a[0], vp, stream))) return rc;
-    if (grad_cond_dev) {
-        NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
-        dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 1);          // one chunk: a fixed summation order
-        chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
-                                                          h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
-                                                          s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
-    if (grad_xyz_dev) {
-        // s_bar g + H v: the point gradient of zb, as in the first-order backward
-        tcl::LinearParams px;
-        px.M = M;
-        px.Ap = d; px.a_ksteps = ks;
-        px.mode = tcl::kModeLinear; px.C = xa; px.ldc = 4;
-        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
-        train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(xa, xb, M, gs, grad_xyz_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
+    w.xs = grad_xyz_dev ? xb : nullptr;
+    if ((rc = adjoint_walk(h, M, w, layer_grads, stream))) return rc;
+    if (grad_cond_dev && (rc = cond_grad(h, n_queries, 1, grad_cond_dev, stream))) return rc;
+    // s_bar g + H v: the point gradient of zb, as in the first-order backward
+    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], xa, xb, gs, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
 
@@ -1169,16 +1109,15 @@ static Layout layout(const StackDims &s, int n_queries, long long n_points)
     Layout F;
     F.base = train::layout(s, n_queries, n_points, 0);
     const size_t M = (size_t)n_queries * n_points, tiles = (size_t)ceil_div((long long)M, 128);
-    size_t off = F.base.total;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    F.sdf = take(M * sizeof(float));
-    F.dl = take(tiles * 8192);
-    F.consts = take(2 * sizeof(float));
+    Carver w{F.base.total};
+    F.sdf = w.take(M * sizeof(float));
+    F.dl = w.take(tiles * 8192);
+    F.consts = w.take(2 * sizeof(float));
     for (int l = 0; l + 1 < s.n_lin; ++l) F.ks_dp = std::max(F.ks_dp, (s.N[l] + 15) / 16);
-    for (int i = 0; i < 2; ++i) F.dp[i] = take(tiles * F.ks_dp * 8192);
-    F.xa = take(M * 4 * sizeof(float));
-    F.xb = take(M * 4 * sizeof(float));
-    F.total = off;
+    for (int i = 0; i < 2; ++i) F.dp[i] = w.take(tiles * F.ks_dp * 8192);
+    F.xa = w.take(M * 4 * sizeof(float));
+    F.xb = w.take(M * 4 * sizeof(float));
+    F.total = w.off;
     return F;
 }
 
@@ -1205,12 +1144,7 @@ __global__ void __launch_bounds__(kThreads) surface_upstream_kernel(const float 
                 v = s > 0.f ? top : (s < 0.f ? -top : 0.f);
             }
         }
-        const uint32_t w0 = (uint32_t)__half_as_ushort(__float2half_rn(v));
-        uint8_t *d = dst + (size_t)(r >> 7) * 8192 + (size_t)((r & 127) >> 3) * 256 + (r & 7) * 16;
-        *reinterpret_cast<uint4 *>(d) = make_uint4(w0, 0, 0, 0);
-        *reinterpret_cast<uint4 *>(d + 128) = make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4 *>(d + 4096 + 128) = make_uint4(0, 0, 0, 0);
+        sdfgrad::store_column0(dst, r, v);
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) {
@@ -1270,45 +1204,16 @@ extern "C" int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, cons
         (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
         return rc;
     const train::GradTargets targets{h, &F.base, ws, n_queries, 0, n_points, gs, nullptr, nullptr, true};
+    // no weights or biases: the condition sums at layers 0 and skip
+    auto cond_sums = [&](int l, const uint8_t *d, int ks) { return train::layer_grads(targets, l, d, ks, nullptr, nullptr, stream); };
 
     // d_{l-1} = s_{l-1} * (d_l W_l) from the packed upstream down to d_0; d_l lives in dp[l & 1]
-    const uint8_t *d = ws + F.dl;
-    int ks = 1;
-    for (int l = last; l >= 1; --l) {
-        if ((rc = train::layer_grads(targets, l, d, ks, nullptr, nullptr, stream))) return rc;     // condition sums at the skip
-        if (l == s.skip && grad_xyz_dev) {
-            tcl::LinearParams px;
-            px.M = M;
-            px.Ap = d; px.a_ksteps = ks;
-            px.mode = tcl::kModeLinear; px.C = xb; px.ldc = 4;
-            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
-        }
-        tcl::LinearParams p;
-        p.M = M;
-        p.Ap = d; p.a_ksteps = ks;
-        p.mode = tcl::kModeMult;
-        p.Mul = reinterpret_cast<const float *>(ws + F.base.s[l - 1]); p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
-        const int ks_next = (s.N[l - 1] + 15) / 16;
-        p.Cp = ws + F.dp[(l - 1) & 1]; p.c_ksteps = ks_next;
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        d = ws + F.dp[(l - 1) & 1];
-        ks = ks_next;
-    }
-    if ((rc = train::layer_grads(targets, 0, d, ks, nullptr, nullptr, stream))) return rc;
-    NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond_dev, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
-    dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, 1);              // one chunk: a fixed summation order
-    chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
-                                                      h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
-                                                      s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    if (grad_xyz_dev) {
-        tcl::LinearParams px;
-        px.M = M;
-        px.Ap = d; px.a_ksteps = ks;
-        px.mode = tcl::kModeLinear; px.C = xa; px.ldc = 4;
-        if ((rc = tcl::launch_linear(c.adj_x0, px, stream))) return rc;
-        train::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(xa, xb, M, gs, grad_xyz_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, ws + F.dl, 1};
+    for (int l = 0; l < last; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + F.base.s[l]); w.D[l] = ws + F.dp[l & 1]; }
+    w.xs = grad_xyz_dev ? xb : nullptr;
+    if ((rc = adjoint_walk(h, M, w, cond_sums, stream))) return rc;
+    if ((rc = cond_grad(h, n_queries, 1, grad_cond_dev, stream))) return rc;           // one chunk: a fixed summation order
+    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], xa, xb, gs, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }

@@ -32,15 +32,19 @@ from .EnsembledDeepSDF import sample_point_feature  # same function in the refer
 _SQRT2 = math.sqrt(2.0)
 
 
-def _native_backward(ctx, grad_out):
+@once_differentiable
+def _native_backward(ctx, engine_backward, p0, *upstream):
+    """Backward of the native Functions below: ``engine_backward(workspace, *upstream, ...)`` computes what
+    ``needs_input_grad`` asks for; the inputs are (engine, xyz, cond, [noise,] lin0.weight, lin0.bias, ...) with the
+    parameters from index ``p0`` on."""
     ws, *params = ctx.saved_tensors                   # raises if a parameter was changed in place since the forward
-    need = ctx.needs_input_grad                       # (engine, xyz, cond, noise, lin0.weight, lin0.bias, ...)
-    gw, gb, g_cond, g_xyz = ctx.engine.train_backward(ws, grad_out, ctx.noise_dim, weights=any(need[4::2]), biases=any(need[5::2]),
-                                                      want_cond=need[2], want_xyz=need[1])
-    grads = [None, g_xyz, g_cond, None]
+    need = ctx.needs_input_grad
+    gw, gb, g_cond, g_xyz = engine_backward(ws, *upstream, weights=any(need[p0::2]), biases=any(need[p0 + 1::2]),
+                                            want_cond=need[2], want_xyz=need[1])
+    grads = [None, g_xyz, g_cond] + [None] * (p0 - 3)
     for i in range(len(params) // 2):
-        grads.append(gw[i] if need[4 + 2 * i] else None)
-        grads.append(gb[i] if need[5 + 2 * i] else None)
+        grads.append(gw[i] if need[p0 + 2 * i] else None)
+        grads.append(gb[i] if need[p0 + 1 + 2 * i] else None)
     return tuple(grads)
 
 
@@ -62,25 +66,7 @@ class _NativeTrainFn(torch.autograd.Function):
         if torch.is_grad_enabled():
             raise RuntimeError('forward_native_grad is differentiable to first order only: a double backward '
                                '(create_graph=True) through it is not supported; use the composite forward() instead')
-        return _native_backward_once(ctx, grad_out)
-
-
-_native_backward_once = once_differentiable(_native_backward)
-
-
-def _sdfgrad_backward(ctx, grad_sdf, grad_grad):
-    ws, *params = ctx.saved_tensors                   # raises if a parameter was changed in place since the forward
-    need = ctx.needs_input_grad                       # (engine, xyz, cond, lin0.weight, lin0.bias, ...)
-    gw, gb, g_cond, g_xyz = ctx.engine.sdfgrad_backward(ws, grad_sdf, grad_grad, weights=any(need[3::2]), biases=any(need[4::2]),
-                                                        want_cond=need[2], want_xyz=need[1])
-    grads = [None, g_xyz, g_cond]
-    for i in range(len(params) // 2):
-        grads.append(gw[i] if need[3 + 2 * i] else None)
-        grads.append(gb[i] if need[4 + 2 * i] else None)
-    return tuple(grads)
-
-
-_sdfgrad_backward_once = once_differentiable(_sdfgrad_backward)
+        return _native_backward(ctx, ctx.engine.train_backward, 4, grad_out, ctx.noise_dim)
 
 
 class _NativeSdfGradFn(torch.autograd.Function):
@@ -101,7 +87,7 @@ class _NativeSdfGradFn(torch.autograd.Function):
         if torch.is_grad_enabled():
             raise RuntimeError('forward_with_gradient_native is differentiable to first order only: a double backward '
                                '(create_graph=True) through it is not supported; use the composite forward() instead')
-        return _sdfgrad_backward_once(ctx, grad_sdf, grad_grad)
+        return _native_backward(ctx, ctx.engine.sdfgrad_backward, 3, grad_sdf, grad_grad)
 
 
 class DeepSDF(nn.Module):
