@@ -109,6 +109,7 @@ typedef struct {
     int out_dim;      /* 3                                                   */
 } nphm_mlp_config;
 
+/* accepts lat_dim >= 1, hidden_dim > lat_dim + 3, 2 <= n_layers <= 10, 1 <= out_dim <= 8 (else NPHM_ERR_INVALID) */
 int nphm_mlp_create(const nphm_mlp_config *cfg, nphm_mlp **out);
 void nphm_mlp_destroy(nphm_mlp *h);
 /* w_dev[l]: (out_l, in_l) row-major, b_dev[l]: (out_l), l = 0..n_layers (keys lin{l}.weight/bias). */

@@ -72,9 +72,10 @@ class FitParams(Structure):
                 ('lr', c_float), ('step', c_int)]
 
 
-def stack_supported(n_hidden_layers: int, hidden: int, cond_dim: int) -> bool:
-    """Configurations ``build_stack`` (csrc/api.cu) accepts; anything else takes the composite PyTorch path."""
-    return 2 <= n_hidden_layers <= 10 and hidden > cond_dim + 3
+def stack_supported(n_hidden_layers: int, hidden: int, cond_dim: int, out_dim: int = 1) -> bool:
+    """Configurations ``nphm_mlp_create`` / ``build_stack`` (csrc/api.cu) accept: 2 to 10 hidden layers, a condition of at
+    least one column, ``hidden > cond_dim + 3`` and 1 to 8 outputs; anything else takes the composite PyTorch path."""
+    return 2 <= n_hidden_layers <= 10 and cond_dim >= 1 and hidden > cond_dim + 3 and 1 <= out_dim <= 8
 
 
 def hidden_width(module, n_lin: int) -> int:

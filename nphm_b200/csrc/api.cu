@@ -309,6 +309,9 @@ extern "C" int nphm_mlp_create(const nphm_mlp_config *cfg, nphm_mlp **out)
     NPHM_REQUIRE(cfg && out, "nphm_mlp_create: NULL argument");
     NPHM_REQUIRE(cfg->lat_dim > 0 && cfg->hidden_dim > 0 && cfg->out_dim >= 1 && cfg->out_dim <= 8,
                  "nphm_mlp_create: unsupported widths (out_dim must be 1..8)");
+    // 2..10 hidden layers: the depths _native.stack_supported sends here and the test suite runs (build_stack would take 11)
+    NPHM_REQUIRE(cfg->n_layers >= 2 && cfg->n_layers <= 10, "nphm_mlp_create: unsupported number of hidden layers %d (2..10)",
+                 cfg->n_layers);
     auto *h = new nphm_mlp();
     h->cfg = *cfg;
     int rc = build_stack(h->dims, cfg->lat_dim, cfg->hidden_dim, cfg->n_layers, cfg->out_dim);

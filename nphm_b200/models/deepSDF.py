@@ -143,8 +143,8 @@ class DeepSDF(nn.Module):
             return False
         n_lin = self.num_layers - 1
         hidden = _native.hidden_width(self, n_lin)
-        if self.out_dim_net > 8 or not _native.stack_supported(n_lin - 1, hidden, self.lat_dim):
-            return False             # depths the native stack builder rejects: PyTorch composite path
+        if not _native.stack_supported(n_lin - 1, hidden, self.lat_dim, self.out_dim_net):
+            return False             # shapes the native stack builder rejects: PyTorch composite path
         if torch.is_grad_enabled() and (xyz.requires_grad or lat_rep.requires_grad
                                         or any(p.requires_grad for p in self.parameters())):
             return False
@@ -157,8 +157,8 @@ class DeepSDF(nn.Module):
         if lat_rep is not None and not (lat_rep.dim() == 2 or lat_rep.shape[1] == 1 or lat_rep.stride(1) == 0):
             return False
         return (xyz.is_cuda and xyz.dtype == torch.float32 and xyz.dim() == 3 and self.num_freq_bands is None
-                and self.beta == 100 and self.out_dim_net <= 8 and next(self.parameters()).dtype == torch.float32
-                and _native.stack_supported(n_lin - 1, _native.hidden_width(self, n_lin), self.lat_dim))
+                and self.beta == 100 and next(self.parameters()).dtype == torch.float32
+                and _native.stack_supported(n_lin - 1, _native.hidden_width(self, n_lin), self.lat_dim, self.out_dim_net))
 
     def _native_train(self, xyz, cond, noise=None):
         """xyz B x N x 3, cond B x lat_dim (differentiable), noise B x N x d or None -> B x N x out_dim."""

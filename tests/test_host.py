@@ -203,6 +203,28 @@ def test_library_exports_every_declared_symbol():
     assert lib.nphm_abi_version() == 1
 
 
+def test_stack_supported_agrees_with_nphm_mlp_create():
+    """``_native.stack_supported`` sends a DeepSDF stack to the native kernels, which have no fallback once chosen: it must
+    accept exactly the shapes ``nphm_mlp_create`` accepts.  Creating a handle runs host code only (no device memory), so this
+    runs without a GPU.  A condition of width 0 is one the library rejects: such a stack takes the composite path."""
+    from ctypes import byref, c_void_p
+    from nphm_b200 import _native
+    L = _native.lib()
+    wrong = []
+    for n_layers in (1, 2, 3, 10, 11):
+        for lat in (0, 1, 5, 64):
+            for hidden in (lat + 3, lat + 4, lat + 100):
+                for out in (0, 1, 2, 8, 9):
+                    h = c_void_p()
+                    rc = L.nphm_mlp_create(byref(_native.MlpConfig(lat, hidden, n_layers, out)), byref(h))
+                    if rc == 0:
+                        L.nphm_mlp_destroy(h)
+                    if (rc == 0) != _native.stack_supported(n_layers, hidden, lat, out):
+                        wrong.append((n_layers, hidden, lat, out, rc))
+    assert not wrong, wrong
+    assert not _native.stack_supported(8, 512, 0) and _native.stack_supported(8, 512, 1)
+
+
 def test_fused_path_refuses_to_run_without_library(monkeypatch):
     """The product path must fail loudly when the CUDA extension is missing."""
     from nphm_b200 import _native
