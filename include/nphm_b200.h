@@ -277,6 +277,20 @@ int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev, const floa
                               long long workspace_bytes, int n_queries, long long n_points, float *const *grad_w_dev,
                               float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream);
 
+/* ---- the same for the members of the ensemble (stage 1 of NPHM, train.py -local): every member k of the handle as a
+ * one-output stack with its weight set, one launch per pass for all members.  Member-major layouts: xyz_local_dev and
+ * grad_xyz_dev [members][B][N][3] in each member's frame (the caller applies the mirror), cond_dev and grad_cond_dev
+ * [members][B][lat_dim_glob + lat_dim_loc], sdf_out_dev [members][B][N], grad_out_dev [members][B][N][3], grad_w_dev[l] /
+ * grad_b_dev[l] in the state_dict layout of ensembled_deep_sdf.lin{l}.weight / bias ([sets][out][in], [sets][out]; a mirrored
+ * set sums its two members).  Workspace contract and determinism as for nphm_mlp_sdfgrad_*; the upstream gradients are
+ * scaled by one power of two per weight set, so a set whose upstream is all zero gets exactly zero gradients. */
+long long nphm_ensemble_sdfgrad_workspace_bytes(const nphm_ensemble *h, int n_batch, long long n_points);
+int nphm_ensemble_sdfgrad_forward(nphm_ensemble *h, const float *xyz_local_dev, const float *cond_dev, int n_batch,
+                                  long long n_points, float *sdf_out_dev, float *grad_out_dev, void *workspace_dev, void *stream);
+int nphm_ensemble_sdfgrad_backward(nphm_ensemble *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
+                                   long long workspace_bytes, int n_batch, long long n_points, float *const *grad_w_dev,
+                                   float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream);
+
 /* ---- fitting with a one-output DeepSDF stack (the NPM baseline's identity decoder): the surface term of
  * inference_identity_space and inference_iterative_root_finding_joint (reference src/NPHM/models/fitting.py:114-125, :229-247)
  *   loss = mean over { p : mask[p] != 0 and |s_p| < clamp } of |s_p|,   s = f(xyz, cond)

@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = (
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
     'nphm_mlp_sdfgrad_workspace_bytes', 'nphm_mlp_sdfgrad_forward', 'nphm_mlp_sdfgrad_backward',
     'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad',
+    'nphm_ensemble_sdfgrad_workspace_bytes', 'nphm_ensemble_sdfgrad_forward', 'nphm_ensemble_sdfgrad_backward',
 )
 
 
@@ -168,6 +169,12 @@ def lib() -> ctypes.CDLL:
     L.nphm_mlp_fit_workspace_bytes.restype = c_longlong
     L.nphm_mlp_fit_surface_grad.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_float, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_ensemble_sdfgrad_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong]
+    L.nphm_ensemble_sdfgrad_workspace_bytes.restype = c_longlong
+    L.nphm_ensemble_sdfgrad_forward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p,
+                                                c_void_p]
+    L.nphm_ensemble_sdfgrad_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_longlong,
+                                                 POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -242,6 +249,7 @@ class EnsembleEngine(_Versioned):
         self.n_lin = n_lin
         self.n_loc = module.num_kps
         self.lat_dim = module.lat_dim
+        self.lat_dim_glob, self.lat_dim_loc = module.lat_dim_glob, module.lat_dim_loc
         self._sig = None
         self.device = None
 
@@ -339,6 +347,43 @@ class EnsembleEngine(_Versioned):
                                                       g_lat.data_ptr(), g_pts.data_ptr(), None, _stream_ptr(dev)),
                   'nphm_ensemble_backward_inputs')
         return sdf, g_lat, g_pts
+
+    # ---------------------------------------------------------------- training through grad_x sdf (second order)
+    def sdfgrad_forward(self, xyz_local: torch.Tensor, cond: torch.Tensor):
+        """Every member's SDF and its gradient in the member's own frame, keeping what the backward needs
+        (nphm_ensemble_sdfgrad_forward): xyz_local members x B x N x 3 (mirror applied), cond members x B x (lat_dim_glob +
+        lat_dim_loc) -> ``(s members x B x N, g members x B x N x 3, workspace)``."""
+        K, B, N, _ = xyz_local.shape
+        dev = xyz_local.device
+        xyz_local = _f32c(xyz_local)
+        cond = _f32c(cond).to(dev)
+        s = torch.empty(K, B, N, device=dev, dtype=torch.float32)
+        g = torch.empty(K, B, N, 3, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            ws = _workspace(lib().nphm_ensemble_sdfgrad_workspace_bytes(self._h, B, N), 'nphm_ensemble_sdfgrad_workspace_bytes', dev)
+            check(lib().nphm_ensemble_sdfgrad_forward(self._h, xyz_local.data_ptr(), cond.data_ptr(), B, N, s.data_ptr(),
+                                                      g.data_ptr(), ws.data_ptr(), _stream_ptr(dev)), 'nphm_ensemble_sdfgrad_forward')
+        return s, g, ws
+
+    def sdfgrad_backward(self, ws: torch.Tensor, grad_s: torch.Tensor, grad_g: torch.Tensor, layer_shapes, weights: bool = True,
+                         biases: bool = True, want_cond: bool = True, want_xyz: bool = True):
+        """Backward of :meth:`sdfgrad_forward` (nphm_ensemble_sdfgrad_backward) for grad_s members x B x N and grad_g
+        members x B x N x 3; ``layer_shapes``: the ``ensembled_deep_sdf.lin{l}.weight`` shapes.  Returns ``(weight grads |
+        None, bias grads | None, d/d cond members x B x C | None, d/d xyz_local members x B x N x 3 | None)``."""
+        K, B, N, _ = grad_g.shape
+        dev = grad_g.device
+        gs, gg = _f32c(grad_s), _f32c(grad_g)
+        gw = [torch.empty(s, device=dev, dtype=torch.float32) for s in layer_shapes] if weights else None
+        gb = [torch.empty(s[:2], device=dev, dtype=torch.float32) for s in layer_shapes] if biases else None
+        C = self.lat_dim_glob + self.lat_dim_loc
+        g_cond = torch.empty(K, B, C, device=dev, dtype=torch.float32) if want_cond else None
+        g_xyz = torch.empty(K, B, N, 3, device=dev, dtype=torch.float32) if want_xyz else None
+        with torch.cuda.device(dev):
+            check(lib().nphm_ensemble_sdfgrad_backward(self._h, gs.data_ptr(), gg.data_ptr(), ws.data_ptr(), ws.numel(), B, N,
+                                                       _ptr_array(gw) if gw else None, _ptr_array(gb) if gb else None,
+                                                       _ptr(g_cond), _ptr(g_xyz), _stream_ptr(dev)),
+                  'nphm_ensemble_sdfgrad_backward')
+        return gw, gb, g_cond, g_xyz
 
     def query_grid(self, latent: torch.Tensor, mini, maxi, res: int, first: int, count: int, quirk_period: int,
                    impl: Optional[int] = None, out: Optional[torch.Tensor] = None):

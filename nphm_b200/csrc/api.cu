@@ -145,7 +145,7 @@ extern "C" int nphm_ensemble_create(const nphm_ensemble_config *cfg, nphm_ensemb
 
 extern "C" void nphm_ensemble_destroy(nphm_ensemble *h)
 {
-    if (h) nphm::fit_packs_destroy(h);
+    if (h) { nphm::fit_packs_destroy(h); nphm::ensemble_chain_destroy(h); }
     delete h;
 }
 
@@ -180,6 +180,7 @@ extern "C" int nphm_ensemble_load_weights(nphm_ensemble *h, const float *const *
     rc = tc_ensemble_pack(h, stream);
     if (rc) return rc;
     fit_packs_destroy(h);                      // packed from the previous weights, rebuilt by the next fitting call
+    ensemble_chain_destroy(h);                 // likewise, by the next SDF-gradient forward
     h->loaded = true;
     return NPHM_OK;
 }

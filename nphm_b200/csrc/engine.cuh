@@ -35,7 +35,7 @@ void fill_descriptors(const StackDims &s, const NetWeights &w, int n_members, in
 
 }  // namespace nphm
 
-namespace nphm { namespace fit { struct BackwardPacks; } }
+namespace nphm { namespace fit { struct BackwardPacks; } struct EnsembleChain; }
 
 struct nphm_ensemble {
     nphm_ensemble_config cfg;
@@ -56,6 +56,8 @@ struct nphm_ensemble {
     // fitting (fit.cu)
     nphm::DeviceBuffer fit_scratch, fit_apply_scratch;
     nphm::fit::BackwardPacks *fit_packs = nullptr;      // adjoint weights of the backward GEMMs, built on first use
+    // stage-1 training through grad_x sdf (mlp_chain.cu): the layer chain of all weight sets, packed on first use
+    nphm::EnsembleChain *sdfgrad = nullptr;
 };
 
 namespace nphm { struct MlpChain; }
@@ -85,6 +87,7 @@ bool chain_packed(const nphm_mlp *h);
 int chain_forward(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, cudaStream_t stream);
 // fitting (fit.cu)
 void fit_packs_destroy(nphm_ensemble *h);
+void ensemble_chain_destroy(nphm_ensemble *h);
 // layer chain (mlp_chain.cu)
 int chain_pack(nphm_mlp *h, cudaStream_t stream);
 void chain_destroy(nphm_mlp *h);

@@ -1217,3 +1217,541 @@ extern "C" int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, cons
     if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], xa, xb, gs, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
+
+// ================================================================================================ the NPHM ensemble through grad_x sdf
+// Stage 1 of the ensemble (reference train.py -local): the SDF-gradient passes above for all members at once.  Member k
+// (weight set sigma(k): k / 2 for the 2 n_symm mirrored members, k - n_symm beyond) sees B queries of N points in its own
+// frame; every pass is one launch over all members (tc_linear batched over gridDim.z = member, tc_wgrad over gridDim.z =
+// weight set).  Rows of one member: Mm = B N in Tm = ceil(Mm / 128) tiles; every per-row buffer is member-major with a
+// whole number of tiles per member, so member k's part starts at k times the member stride.  Per-(member, query) bias
+// rows carry the folded condition constants.  fp16 range: one power of two per weight set (its members' s_bar and g_bar
+// can differ by orders of magnitude from the other sets', through the blend weights); an all-zero set gets scale 1 and
+// exactly zero gradients.
+namespace nphm {
+struct EnsembleChain {
+    bool packed = false;
+    tcl::PackedLinear fwd[kMaxLayers], adj[kMaxLayers], adj_x0, adj_xs;     // all weight sets back to back
+    int ld[kMaxLayers];
+    DeviceBuffer partials, sums, sums0, sumss;
+};
+
+void ensemble_chain_destroy(nphm_ensemble *h)
+{
+    delete h->sdfgrad;
+    h->sdfgrad = nullptr;
+}
+
+namespace esdf {
+
+__device__ __forceinline__ int dset(int m, int n_symm) { return m < 2 * n_symm ? m >> 1 : m - n_symm; }
+
+static int pack(nphm_ensemble *h, cudaStream_t stream)
+{
+    if (!h->sdfgrad) h->sdfgrad = new EnsembleChain();
+    EnsembleChain &c = *h->sdfgrad;
+    if (c.packed) return NPHM_OK;
+    const StackDims &s = h->dims;
+    const int S = h->n_sets;
+    int rc;
+    for (int l = 0; l < s.n_lin; ++l) {
+        const float *W = h->weights.W[l].as<float>();
+        const int ldw = s.in_total[l];
+        const long long ws = (long long)s.N[l] * ldw;
+        const float scale = l == s.skip ? chain::kInvSqrt2 : 1.0f;
+        if ((rc = c.fwd[l].pack(W, ldw, s.N[l], s.K[l], 0, 0, false, scale, stream, S, ws, nullptr, 0, l + 1 == s.skip ? 3 : 0,
+                                kChainNt)))
+            return rc;
+        if (l >= 1 && (rc = c.adj[l].pack(W, ldw, s.N[l - 1], s.N[l], 0, 0, true, scale, stream, S, ws, nullptr, 0, 0, kChainNt)))
+            return rc;
+        c.ld[l] = pad4(s.N[l]);
+    }
+    if ((rc = c.adj_x0.pack(h->weights.W[0].as<float>(), s.in_total[0], 3, s.N[0], 0, 0, true, 1.0f, stream, S,
+                            (long long)s.N[0] * s.in_total[0])))
+        return rc;
+    if ((rc = c.adj_xs.pack(h->weights.W[s.skip].as<float>(), s.in_total[s.skip], 3, s.N[s.skip], s.N[s.skip - 1], 0, true,
+                            chain::kInvSqrt2, stream, S, (long long)s.N[s.skip] * s.in_total[s.skip])))
+        return rc;
+    c.packed = true;
+    return NPHM_OK;
+}
+
+// workspace: pieces of all members (member stride m_*) laid out like sdfgrad::Layout, plus the folded constants and the
+// condition of every (member, query) and one scale pair per weight set
+struct Layout {
+    size_t cvec = 0, cond = 0, gs = 0, consts = 0, x0p = 0, hp[kMaxLayers] = {}, s[kMaxLayers] = {}, unit = 0, a[kMaxLayers] = {};
+    size_t tg[kMaxLayers] = {}, zg[kMaxLayers] = {}, dp[2] = {}, dl = 0, vp = 0, v4 = 0, xa = 0, xb = 0, total = 0;
+    long long m_hp[kMaxLayers] = {}, m_s[kMaxLayers] = {}, m_a[kMaxLayers] = {}, m_dp = 0, m_one = 0, m_row4 = 0;
+    int ks_h[kMaxLayers] = {}, ks_a[kMaxLayers] = {}, ks_dp = 1;
+};
+
+static Layout layout(const nphm_ensemble *h, int n_batch, long long n_points)
+{
+    const StackDims &s = h->dims;
+    const int K = h->n_members;
+    const long long Mm = (long long)n_batch * n_points, T = ceil_div(Mm, 128);
+    Layout G;
+    Carver w;
+    G.cvec = w.take((size_t)K * n_batch * s.cvec_stride * sizeof(float));
+    G.cond = w.take((size_t)K * n_batch * s.cond_dim * sizeof(float));
+    G.gs = w.take((size_t)h->n_sets * 2 * sizeof(float));
+    G.consts = w.take(2 * sizeof(float));
+    G.m_one = T * 8192;
+    G.m_row4 = Mm * 4 * sizeof(float);
+    G.x0p = w.take((size_t)K * G.m_one);
+    for (int l = 0; l + 1 < s.n_lin; ++l) {
+        G.ks_h[l] = (s.N[l] + (l + 1 == s.skip ? 3 : 0) + 15) / 16;
+        G.ks_a[l] = (s.N[l] + 15) / 16;
+        G.ks_dp = std::max(G.ks_dp, G.ks_a[l]);
+        G.m_hp[l] = T * G.ks_h[l] * 8192;
+        G.m_s[l] = T * 128 * pad4(s.N[l]) * sizeof(float);
+        G.m_a[l] = T * G.ks_a[l] * 8192;
+        G.hp[l] = w.take((size_t)K * G.m_hp[l]);
+        G.s[l] = w.take((size_t)K * G.m_s[l]);
+        G.a[l] = w.take((size_t)K * G.m_a[l]);
+        G.tg[l] = w.take((size_t)K * G.m_hp[l]);
+        G.zg[l] = w.take((size_t)K * G.m_s[l]);
+    }
+    G.m_dp = T * G.ks_dp * 8192;
+    G.unit = w.take((size_t)K * G.m_one);
+    for (int i = 0; i < 2; ++i) G.dp[i] = w.take((size_t)K * G.m_dp);
+    G.dl = w.take((size_t)K * G.m_one);
+    G.vp = w.take((size_t)K * G.m_one);
+    G.v4 = w.take((size_t)K * G.m_row4);
+    G.xa = w.take((size_t)K * G.m_row4);
+    G.xb = w.take((size_t)K * G.m_row4);
+    G.total = w.off;
+    return G;
+}
+
+// cvec[k][q][coff_l + n]: b_l[sigma][n], plus at the folded layers scale_l * W_l[sigma][n][K_l:] . cond[k][q], summed in the
+// order of simt.cu's cvec_kernel (so a member's constants equal those of its weight set as a single stack).  grid (members,
+// queries), one warp per output row
+__global__ void cvec_kernel(const PackSpec spec, const float *__restrict__ cond, int n_batch, float *__restrict__ cvec)
+{
+    const int m = blockIdx.x, q = blockIdx.y, C = spec.cond_dim, set = dset(m, spec.n_symm);
+    const float *u = cond + ((size_t)m * n_batch + q) * C;
+    float *out = cvec + ((size_t)m * n_batch + q) * spec.cvec_stride;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+    for (int l = 0; l < spec.n_layers; ++l) {
+        const PackLayer &pl = spec.L[l];
+        for (int n = warp; n < pl.Npad; n += wpb) {
+            float v = 0.f;
+            if (n < pl.N) {
+                v = pl.b[(size_t)set * pl.N + n];
+                if (pl.folded) {
+                    const float *w = pl.W + ((size_t)set * pl.N + n) * pl.in_total + pl.K;
+                    float s = 0.f;
+                    for (int j = lane; j < C; j += 32) s = fmaf(w[j], u[j], s);
+#pragma unroll
+                    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+                    v = fmaf(s, pl.scale, v);
+                }
+            }
+            if (lane == 0) out[pl.coff + n] = v;
+        }
+    }
+}
+
+// member-batched train::pack_rows_kernel: member m = blockIdx.y reads src + m src_stride (floats), writes dst + m dst_stride
+// (bytes); scale (optional): the pair of m's weight set, scale[2 sigma(m)]
+__global__ void pack_rows_kernel(const float *__restrict__ src, int ld, int width, long long M, long long src_stride,
+                                 const float *__restrict__ scale, int n_symm, uint8_t *__restrict__ dst, long long dst_stride)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int m = blockIdx.y;
+    if (idx >= (M + 127) / 128 * 128 * 2) return;
+    const long long row = idx / 2;
+    const int g = (int)(idx % 2);
+    const float sc = scale ? scale[2 * dset(m, n_symm)] : 1.0f;
+    const float *sr = src + (size_t)m * src_stride;
+    float v[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int c = 8 * g + i;
+        v[i] = (row < M && c < width) ? sr[(size_t)row * ld + c] * sc : 0.f;
+    }
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) tc::split2(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
+    uint8_t *d = dst + (size_t)m * dst_stride + (size_t)(row >> 7) * 8192 + (size_t)((row & 127) >> 3) * 256 + g * 128 + (row & 7) * 16;
+    *reinterpret_cast<uint4 *>(d) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
+
+// the unit column of every member (sdfgrad::unit_column_kernel); grid (row blocks, members)
+__global__ void unit_column_kernel(long long M, uint8_t *__restrict__ dst, long long stride, float *__restrict__ consts)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0 && blockIdx.y == 0) { consts[0] = ldexpf(1.0f, train::kGradExp); consts[1] = ldexpf(1.0f, -train::kGradExp); }
+    if (r >= (M + 127) / 128 * 128) return;
+    sdfgrad::store_column0(dst + (size_t)blockIdx.y * stride, r, r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
+}
+
+// gs[2 z] = 2^(kGradExp - e), gs[2 z + 1] = its inverse, 2^e <= max |.| < 2^(e+1) over the rows of set z's members of s_bar
+// (M per member) and g_bar (3 M); 1 for an all-zero or non-finite set.  One block per set.
+__global__ void set_scale_kernel(const float *__restrict__ gsdf, const float *__restrict__ ggrad, long long M, int n_symm,
+                                 float *__restrict__ gs)
+{
+    __shared__ float red[32];
+    const int z = blockIdx.x;
+    const int m0 = z < n_symm ? 2 * z : z + n_symm, n_mem = z < n_symm ? 2 : 1;
+    float mx = 0.f;
+    for (int k = 0; k < n_mem; ++k) {
+        const float *a = gsdf + (size_t)(m0 + k) * M, *b = ggrad + (size_t)(m0 + k) * M * 3;
+        for (long long i = threadIdx.x; i < M; i += blockDim.x) mx = fmaxf(mx, fabsf(a[i]));
+        for (long long i = threadIdx.x; i < 3 * M; i += blockDim.x) mx = fmaxf(mx, fabsf(b[i]));
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) mx = fmaxf(mx, red[w]);
+        const int e = (mx > 0.f && isfinite(mx)) ? max(-100, min(100, ilogbf(mx))) - train::kGradExp : 0;
+        gs[2 * z] = ldexpf(1.0f, -e);
+        gs[2 * z + 1] = ldexpf(1.0f, e);
+    }
+}
+
+// V[m][r] = (g_bar[m][r] * gs[2 sigma(m)] 2^-kGradExp, 0), ld 4
+__global__ void direction_kernel(const float *__restrict__ gg, long long M, int members, const float *__restrict__ gs, int n_symm,
+                                 float *__restrict__ V)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)members * M * 4) return;
+    const long long r = idx >> 2;
+    const int c = (int)(idx & 3), m = (int)(r / M);
+    V[idx] = c < 3 ? gg[r * 3 + c] * (gs[2 * dset(m, n_symm)] * ldexpf(1.0f, -train::kGradExp)) : 0.f;
+}
+
+// out[m][r][i] = (a[m][r][i] + b[m][r][i]) * scale[sstride sigma(m) + 1]   (a, b: ld 4)
+__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, int members,
+                                const float *__restrict__ scale, int sstride, int n_symm, float *__restrict__ out)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)members * M * 3) return;
+    const long long r = idx / 3;
+    const int i = (int)(idx % 3), m = (int)(r / M);
+    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * scale[sstride * dset(m, n_symm) + 1];
+}
+
+// train::query_sums_kernel over the members (blockIdx.z): out[m][q][c] = gs[2 sigma(m) + 1] * sum over the rows of (m, q)
+__global__ void __launch_bounds__(256) query_sums_kernel(const uint8_t *__restrict__ X, int ks, long long stride, long long n_points,
+                                                         int n_batch, int n_cols, const float *__restrict__ gs, int n_symm,
+                                                         float *__restrict__ out)
+{
+    __shared__ float part[16][17];
+    const int c = threadIdx.x & 15, rl = threadIdx.x >> 4, j = blockIdx.x, q = blockIdx.y, m = blockIdx.z;
+    const uint8_t *Xm = X + (size_t)m * stride;
+    const long long r1 = (long long)(q + 1) * n_points;
+    float s = 0.f;
+    for (long long r = (long long)q * n_points + rl; r < r1; r += 16) {
+        const uint8_t *p = Xm + ((size_t)(r >> 7) * ks + j) * 8192 + (size_t)((r & 127) >> 3) * 256 + (c >> 3) * 128 + (r & 7) * 16 + (c & 7) * 2;
+        s += __half2float(*reinterpret_cast<const __half *>(p)) + __half2float(*reinterpret_cast<const __half *>(p + 4096));
+    }
+    part[rl][c] = s;
+    __syncthreads();
+    if (rl == 0 && j * 16 + c < n_cols) {
+        float t = 0.f;
+        for (int i = 0; i < 16; ++i) t += part[i][c];
+        out[((size_t)m * n_batch + q) * n_cols + j * 16 + c] = t * gs[2 * dset(m, n_symm) + 1];
+    }
+}
+
+// gb[z][c] = sum over the members of set z (in order) and their queries of sums[m][q][c]; grid (column blocks, sets)
+__global__ void bias_grad_kernel(const float *__restrict__ sums, int n_batch, int n, int n_symm, float *__restrict__ gb)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x, z = blockIdx.y;
+    if (c >= n) return;
+    const int m0 = z < n_symm ? 2 * z : z + n_symm, n_mem = z < n_symm ? 2 : 1;
+    float t = 0.f;
+    for (int k = 0; k < n_mem; ++k)
+        for (int q = 0; q < n_batch; ++q) t += sums[((size_t)(m0 + k) * n_batch + q) * n + c];
+    gb[(size_t)z * n + c] = t;
+}
+
+// condition columns of layer 0 / skip: dW[z][n][c0 + j] = scale * sum over set z's members m and queries q of
+// sums[m][q][n] cond[m][q][j]; grid (blocks of N x cond_dim, sets)
+__global__ void cond_outer_kernel(const float *__restrict__ sums, const float *__restrict__ cond, int n_batch, int N, int cond_dim,
+                                  int n_symm, float scale, float *__restrict__ dW, int ldw, long long w_stride, int c0)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int z = blockIdx.y;
+    if (idx >= (long long)N * cond_dim) return;
+    const int n = (int)(idx / cond_dim), j = (int)(idx % cond_dim);
+    const int m0 = z < n_symm ? 2 * z : z + n_symm, n_mem = z < n_symm ? 2 : 1;
+    float t = 0.f;
+    for (int k = 0; k < n_mem; ++k)
+        for (int q = 0; q < n_batch; ++q) {
+            const size_t mq = (size_t)(m0 + k) * n_batch + q;
+            t = fmaf(sums[mq * N + n], cond[mq * cond_dim + j], t);
+        }
+    dW[(size_t)z * w_stride + (size_t)n * ldw + c0 + j] = scale * t;
+}
+
+// grad_cond[m][q][j] = sum_n W0[sigma][n][3 + j] S0[m][q][n] + sum_n Ws[sigma][n][c0s + j] Ss[m][q][n] / sqrt(2), fixed order;
+// grid (column blocks, queries, members)
+__global__ void cond_grad_kernel(const float *__restrict__ W0, int ld0, int N0, const float *__restrict__ S0,
+                                 const float *__restrict__ Ws, int lds, int Ns, int c0s, const float *__restrict__ Ss, int cond_dim,
+                                 int n_batch, int n_symm, float *__restrict__ out)
+{
+    const int j = blockIdx.x * blockDim.x + threadIdx.x, q = blockIdx.y, m = blockIdx.z, set = dset(m, n_symm);
+    if (j >= cond_dim) return;
+    const size_t mq = (size_t)m * n_batch + q;
+    const float *w0 = W0 + (size_t)set * N0 * ld0, *ws = Ws + (size_t)set * Ns * lds;
+    float s = 0.f, t = 0.f;
+    for (int n = 0; n < N0; ++n) s = fmaf(w0[(size_t)n * ld0 + 3 + j], S0[mq * N0 + n], s);
+    for (int n = 0; n < Ns; ++n) t = fmaf(ws[(size_t)n * lds + c0s + j], Ss[mq * Ns + n], t);
+    out[mq * cond_dim + j] = fmaf(t, chain::kInvSqrt2, s);
+}
+
+static int ready(nphm_ensemble *h, const char *who)
+{
+    NPHM_REQUIRE(h && h->loaded, "%s: weights not loaded", who);
+    const StackDims &s = h->dims;
+    if (s.N[s.n_lin - 1] != 1 || s.skip < 1 || s.skip >= s.n_lin - 1) {
+        set_error("%s: needs a one-output stack with its skip below the output layer", who);
+        return NPHM_ERR_UNSUPPORTED;
+    }
+    return NPHM_OK;
+}
+
+// d_{l-1} = s_{l-1} * (d_l W_l) (+ coupling) over all members, from the packed top (ks 1, member stride top_stride) down to
+// d_0 in D[0]; hook(l, d_l, ks_l, member stride of d_l) before each descent and at the bottom (the adjoint_walk of the
+// layer chain, batched).  xs: optional [members][M][4] skip-layer point gradient.
+template <class Hook>
+static int walk(nphm_ensemble *h, long long Mm, const uint8_t *top, long long top_stride, uint8_t *const *D, const long long *D_stride,
+                const float *const *S, const long long *S_stride, const float *const *cz, const uint8_t *const *ca,
+                const long long *ca_stride, float *xs, Hook &&hook, cudaStream_t stream)
+{
+    EnsembleChain &c = *h->sdfgrad;
+    const StackDims &s = h->dims;
+    const uint8_t *d = top;
+    long long ds = top_stride;
+    int dks = 1, rc;
+    for (int l = s.n_lin - 1; l >= 1; --l) {
+        if ((rc = hook(l, d, dks, ds))) return rc;
+        tcl::LinearParams p0;
+        p0.M = Mm; p0.batch = h->n_members; p0.w_pairs = h->cfg.n_symm_pairs;
+        p0.Ap = d; p0.a_ksteps = dks; p0.sAp = ds;
+        if (l == s.skip && xs) {
+            tcl::LinearParams px = p0;
+            px.mode = tcl::kModeLinear; px.C = xs; px.ldc = 4; px.sC = Mm * 4;
+            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+        }
+        const int ks = (s.N[l - 1] + 15) / 16;
+        tcl::LinearParams p = p0;
+        p.mode = tcl::kModeMult;
+        p.Mul = S[l - 1]; p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1; p.sMul = S_stride[l - 1] / 4;
+        if (cz) {
+            p.cpl_z = cz[l - 1]; p.sCplZ = S_stride[l - 1] / 4;
+            p.cpl_a = ca[l - 1]; p.sCplA = ca_stride[l - 1]; p.cpl_a_steps = ks; p.cpl_coef = chain::kBeta;
+        }
+        p.Cp = D[l - 1]; p.c_ksteps = ks; p.sCp = D_stride[l - 1];
+        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
+        d = D[l - 1]; ds = D_stride[l - 1]; dks = ks;
+    }
+    return hook(0, d, dks, ds);
+}
+
+// the point gradient (d_0 W_0[:, 0:3]^T + xs) * scale[sstride sigma + 1] of every member
+static int xyz_grad(nphm_ensemble *h, long long Mm, const uint8_t *d0, long long d0_stride, float *xa, const float *xs,
+                    const float *scale, int sstride, float *out, cudaStream_t stream)
+{
+    tcl::LinearParams p;
+    p.M = Mm; p.batch = h->n_members; p.w_pairs = h->cfg.n_symm_pairs;
+    p.Ap = d0; p.a_ksteps = (h->dims.N[0] + 15) / 16; p.sAp = d0_stride;
+    p.mode = tcl::kModeLinear; p.C = xa; p.ldc = 4; p.sC = Mm * 4;
+    int rc = tcl::launch_linear(h->sdfgrad->adj_x0, p, stream);
+    if (rc) return rc;
+    xyz_grad_kernel<<<(unsigned)ceil_div(h->n_members * Mm * 3, 256), 256, 0, stream>>>(xa, xs, Mm, h->n_members, scale, sstride,
+                                                                                        h->cfg.n_symm_pairs, out);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+}  // namespace esdf
+}  // namespace nphm
+
+extern "C" long long nphm_ensemble_sdfgrad_workspace_bytes(const nphm_ensemble *h, int n_batch, long long n_points)
+{
+    if (!h || !h->loaded || n_batch < 1 || n_points < 1) {
+        set_error("nphm_ensemble_sdfgrad_workspace_bytes: bad arguments");
+        return -1;
+    }
+    return (long long)esdf::layout(h, n_batch, n_points).total;
+}
+
+extern "C" int nphm_ensemble_sdfgrad_forward(nphm_ensemble *h, const float *xyz_local_dev, const float *cond_dev, int n_batch,
+                                             long long n_points, float *sdf_out_dev, float *grad_out_dev, void *workspace_dev,
+                                             void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = esdf::ready(h, "nphm_ensemble_sdfgrad_forward");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_batch >= 1 && n_points >= 1 && xyz_local_dev && cond_dev && sdf_out_dev && grad_out_dev && workspace_dev,
+                 "nphm_ensemble_sdfgrad_forward: bad arguments");
+    if ((rc = esdf::pack(h, stream))) return rc;
+    EnsembleChain &c = *h->sdfgrad;
+    const StackDims &s = h->dims;
+    const esdf::Layout G = esdf::layout(h, n_batch, n_points);
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const int K = h->n_members, n_symm = h->cfg.n_symm_pairs;
+    const long long Mm = (long long)n_batch * n_points, T = ceil_div(Mm, 128);
+    float *cvec = reinterpret_cast<float *>(ws + G.cvec), *consts = reinterpret_cast<float *>(ws + G.consts);
+    esdf::cvec_kernel<<<dim3((unsigned)K, (unsigned)n_batch), 256, 0, stream>>>(h->spec, cond_dev, n_batch, cvec);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(ws + G.cond, cond_dev, (size_t)K * n_batch * s.cond_dim * sizeof(float), cudaMemcpyDeviceToDevice,
+                                    stream));
+    esdf::pack_rows_kernel<<<dim3((unsigned)ceil_div(T * 128 * 2, 256), (unsigned)K), 256, 0, stream>>>(
+        xyz_local_dev, 3, 3, Mm, Mm * 3, nullptr, n_symm, ws + G.x0p, G.m_one);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    // value pass: h_l packed, S_l blocked; the output layer writes s row-major
+    for (int l = 0; l < s.n_lin; ++l) {
+        const tcl::PackedLinear &W = c.fwd[l];
+        tcl::LinearParams p;
+        p.M = Mm; p.batch = K; p.w_pairs = n_symm;
+        if (l == 0) { p.A1 = xyz_local_dev; p.lda1 = 3; p.K1 = 3; p.sA1 = Mm * 3; }
+        else { p.Ap = ws + G.hp[l - 1]; p.a_ksteps = W.ksteps; p.sAp = G.m_hp[l - 1]; }
+        p.bias = cvec + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = n_points; p.sBias = (long long)n_batch * s.cvec_stride;
+        if (l == s.n_lin - 1) {
+            p.mode = tcl::kModeLinear;
+            p.C = sdf_out_dev; p.ldc = 1; p.sC = Mm;
+        } else {
+            p.mode = tcl::kModeSoftplus;
+            p.Cp = ws + G.hp[l]; p.c_ksteps = G.ks_h[l]; p.sCp = G.m_hp[l];
+            if (l + 1 == s.skip) { p.app = xyz_local_dev; p.app_ld = 3; p.app_w = 3; p.sApp = Mm * 3; }
+            p.Dv = reinterpret_cast<float *>(ws + G.s[l]); p.lddv = c.ld[l]; p.dv_blocked = 1; p.sDv = G.m_s[l] / 4;
+        }
+        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
+    }
+    esdf::unit_column_kernel<<<dim3((unsigned)ceil_div(T * 128, 256), (unsigned)K), 256, 0, stream>>>(Mm, ws + G.unit, G.m_one, consts);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    // a_{l-1} = S_{l-1} * (a_l W_l) from the unit column down to a_0
+    uint8_t *A[kMaxLayers];
+    const float *S[kMaxLayers];
+    for (int l = 0; l + 1 < s.n_lin; ++l) { A[l] = ws + G.a[l]; S[l] = reinterpret_cast<const float *>(ws + G.s[l]); }
+    float *xa = reinterpret_cast<float *>(ws + G.xa), *xb = reinterpret_cast<float *>(ws + G.xb);
+    auto none = [](int, const uint8_t *, int, long long) { return NPHM_OK; };
+    if ((rc = esdf::walk(h, Mm, ws + G.unit, G.m_one, A, G.m_a, S, G.m_s, nullptr, nullptr, nullptr, xb, none, stream))) return rc;
+    return esdf::xyz_grad(h, Mm, A[0], G.m_a[0], xa, xb, consts, 0, grad_out_dev, stream);
+}
+
+extern "C" int nphm_ensemble_sdfgrad_backward(nphm_ensemble *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
+                                              long long workspace_bytes, int n_batch, long long n_points, float *const *grad_w_dev,
+                                              float *const *grad_b_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = esdf::ready(h, "nphm_ensemble_sdfgrad_backward");
+    if (rc) return rc;
+    NPHM_REQUIRE(n_batch >= 1 && n_points >= 1 && grad_sdf_dev && grad_grad_dev && workspace_dev,
+                 "nphm_ensemble_sdfgrad_backward: bad arguments");
+    NPHM_REQUIRE(h->sdfgrad && h->sdfgrad->packed, "nphm_ensemble_sdfgrad_backward: no forward since the last weight load");
+    // the caller states the shape the workspace was made for; checked against its size, without reading it back
+    NPHM_REQUIRE(workspace_bytes == (long long)esdf::layout(h, n_batch, n_points).total,
+                 "nphm_ensemble_sdfgrad_backward: a workspace of %lld bytes does not hold an SDF-gradient forward of this ensemble "
+                 "at %d x %lld points", workspace_bytes, n_batch, n_points);
+    EnsembleChain &c = *h->sdfgrad;
+    const StackDims &s = h->dims;
+    const esdf::Layout G = esdf::layout(h, n_batch, n_points);
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const int K = h->n_members, n_symm = h->cfg.n_symm_pairs, n_sets = h->n_sets, last = s.n_lin - 1;
+    const long long Mm = (long long)n_batch * n_points, T = ceil_div(Mm, 128);
+    float *gs = reinterpret_cast<float *>(ws + G.gs);
+    const float *cond = reinterpret_cast<const float *>(ws + G.cond);
+    float *v4 = reinterpret_cast<float *>(ws + G.v4);
+    float *xa = reinterpret_cast<float *>(ws + G.xa), *xb = reinterpret_cast<float *>(ws + G.xb);
+
+    // one power of two per weight set; zb_L = s_bar packed, the direction as rows and packed
+    esdf::set_scale_kernel<<<n_sets, 1024, 0, stream>>>(grad_sdf_dev, grad_grad_dev, Mm, n_symm, gs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    const dim3 pack_grid((unsigned)ceil_div(T * 128 * 2, 256), (unsigned)K);
+    esdf::pack_rows_kernel<<<pack_grid, 256, 0, stream>>>(grad_sdf_dev, 1, 1, Mm, Mm, gs, n_symm, ws + G.dl, G.m_one);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    esdf::direction_kernel<<<(unsigned)ceil_div(K * Mm * 4, 256), 256, 0, stream>>>(grad_grad_dev, Mm, K, gs, n_symm, v4);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    esdf::pack_rows_kernel<<<pack_grid, 256, 0, stream>>>(v4, 4, 3, Mm, Mm * 4, nullptr, n_symm, ws + G.vp, G.m_one);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+
+    // tangent pass: ht_l packed (tg), zt_l blocked fp32 (zg)
+    for (int l = 0; l < last; ++l) {
+        const tcl::PackedLinear &W = c.fwd[l];
+        tcl::LinearParams p;
+        p.M = Mm; p.batch = K; p.w_pairs = n_symm;
+        if (l == 0) { p.A1 = v4; p.lda1 = 4; p.K1 = 3; p.sA1 = Mm * 4; }
+        else { p.Ap = ws + G.tg[l - 1]; p.a_ksteps = W.ksteps; p.sAp = G.m_hp[l - 1]; }
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + G.s[l]); p.ldmul = c.ld[l]; p.mul_div = 1; p.mul_blocked = 1; p.sMul = G.m_s[l] / 4;
+        p.Cp = ws + G.tg[l]; p.c_ksteps = G.ks_h[l]; p.sCp = G.m_hp[l];
+        if (l + 1 == s.skip) { p.app = v4; p.app_ld = 4; p.app_w = 3; p.sApp = Mm * 4; }
+        p.Dv = reinterpret_cast<float *>(ws + G.zg[l]); p.lddv = c.ld[l]; p.dv_blocked = 1; p.sDv = G.m_s[l] / 4;
+        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
+    }
+
+    int max_n = 1;
+    for (int l = 0; l <= last; ++l) max_n = std::max(max_n, s.N[l]);
+    const size_t mq = (size_t)K * n_batch;
+    if ((rc = c.sums.reserve(mq * max_n * sizeof(float))) || (rc = c.sums0.reserve(mq * s.N[0] * sizeof(float))) ||
+        (rc = c.sumss.reserve(mq * s.N[s.skip] * sizeof(float))))
+        return rc;
+    // dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1} per weight set (a_L: the unit column, ht_{-1}: the direction), db_l, and the
+    // condition columns of layers 0 and skip from the per-(member, query) sums of zb_l
+    auto layer_grads = [&](int l, const uint8_t *d, int ks, long long ds) {
+        float *gw = grad_w_dev ? grad_w_dev[l] : nullptr, *gb = grad_b_dev ? grad_b_dev[l] : nullptr;
+        const bool cond_layer = l == 0 || l == s.skip;
+        const float sc = l == s.skip ? chain::kInvSqrt2 : 1.0f;
+        const long long wstride = (long long)s.N[l] * s.in_total[l];
+        if (gw) {
+            const uint8_t *H = l == 0 ? ws + G.x0p : ws + G.hp[l - 1], *H2 = l == 0 ? ws + G.vp : ws + G.tg[l - 1];
+            const long long sH = l == 0 ? G.m_one : G.m_hp[l - 1];
+            const int hks = l == 0 ? 1 : G.ks_h[l - 1];
+            const int Kc = l == 0 ? 3 : l == s.skip ? s.N[l - 1] + 3 : s.N[l - 1];
+            const uint8_t *D2 = l == last ? ws + G.unit : ws + G.a[l];
+            const long long sD2 = l == last ? G.m_one : G.m_a[l];
+            int r = wgrad::launch_sets(d, ks, H, hks, Mm, s.N[l], Kc, sc, gs + 1, 2, gw, s.in_total[l], wstride, n_sets, n_symm, ds,
+                                       sH, sD2, sH, c.partials, stream, D2, H2);
+            if (r) return r;
+        }
+        float *sums = l == 0 ? c.sums0.as<float>() : l == s.skip ? c.sumss.as<float>() : c.sums.as<float>();
+        if (gb || (cond_layer && (gw || grad_cond_dev))) {
+            esdf::query_sums_kernel<<<dim3((unsigned)ks, (unsigned)n_batch, (unsigned)K), 256, 0, stream>>>(
+                d, ks, ds, n_points, n_batch, s.N[l], gs, n_symm, sums);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+        if (gb) {
+            esdf::bias_grad_kernel<<<dim3((unsigned)ceil_div(s.N[l], 128), (unsigned)n_sets), 128, 0, stream>>>(sums, n_batch, s.N[l],
+                                                                                                              n_symm, gb);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+        if (cond_layer && gw) {
+            const long long total = (long long)s.N[l] * s.cond_dim;
+            esdf::cond_outer_kernel<<<dim3((unsigned)ceil_div(total, 256), (unsigned)n_sets), 256, 0, stream>>>(
+                sums, cond, n_batch, s.N[l], s.cond_dim, n_symm, sc, gw, s.in_total[l], wstride, l == 0 ? 3 : s.N[l - 1] + 3);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+        return NPHM_OK;
+    };
+    // value adjoint with the coupling, from zb_L = s_bar (dl) down to zb_0; zb_l lives in dp[l & 1]
+    uint8_t *D[kMaxLayers];
+    const float *S[kMaxLayers], *Z[kMaxLayers];
+    const uint8_t *A[kMaxLayers];
+    long long D_stride[kMaxLayers];
+    for (int l = 0; l < last; ++l) {
+        D[l] = ws + G.dp[l & 1]; D_stride[l] = G.m_dp;
+        S[l] = reinterpret_cast<const float *>(ws + G.s[l]);
+        Z[l] = reinterpret_cast<const float *>(ws + G.zg[l]);
+        A[l] = ws + G.a[l];
+    }
+    if ((rc = esdf::walk(h, Mm, ws + G.dl, G.m_one, D, D_stride, S, G.m_s, Z, A, G.m_a, grad_xyz_dev ? xb : nullptr, layer_grads,
+                         stream)))
+        return rc;
+    if (grad_cond_dev) {
+        esdf::cond_grad_kernel<<<dim3((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_batch, (unsigned)K), 128, 0, stream>>>(
+            h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.sums0.as<float>(), h->weights.W[s.skip].as<float>(),
+            s.in_total[s.skip], s.N[s.skip], s.N[s.skip - 1] + 3, c.sumss.as<float>(), s.cond_dim, n_batch, n_symm, grad_cond_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    // s_bar g + H v per member
+    if (grad_xyz_dev && (rc = esdf::xyz_grad(h, Mm, D[0], D_stride[0], xa, xb, gs, 2, grad_xyz_dev, stream))) return rc;
+    return NPHM_OK;
+}

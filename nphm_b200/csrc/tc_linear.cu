@@ -283,7 +283,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
         // ---------------- epilogue: thread = row, 16 accumulator columns at a time (units of this warp's parity)
         TCL_EVT(threadIdx.x == 0, 9, 1);
         const float *drow = dtile + (size_t)t * dp;
-        const float *bias = p.bias ? p.bias + (size_t)(row_ok ? row / p.rows_per_bias : 0) * p.ldb : nullptr;
+        const float *bias = p.bias ? p.bias + (size_t)z * p.sBias + (size_t)(row_ok ? row / p.rows_per_bias : 0) * p.ldb : nullptr;
         const bool mul_blk = p.blocked || p.mul_blocked;
         const long long mrow = row_ok ? row / p.mul_div : 0;                     // multiplier row (tangent passes: 3 rows per point)
         const float *mul = !p.Mul ? nullptr
@@ -293,14 +293,14 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
         float *const Cz = p.C ? p.C + (size_t)z * p.sC : nullptr;
         uint8_t *const cp = PACKED_C ? p.Cp + (size_t)z * p.sCp + (size_t)blockIdx.x * p.c_tile_steps * kPackedStep +
                                        (size_t)(t >> 3) * 256 + (size_t)(t & 7) * 16 : nullptr;
-        const float *app = (p.app && row_ok) ? p.app + (size_t)row * p.app_ld : nullptr;       // appended input columns (skip connection)
+        const float *app = (p.app && row_ok) ? p.app + (size_t)z * p.sApp + (size_t)row * p.app_ld : nullptr;       // appended input columns (skip connection)
         const int app_hot = p.app_onehot ? (int)(row % p.app_w) : -1;
         const bool aux_blk = MODE == kModeMult ? mul_blk : false;
         const float *aux_src = MODE == kModeMult ? mul : bias;        // bias (LINEAR / SOFTPLUS) or multiplier (MULT)
         const int aux_ld = MODE == kModeMult ? p.ldmul : p.ldb;
         const bool aux_vec = aux_src && (aux_ld % 4 == 0) && ((n0 & 3) == 0) && ((reinterpret_cast<uintptr_t>(aux_src) & 15) == 0);
         const bool c_vec = (p.ldc % 4 == 0) && ((n0 & 3) == 0) && ((reinterpret_cast<uintptr_t>(Cz) & 15) == 0);
-        const bool d_vec = p.Dv && (p.lddv % 4 == 0) && ((n0 & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.Dv) & 15) == 0);
+        const bool d_vec = p.Dv && (p.lddv % 4 == 0) && (p.sDv % 4 == 0) && ((n0 & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.Dv) & 15) == 0);
         // FULL: all 16 columns of the unit exist (no per-column guards, constant address offsets)
         auto finish_unit = [&](int c0, auto full_c) {
             constexpr bool FULL = decltype(full_c)::value;
@@ -335,8 +335,8 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
             float cpl[16];
             const bool coupled = MODE == kModeMult && p.cpl_z && ((n0 + c0) >> 4) < p.cpl_a_steps;
             if (coupled) {
-                const float *zb = p.cpl_z + (size_t)blockIdx.x * p.ldmul * 128 + (size_t)(n0 + c0) * 128 + t;
-                const uint8_t *ab = p.cpl_a + ((size_t)blockIdx.x * p.cpl_a_steps + ((n0 + c0) >> 4)) * kPackedStep +
+                const float *zb = p.cpl_z + (size_t)z * p.sCplZ + (size_t)blockIdx.x * p.ldmul * 128 + (size_t)(n0 + c0) * 128 + t;
+                const uint8_t *ab = p.cpl_a + (size_t)z * p.sCplA + ((size_t)blockIdx.x * p.cpl_a_steps + ((n0 + c0) >> 4)) * kPackedStep +
                                     (size_t)(t >> 3) * 256 + (size_t)(t & 7) * 16;
                 const uint4 h0 = *reinterpret_cast<const uint4 *>(ab), h1 = *reinterpret_cast<const uint4 *>(ab + 128);
                 const uint4 l0 = *reinterpret_cast<const uint4 *>(ab + 4096), l1 = *reinterpret_cast<const uint4 *>(ab + 4096 + 128);
@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
             }
             TCL_EVT(threadIdx.x == 0, 14, c0 >> 4);
             if (p.Dv && (p.blocked || p.dv_blocked)) {
-                float *db = p.Dv + (size_t)blockIdx.x * p.lddv * 128 + (size_t)(n0 + c0) * 128 + t;
+                float *db = p.Dv + (size_t)z * p.sDv + (size_t)blockIdx.x * p.lddv * 128 + (size_t)(n0 + c0) * 128 + t;
 #pragma unroll
                 for (int e = 0; e < 16; ++e)
                     if (FULL || n0 + c0 + e < p.N) db[e * 128] = dv[e];
@@ -432,7 +432,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
                     if (FULL || n0 + c0 + e < p.N) crow[e] = o[e];
             }
             if (p.Dv && !p.dv_blocked) {
-                float *dvrow = p.Dv + (size_t)row * p.lddv + n0 + c0;
+                float *dvrow = p.Dv + (size_t)z * p.sDv + (size_t)row * p.lddv + n0 + c0;
                 if (FULL && d_vec) {
 #pragma unroll
                     for (int i = 0; i < 4; ++i)
@@ -522,13 +522,12 @@ int launch_linear(const PackedLinear &w, LinearParams p, cudaStream_t stream)
                  "tc_linear: packed output misconfigured");
     NPHM_REQUIRE(p.app_w == 0 || p.Cp, "tc_linear: appended columns need a packed output");
     NPHM_REQUIRE(p.mode != kModeMult || (p.Mul && p.mul_div > 0), "tc_linear: multiplier missing");
-    NPHM_REQUIRE(!p.cpl_z || (p.mode == kModeMult && p.cpl_a && p.cpl_a_steps > 0 && (p.blocked || p.mul_blocked) && p.mul_div <= 1 &&
-                              p.batch == 1),
+    NPHM_REQUIRE(!p.cpl_z || (p.mode == kModeMult && p.cpl_a && p.cpl_a_steps > 0 && (p.blocked || p.mul_blocked) && p.mul_div <= 1),
                  "tc_linear: the coupling term needs the multiplier epilogue with a blocked multiplier, one row per multiplier row");
     NPHM_REQUIRE(!p.blocked || (!p.bias && !p.A2 && !p.a2_onehot && p.mul_div <= 1),
                  "tc_linear: the blocked layout supports the plain and the multiplier epilogue only");
-    NPHM_REQUIRE(p.batch >= 1 && (p.batch == 1 || (!p.Dv && !p.bias && !p.A2 && !p.a2_onehot && !p.app)),
-                 "tc_linear: batched launches support the plain and the multiplier epilogue only");
+    NPHM_REQUIRE(p.batch >= 1 && (p.batch == 1 || (!p.A2 && !p.a2_onehot && !p.app_onehot)),
+                 "tc_linear: batched launches take no second or one-hot input");
     if (p.batch > 1) {
         const int last = p.batch - 1, need = (last < 2 * p.w_pairs ? (last >> 1) : last - p.w_pairs) + 1;
         NPHM_REQUIRE(need <= w.sets, "tc_linear: batch of %d needs %d weight sets, %d packed", p.batch, need, w.sets);

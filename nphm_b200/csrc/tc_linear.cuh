@@ -38,6 +38,8 @@ struct LinearParams {
     // batched launch (gridDim.z): entry z reads A1 + z sA1, Mul + z sMul, row_scale + z sRow, writes C + z sC (strides in floats)
     // and uses weight set z/2 for z < 2 w_pairs, z - w_pairs beyond (the mirrored pairs of the ensemble share weights)
     int batch = 1; long long sA1 = 0, sC = 0, sMul = 0, sRow = 0; int w_pairs = 0;
+    // and (strides in floats / bytes) bias + z sBias, Dv + z sDv, app + z sApp, cpl_z + z sCplZ, cpl_a + z sCplA
+    long long sBias = 0, sDv = 0, sApp = 0, sCplZ = 0, sCplA = 0;
     const int *live = nullptr;                               // optional device counter: the launch does nothing when *live == 0
     // filled by launch_linear from the packed weights
     const uint8_t *W = nullptr; long long w_stride = 0; int N = 0, Nt = 0, ksteps = 0, stages = 0;

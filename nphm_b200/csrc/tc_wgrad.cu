@@ -47,25 +47,35 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
 
 // partial[split][n][k] (ld kb_count * 64) of output tile (blockIdx.x / kb_count, blockIdx.x % kb_count) over row tiles
 // [split * tiles_per_split, ...) of the row_tiles tiles of (D, H) followed, with D2 given, by the row_tiles tiles of (D2, H2)
+// Set-batched (gridDim.z = weight set, Members): set z reduces over the row tiles of its members m0 (and m0 + 1 for the
+// w_pairs mirrored pairs), member after member, each with its pairs in the order above; member m's operands start at
+// D + m sD (bytes), and so on.  One set (gridDim.z = 1, w_pairs = 0): member 0, the plain launch.
+struct Members { int w_pairs; long long sD, sH, sD2, sH2; };
+
 __global__ void __launch_bounds__(kThreads) wgrad_kernel(const uint8_t *__restrict__ D, int ks_d, const uint8_t *__restrict__ H,
                                                          int ks_h, const uint8_t *__restrict__ D2, const uint8_t *__restrict__ H2,
                                                          long long M, int row_tiles, int tiles_per_split, int nb_count,
-                                                         int kb_count, float *__restrict__ partial)
+                                                         int kb_count, const Members mem, float *__restrict__ partial)
 {
     extern __shared__ __align__(128) uint8_t smem[];
-    const int nb = blockIdx.x / kb_count, kb = blockIdx.x % kb_count, split = blockIdx.y;
-    const int t0 = split * tiles_per_split, t1 = min(D2 ? 2 * row_tiles : row_tiles, t0 + tiles_per_split);
+    const int nb = blockIdx.x / kb_count, kb = blockIdx.x % kb_count, split = blockIdx.y, set = blockIdx.z;
+    const int m0 = set < mem.w_pairs ? 2 * set : set + mem.w_pairs, n_mem = set < mem.w_pairs ? 2 : 1;
+    const int per_mem = D2 ? 2 * row_tiles : row_tiles;
+    const int t0 = split * tiles_per_split, t1 = min(n_mem * per_mem, t0 + tiles_per_split);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wn = warp >> 1, wk = warp & 1;
 
     // one stage: 2 operands x 4 k-steps x 512 lines of 16 bytes; line -> row of the tile: ((line & 255) >> 4) * 8 + (line & 7)
     auto load = [&](int t, int s) {
         const uint32_t dst0 = smem_u32(smem + (size_t)s * kStageBytes);
+        const int m = m0 + t / per_mem;
+        t %= per_mem;
         const bool second = t >= row_tiles;
         if (second) t -= row_tiles;
+        const uint8_t *bd = second ? D2 + m * mem.sD2 : D + m * mem.sD, *bh = second ? H2 + m * mem.sH2 : H + m * mem.sH;
         for (int i = threadIdx.x; i < 2 * 4 * 512; i += kThreads) {
             const int op = i >> 11, u = (i >> 9) & 3, line = i & 511;
-            const uint8_t *base = op ? (second ? H2 : H) : (second ? D2 : D);
+            const uint8_t *base = op ? bh : bd;
             const int ks = op ? ks_h : ks_d, j = (op ? kb : nb) * 4 + u;
             const int r = ((line & 255) >> 4) * 8 + (line & 7);
             const bool ok = j < ks && (long long)t * 128 + r < M;
@@ -124,7 +134,7 @@ __global__ void __launch_bounds__(kThreads) wgrad_kernel(const uint8_t *__restri
         __syncthreads();                           // stage s is refilled at the next iteration
     }
     const int ldk = kb_count * kTile;
-    float *out = partial + (size_t)split * nb_count * kTile * ldk;
+    float *out = partial + ((size_t)set * gridDim.y + split) * nb_count * kTile * ldk;
 #pragma unroll
     for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
@@ -136,32 +146,37 @@ __global__ void __launch_bounds__(kThreads) wgrad_kernel(const uint8_t *__restri
         }
 }
 
-// dW[n][k] = scale * inv_scale * sum over the splits, in split order
+// dW[n][k] = scale * inv_scale * sum over the splits, in split order; set z = blockIdx.y: partials, dW + z dw_stride,
+// inv_scale + z inv_stride
 __global__ void wgrad_finish_kernel(const float *__restrict__ partial, int splits, int ldn, int ldk, int N, int K, float scale,
-                                    const float *__restrict__ inv_scale, float *__restrict__ dW, int ldw)
+                                    const float *__restrict__ inv_scale, int inv_stride, float *__restrict__ dW, int ldw,
+                                    long long dw_stride)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)N * K) return;
-    const int n = (int)(idx / K), k = (int)(idx % K);
+    const int n = (int)(idx / K), k = (int)(idx % K), set = blockIdx.y;
+    const float *part = partial + (size_t)set * splits * ldn * ldk;
     float s = 0.f;
-    for (int i = 0; i < splits; ++i) s += partial[((size_t)i * ldn + n) * ldk + k];
-    dW[(size_t)n * ldw + k] = s * (scale * inv_scale[0]);
+    for (int i = 0; i < splits; ++i) s += part[((size_t)i * ldn + n) * ldk + k];
+    dW[(size_t)set * dw_stride + (size_t)n * ldw + k] = s * (scale * inv_scale[(size_t)set * inv_stride]);
 }
 
-int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
-           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream, const uint8_t *D2,
-           const uint8_t *H2)
+int launch_sets(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
+                const float *inv_scale_dev, int inv_stride, float *dW, int ldw, long long dw_stride, int sets, int w_pairs,
+                long long sD, long long sH, long long sD2, long long sH2, DeviceBuffer &partials, cudaStream_t stream,
+                const uint8_t *D2, const uint8_t *H2)
 {
-    NPHM_REQUIRE(M > 0 && N <= d_ksteps * 16 && K <= h_ksteps * 16 && !D2 == !H2, "wgrad: bad operand shapes");
+    NPHM_REQUIRE(M > 0 && N <= d_ksteps * 16 && K <= h_ksteps * 16 && !D2 == !H2 && sets >= 1 && w_pairs >= 0 && w_pairs <= sets,
+                 "wgrad: bad operand shapes");
     const int nb_count = (d_ksteps + 3) / 4, kb_count = (h_ksteps + 3) / 4;
-    const int row_tiles = (int)ceil_div(M, 128), all_tiles = D2 ? 2 * row_tiles : row_tiles;
+    const int row_tiles = (int)ceil_div(M, 128), all_tiles = (w_pairs ? 2 : 1) * (D2 ? 2 * row_tiles : row_tiles);
     const int tiles = nb_count * kb_count;
-    int splits = std::max(1, std::min(all_tiles, (int)ceil_div(2LL * sm_count(), tiles)));
+    int splits = std::max(1, std::min(all_tiles, (int)ceil_div(2LL * sm_count(), (long long)tiles * sets)));
     const int tiles_per_split = (int)ceil_div(all_tiles, splits);
     splits = (int)ceil_div(all_tiles, tiles_per_split);
     const int ldn = nb_count * kTile, ldk = kb_count * kTile;
     int rc;
-    if ((rc = partials.reserve((size_t)splits * ldn * ldk * sizeof(float)))) return rc;
+    if ((rc = partials.reserve((size_t)sets * splits * ldn * ldk * sizeof(float)))) return rc;
     static bool smem_set[64] = {};                 // the attribute is per device: set once on each
     int dev = 0;
     NPHM_CUDA_CHECK(cudaGetDevice(&dev));
@@ -169,14 +184,24 @@ int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long 
         NPHM_CUDA_CHECK(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
         if (dev < 64) smem_set[dev] = true;
     }
-    wgrad_kernel<<<dim3(tiles, splits), kThreads, kSmem, stream>>>(D, d_ksteps, H, h_ksteps, D2, H2, M, row_tiles, tiles_per_split,
-                                                                   nb_count, kb_count, partials.as<float>());
+    const Members mem{w_pairs, sD, sH, sD2, sH2};
+    wgrad_kernel<<<dim3(tiles, splits, sets), kThreads, kSmem, stream>>>(D, d_ksteps, H, h_ksteps, D2, H2, M, row_tiles,
+                                                                         tiles_per_split, nb_count, kb_count, mem,
+                                                                         partials.as<float>());
     NPHM_CUDA_CHECK(cudaGetLastError());
     const long long total = (long long)N * K;
-    wgrad_finish_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(partials.as<float>(), splits, ldn, ldk, N, K, scale,
-                                                                            inv_scale_dev, dW, ldw);
+    wgrad_finish_kernel<<<dim3((unsigned)ceil_div(total, 256), sets), 256, 0, stream>>>(
+        partials.as<float>(), splits, ldn, ldk, N, K, scale, inv_scale_dev, inv_stride, dW, ldw, dw_stride);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
+}
+
+int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
+           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream, const uint8_t *D2,
+           const uint8_t *H2)
+{
+    return launch_sets(D, d_ksteps, H, h_ksteps, M, N, K, scale, inv_scale_dev, 0, dW, ldw, 0, 1, 0, 0, 0, 0, 0, partials, stream,
+                       D2, H2);
 }
 
 }  // namespace wgrad

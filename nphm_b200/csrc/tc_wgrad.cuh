@@ -15,5 +15,13 @@ int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long 
            const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream,
            const uint8_t *D2 = nullptr, const uint8_t *H2 = nullptr);
 
+// Set-batched: `sets` weight sets in one launch (gridDim.z).  Set z sums over the rows of its members, z < w_pairs: 2z and
+// 2z + 1, else z + w_pairs, in one fixed order (member by member, both pairs of each); member m's operands start at
+// D + m sD, H + m sH, D2 + m sD2, H2 + m sH2 (bytes).  Writes dW + z dw_stride with the factor inv_scale_dev[z inv_stride].
+int launch_sets(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
+                const float *inv_scale_dev, int inv_stride, float *dW, int ldw, long long dw_stride, int sets, int w_pairs,
+                long long sD, long long sH, long long sD2, long long sH2, DeviceBuffer &partials, cudaStream_t stream,
+                const uint8_t *D2 = nullptr, const uint8_t *H2 = nullptr);
+
 }  // namespace wgrad
 }  // namespace nphm

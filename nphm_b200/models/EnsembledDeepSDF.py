@@ -28,6 +28,32 @@ from .. import _native
 from . import _composite
 
 
+class _NativeEnsembleSdfGradFn(torch.autograd.Function):
+    """The members of ``FastEnsembleDeepSDFMirrored`` on the native kernels (``nphm_ensemble_sdfgrad_forward`` /
+    ``_backward``): xyz_local members x B x N x 3 (each member's frame, mirror applied), cond members x B x (G + L), then the
+    ``ensembled_deep_sdf.lin{l}.weight / bias`` parameters -> (s members x B x N, grad_local s members x B x N x 3).  The
+    backward takes upstream gradients of both outputs; differentiable to first order only."""
+
+    @staticmethod
+    def forward(ctx, engine, xyz_local, cond, *params):
+        s, g, ws = engine.sdfgrad_forward(xyz_local, cond)
+        ctx.engine = engine
+        ctx.layer_shapes = [tuple(p.shape) for p in params[0::2]]
+        ctx.save_for_backward(ws, *params)
+        return s, g
+
+    @staticmethod
+    def backward(ctx, grad_s, grad_g):
+        if torch.is_grad_enabled():
+            raise RuntimeError('forward_with_gradient_native is differentiable to first order only: a double backward '
+                               '(create_graph=True) through it is not supported; use the composite forward() instead')
+        from .deepSDF import _native_backward
+
+        def engine_backward(ws, gs, gg, **kw):
+            return ctx.engine.sdfgrad_backward(ws, gs, gg, ctx.layer_shapes, **kw)
+        return _native_backward(ctx, engine_backward, 3, grad_s, grad_g)
+
+
 def _member_to_set(ensemble_size: int, n_symm: int) -> torch.Tensor:
     """member k -> weight-set index (reference :43-45): pairs (2i,2i+1), i<n_symm share set i."""
     k = torch.arange(ensemble_size)
@@ -165,6 +191,48 @@ class FastEnsembleDeepSDFMirrored(nn.Module):
         if not _native.stack_supported(n_lin - 1, _native.hidden_width(e, n_lin), self.lat_dim_glob + self.lat_dim_loc):
             return False             # depth / width the native stack builder rejects: composite path
         return (xyz.dtype == torch.float32 and self.out_dim == 1 and self.input_dim == 3)
+
+    def _sdfgrad_unsupported(self, xyz: torch.Tensor, lat_rep: torch.Tensor) -> Optional[str]:
+        if not (xyz.is_cuda and lat_rep.is_cuda):
+            return 'needs CUDA points and codes'
+        if xyz.dtype != torch.float32 or any(p.dtype != torch.float32 for p in self.parameters()):
+            return 'needs fp32 points and parameters'
+        if not self.training:
+            return 'needs training mode (the eval-mode quirk stays on the composite path)'
+        e = self.ensembled_deep_sdf
+        n_lin = e.num_layers - 1
+        if not (self.out_dim == 1 and self.input_dim == 3 and
+                _native.stack_supported(n_lin - 1, _native.hidden_width(e, n_lin), self.lat_dim_glob + self.lat_dim_loc)):
+            return 'needs a one-output member stack the native builder accepts'
+        if xyz.dim() != 3 or xyz.shape[-1] != 3 or lat_rep.dim() != 3 or lat_rep.shape[-1] != self.lat_dim:
+            return 'needs B x N x 3 points and B x 1 x lat_dim codes'
+        if lat_rep.shape[1] != 1 and lat_rep.stride(1) != 0:
+            return 'needs one code per batch element (B x 1 x lat_dim)'
+        return None
+
+    def sdfgrad_supported(self, xyz: torch.Tensor, lat_rep: torch.Tensor) -> bool:
+        """Whether :meth:`forward_with_gradient_native` takes these inputs."""
+        return self._sdfgrad_unsupported(xyz, lat_rep) is None
+
+    def forward_with_gradient_native(self, xyz: torch.Tensor, lat_rep: torch.Tensor):
+        """``(sdf B x N x 1, d sdf / d xyz B x N x 3, anchors B x n_loc x 3)``: the training-mode forward followed by
+        ``gradient(sdf, xyz)``, with the members' values, gradients and second-order backward on the native kernels (one
+        launch per pass for all members) and the anchors, frames and Gaussian blend in autograd
+        (``_composite.ensemble_blend_with_gradient``).  Differentiable to first order in the parameters and ``lat_rep``; the
+        points get no gradient.  Raises ``ValueError`` naming what it does not support."""
+        reason = self._sdfgrad_unsupported(xyz, lat_rep)
+        if reason is not None:
+            raise ValueError('forward_with_gradient_native: ' + reason)
+        lat = lat_rep[:, :1]
+        anchors, local, cond = _composite.member_frames(self, xyz.detach(), lat)
+        e = self.ensembled_deep_sdf
+        params = []
+        for i in range(e.num_layers - 1):
+            lin = getattr(e, 'lin%d' % i)
+            params += [lin.weight, lin.bias]
+        s, g = _NativeEnsembleSdfGradFn.apply(self.engine(), local, cond[:, :, 0], *params)
+        sdf, grad = _composite.ensemble_blend_with_gradient(self, xyz.detach(), anchors, s, g)
+        return sdf, grad, anchors
 
     def engine(self) -> "_native.EnsembleEngine":
         """Native handle holding the packed weights; rebuilt when parameters change."""

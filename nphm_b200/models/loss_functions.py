@@ -19,7 +19,10 @@ ensemble - ``anchors``, ``symm_dist``, ``middle_dist``).  Two ways to get the SD
 With ``native=True`` and a ``DeepSDF`` decoder (the NPM baseline) the loss takes a third way, with or without autograd:
 ``DeepSDF.forward_with_gradient_native`` evaluates the four point sets in one call (concatenated along the points of each
 query) and differentiates the SDF and its spatial gradient natively, second-order terms included.  ``native=None`` keeps the
-composite path for it.
+composite path for it.  With ``native=True``, the ensemble in training mode on CUDA and autograd recording, the ensemble takes
+the same way: ``FastEnsembleDeepSDFMirrored.forward_with_gradient_native`` runs the members' passes natively (one launch per
+pass for all members) and the anchors and blend in autograd.  Under ``torch.no_grad()`` ``native=True`` keeps the evaluation
+path above.
 
 ``compute_loss_corresp_forward`` is first order (no gradient with respect to the points is used), so its decoder calls run
 natively to the weights: ``DeformationNetwork.forward_native_grad`` (forward and backward on the tensor cores, the compressor
@@ -85,17 +88,31 @@ def _sdfgrad_native(decoder, batch_cuda, glob_cond):
     return dict(zip(_POINT_SETS, sdf.split(sizes, dim=1))), dict(zip(_POINT_SETS, g.split(sizes, dim=1)))
 
 
+def _ensemble_sdfgrad_native(decoder, batch_cuda, glob_cond):
+    """The ensemble's ``forward_with_gradient_native`` on all four point sets in one call -> ({name: sdf},
+    {name: d sdf / d x}, anchors)."""
+    sets = [batch_cuda[name] for name in _POINT_SETS]
+    pts = torch.cat(sets, dim=1)
+    sdf, g, anchors = decoder.forward_with_gradient_native(pts, glob_cond)
+    sizes = [p.shape[1] for p in sets]
+    return dict(zip(_POINT_SETS, sdf.split(sizes, dim=1))), dict(zip(_POINT_SETS, g.split(sizes, dim=1))), anchors
+
+
 def actual_compute_loss(batch_cuda, decoder, glob_cond, native=None):
     is_ensemble = isinstance(decoder, FastEnsembleDeepSDFMirrored)
     anchor_preds = batch_cuda['gt_anchors'] if hasattr(decoder, 'anchors') else None
     sdfgrad = native is not None and bool(native) and isinstance(decoder, DeepSDF)
+    explicit = native is not None and bool(native)
     if native is None:
         native = not torch.is_grad_enabled()
     native = bool(native) and is_ensemble and decoder.training and batch_cuda['points_face'].is_cuda
+    ensemble_sdfgrad = native and explicit and torch.is_grad_enabled()
 
     pred, grad, anchors = {}, {}, None
     if sdfgrad:
         pred, grad = _sdfgrad_native(decoder, batch_cuda, glob_cond)
+    elif ensemble_sdfgrad:
+        pred, grad, anchors = _ensemble_sdfgrad_native(decoder, batch_cuda, glob_cond)
     elif native:
         with torch.no_grad():
             for name in _POINT_SETS:

@@ -22,14 +22,27 @@ init), 32 samples x (750 face + 50 non-face + 800 near + 93 far) points, the npm
 Native (forward_with_gradient_native: SDF, spatial gradient and their weight gradients on the tensor cores, one call per
 loss) and composite (PyTorch double backward) steps alternate; also reports the peak device memory of each path (torch's
 peak plus what the path holds outside torch's allocator) and, for the first step, the largest relative difference between
-the native and the composite gradients."""
-import argparse, json, os, subprocess, sys
+the native and the composite gradients.
+
+    python tools/bench_train.py --stage 1 --decoder nphm --steps 10 --warmup 2
+
+Stage 1 of the NPHM ensemble (train.py -local) at scripts/configs/nphm.yaml settings: FastEnsembleDeepSDFMirrored (39 local
++ 1 global member, 16 symmetric pairs, 99 -> 200 x 4 -> 1), the same 32 x (750 + 50 + 800 + 93) points with ground-truth
+anchors, the nphm.yaml lambdas, AdamW (lr 5e-4, weight decay 0.01) on the decoder, SparseAdam (lr_lat 1e-3) on
+Embedding(., 1344, max_norm 1, sparse) codes, clip_grad_norm_ 0.1 on both.  Native (forward_with_gradient_native: the
+members' passes on the tensor cores, one launch per pass for all 40 members, anchors and blend in autograd) and composite
+steps alternate, with peak memory and the first step's gradient difference as above.  If the batch does not fit, the line
+says so and both are measured at the largest halved batch that does.  --profile --stage 1 --decoder nphm: the kernel
+breakdown of native ensemble steps."""
+import argparse, gc, json, os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import torch
 
 LAMBDAS = {'corresp': 100.0, 'loss_reg_zero': 5.0e-05, 'lat_reg': 5.0e-05}          # nphm_def.yaml
 LAMBDAS_SHAPE = {'surf_sdf': 2.0, 'normals': 0.3, 'space_sdf': 0.01, 'grad': 0.1, 'lat_reg': 0.002}   # npm.yaml
+LAMBDAS_NPHM = {'surf_sdf': 2.0, 'normals': 0.3, 'space_sdf': 0.01, 'grad': 0.1, 'lat_reg': 0.01, 'anchors': 7.5,
+                'symm_dist': 0.01, 'middle_dist': 0.0}                                                       # nphm.yaml
 SHAPE_SETS = (('points_face', 750), ('points_non_face', 50), ('sup_grad_near', 800), ('sup_grad_far', 93))
 
 def gpu_info():
@@ -115,9 +128,25 @@ def setup_shape(dev):
     return dec, codes, opt, opt_lat
 
 
-def batch_shape(B, dev, step):
+def setup_nphm(dev):
+    from conftest import make_ensemble
+    dec = make_ensemble(0, device=dev).train()
+    torch.manual_seed(0)
+    codes = torch.nn.Embedding(64, dec.lat_dim, max_norm=1.0, sparse=True).to(dev)
+    with torch.no_grad():
+        codes.weight.mul_(0.01)
+    opt = torch.optim.AdamW(dec.parameters(), lr=5e-4, weight_decay=0.01)
+    opt_lat = torch.optim.SparseAdam(codes.parameters(), lr=1e-3)
+    return dec, codes, opt, opt_lat
+
+
+def batch_shape(B, dev, step, anchors=False):
+    """Sphere-like point sets of SHAPE_SETS with unit normals; anchors: also ground-truth anchors near the mean ones."""
     g = torch.Generator().manual_seed(step)
     out = {'idx': torch.randint(0, 64, (B, 1), generator=g)}
+    if anchors:
+        from conftest import mean_anchors
+        out['gt_anchors'] = mean_anchors().reshape(1, 39, 3) + 0.01 * torch.randn(B, 39, 3, generator=g)
     for name, n in SHAPE_SETS:
         d = torch.randn(B, n, 3, generator=g)
         d = d / d.norm(dim=-1, keepdim=True)
@@ -131,7 +160,7 @@ def batch_shape(B, dev, step):
     return out
 
 
-def train_step_shape(state, b, native, ev, keep=None):
+def train_step_shape(state, b, native, ev, keep=None, lambdas=LAMBDAS_SHAPE):
     """One step; `keep` (a dict): receives copies of the gradients before clipping, taken between the timed phases."""
     from nphm_b200.models.loss_functions import compute_loss
     dec, codes, opt, opt_lat = state
@@ -140,7 +169,7 @@ def train_step_shape(state, b, native, ev, keep=None):
     opt_lat.zero_grad()
     losses = compute_loss(dict(b), dec, codes, 'cuda', native=native)
     tot = 0
-    for k, lam in LAMBDAS_SHAPE.items():
+    for k, lam in lambdas.items():
         tot = tot + lam * losses[k]
     ev[1].record()
     tot.backward()
@@ -214,11 +243,36 @@ def run_mode(mode, args, dev):
     return run(lambda: setup(mode, dev), lambda step: batch(32, 1000, dev, step), train_step, args)
 
 
-def profile_native(dev, stage=2, steps=5):
+def run_nphm(args, dev, name, power):
+    """Native and composite ensemble steps at B = 32, halving B after an out-of-memory error."""
+    out = {'metric': 'stage1_nphm_train_step', 'gpu': name, 'power_limit': power, 'steps': args.steps,
+           'timing': 'median of CUDA-event times per step, native and composite alternated'}
+    B = 32
+    while B >= 1:
+        oom = False
+        try:
+            out['nphm'] = run(lambda: setup_nphm(dev), lambda step: batch_shape(B, dev, step, anchors=True),
+                              lambda *a: train_step_shape(*a, lambdas=LAMBDAS_NPHM), args, compare_first=True)
+            out['batch'] = '%d x (750 + 50 + 800 + 93) points' % B
+            return out
+        except torch.cuda.OutOfMemoryError:
+            oom = True
+        if oom:                                        # outside the handler: the failed attempt's frames are released
+            out.setdefault('out_of_memory_at_batch', []).append(B)
+            gc.collect()
+            torch.cuda.empty_cache()
+            B //= 2
+    return out
+
+
+def profile_native(dev, stage=2, steps=5, decoder='npm'):
     """CUDA time per kernel (ms per step, largest first) of native steps (stage 2: `compress`, stage 1: NPM), from
     torch.profiler."""
     from torch.profiler import ProfilerActivity, profile
-    if stage == 1:
+    if stage == 1 and decoder == 'nphm':
+        state, batch_fn = setup_nphm(dev), lambda step: batch_shape(32, dev, step, anchors=True)
+        step_fn = lambda *a: train_step_shape(*a, lambdas=LAMBDAS_NPHM)           # noqa: E731
+    elif stage == 1:
         state, step_fn, batch_fn = setup_shape(dev), train_step_shape, lambda step: batch_shape(32, dev, step)
     else:
         state, step_fn, batch_fn = setup('compress', dev), train_step, lambda step: batch(32, 1000, dev, step)
@@ -248,16 +302,23 @@ def main():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--stage', type=int, choices=(1, 2), default=2,
                     help='2: expression space (train_corresp.py), 1: NPM shape space (train.py without -local)')
+    ap.add_argument('--decoder', choices=('npm', 'nphm'), default='npm',
+                    help='stage 1: npm (DeepSDF, train.py) or nphm (the ensemble, train.py -local)')
     ap.add_argument('--profile', action='store_true',
                     help='instead: torch.profiler over 5 native steps of the stage, CUDA time per kernel of the step (JSON)')
     args = ap.parse_args()
     if args.steps < 1:
         ap.error('--steps must be >= 1')
+    if args.decoder == 'nphm' and args.stage != 1:
+        ap.error('--decoder nphm: stage 1 only')
     dev = torch.device('cuda', torch.cuda.current_device())
     name, power = gpu_info()
     if args.profile:
         print(json.dumps({'metric': 'stage%d_native_kernels' % args.stage, 'gpu': name, 'power_limit': power,
-                          **profile_native(dev, args.stage)}))
+                          **profile_native(dev, args.stage, decoder=args.decoder)}))
+        return
+    if args.stage == 1 and args.decoder == 'nphm':
+        print(json.dumps(run_nphm(args, dev, name, power)))
         return
     if args.stage == 1:
         out = {'metric': 'stage1_train_step', 'gpu': name, 'power_limit': power,
