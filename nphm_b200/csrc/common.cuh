@@ -31,6 +31,15 @@ void set_error(const char *fmt, ...);
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 inline long long ceil_div(long long a, long long b) { return (a + b - 1) / b; }
 
+// Members and weight sets of an ensemble: members 2z and 2z + 1 of the first 2 n_symm are a mirrored pair sharing weight
+// set z; every later member m has its own set m - n_symm.  A plain MLP is one member, n_symm = 0.
+__host__ __device__ __forceinline__ int member_set(int m, int n_symm) { return m < 2 * n_symm ? m >> 1 : m - n_symm; }
+struct SetMembers { int first, count; };
+__host__ __device__ __forceinline__ SetMembers set_members(int z, int n_symm)
+{
+    return z < n_symm ? SetMembers{2 * z, 2} : SetMembers{z + n_symm, 1};
+}
+
 int sm_count();
 
 // ---------------------------------------------------------------------------------------------

@@ -35,7 +35,7 @@ void fill_descriptors(const StackDims &s, const NetWeights &w, int n_members, in
 
 }  // namespace nphm
 
-namespace nphm { namespace fit { struct BackwardPacks; } struct EnsembleChain; }
+namespace nphm { namespace fit { struct BackwardPacks; } struct PackedChain; }
 
 struct nphm_ensemble {
     nphm_ensemble_config cfg;
@@ -57,7 +57,7 @@ struct nphm_ensemble {
     nphm::DeviceBuffer fit_scratch, fit_apply_scratch;
     nphm::fit::BackwardPacks *fit_packs = nullptr;      // adjoint weights of the backward GEMMs, built on first use
     // stage-1 training through grad_x sdf (mlp_chain.cu): the layer chain of all weight sets, packed on first use
-    nphm::EnsembleChain *sdfgrad = nullptr;
+    nphm::PackedChain *sdfgrad = nullptr;
 };
 
 namespace nphm { struct MlpChain; }

@@ -70,25 +70,27 @@ __global__ void __launch_bounds__(256) column_sums_packed_kernel(const uint8_t *
     }
 }
 
-// grad_cond[q][j] = sum_n W0[n][3 + j] * S0[q][n]  +  sum_n Ws[n][Nh + 3 + j] * Ss[q][n] / sqrt(2)
+// grad_cond[m][q][j] = sum_n W0[n][3 + j] * S0[m][q][n]  +  sum_n Ws[n][c0s + j] * Ss[m][q][n] / sqrt(2), W0 and Ws those of
+// member m's weight set.  grid (column blocks, queries, members x chunks of the n range): one chunk writes its sum in a fixed
+// order; more add their partial sums with float atomics to an `out` the caller has zeroed.
 __global__ void cond_grad_kernel(const float *__restrict__ W0, int ld0, int N0, const float *__restrict__ S0,
-                                 const float *__restrict__ Ws, int lds, int Ns, int skip_col0, const float *__restrict__ Ss,
-                                 int cond_dim, float *__restrict__ out)
+                                 const float *__restrict__ Ws, int lds, int Ns, int c0s, const float *__restrict__ Ss, int cond_dim,
+                                 int n_queries, int n_symm, int chunks, float *__restrict__ out)
 {
-    // grid (column blocks, queries, chunks of the n range): `out` is zeroed by the caller, the chunks add their partial sums
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    const int q = blockIdx.y;
+    const int j = blockIdx.x * blockDim.x + threadIdx.x, q = blockIdx.y;
+    const int m = blockIdx.z / chunks, chunk = blockIdx.z % chunks, set = member_set(m, n_symm);
     if (j >= cond_dim) return;
-    const int c0 = (N0 + gridDim.z - 1) / gridDim.z, a0 = blockIdx.z * c0, b0 = min(N0, a0 + c0);
+    const size_t mq = (size_t)m * n_queries + q;
+    const float *w0 = W0 + (size_t)set * N0 * ld0, *ws = Ws + (size_t)set * Ns * lds;
+    const int c0 = (N0 + chunks - 1) / chunks, a0 = chunk * c0, b0 = min(N0, a0 + c0);
     float s = 0.f;
-    for (int n = a0; n < b0; ++n) s = fmaf(W0[(size_t)n * ld0 + 3 + j], S0[(size_t)q * N0 + n], s);
-    if (Ws) {
-        const int c1 = (Ns + gridDim.z - 1) / gridDim.z, a1 = blockIdx.z * c1, b1 = min(Ns, a1 + c1);
-        float t = 0.f;
-        for (int n = a1; n < b1; ++n) t = fmaf(Ws[(size_t)n * lds + skip_col0 + j], Ss[(size_t)q * Ns + n], t);
-        s = fmaf(t, kInvSqrt2, s);
-    }
-    atomicAdd(out + (size_t)q * cond_dim + j, s);
+    for (int n = a0; n < b0; ++n) s = fmaf(w0[(size_t)n * ld0 + 3 + j], S0[mq * N0 + n], s);
+    const int c1 = (Ns + chunks - 1) / chunks, a1 = chunk * c1, b1 = min(Ns, a1 + c1);
+    float t = 0.f;
+    for (int n = a1; n < b1; ++n) t = fmaf(ws[(size_t)n * lds + c0s + j], Ss[mq * Ns + n], t);
+    s = fmaf(t, kInvSqrt2, s);
+    if (chunks == 1) out[mq * cond_dim + j] = s;
+    else atomicAdd(out + mq * cond_dim + j, s);
 }
 
 // out[(q, n)][i][j] = T[(q, n, j)][i]   (tangent rows -> Jacobian layout B x N x out x 3)
@@ -116,31 +118,43 @@ __global__ void inverse_plus_identity_kernel(float *__restrict__ J, long long n)
     m[6] = C * inv; m[7] = -(a * h - b * g) * inv; m[8] = (a * e - b * d) * inv;
 }
 
-// grad_xyz[r][i] = (a[r][i] + b[r][i]) * scale[1]   (a, b: ld 4; scale == nullptr: 1)
-__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, const float *__restrict__ scale,
-                                float *__restrict__ out)
+// grad_xyz[m][r][i] = (a[m][r][i] + b[m][r][i]) * scale[sstride set(m) + 1]   (a, b: ld 4; scale == nullptr: 1)
+__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, int members,
+                                const float *__restrict__ scale, int sstride, int n_symm, float *__restrict__ out)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= M * 3) return;
+    if (idx >= (long long)members * M * 3) return;
     const long long r = idx / 3;
-    const int i = (int)(idx % 3);
-    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * (scale ? scale[1] : 1.0f);
+    const int i = (int)(idx % 3), m = (int)(r / M);
+    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * (scale ? scale[sstride * member_set(m, n_symm) + 1] : 1.0f);
 }
 
 }  // namespace chain
 
-// ------------------------------------------------------------------------------------------------ packed stack
-struct MlpChain {
+// ------------------------------------------------------------------------------------------------ members and packed stack
+// The passes run over `count` members at once: tc_linear's batched launch over gridDim.z = member, tc_wgrad's over gridDim.z =
+// weight set.  Member m uses weight set member_set(m, n_symm) of `sets` sets packed back to back, and its part of every per-row
+// buffer starts at m times that buffer's member stride.  A DeepSDF handle is {1, 0, 1}, the NPHM ensemble {40, 16, 24}.
+struct Members {
+    int count = 1, n_symm = 0, sets = 1;
+};
+
+struct PackedChain {
     bool packed = false;
-    int n_lin = 0;
     tcl::PackedLinear fwd[kMaxLayers];        // B = W_l restricted to its point-dependent columns (1/sqrt2 folded at the skip)
     tcl::PackedLinear adj[kMaxLayers];        // B = W_l^T (input-activation columns only)
     tcl::PackedLinear adj_x0, adj_xs;         // W_0[:, 0:3]^T and W_skip[:, Nh:Nh+3]^T / sqrt2  (gradient w.r.t. xyz)
+    int ld[kMaxLayers];
+    // scratch of the backwards: GEMM partials, per-(member, query) column sums of d_0, d_skip and the other layers
+    DeviceBuffer partials, sums0, sumss, sums;
+};
+
+// what only the DeepSDF handle has
+struct MlpChain : PackedChain {
     // activations between the layers live in the packed operand format (Hp: values, Tp: tangents, Dp: adjoints), the
     // activation derivatives S in the blocked fp32 layout ([128-row tile][feature][128]) - every access of the passes is coalesced
     DeviceBuffer Hp[kMaxLayers], S[kMaxLayers], Tp[2], Dp[2], Tlast, out_tmp;
     DeviceBuffer Fp[2];                       // ping-pong activations of the forward-only pass (forward_pass)
-    int ld[kMaxLayers];
     long long value_rows = 0;                 // rows of the last value pass that kept the activation derivatives
     bool have_deriv = false;
     // training (nphm_mlp_train_forward / _backward) with condition noise: layers 0, skip - 1 and skip take `train_nd` > 0
@@ -148,42 +162,61 @@ struct MlpChain {
     // appends them); packed on first use after every weight load.
     tcl::PackedLinear tfwd[kMaxLayers];
     int train_nd = -1;
-    // scratch of the backwards: the packed top adjoint, GEMM partials, per-query column sums (of d_0, d_skip and the other
-    // layers), the two [M][4] point-gradient parts (d_0 and d_skip times their layer's xyz columns)
-    DeviceBuffer Dl, wg_partials, gscale, qsums, qsums0, qsumss, xtmp, xs_tmp;
+    // scratch of the first-order backwards: the packed top adjoint, its scale pair, the two [M][4] point-gradient parts (d_0
+    // and d_skip times their layer's xyz columns)
+    DeviceBuffer Dl, gscale, xtmp, xs_tmp;
 };
+
+// the stack a pass runs on
+struct Stack {
+    const StackDims &s;
+    const NetWeights &w;
+    PackedChain &c;
+    Members m;
+};
+
+static Stack stack(nphm_mlp *h) { return Stack{h->dims, h->weights, *h->chain, Members{}}; }
 
 static int pad4(int n) { return (n + 3) / 4 * 4; }
 constexpr int kChainNt = 128;
 
-int chain_pack(nphm_mlp *h, cudaStream_t stream)
+// packs `sets` weight sets, set z of layer l at W_l + z N_l in_total_l
+static int pack_chain(PackedChain &c, const StackDims &s, const NetWeights &wts, int sets, cudaStream_t stream)
 {
-    if (!h->chain) h->chain = new MlpChain();
-    MlpChain &c = *h->chain;
-    const StackDims &s = h->dims;
-    c.n_lin = s.n_lin;
     int rc;
     for (int l = 0; l < s.n_lin; ++l) {
-        const float *W = h->weights.W[l].as<float>();
+        const float *W = wts.W[l].as<float>();
         const int ldw = s.in_total[l];
+        const long long wst = (long long)s.N[l] * ldw;
         const float scale = l == s.skip ? chain::kInvSqrt2 : 1.0f;
         // forward: point-dependent leading columns (xyz | h_{l-1} | [h_{skip-1}, xyz])
         // (the layer in front of the skip layer reserves 3 output columns: its epilogue appends xyz / the tangent seeds)
         // tiles of <= 128 output columns: the passes run on a few thousand rows (fitting), where CTAs count more than tile width
-        if ((rc = c.fwd[l].pack(W, ldw, s.N[l], s.K[l], 0, 0, false, scale, stream, 1, 0, nullptr, 0, l + 1 == s.skip ? 3 : 0,
+        if ((rc = c.fwd[l].pack(W, ldw, s.N[l], s.K[l], 0, 0, false, scale, stream, sets, wst, nullptr, 0, l + 1 == s.skip ? 3 : 0,
                                 kChainNt)))
             return rc;
         // adjoint w.r.t. the input activations of layer l (l >= 1): columns [0, N_{l-1})
-        if (l >= 1 && (rc = c.adj[l].pack(W, ldw, s.N[l - 1], s.N[l], 0, 0, true, scale, stream, 1, 0, nullptr, 0, 0, kChainNt)))
+        if (l >= 1 && (rc = c.adj[l].pack(W, ldw, s.N[l - 1], s.N[l], 0, 0, true, scale, stream, sets, wst, nullptr, 0, 0, kChainNt)))
             return rc;
         c.ld[l] = pad4(s.N[l]);
     }
-    if ((rc = c.adj_x0.pack(h->weights.W[0].as<float>(), s.in_total[0], 3, s.N[0], 0, 0, true, 1.0f, stream))) return rc;
+    if ((rc = c.adj_x0.pack(wts.W[0].as<float>(), s.in_total[0], 3, s.N[0], 0, 0, true, 1.0f, stream, sets,
+                            (long long)s.N[0] * s.in_total[0])))
+        return rc;
     if (s.skip > 0 && s.skip < s.n_lin &&
-        (rc = c.adj_xs.pack(h->weights.W[s.skip].as<float>(), s.in_total[s.skip], 3, s.N[s.skip], s.N[s.skip - 1], 0, true,
-                            chain::kInvSqrt2, stream))) return rc;
+        (rc = c.adj_xs.pack(wts.W[s.skip].as<float>(), s.in_total[s.skip], 3, s.N[s.skip], s.N[s.skip - 1], 0, true,
+                            chain::kInvSqrt2, stream, sets, (long long)s.N[s.skip] * s.in_total[s.skip])))
+        return rc;
     c.packed = true;
-    c.train_nd = -1;
+    return NPHM_OK;
+}
+
+int chain_pack(nphm_mlp *h, cudaStream_t stream)
+{
+    if (!h->chain) h->chain = new MlpChain();
+    int rc = pack_chain(*h->chain, h->dims, h->weights, 1, stream);
+    if (rc) return rc;
+    h->chain->train_nd = -1;
     return NPHM_OK;
 }
 
@@ -204,37 +237,39 @@ struct Carver {
 // the layers that take the per-row condition noise as extra input columns (training, MlpChain::tfwd)
 static bool noise_layer(const StackDims &s, int l) { return l == 0 || l + 1 == s.skip || l == s.skip; }
 
-// packed forward weights of layer l with nd noise columns
-static const tcl::PackedLinear &fwd_layer(const MlpChain &c, const StackDims &s, int l, int nd)
-{
-    return nd > 0 && noise_layer(s, l) ? c.tfwd[l] : c.fwd[l];
-}
+// the per-row buffers of a value pass over M rows per member; member m's part of each at m times its stride (floats; bytes
+// for the packed Hp)
+struct ValueRows {
+    const float *X = nullptr; int ldx = 3; long long sX = 0;     // rows [xyz | nd noise columns]: the input of layer 0 and the
+    int nd = 0;                                                 // columns appended behind layer skip - 1
+    const tcl::PackedLinear *tfwd = nullptr;                    // nd > 0: the packs of the noise layers (MlpChain::tfwd)
+    const float *bias = nullptr; long long rows_per_bias = 0, sBias = 0;     // the per-query constants of the first query
+    uint8_t *Hp[kMaxLayers] = {}; long long sHp[kMaxLayers] = {};           // h_l, packed
+    float *S[kMaxLayers] = {}; long long sS[kMaxLayers] = {};               // s_l, blocked (optional)
+    float *out = nullptr; long long sOut = 0;                                // the output layer, row-major
+    const int *live = nullptr;                                               // see forward_pass
+};
 
-// value pass over M rows, softplus layers 0 .. n_lin - 2 and the linear output layer.  X: rows [xyz | nd noise columns]
-// (ld ldx), the input of layer 0 and the columns appended behind layer skip - 1.  Layer l < n_lin - 1 writes h_l packed to
-// Hp[l] and, if S is given, s_l blocked to S[l]; the output layer writes `out` row-major.  bias: the per-query constants of
-// the first query, rows_per_bias rows per query.  live: see forward_pass.
-static int value_layers(nphm_mlp *h, long long M, const float *X, int ldx, int nd, const float *bias, long long rows_per_bias,
-                        uint8_t *const *Hp, float *const *S, float *out, const int *live, cudaStream_t stream)
+// value pass: softplus layers 0 .. n_lin - 2 and the linear output layer
+static int value_layers(const Stack &k, long long M, const ValueRows &v, cudaStream_t stream)
 {
-    MlpChain &c = *h->chain;
-    const StackDims &s = h->dims;
+    const StackDims &s = k.s;
     for (int l = 0; l < s.n_lin; ++l) {
-        const tcl::PackedLinear &W = fwd_layer(c, s, l, nd);
+        const tcl::PackedLinear &W = v.nd > 0 && noise_layer(s, l) ? v.tfwd[l] : k.c.fwd[l];
         tcl::LinearParams p;
-        p.M = M;
-        p.live = live;
-        if (l == 0) { p.A1 = X; p.lda1 = ldx; p.K1 = 3 + nd; }
-        else { p.Ap = Hp[l - 1]; p.a_ksteps = W.ksteps; }        // at the skip layer: [h | xyz | noise], appended below
-        p.bias = bias + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = rows_per_bias;
+        p.M = M; p.batch = k.m.count; p.w_pairs = k.m.n_symm;
+        p.live = v.live;
+        if (l == 0) { p.A1 = v.X; p.lda1 = v.ldx; p.K1 = 3 + v.nd; p.sA1 = v.sX; }
+        else { p.Ap = v.Hp[l - 1]; p.a_ksteps = W.ksteps; p.sAp = v.sHp[l - 1]; }   // at the skip layer: [h | xyz | noise]
+        p.bias = v.bias + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = v.rows_per_bias; p.sBias = v.sBias;
         if (l == s.n_lin - 1) {
             p.mode = tcl::kModeLinear;
-            p.C = out; p.ldc = s.N[l];
+            p.C = v.out; p.ldc = s.N[l]; p.sC = v.sOut;
         } else {
             p.mode = tcl::kModeSoftplus;
-            p.Cp = Hp[l]; p.c_ksteps = W.packed_ksteps_out();
-            if (l + 1 == s.skip) { p.app = X; p.app_ld = ldx; p.app_w = 3 + nd; }
-            if (S) { p.Dv = S[l]; p.lddv = c.ld[l]; p.dv_blocked = 1; }
+            p.Cp = v.Hp[l]; p.c_ksteps = W.packed_ksteps_out(); p.sCp = v.sHp[l];
+            if (l + 1 == s.skip) { p.app = v.X; p.app_ld = v.ldx; p.app_w = 3 + v.nd; p.sApp = v.sX; }
+            if (v.S[l]) { p.Dv = v.S[l]; p.lddv = k.c.ld[l]; p.dv_blocked = 1; p.sDv = v.sS[l]; }
         }
         int rc = tcl::launch_linear(W, p, stream);
         if (rc) return rc;
@@ -250,17 +285,18 @@ static int value_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_
     MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
     const long long M = (long long)n_queries * n_points;
-    uint8_t *Hp[kMaxLayers];
-    float *S[kMaxLayers];
+    ValueRows v;
+    v.X = xyz;
+    v.bias = h->cvec.as<float>(); v.rows_per_bias = n_points;
+    v.out = out;
     int rc;
     for (int l = 0; l + 1 < s.n_lin; ++l) {
         if ((rc = c.Hp[l].reserve(packed_bytes(M, c.fwd[l].packed_ksteps_out())))) return rc;
         if (want_deriv && (rc = c.S[l].reserve((size_t)ceil_div(M, 128) * 128 * c.ld[l] * sizeof(float)))) return rc;
-        Hp[l] = c.Hp[l].as<uint8_t>();
-        S[l] = c.S[l].as<float>();
+        v.Hp[l] = c.Hp[l].as<uint8_t>();
+        if (want_deriv) v.S[l] = c.S[l].as<float>();
     }
-    if ((rc = value_layers(h, M, xyz, 3, 0, h->cvec.as<float>(), n_points, Hp, want_deriv ? S : nullptr, out, nullptr, stream)))
-        return rc;
+    if ((rc = value_layers(stack(h), M, v, stream))) return rc;
     c.value_rows = M;
     c.have_deriv = want_deriv;
     return NPHM_OK;
@@ -284,99 +320,105 @@ static int forward_pass(nphm_mlp *h, const float *xyz, int n_queries, long long 
     const long long max_rows = std::min((long long)n_queries, qpc) * ppc;
     for (int b = 0; b < 2; ++b)
         if ((rc = c.Fp[b].reserve(packed_bytes(max_rows, ks_max)))) return rc;
-    uint8_t *Hp[kMaxLayers];
-    for (int l = 0; l + 1 < s.n_lin; ++l) Hp[l] = c.Fp[l & 1].as<uint8_t>();
+    ValueRows v;
+    v.live = live;
+    for (int l = 0; l + 1 < s.n_lin; ++l) v.Hp[l] = c.Fp[l & 1].as<uint8_t>();
     const int out_dim = s.N[s.n_lin - 1];
     for (long long q0 = 0; q0 < n_queries; q0 += qpc) {
         const long long nq = std::min(qpc, (long long)n_queries - q0);
         for (long long p0 = 0; p0 < n_points; p0 += ppc) {
             const long long np = std::min(ppc, n_points - p0);       // nq > 1 only with whole queries (np == n_points)
             const size_t row0 = (size_t)q0 * n_points + p0;
-            if ((rc = value_layers(h, nq * np, xyz + row0 * 3, 3, 0, h->cvec.as<float>() + (size_t)q0 * s.cvec_stride, np, Hp,
-                                   nullptr, out + row0 * out_dim, live, stream)))
-                return rc;
+            v.X = xyz + row0 * 3;
+            v.bias = h->cvec.as<float>() + (size_t)q0 * s.cvec_stride; v.rows_per_bias = np;
+            v.out = out + row0 * out_dim;
+            if ((rc = value_layers(stack(h), nq * np, v, stream))) return rc;
         }
     }
     c.have_deriv = false;
     return NPHM_OK;
 }
 
-// the adjoint of a layer's pre-activations: row-major fp32 rows (the caller's output gradient) or packed (ks k-steps)
+// the adjoint of a layer's pre-activations: row-major fp32 rows (the caller's output gradient) or packed (ks k-steps); member
+// m's part at m times `stride` (floats or bytes)
 struct Adjoint {
     const float *rows = nullptr; int ld = 0;
     const uint8_t *packed = nullptr; int ks = 0;
+    long long stride = 0;
 };
 
-// what one adjoint walk reads and writes; per-layer entries for l < L = n_lin - 1
+// what one adjoint walk reads and writes; per-layer entries for l < L = n_lin - 1, member strides in floats (S, cpl_z) or
+// bytes (D, cpl_a)
 struct AdjointWalk {
-    Adjoint top;                                   // d_L
-    const float *S[kMaxLayers] = {};               // s_l, blocked fp32
-    uint8_t *D[kMaxLayers] = {};                   // where d_l goes, packed
-    const float *cpl_z[kMaxLayers] = {};           // optional coupling of the SDF-gradient backward:
-    const uint8_t *cpl_a[kMaxLayers] = {};         //   d_l += kBeta (1 - s_l) * cpl_z[l] * cpl_a[l]
-    float *xs = nullptr;                           // optional [M][4]: d_skip W_skip[:, Nh:Nh+3]^T / sqrt2
+    Adjoint top;                                                      // d_L
+    const float *S[kMaxLayers] = {}; long long sS[kMaxLayers] = {};   // s_l, blocked fp32
+    uint8_t *D[kMaxLayers] = {}; long long sD[kMaxLayers] = {};       // where d_l goes, packed
+    const float *cpl_z[kMaxLayers] = {};                              // optional coupling of the SDF-gradient backward:
+    const uint8_t *cpl_a[kMaxLayers] = {}; long long sA[kMaxLayers] = {};   // d_l += kBeta (1 - s_l) * cpl_z[l] * cpl_a[l]
+    float *xs = nullptr;                                              // optional [members][M][4]: d_skip W_skip[:, Nh:Nh+3]^T / sqrt2
 };
 
-// d_{l-1} = s_{l-1} * (d_l W_l) from d_L down to d_0 (left in w.D[0]).  hook(l, d_l, ks) runs for l = L .. 1 before the
-// descent below layer l (d_L given as rows: d_l == nullptr) and for l = 0 at the bottom.
+// d_{l-1} = s_{l-1} * (d_l W_l) from d_L down to d_0 (left in w.D[0]) for every member.  hook(l, d_l) runs for l = L .. 1
+// before the descent below layer l and for l = 0 at the bottom.
 template <class Hook>
-static int adjoint_walk(nphm_mlp *h, long long M, const AdjointWalk &w, Hook &&hook, cudaStream_t stream)
+static int adjoint_walk(const Stack &k, long long M, const AdjointWalk &w, Hook &&hook, cudaStream_t stream)
 {
-    MlpChain &c = *h->chain;
-    const StackDims &s = h->dims;
+    const StackDims &s = k.s;
     Adjoint d = w.top;
     int rc;
     for (int l = s.n_lin - 1; l >= 1; --l) {
-        if ((rc = hook(l, d.packed, d.ks))) return rc;
+        if ((rc = hook(l, d))) return rc;
+        tcl::LinearParams p;
+        p.M = M; p.batch = k.m.count; p.w_pairs = k.m.n_symm;
+        if (d.packed) { p.Ap = d.packed; p.a_ksteps = d.ks; p.sAp = d.stride; }
+        else { p.A1 = d.rows; p.lda1 = d.ld; p.K1 = s.N[l]; p.sA1 = d.stride; }
         if (l == s.skip && w.xs) {                 // d_skip is packed: chain_ready keeps the skip layer below the output layer
-            tcl::LinearParams px;
-            px.M = M;
-            px.Ap = d.packed; px.a_ksteps = d.ks;
-            px.mode = tcl::kModeLinear; px.C = w.xs; px.ldc = 4;
-            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
+            tcl::LinearParams px = p;
+            px.mode = tcl::kModeLinear; px.C = w.xs; px.ldc = 4; px.sC = M * 4;
+            if ((rc = tcl::launch_linear(k.c.adj_xs, px, stream))) return rc;
         }
         const int ks = (s.N[l - 1] + 15) / 16;
-        tcl::LinearParams p;
-        p.M = M;
-        if (d.packed) { p.Ap = d.packed; p.a_ksteps = d.ks; }
-        else { p.A1 = d.rows; p.lda1 = d.ld; p.K1 = s.N[l]; }
         p.mode = tcl::kModeMult;
-        p.Mul = w.S[l - 1]; p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1;
-        if (w.cpl_a[l - 1]) { p.cpl_z = w.cpl_z[l - 1]; p.cpl_a = w.cpl_a[l - 1]; p.cpl_a_steps = ks; p.cpl_coef = chain::kBeta; }
-        p.Cp = w.D[l - 1]; p.c_ksteps = ks;
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        d = Adjoint{nullptr, 0, w.D[l - 1], ks};
+        p.Mul = w.S[l - 1]; p.ldmul = k.c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1; p.sMul = w.sS[l - 1];
+        if (w.cpl_a[l - 1]) {
+            p.cpl_z = w.cpl_z[l - 1]; p.sCplZ = w.sS[l - 1];
+            p.cpl_a = w.cpl_a[l - 1]; p.sCplA = w.sA[l - 1]; p.cpl_a_steps = ks; p.cpl_coef = chain::kBeta;
+        }
+        p.Cp = w.D[l - 1]; p.c_ksteps = ks; p.sCp = w.sD[l - 1];
+        if ((rc = tcl::launch_linear(k.c.adj[l], p, stream))) return rc;
+        d = Adjoint{nullptr, 0, w.D[l - 1], ks, w.sD[l - 1]};
     }
-    return hook(0, d.packed, d.ks);
+    return hook(0, d);
 }
 
-// grad_cond [q][cond_dim] from the per-query column sums of d_0 (qsums0) and d_skip (qsumss).  chunks: CTAs per output over
-// the n range, added with float atomics; 1 keeps a fixed summation order.
-static int cond_grad(nphm_mlp *h, int n_queries, int chunks, float *grad_cond, cudaStream_t stream)
+// grad_cond [members][q][cond_dim] from the per-(member, query) column sums of d_0 (sums0) and d_skip (sumss).  chunks: CTAs
+// per output over the n range, added with float atomics; 1 keeps a fixed summation order.
+static int cond_grad(const Stack &k, int n_queries, int chunks, float *grad_cond, cudaStream_t stream)
 {
-    MlpChain &c = *h->chain;
-    const StackDims &s = h->dims;
-    NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond, 0, (size_t)n_queries * s.cond_dim * sizeof(float), stream));
-    dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, (unsigned)chunks);
-    chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.qsums0.as<float>(),
-                                                      h->weights.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
-                                                      s.N[s.skip - 1] + 3, c.qsumss.as<float>(), s.cond_dim, grad_cond);
+    const StackDims &s = k.s;
+    if (chunks > 1) NPHM_CUDA_CHECK(cudaMemsetAsync(grad_cond, 0, (size_t)k.m.count * n_queries * s.cond_dim * sizeof(float), stream));
+    dim3 grid((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_queries, (unsigned)(k.m.count * chunks));
+    chain::cond_grad_kernel<<<grid, 128, 0, stream>>>(k.w.W[0].as<float>(), s.in_total[0], s.N[0], k.c.sums0.as<float>(),
+                                                      k.w.W[s.skip].as<float>(), s.in_total[s.skip], s.N[s.skip],
+                                                      s.N[s.skip - 1] + 3, k.c.sumss.as<float>(), s.cond_dim, n_queries,
+                                                      k.m.n_symm, chunks, grad_cond);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
 
-// grad_xyz = (d_0 W_0[:, 0:3]^T + xs) * scale[1] (scale == nullptr: 1): d_0 packed (w.D[0] of the walk), x0 an [M][4]
-// temporary, xs the walk's skip-layer part
-static int xyz_grad(nphm_mlp *h, long long M, const uint8_t *d0, float *x0, const float *xs, const float *scale, float *grad_xyz,
-                    cudaStream_t stream)
+// grad_xyz = (d_0 W_0[:, 0:3]^T + xs) * scale[sstride set + 1] (scale == nullptr: 1): d_0 packed (w.D[0] of the walk, member
+// stride d0_stride), x0 an [members][M][4] temporary, xs the walk's skip-layer part
+static int xyz_grad(const Stack &k, long long M, const uint8_t *d0, long long d0_stride, float *x0, const float *xs,
+                    const float *scale, int sstride, float *grad_xyz, cudaStream_t stream)
 {
     tcl::LinearParams p;
-    p.M = M;
-    p.Ap = d0; p.a_ksteps = (h->dims.N[0] + 15) / 16;
-    p.mode = tcl::kModeLinear; p.C = x0; p.ldc = 4;
-    int rc = tcl::launch_linear(h->chain->adj_x0, p, stream);
+    p.M = M; p.batch = k.m.count; p.w_pairs = k.m.n_symm;
+    p.Ap = d0; p.a_ksteps = (k.s.N[0] + 15) / 16; p.sAp = d0_stride;
+    p.mode = tcl::kModeLinear; p.C = x0; p.ldc = 4; p.sC = M * 4;
+    int rc = tcl::launch_linear(k.c.adj_x0, p, stream);
     if (rc) return rc;
-    chain::xyz_grad_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(x0, xs, M, scale, grad_xyz);
+    chain::xyz_grad_kernel<<<(unsigned)ceil_div(k.m.count * M * 3, 256), 256, 0, stream>>>(x0, xs, M, k.m.count, scale, sstride,
+                                                                                          k.m.n_symm, grad_xyz);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
@@ -504,29 +546,30 @@ extern "C" int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const
     for (int l = 1; l <= L; ++l) max_ks = std::max(max_ks, (s.N[l - 1] + 15) / 16);
     for (int i = 0; i < 2; ++i)
         if ((rc = c.Dp[i].reserve(packed_bytes(M, max_ks)))) return rc;
-    if ((rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
-        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
+    if ((rc = c.sums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
+        (rc = c.sumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
         return rc;
     if (grad_xyz_dev && ((rc = c.xtmp.reserve((size_t)M * 4 * sizeof(float))) || (rc = c.xs_tmp.reserve((size_t)M * 4 * sizeof(float)))))
         return rc;
-    NPHM_CUDA_CHECK(cudaMemsetAsync(c.qsums0.ptr, 0, (size_t)n_queries * s.N[0] * sizeof(float), stream));
-    NPHM_CUDA_CHECK(cudaMemsetAsync(c.qsumss.ptr, 0, (size_t)n_queries * s.N[s.skip] * sizeof(float), stream));
+    NPHM_CUDA_CHECK(cudaMemsetAsync(c.sums0.ptr, 0, (size_t)n_queries * s.N[0] * sizeof(float), stream));
+    NPHM_CUDA_CHECK(cudaMemsetAsync(c.sumss.ptr, 0, (size_t)n_queries * s.N[s.skip] * sizeof(float), stream));
     // the output layer's adjoint is the caller's grad_out as it is; d_l lives in Dp[l & 1]
     AdjointWalk w;
-    w.top = Adjoint{grad_out_dev, out_dim, nullptr, 0};
+    w.top = Adjoint{grad_out_dev, out_dim, nullptr, 0, 0};
     for (int l = 0; l < L; ++l) { w.S[l] = c.S[l].as<float>(); w.D[l] = c.Dp[l & 1].as<uint8_t>(); }
     w.xs = grad_xyz_dev ? c.xs_tmp.as<float>() : nullptr;
     // the column sums of d_0 and d_skip feed the condition gradient
-    auto col_sums = [&](int l, const uint8_t *d, int ks) {
+    auto col_sums = [&](int l, const Adjoint &d) {
         if (l != 0 && l != s.skip) return NPHM_OK;
-        chain::column_sums_packed_kernel<<<dim3((unsigned)ceil_div(M, 128), (unsigned)ks), 256, 0, stream>>>(
-            d, ks, M, n_points, s.N[l], l == 0 ? c.qsums0.as<float>() : c.qsumss.as<float>());
+        chain::column_sums_packed_kernel<<<dim3((unsigned)ceil_div(M, 128), (unsigned)d.ks), 256, 0, stream>>>(
+            d.packed, d.ks, M, n_points, s.N[l], l == 0 ? c.sums0.as<float>() : c.sumss.as<float>());
         NPHM_CUDA_CHECK(cudaGetLastError());
         return NPHM_OK;
     };
-    if ((rc = adjoint_walk(h, M, w, col_sums, stream))) return rc;
-    if (grad_cond_dev && (rc = cond_grad(h, n_queries, 16, grad_cond_dev, stream))) return rc;
-    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], c.xtmp.as<float>(), w.xs, nullptr, grad_xyz_dev, stream))) return rc;
+    const Stack k = stack(h);
+    if ((rc = adjoint_walk(k, M, w, col_sums, stream))) return rc;
+    if (grad_cond_dev && (rc = cond_grad(k, n_queries, 16, grad_cond_dev, stream))) return rc;
+    if (grad_xyz_dev && (rc = xyz_grad(k, M, w.D[0], 0, c.xtmp.as<float>(), w.xs, nullptr, 0, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
 
@@ -557,6 +600,9 @@ extern "C" int nphm_mlp_inverse_jacobian(nphm_mlp *h, const float *xyz_dev, cons
 // fp16 range: the upstream gradient of the loss is of order 1e-5, where the hi part of the fp16 split is subnormal and the lo
 // part is lost.  The backward scales it on the device by a power of two (its largest magnitude to 2^10) and undoes the scale in
 // the fp32 epilogues of the gradients (grad_scale_kernel).
+//
+// The kernels below are member-indexed (Members): member m reads and writes its part of a per-row buffer at m times its member
+// stride and uses the scale pair of its weight set, scale[2 set], scale[2 set + 1].
 namespace nphm {
 namespace train {
 
@@ -596,43 +642,52 @@ __global__ void stage_x0_kernel(const float *__restrict__ xyz, const float *__re
     X0[idx] = c < 3 ? xyz[r * 3 + c] : (c < 3 + nd ? noise[r * nd + c - 3] : 0.f);
 }
 
-// fp32 rows [M][ld] (the first `width` columns, times scale[0] if given) -> packed operand tiles of `ks` k-steps
-// (tc_linear.cuh); the rows of the last tile beyond M are zero.  Thread = (row, 8 columns).
-__global__ void pack_rows_kernel(const float *__restrict__ src, int ld, int width, long long M, int ks, const float *__restrict__ scale,
-                                 uint8_t *__restrict__ dst)
+// fp32 rows [M][ld] (the first `width` columns, times scale[2 set] if given) -> packed operand tiles of `ks` k-steps
+// (tc_linear.cuh); the rows of the last tile beyond M are zero.  Thread = (row, 8 columns); grid (row blocks, members):
+// member m reads src + m src_stride (floats), writes dst + m dst_stride (bytes).
+__global__ void pack_rows_kernel(const float *__restrict__ src, int ld, int width, long long M, int ks, long long src_stride,
+                                 const float *__restrict__ scale, int n_symm, uint8_t *__restrict__ dst, long long dst_stride)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int m = blockIdx.y;
     if (idx >= (M + 127) / 128 * 128 * 2 * ks) return;
     const long long row = idx / (2 * ks);
     const int g = (int)(idx % (2 * ks));
-    const float sc = scale ? scale[0] : 1.0f;
+    const float sc = scale ? scale[2 * member_set(m, n_symm)] : 1.0f;
+    const float *sr = src + (size_t)m * src_stride;
     float v[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int c = 8 * g + i;
-        v[i] = (row < M && c < width) ? src[(size_t)row * ld + c] * sc : 0.f;
+        v[i] = (row < M && c < width) ? sr[(size_t)row * ld + c] * sc : 0.f;
     }
     uint32_t hi[4], lo[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) tc::split2(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
-    uint8_t *d = dst + ((size_t)(row >> 7) * ks + (g >> 1)) * 8192 + (size_t)((row & 127) >> 3) * 256 + (g & 1) * 128 + (row & 7) * 16;
+    uint8_t *d = dst + (size_t)m * dst_stride + ((size_t)(row >> 7) * ks + (g >> 1)) * 8192 + (size_t)((row & 127) >> 3) * 256 +
+                 (g & 1) * 128 + (row & 7) * 16;
     *reinterpret_cast<uint4 *>(d) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
     *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
 
-// scale[0] = 2^(kGradExp - e) with 2^e <= max |g| < 2^(e+1) (1 for an all-zero or non-finite g), scale[1] = 1 / scale[0].
+// scale[2 z] = 2^(kGradExp - e) with 2^e <= max |.| < 2^(e+1) over the parts of weight set z's members of g (n values per
+// member) and g2 (optional, n2 values per member); 1 for an all-zero or non-finite set; scale[2 z + 1] = 1 / scale[2 z].
 // kGradExp: the adjoint shrinks layer by layer (~0.3x per 512-wide layer at initialisation), and an fp16 hi | lo pair only
 // keeps its 22 bits while |x| >= 2^-3 (below that lo is subnormal): the top of the chain starts at 2^10 so that d_0 is still
-// in that range, which leaves 2^5 of headroom below the fp16 maximum for an adjoint that grows instead.  One block.
-// g2 (optional, n2 values): the maximum is taken over both arrays.
+// in that range, which leaves 2^5 of headroom below the fp16 maximum for an adjoint that grows instead.  One block per set.
 constexpr int kGradExp = 10;
-__global__ void grad_scale_kernel(const float *__restrict__ g, long long n, const float *__restrict__ g2, long long n2,
+__global__ void grad_scale_kernel(const float *__restrict__ g, long long n, const float *__restrict__ g2, long long n2, int n_symm,
                                   float *__restrict__ scale)
 {
     __shared__ float red[32];
+    const int z = blockIdx.x;
+    const SetMembers sm = set_members(z, n_symm);
     float m = 0.f;
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(g[i]));
-    for (long long i = threadIdx.x; i < n2; i += blockDim.x) m = fmaxf(m, fabsf(g2[i]));
+    for (int k = 0; k < sm.count; ++k) {
+        const float *a = g + (size_t)(sm.first + k) * n, *b = g2 + (size_t)(sm.first + k) * n2;
+        for (long long i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(a[i]));
+        for (long long i = threadIdx.x; i < n2; i += blockDim.x) m = fmaxf(m, fabsf(b[i]));
+    }
 #pragma unroll
     for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
@@ -640,22 +695,24 @@ __global__ void grad_scale_kernel(const float *__restrict__ g, long long n, cons
     if (threadIdx.x == 0) {
         for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, red[w]);
         const int e = (m > 0.f && isfinite(m)) ? max(-100, min(100, ilogbf(m))) - kGradExp : 0;
-        scale[0] = ldexpf(1.0f, -e);
-        scale[1] = ldexpf(1.0f, e);
+        scale[2 * z] = ldexpf(1.0f, -e);
+        scale[2 * z + 1] = ldexpf(1.0f, e);
     }
 }
 
-// out[q][c] = scale[1] * (sum over the rows of query q of the packed X[row][c]), in a fixed order.  grid (k-steps, queries),
-// 256 threads = 16 columns x 16 row lanes.
-__global__ void __launch_bounds__(256) query_sums_kernel(const uint8_t *__restrict__ X, int ks, long long n_points, int n_cols,
-                                                         const float *__restrict__ scale, float *__restrict__ out)
+// out[m][q][c] = scale[2 set(m) + 1] * (sum over the rows of (m, q) of the packed X[row][c]), in a fixed order.  grid (k-steps,
+// queries, members), 256 threads = 16 columns x 16 row lanes.
+__global__ void __launch_bounds__(256) query_sums_kernel(const uint8_t *__restrict__ X, int ks, long long stride, long long n_points,
+                                                         int n_queries, int n_cols, const float *__restrict__ scale, int n_symm,
+                                                         float *__restrict__ out)
 {
     __shared__ float part[16][17];
-    const int c = threadIdx.x & 15, rl = threadIdx.x >> 4, j = blockIdx.x, q = blockIdx.y;
+    const int c = threadIdx.x & 15, rl = threadIdx.x >> 4, j = blockIdx.x, q = blockIdx.y, m = blockIdx.z;
+    const uint8_t *Xm = X + (size_t)m * stride;
     const long long r1 = (long long)(q + 1) * n_points;
     float s = 0.f;
     for (long long r = (long long)q * n_points + rl; r < r1; r += 16) {
-        const uint8_t *p = X + ((size_t)(r >> 7) * ks + j) * 8192 + (size_t)((r & 127) >> 3) * 256 + (c >> 3) * 128 + (r & 7) * 16 + (c & 7) * 2;
+        const uint8_t *p = Xm + ((size_t)(r >> 7) * ks + j) * 8192 + (size_t)((r & 127) >> 3) * 256 + (c >> 3) * 128 + (r & 7) * 16 + (c & 7) * 2;
         s += __half2float(*reinterpret_cast<const __half *>(p)) + __half2float(*reinterpret_cast<const __half *>(p + 4096));
     }
     part[rl][c] = s;
@@ -663,81 +720,124 @@ __global__ void __launch_bounds__(256) query_sums_kernel(const uint8_t *__restri
     if (rl == 0 && j * 16 + c < n_cols) {
         float t = 0.f;
         for (int i = 0; i < 16; ++i) t += part[i][c];
-        out[(size_t)q * n_cols + j * 16 + c] = t * scale[1];
+        out[((size_t)m * n_queries + q) * n_cols + j * 16 + c] = t * scale[2 * member_set(m, n_symm) + 1];
     }
 }
 
-// out[c] = sum_q sums[q][c]  (bias gradient)
-__global__ void sum_queries_kernel(const float *__restrict__ sums, int n_queries, int n, float *__restrict__ out)
+// out[z][c] = sum over the members of weight set z (in order) and their queries of sums[m][q][c]  (bias gradient); grid
+// (column blocks, sets)
+__global__ void sum_queries_kernel(const float *__restrict__ sums, int n_queries, int n, int n_symm, float *__restrict__ out)
 {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    const int c = blockIdx.x * blockDim.x + threadIdx.x, z = blockIdx.y;
     if (c >= n) return;
+    const SetMembers sm = set_members(z, n_symm);
     float t = 0.f;
-    for (int q = 0; q < n_queries; ++q) t += sums[(size_t)q * n + c];
-    out[c] = t;
+    for (int k = 0; k < sm.count; ++k)
+        for (int q = 0; q < n_queries; ++q) t += sums[((size_t)(sm.first + k) * n_queries + q) * n + c];
+    out[(size_t)z * n + c] = t;
 }
 
-// per-query condition columns of layer 0 / skip:  dW[n][c0 + j] = (j < nd ? dW[n][c0 + j] : 0) + scale * sum_q sums[q][n] cond[q][j]
-// (the first nd columns already hold the noise part from the GEMM)
+// per-query condition columns of layer 0 / skip of weight set z:
+//   dW[z][n][c0 + j] = (j < nd ? dW[z][n][c0 + j] : 0) + scale * sum over set z's members m and queries q of sums[m][q][n] cond[m][q][j]
+// (the first nd columns already hold the noise part from the GEMM); grid (blocks of N x cond_dim, sets)
 __global__ void cond_outer_kernel(const float *__restrict__ sums, const float *__restrict__ cond, int n_queries, int N, int cond_dim,
-                                  int nd, float scale, float *__restrict__ dW, int ldw, int c0)
+                                  int nd, int n_symm, float scale, float *__restrict__ dW, int ldw, long long w_stride, int c0)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int z = blockIdx.y;
     if (idx >= (long long)N * cond_dim) return;
     const int n = (int)(idx / cond_dim), j = (int)(idx % cond_dim);
+    const SetMembers sm = set_members(z, n_symm);
     float t = 0.f;
-    for (int q = 0; q < n_queries; ++q) t = fmaf(sums[(size_t)q * N + n], cond[(size_t)q * cond_dim + j], t);
-    float *w = dW + (size_t)n * ldw + c0 + j;
+    for (int k = 0; k < sm.count; ++k)
+        for (int q = 0; q < n_queries; ++q) {
+            const size_t mq = (size_t)(sm.first + k) * n_queries + q;
+            t = fmaf(sums[mq * N + n], cond[mq * cond_dim + j], t);
+        }
+    float *w = dW + (size_t)z * w_stride + (size_t)n * ldw + c0 + j;
     *w = (j < nd ? *w : 0.f) + scale * t;
 }
 
-// what the gradients of one layer need: the forward's workspace and the caller's outputs
+// what the gradients of one layer read from the forward, and the caller's outputs; member strides in bytes
 struct GradTargets {
-    nphm_mlp *h;
-    const Layout *L;
-    const uint8_t *ws;
-    int n_queries, nd;
-    long long n_points;
-    const float *gs;                          // device [scale, 1 / scale] of the adjoints
-    float *const *grad_w, *const *grad_b;
-    bool want_cond;
+    const float *cond = nullptr;                       // [members][queries][cond_dim]
+    const uint8_t *in[kMaxLayers] = {};                // the input of layer l, packed (layer 0: [xyz | noise])
+    int ks_in[kMaxLayers] = {};
+    long long s_in[kMaxLayers] = {};
+    const uint8_t *D2[kMaxLayers] = {}, *H2[kMaxLayers] = {};   // optional second operand pair of dW_l (H2: k-steps and
+    long long sD2[kMaxLayers] = {};                             // member stride of `in`)
+    int n_queries = 0, nd = 0;
+    long long n_points = 0;
+    const float *gs = nullptr;                         // [scale, 1 / scale] of the adjoints, per weight set
+    float *const *grad_w = nullptr, *const *grad_b = nullptr;
+    bool want_cond = false;
 };
 
-// weight, bias and condition-column gradients of layer l from its pre-activation adjoint d (packed, ks k-steps, scaled by
-// gs[0]); with (d2, h2): + d2^T h2 in the weight gradient (a second operand pair over the same rows and k-steps)
-static int layer_grads(const GradTargets &g, int l, const uint8_t *d, int ks, const uint8_t *d2, const uint8_t *h2,
-                       cudaStream_t stream)
+// the targets of a forward in the training layout L
+static GradTargets targets(const StackDims &s, const Layout &L, const uint8_t *ws, int n_queries, long long n_points, int nd,
+                           const float *gs)
 {
-    MlpChain &c = *g.h->chain;
-    const StackDims &s = g.h->dims;
+    GradTargets g;
+    g.cond = reinterpret_cast<const float *>(ws + L.cond);
+    for (int l = 0; l < s.n_lin; ++l) {
+        g.in[l] = l == 0 ? ws + L.x0p : ws + L.hp[l - 1];
+        g.ks_in[l] = l == 0 ? L.ks_x0 : L.ks_h[l - 1];
+    }
+    g.n_queries = n_queries; g.nd = nd; g.n_points = n_points;
+    g.gs = gs;
+    return g;
+}
+
+// weight, bias and condition-column gradients of layer l of every weight set from its pre-activation adjoint d (packed,
+// scaled by the set's gs[2 set]); with D2[l]: + D2^T H2 in the weight gradient (a second operand pair over the same rows)
+static int layer_grads(const Stack &k, const GradTargets &g, int l, const Adjoint &d, cudaStream_t stream)
+{
+    PackedChain &c = k.c;
+    const StackDims &s = k.s;
+    const Members &mb = k.m;
     const long long M = (long long)g.n_queries * g.n_points;
     const int nd = g.nd;
     float *gw = g.grad_w ? g.grad_w[l] : nullptr, *gb = g.grad_b ? g.grad_b[l] : nullptr;
     const bool cond_layer = l == 0 || l == s.skip;
     const float sc = l == s.skip ? chain::kInvSqrt2 : 1.0f;
-    const float *cond = reinterpret_cast<const float *>(g.ws + g.L->cond);
+    const long long wstride = (long long)s.N[l] * s.in_total[l];
     if (gw) {
-        const uint8_t *H = l == 0 ? g.ws + g.L->x0p : g.ws + g.L->hp[l - 1];
-        const int hks = l == 0 ? g.L->ks_x0 : g.L->ks_h[l - 1];
         const int K = l == 0 ? 3 + nd : l == s.skip ? s.N[l - 1] + 3 + nd : s.N[l - 1];
-        int r = wgrad::launch(d, ks, H, hks, M, s.N[l], K, sc, g.gs + 1, gw, s.in_total[l], c.wg_partials, stream, d2, h2);
+        int r = wgrad::launch_sets(d.packed, d.ks, g.in[l], g.ks_in[l], M, s.N[l], K, sc, g.gs + 1, 2, gw, s.in_total[l], wstride,
+                                   mb.sets, mb.n_symm, d.stride, g.s_in[l], g.sD2[l], g.s_in[l], c.partials, stream, g.D2[l], g.H2[l]);
         if (r) return r;
     }
-    float *sums = l == 0 ? c.qsums0.as<float>() : l == s.skip ? c.qsumss.as<float>() : c.qsums.as<float>();
+    float *sums = l == 0 ? c.sums0.as<float>() : l == s.skip ? c.sumss.as<float>() : c.sums.as<float>();
     if (gb || (cond_layer && (gw || g.want_cond))) {
-        query_sums_kernel<<<dim3((unsigned)ks, (unsigned)g.n_queries), 256, 0, stream>>>(d, ks, g.n_points, s.N[l], g.gs, sums);
+        query_sums_kernel<<<dim3((unsigned)d.ks, (unsigned)g.n_queries, (unsigned)mb.count), 256, 0, stream>>>(
+            d.packed, d.ks, d.stride, g.n_points, g.n_queries, s.N[l], g.gs, mb.n_symm, sums);
         NPHM_CUDA_CHECK(cudaGetLastError());
     }
     if (gb) {
-        sum_queries_kernel<<<(unsigned)ceil_div(s.N[l], 128), 128, 0, stream>>>(sums, g.n_queries, s.N[l], gb);
+        sum_queries_kernel<<<dim3((unsigned)ceil_div(s.N[l], 128), (unsigned)mb.sets), 128, 0, stream>>>(sums, g.n_queries, s.N[l],
+                                                                                                          mb.n_symm, gb);
         NPHM_CUDA_CHECK(cudaGetLastError());
     }
     if (cond_layer && gw) {
         const long long total = (long long)s.N[l] * s.cond_dim;
-        cond_outer_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(
-            sums, cond, g.n_queries, s.N[l], s.cond_dim, nd, sc, gw, s.in_total[l], l == 0 ? 3 : s.N[l - 1] + 3);
+        cond_outer_kernel<<<dim3((unsigned)ceil_div(total, 256), (unsigned)mb.sets), 256, 0, stream>>>(
+            sums, g.cond, g.n_queries, s.N[l], s.cond_dim, nd, mb.n_symm, sc, gw, s.in_total[l], wstride,
+            l == 0 ? 3 : s.N[l - 1] + 3);
         NPHM_CUDA_CHECK(cudaGetLastError());
     }
+    return NPHM_OK;
+}
+
+// the per-(member, query) column sums the layer gradients and cond_grad use
+static int reserve_sums(const Stack &k, int n_queries)
+{
+    const StackDims &s = k.s;
+    int max_n = 1, rc;
+    for (int l = 0; l < s.n_lin; ++l) max_n = std::max(max_n, s.N[l]);
+    const size_t mq = (size_t)k.m.count * n_queries;
+    if ((rc = k.c.sums.reserve(mq * max_n * sizeof(float))) || (rc = k.c.sums0.reserve(mq * s.N[0] * sizeof(float))) ||
+        (rc = k.c.sumss.reserve(mq * s.N[s.skip] * sizeof(float))))
+        return rc;
     return NPHM_OK;
 }
 
@@ -791,14 +891,16 @@ extern "C" int nphm_mlp_train_forward(nphm_mlp *h, const float *xyz_dev, const f
     train::stage_x0_kernel<<<(unsigned)ceil_div(M * L.ldx, 256), 256, 0, stream>>>(xyz_dev, cond_noise_dev, noise_dim, M, L.ldx, X0);
     NPHM_CUDA_CHECK(cudaGetLastError());
     train::pack_rows_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128 * 2 * L.ks_x0, 256), 256, 0, stream>>>(
-        X0, L.ldx, 3 + noise_dim, M, L.ks_x0, nullptr, ws + L.x0p);
+        X0, L.ldx, 3 + noise_dim, M, L.ks_x0, 0, nullptr, 0, ws + L.x0p, 0);
     NPHM_CUDA_CHECK(cudaGetLastError());
     NPHM_CUDA_CHECK(cudaMemcpyAsync(ws + L.cond, cond_dev, (size_t)n_queries * s.cond_dim * sizeof(float), cudaMemcpyDeviceToDevice,
                                     stream));
-    uint8_t *Hp[kMaxLayers];
-    float *S[kMaxLayers];
-    for (int l = 0; l + 1 < s.n_lin; ++l) { Hp[l] = ws + L.hp[l]; S[l] = reinterpret_cast<float *>(ws + L.s[l]); }
-    return value_layers(h, M, X0, L.ldx, noise_dim, h->cvec.as<float>(), n_points, Hp, S, out_dev, nullptr, stream);
+    ValueRows v;
+    v.X = X0; v.ldx = L.ldx; v.nd = noise_dim; v.tfwd = h->chain->tfwd;
+    v.bias = h->cvec.as<float>(); v.rows_per_bias = n_points;
+    for (int l = 0; l + 1 < s.n_lin; ++l) { v.Hp[l] = ws + L.hp[l]; v.S[l] = reinterpret_cast<float *>(ws + L.s[l]); }
+    v.out = out_dev;
+    return value_layers(stack(h), M, v, stream);
 }
 
 extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, const void *workspace_dev,
@@ -817,44 +919,42 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
                  "nphm_mlp_train_backward: a workspace of %lld bytes does not hold a training forward of this network at %d x %lld "
                  "points with %d noise columns", workspace_bytes, n_queries, n_points, nd);
     const train::Layout L = train::layout(s, n_queries, n_points, nd);
+    const Stack k = stack(h);
     const long long M = (long long)n_queries * n_points;
     const int last = s.n_lin - 1, out_dim = s.N[last];
 
     // upstream gradient scaled by 2^-e into the packed d_L
     if ((rc = c.gscale.reserve(2 * sizeof(float)))) return rc;
     const float *gs = c.gscale.as<float>();
-    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_out_dev, M * out_dim, nullptr, 0, c.gscale.as<float>());
+    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_out_dev, M * out_dim, nullptr, 0, 0, c.gscale.as<float>());
     NPHM_CUDA_CHECK(cudaGetLastError());
     const int ks_out = (out_dim + 15) / 16;
     if ((rc = c.Dl.reserve(packed_bytes(M, ks_out)))) return rc;
     train::pack_rows_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128 * 2 * ks_out, 256), 256, 0, stream>>>(
-        grad_out_dev, out_dim, out_dim, M, ks_out, gs, c.Dl.as<uint8_t>());
+        grad_out_dev, out_dim, out_dim, M, ks_out, 0, gs, 0, c.Dl.as<uint8_t>(), 0);
     NPHM_CUDA_CHECK(cudaGetLastError());
 
-    int max_ks = 1, max_n = 1;
+    int max_ks = 1;
     for (int l = 1; l <= last; ++l) max_ks = std::max(max_ks, (s.N[l - 1] + 15) / 16);
-    for (int l = 0; l <= last; ++l) max_n = std::max(max_n, s.N[l]);
     for (int i = 0; i < 2; ++i)
         if ((rc = c.Dp[i].reserve(packed_bytes(M, max_ks)))) return rc;
-    if ((rc = c.qsums.reserve((size_t)n_queries * max_n * sizeof(float))) ||
-        (rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
-        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
-        return rc;
+    if ((rc = train::reserve_sums(k, n_queries))) return rc;
     if (grad_xyz_dev && ((rc = c.xtmp.reserve((size_t)M * 4 * sizeof(float))) || (rc = c.xs_tmp.reserve((size_t)M * 4 * sizeof(float)))))
         return rc;
 
-    const train::GradTargets tg{h, &L, ws, n_queries, nd, n_points, gs, grad_w_dev, grad_b_dev, grad_cond_dev != nullptr};
-    auto layer_grads = [&](int l, const uint8_t *d, int ks) { return train::layer_grads(tg, l, d, ks, nullptr, nullptr, stream); };
+    train::GradTargets tg = train::targets(s, L, ws, n_queries, n_points, nd, gs);
+    tg.grad_w = grad_w_dev; tg.grad_b = grad_b_dev; tg.want_cond = grad_cond_dev != nullptr;
+    auto layer_grads = [&](int l, const Adjoint &d) { return train::layer_grads(k, tg, l, d, stream); };
 
     // d_L in Dl, d_l in Dp[l & 1]
     AdjointWalk w;
-    w.top = Adjoint{nullptr, 0, c.Dl.as<uint8_t>(), ks_out};
+    w.top = Adjoint{nullptr, 0, c.Dl.as<uint8_t>(), ks_out, 0};
     for (int l = 0; l < last; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + L.s[l]); w.D[l] = c.Dp[l & 1].as<uint8_t>(); }
     w.xs = grad_xyz_dev ? c.xs_tmp.as<float>() : nullptr;
-    if ((rc = adjoint_walk(h, M, w, layer_grads, stream))) return rc;
+    if ((rc = adjoint_walk(k, M, w, layer_grads, stream))) return rc;
     // the noise does not change the gradient with respect to the condition; one chunk: a fixed summation order
-    if (grad_cond_dev && (rc = cond_grad(h, n_queries, 1, grad_cond_dev, stream))) return rc;
-    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], c.xtmp.as<float>(), w.xs, gs, grad_xyz_dev, stream))) return rc;
+    if (grad_cond_dev && (rc = cond_grad(k, n_queries, 1, grad_cond_dev, stream))) return rc;
+    if (grad_xyz_dev && (rc = xyz_grad(k, M, w.D[0], 0, c.xtmp.as<float>(), w.xs, gs, 2, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
 
@@ -871,50 +971,67 @@ extern "C" int nphm_mlp_train_backward(nphm_mlp *h, const float *grad_out_dev, c
 //             dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1} (one GEMM over both pairs), db_l = sum zb_l, condition and xyz as the
 //             first-order backward does from zb
 // fp16 range: a starts at 2^kGradExp (the unit column), so it spends the chain where an fp16 hi | lo pair keeps its bits;
-// s_bar and g_bar (~1e-5 at the NPM batch) share one device-side power of two sigma that brings their largest magnitude to
-// 2^kGradExp (grad_scale_kernel over both).  The direction is v' = sigma 2^-kGradExp g_bar, so zt' a' and a' ht' carry the same
-// scale sigma as zb': the coupling keeps its plain coefficient 100 and the GEMM adds the two pairs as they are; the fp32
-// epilogues multiply by 1 / sigma.
+// s_bar and g_bar (~1e-5 at the NPM batch) share one device-side power of two sigma per weight set that brings their largest
+// magnitude to 2^kGradExp (grad_scale_kernel over both).  The direction is v' = sigma 2^-kGradExp g_bar, so zt' a' and a' ht'
+// carry the same scale sigma as zb': the coupling keeps its plain coefficient 100 and the GEMM adds the two pairs as they are;
+// the fp32 epilogues multiply by 1 / sigma.
+// Members: the passes run for every member at once (Members), one launch per pass.  A DeepSDF handle is the one-member case;
+// the NPHM ensemble (reference train.py -local) runs its 40 members, each on B queries of N points in its own frame.  A
+// weight set gets its own sigma: through the blend weights, its members' s_bar and g_bar can differ by orders of magnitude
+// from the other sets'; an all-zero set gets scale 1 and exactly zero gradients.
 // Memory: everything per row lives in the caller's workspace, the backward's scratch included (its tail: the tangents, the
 // adjoint ping-pong, the direction), so it is counted and released by the caller's allocator; the handle keeps only
 // buffers of the layer widths (GEMM partials, per-query sums).
 namespace nphm {
 namespace sdfgrad {
 
-// workspace of one forward: the first-order training layout without noise, then the unit column, its scale pair and a_l;
-// then the scratch of the calls: ht_l packed (tg) and zt_l blocked fp32 (zg), the ping-pong of zb (dp), zb_L (dl), the
-// direction as rows of 4 (v4) and packed (vp), and two [M][4] point-gradient temporaries (xa, xb)
+// workspace of one forward and its backward: the per-(member, query) folded constants (cvec, when they do not live on the
+// handle) and condition, one scale pair per weight set (gs) and the forward's (consts), the packed xyz rows (x0p), h_l
+// packed, s_l blocked, the unit column and a_l; then the scratch of the backward: ht_l packed (tg) and zt_l blocked fp32
+// (zg), the ping-pong of zb (dp), zb_L (dl), the direction as rows of 4 (v4) and packed (vp), and two [M][4] point-gradient
+// temporaries (xa, xb).  Every per-row piece holds a whole number of 128-row tiles per member; m_* are the member strides
+// (bytes).
 struct Layout {
-    train::Layout base;
-    size_t unit = 0, consts = 0, a[kMaxLayers] = {}, total = 0;
-    int ks_a[kMaxLayers] = {}, ks_dp = 1;
-    size_t tg[kMaxLayers] = {}, zg[kMaxLayers] = {}, dp[2] = {}, dl = 0, v4 = 0, vp = 0, xa = 0, xb = 0;
+    size_t cvec = 0, cond = 0, gs = 0, consts = 0, x0p = 0, hp[kMaxLayers] = {}, s[kMaxLayers] = {}, unit = 0, a[kMaxLayers] = {};
+    size_t tg[kMaxLayers] = {}, zg[kMaxLayers] = {}, dp[2] = {}, dl = 0, vp = 0, v4 = 0, xa = 0, xb = 0, total = 0;
+    long long m_hp[kMaxLayers] = {}, m_s[kMaxLayers] = {}, m_a[kMaxLayers] = {}, m_dp = 0, m_one = 0, m_row4 = 0;
+    int ks_h[kMaxLayers] = {}, ks_a[kMaxLayers] = {}, ks_dp = 1;
 };
 
-static Layout layout(const StackDims &s, int n_queries, long long n_points)
+static Layout layout(const StackDims &s, const Members &mb, int n_queries, long long n_points, bool with_cvec)
 {
+    const int K = mb.count;
+    const long long Mm = (long long)n_queries * n_points, T = ceil_div(Mm, 128);
     Layout G;
-    G.base = train::layout(s, n_queries, n_points, 0);
-    const long long tiles = ceil_div((long long)n_queries * n_points, 128);
-    Carver w{G.base.total};
-    G.unit = w.take((size_t)tiles * 8192);
+    Carver w;
+    G.cvec = w.take(with_cvec ? (size_t)K * n_queries * s.cvec_stride * sizeof(float) : 0);
+    G.cond = w.take((size_t)K * n_queries * s.cond_dim * sizeof(float));
+    G.gs = w.take((size_t)mb.sets * 2 * sizeof(float));
     G.consts = w.take(2 * sizeof(float));
+    G.m_one = T * 8192;
+    G.m_row4 = Mm * 4 * sizeof(float);
+    G.x0p = w.take((size_t)K * G.m_one);
     for (int l = 0; l + 1 < s.n_lin; ++l) {
+        G.ks_h[l] = (s.N[l] + (l + 1 == s.skip ? 3 : 0) + 15) / 16;
         G.ks_a[l] = (s.N[l] + 15) / 16;
-        G.a[l] = w.take((size_t)tiles * G.ks_a[l] * 8192);
+        G.ks_dp = std::max(G.ks_dp, G.ks_a[l]);
+        G.m_hp[l] = T * G.ks_h[l] * 8192;
+        G.m_s[l] = T * 128 * pad4(s.N[l]) * sizeof(float);
+        G.m_a[l] = T * G.ks_a[l] * 8192;
+        G.hp[l] = w.take((size_t)K * G.m_hp[l]);
+        G.s[l] = w.take((size_t)K * G.m_s[l]);
+        G.a[l] = w.take((size_t)K * G.m_a[l]);
+        G.tg[l] = w.take((size_t)K * G.m_hp[l]);
+        G.zg[l] = w.take((size_t)K * G.m_s[l]);
     }
-    const size_t M = (size_t)n_queries * n_points;
-    for (int l = 0; l + 1 < s.n_lin; ++l) {
-        G.tg[l] = w.take((size_t)tiles * G.base.ks_h[l] * 8192);
-        G.zg[l] = w.take((size_t)tiles * 128 * pad4(s.N[l]) * sizeof(float));
-        G.ks_dp = std::max(G.ks_dp, G.ks_a[l]);                 // zb_l, l < L, in the operand format
-    }
-    for (int i = 0; i < 2; ++i) G.dp[i] = w.take((size_t)tiles * G.ks_dp * 8192);
-    G.dl = w.take((size_t)tiles * 8192);
-    G.vp = w.take((size_t)tiles * 8192);
-    G.v4 = w.take(M * 4 * sizeof(float));
-    G.xa = w.take(M * 4 * sizeof(float));
-    G.xb = w.take(M * 4 * sizeof(float));
+    G.m_dp = T * G.ks_dp * 8192;
+    G.unit = w.take((size_t)K * G.m_one);
+    for (int i = 0; i < 2; ++i) G.dp[i] = w.take((size_t)K * G.m_dp);
+    G.dl = w.take((size_t)K * G.m_one);
+    G.vp = w.take((size_t)K * G.m_one);
+    G.v4 = w.take((size_t)K * G.m_row4);
+    G.xa = w.take((size_t)K * G.m_row4);
+    G.xb = w.take((size_t)K * G.m_row4);
     G.total = w.off;
     return G;
 }
@@ -930,24 +1047,25 @@ __device__ __forceinline__ void store_column0(uint8_t *__restrict__ dst, long lo
     *reinterpret_cast<uint4 *>(d + 4096 + 128) = make_uint4(0, 0, 0, 0);
 }
 
-// packed one-column operand: column 0 = 2^kGradExp on the rows < M, everything else 0; consts = {2^E, 2^-E}.
-// Thread = row of the padded tiles.
-__global__ void unit_column_kernel(long long M, uint8_t *__restrict__ dst, float *__restrict__ consts)
+// packed one-column operand of every member (member m at dst + m stride): column 0 = 2^kGradExp on the rows < M, everything
+// else 0; consts = {2^E, 2^-E}.  grid (row blocks of the padded tiles, members), thread = row.
+__global__ void unit_column_kernel(long long M, uint8_t *__restrict__ dst, long long stride, float *__restrict__ consts)
 {
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r == 0) { consts[0] = ldexpf(1.0f, train::kGradExp); consts[1] = ldexpf(1.0f, -train::kGradExp); }
+    if (r == 0 && blockIdx.y == 0) { consts[0] = ldexpf(1.0f, train::kGradExp); consts[1] = ldexpf(1.0f, -train::kGradExp); }
     if (r >= (M + 127) / 128 * 128) return;
-    store_column0(dst, r, r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
+    store_column0(dst + (size_t)blockIdx.y * stride, r, r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
 }
 
-// V[r] = (g_bar[r] * scale[0] * 2^-kGradExp, 0): the tangent direction, ld 4
-__global__ void direction_kernel(const float *__restrict__ gg, long long M, const float *__restrict__ scale, float *__restrict__ V)
+// V[m][r] = (g_bar[m][r] * scale[2 set(m)] * 2^-kGradExp, 0): the tangent direction, ld 4
+__global__ void direction_kernel(const float *__restrict__ gg, long long M, int members, const float *__restrict__ scale, int n_symm,
+                                 float *__restrict__ V)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= M * 4) return;
+    if (idx >= (long long)members * M * 4) return;
     const long long r = idx >> 2;
-    const int c = (int)(idx & 3);
-    V[idx] = c < 3 ? gg[r * 3 + c] * (scale[0] * ldexpf(1.0f, -train::kGradExp)) : 0.f;
+    const int c = (int)(idx & 3), m = (int)(r / M);
+    V[idx] = c < 3 ? gg[r * 3 + c] * (scale[2 * member_set(m, n_symm)] * ldexpf(1.0f, -train::kGradExp)) : 0.f;
 }
 
 static int ready(nphm_mlp *h, const char *who)
@@ -961,6 +1079,115 @@ static int ready(nphm_mlp *h, const char *who)
     return NPHM_OK;
 }
 
+// s and g = grad_x s of every member at xyz [members][B][N][3]; cond [members][B][cond_dim], cvec the folded constants
+// [members][B][cvec_stride]
+static int forward(const Stack &k, const Layout &G, const float *xyz, const float *cond, const float *cvec, int n_queries,
+                   long long n_points, float *sdf_out, float *grad_out, uint8_t *ws, cudaStream_t stream)
+{
+    const StackDims &s = k.s;
+    const int K = k.m.count;
+    const long long M = (long long)n_queries * n_points, T = ceil_div(M, 128);
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(ws + G.cond, cond, (size_t)K * n_queries * s.cond_dim * sizeof(float), cudaMemcpyDeviceToDevice,
+                                    stream));
+    train::pack_rows_kernel<<<dim3((unsigned)ceil_div(T * 128 * 2, 256), (unsigned)K), 256, 0, stream>>>(
+        xyz, 3, 3, M, 1, M * 3, nullptr, k.m.n_symm, ws + G.x0p, G.m_one);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    // value pass: h_l packed, S_l blocked; the output layer writes s row-major
+    ValueRows v;
+    v.X = xyz; v.sX = M * 3;
+    v.bias = cvec; v.rows_per_bias = n_points; v.sBias = (long long)n_queries * s.cvec_stride;
+    for (int l = 0; l + 1 < s.n_lin; ++l) {
+        v.Hp[l] = ws + G.hp[l]; v.sHp[l] = G.m_hp[l];
+        v.S[l] = reinterpret_cast<float *>(ws + G.s[l]); v.sS[l] = G.m_s[l] / 4;
+    }
+    v.out = sdf_out; v.sOut = M;
+    int rc;
+    if ((rc = value_layers(k, M, v, stream))) return rc;
+    float *consts = reinterpret_cast<float *>(ws + G.consts);
+    unit_column_kernel<<<dim3((unsigned)ceil_div(T * 128, 256), (unsigned)K), 256, 0, stream>>>(M, ws + G.unit, G.m_one, consts);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    // a_{l-1} = S_{l-1} * (a_l W_l) from the unit column down to a_0, kept in the workspace
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, ws + G.unit, 1, G.m_one};
+    for (int l = 0; l + 1 < s.n_lin; ++l) { w.S[l] = v.S[l]; w.sS[l] = v.sS[l]; w.D[l] = ws + G.a[l]; w.sD[l] = G.m_a[l]; }
+    w.xs = reinterpret_cast<float *>(ws + G.xb);
+    if ((rc = adjoint_walk(k, M, w, [](int, const Adjoint &) { return NPHM_OK; }, stream))) return rc;
+    return xyz_grad(k, M, w.D[0], w.sD[0], reinterpret_cast<float *>(ws + G.xa), w.xs, consts, 0, grad_out, stream);
+}
+
+// weight, bias, condition and point gradients of every member from s_bar [members][B][N] and g_bar [members][B][N][3]
+static int backward(const Stack &k, const Layout &G, const float *grad_sdf, const float *grad_grad, uint8_t *ws, int n_queries,
+                    long long n_points, float *const *grad_w, float *const *grad_b, float *grad_cond, float *grad_xyz,
+                    cudaStream_t stream)
+{
+    const StackDims &s = k.s;
+    const Members &mb = k.m;
+    const int K = mb.count, last = s.n_lin - 1;
+    const long long M = (long long)n_queries * n_points, T = ceil_div(M, 128);
+    float *const gs = reinterpret_cast<float *>(ws + G.gs), *const v4 = reinterpret_cast<float *>(ws + G.v4);
+    float *const xa = reinterpret_cast<float *>(ws + G.xa), *const xb = reinterpret_cast<float *>(ws + G.xb);
+
+    // one power of two per weight set for both upstream gradients; zb_L = s_bar packed, the direction as rows and packed
+    train::grad_scale_kernel<<<mb.sets, 1024, 0, stream>>>(grad_sdf, M, grad_grad, M * 3, mb.n_symm, gs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    const dim3 pack_grid((unsigned)ceil_div(T * 128 * 2, 256), (unsigned)K);
+    train::pack_rows_kernel<<<pack_grid, 256, 0, stream>>>(grad_sdf, 1, 1, M, 1, M, gs, mb.n_symm, ws + G.dl, G.m_one);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    direction_kernel<<<(unsigned)ceil_div(K * M * 4, 256), 256, 0, stream>>>(grad_grad, M, K, gs, mb.n_symm, v4);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    train::pack_rows_kernel<<<pack_grid, 256, 0, stream>>>(v4, 4, 3, M, 1, M * 4, nullptr, mb.n_symm, ws + G.vp, G.m_one);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+
+    // tangent pass: ht_l packed (tg, the next layer's input and the GEMM's second H), zt_l blocked fp32 (zg)
+    int rc;
+    for (int l = 0; l < last; ++l) {
+        const tcl::PackedLinear &W = k.c.fwd[l];
+        tcl::LinearParams p;
+        p.M = M; p.batch = K; p.w_pairs = mb.n_symm;
+        if (l == 0) { p.A1 = v4; p.lda1 = 4; p.K1 = 3; p.sA1 = M * 4; }
+        else { p.Ap = ws + G.tg[l - 1]; p.a_ksteps = W.ksteps; p.sAp = G.m_hp[l - 1]; }
+        p.mode = tcl::kModeMult;
+        p.Mul = reinterpret_cast<const float *>(ws + G.s[l]); p.ldmul = k.c.ld[l]; p.mul_div = 1; p.mul_blocked = 1; p.sMul = G.m_s[l] / 4;
+        p.Cp = ws + G.tg[l]; p.c_ksteps = G.ks_h[l]; p.sCp = G.m_hp[l];
+        if (l + 1 == s.skip) { p.app = v4; p.app_ld = 4; p.app_w = 3; p.sApp = M * 4; }
+        p.Dv = reinterpret_cast<float *>(ws + G.zg[l]); p.lddv = k.c.ld[l]; p.dv_blocked = 1; p.sDv = G.m_s[l] / 4;
+        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
+    }
+
+    if ((rc = train::reserve_sums(k, n_queries))) return rc;
+    // dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1}  (a_L: the unit column, ht_{-1}: the direction)
+    train::GradTargets g;
+    g.cond = reinterpret_cast<const float *>(ws + G.cond);
+    for (int l = 0; l <= last; ++l) {
+        g.in[l] = l == 0 ? ws + G.x0p : ws + G.hp[l - 1];
+        g.ks_in[l] = l == 0 ? 1 : G.ks_h[l - 1];
+        g.s_in[l] = l == 0 ? G.m_one : G.m_hp[l - 1];
+        g.D2[l] = l == last ? ws + G.unit : ws + G.a[l];
+        g.sD2[l] = l == last ? G.m_one : G.m_a[l];
+        g.H2[l] = l == 0 ? ws + G.vp : ws + G.tg[l - 1];
+    }
+    g.n_queries = n_queries; g.n_points = n_points;
+    g.gs = gs;
+    g.grad_w = grad_w; g.grad_b = grad_b; g.want_cond = grad_cond != nullptr;
+    auto layer_grads = [&](int l, const Adjoint &d) { return train::layer_grads(k, g, l, d, stream); };
+
+    // value adjoint with the coupling, from zb_L = s_bar (in dl) down to zb_0; zb_l lives in dp[l & 1]
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, ws + G.dl, 1, G.m_one};
+    for (int l = 0; l < last; ++l) {
+        w.S[l] = reinterpret_cast<const float *>(ws + G.s[l]); w.sS[l] = G.m_s[l] / 4;
+        w.D[l] = ws + G.dp[l & 1]; w.sD[l] = G.m_dp;
+        w.cpl_z[l] = reinterpret_cast<const float *>(ws + G.zg[l]);
+        w.cpl_a[l] = ws + G.a[l]; w.sA[l] = G.m_a[l];
+    }
+    w.xs = grad_xyz ? xb : nullptr;
+    if ((rc = adjoint_walk(k, M, w, layer_grads, stream))) return rc;
+    if (grad_cond && (rc = cond_grad(k, n_queries, 1, grad_cond, stream))) return rc;
+    // s_bar g + H v: the point gradient of zb, as in the first-order backward
+    if (grad_xyz && (rc = xyz_grad(k, M, w.D[0], w.sD[0], xa, xb, gs, 2, grad_xyz, stream))) return rc;
+    return NPHM_OK;
+}
+
 }  // namespace sdfgrad
 }  // namespace nphm
 
@@ -970,7 +1197,7 @@ extern "C" long long nphm_mlp_sdfgrad_workspace_bytes(const nphm_mlp *h, int n_q
         set_error("nphm_mlp_sdfgrad_workspace_bytes: bad arguments");
         return -1;
     }
-    return (long long)sdfgrad::layout(h->dims, n_queries, n_points).total;
+    return (long long)sdfgrad::layout(h->dims, Members{}, n_queries, n_points, false).total;
 }
 
 extern "C" int nphm_mlp_sdfgrad_forward(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
@@ -981,22 +1208,10 @@ extern "C" int nphm_mlp_sdfgrad_forward(nphm_mlp *h, const float *xyz_dev, const
     if (rc) return rc;
     NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && sdf_out_dev && grad_out_dev && workspace_dev,
                  "nphm_mlp_sdfgrad_forward: bad arguments");
-    const StackDims &s = h->dims;
-    const sdfgrad::Layout G = sdfgrad::layout(s, n_queries, n_points);
-    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
-    const long long M = (long long)n_queries * n_points;
-    // value pass: the first-order training forward fills the leading part of the workspace
-    if ((rc = nphm_mlp_train_forward(h, xyz_dev, cond_dev, nullptr, 0, n_queries, n_points, sdf_out_dev, ws, stream_))) return rc;
-    float *consts = reinterpret_cast<float *>(ws + G.consts);
-    sdfgrad::unit_column_kernel<<<(unsigned)ceil_div(ceil_div(M, 128) * 128, 256), 256, 0, stream>>>(M, ws + G.unit, consts);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    // a_{l-1} = S_{l-1} * (a_l W_l) from the unit column down to a_0, kept in the workspace
-    AdjointWalk w;
-    w.top = Adjoint{nullptr, 0, ws + G.unit, 1};
-    for (int l = 0; l + 1 < s.n_lin; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + G.base.s[l]); w.D[l] = ws + G.a[l]; }
-    w.xs = reinterpret_cast<float *>(ws + G.xb);
-    if ((rc = adjoint_walk(h, M, w, [](int, const uint8_t *, int) { return NPHM_OK; }, stream))) return rc;
-    return xyz_grad(h, M, w.D[0], reinterpret_cast<float *>(ws + G.xa), w.xs, consts, grad_out_dev, stream);
+    const sdfgrad::Layout G = sdfgrad::layout(h->dims, Members{}, n_queries, n_points, false);
+    if ((rc = mlp_prepare(h, cond_dev, n_queries, stream))) return rc;
+    return sdfgrad::forward(stack(h), G, xyz_dev, cond_dev, h->cvec.as<float>(), n_queries, n_points, sdf_out_dev, grad_out_dev,
+                            static_cast<uint8_t *>(workspace_dev), stream);
 }
 
 extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
@@ -1008,78 +1223,13 @@ extern "C" int nphm_mlp_sdfgrad_backward(nphm_mlp *h, const float *grad_sdf_dev,
     if (rc) return rc;
     NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && grad_sdf_dev && grad_grad_dev && workspace_dev,
                  "nphm_mlp_sdfgrad_backward: bad arguments");
-    MlpChain &c = *h->chain;
-    const StackDims &s = h->dims;
-    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const sdfgrad::Layout G = sdfgrad::layout(h->dims, Members{}, n_queries, n_points, false);
     // the caller states the shape the workspace was made for; checked against its size, without reading it back
-    NPHM_REQUIRE(workspace_bytes == (long long)sdfgrad::layout(s, n_queries, n_points).total,
+    NPHM_REQUIRE(workspace_bytes == (long long)G.total,
                  "nphm_mlp_sdfgrad_backward: a workspace of %lld bytes does not hold an SDF-gradient forward of this network at "
                  "%d x %lld points", workspace_bytes, n_queries, n_points);
-    const sdfgrad::Layout G = sdfgrad::layout(s, n_queries, n_points);
-    const train::Layout &L = G.base;
-    const long long M = (long long)n_queries * n_points, tiles = ceil_div(M, 128);
-    const int last = s.n_lin - 1;
-
-    // one power of two for both upstream gradients; zb_L = s_bar packed, the direction as rows and packed
-    if ((rc = c.gscale.reserve(2 * sizeof(float)))) return rc;
-    const float *gs = c.gscale.as<float>();
-    train::grad_scale_kernel<<<1, 1024, 0, stream>>>(grad_sdf_dev, M, grad_grad_dev, M * 3, c.gscale.as<float>());
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    uint8_t *const dl = ws + G.dl, *const vp = ws + G.vp;
-    float *const v4 = reinterpret_cast<float *>(ws + G.v4);
-    float *const xa = reinterpret_cast<float *>(ws + G.xa), *const xb = reinterpret_cast<float *>(ws + G.xb);
-    auto tg = [&](int l) { return ws + G.tg[l]; };
-    auto zg = [&](int l) { return reinterpret_cast<float *>(ws + G.zg[l]); };
-    const unsigned pack_blocks = (unsigned)ceil_div(tiles * 128 * 2, 256);
-    train::pack_rows_kernel<<<pack_blocks, 256, 0, stream>>>(grad_sdf_dev, 1, 1, M, 1, gs, dl);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    sdfgrad::direction_kernel<<<(unsigned)ceil_div(M * 4, 256), 256, 0, stream>>>(grad_grad_dev, M, gs, v4);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    train::pack_rows_kernel<<<pack_blocks, 256, 0, stream>>>(v4, 4, 3, M, 1, nullptr, vp);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-
-    // tangent pass: ht_l packed (tg, the next layer's input and the GEMM's second H), zt_l blocked fp32 (zg)
-    for (int l = 0; l < last; ++l) {
-        const tcl::PackedLinear &W = c.fwd[l];
-        tcl::LinearParams p;
-        p.M = M;
-        if (l == 0) { p.A1 = v4; p.lda1 = 4; p.K1 = 3; }
-        else { p.Ap = tg(l - 1); p.a_ksteps = W.ksteps; }
-        p.mode = tcl::kModeMult;
-        p.Mul = reinterpret_cast<const float *>(ws + L.s[l]); p.ldmul = c.ld[l]; p.mul_div = 1; p.mul_blocked = 1;
-        p.Cp = tg(l); p.c_ksteps = L.ks_h[l];
-        if (l + 1 == s.skip) { p.app = v4; p.app_ld = 4; p.app_w = 3; }
-        p.Dv = zg(l); p.lddv = c.ld[l]; p.dv_blocked = 1;
-        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
-    }
-
-    int max_n = 1;
-    for (int l = 0; l <= last; ++l) max_n = std::max(max_n, s.N[l]);
-    if ((rc = c.qsums.reserve((size_t)n_queries * max_n * sizeof(float))) ||
-        (rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
-        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
-        return rc;
-    const train::GradTargets targets{h, &L, ws, n_queries, 0, n_points, gs, grad_w_dev, grad_b_dev, grad_cond_dev != nullptr};
-    // dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1}  (a_L: the unit column, ht_{-1}: the direction)
-    auto layer_grads = [&](int l, const uint8_t *d, int ks) {
-        return train::layer_grads(targets, l, d, ks, l == last ? ws + G.unit : ws + G.a[l], l ? tg(l - 1) : vp, stream);
-    };
-
-    // value adjoint with the coupling, from zb_L = s_bar (in dl) down to zb_0; zb_l lives in dp[l & 1]
-    AdjointWalk w;
-    w.top = Adjoint{nullptr, 0, dl, 1};
-    for (int l = 0; l < last; ++l) {
-        w.S[l] = reinterpret_cast<const float *>(ws + L.s[l]);
-        w.D[l] = ws + G.dp[l & 1];
-        w.cpl_z[l] = zg(l);
-        w.cpl_a[l] = ws + G.a[l];
-    }
-    w.xs = grad_xyz_dev ? xb : nullptr;
-    if ((rc = adjoint_walk(h, M, w, layer_grads, stream))) return rc;
-    if (grad_cond_dev && (rc = cond_grad(h, n_queries, 1, grad_cond_dev, stream))) return rc;
-    // s_bar g + H v: the point gradient of zb, as in the first-order backward
-    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], xa, xb, gs, grad_xyz_dev, stream))) return rc;
-    return NPHM_OK;
+    return sdfgrad::backward(stack(h), G, grad_sdf_dev, grad_grad_dev, static_cast<uint8_t *>(workspace_dev), n_queries, n_points,
+                             grad_w_dev, grad_b_dev, grad_cond_dev, grad_xyz_dev, stream);
 }
 
 // ================================================================================================ fitting a one-output stack
@@ -1186,13 +1336,13 @@ extern "C" int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, cons
     if (rc) return rc;
     NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && loss_terms_dev && grad_cond_dev && workspace_dev,
                  "nphm_mlp_fit_surface_grad: bad arguments");
-    MlpChain &c = *h->chain;
     const StackDims &s = h->dims;
     const fitsurf::Layout F = fitsurf::layout(s, n_queries, n_points);
     NPHM_REQUIRE(workspace_bytes == (long long)F.total,
                  "nphm_mlp_fit_surface_grad: a workspace of %lld bytes does not fit this network at %d x %lld points (needs %lld)",
                  workspace_bytes, n_queries, n_points, (long long)F.total);
     uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const Stack k = stack(h);
     const long long M = (long long)n_queries * n_points;
     const int last = s.n_lin - 1;
     float *const sdf = reinterpret_cast<float *>(ws + F.sdf), *const gs = reinterpret_cast<float *>(ws + F.consts);
@@ -1200,40 +1350,27 @@ extern "C" int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, cons
     if ((rc = nphm_mlp_train_forward(h, xyz_dev, cond_dev, nullptr, 0, n_queries, n_points, sdf, ws, stream_))) return rc;
     fitsurf::surface_upstream_kernel<<<1, fitsurf::kThreads, 0, stream>>>(sdf, mask_dev, M, clamp, ws + F.dl, gs, loss_terms_dev);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    if ((rc = c.qsums0.reserve((size_t)n_queries * s.N[0] * sizeof(float))) ||
-        (rc = c.qsumss.reserve((size_t)n_queries * s.N[s.skip] * sizeof(float))))
-        return rc;
-    const train::GradTargets targets{h, &F.base, ws, n_queries, 0, n_points, gs, nullptr, nullptr, true};
+    if ((rc = train::reserve_sums(k, n_queries))) return rc;
+    train::GradTargets tg = train::targets(s, F.base, ws, n_queries, n_points, 0, gs);
+    tg.want_cond = true;
     // no weights or biases: the condition sums at layers 0 and skip
-    auto cond_sums = [&](int l, const uint8_t *d, int ks) { return train::layer_grads(targets, l, d, ks, nullptr, nullptr, stream); };
+    auto cond_sums = [&](int l, const Adjoint &d) { return train::layer_grads(k, tg, l, d, stream); };
 
     // d_{l-1} = s_{l-1} * (d_l W_l) from the packed upstream down to d_0; d_l lives in dp[l & 1]
     AdjointWalk w;
-    w.top = Adjoint{nullptr, 0, ws + F.dl, 1};
+    w.top = Adjoint{nullptr, 0, ws + F.dl, 1, 0};
     for (int l = 0; l < last; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + F.base.s[l]); w.D[l] = ws + F.dp[l & 1]; }
     w.xs = grad_xyz_dev ? xb : nullptr;
-    if ((rc = adjoint_walk(h, M, w, cond_sums, stream))) return rc;
-    if ((rc = cond_grad(h, n_queries, 1, grad_cond_dev, stream))) return rc;           // one chunk: a fixed summation order
-    if (grad_xyz_dev && (rc = xyz_grad(h, M, w.D[0], xa, xb, gs, grad_xyz_dev, stream))) return rc;
+    if ((rc = adjoint_walk(k, M, w, cond_sums, stream))) return rc;
+    if ((rc = cond_grad(k, n_queries, 1, grad_cond_dev, stream))) return rc;           // one chunk: a fixed summation order
+    if (grad_xyz_dev && (rc = xyz_grad(k, M, w.D[0], 0, xa, xb, gs, 2, grad_xyz_dev, stream))) return rc;
     return NPHM_OK;
 }
 
 // ================================================================================================ the NPHM ensemble through grad_x sdf
-// Stage 1 of the ensemble (reference train.py -local): the SDF-gradient passes above for all members at once.  Member k
-// (weight set sigma(k): k / 2 for the 2 n_symm mirrored members, k - n_symm beyond) sees B queries of N points in its own
-// frame; every pass is one launch over all members (tc_linear batched over gridDim.z = member, tc_wgrad over gridDim.z =
-// weight set).  Rows of one member: Mm = B N in Tm = ceil(Mm / 128) tiles; every per-row buffer is member-major with a
-// whole number of tiles per member, so member k's part starts at k times the member stride.  Per-(member, query) bias
-// rows carry the folded condition constants.  fp16 range: one power of two per weight set (its members' s_bar and g_bar
-// can differ by orders of magnitude from the other sets', through the blend weights); an all-zero set gets scale 1 and
-// exactly zero gradients.
+// Stage 1 of the ensemble (reference train.py -local): the SDF-gradient passes above with the ensemble's members.  Member k
+// sees B queries of N points in its own frame; its per-(member, query) bias rows carry the folded condition constants.
 namespace nphm {
-struct EnsembleChain {
-    bool packed = false;
-    tcl::PackedLinear fwd[kMaxLayers], adj[kMaxLayers], adj_x0, adj_xs;     // all weight sets back to back
-    int ld[kMaxLayers];
-    DeviceBuffer partials, sums, sums0, sumss;
-};
 
 void ensemble_chain_destroy(nphm_ensemble *h)
 {
@@ -1243,84 +1380,15 @@ void ensemble_chain_destroy(nphm_ensemble *h)
 
 namespace esdf {
 
-__device__ __forceinline__ int dset(int m, int n_symm) { return m < 2 * n_symm ? m >> 1 : m - n_symm; }
+static Members members(const nphm_ensemble *h) { return Members{h->n_members, h->cfg.n_symm_pairs, h->n_sets}; }
+static Stack stack(nphm_ensemble *h) { return Stack{h->dims, h->weights, *h->sdfgrad, members(h)}; }
 
+// the packed chain of all weight sets, built on the first call after a weight load
 static int pack(nphm_ensemble *h, cudaStream_t stream)
 {
-    if (!h->sdfgrad) h->sdfgrad = new EnsembleChain();
-    EnsembleChain &c = *h->sdfgrad;
-    if (c.packed) return NPHM_OK;
-    const StackDims &s = h->dims;
-    const int S = h->n_sets;
-    int rc;
-    for (int l = 0; l < s.n_lin; ++l) {
-        const float *W = h->weights.W[l].as<float>();
-        const int ldw = s.in_total[l];
-        const long long ws = (long long)s.N[l] * ldw;
-        const float scale = l == s.skip ? chain::kInvSqrt2 : 1.0f;
-        if ((rc = c.fwd[l].pack(W, ldw, s.N[l], s.K[l], 0, 0, false, scale, stream, S, ws, nullptr, 0, l + 1 == s.skip ? 3 : 0,
-                                kChainNt)))
-            return rc;
-        if (l >= 1 && (rc = c.adj[l].pack(W, ldw, s.N[l - 1], s.N[l], 0, 0, true, scale, stream, S, ws, nullptr, 0, 0, kChainNt)))
-            return rc;
-        c.ld[l] = pad4(s.N[l]);
-    }
-    if ((rc = c.adj_x0.pack(h->weights.W[0].as<float>(), s.in_total[0], 3, s.N[0], 0, 0, true, 1.0f, stream, S,
-                            (long long)s.N[0] * s.in_total[0])))
-        return rc;
-    if ((rc = c.adj_xs.pack(h->weights.W[s.skip].as<float>(), s.in_total[s.skip], 3, s.N[s.skip], s.N[s.skip - 1], 0, true,
-                            chain::kInvSqrt2, stream, S, (long long)s.N[s.skip] * s.in_total[s.skip])))
-        return rc;
-    c.packed = true;
-    return NPHM_OK;
-}
-
-// workspace: pieces of all members (member stride m_*) laid out like sdfgrad::Layout, plus the folded constants and the
-// condition of every (member, query) and one scale pair per weight set
-struct Layout {
-    size_t cvec = 0, cond = 0, gs = 0, consts = 0, x0p = 0, hp[kMaxLayers] = {}, s[kMaxLayers] = {}, unit = 0, a[kMaxLayers] = {};
-    size_t tg[kMaxLayers] = {}, zg[kMaxLayers] = {}, dp[2] = {}, dl = 0, vp = 0, v4 = 0, xa = 0, xb = 0, total = 0;
-    long long m_hp[kMaxLayers] = {}, m_s[kMaxLayers] = {}, m_a[kMaxLayers] = {}, m_dp = 0, m_one = 0, m_row4 = 0;
-    int ks_h[kMaxLayers] = {}, ks_a[kMaxLayers] = {}, ks_dp = 1;
-};
-
-static Layout layout(const nphm_ensemble *h, int n_batch, long long n_points)
-{
-    const StackDims &s = h->dims;
-    const int K = h->n_members;
-    const long long Mm = (long long)n_batch * n_points, T = ceil_div(Mm, 128);
-    Layout G;
-    Carver w;
-    G.cvec = w.take((size_t)K * n_batch * s.cvec_stride * sizeof(float));
-    G.cond = w.take((size_t)K * n_batch * s.cond_dim * sizeof(float));
-    G.gs = w.take((size_t)h->n_sets * 2 * sizeof(float));
-    G.consts = w.take(2 * sizeof(float));
-    G.m_one = T * 8192;
-    G.m_row4 = Mm * 4 * sizeof(float);
-    G.x0p = w.take((size_t)K * G.m_one);
-    for (int l = 0; l + 1 < s.n_lin; ++l) {
-        G.ks_h[l] = (s.N[l] + (l + 1 == s.skip ? 3 : 0) + 15) / 16;
-        G.ks_a[l] = (s.N[l] + 15) / 16;
-        G.ks_dp = std::max(G.ks_dp, G.ks_a[l]);
-        G.m_hp[l] = T * G.ks_h[l] * 8192;
-        G.m_s[l] = T * 128 * pad4(s.N[l]) * sizeof(float);
-        G.m_a[l] = T * G.ks_a[l] * 8192;
-        G.hp[l] = w.take((size_t)K * G.m_hp[l]);
-        G.s[l] = w.take((size_t)K * G.m_s[l]);
-        G.a[l] = w.take((size_t)K * G.m_a[l]);
-        G.tg[l] = w.take((size_t)K * G.m_hp[l]);
-        G.zg[l] = w.take((size_t)K * G.m_s[l]);
-    }
-    G.m_dp = T * G.ks_dp * 8192;
-    G.unit = w.take((size_t)K * G.m_one);
-    for (int i = 0; i < 2; ++i) G.dp[i] = w.take((size_t)K * G.m_dp);
-    G.dl = w.take((size_t)K * G.m_one);
-    G.vp = w.take((size_t)K * G.m_one);
-    G.v4 = w.take((size_t)K * G.m_row4);
-    G.xa = w.take((size_t)K * G.m_row4);
-    G.xb = w.take((size_t)K * G.m_row4);
-    G.total = w.off;
-    return G;
+    if (!h->sdfgrad) h->sdfgrad = new PackedChain();
+    if (h->sdfgrad->packed) return NPHM_OK;
+    return pack_chain(*h->sdfgrad, h->dims, h->weights, h->n_sets, stream);
 }
 
 // cvec[k][q][coff_l + n]: b_l[sigma][n], plus at the folded layers scale_l * W_l[sigma][n][K_l:] . cond[k][q], summed in the
@@ -1328,7 +1396,7 @@ static Layout layout(const nphm_ensemble *h, int n_batch, long long n_points)
 // queries), one warp per output row
 __global__ void cvec_kernel(const PackSpec spec, const float *__restrict__ cond, int n_batch, float *__restrict__ cvec)
 {
-    const int m = blockIdx.x, q = blockIdx.y, C = spec.cond_dim, set = dset(m, spec.n_symm);
+    const int m = blockIdx.x, q = blockIdx.y, C = spec.cond_dim, set = member_set(m, spec.n_symm);
     const float *u = cond + ((size_t)m * n_batch + q) * C;
     float *out = cvec + ((size_t)m * n_batch + q) * spec.cvec_stride;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
@@ -1352,159 +1420,6 @@ __global__ void cvec_kernel(const PackSpec spec, const float *__restrict__ cond,
     }
 }
 
-// member-batched train::pack_rows_kernel: member m = blockIdx.y reads src + m src_stride (floats), writes dst + m dst_stride
-// (bytes); scale (optional): the pair of m's weight set, scale[2 sigma(m)]
-__global__ void pack_rows_kernel(const float *__restrict__ src, int ld, int width, long long M, long long src_stride,
-                                 const float *__restrict__ scale, int n_symm, uint8_t *__restrict__ dst, long long dst_stride)
-{
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int m = blockIdx.y;
-    if (idx >= (M + 127) / 128 * 128 * 2) return;
-    const long long row = idx / 2;
-    const int g = (int)(idx % 2);
-    const float sc = scale ? scale[2 * dset(m, n_symm)] : 1.0f;
-    const float *sr = src + (size_t)m * src_stride;
-    float v[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int c = 8 * g + i;
-        v[i] = (row < M && c < width) ? sr[(size_t)row * ld + c] * sc : 0.f;
-    }
-    uint32_t hi[4], lo[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) tc::split2(v[2 * i], v[2 * i + 1], hi[i], lo[i]);
-    uint8_t *d = dst + (size_t)m * dst_stride + (size_t)(row >> 7) * 8192 + (size_t)((row & 127) >> 3) * 256 + g * 128 + (row & 7) * 16;
-    *reinterpret_cast<uint4 *>(d) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    *reinterpret_cast<uint4 *>(d + 4096) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-}
-
-// the unit column of every member (sdfgrad::unit_column_kernel); grid (row blocks, members)
-__global__ void unit_column_kernel(long long M, uint8_t *__restrict__ dst, long long stride, float *__restrict__ consts)
-{
-    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r == 0 && blockIdx.y == 0) { consts[0] = ldexpf(1.0f, train::kGradExp); consts[1] = ldexpf(1.0f, -train::kGradExp); }
-    if (r >= (M + 127) / 128 * 128) return;
-    sdfgrad::store_column0(dst + (size_t)blockIdx.y * stride, r, r < M ? ldexpf(1.0f, train::kGradExp) : 0.f);
-}
-
-// gs[2 z] = 2^(kGradExp - e), gs[2 z + 1] = its inverse, 2^e <= max |.| < 2^(e+1) over the rows of set z's members of s_bar
-// (M per member) and g_bar (3 M); 1 for an all-zero or non-finite set.  One block per set.
-__global__ void set_scale_kernel(const float *__restrict__ gsdf, const float *__restrict__ ggrad, long long M, int n_symm,
-                                 float *__restrict__ gs)
-{
-    __shared__ float red[32];
-    const int z = blockIdx.x;
-    const int m0 = z < n_symm ? 2 * z : z + n_symm, n_mem = z < n_symm ? 2 : 1;
-    float mx = 0.f;
-    for (int k = 0; k < n_mem; ++k) {
-        const float *a = gsdf + (size_t)(m0 + k) * M, *b = ggrad + (size_t)(m0 + k) * M * 3;
-        for (long long i = threadIdx.x; i < M; i += blockDim.x) mx = fmaxf(mx, fabsf(a[i]));
-        for (long long i = threadIdx.x; i < 3 * M; i += blockDim.x) mx = fmaxf(mx, fabsf(b[i]));
-    }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) mx = fmaxf(mx, red[w]);
-        const int e = (mx > 0.f && isfinite(mx)) ? max(-100, min(100, ilogbf(mx))) - train::kGradExp : 0;
-        gs[2 * z] = ldexpf(1.0f, -e);
-        gs[2 * z + 1] = ldexpf(1.0f, e);
-    }
-}
-
-// V[m][r] = (g_bar[m][r] * gs[2 sigma(m)] 2^-kGradExp, 0), ld 4
-__global__ void direction_kernel(const float *__restrict__ gg, long long M, int members, const float *__restrict__ gs, int n_symm,
-                                 float *__restrict__ V)
-{
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (long long)members * M * 4) return;
-    const long long r = idx >> 2;
-    const int c = (int)(idx & 3), m = (int)(r / M);
-    V[idx] = c < 3 ? gg[r * 3 + c] * (gs[2 * dset(m, n_symm)] * ldexpf(1.0f, -train::kGradExp)) : 0.f;
-}
-
-// out[m][r][i] = (a[m][r][i] + b[m][r][i]) * scale[sstride sigma(m) + 1]   (a, b: ld 4)
-__global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__restrict__ b, long long M, int members,
-                                const float *__restrict__ scale, int sstride, int n_symm, float *__restrict__ out)
-{
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (long long)members * M * 3) return;
-    const long long r = idx / 3;
-    const int i = (int)(idx % 3), m = (int)(r / M);
-    out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * scale[sstride * dset(m, n_symm) + 1];
-}
-
-// train::query_sums_kernel over the members (blockIdx.z): out[m][q][c] = gs[2 sigma(m) + 1] * sum over the rows of (m, q)
-__global__ void __launch_bounds__(256) query_sums_kernel(const uint8_t *__restrict__ X, int ks, long long stride, long long n_points,
-                                                         int n_batch, int n_cols, const float *__restrict__ gs, int n_symm,
-                                                         float *__restrict__ out)
-{
-    __shared__ float part[16][17];
-    const int c = threadIdx.x & 15, rl = threadIdx.x >> 4, j = blockIdx.x, q = blockIdx.y, m = blockIdx.z;
-    const uint8_t *Xm = X + (size_t)m * stride;
-    const long long r1 = (long long)(q + 1) * n_points;
-    float s = 0.f;
-    for (long long r = (long long)q * n_points + rl; r < r1; r += 16) {
-        const uint8_t *p = Xm + ((size_t)(r >> 7) * ks + j) * 8192 + (size_t)((r & 127) >> 3) * 256 + (c >> 3) * 128 + (r & 7) * 16 + (c & 7) * 2;
-        s += __half2float(*reinterpret_cast<const __half *>(p)) + __half2float(*reinterpret_cast<const __half *>(p + 4096));
-    }
-    part[rl][c] = s;
-    __syncthreads();
-    if (rl == 0 && j * 16 + c < n_cols) {
-        float t = 0.f;
-        for (int i = 0; i < 16; ++i) t += part[i][c];
-        out[((size_t)m * n_batch + q) * n_cols + j * 16 + c] = t * gs[2 * dset(m, n_symm) + 1];
-    }
-}
-
-// gb[z][c] = sum over the members of set z (in order) and their queries of sums[m][q][c]; grid (column blocks, sets)
-__global__ void bias_grad_kernel(const float *__restrict__ sums, int n_batch, int n, int n_symm, float *__restrict__ gb)
-{
-    const int c = blockIdx.x * blockDim.x + threadIdx.x, z = blockIdx.y;
-    if (c >= n) return;
-    const int m0 = z < n_symm ? 2 * z : z + n_symm, n_mem = z < n_symm ? 2 : 1;
-    float t = 0.f;
-    for (int k = 0; k < n_mem; ++k)
-        for (int q = 0; q < n_batch; ++q) t += sums[((size_t)(m0 + k) * n_batch + q) * n + c];
-    gb[(size_t)z * n + c] = t;
-}
-
-// condition columns of layer 0 / skip: dW[z][n][c0 + j] = scale * sum over set z's members m and queries q of
-// sums[m][q][n] cond[m][q][j]; grid (blocks of N x cond_dim, sets)
-__global__ void cond_outer_kernel(const float *__restrict__ sums, const float *__restrict__ cond, int n_batch, int N, int cond_dim,
-                                  int n_symm, float scale, float *__restrict__ dW, int ldw, long long w_stride, int c0)
-{
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int z = blockIdx.y;
-    if (idx >= (long long)N * cond_dim) return;
-    const int n = (int)(idx / cond_dim), j = (int)(idx % cond_dim);
-    const int m0 = z < n_symm ? 2 * z : z + n_symm, n_mem = z < n_symm ? 2 : 1;
-    float t = 0.f;
-    for (int k = 0; k < n_mem; ++k)
-        for (int q = 0; q < n_batch; ++q) {
-            const size_t mq = (size_t)(m0 + k) * n_batch + q;
-            t = fmaf(sums[mq * N + n], cond[mq * cond_dim + j], t);
-        }
-    dW[(size_t)z * w_stride + (size_t)n * ldw + c0 + j] = scale * t;
-}
-
-// grad_cond[m][q][j] = sum_n W0[sigma][n][3 + j] S0[m][q][n] + sum_n Ws[sigma][n][c0s + j] Ss[m][q][n] / sqrt(2), fixed order;
-// grid (column blocks, queries, members)
-__global__ void cond_grad_kernel(const float *__restrict__ W0, int ld0, int N0, const float *__restrict__ S0,
-                                 const float *__restrict__ Ws, int lds, int Ns, int c0s, const float *__restrict__ Ss, int cond_dim,
-                                 int n_batch, int n_symm, float *__restrict__ out)
-{
-    const int j = blockIdx.x * blockDim.x + threadIdx.x, q = blockIdx.y, m = blockIdx.z, set = dset(m, n_symm);
-    if (j >= cond_dim) return;
-    const size_t mq = (size_t)m * n_batch + q;
-    const float *w0 = W0 + (size_t)set * N0 * ld0, *ws = Ws + (size_t)set * Ns * lds;
-    float s = 0.f, t = 0.f;
-    for (int n = 0; n < N0; ++n) s = fmaf(w0[(size_t)n * ld0 + 3 + j], S0[mq * N0 + n], s);
-    for (int n = 0; n < Ns; ++n) t = fmaf(ws[(size_t)n * lds + c0s + j], Ss[mq * Ns + n], t);
-    out[mq * cond_dim + j] = fmaf(t, chain::kInvSqrt2, s);
-}
-
 static int ready(nphm_ensemble *h, const char *who)
 {
     NPHM_REQUIRE(h && h->loaded, "%s: weights not loaded", who);
@@ -1513,60 +1428,6 @@ static int ready(nphm_ensemble *h, const char *who)
         set_error("%s: needs a one-output stack with its skip below the output layer", who);
         return NPHM_ERR_UNSUPPORTED;
     }
-    return NPHM_OK;
-}
-
-// d_{l-1} = s_{l-1} * (d_l W_l) (+ coupling) over all members, from the packed top (ks 1, member stride top_stride) down to
-// d_0 in D[0]; hook(l, d_l, ks_l, member stride of d_l) before each descent and at the bottom (the adjoint_walk of the
-// layer chain, batched).  xs: optional [members][M][4] skip-layer point gradient.
-template <class Hook>
-static int walk(nphm_ensemble *h, long long Mm, const uint8_t *top, long long top_stride, uint8_t *const *D, const long long *D_stride,
-                const float *const *S, const long long *S_stride, const float *const *cz, const uint8_t *const *ca,
-                const long long *ca_stride, float *xs, Hook &&hook, cudaStream_t stream)
-{
-    EnsembleChain &c = *h->sdfgrad;
-    const StackDims &s = h->dims;
-    const uint8_t *d = top;
-    long long ds = top_stride;
-    int dks = 1, rc;
-    for (int l = s.n_lin - 1; l >= 1; --l) {
-        if ((rc = hook(l, d, dks, ds))) return rc;
-        tcl::LinearParams p0;
-        p0.M = Mm; p0.batch = h->n_members; p0.w_pairs = h->cfg.n_symm_pairs;
-        p0.Ap = d; p0.a_ksteps = dks; p0.sAp = ds;
-        if (l == s.skip && xs) {
-            tcl::LinearParams px = p0;
-            px.mode = tcl::kModeLinear; px.C = xs; px.ldc = 4; px.sC = Mm * 4;
-            if ((rc = tcl::launch_linear(c.adj_xs, px, stream))) return rc;
-        }
-        const int ks = (s.N[l - 1] + 15) / 16;
-        tcl::LinearParams p = p0;
-        p.mode = tcl::kModeMult;
-        p.Mul = S[l - 1]; p.ldmul = c.ld[l - 1]; p.mul_div = 1; p.mul_blocked = 1; p.sMul = S_stride[l - 1] / 4;
-        if (cz) {
-            p.cpl_z = cz[l - 1]; p.sCplZ = S_stride[l - 1] / 4;
-            p.cpl_a = ca[l - 1]; p.sCplA = ca_stride[l - 1]; p.cpl_a_steps = ks; p.cpl_coef = chain::kBeta;
-        }
-        p.Cp = D[l - 1]; p.c_ksteps = ks; p.sCp = D_stride[l - 1];
-        if ((rc = tcl::launch_linear(c.adj[l], p, stream))) return rc;
-        d = D[l - 1]; ds = D_stride[l - 1]; dks = ks;
-    }
-    return hook(0, d, dks, ds);
-}
-
-// the point gradient (d_0 W_0[:, 0:3]^T + xs) * scale[sstride sigma + 1] of every member
-static int xyz_grad(nphm_ensemble *h, long long Mm, const uint8_t *d0, long long d0_stride, float *xa, const float *xs,
-                    const float *scale, int sstride, float *out, cudaStream_t stream)
-{
-    tcl::LinearParams p;
-    p.M = Mm; p.batch = h->n_members; p.w_pairs = h->cfg.n_symm_pairs;
-    p.Ap = d0; p.a_ksteps = (h->dims.N[0] + 15) / 16; p.sAp = d0_stride;
-    p.mode = tcl::kModeLinear; p.C = xa; p.ldc = 4; p.sC = Mm * 4;
-    int rc = tcl::launch_linear(h->sdfgrad->adj_x0, p, stream);
-    if (rc) return rc;
-    xyz_grad_kernel<<<(unsigned)ceil_div(h->n_members * Mm * 3, 256), 256, 0, stream>>>(xa, xs, Mm, h->n_members, scale, sstride,
-                                                                                        h->cfg.n_symm_pairs, out);
-    NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
 
@@ -1579,7 +1440,7 @@ extern "C" long long nphm_ensemble_sdfgrad_workspace_bytes(const nphm_ensemble *
         set_error("nphm_ensemble_sdfgrad_workspace_bytes: bad arguments");
         return -1;
     }
-    return (long long)esdf::layout(h, n_batch, n_points).total;
+    return (long long)sdfgrad::layout(h->dims, esdf::members(h), n_batch, n_points, true).total;
 }
 
 extern "C" int nphm_ensemble_sdfgrad_forward(nphm_ensemble *h, const float *xyz_local_dev, const float *cond_dev, int n_batch,
@@ -1592,49 +1453,13 @@ extern "C" int nphm_ensemble_sdfgrad_forward(nphm_ensemble *h, const float *xyz_
     NPHM_REQUIRE(n_batch >= 1 && n_points >= 1 && xyz_local_dev && cond_dev && sdf_out_dev && grad_out_dev && workspace_dev,
                  "nphm_ensemble_sdfgrad_forward: bad arguments");
     if ((rc = esdf::pack(h, stream))) return rc;
-    EnsembleChain &c = *h->sdfgrad;
-    const StackDims &s = h->dims;
-    const esdf::Layout G = esdf::layout(h, n_batch, n_points);
+    const sdfgrad::Layout G = sdfgrad::layout(h->dims, esdf::members(h), n_batch, n_points, true);
     uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
-    const int K = h->n_members, n_symm = h->cfg.n_symm_pairs;
-    const long long Mm = (long long)n_batch * n_points, T = ceil_div(Mm, 128);
-    float *cvec = reinterpret_cast<float *>(ws + G.cvec), *consts = reinterpret_cast<float *>(ws + G.consts);
-    esdf::cvec_kernel<<<dim3((unsigned)K, (unsigned)n_batch), 256, 0, stream>>>(h->spec, cond_dev, n_batch, cvec);
+    float *cvec = reinterpret_cast<float *>(ws + G.cvec);
+    esdf::cvec_kernel<<<dim3((unsigned)h->n_members, (unsigned)n_batch), 256, 0, stream>>>(h->spec, cond_dev, n_batch, cvec);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    NPHM_CUDA_CHECK(cudaMemcpyAsync(ws + G.cond, cond_dev, (size_t)K * n_batch * s.cond_dim * sizeof(float), cudaMemcpyDeviceToDevice,
-                                    stream));
-    esdf::pack_rows_kernel<<<dim3((unsigned)ceil_div(T * 128 * 2, 256), (unsigned)K), 256, 0, stream>>>(
-        xyz_local_dev, 3, 3, Mm, Mm * 3, nullptr, n_symm, ws + G.x0p, G.m_one);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    // value pass: h_l packed, S_l blocked; the output layer writes s row-major
-    for (int l = 0; l < s.n_lin; ++l) {
-        const tcl::PackedLinear &W = c.fwd[l];
-        tcl::LinearParams p;
-        p.M = Mm; p.batch = K; p.w_pairs = n_symm;
-        if (l == 0) { p.A1 = xyz_local_dev; p.lda1 = 3; p.K1 = 3; p.sA1 = Mm * 3; }
-        else { p.Ap = ws + G.hp[l - 1]; p.a_ksteps = W.ksteps; p.sAp = G.m_hp[l - 1]; }
-        p.bias = cvec + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = n_points; p.sBias = (long long)n_batch * s.cvec_stride;
-        if (l == s.n_lin - 1) {
-            p.mode = tcl::kModeLinear;
-            p.C = sdf_out_dev; p.ldc = 1; p.sC = Mm;
-        } else {
-            p.mode = tcl::kModeSoftplus;
-            p.Cp = ws + G.hp[l]; p.c_ksteps = G.ks_h[l]; p.sCp = G.m_hp[l];
-            if (l + 1 == s.skip) { p.app = xyz_local_dev; p.app_ld = 3; p.app_w = 3; p.sApp = Mm * 3; }
-            p.Dv = reinterpret_cast<float *>(ws + G.s[l]); p.lddv = c.ld[l]; p.dv_blocked = 1; p.sDv = G.m_s[l] / 4;
-        }
-        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
-    }
-    esdf::unit_column_kernel<<<dim3((unsigned)ceil_div(T * 128, 256), (unsigned)K), 256, 0, stream>>>(Mm, ws + G.unit, G.m_one, consts);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    // a_{l-1} = S_{l-1} * (a_l W_l) from the unit column down to a_0
-    uint8_t *A[kMaxLayers];
-    const float *S[kMaxLayers];
-    for (int l = 0; l + 1 < s.n_lin; ++l) { A[l] = ws + G.a[l]; S[l] = reinterpret_cast<const float *>(ws + G.s[l]); }
-    float *xa = reinterpret_cast<float *>(ws + G.xa), *xb = reinterpret_cast<float *>(ws + G.xb);
-    auto none = [](int, const uint8_t *, int, long long) { return NPHM_OK; };
-    if ((rc = esdf::walk(h, Mm, ws + G.unit, G.m_one, A, G.m_a, S, G.m_s, nullptr, nullptr, nullptr, xb, none, stream))) return rc;
-    return esdf::xyz_grad(h, Mm, A[0], G.m_a[0], xa, xb, consts, 0, grad_out_dev, stream);
+    return sdfgrad::forward(esdf::stack(h), G, xyz_local_dev, cond_dev, cvec, n_batch, n_points, sdf_out_dev, grad_out_dev, ws,
+                            stream);
 }
 
 extern "C" int nphm_ensemble_sdfgrad_backward(nphm_ensemble *h, const float *grad_sdf_dev, const float *grad_grad_dev, void *workspace_dev,
@@ -1647,111 +1472,11 @@ extern "C" int nphm_ensemble_sdfgrad_backward(nphm_ensemble *h, const float *gra
     NPHM_REQUIRE(n_batch >= 1 && n_points >= 1 && grad_sdf_dev && grad_grad_dev && workspace_dev,
                  "nphm_ensemble_sdfgrad_backward: bad arguments");
     NPHM_REQUIRE(h->sdfgrad && h->sdfgrad->packed, "nphm_ensemble_sdfgrad_backward: no forward since the last weight load");
+    const sdfgrad::Layout G = sdfgrad::layout(h->dims, esdf::members(h), n_batch, n_points, true);
     // the caller states the shape the workspace was made for; checked against its size, without reading it back
-    NPHM_REQUIRE(workspace_bytes == (long long)esdf::layout(h, n_batch, n_points).total,
+    NPHM_REQUIRE(workspace_bytes == (long long)G.total,
                  "nphm_ensemble_sdfgrad_backward: a workspace of %lld bytes does not hold an SDF-gradient forward of this ensemble "
                  "at %d x %lld points", workspace_bytes, n_batch, n_points);
-    EnsembleChain &c = *h->sdfgrad;
-    const StackDims &s = h->dims;
-    const esdf::Layout G = esdf::layout(h, n_batch, n_points);
-    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
-    const int K = h->n_members, n_symm = h->cfg.n_symm_pairs, n_sets = h->n_sets, last = s.n_lin - 1;
-    const long long Mm = (long long)n_batch * n_points, T = ceil_div(Mm, 128);
-    float *gs = reinterpret_cast<float *>(ws + G.gs);
-    const float *cond = reinterpret_cast<const float *>(ws + G.cond);
-    float *v4 = reinterpret_cast<float *>(ws + G.v4);
-    float *xa = reinterpret_cast<float *>(ws + G.xa), *xb = reinterpret_cast<float *>(ws + G.xb);
-
-    // one power of two per weight set; zb_L = s_bar packed, the direction as rows and packed
-    esdf::set_scale_kernel<<<n_sets, 1024, 0, stream>>>(grad_sdf_dev, grad_grad_dev, Mm, n_symm, gs);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    const dim3 pack_grid((unsigned)ceil_div(T * 128 * 2, 256), (unsigned)K);
-    esdf::pack_rows_kernel<<<pack_grid, 256, 0, stream>>>(grad_sdf_dev, 1, 1, Mm, Mm, gs, n_symm, ws + G.dl, G.m_one);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    esdf::direction_kernel<<<(unsigned)ceil_div(K * Mm * 4, 256), 256, 0, stream>>>(grad_grad_dev, Mm, K, gs, n_symm, v4);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    esdf::pack_rows_kernel<<<pack_grid, 256, 0, stream>>>(v4, 4, 3, Mm, Mm * 4, nullptr, n_symm, ws + G.vp, G.m_one);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-
-    // tangent pass: ht_l packed (tg), zt_l blocked fp32 (zg)
-    for (int l = 0; l < last; ++l) {
-        const tcl::PackedLinear &W = c.fwd[l];
-        tcl::LinearParams p;
-        p.M = Mm; p.batch = K; p.w_pairs = n_symm;
-        if (l == 0) { p.A1 = v4; p.lda1 = 4; p.K1 = 3; p.sA1 = Mm * 4; }
-        else { p.Ap = ws + G.tg[l - 1]; p.a_ksteps = W.ksteps; p.sAp = G.m_hp[l - 1]; }
-        p.mode = tcl::kModeMult;
-        p.Mul = reinterpret_cast<const float *>(ws + G.s[l]); p.ldmul = c.ld[l]; p.mul_div = 1; p.mul_blocked = 1; p.sMul = G.m_s[l] / 4;
-        p.Cp = ws + G.tg[l]; p.c_ksteps = G.ks_h[l]; p.sCp = G.m_hp[l];
-        if (l + 1 == s.skip) { p.app = v4; p.app_ld = 4; p.app_w = 3; p.sApp = Mm * 4; }
-        p.Dv = reinterpret_cast<float *>(ws + G.zg[l]); p.lddv = c.ld[l]; p.dv_blocked = 1; p.sDv = G.m_s[l] / 4;
-        if ((rc = tcl::launch_linear(W, p, stream))) return rc;
-    }
-
-    int max_n = 1;
-    for (int l = 0; l <= last; ++l) max_n = std::max(max_n, s.N[l]);
-    const size_t mq = (size_t)K * n_batch;
-    if ((rc = c.sums.reserve(mq * max_n * sizeof(float))) || (rc = c.sums0.reserve(mq * s.N[0] * sizeof(float))) ||
-        (rc = c.sumss.reserve(mq * s.N[s.skip] * sizeof(float))))
-        return rc;
-    // dW_l = zb_l^T h_{l-1} + a_l^T ht_{l-1} per weight set (a_L: the unit column, ht_{-1}: the direction), db_l, and the
-    // condition columns of layers 0 and skip from the per-(member, query) sums of zb_l
-    auto layer_grads = [&](int l, const uint8_t *d, int ks, long long ds) {
-        float *gw = grad_w_dev ? grad_w_dev[l] : nullptr, *gb = grad_b_dev ? grad_b_dev[l] : nullptr;
-        const bool cond_layer = l == 0 || l == s.skip;
-        const float sc = l == s.skip ? chain::kInvSqrt2 : 1.0f;
-        const long long wstride = (long long)s.N[l] * s.in_total[l];
-        if (gw) {
-            const uint8_t *H = l == 0 ? ws + G.x0p : ws + G.hp[l - 1], *H2 = l == 0 ? ws + G.vp : ws + G.tg[l - 1];
-            const long long sH = l == 0 ? G.m_one : G.m_hp[l - 1];
-            const int hks = l == 0 ? 1 : G.ks_h[l - 1];
-            const int Kc = l == 0 ? 3 : l == s.skip ? s.N[l - 1] + 3 : s.N[l - 1];
-            const uint8_t *D2 = l == last ? ws + G.unit : ws + G.a[l];
-            const long long sD2 = l == last ? G.m_one : G.m_a[l];
-            int r = wgrad::launch_sets(d, ks, H, hks, Mm, s.N[l], Kc, sc, gs + 1, 2, gw, s.in_total[l], wstride, n_sets, n_symm, ds,
-                                       sH, sD2, sH, c.partials, stream, D2, H2);
-            if (r) return r;
-        }
-        float *sums = l == 0 ? c.sums0.as<float>() : l == s.skip ? c.sumss.as<float>() : c.sums.as<float>();
-        if (gb || (cond_layer && (gw || grad_cond_dev))) {
-            esdf::query_sums_kernel<<<dim3((unsigned)ks, (unsigned)n_batch, (unsigned)K), 256, 0, stream>>>(
-                d, ks, ds, n_points, n_batch, s.N[l], gs, n_symm, sums);
-            NPHM_CUDA_CHECK(cudaGetLastError());
-        }
-        if (gb) {
-            esdf::bias_grad_kernel<<<dim3((unsigned)ceil_div(s.N[l], 128), (unsigned)n_sets), 128, 0, stream>>>(sums, n_batch, s.N[l],
-                                                                                                              n_symm, gb);
-            NPHM_CUDA_CHECK(cudaGetLastError());
-        }
-        if (cond_layer && gw) {
-            const long long total = (long long)s.N[l] * s.cond_dim;
-            esdf::cond_outer_kernel<<<dim3((unsigned)ceil_div(total, 256), (unsigned)n_sets), 256, 0, stream>>>(
-                sums, cond, n_batch, s.N[l], s.cond_dim, n_symm, sc, gw, s.in_total[l], wstride, l == 0 ? 3 : s.N[l - 1] + 3);
-            NPHM_CUDA_CHECK(cudaGetLastError());
-        }
-        return NPHM_OK;
-    };
-    // value adjoint with the coupling, from zb_L = s_bar (dl) down to zb_0; zb_l lives in dp[l & 1]
-    uint8_t *D[kMaxLayers];
-    const float *S[kMaxLayers], *Z[kMaxLayers];
-    const uint8_t *A[kMaxLayers];
-    long long D_stride[kMaxLayers];
-    for (int l = 0; l < last; ++l) {
-        D[l] = ws + G.dp[l & 1]; D_stride[l] = G.m_dp;
-        S[l] = reinterpret_cast<const float *>(ws + G.s[l]);
-        Z[l] = reinterpret_cast<const float *>(ws + G.zg[l]);
-        A[l] = ws + G.a[l];
-    }
-    if ((rc = esdf::walk(h, Mm, ws + G.dl, G.m_one, D, D_stride, S, G.m_s, Z, A, G.m_a, grad_xyz_dev ? xb : nullptr, layer_grads,
-                         stream)))
-        return rc;
-    if (grad_cond_dev) {
-        esdf::cond_grad_kernel<<<dim3((unsigned)ceil_div(s.cond_dim, 128), (unsigned)n_batch, (unsigned)K), 128, 0, stream>>>(
-            h->weights.W[0].as<float>(), s.in_total[0], s.N[0], c.sums0.as<float>(), h->weights.W[s.skip].as<float>(),
-            s.in_total[s.skip], s.N[s.skip], s.N[s.skip - 1] + 3, c.sumss.as<float>(), s.cond_dim, n_batch, n_symm, grad_cond_dev);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
-    // s_bar g + H v per member
-    if (grad_xyz_dev && (rc = esdf::xyz_grad(h, Mm, D[0], D_stride[0], xa, xb, gs, 2, grad_xyz_dev, stream))) return rc;
-    return NPHM_OK;
+    return sdfgrad::backward(esdf::stack(h), G, grad_sdf_dev, grad_grad_dev, static_cast<uint8_t *>(workspace_dev), n_batch, n_points,
+                             grad_w_dev, grad_b_dev, grad_cond_dev, grad_xyz_dev, stream);
 }

@@ -178,7 +178,7 @@ __global__ void cvec_kernel(const PackSpec spec, const float *__restrict__ laten
         else u[j] = lat[j];
     }
     __syncthreads();
-    const int set = m < 2 * spec.n_symm ? (m >> 1) : m - spec.n_symm;
+    const int set = member_set(m, spec.n_symm);
     float *out = cvec + ((size_t)qi * spec.n_members + m) * spec.cvec_stride;
     // one warp per output row (coalesced reads of the weight row, shuffle reduction); blockIdx.z strides over the rows
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;

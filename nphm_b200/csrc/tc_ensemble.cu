@@ -74,7 +74,7 @@ __global__ void records_kernel(const float *__restrict__ cvec, int cvec_stride, 
                                const float *__restrict__ anchors, int n_members, int n_symm, float *__restrict__ recs)
 {
     const int m = blockIdx.x, qi = blockIdx.y;
-    const int set = m < 2 * n_symm ? (m >> 1) : m - n_symm;
+    const int set = member_set(m, n_symm);
     const float *cv = cvec + ((size_t)qi * n_members + m) * cvec_stride;
     float *rec = recs + ((size_t)qi * n_members + m) * kRecFloats;
     const int d_in = 3 + kCond;
@@ -112,7 +112,7 @@ __global__ void l2_slab_kernel(const uint8_t *__restrict__ weights, const float 
                                const int *__restrict__ coff, int n_members, int n_symm, uint8_t *__restrict__ out)
 {
     const int m = blockIdx.x, qi = blockIdx.y;
-    const int set = m < 2 * n_symm ? (m >> 1) : m - n_symm;
+    const int set = member_set(m, n_symm);
     const uint4 *src = reinterpret_cast<const uint4 *>(weights + (size_t)set * kSetBytes + kL1Bytes + (size_t)(kKS2 - 1) * kSlabBytes);
     uint8_t *dst = out + ((size_t)qi * n_members + m) * kSlabBytes;
     for (int i = threadIdx.x; i < kSlabBytes / 16; i += blockDim.x) reinterpret_cast<uint4 *>(dst)[i] = src[i];

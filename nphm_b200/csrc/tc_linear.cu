@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearPara
     const long long row0 = (long long)blockIdx.x * 128;
     const int nt_idx = blockIdx.y;
     const int z = blockIdx.z;                             // batch entry: own A / C / Mul / row scale, weights of set(z)
-    const int wset = z < 2 * p.w_pairs ? (z >> 1) : z - p.w_pairs;
+    const int wset = member_set(z, p.w_pairs);
     const int n0 = nt_idx * p.Nt;
 
     TCL_EVT(threadIdx.x == 0, 10, 0);
@@ -529,7 +529,7 @@ int launch_linear(const PackedLinear &w, LinearParams p, cudaStream_t stream)
     NPHM_REQUIRE(p.batch >= 1 && (p.batch == 1 || (!p.A2 && !p.a2_onehot && !p.app_onehot)),
                  "tc_linear: batched launches take no second or one-hot input");
     if (p.batch > 1) {
-        const int last = p.batch - 1, need = (last < 2 * p.w_pairs ? (last >> 1) : last - p.w_pairs) + 1;
+        const int need = member_set(p.batch - 1, p.w_pairs) + 1;
         NPHM_REQUIRE(need <= w.sets, "tc_linear: batch of %d needs %d weight sets, %d packed", p.batch, need, w.sets);
     }
     if (p.a_tile_steps <= 0) p.a_tile_steps = p.a_ksteps;

@@ -59,7 +59,8 @@ __global__ void __launch_bounds__(kThreads) wgrad_kernel(const uint8_t *__restri
 {
     extern __shared__ __align__(128) uint8_t smem[];
     const int nb = blockIdx.x / kb_count, kb = blockIdx.x % kb_count, split = blockIdx.y, set = blockIdx.z;
-    const int m0 = set < mem.w_pairs ? 2 * set : set + mem.w_pairs, n_mem = set < mem.w_pairs ? 2 : 1;
+    const SetMembers sm = set_members(set, mem.w_pairs);
+    const int m0 = sm.first, n_mem = sm.count;
     const int per_mem = D2 ? 2 * row_tiles : row_tiles;
     const int t0 = split * tiles_per_split, t1 = min(n_mem * per_mem, t0 + tiles_per_split);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -194,14 +195,6 @@ int launch_sets(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, 
         partials.as<float>(), splits, ldn, ldk, N, K, scale, inv_scale_dev, inv_stride, dW, ldw, dw_stride);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
-}
-
-int launch(const uint8_t *D, int d_ksteps, const uint8_t *H, int h_ksteps, long long M, int N, int K, float scale,
-           const float *inv_scale_dev, float *dW, int ldw, DeviceBuffer &partials, cudaStream_t stream, const uint8_t *D2,
-           const uint8_t *H2)
-{
-    return launch_sets(D, d_ksteps, H, h_ksteps, M, N, K, scale, inv_scale_dev, 0, dW, ldw, 0, 1, 0, 0, 0, 0, 0, partials, stream,
-                       D2, H2);
 }
 
 }  // namespace wgrad
