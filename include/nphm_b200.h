@@ -333,6 +333,36 @@ int nphm_fit_apply_gradient(nphm_ensemble *h, float *latent_dev, float *adam_m_d
                             const nphm_fit_params *fp, const float *surface_grad_dev, const float *surface_stats_dev,
                             const float *grad_anchors_dev, int apply_update, float *loss_terms_dev, float *grad_out_dev,
                             void *stream);
+
+/* ---- scan-batched fitting: S independent scans (or subjects) in one launch sequence per iteration, each with its own latent
+ * code, Adam moments and points; all scans share fp (schedule, clamp, lr, Adam step).  The result for scan s is what the
+ * single-scan call gives on that scan alone (up to the order of floating-point sums): a scan is reduced only over its own
+ * points, and a scan with nothing kept behaves as the single-scan call does (NaN surface loss, zero surface gradient).
+ * Layouts: points_dev [S][n_points][3], mask_dev [S][n_points] bytes (may be NULL = all valid; rows with mask 0 are left out of
+ * the loss - padding of a shorter scan, which should repeat one of its valid points so that it stays finite), latents_dev /
+ * adam_m_dev / adam_v_dev / grad_out_dev / grad_latent_dev [S][lat_dim], loss_terms_dev [S][8], grad_points_dev [S][n_points][3].
+ * The workspace is the caller's: workspace_bytes (checked, NPHM_ERR_CAPACITY when short) >= nphm_fit_batch_workspace_bytes.
+ * The step and the surface gradient run only on the tensor-core configuration (hidden 200, 4 hidden layers, condition 96):
+ * NPHM_ERR_UNSUPPORTED otherwise.  Nothing is read back from the device. */
+/* bytes of scratch for n_scans scans of n_points observation points each (-1: bad arguments) */
+long long nphm_fit_batch_workspace_bytes(const nphm_ensemble *h, int n_scans, long long n_points);
+/* == nphm_fit_identity_step per scan, with an optional point mask */
+int nphm_fit_identity_step_batched(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
+                                   long long n_points, float *latents_dev, float *adam_m_dev, float *adam_v_dev,
+                                   const nphm_fit_params *fp, int apply_update, float *loss_terms_dev, float *grad_out_dev,
+                                   void *workspace_dev, long long workspace_bytes, void *stream);
+/* == nphm_fit_surface_grad per scan; loss_terms_dev and grad_latent_dev are required */
+int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
+                                  long long n_points, const float *latents_dev, float clamp, float *loss_terms_dev,
+                                  float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, long long workspace_bytes,
+                                  void *stream);
+/* == nphm_fit_apply_gradient per scan: surface_grad_dev [S][lat_dim], surface_stats_dev [S][2], grad_anchors_dev
+ * [S][n_loc*3] (may be NULL), loss_terms_dev [S][8] and grad_out_dev [S][lat_dim] (may be NULL).  Any ensemble configuration;
+ * the scratch is the handle's. */
+int nphm_fit_apply_gradient_batched(nphm_ensemble *h, int n_scans, float *latents_dev, float *adam_m_dev, float *adam_v_dev,
+                                    const nphm_fit_params *fp, const float *surface_grad_dev, const float *surface_stats_dev,
+                                    const float *grad_anchors_dev, int apply_update, float *loss_terms_dev, float *grad_out_dev,
+                                    void *stream);
 /* torch.optim.Adam.step() (lr, betas 0.9/0.999, eps 1e-8) on a dense fp32 tensor: the expression codes of the joint fitter
  * (reference src/NPHM/models/fitting.py:36,169).  step is the 1-based step count. */
 int nphm_adam_step(float *param_dev, const float *grad_dev, float *adam_m_dev, float *adam_v_dev, long long n, float lr,

@@ -31,6 +31,8 @@ EXPORTED_SYMBOLS = (
     'nphm_mlp_query_layers', 'nphm_mlp_jacobian', 'nphm_mlp_backward_inputs', 'nphm_mlp_inverse_jacobian', 'nphm_adam_step',
     'nphm_mc_workspace_bytes', 'nphm_mc_count', 'nphm_mc_emit', 'nphm_marching_cubes_host',
     'nphm_fit_workspace_bytes', 'nphm_fit_identity_step', 'nphm_fit_surface_grad', 'nphm_fit_apply_gradient',
+    'nphm_fit_batch_workspace_bytes', 'nphm_fit_identity_step_batched', 'nphm_fit_surface_grad_batched',
+    'nphm_fit_apply_gradient_batched',
     'nphm_ensemble_backward_inputs', 'nphm_ensemble_anchors',
     'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
@@ -146,6 +148,14 @@ def lib() -> ctypes.CDLL:
                                                 c_void_p, c_void_p]
     L.nphm_fit_apply_gradient.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(FitParams), c_void_p, c_void_p,
                                           c_void_p, c_int, c_void_p, c_void_p, c_void_p]
+    L.nphm_fit_batch_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong]
+    L.nphm_fit_batch_workspace_bytes.restype = c_longlong
+    L.nphm_fit_identity_step_batched.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p,
+                                                 POINTER(FitParams), c_int, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_fit_surface_grad_batched.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_float, c_void_p,
+                                                c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_fit_apply_gradient_batched.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, POINTER(FitParams), c_void_p,
+                                                  c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
     L.nphm_adam_step.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_float, c_int, c_void_p]
     L.nphm_mlp_inverse_jacobian.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p]
     L.nphm_broyden_workspace_bytes.argtypes = [c_longlong]

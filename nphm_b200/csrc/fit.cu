@@ -51,10 +51,16 @@ struct Weights {
     const float *pos_w[3], *pos_b[3], *mean_anchors;
 };
 
+// Scan-batched calls (nphm_fit_*_batched) fit S independent scans of n points each in one launch sequence.  Point rows are
+// [scan][n] (points, mask, member_s, out, S, gsign, grad_points); the tensor-core buffers (acts, the upstream gradients, the
+// packed deltas) are [member][scan][tile][128]: every scan owns whole 128-row tiles.  The per-point kernels run on grids whose
+// y index (or tile) is the scan, so no CTA straddles two scans.  Per-scan accumulators: acc [scan][member][2H], blend_acc and
+// ganch [scan][n_loc * 3], stats [scan][8], grad [scan][lat_dim]; anchors / cvec come per scan from ensemble_prepare.
 struct Buffers {
-    const float *points;            // n x 3
-    long long n;
-    const float *anchors;           // n_loc x 3
+    const float *points;            // S x n x 3
+    long long n;                    // points per scan
+    long long tiles_per_scan;       // ceil(n / 128)
+    const float *anchors;           // S x n_loc x 3
     const float *cvec;              // [members][cvec_stride]
     float *member_s;                // n x members
     const unsigned char *mask;      // optional n: 0 = the point is excluded from the loss (joint fitter: failed correspondences)
@@ -230,14 +236,16 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
                                                            long long gs_stride)
 {
     __shared__ float s_anch[64 * 3], s_acc[64 * 3];
-    const int lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < d.n_loc * 3; i += blockDim.x) { s_anch[i] = b.anchors[i]; s_acc[i] = 0.f; }
+    const int lane = threadIdx.x & 31, scan = blockIdx.y;
+    for (int i = threadIdx.x; i < d.n_loc * 3; i += blockDim.x) { s_anch[i] = b.anchors[(size_t)scan * d.n_loc * 3 + i]; s_acc[i] = 0.f; }
     __syncthreads();
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool ok = idx < b.n;
+    const long long i_scan = (long long)blockIdx.x * blockDim.x + threadIdx.x;     // point of the scan
+    const long long idx = scan * b.n + i_scan;                                     // row of the point arrays
+    const bool ok = i_scan < b.n;
     float x = 0.f, y = 0.f, z = 0.f, g_out = 0.f, Sp = 1.f, outv = 0.f;
     if (ok) {
-        const float inv_count = b.stats[0] > 0.f ? 1.0f / b.stats[0] : 0.f;
+        const float *stats = b.stats + (size_t)scan * 8;
+        const float inv_count = stats[0] > 0.f ? 1.0f / stats[0] : 0.f;
         x = b.points[idx * 3]; y = b.points[idx * 3 + 1]; z = b.points[idx * 3 + 2];
         g_out = lambda_surface * b.gsign[idx] * inv_count;
         Sp = b.S[idx] + 1e-6f;
@@ -266,7 +274,7 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
                 c[0] = coef * dx; c[1] = coef * dy; c[2] = coef * dz;
                 gx[0] -= c[0]; gx[1] -= c[1]; gx[2] -= c[2];                  // d w_k / d x = - d w_k / d a_k
             }
-            gs[(size_t)m * gs_stride + idx] = gsv;
+            gs[(size_t)m * gs_stride + scan * b.tiles_per_scan * 128 + i_scan] = gsv;
         }
         if (has_anchor) {
 #pragma unroll
@@ -281,7 +289,7 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
     if (ok && b.grad_points) { b.grad_points[idx * 3] = gx[0]; b.grad_points[idx * 3 + 1] = gx[1]; b.grad_points[idx * 3 + 2] = gx[2]; }
     __syncthreads();
     for (int i = threadIdx.x; i < d.n_loc * 3; i += blockDim.x)
-        if (s_acc[i] != 0.f) atomicAdd(b.blend_acc + i, s_acc[i]);
+        if (s_acc[i] != 0.f) atomicAdd(b.blend_acc + (size_t)scan * d.n_loc * 3 + i, s_acc[i]);
 }
 
 // one CTA per (128-point tile, member): g_s-weighted sums of delta0 / delta2 over the points (-> acc) and (POINTS) the gradient
@@ -308,12 +316,13 @@ __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d
     const int g = warp & 3, ch = warp >> 2, r8 = lane >> 2, pr = lane & 3;
     const int m = blockIdx.y;
     const int set = m < 2 * d.n_symm ? (m >> 1) : m - d.n_symm;
-    const long long row0 = (long long)blockIdx.x * 128;
+    const int scan = (int)(blockIdx.x / b.tiles_per_scan);
+    const long long row0 = ((long long)blockIdx.x - scan * b.tiles_per_scan) * 128;      // first point of the tile in its scan
     for (int i = threadIdx.x; i < 2 * kStepsH * 16; i += blockDim.x) (&s_sum[0][0])[i] = 0.f;
-    // upstream gradient of s_m per point (zero beyond the last point: the padding rows of a tile hold garbage)
+    // upstream gradient of s_m per point (zero beyond the scan's last point: the padding rows of a tile hold garbage)
     if (threadIdx.x < 128) {
         const long long row = row0 + threadIdx.x;
-        s_up[threadIdx.x] = row < b.n ? gs[(size_t)m * tiles * 128 + row] * (1.0f / kDeltaScale) : 0.f;
+        s_up[threadIdx.x] = row < b.n ? gs[((size_t)m * tiles + blockIdx.x) * 128 + threadIdx.x] * (1.0f / kDeltaScale) : 0.f;
     }
     if (POINTS) {
         const int in0 = 3 + d.C;
@@ -386,11 +395,11 @@ __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d
             float v = s_g[0][pt][a] + s_g[1][pt][a];
             if (a == 0 && mirror) v = -v;
             const long long row = row0 + pt;
-            if (row < b.n && v != 0.f) atomicAdd(b.grad_points + row * 3 + a, v);
+            if (row < b.n && v != 0.f) atomicAdd(b.grad_points + (scan * b.n + row) * 3 + a, v);
         }
     }
     __syncthreads();
-    float *acc = b.acc + (size_t)m * 2 * d.H;
+    float *acc = b.acc + ((size_t)scan * d.n_members + m) * 2 * d.H;
     for (int i = threadIdx.x; i < 2 * d.H; i += blockDim.x) {
         const float v = i < d.H ? s_sum[0][i] : s_sum[1][i - d.H];          // acc = [sum delta0 | sum delta2]
         if (v != 0.f) atomicAdd(acc + i, v);
@@ -400,15 +409,18 @@ __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d
 // sdf = sum_k w_k s_k / (sum_k w_k + 1e-6); kept = |sdf| < clamp   (fitting.py:234-246)
 __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
 {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int scan = blockIdx.y;
+    const long long i_scan = (long long)blockIdx.x * blockDim.x + threadIdx.x;     // point of the scan
+    const long long idx = scan * b.n + i_scan;                                     // row of the point arrays
+    const float *anchors = b.anchors + (size_t)scan * d.n_loc * 3;
     float cnt = 0.f, sum = 0.f;
-    if (idx < b.n) {
+    if (i_scan < b.n) {
         const float x = b.points[idx * 3], y = b.points[idx * 3 + 1], z = b.points[idx * 3 + 2];
         float num = 0.f, den = 0.f;
         for (int k = 0; k < d.n_members; ++k) {
             float dd;
             if (k < d.n_loc) {
-                const float dx = b.anchors[k * 3] - x, dy = b.anchors[k * 3 + 1] - y, dz = b.anchors[k * 3 + 2] - z;
+                const float dx = anchors[k * 3] - x, dy = anchors[k * 3 + 1] - y, dz = anchors[k * 3 + 2] - z;
                 const float nrm = sqrtf(dx * dx + dy * dy + dz * dz) + 10e-6f;
                 dd = -(nrm * nrm);
             } else {
@@ -425,7 +437,7 @@ __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
         if (b.upstream) {
             // plain vector-Jacobian product: the "loss" is sum_p upstream_p * sdf_p (count fixed to 1 so nothing is averaged)
             b.gsign[idx] = (!b.mask || b.mask[idx]) ? b.upstream[idx] : 0.f;
-            if (idx == 0) cnt = 1.f;
+            if (i_scan == 0) cnt = 1.f;
             sum = b.gsign[idx] * out;
         } else {
             const bool kept = l < clamp && (!b.mask || b.mask[idx]);
@@ -438,17 +450,19 @@ __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
         cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
         sum += __shfl_xor_sync(0xffffffffu, sum, o);
     }
-    if ((threadIdx.x & 31) == 0 && (cnt != 0.f || sum != 0.f)) { atomicAdd(b.stats + 0, cnt); atomicAdd(b.stats + 1, sum); }
+    float *stats = b.stats + (size_t)scan * 8;
+    if ((threadIdx.x & 31) == 0 && (cnt != 0.f || sum != 0.f)) { atomicAdd(stats + 0, cnt); atomicAdd(stats + 1, sum); }
 }
 
 // per member: g_u = W0u^T D0 + W2u^T D2 / sqrt2 ; g_c = W0x^T D0 + W2x^T D2 / sqrt2
-// block = 128 columns x kGradSlices slices of the hidden index (partial sums through shared memory)
+// block = 128 columns x kGradSlices slices of the hidden index (partial sums through shared memory); grid (members, scans)
 constexpr int kGradSlices = 4;
 __global__ void __launch_bounds__(128 * kGradSlices) fit_member_grad_kernel(const Dims d, const Weights w, const Buffers b)
 {
-    const int m = blockIdx.x;
+    const int m = blockIdx.x, scan = blockIdx.y;
     const int set = m < 2 * d.n_symm ? (m >> 1) : m - d.n_symm;
-    const float *D0 = b.acc + (size_t)m * 2 * d.H, *D2 = D0 + d.H;
+    const float *D0 = b.acc + ((size_t)scan * d.n_members + m) * 2 * d.H, *D2 = D0 + d.H;
+    float *grad = b.grad + (size_t)scan * d.lat_dim;
     const int in0 = 3 + d.C, in2 = d.H;                 // row lengths of W0 / W2 in the reference layout
     const float *W0 = w.W[0] + (size_t)set * d.H * in0;
     const float *W2 = w.W[2] + (size_t)set * d.H * in2;
@@ -477,8 +491,8 @@ __global__ void __launch_bounds__(128 * kGradSlices) fit_member_grad_kernel(cons
             if (j < 3) gc[j] = g;
             else {
                 const int u = j - 3;
-                if (u < d.G) atomicAdd(b.grad + u, g);
-                else b.grad[d.G + m * d.Lc + (u - d.G)] = g;
+                if (u < d.G) atomicAdd(grad + u, g);
+                else grad[d.G + m * d.Lc + (u - d.G)] = g;
             }
         }
         __syncthreads();
@@ -487,7 +501,8 @@ __global__ void __launch_bounds__(128 * kGradSlices) fit_member_grad_kernel(cons
         const bool mirror = (m & 1) && m < 2 * d.n_symm;
         // c = x - a (x component negated for mirrored members)  =>  d c / d a = -1 (+1 for the mirrored x)
         const float sign = (threadIdx.x == 0 && mirror) ? 1.0f : -1.0f;
-        b.ganch[m * 3 + threadIdx.x] = b.blend_acc[m * 3 + threadIdx.x] + sign * gc[threadIdx.x];
+        const size_t a = (size_t)scan * d.n_loc * 3 + m * 3 + threadIdx.x;
+        b.ganch[a] = b.blend_acc[a] + sign * gc[threadIdx.x];
     }
 }
 
@@ -497,12 +512,21 @@ struct FinalizeArgs {
     int apply_update;
 };
 
-// mlp_pos backward (anchor gradient -> z_glob), regularisers (fitting.py:252-268), loss terms, Adam
+// mlp_pos backward (anchor gradient -> z_glob), regularisers (fitting.py:252-268), loss terms, Adam; one CTA per scan (the
+// latent, Adam moments, loss terms and gradient outputs are [scan][...])
 __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const Weights w, const Buffers b, float *latent,
                                                            float *adam_m, float *adam_v, const FinalizeArgs a,
                                                            float *loss_terms, float *grad_out)
 {
     extern __shared__ float sh[];
+    const int scan = blockIdx.x;
+    latent += (size_t)scan * d.lat_dim;
+    if (adam_m) adam_m += (size_t)scan * d.lat_dim;
+    if (adam_v) adam_v += (size_t)scan * d.lat_dim;
+    if (loss_terms) loss_terms += (size_t)scan * 8;
+    if (grad_out) grad_out += (size_t)scan * d.lat_dim;
+    float *const grad = b.grad + (size_t)scan * d.lat_dim;
+    const float *const ganch = b.ganch + (size_t)scan * d.n_loc * 3, *const stats = b.stats + (size_t)scan * 8;
     float *h0 = sh, *h1 = h0 + d.pos_hid, *g1 = h1 + d.pos_hid, *g0 = g1 + d.pos_hid, *red = g0 + d.pos_hid;
     const int tid = threadIdx.x, nt = blockDim.x;
     const int Hd = d.pos_hid, G = d.G, O = d.n_loc * 3;
@@ -549,9 +573,9 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
             __syncthreads();
         }
     };
-    matvec_t(w.pos_w[2], Hd, O, Hd, b.ganch, [&](int j, float t) { g1[j] = h1[j] > 0.f ? t : 0.f; });
+    matvec_t(w.pos_w[2], Hd, O, Hd, ganch, [&](int j, float t) { g1[j] = h1[j] > 0.f ? t : 0.f; });
     matvec_t(w.pos_w[1], Hd, Hd, Hd, g1, [&](int j, float t) { g0[j] = h0[j] > 0.f ? t : 0.f; });
-    matvec_t(w.pos_w[0], G, Hd, G, g0, [&](int j, float t) { b.grad[j] += t; });
+    matvec_t(w.pos_w[0], G, Hd, G, g0, [&](int j, float t) { grad[j] += t; });
     // regularisers
     float part[4] = {0.f, 0.f, 0.f, 0.f};        // reg_global, reg_loc, reg_unobserved, (unused)
     const int unobs[3] = {30, 31, 39};
@@ -564,7 +588,7 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
             const int k = (j - G) / d.Lc;
             if (k == unobs[0] || k == unobs[1] || k == unobs[2]) { part[2] += zj * zj; g += a.lambda_reg_unobserved * 2.f * zj; }
         }
-        b.grad[j] += g;
+        grad[j] += g;
     }
     for (int i = 0; i < 3; ++i) {
         float v = part[i];
@@ -585,8 +609,8 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
         if (nrm > 0.f) {
             for (int j = tid & 31; j < d.Lc; j += 32) {
                 const float g = a.lambda_symm_dist * (za[j] - zb[j]) / (nrm * d.n_symm);
-                b.grad[G + (2 * pair) * d.Lc + j] += g;
-                b.grad[G + (2 * pair + 1) * d.Lc + j] -= g;
+                grad[G + (2 * pair) * d.Lc + j] += g;
+                grad[G + (2 * pair + 1) * d.Lc + j] -= g;
             }
         }
         if ((tid & 31) == 0) symm_local += nrm;
@@ -596,15 +620,15 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
     if (tid == 0 && loss_terms) {
         float rg = 0.f, rl = 0.f, ru = 0.f, sy = 0.f;
         for (int wi = 0; wi < nt / 32; ++wi) { rg += red[wi]; rl += red[32 + wi]; ru += red[64 + wi]; sy += red[96 + wi]; }
-        loss_terms[0] = b.stats[1] / b.stats[0];      // surface = mean |sdf| over kept points (NaN if none, like torch)
+        loss_terms[0] = stats[1] / stats[0];      // surface = mean |sdf| over kept points (NaN if none, like torch)
         loss_terms[1] = rg; loss_terms[2] = rl; loss_terms[3] = ru;
         loss_terms[4] = d.n_symm ? sy / d.n_symm : 0.f;
-        loss_terms[5] = b.stats[0];
+        loss_terms[5] = stats[0];
     }
     __syncthreads();
     // Adam (torch 2.x single-tensor update order)
     for (int j = tid; j < d.lat_dim; j += nt) {
-        const float g = b.grad[j];
+        const float g = grad[j];
         if (grad_out) grad_out[j] = g;
         if (a.apply_update) {
             float mm = adam_m[j], vv = adam_v[j];
@@ -643,6 +667,10 @@ int backward_packs(nphm_ensemble *h, cudaStream_t stream)
     h->fit_packs = bp;
     return NPHM_OK;
 }
+// fit_finalize_kernel over n_scans scans with the Adam constants of fp
+int launch_finalize(const Dims &d, const Weights &w, const Buffers &b, int n_scans, float *latent_dev, float *adam_m_dev,
+                    float *adam_v_dev, const nphm_fit_params *fp, int apply_update, float *loss_terms_dev, float *grad_out_dev,
+                    cudaStream_t stream);
 }}
 namespace nphm {
 void fit_packs_destroy(nphm_ensemble *h)
@@ -652,29 +680,43 @@ void fit_packs_destroy(nphm_ensemble *h)
 }
 }
 
-extern "C" long long nphm_fit_workspace_bytes(const nphm_ensemble *h, long long n_points)
+extern "C" long long nphm_fit_batch_workspace_bytes(const nphm_ensemble *h, int n_scans, long long n_points)
 {
-    if (!h || n_points < 0) return -1;
-    long long floats = n_points * (h->n_members + 3) + (long long)h->n_members * 2 * h->cfg.hidden_dim +
-                       (long long)h->cfg.n_loc * 6 + 8 + h->lat_dim;
-    // activation derivatives handed from the tensor-core forward to the backward GEMMs ([member][tile][kActLd][128], layers 0-2) and the upstream gradient of every member output ([member][rows])
-    const long long tiles = (n_points + 127) / 128;
+    if (!h || n_scans < 1 || n_points < 0) return -1;
+    const long long S = n_scans;
+    long long floats = S * (n_points * (h->n_members + 3) + (long long)h->n_members * 2 * h->cfg.hidden_dim +
+                            (long long)h->cfg.n_loc * 6 + 8 + h->lat_dim);
+    // activation derivatives handed from the tensor-core forward to the backward GEMMs ([member][tile][kActLd][128], layers 0-2) and the upstream gradient of every member output ([member][rows]); every scan owns whole tiles
+    const long long tiles = S * ((n_points + 127) / 128);
     floats += (long long)h->n_members * tiles * 128 * (nphm::tc::kActLd + 1);
     // operand-ready (packed) sigma'3 / deltas of the backward GEMMs
     return floats * 4 + (long long)h->n_members * tiles * nphm::fit::kPackedPerTile * 8192 + 1024;
 }
 
-static int fit_step_impl(nphm_ensemble *h, const float *points_dev, long long n_points, float *latent_dev,
+extern "C" long long nphm_fit_workspace_bytes(const nphm_ensemble *h, long long n_points)
+{
+    return nphm_fit_batch_workspace_bytes(h, 1, n_points);
+}
+
+// One fitting step for n_scans scans of n_points each (layouts: fit::Buffers).  workspace_bytes < 0: the single-scan entry
+// points, whose workspace is unsized (NULL = the handle's scratch).
+static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans, long long n_points, float *latent_dev,
                          float *adam_m_dev, float *adam_v_dev, const nphm_fit_params *fp, int apply_update,
                          float *loss_terms_dev, float *grad_out_dev, const unsigned char *mask_dev, float *grad_points_dev,
-                         void *workspace_dev, void *stream_, const float *upstream_dev = nullptr, float *sdf_out_dev = nullptr)
+                         void *workspace_dev, long long workspace_bytes, void *stream_, const float *upstream_dev = nullptr,
+                         float *sdf_out_dev = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     NPHM_REQUIRE(h && h->loaded, "nphm_fit_identity_step: weights not loaded");
-    NPHM_REQUIRE(points_dev && latent_dev && fp && n_points > 0, "nphm_fit_identity_step: NULL argument or no points");
+    NPHM_REQUIRE(points_dev && latent_dev && fp && n_points > 0 && n_scans >= 1, "nphm_fit_identity_step: NULL argument or no points");
     NPHM_REQUIRE(!apply_update || (adam_m_dev && adam_v_dev), "nphm_fit_identity_step: Adam state is NULL");
     if (h->dims.n_lin != 5 || h->dims.skip != 2) {
         set_error("nphm_fit_identity_step: only ensembles with 4 hidden layers are supported");
+        return NPHM_ERR_UNSUPPORTED;
+    }
+    const bool tc_path = tc_ensemble_supported(h) && h->tc_ready;
+    if (n_scans > 1 && !tc_path) {
+        set_error("scan-batched fitting needs the tensor-core configuration (hidden 200, 4 layers, condition 96)");
         return NPHM_ERR_UNSUPPORTED;
     }
     fit::Dims d{};
@@ -698,23 +740,31 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, long long n_
     w.mean_anchors = h->mean_anchors.as<float>();
 
     int rc;
+    const long long need = nphm_fit_batch_workspace_bytes(h, n_scans, n_points);
     float *ws = static_cast<float *>(workspace_dev);
+    if (workspace_bytes >= 0 && workspace_bytes < need) {
+        set_error("fitting workspace too small: %lld bytes for %d scans of %lld points, %lld needed", workspace_bytes, n_scans,
+                  n_points, need);
+        return NPHM_ERR_CAPACITY;
+    }
     if (!ws) {
-        if ((rc = h->fit_scratch.reserve((size_t)nphm_fit_workspace_bytes(h, n_points)))) return rc;
+        if ((rc = h->fit_scratch.reserve((size_t)need))) return rc;
         ws = h->fit_scratch.as<float>();
     }
-    if ((rc = ensemble_prepare(h, latent_dev, 1, stream))) return rc;      // anchors + folded constants
+    if ((rc = ensemble_prepare(h, latent_dev, n_scans, stream))) return rc;      // per-scan anchors + folded constants
+    const long long S = n_scans, rows_total = S * ceil_div(n_points, 128) * 128;    // rows of all tiles of all scans
     fit::Buffers b{};
-    b.points = points_dev; b.n = n_points; b.anchors = h->anchors.as<float>(); b.cvec = h->cvec.as<float>();
+    b.points = points_dev; b.n = n_points; b.tiles_per_scan = ceil_div(n_points, 128);
+    b.anchors = h->anchors.as<float>(); b.cvec = h->cvec.as<float>();
     float *p = ws;
-    b.member_s = p; p += n_points * h->n_members;
-    b.out = p; p += n_points; b.S = p; p += n_points; b.gsign = p; p += n_points;
+    b.member_s = p; p += S * n_points * h->n_members;
+    b.out = p; p += S * n_points; b.S = p; p += S * n_points; b.gsign = p; p += S * n_points;
     float *zero_begin = p;
-    b.acc = p; p += (size_t)h->n_members * 2 * d.H;
-    b.blend_acc = p; p += d.n_loc * 3;
-    b.stats = p; p += 8;
-    b.ganch = p; p += d.n_loc * 3;
-    b.grad = p; p += d.lat_dim;
+    b.acc = p; p += S * h->n_members * 2 * d.H;
+    b.blend_acc = p; p += S * d.n_loc * 3;
+    b.stats = p; p += S * 8;
+    b.ganch = p; p += S * d.n_loc * 3;
+    b.grad = p; p += S * d.lat_dim;
     NPHM_CUDA_CHECK(cudaMemsetAsync(zero_begin, 0, (size_t)(p - zero_begin) * sizeof(float), stream));
     p += (4 - ((p - ws) & 3)) & 3;                                  // 16-byte alignment of the activation block
     float *acts = p;
@@ -728,41 +778,41 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, long long n_
     dim3 grid(tiles, h->n_members);
     NPHM_CUDA_CHECK(cudaFuncSetAttribute(fit::fit_member_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     NPHM_CUDA_CHECK(cudaFuncSetAttribute(fit::fit_member_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (tc_ensemble_supported(h) && h->tc_ready) {
-        // forward pass on the tensor-core kernel: member outputs s_k -> member_s (the blended output is recomputed by
-        // fit_blend_kernel together with the loss bookkeeping)
+    if (tc_path) {
+        // forward pass on the tensor-core kernel, one query per scan: member outputs s_k -> member_s (the blended output is
+        // recomputed by fit_blend_kernel together with the loss bookkeeping)
         SimtQuery q{};
-        q.xyz = points_dev; q.first = 0; q.total = n_points; q.n_points = n_points; q.n_queries = 1; q.quirk_period = 0;
+        q.xyz = points_dev; q.first = 0; q.total = n_points; q.n_points = n_points; q.n_queries = n_scans; q.quirk_period = 0;
         q.cvec = h->cvec.as<float>(); q.anchors = h->anchors.as<float>(); q.blend = 1;
         q.out = b.out; q.members_out = b.member_s; q.exact = 1;
         q.acts_out = acts;
-        {
-            const long long rows = ceil_div(n_points, 128) * 128;
-            q.acts_packed_out = reinterpret_cast<unsigned char *>(acts + (size_t)h->n_members * rows * (tc::kActLd + 1));
-            // sigma'3 lands in the first kStepsH k-steps of every (member, tile) block of kPackedPerTile k-steps
-            q.acts_packed_tile_steps = fit::kPackedPerTile;
-        }
+        q.acts_packed_out = reinterpret_cast<unsigned char *>(acts + (size_t)h->n_members * rows_total * (tc::kActLd + 1));
+        // sigma'3 lands in the first kStepsH k-steps of every (member, tile) block of kPackedPerTile k-steps
+        q.acts_packed_tile_steps = fit::kPackedPerTile;
         if ((rc = tc_ensemble_launch(h, q, stream))) return rc;
         b.acts = acts;
     } else {
         fit::fit_member_kernel<false><<<grid, fit::kThreads, smem, stream>>>(d, w, b, fp->lambda_surface);
         NPHM_CUDA_CHECK(cudaGetLastError());
     }
-    fit::fit_blend_kernel<<<(unsigned)ceil_div(n_points, 128), 128, 0, stream>>>(d, b, fp->clamp);
+    fit::fit_blend_kernel<<<dim3((unsigned)ceil_div(n_points, 128), n_scans), 128, 0, stream>>>(d, b, fp->clamp);
     NPHM_CUDA_CHECK(cudaGetLastError());
     if (b.acts) {
-        const long long rows = ceil_div(n_points, 128) * 128, n_tiles = rows / 128;
-        float *gs = acts + (size_t)h->n_members * rows * tc::kActLd;
-        uint8_t *packed = reinterpret_cast<uint8_t *>(gs + (size_t)h->n_members * rows);
+        const long long n_tiles = rows_total / 128;
+        float *gs = acts + (size_t)h->n_members * rows_total * tc::kActLd;
+        uint8_t *packed = reinterpret_cast<uint8_t *>(gs + (size_t)h->n_members * rows_total);
         if ((rc = fit::backward_packs(h, stream))) return rc;
         const fit::BackwardPacks &bp = *h->fit_packs;
-        fit::fit_upstream_kernel<<<(unsigned)ceil_div(n_points, 256), 256, 0, stream>>>(d, b, fp->lambda_surface, gs, rows);
+        fit::fit_upstream_kernel<<<dim3((unsigned)ceil_div(n_points, 256), n_scans), 256, 0, stream>>>(d, b, fp->lambda_surface, gs,
+                                                                                                       rows_total);
         NPHM_CUDA_CHECK(cudaGetLastError());
         // per (member, tile): packed [sigma'3 -> delta2 (13 k-steps) | delta1 (7) | delta0 (13)], blocked fp32 sigma'0 | sigma'1 | sigma'2
         uint8_t *p32 = packed, *p1 = packed + (size_t)fit::kStepsH * 8192, *p0 = p1 + (size_t)fit::kStepsN1 * 8192;
         tcl::LinearParams lp{};
-        lp.M = n_points; lp.mode = tcl::kModeMult; lp.batch = h->n_members; lp.w_pairs = d.n_symm;
-        lp.mul_blocked = 1; lp.ldmul = tc::kActLd; lp.sMul = rows * tc::kActLd;
+        // the GEMM rows are those of all tiles, up to the last point of the last scan (the rows are independent; the padding
+        // rows between two scans carry finite activations of a clamped point and a zero upstream gradient)
+        lp.M = rows_total - b.tiles_per_scan * 128 + n_points; lp.mode = tcl::kModeMult; lp.batch = h->n_members; lp.w_pairs = d.n_symm;
+        lp.mul_blocked = 1; lp.ldmul = tc::kActLd; lp.sMul = rows_total * tc::kActLd;
         lp.sAp = lp.sCp = (long long)n_tiles * fit::kPackedPerTile * 8192;
         // strides between the tiles of one member: tc_linear indexes packed tiles with a_ksteps / c_ksteps, so a tile pitch of
         // kPackedPerTile k-steps is expressed through those counts
@@ -787,31 +837,28 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, long long n_
         fit::fit_member_kernel<true><<<grid, fit::kThreads, smem, stream>>>(d, w, b, fp->lambda_surface);
     }
     NPHM_CUDA_CHECK(cudaGetLastError());
-    fit::fit_member_grad_kernel<<<h->n_members, 128 * fit::kGradSlices, 0, stream>>>(d, w, b);
+    fit::fit_member_grad_kernel<<<dim3(h->n_members, n_scans), 128 * fit::kGradSlices, 0, stream>>>(d, w, b);
     NPHM_CUDA_CHECK(cudaGetLastError());
-
-    fit::FinalizeArgs a{};
-    a.lambda_surface = fp->lambda_surface; a.lambda_reg_global = fp->lambda_reg_global; a.lambda_reg_loc = fp->lambda_reg_loc;
-    a.lambda_reg_unobserved = fp->lambda_reg_unobserved; a.lambda_symm_dist = fp->lambda_symm_dist;
-    const double beta1 = 0.9, beta2 = 0.999;
-    const int step = fp->step > 0 ? fp->step : 1;
-    const double bc1 = 1.0 - std::pow(beta1, step), bc2 = 1.0 - std::pow(beta2, step);
-    a.step_size = (float)((double)fp->lr / bc1);
-    a.bc2_sqrt = (float)std::sqrt(bc2);
-    a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
-    a.eps = 1e-8f; a.apply_update = apply_update;
-    const size_t fsm = (size_t)(4 * d.pos_hid + 128 + 1024) * sizeof(float);
-    fit::fit_finalize_kernel<<<1, 1024, fsm, stream>>>(d, w, b, latent_dev, adam_m_dev, adam_v_dev, a, loss_terms_dev, grad_out_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return NPHM_OK;
+    return fit::launch_finalize(d, w, b, n_scans, latent_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
+                                grad_out_dev, stream);
 }
 
 extern "C" int nphm_fit_identity_step(nphm_ensemble *h, const float *points_dev, long long n_points, float *latent_dev,
                                       float *adam_m_dev, float *adam_v_dev, const nphm_fit_params *fp, int apply_update,
                                       float *loss_terms_dev, float *grad_out_dev, void *workspace_dev, void *stream)
 {
-    return fit_step_impl(h, points_dev, n_points, latent_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
-                         grad_out_dev, nullptr, nullptr, workspace_dev, stream);
+    return fit_step_impl(h, points_dev, 1, n_points, latent_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
+                         grad_out_dev, nullptr, nullptr, workspace_dev, -1, stream);
+}
+
+static nphm_fit_params surface_params(float clamp)
+{
+    nphm_fit_params fp{};
+    fp.lambda_surface = 1.0f;           // the regularisers of the latent code stay with the caller
+    fp.clamp = clamp;
+    fp.lr = 0.f;
+    fp.step = 1;
+    return fp;
 }
 
 extern "C" int nphm_fit_surface_grad(nphm_ensemble *h, const float *points_dev, long long n_points, const float *latent_dev,
@@ -819,13 +866,45 @@ extern "C" int nphm_fit_surface_grad(nphm_ensemble *h, const float *points_dev, 
                                      float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, void *stream)
 {
     NPHM_REQUIRE(grad_latent_dev, "nphm_fit_surface_grad: grad_latent_dev is NULL");
-    nphm_fit_params fp{};
-    fp.lambda_surface = 1.0f;           // the regularisers of the latent code stay with the caller
-    fp.clamp = clamp;
-    fp.lr = 0.f;
-    fp.step = 1;
-    return fit_step_impl(h, points_dev, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, loss_terms_dev,
-                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, stream);
+    const nphm_fit_params fp = surface_params(clamp);
+    return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, loss_terms_dev,
+                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream);
+}
+
+// the scan-batched entry points run only on the tensor-core path (no batched FFMA fallback)
+static int require_batched(nphm_ensemble *h, const char *what, int n_scans, const void *workspace_dev)
+{
+    NPHM_REQUIRE(h && h->loaded, "%s: weights not loaded", what);
+    NPHM_REQUIRE(n_scans >= 1 && workspace_dev, "%s: n_scans < 1 or NULL workspace", what);
+    if (!(tc_ensemble_supported(h) && h->tc_ready)) {
+        set_error("%s: needs the tensor-core configuration (hidden 200, 4 layers, condition 96)", what);
+        return NPHM_ERR_UNSUPPORTED;
+    }
+    return NPHM_OK;
+}
+
+extern "C" int nphm_fit_identity_step_batched(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
+                                              long long n_points, float *latents_dev, float *adam_m_dev, float *adam_v_dev,
+                                              const nphm_fit_params *fp, int apply_update, float *loss_terms_dev,
+                                              float *grad_out_dev, void *workspace_dev, long long workspace_bytes, void *stream)
+{
+    int rc;
+    if ((rc = require_batched(h, "nphm_fit_identity_step_batched", n_scans, workspace_dev))) return rc;
+    return fit_step_impl(h, points_dev, n_scans, n_points, latents_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
+                         grad_out_dev, mask_dev, nullptr, workspace_dev, workspace_bytes, stream);
+}
+
+extern "C" int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
+                                             long long n_points, const float *latents_dev, float clamp, float *loss_terms_dev,
+                                             float *grad_latent_dev, float *grad_points_dev, void *workspace_dev,
+                                             long long workspace_bytes, void *stream)
+{
+    int rc;
+    if ((rc = require_batched(h, "nphm_fit_surface_grad_batched", n_scans, workspace_dev))) return rc;
+    NPHM_REQUIRE(loss_terms_dev && grad_latent_dev, "nphm_fit_surface_grad_batched: NULL loss terms or gradient");
+    const nphm_fit_params fp = surface_params(clamp);
+    return fit_step_impl(h, points_dev, n_scans, n_points, const_cast<float *>(latents_dev), nullptr, nullptr, &fp, 0,
+                         loss_terms_dev, grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, workspace_bytes, stream);
 }
 
 // Vector-Jacobian product of the ensemble forward w.r.t. its inputs (SURVEY.md 8b: nphm_ensemble_backward_inputs):
@@ -838,25 +917,22 @@ extern "C" int nphm_ensemble_backward_inputs(nphm_ensemble *h, const float *poin
                                              float *grad_points_dev, void *workspace_dev, void *stream)
 {
     NPHM_REQUIRE(grad_sdf_dev && grad_latent_dev, "nphm_ensemble_backward_inputs: NULL gradient pointer");
-    nphm_fit_params fp{};
-    fp.lambda_surface = 1.0f;
-    fp.clamp = 0.f;
-    fp.lr = 0.f;
-    fp.step = 1;
-    return fit_step_impl(h, points_dev, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, nullptr,
-                         grad_latent_dev, nullptr, grad_points_dev, workspace_dev, stream, grad_sdf_dev, sdf_out_dev);
+    const nphm_fit_params fp = surface_params(0.f);
+    return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, nullptr,
+                         grad_latent_dev, nullptr, grad_points_dev, workspace_dev, -1, stream, grad_sdf_dev, sdf_out_dev);
 }
 
 // ------------------------------------------------------------------------------------------------ sharded fitting
 namespace nphm { namespace fit {
+// per scan: grad = lambda g, ganch = lambda ganch_in, stats[0..1] = stats_in[0..1]   (g [S][n], ganch_in [S][n_anch], stats_in [S][2])
 __global__ void load_external_gradient_kernel(const float *__restrict__ g, const float *__restrict__ stats_in, float lambda,
-                                              int n, float *__restrict__ grad, float *__restrict__ stats,
+                                              int n, int n_scans, float *__restrict__ grad, float *__restrict__ stats,
                                               const float *__restrict__ ganch_in, int n_anch, float *__restrict__ ganch)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) grad[i] = lambda * g[i];
-    if (ganch_in && i < n_anch) ganch[i] = lambda * ganch_in[i];
-    if (i == 0) { stats[0] = stats_in[0]; stats[1] = stats_in[1]; }
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < (long long)n_scans * n) grad[i] = lambda * g[i];
+    if (ganch_in && i < (long long)n_scans * n_anch) ganch[i] = lambda * ganch_in[i];
+    if (i < n_scans) { stats[i * 8] = stats_in[i * 2]; stats[i * 8 + 1] = stats_in[i * 2 + 1]; }
 }
 
 // torch.optim.Adam (betas 0.9 / 0.999, eps 1e-8, no weight decay; torch 2.x single-tensor update order) on a dense tensor
@@ -873,43 +949,12 @@ __global__ void adam_dense_kernel(float *__restrict__ param, const float *__rest
     param[i] = param[i] - step_size * (mm / denom);
     m[i] = mm; v[i] = vv;
 }
-}}
 
-// Second half of a fitting iteration when the surface term was evaluated elsewhere - e.g. on the shards of a point-sharded
-// fit (nphm_b200/distributed.py: every rank calls nphm_fit_surface_grad on its points, ONE all-reduce combines
-// [n_r * grad_r, n_r * loss_r, n_r], then every rank calls this with the identical global mean gradient): adds the
-// regularisers of fitting.py:252-268 and applies the Adam update exactly like nphm_fit_identity_step.
-// surface_grad_dev: d(mean |sdf| over the kept points)/d latent (lat_dim, un-weighted); surface_stats_dev: [n_kept, sum |sdf|].
-extern "C" int nphm_fit_apply_gradient(nphm_ensemble *h, float *latent_dev, float *adam_m_dev, float *adam_v_dev,
-                                       const nphm_fit_params *fp, const float *surface_grad_dev, const float *surface_stats_dev,
-                                       const float *grad_anchors_dev, int apply_update, float *loss_terms_dev,
-                                       float *grad_out_dev, void *stream_)
+int launch_finalize(const Dims &d, const Weights &w, const Buffers &b, int n_scans, float *latent_dev, float *adam_m_dev,
+                    float *adam_v_dev, const nphm_fit_params *fp, int apply_update, float *loss_terms_dev, float *grad_out_dev,
+                    cudaStream_t stream)
 {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    NPHM_REQUIRE(h && h->loaded, "nphm_fit_apply_gradient: weights not loaded");
-    NPHM_REQUIRE(latent_dev && adam_m_dev && adam_v_dev && fp && surface_grad_dev && surface_stats_dev,
-                 "nphm_fit_apply_gradient: NULL argument");
-    fit::Dims d{};
-    d.n_members = h->n_members; d.n_symm = h->cfg.n_symm_pairs; d.n_loc = h->cfg.n_loc;
-    d.H = h->cfg.hidden_dim; d.N1 = h->dims.N[1]; d.C = h->dims.cond_dim; d.G = h->cfg.lat_dim_glob; d.Lc = h->cfg.lat_dim_loc;
-    d.lat_dim = h->lat_dim; d.pos_hid = h->cfg.pos_mlp_dim; d.cvec_stride = h->dims.cvec_stride;
-    fit::Weights w{};
-    for (int i = 0; i < 3; ++i) { w.pos_w[i] = h->pos_w[i].as<float>(); w.pos_b[i] = h->pos_b[i].as<float>(); }
-    w.mean_anchors = h->mean_anchors.as<float>();
-    int rc;
-    const size_t floats = (size_t)d.n_loc * 3 + 8 + d.lat_dim;
-    if ((rc = h->fit_apply_scratch.reserve(floats * sizeof(float)))) return rc;
-    float *p = h->fit_apply_scratch.as<float>();
-    fit::Buffers b{};
-    b.ganch = p; p += d.n_loc * 3;           // zero unless the caller brings an anchor gradient of its own (joint fitter)
-    b.stats = p; p += 8;
-    b.grad = p;
-    NPHM_CUDA_CHECK(cudaMemsetAsync(h->fit_apply_scratch.ptr, 0, floats * sizeof(float), stream));
-    fit::load_external_gradient_kernel<<<(d.lat_dim + 255) / 256, 256, 0, stream>>>(surface_grad_dev, surface_stats_dev,
-                                                                                   fp->lambda_surface, d.lat_dim, b.grad, b.stats,
-                                                                                   grad_anchors_dev, d.n_loc * 3, b.ganch);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    fit::FinalizeArgs a{};
+    FinalizeArgs a{};
     a.lambda_surface = fp->lambda_surface; a.lambda_reg_global = fp->lambda_reg_global; a.lambda_reg_loc = fp->lambda_reg_loc;
     a.lambda_reg_unobserved = fp->lambda_reg_unobserved; a.lambda_symm_dist = fp->lambda_symm_dist;
     const double beta1 = 0.9, beta2 = 0.999;
@@ -920,9 +965,68 @@ extern "C" int nphm_fit_apply_gradient(nphm_ensemble *h, float *latent_dev, floa
     a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
     a.eps = 1e-8f; a.apply_update = apply_update;
     const size_t fsm = (size_t)(4 * d.pos_hid + 128 + 1024) * sizeof(float);
-    fit::fit_finalize_kernel<<<1, 1024, fsm, stream>>>(d, w, b, latent_dev, adam_m_dev, adam_v_dev, a, loss_terms_dev, grad_out_dev);
+    fit_finalize_kernel<<<n_scans, 1024, fsm, stream>>>(d, w, b, latent_dev, adam_m_dev, adam_v_dev, a, loss_terms_dev, grad_out_dev);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
+}
+}}
+
+static int apply_gradient_impl(nphm_ensemble *h, int n_scans, float *latent_dev, float *adam_m_dev, float *adam_v_dev,
+                               const nphm_fit_params *fp, const float *surface_grad_dev, const float *surface_stats_dev,
+                               const float *grad_anchors_dev, int apply_update, float *loss_terms_dev, float *grad_out_dev,
+                               void *stream_)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    NPHM_REQUIRE(h && h->loaded, "nphm_fit_apply_gradient: weights not loaded");
+    NPHM_REQUIRE(n_scans >= 1 && latent_dev && adam_m_dev && adam_v_dev && fp && surface_grad_dev && surface_stats_dev,
+                 "nphm_fit_apply_gradient: NULL argument or n_scans < 1");
+    fit::Dims d{};
+    d.n_members = h->n_members; d.n_symm = h->cfg.n_symm_pairs; d.n_loc = h->cfg.n_loc;
+    d.H = h->cfg.hidden_dim; d.N1 = h->dims.N[1]; d.C = h->dims.cond_dim; d.G = h->cfg.lat_dim_glob; d.Lc = h->cfg.lat_dim_loc;
+    d.lat_dim = h->lat_dim; d.pos_hid = h->cfg.pos_mlp_dim; d.cvec_stride = h->dims.cvec_stride;
+    fit::Weights w{};
+    for (int i = 0; i < 3; ++i) { w.pos_w[i] = h->pos_w[i].as<float>(); w.pos_b[i] = h->pos_b[i].as<float>(); }
+    w.mean_anchors = h->mean_anchors.as<float>();
+    int rc;
+    const size_t floats = (size_t)n_scans * (d.n_loc * 3 + 8 + d.lat_dim);
+    if ((rc = h->fit_apply_scratch.reserve(floats * sizeof(float)))) return rc;
+    float *p = h->fit_apply_scratch.as<float>();
+    fit::Buffers b{};
+    b.ganch = p; p += (size_t)n_scans * d.n_loc * 3;     // zero unless the caller brings an anchor gradient of its own (joint fitter)
+    b.stats = p; p += (size_t)n_scans * 8;
+    b.grad = p;
+    NPHM_CUDA_CHECK(cudaMemsetAsync(h->fit_apply_scratch.ptr, 0, floats * sizeof(float), stream));
+    const long long n_threads = (long long)n_scans * (d.lat_dim > d.n_loc * 3 ? d.lat_dim : d.n_loc * 3);
+    fit::load_external_gradient_kernel<<<(unsigned)((n_threads + 255) / 256), 256, 0, stream>>>(
+        surface_grad_dev, surface_stats_dev, fp->lambda_surface, d.lat_dim, n_scans, b.grad, b.stats, grad_anchors_dev, d.n_loc * 3,
+        b.ganch);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return fit::launch_finalize(d, w, b, n_scans, latent_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev, grad_out_dev,
+                                stream);
+}
+
+// Second half of a fitting iteration when the surface term was evaluated elsewhere - e.g. on the shards of a point-sharded
+// fit (nphm_b200/distributed.py: every rank calls nphm_fit_surface_grad on its points, ONE all-reduce combines
+// [n_r * grad_r, n_r * loss_r, n_r], then every rank calls this with the identical global mean gradient): adds the
+// regularisers of fitting.py:252-268 and applies the Adam update exactly like nphm_fit_identity_step.
+// surface_grad_dev: d(mean |sdf| over the kept points)/d latent (lat_dim, un-weighted); surface_stats_dev: [n_kept, sum |sdf|].
+extern "C" int nphm_fit_apply_gradient(nphm_ensemble *h, float *latent_dev, float *adam_m_dev, float *adam_v_dev,
+                                       const nphm_fit_params *fp, const float *surface_grad_dev, const float *surface_stats_dev,
+                                       const float *grad_anchors_dev, int apply_update, float *loss_terms_dev,
+                                       float *grad_out_dev, void *stream)
+{
+    return apply_gradient_impl(h, 1, latent_dev, adam_m_dev, adam_v_dev, fp, surface_grad_dev, surface_stats_dev, grad_anchors_dev,
+                               apply_update, loss_terms_dev, grad_out_dev, stream);
+}
+
+// The same for n_scans independent scans sharing fp (schedule, lr, Adam step): every argument gains a leading scan axis.
+extern "C" int nphm_fit_apply_gradient_batched(nphm_ensemble *h, int n_scans, float *latents_dev, float *adam_m_dev,
+                                               float *adam_v_dev, const nphm_fit_params *fp, const float *surface_grad_dev,
+                                               const float *surface_stats_dev, const float *grad_anchors_dev, int apply_update,
+                                               float *loss_terms_dev, float *grad_out_dev, void *stream)
+{
+    return apply_gradient_impl(h, n_scans, latents_dev, adam_m_dev, adam_v_dev, fp, surface_grad_dev, surface_stats_dev,
+                               grad_anchors_dev, apply_update, loss_terms_dev, grad_out_dev, stream);
 }
 
 // torch.optim.Adam.step() on a dense fp32 tensor (reference src/NPHM/models/fitting.py:36,169: the expression codes of the joint

@@ -235,7 +235,8 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     p.n_queries = q.n_queries; p.quirk_period = q.quirk_period; p.out = q.out; p.members_out = q.members_out; p.acts_out = q.acts_out; p.acts_packed_out = q.acts_packed_out; p.acts_packed_tile_steps = q.acts_packed_tile_steps;
     p.n_members = h->n_members; p.n_symm = h->cfg.n_symm_pairs;
     const bool prune = h->tc_prune && !q.exact;
-    NPHM_REQUIRE(!q.acts_out || (q.n_queries == 1 && q.exact && q.acts_packed_out && q.acts_packed_tile_steps >= tc::kActPackedSteps), "activation dump needs a single exact query");
+    NPHM_REQUIRE(!q.acts_out || (q.exact && q.acts_packed_out && q.acts_packed_tile_steps >= tc::kActPackedSteps),
+                 "activation dump needs an exact query");
     p.anchors = q.anchors; p.prune_tau = h->tc_prune_tau;
     p.blocked = 0; p.px0 = p.px1 = 0; p.by = p.bz = 1;
     long long n_tiles = ceil_div(q.n_points, 128) * q.n_queries;
@@ -251,8 +252,9 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     p.n_tiles = n_tiles;
     p.member_groups = 1;
     if (q.acts_out) {
-        // fitting: a few dozen tiles - split the members of a tile over several CTAs so that every SM has work.  Cost model:
-        // waves * (members per group + pipeline fill of a work item); groups must all be non-empty.
+        // fitting: a few dozen tiles per scan - split the members of a tile over several CTAs so that every SM has work.  Cost
+        // model: waves * (members per group + pipeline fill of a work item); groups must all be non-empty.  With many scans in
+        // one launch (hundreds of tiles) it keeps whole tiles (one group): the waves are already full.
         double best = 1e30;
         for (int g = 1; g <= h->n_members; ++g) {
             const int per = (h->n_members + g - 1) / g;

@@ -236,8 +236,9 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 cx[i] *= kS; cy[i] *= kS; cz[i] *= kS;                 // coordinates in log2 units
             }
             // activation derivatives for the fitting backward, sigma'(pre) = 1 - 2^(-softplus) (log2 units): per (member, tile) a
-            // block of kActLd features x 128 points, feature-major.  Columns beyond a layer's width receive don't-care values.
-            float *const ab = ACTS ? p.acts_out + ((size_t)m * tiles_per_query + (tile % tiles_per_query)) * kActLd * 128 : nullptr;
+            // block of kActLd features x 128 points, feature-major, tiles numbered over all queries (the tiles of query qi follow
+            // those of query qi - 1).  Columns beyond a layer's width receive don't-care values.
+            float *const ab = ACTS ? p.acts_out + ((size_t)m * n_tiles + tile) * kActLd * 128 : nullptr;
             auto save_act = [&](int off, int col, int r, float v) {
                 if (ACTS) {
                     float ex;
@@ -350,7 +351,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
             float part[2] = {0.f, 0.f};
             // sigma'3 is the A operand of the first backward GEMM: saved operand-ready (tc_linear.cuh "packed": per k-step = unit
             // of 16 features [128 x 16 fp16 hi | 128 x 16 fp16 lo], core-matrix order), zeros in the K padding
-            uint8_t *const pk = ACTS ? p.acts_packed_out + ((size_t)m * tiles_per_query + (tile % tiles_per_query)) * p.acts_packed_tile_steps * 8192
+            uint8_t *const pk = ACTS ? p.acts_packed_out + ((size_t)m * n_tiles + tile) * p.acts_packed_tile_steps * 8192
                                      : nullptr;
             auto out_layer = [&](const auto &acc, int col0, int units) {
 #pragma unroll

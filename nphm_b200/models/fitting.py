@@ -53,16 +53,24 @@ def _clamp_for_iteration(j, step_scale):
     return clamp
 
 
-def _sample_observations(all_obs):
-    """Reference sampling order on the global CPU generator (:214-222)."""
-    num_observations = len(all_obs)
-    sampled_observations_idx = torch.randint(0, num_observations, [NUM_OBSERVATIONS_PER_BATCH])
+def _sample_indices(sizes, generator=None):
+    """The draws of one iteration's sampling (:214-222): which observations, and which points of each.  ``generator=None``:
+    torch's global CPU generator, as in the reference."""
+    sampled_observations_idx = torch.randint(0, len(sizes), [NUM_OBSERVATIONS_PER_BATCH], generator=generator)
+    subsample_idx = []
+    for i in range(NUM_OBSERVATIONS_PER_BATCH):
+        n = sizes[int(sampled_observations_idx[i])]
+        subsample_idx.append(torch.randint(0, n, [min(NUM_POINTS_PER_OBSERVATION, n)], generator=generator))
+    return sampled_observations_idx, subsample_idx
+
+
+def _sample_observations(all_obs, generator=None):
+    """Reference sampling order on the global CPU generator (:214-222), or on ``generator``."""
+    sampled_observations_idx, subsample_idx = _sample_indices([o.shape[0] for o in all_obs], generator)
     sampled_points = []
     for i in range(NUM_OBSERVATIONS_PER_BATCH):
-        sampled_idx = sampled_observations_idx[i]
-        n_samps = min(NUM_POINTS_PER_OBSERVATION, all_obs[sampled_idx].shape[0])
-        subsample_idx = torch.randint(0, all_obs[sampled_idx].shape[0], [n_samps])
-        sampled_points.append(all_obs[sampled_idx][subsample_idx.to(all_obs[sampled_idx].device), :])
+        obs = all_obs[sampled_observations_idx[i]]
+        sampled_points.append(obs[subsample_idx[i].to(obs.device), :])
     return torch.stack(sampled_points, dim=0), sampled_observations_idx
 
 
@@ -561,3 +569,268 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
         opt.step()
         opt_expr.step()
     return lat_rep, lat_rep_shape, anchors
+
+
+# ------------------------------------------------------------------------------------------ many scans in one launch sequence
+def _sampling_plan(scans, n_iters: int):
+    """One generator per scan that replays, for that scan, the draws the sequential fits would take from the global CPU
+    generator: scan k's fit starts where scan k-1's ended.  The global generator is walked forward over every scan's
+    ``n_iters`` iterations (indices only, nothing is gathered), so afterwards it is where the sequential calls leave it."""
+    gens = []
+    for all_obs in scans:
+        g = torch.Generator()
+        g.set_state(torch.get_rng_state())
+        gens.append(g)
+        sizes = [o.shape[0] for o in all_obs]
+        for _ in range(n_iters):
+            _sample_indices(sizes)
+    return gens
+
+
+def _pad_scans(points: List[torch.Tensor]):
+    """Per-scan point sets (n_k x 3) -> (S x n x 3, S x n mask bytes or None).  Missing rows repeat the scan's first point
+    (finite through every kernel) and are masked out of the loss."""
+    n = max(p.shape[0] for p in points)
+    if all(p.shape[0] == n for p in points):
+        return torch.stack(points).contiguous(), None
+    padded, masks = [], []
+    for p in points:
+        extra = n - p.shape[0]
+        padded.append(torch.cat([p, p[:1].expand(extra, 3)]) if extra else p)
+        m = torch.ones(n, dtype=torch.uint8, device=p.device)
+        m[p.shape[0]:] = 0
+        masks.append(m)
+    return torch.stack(padded).contiguous(), torch.stack(masks).contiguous()
+
+
+def _sequential(fit_one, scans, lambdas, *args):
+    """The batched functions' contract, run one scan after another: every call gets a fresh copy of ``lambdas`` and the
+    caller's dict ends as one call leaves it."""
+    start, out = dict(lambdas), []
+    for all_obs in scans:
+        lam = dict(start)
+        out.append(fit_one(all_obs, lam, *args))
+        lambdas.update(lam)
+    return out
+
+
+def _tc_ensemble(decoder) -> bool:
+    """The scan-batched kernels need the tensor-core configuration (csrc tc_ensemble_supported): hidden width 200 and a
+    condition of 96 (lat_dim_glob + lat_dim_loc); the 4 hidden layers are checked by :func:`_fused_identity`."""
+    e = decoder.ensembled_deep_sdf
+    return _native.hidden_width(e, e.num_layers - 1) == 200 and decoder.lat_dim_glob + decoder.lat_dim_loc == 96
+
+
+class BatchedIdentityFitter:
+    """:class:`IdentityFitter` for S scans at once (``nphm_fit_identity_step_batched``): latents and Adam moments S x D on the
+    device, one launch sequence per iteration for all scans."""
+
+    def __init__(self, decoder: FastEnsembleDeepSDFMirrored, n_scans: int, device):
+        self.device = device
+        self.engine = decoder.engine()
+        self.latents = torch.zeros(n_scans, decoder.lat_dim, device=device, dtype=torch.float32)
+        self.m = torch.zeros_like(self.latents)
+        self.v = torch.zeros_like(self.latents)
+        self.loss_terms = torch.zeros(n_scans, 8, device=device, dtype=torch.float32)
+        self.grad = torch.zeros_like(self.latents)
+        self.t = 0
+        self._ws = None
+
+    def step(self, points: List[torch.Tensor], lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
+        """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ)."""
+        pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in points])
+        S, n = pts.shape[0], pts.shape[1]
+        if apply_update:
+            self.t += 1
+        fp = _native.FitParams(float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0)),
+                               float(lambdas.get('reg_loc', 0.0)), float(lambdas.get('reg_unobserved', 0.0)),
+                               float(lambdas.get('symm_dist', 0.0)), float(clamp), float(lr), max(self.t, 1))
+        lib = _native.lib()
+        with torch.cuda.device(self.device):
+            if self._ws is None or self._ws[0] != (S, n):
+                self._ws = ((S, n), _native._workspace(lib.nphm_fit_batch_workspace_bytes(self.engine.handle, S, n),
+                                                       'nphm_fit_batch_workspace_bytes', self.device))
+            ws = self._ws[1]
+            _native.check(lib.nphm_fit_identity_step_batched(
+                self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, self.latents.data_ptr(), self.m.data_ptr(),
+                self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
+                ws.data_ptr(), ws.numel(), torch.cuda.current_stream(self.device).cuda_stream),
+                'nphm_fit_identity_step_batched')
+
+
+def _scans_device(scans):
+    devs = {o.device for all_obs in scans for o in all_obs}
+    return devs.pop() if len(devs) == 1 else None
+
+
+def inference_identity_space_batched(decoder,
+                                     scans: List[List[torch.Tensor]],
+                                     lambdas,
+                                     n_steps,
+                                     schedule_cfg: Dict,
+                                     step_scale=1,
+                                     lr_scale=1):
+    """:func:`inference_identity_space` for several scans (``scans[k]``: the observations of scan k) at once.  Returns
+    ``[(lat_rep_shape, anchors)]`` in scan order - what the single-scan function gives when called on each scan in turn, each
+    call with a fresh copy of ``lambdas``; the global CPU generator and ``lambdas`` end as those calls leave them.  Runs all
+    scans in one launch sequence per iteration (:class:`BatchedIdentityFitter`) for the fused ensemble in training mode on
+    CUDA; any other configuration calls the single-scan function scan by scan."""
+    if not scans:
+        return []
+    device = _scans_device(scans)
+    if device is None or device.type != 'cuda' or not (_fused_identity(decoder) and _tc_ensemble(decoder)):
+        return _sequential(lambda obs, lam: inference_identity_space(decoder, obs, lam, n_steps, schedule_cfg, step_scale,
+                                                                     lr_scale), scans, lambdas)
+    n_iters = int(n_steps * step_scale)
+    gens = _sampling_plan(scans, n_iters)
+    fitter = BatchedIdentityFitter(decoder, len(scans), device)
+    lr = 0.01 * lr_scale
+    z_prev = fitter.latents.clone()
+    for j in range(n_iters):
+        lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
+        obs = [_sample_observations(all_obs, g)[0] for all_obs, g in zip(scans, gens)]
+        z_prev.copy_(fitter.latents)
+        fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+    out = []
+    with torch.no_grad():
+        for k in range(len(scans)):
+            _, anchors = fitter.engine.query(torch.zeros(1, 1, 3, device=device), z_prev[k].reshape(1, -1), eval_quirk=False)
+            out.append((fitter.latents[k].reshape(1, 1, -1).clone().requires_grad_(True), anchors))
+    return out
+
+
+class BatchedJointFitter:
+    """:class:`JointFitter` for S subjects at once.  Per iteration, for the 5 sampled observations of every subject:
+        anchors of the S identity codes (nphm_ensemble_anchors), condition rows [compressor([z_id | anchors])[subject] | z_ex[row]]
+        J0^-1, Broyden and J^-1 on all 5 S rows (per-row conditions; shorter subjects padded, the padding masked)
+        nphm_fit_surface_grad_batched: per-subject surface term, d/d z_id and d/d point
+        u = -J^-T g_x, one adjoint pass, the compressor adjoint summed per subject
+        nphm_fit_apply_gradient_batched (regularisers, mlp_pos backward, Adam per subject)
+        one nphm_adam_step over the expression codes of all subjects (element-wise, shared step and lr: the same as per subject).
+    The expression codes are one (sum n_obs) x E tensor; subject k's rows start at ``offsets[k]``."""
+
+    def __init__(self, decoder, decoder_expr, num_observations: List[int], device):
+        self.dec, self.dfn, self.device = decoder, decoder_expr, device
+        self.eng = decoder.engine()
+        self.mlp = decoder_expr.defDeepSDF.engine()
+        E, S = decoder_expr.lat_dim_expr, len(num_observations)
+        self.num_observations = list(num_observations)
+        self.offsets = [sum(self.num_observations[:k]) for k in range(S)]
+        self.z_id = torch.zeros(S, decoder.lat_dim, device=device)
+        self.m_id, self.v_id = torch.zeros_like(self.z_id), torch.zeros_like(self.z_id)
+        self.z_ex = torch.zeros(sum(self.num_observations), E, device=device)
+        self.m_ex, self.v_ex = torch.zeros_like(self.z_ex), torch.zeros_like(self.z_ex)
+        self.loss_terms = torch.zeros(S, 8, device=device)
+        self.t = 0
+        self.anchors = None
+        self.early_exit = bool(int(os.environ.get('NPHM_BROYDEN_EARLY_EXIT', '0')))
+        self._ws = None
+
+    def step(self, obs: List[torch.Tensor], obs_idx: List[torch.Tensor], lambdas, clamp, lr, apply_update: bool = True):
+        """One iteration; ``obs[k]`` (5 x n_k x 3) and ``obs_idx[k]`` (5, on the device) are subject k's sample.  With
+        ``apply_update=False`` nothing is modified and ``(d loss / d z_id (S x D), [d loss / d z_ex of subject k])`` is returned."""
+        nat, dev = _native, self.device
+        S, D = self.z_id.shape
+        nb = obs[0].shape[0]
+        n_point = max(o.shape[1] for o in obs)
+        if apply_update:
+            self.t += 1
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        lib = nat.lib()
+        with torch.no_grad(), torch.cuda.device(dev):
+            anchors = self.eng.anchors(self.z_id)                                        # S x K x 3, pre-update codes
+            self.anchors = anchors
+            lin = self.dfn.compressor[0] if isinstance(self.dfn.compressor, torch.nn.Sequential) else self.dfn.compressor
+            Wc, bc = lin.weight, lin.bias
+            first = torch.cat([self.z_id, anchors.reshape(S, -1)], dim=1)
+            c32 = (Wc[None] * first[:, None, :]).sum(2) + bc                             # S x 32
+            rows = torch.cat([idx + off for idx, off in zip(obs_idx, self.offsets)])    # rows of z_ex, 5 S
+            cond = torch.cat([c32.repeat_interleave(nb, dim=0), self.z_ex[rows]], dim=1).contiguous()
+            # every subject padded to n_point points per observation (the padding repeats a point and is masked below)
+            keep = None
+            if any(o.shape[1] != n_point for o in obs):
+                keep = torch.ones(S, nb, n_point, dtype=torch.bool, device=dev)
+                for k, o in enumerate(obs):
+                    keep[k, :, o.shape[1]:] = False
+            obs_all = torch.cat([o if o.shape[1] == n_point else torch.cat([o, o[:, :1].expand(nb, n_point - o.shape[1], 3)], dim=1)
+                                 for o in obs]).to(torch.float32).contiguous()                 # 5 S x n_point x 3
+            _, j0_inv = self.mlp.inverse_jacobian(obs_all, cond)
+            p, _, valid, _ = self.mlp.broyden_search(obs_all, cond, obs_all, j0_inv, max_steps=15, cvg_thresh=1e-6,
+                                                     dvg_thresh=0.2, early_exit=self.early_exit)
+            _, j_inv = self.mlp.inverse_jacobian(p, cond)
+            n = nb * n_point
+            pts = p.reshape(S, n, 3).contiguous()
+            valid = valid.reshape(S, nb, n_point)
+            mask = (valid if keep is None else valid & keep).reshape(S, n).to(torch.uint8).contiguous()
+            if self._ws is None or self._ws[0] != (S, n):
+                self._ws = ((S, n), nat._workspace(lib.nphm_fit_batch_workspace_bytes(self.eng.handle, S, n),
+                                                   'nphm_fit_batch_workspace_bytes', dev))
+            ws = self._ws[1]
+            terms = torch.empty(S, 8, device=dev)
+            g_lat = torch.empty(S, D, device=dev)
+            g_pts = torch.empty_like(pts)
+            nat.check(lib.nphm_fit_surface_grad_batched(self.eng.handle, pts.data_ptr(), mask.data_ptr(), S, n, self.z_id.data_ptr(),
+                                                        float(clamp), terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(),
+                                                        ws.data_ptr(), ws.numel(), stream), 'nphm_fit_surface_grad_batched')
+            u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # 5 S x (32 + E)
+            g_c32 = g_cond[:, :32].reshape(S, nb, 32).sum(1)
+            g_first = (Wc[None] * g_c32[:, :, None]).sum(1)                              # compressor^T, S x (D + 3 K)
+            g_zid = (g_lat + g_first[:, :D]).contiguous()
+            g_anchors = g_first[:, D:].contiguous()
+            stats = torch.stack([terms[:, 5], terms[:, 0] * terms[:, 5]], dim=1).nan_to_num_(0.0).contiguous()
+            lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
+            g_zex = torch.zeros_like(self.z_ex)
+            g_zex.index_add_(0, rows, lam_s * g_cond[:, 32:] + (2.0 * lam_e / nb) * self.z_ex[rows])
+            fp = nat.FitParams(lam_s, float(lambdas.get('reg_global', 0.0)), float(lambdas.get('reg_loc', 0.0)),
+                               float(lambdas.get('reg_unobserved', 0.0)), float(lambdas.get('symm_dist', 0.0)), float(clamp),
+                               float(lr), max(self.t, 1))
+            g_total = None if apply_update else torch.empty(S, D, device=dev)
+            nat.check(lib.nphm_fit_apply_gradient_batched(self.eng.handle, S, self.z_id.data_ptr(), self.m_id.data_ptr(),
+                                                          self.v_id.data_ptr(), ctypes.byref(fp), g_zid.data_ptr(),
+                                                          stats.data_ptr(), g_anchors.data_ptr(), int(apply_update),
+                                                          self.loss_terms.data_ptr(), nat._ptr(g_total), stream),
+                      'nphm_fit_apply_gradient_batched')
+            if not apply_update:
+                return g_total, [g_zex[o:o + c] for o, c in zip(self.offsets, self.num_observations)]
+            nat.check(lib.nphm_adam_step(self.z_ex.data_ptr(), g_zex.data_ptr(), self.m_ex.data_ptr(), self.v_ex.data_ptr(),
+                                         self.z_ex.numel(), float(lr), self.t, stream), 'nphm_adam_step')
+            return None
+
+
+def inference_iterative_root_finding_joint_batched(decoder,
+                                                   decoder_expr,
+                                                   subjects: List[List[torch.Tensor]],
+                                                   lambdas,
+                                                   n_steps,
+                                                   schedule_cfg: Dict,
+                                                   step_scale=1,
+                                                   lr_scale=1):
+    """:func:`inference_iterative_root_finding_joint` for several subjects (``subjects[k]``: the observations of subject k) at
+    once.  Returns ``[(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)]`` in subject order, under the contract of
+    :func:`inference_identity_space_batched`.  The shipped configuration (see :func:`_native_joint`) runs all subjects in one
+    launch sequence per iteration (:class:`BatchedJointFitter`); anything else - the NPM baseline, CPU, other deformation
+    modes, ``NPHM_JOINT_AUTOGRAD=1`` - calls the single-subject function subject by subject."""
+    if not subjects:
+        return []
+    device = _scans_device(subjects)
+    if (device is None or os.environ.get('NPHM_JOINT_AUTOGRAD') or not _native_joint(decoder, decoder_expr, device)
+            or not _tc_ensemble(decoder)):
+        return _sequential(lambda obs, lam: inference_iterative_root_finding_joint(decoder, decoder_expr, obs, lam, n_steps,
+                                                                                   schedule_cfg, step_scale, lr_scale),
+                           subjects, lambdas)
+    n_iters = int(n_steps * step_scale)
+    gens = _sampling_plan(subjects, n_iters)
+    fitter = BatchedJointFitter(decoder, decoder_expr, [len(s) for s in subjects], device)
+    lr = 0.01 * lr_scale
+    for j in range(n_iters):
+        lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
+        sample = [_sample_observations(all_obs, g) for all_obs, g in zip(subjects, gens)]
+        fitter.step([o for o, _ in sample], [i.long().to(device) for _, i in sample], lambdas,
+                    _clamp_for_iteration(j, step_scale), lr)
+    out = []
+    for k, (off, cnt) in enumerate(zip(fitter.offsets, fitter.num_observations)):
+        lat_rep = fitter.z_ex[off:off + cnt].reshape(cnt, 1, -1).clone().requires_grad_(True)
+        lat_rep_shape = fitter.z_id[k].reshape(1, 1, -1).clone().requires_grad_(True)
+        out.append((lat_rep, lat_rep_shape, None if fitter.anchors is None else fitter.anchors[k:k + 1].clone()))
+    return out
