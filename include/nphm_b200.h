@@ -376,6 +376,28 @@ int nphm_adam_step(float *param_dev, const float *grad_dev, float *adam_m_dev, f
 int nphm_nearest_neighbors(const float *src_dev, long long n_src, const float *tgt_dev, long long n_tgt,
                            double *dist_dev, long long *idx_dev, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Depth / normal rendering of a triangle mesh into V views in one call: the images pyrender hands to `render_glcam`
+ * (reference src/NPHM/evaluation/render_utils.py:26-89), which `gen_render_samples` (:169-201) and
+ * scripts/data_processing/generate_single_view_observations.py back-project into point clouds.
+ * verts_dev: n_verts x 3 fp32 (world); faces_dev: n_faces x 3 int32, every index in [0, n_verts) - a PRECONDITION, not checked
+ * here (the Python layer checks it); n_faces == 0 renders all background.  world_to_eye_dev: V x 3 x 4 fp64 (row-major, the
+ * inverse of the camera pose; the camera looks down -z with +y up); intrinsics_dev: V x 4 fp64 (fx, fy, cx, cy).
+ * Pixel (r, c) of a height x width image (row 0 at the top) samples the eye ray ((c + 0.5 - cx)/fx, (cy - r - 0.5)/fy, -1).
+ * Outputs, V x height x width, row-major: depth_dev fp32 eye depth (-z_eye, fragments kept for znear <= d <= zfar; 0 =
+ * background), normals_dev 3 bytes per pixel round(clamp(0.5 n + 0.5, 0, 1) * 255) of the unit world-space face normal
+ * cross(v1 - v0, v2 - v0), not flipped toward the camera (0, 0, 0 = background), tri_dev (may be NULL) the winning face
+ * (-1 = background).  Nearest depth wins, ties go to the lower face index; faces are not culled.  Bitwise deterministic.
+ * workspace_bytes (checked, NPHM_ERR_CAPACITY when short) >= nphm_render_workspace_bytes(n_views, height, width).
+ * Needs 1 <= n_views <= 65535, height, width >= 1, 0 < znear < zfar (else NPHM_ERR_INVALID).
+ * ---------------------------------------------------------------------------------------------- */
+/* bytes of scratch for n_views views of height x width (-1: bad arguments) */
+long long nphm_render_workspace_bytes(int n_views, int height, int width);
+int nphm_render_depth_normals(const float *verts_dev, long long n_verts, const int *faces_dev, long long n_faces,
+                              const double *world_to_eye_dev, const double *intrinsics_dev, int n_views, double znear,
+                              double zfar, int height, int width, float *depth_dev, unsigned char *normals_dev, int *tri_dev,
+                              void *workspace_dev, long long workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

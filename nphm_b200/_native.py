@@ -39,6 +39,7 @@ EXPORTED_SYMBOLS = (
     'nphm_mlp_sdfgrad_workspace_bytes', 'nphm_mlp_sdfgrad_forward', 'nphm_mlp_sdfgrad_backward',
     'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad',
     'nphm_ensemble_sdfgrad_workspace_bytes', 'nphm_ensemble_sdfgrad_forward', 'nphm_ensemble_sdfgrad_backward',
+    'nphm_render_workspace_bytes', 'nphm_render_depth_normals',
 )
 
 
@@ -185,6 +186,10 @@ def lib() -> ctypes.CDLL:
                                                 c_void_p]
     L.nphm_ensemble_sdfgrad_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_longlong,
                                                  POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
+    L.nphm_render_workspace_bytes.argtypes = [c_int, c_int, c_int]
+    L.nphm_render_workspace_bytes.restype = c_longlong
+    L.nphm_render_depth_normals.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_double,
+                                            c_double, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -744,3 +749,35 @@ def nearest_neighbors(src: torch.Tensor, tgt: torch.Tensor):
         check(lib().nphm_nearest_neighbors(s.data_ptr(), s.shape[0], t.data_ptr(), t.shape[0], dist.data_ptr(), idx.data_ptr(),
                                            _stream_ptr(dev)), 'nphm_nearest_neighbors')
     return dist, idx
+
+
+# ------------------------------------------------------------------------------------------ rendering
+def render_depth_normals(verts: torch.Tensor, faces: torch.Tensor, world_to_eye: torch.Tensor, intrinsics: torch.Tensor,
+                         height: int, width: int, znear: float = 0.1, zfar: float = 2.0, want_tri: bool = False):
+    """Rasterize one mesh into V views in one call (nphm_render_depth_normals).  verts (n, 3) and faces (m, 3) on a CUDA device,
+    world_to_eye (V, 3, 4) and intrinsics (V, 4: fx fy cx cy).  Returns ``(depth (V, H, W) float32 eye depth, 0 = background;
+    normals (V, H, W, 3) uint8; triangle index (V, H, W) int32, -1 = background | None)``.  Face indices outside
+    ``[0, n_verts)`` raise ``ValueError`` before the call."""
+    assert verts.is_cuda and verts.shape[-1] == 3 and faces.shape[-1] == 3
+    dev = verts.device
+    v = _f32c(verts).reshape(-1, 3)
+    f = faces.detach().to(device=dev, dtype=torch.int64).reshape(-1, 3)
+    if f.numel() and (int(f.min()) < 0 or int(f.max()) >= v.shape[0]):
+        raise ValueError('face indices must lie in [0, %d) (got [%d, %d])' % (v.shape[0], int(f.min()), int(f.max())))
+    f = f.to(torch.int32).contiguous()
+    w2e = world_to_eye.detach().to(device=dev, dtype=torch.float64).reshape(-1, 12).contiguous()
+    intr = intrinsics.detach().to(device=dev, dtype=torch.float64).reshape(-1, 4).contiguous()
+    V = w2e.shape[0]
+    assert intr.shape[0] == V
+    H, W = int(height), int(width)
+    L = lib()
+    n_pix = V * max(H, 0) * max(W, 0)
+    depth = torch.empty(n_pix, device=dev, dtype=torch.float32)
+    normals = torch.empty(n_pix * 3, device=dev, dtype=torch.uint8)
+    tri = torch.empty(n_pix, device=dev, dtype=torch.int32) if want_tri else None
+    with torch.cuda.device(dev):
+        ws = _workspace(L.nphm_render_workspace_bytes(V, H, W), 'nphm_render_workspace_bytes', dev)
+        check(L.nphm_render_depth_normals(v.data_ptr(), v.shape[0], f.data_ptr(), f.shape[0], w2e.data_ptr(), intr.data_ptr(), V,
+                                          float(znear), float(zfar), H, W, depth.data_ptr(), normals.data_ptr(), _ptr(tri),
+                                          ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'nphm_render_depth_normals')
+    return (depth.view(V, H, W), normals.view(V, H, W, 3), None if tri is None else tri.view(V, H, W))
