@@ -305,6 +305,17 @@ long long nphm_mlp_fit_workspace_bytes(const nphm_mlp *h, int n_queries, long lo
 int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
                               const unsigned char *mask_dev, float clamp, float *loss_terms_dev, float *grad_cond_dev,
                               float *grad_xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream);
+/* The same surface term per scan, for S scans of n points in one launch sequence (the scan-batched NPM fitters): scan k has its
+ * own kept set (mask != 0 and |s| < clamp over its own rows), its own loss and its own gradients.  xyz_dev [S][n][3], cond_dev
+ * [S][lat_dim], mask_dev [S][n] bytes (may be NULL = all valid).  loss_terms_dev [S][8] in the layout above; grad_cond_dev
+ * [S][lat_dim] = d loss_k / d cond_k, grad_xyz_dev [S][n][3] (may be NULL) = d loss_k / d xyz over scan k's rows.  A scan with
+ * nothing kept gets a NaN loss and exactly zero gradients and leaves the others unaffected.  The workspace is that of
+ * nphm_mlp_fit_workspace_bytes(h, S, n) (checked: NPHM_ERR_INVALID on a mismatch).  Bitwise deterministic; nothing is read back
+ * from the device.  Scan k's result equals a single call on its rows up to one rounding of the gradients (the factor 1 / n_kept
+ * is applied after the chain). */
+int nphm_mlp_fit_surface_grad_batched(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, const unsigned char *mask_dev,
+                                      int n_scans, long long n_points, float clamp, float *loss_terms_dev, float *grad_cond_dev,
+                                      float *grad_xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream);
 
 /* anchors_dev [n_queries][n_loc][3] = mlp_pos(z_glob) + mean anchors (reference src/NPHM/models/EnsembledDeepSDF.py:228-229)
  * without evaluating the ensemble - what the fitters read from `decoder(zeros(1,1,3), lat)[1]` (fitting.py:59, :211). */

@@ -37,7 +37,7 @@ EXPORTED_SYMBOLS = (
     'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
     'nphm_mlp_sdfgrad_workspace_bytes', 'nphm_mlp_sdfgrad_forward', 'nphm_mlp_sdfgrad_backward',
-    'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad',
+    'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad', 'nphm_mlp_fit_surface_grad_batched',
     'nphm_ensemble_sdfgrad_workspace_bytes', 'nphm_ensemble_sdfgrad_forward', 'nphm_ensemble_sdfgrad_backward',
     'nphm_render_workspace_bytes', 'nphm_render_depth_normals',
 )
@@ -180,6 +180,8 @@ def lib() -> ctypes.CDLL:
     L.nphm_mlp_fit_workspace_bytes.restype = c_longlong
     L.nphm_mlp_fit_surface_grad.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_float, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_mlp_fit_surface_grad_batched.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_float, c_void_p,
+                                                    c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
     L.nphm_ensemble_sdfgrad_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong]
     L.nphm_ensemble_sdfgrad_workspace_bytes.restype = c_longlong
     L.nphm_ensemble_sdfgrad_forward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p,
@@ -638,6 +640,27 @@ class MlpEngine(_Versioned):
             check(lib().nphm_mlp_fit_surface_grad(self._h, xyz.data_ptr(), cond.data_ptr(), B, N, _ptr(m), float(clamp),
                                                   terms.data_ptr(), g_cond.data_ptr(), _ptr(g_xyz), ws.data_ptr(), ws.numel(),
                                                   _stream_ptr(dev)), 'nphm_mlp_fit_surface_grad')
+        return terms, g_cond, g_xyz
+
+    def fit_surface_grad_batched(self, xyz: torch.Tensor, cond: torch.Tensor, mask: Optional[torch.Tensor], clamp: float,
+                                 want_xyz: bool = True, workspace: Optional[torch.Tensor] = None, out=None):
+        """:meth:`fit_surface_grad` per scan (nphm_mlp_fit_surface_grad_batched): xyz S x n x 3, cond S x lat_dim, mask S x n (or
+        None: all valid); scan k's loss is the mean |s| over its own kept points.  Returns ``(loss_terms S x 8, d loss_k / d cond_k
+        S x lat_dim, d loss_k / d xyz  S x n x 3 | None)``.  ``workspace``: one of :meth:`fit_workspace` at ``(S, n)``."""
+        S, N, _ = xyz.shape
+        dev = xyz.device
+        xyz = _f32c(xyz)
+        cond = _f32c(cond).to(dev)
+        m = None if mask is None else mask.reshape(-1).to(torch.uint8).contiguous()
+        if out is None:
+            out = (torch.zeros(S, 8, device=dev, dtype=torch.float32), torch.empty(S, self.lat_dim, device=dev, dtype=torch.float32),
+                   torch.empty(S, N, 3, device=dev, dtype=torch.float32) if want_xyz else None)
+        terms, g_cond, g_xyz = out
+        with torch.cuda.device(dev):
+            ws = self.fit_workspace(S, N, dev) if workspace is None else workspace
+            check(lib().nphm_mlp_fit_surface_grad_batched(self._h, xyz.data_ptr(), cond.data_ptr(), _ptr(m), S, N, float(clamp),
+                                                          terms.data_ptr(), g_cond.data_ptr(), _ptr(g_xyz), ws.data_ptr(),
+                                                          ws.numel(), _stream_ptr(dev)), 'nphm_mlp_fit_surface_grad_batched')
         return terms, g_cond, g_xyz
 
     def broyden_search(self, obs: torch.Tensor, cond: torch.Tensor, x_init: torch.Tensor, J_inv_init: torch.Tensor,

@@ -1271,11 +1271,14 @@ static Layout layout(const StackDims &s, int n_queries, long long n_points)
     return F;
 }
 
-// One block.  Row r of the padded tiles: column 0 of the packed adjoint = 2^kGradExp sign(s_r) if r is kept, else 0 (sign(0) = 0,
-// as torch's abs backward).  n_kept and sum |s| are reduced in a fixed order (strided per thread, then a fixed tree), so the
-// call is bitwise deterministic.  gs = {2^kGradExp, 2^-kGradExp / n_kept}; loss_terms = [loss, 0, 0, 0, 0, n_kept].
+// One block per group of `n` consecutive rows (the single call: one group of all rows; the batched call: one group per scan).
+// Row r of the padded tiles: column 0 of the packed adjoint = 2^kGradExp sign(s_r) if r is kept, else 0 (sign(0) = 0, as torch's
+// abs backward); the last group's block also zeroes the padding rows of the last tile.  A group's n_kept and sum |s| are reduced
+// in a fixed order (strided per thread, then a fixed tree), so the call is bitwise deterministic.  Group g writes loss_terms
+// [g][8] = [loss, 0, 0, 0, 0, n_kept].  gs = {2^kGradExp, 2^-kGradExp / n_kept} with one group; with per_group the factor is
+// the uniform 2^-kGradExp and scan_factor_kernel applies each group's 1 / n_kept after the chain.
 __global__ void __launch_bounds__(kThreads) surface_upstream_kernel(const float *__restrict__ sdf, const unsigned char *__restrict__ mask,
-                                                                     long long M, float clamp, uint8_t *__restrict__ dst,
+                                                                     long long n, float clamp, bool per_group, uint8_t *__restrict__ dst,
                                                                      float *__restrict__ gs, float *__restrict__ loss_terms)
 {
     __shared__ float w_sum[kThreads / 32];
@@ -1283,10 +1286,11 @@ __global__ void __launch_bounds__(kThreads) surface_upstream_kernel(const float 
     const float top = ldexpf(1.0f, train::kGradExp);
     float sum = 0.f;
     int cnt = 0;
-    const long long rows = (M + 127) / 128 * 128;
-    for (long long r = threadIdx.x; r < rows; r += kThreads) {
+    const long long r0 = (long long)blockIdx.x * n, r1 = r0 + n;
+    const long long rows = blockIdx.x + 1 == gridDim.x ? (r1 + 127) / 128 * 128 : r1;
+    for (long long r = r0 + threadIdx.x; r < rows; r += kThreads) {
         float v = 0.f;
-        if (r < M) {
+        if (r < r1) {
             const float s = sdf[r], a = fabsf(s);
             if ((!mask || mask[r]) && a < clamp) {
                 sum += a;
@@ -1305,14 +1309,78 @@ __global__ void __launch_bounds__(kThreads) surface_upstream_kernel(const float 
     __syncthreads();
     if (threadIdx.x == 0) {
         float t = 0.f;
-        int n = 0;
-        for (int w = 0; w < kThreads / 32; ++w) { t += w_sum[w]; n += w_cnt[w]; }
-        gs[0] = top;
-        gs[1] = n > 0 ? ldexpf(1.0f, -train::kGradExp) / (float)n : 0.f;
-        loss_terms[0] = t / (float)n;                   // NaN when nothing is kept, like torch's mean of an empty tensor
-        loss_terms[1] = loss_terms[2] = loss_terms[3] = loss_terms[4] = 0.f;
-        loss_terms[5] = (float)n;
+        int k = 0;
+        for (int w = 0; w < kThreads / 32; ++w) { t += w_sum[w]; k += w_cnt[w]; }
+        if (blockIdx.x == 0) {
+            gs[0] = top;
+            gs[1] = per_group ? ldexpf(1.0f, -train::kGradExp) : k > 0 ? ldexpf(1.0f, -train::kGradExp) / (float)k : 0.f;
+        }
+        float *lt = loss_terms + (size_t)blockIdx.x * 8;
+        lt[0] = t / (float)k;                           // NaN when nothing is kept, like torch's mean of an empty tensor
+        lt[1] = lt[2] = lt[3] = lt[4] = 0.f;
+        lt[5] = (float)k;
     }
+}
+
+// grad_cond[q] and the rows of query q of grad_xyz (may be NULL) times 1 / n_kept of group q (loss_terms[q][5]; 0 when nothing is
+// kept).  grid (blocks over max(cond_dim, 3 n), queries)
+__global__ void scan_factor_kernel(const float *__restrict__ loss_terms, int cond_dim, long long n3, float *__restrict__ grad_cond,
+                                   float *__restrict__ grad_xyz)
+{
+    const int q = blockIdx.y;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const float k = loss_terms[(size_t)q * 8 + 5], f = k > 0.f ? 1.0f / k : 0.f;
+    if (i < cond_dim) grad_cond[(size_t)q * cond_dim + i] *= f;
+    if (grad_xyz && i < n3) grad_xyz[(size_t)q * n3 + i] *= f;
+}
+
+// The surface term of one loss over all queries (per_query false) or of one loss per query (per_query: query q = scan q).
+static int surface_grad(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
+                        const unsigned char *mask_dev, float clamp, bool per_query, float *loss_terms_dev, float *grad_cond_dev,
+                        float *grad_xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream_, const char *who)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    int rc = sdfgrad::ready(h, who);
+    if (rc) return rc;
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && loss_terms_dev && grad_cond_dev && workspace_dev,
+                 "%s: bad arguments", who);
+    const StackDims &s = h->dims;
+    const Layout F = layout(s, n_queries, n_points);
+    NPHM_REQUIRE(workspace_bytes == (long long)F.total,
+                 "%s: a workspace of %lld bytes does not fit this network at %d x %lld points (needs %lld)",
+                 who, workspace_bytes, n_queries, n_points, (long long)F.total);
+    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
+    const Stack k = stack(h);
+    const long long M = (long long)n_queries * n_points;
+    const int last = s.n_lin - 1;
+    float *const sdf = reinterpret_cast<float *>(ws + F.sdf), *const gs = reinterpret_cast<float *>(ws + F.consts);
+    float *const xa = reinterpret_cast<float *>(ws + F.xa), *const xb = reinterpret_cast<float *>(ws + F.xb);
+    if ((rc = nphm_mlp_train_forward(h, xyz_dev, cond_dev, nullptr, 0, n_queries, n_points, sdf, ws, stream_))) return rc;
+    surface_upstream_kernel<<<per_query ? (unsigned)n_queries : 1u, kThreads, 0, stream>>>(sdf, mask_dev, per_query ? n_points : M,
+                                                                                         clamp, per_query, ws + F.dl, gs,
+                                                                                         loss_terms_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    if ((rc = train::reserve_sums(k, n_queries))) return rc;
+    train::GradTargets tg = train::targets(s, F.base, ws, n_queries, n_points, 0, gs);
+    tg.want_cond = true;
+    // no weights or biases: the condition sums at layers 0 and skip
+    auto cond_sums = [&](int l, const Adjoint &d) { return train::layer_grads(k, tg, l, d, stream); };
+
+    // d_{l-1} = s_{l-1} * (d_l W_l) from the packed upstream down to d_0; d_l lives in dp[l & 1]
+    AdjointWalk w;
+    w.top = Adjoint{nullptr, 0, ws + F.dl, 1, 0};
+    for (int l = 0; l < last; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + F.base.s[l]); w.D[l] = ws + F.dp[l & 1]; }
+    w.xs = grad_xyz_dev ? xb : nullptr;
+    if ((rc = adjoint_walk(k, M, w, cond_sums, stream))) return rc;
+    if ((rc = cond_grad(k, n_queries, 1, grad_cond_dev, stream))) return rc;           // one chunk: a fixed summation order
+    if (grad_xyz_dev && (rc = xyz_grad(k, M, w.D[0], 0, xa, xb, gs, 2, grad_xyz_dev, stream))) return rc;
+    if (per_query) {
+        const long long n3 = grad_xyz_dev ? 3 * n_points : 0;
+        const dim3 grid((unsigned)ceil_div(std::max((long long)s.cond_dim, n3), 256), (unsigned)n_queries);
+        scan_factor_kernel<<<grid, 256, 0, stream>>>(loss_terms_dev, s.cond_dim, n3, grad_cond_dev, grad_xyz_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    return NPHM_OK;
 }
 
 }  // namespace fitsurf
@@ -1331,40 +1399,17 @@ extern "C" int nphm_mlp_fit_surface_grad(nphm_mlp *h, const float *xyz_dev, cons
                                          const unsigned char *mask_dev, float clamp, float *loss_terms_dev, float *grad_cond_dev,
                                          float *grad_xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream_)
 {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    int rc = sdfgrad::ready(h, "nphm_mlp_fit_surface_grad");
-    if (rc) return rc;
-    NPHM_REQUIRE(n_queries >= 1 && n_points >= 1 && xyz_dev && cond_dev && loss_terms_dev && grad_cond_dev && workspace_dev,
-                 "nphm_mlp_fit_surface_grad: bad arguments");
-    const StackDims &s = h->dims;
-    const fitsurf::Layout F = fitsurf::layout(s, n_queries, n_points);
-    NPHM_REQUIRE(workspace_bytes == (long long)F.total,
-                 "nphm_mlp_fit_surface_grad: a workspace of %lld bytes does not fit this network at %d x %lld points (needs %lld)",
-                 workspace_bytes, n_queries, n_points, (long long)F.total);
-    uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
-    const Stack k = stack(h);
-    const long long M = (long long)n_queries * n_points;
-    const int last = s.n_lin - 1;
-    float *const sdf = reinterpret_cast<float *>(ws + F.sdf), *const gs = reinterpret_cast<float *>(ws + F.consts);
-    float *const xa = reinterpret_cast<float *>(ws + F.xa), *const xb = reinterpret_cast<float *>(ws + F.xb);
-    if ((rc = nphm_mlp_train_forward(h, xyz_dev, cond_dev, nullptr, 0, n_queries, n_points, sdf, ws, stream_))) return rc;
-    fitsurf::surface_upstream_kernel<<<1, fitsurf::kThreads, 0, stream>>>(sdf, mask_dev, M, clamp, ws + F.dl, gs, loss_terms_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    if ((rc = train::reserve_sums(k, n_queries))) return rc;
-    train::GradTargets tg = train::targets(s, F.base, ws, n_queries, n_points, 0, gs);
-    tg.want_cond = true;
-    // no weights or biases: the condition sums at layers 0 and skip
-    auto cond_sums = [&](int l, const Adjoint &d) { return train::layer_grads(k, tg, l, d, stream); };
+    return fitsurf::surface_grad(h, xyz_dev, cond_dev, n_queries, n_points, mask_dev, clamp, false, loss_terms_dev, grad_cond_dev,
+                                 grad_xyz_dev, workspace_dev, workspace_bytes, stream_, "nphm_mlp_fit_surface_grad");
+}
 
-    // d_{l-1} = s_{l-1} * (d_l W_l) from the packed upstream down to d_0; d_l lives in dp[l & 1]
-    AdjointWalk w;
-    w.top = Adjoint{nullptr, 0, ws + F.dl, 1, 0};
-    for (int l = 0; l < last; ++l) { w.S[l] = reinterpret_cast<const float *>(ws + F.base.s[l]); w.D[l] = ws + F.dp[l & 1]; }
-    w.xs = grad_xyz_dev ? xb : nullptr;
-    if ((rc = adjoint_walk(k, M, w, cond_sums, stream))) return rc;
-    if ((rc = cond_grad(k, n_queries, 1, grad_cond_dev, stream))) return rc;           // one chunk: a fixed summation order
-    if (grad_xyz_dev && (rc = xyz_grad(k, M, w.D[0], 0, xa, xb, gs, 2, grad_xyz_dev, stream))) return rc;
-    return NPHM_OK;
+extern "C" int nphm_mlp_fit_surface_grad_batched(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, const unsigned char *mask_dev,
+                                                 int n_scans, long long n_points, float clamp, float *loss_terms_dev,
+                                                 float *grad_cond_dev, float *grad_xyz_dev, void *workspace_dev,
+                                                 long long workspace_bytes, void *stream_)
+{
+    return fitsurf::surface_grad(h, xyz_dev, cond_dev, n_scans, n_points, mask_dev, clamp, true, loss_terms_dev, grad_cond_dev,
+                                 grad_xyz_dev, workspace_dev, workspace_bytes, stream_, "nphm_mlp_fit_surface_grad_batched");
 }
 
 // ================================================================================================ the NPHM ensemble through grad_x sdf

@@ -366,8 +366,12 @@ def _native_npm_joint(decoder, decoder_expr, device) -> bool:
     return next(decoder.parameters()).device == device and next(decoder_expr.parameters()).device == device
 
 
-def _pow2_scale(x: torch.Tensor) -> torch.Tensor:
-    """A power of two (0-dim tensor, computed on the device) that brings the largest magnitude of ``x`` to [2^9, 2^10)."""
+def _pow2_scale(x: torch.Tensor, groups: int = 0) -> torch.Tensor:
+    """A power of two (0-dim tensor, computed on the device) that brings the largest magnitude of ``x`` to [2^9, 2^10); with
+    ``groups``, one such power per group (a ``groups`` tensor) of ``x`` split into ``groups`` equal parts along its first axis."""
+    if groups:
+        _, e = torch.frexp(x.reshape(groups, -1).abs().amax(1))
+        return torch.ldexp(torch.ones(groups, device=x.device), 10 - e)
     _, e = torch.frexp(x.abs().amax())
     return torch.ldexp(torch.ones((), device=x.device), 10 - e)
 
@@ -673,18 +677,27 @@ def inference_identity_space_batched(decoder,
     """:func:`inference_identity_space` for several scans (``scans[k]``: the observations of scan k) at once.  Returns
     ``[(lat_rep_shape, anchors)]`` in scan order - what the single-scan function gives when called on each scan in turn, each
     call with a fresh copy of ``lambdas``; the global CPU generator and ``lambdas`` end as those calls leave them.  Runs all
-    scans in one launch sequence per iteration (:class:`BatchedIdentityFitter`) for the fused ensemble in training mode on
-    CUDA; any other configuration calls the single-scan function scan by scan."""
+    scans in one launch sequence per iteration for the fused ensemble in training mode on CUDA (:class:`BatchedIdentityFitter`)
+    and for the NPM baseline's ``DeepSDF`` on CUDA (:class:`BatchedNpmIdentityFitter`); any other configuration calls the
+    single-scan function scan by scan."""
     if not scans:
         return []
     device = _scans_device(scans)
-    if device is None or device.type != 'cuda' or not (_fused_identity(decoder) and _tc_ensemble(decoder)):
+    npm = device is not None and device.type == 'cuda' and _native_npm_decoder(decoder, 1)
+    if not npm and (device is None or device.type != 'cuda' or not (_fused_identity(decoder) and _tc_ensemble(decoder))):
         return _sequential(lambda obs, lam: inference_identity_space(decoder, obs, lam, n_steps, schedule_cfg, step_scale,
                                                                      lr_scale), scans, lambdas)
     n_iters = int(n_steps * step_scale)
     gens = _sampling_plan(scans, n_iters)
-    fitter = BatchedIdentityFitter(decoder, len(scans), device)
     lr = 0.01 * lr_scale
+    if npm:
+        fitter = BatchedNpmIdentityFitter(decoder, len(scans), device)
+        for j in range(n_iters):
+            lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
+            obs = [_sample_observations(all_obs, g)[0] for all_obs, g in zip(scans, gens)]
+            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+        return [(fitter.latents[k].reshape(1, 1, -1).clone().requires_grad_(True), None) for k in range(len(scans))]
+    fitter = BatchedIdentityFitter(decoder, len(scans), device)
     z_prev = fitter.latents.clone()
     for j in range(n_iters):
         lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
@@ -798,6 +811,123 @@ class BatchedJointFitter:
             return None
 
 
+class BatchedNpmIdentityFitter:
+    """:class:`NpmIdentityFitter` for S scans at once: latents, Adam moments and ``grad`` S x D, ``loss_terms`` S x 8.  Per
+    iteration one surface call over all scans (``nphm_mlp_fit_surface_grad_batched``, scan k = query k with condition z_k and
+    its own loss), ``grad = lambda_s g_cond + 2 lambda_g z`` and one ``nphm_adam_step`` over the S D elements (Adam is
+    element-wise and the scans share the step and lr)."""
+
+    def __init__(self, decoder, n_scans: int, device):
+        self.device = device
+        self.engine = decoder.engine()
+        self.latents = torch.zeros(n_scans, decoder.lat_dim, device=device, dtype=torch.float32)
+        self.m = torch.zeros_like(self.latents)
+        self.v = torch.zeros_like(self.latents)
+        self.loss_terms = torch.zeros(n_scans, 8, device=device, dtype=torch.float32)
+        self.grad = torch.zeros_like(self.latents)
+        self.t = 0
+        self._ws = None
+
+    def step(self, points: List[torch.Tensor], lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
+        """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ)."""
+        pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in points])
+        S, n = pts.shape[0], pts.shape[1]
+        if apply_update:
+            self.t += 1
+        lam_s, lam_g = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0))
+        with torch.no_grad(), torch.cuda.device(self.device):
+            if self._ws is None or self._ws[0] != (S, n):
+                self._ws = ((S, n), self.engine.fit_workspace(S, n, self.device))
+            terms, g_cond, _ = self.engine.fit_surface_grad_batched(pts, self.latents, mask, clamp, want_xyz=False,
+                                                                    workspace=self._ws[1])
+            self.loss_terms.copy_(terms)
+            torch.add(lam_s * g_cond, self.latents, alpha=2.0 * lam_g, out=self.grad)
+            if apply_update:
+                _native.check(_native.lib().nphm_adam_step(self.latents.data_ptr(), self.grad.data_ptr(), self.m.data_ptr(),
+                                                           self.v.data_ptr(), self.latents.numel(), float(lr), self.t,
+                                                           torch.cuda.current_stream(self.device).cuda_stream), 'nphm_adam_step')
+
+
+class BatchedNpmJointFitter:
+    """:class:`NpmJointFitter` for S subjects at once, with the padding and row bookkeeping of :class:`BatchedJointFitter`.  Per
+    iteration, for the 5 sampled observations of every subject:
+        condition rows [z_id[subject] | z_ex[row]]; J0^-1, sync-free Broyden and J^-1 on all 5 S rows
+        nphm_mlp_fit_surface_grad_batched (mask = valid and not padding): per-subject surface term, d/d z_id and d/d point
+        u = -J^-T g_x, scaled by one power of two per subject (its largest magnitude to 2^10 over that subject's rows, so that
+        each subject feeds the fp16 adjoint what its single-subject call would); one adjoint pass with the value pass reused,
+        the g_cond rows divided by their subject's scale
+        z_id: g_cond[:, :D] summed per subject; z_ex rows: g_cond[:, D:] + reg_expr; two nphm_adam_step calls.
+    The expression codes are one (sum n_obs) x 200 tensor; subject k's rows start at ``offsets[k]``.  Memory grows linearly with
+    S: the Jacobian, Broyden and adjoint buffers of 5 S n_point rows through the expression stack, about 1.4 GB per subject of
+    5 x 1000 points (22.7 GB peak at S = 16, tools/bench_fit_batched.py --decoder npm), so an 80 GB card holds about 50
+    subjects per batch; the caller chooses S, nothing is split."""
+
+    def __init__(self, decoder, decoder_expr, num_observations: List[int], device):
+        self.device = device
+        self.eng = decoder.engine()
+        self.mlp = decoder_expr.engine()
+        D, S = decoder.lat_dim, len(num_observations)
+        self.num_observations = list(num_observations)
+        self.offsets = [sum(self.num_observations[:k]) for k in range(S)]
+        self.z_id = torch.zeros(S, D, device=device)
+        self.m_id, self.v_id = torch.zeros_like(self.z_id), torch.zeros_like(self.z_id)
+        self.z_ex = torch.zeros(sum(self.num_observations), decoder_expr.lat_dim - D, device=device)
+        self.m_ex, self.v_ex = torch.zeros_like(self.z_ex), torch.zeros_like(self.z_ex)
+        self.loss_terms = torch.zeros(S, 8, device=device)
+        self.t = 0
+        self.anchors = None                     # a DeepSDF has no anchors
+        self.early_exit = bool(int(os.environ.get('NPHM_BROYDEN_EARLY_EXIT', '0')))
+        self._ws = None
+
+    def step(self, obs: List[torch.Tensor], obs_idx: List[torch.Tensor], lambdas, clamp, lr, apply_update: bool = True):
+        """One iteration; ``obs[k]`` (5 x n_k x 3) and ``obs_idx[k]`` (5, on the device) are subject k's sample.  With
+        ``apply_update=False`` nothing is modified and ``(d loss / d z_id (S x D), [d loss / d z_ex of subject k])`` is returned."""
+        nat, dev = _native, self.device
+        S, D = self.z_id.shape
+        nb = obs[0].shape[0]
+        n_point = max(o.shape[1] for o in obs)
+        if apply_update:
+            self.t += 1
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
+        lam_g = float(lambdas.get('reg_global', 0.0))
+        with torch.no_grad(), torch.cuda.device(dev):
+            rows = torch.cat([idx + off for idx, off in zip(obs_idx, self.offsets)])    # rows of z_ex, 5 S
+            cond = torch.cat([self.z_id.repeat_interleave(nb, dim=0), self.z_ex[rows]], dim=1).contiguous()
+            keep = None
+            if any(o.shape[1] != n_point for o in obs):
+                keep = torch.ones(S, nb, n_point, dtype=torch.bool, device=dev)
+                for k, o in enumerate(obs):
+                    keep[k, :, o.shape[1]:] = False
+            obs_all = torch.cat([o if o.shape[1] == n_point else torch.cat([o, o[:, :1].expand(nb, n_point - o.shape[1], 3)], dim=1)
+                                 for o in obs]).to(torch.float32).contiguous()                 # 5 S x n_point x 3
+            _, j0_inv = self.mlp.inverse_jacobian(obs_all, cond)
+            p, _, valid, _ = self.mlp.broyden_search(obs_all, cond, obs_all, j0_inv, max_steps=15, cvg_thresh=1e-6,
+                                                     dvg_thresh=0.2, early_exit=self.early_exit)
+            _, j_inv = self.mlp.inverse_jacobian(p, cond)
+            n = nb * n_point
+            valid = valid.reshape(S, nb, n_point)
+            mask = (valid if keep is None else valid & keep).reshape(S, n)
+            if self._ws is None or self._ws[0] != (S, n):
+                self._ws = ((S, n), self.eng.fit_workspace(S, n, dev))
+            terms, g_lat, g_pts = self.eng.fit_surface_grad_batched(p.reshape(S, n, 3), self.z_id, mask, clamp,
+                                                                    workspace=self._ws[1])
+            self.loss_terms.copy_(terms)
+            u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
+            sc = _pow2_scale(u, S).repeat_interleave(nb)                                 # per subject, one entry per row
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u * sc[:, None, None], reuse_value_pass=True)
+            g_cond = g_cond / sc[:, None]
+            g_zid = lam_s * (g_lat + g_cond[:, :D].reshape(S, nb, D).sum(1)) + (2.0 * lam_g) * self.z_id
+            g_zex = torch.zeros_like(self.z_ex)
+            g_zex.index_add_(0, rows, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[rows])
+            if not apply_update:
+                return g_zid, [g_zex[o:o + c] for o, c in zip(self.offsets, self.num_observations)]
+            for z, g, m, v in ((self.z_id, g_zid, self.m_id, self.v_id), (self.z_ex, g_zex, self.m_ex, self.v_ex)):
+                nat.check(nat.lib().nphm_adam_step(z.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), z.numel(), float(lr),
+                                                   self.t, stream), 'nphm_adam_step')
+            return None
+
+
 def inference_iterative_root_finding_joint_batched(decoder,
                                                    decoder_expr,
                                                    subjects: List[List[torch.Tensor]],
@@ -809,19 +939,26 @@ def inference_iterative_root_finding_joint_batched(decoder,
     """:func:`inference_iterative_root_finding_joint` for several subjects (``subjects[k]``: the observations of subject k) at
     once.  Returns ``[(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)]`` in subject order, under the contract of
     :func:`inference_identity_space_batched`.  The shipped configuration (see :func:`_native_joint`) runs all subjects in one
-    launch sequence per iteration (:class:`BatchedJointFitter`); anything else - the NPM baseline, CPU, other deformation
-    modes, ``NPHM_JOINT_AUTOGRAD=1`` - calls the single-subject function subject by subject."""
+    launch sequence per iteration (:class:`BatchedJointFitter`), and so does the NPM baseline (see :func:`_native_npm_joint`,
+    :class:`BatchedNpmJointFitter`); anything else - CPU, other decoders or deformation modes, ``NPHM_JOINT_AUTOGRAD=1`` -
+    calls the single-subject function subject by subject.  Memory grows linearly with the number of subjects; all subjects
+    must fit on the device at once (nothing is split into smaller batches)."""
     if not subjects:
         return []
     device = _scans_device(subjects)
-    if (device is None or os.environ.get('NPHM_JOINT_AUTOGRAD') or not _native_joint(decoder, decoder_expr, device)
-            or not _tc_ensemble(decoder)):
+    batched = None
+    if device is not None and not os.environ.get('NPHM_JOINT_AUTOGRAD'):
+        if _native_npm_joint(decoder, decoder_expr, device):
+            batched = BatchedNpmJointFitter
+        elif _native_joint(decoder, decoder_expr, device) and _tc_ensemble(decoder):
+            batched = BatchedJointFitter
+    if batched is None:
         return _sequential(lambda obs, lam: inference_iterative_root_finding_joint(decoder, decoder_expr, obs, lam, n_steps,
                                                                                    schedule_cfg, step_scale, lr_scale),
                            subjects, lambdas)
     n_iters = int(n_steps * step_scale)
     gens = _sampling_plan(subjects, n_iters)
-    fitter = BatchedJointFitter(decoder, decoder_expr, [len(s) for s in subjects], device)
+    fitter = batched(decoder, decoder_expr, [len(s) for s in subjects], device)
     lr = 0.01 * lr_scale
     for j in range(n_iters):
         lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)

@@ -1,10 +1,13 @@
 #!/usr/bin/env python
 """Scan-batched fitting on one GPU: S scans in one launch sequence per iteration against the sequential native path.
 
-    python tools/bench_fit_batched.py [--scans 1 2 4 8 16] [--iters 50] [--reps 3] [--profile DIR]
+    python tools/bench_fit_batched.py [--decoder {nphm,npm}] [--scans 1 2 4 8 16] [--iters 50] [--reps 3] [--profile DIR]
 
 Identity: BatchedIdentityFitter.step on S scans of 5 x 1000 points vs S IdentityFitter.step calls.  Joint:
-BatchedJointFitter.step on S subjects (3 observations each, 5 x 1000 sampled points) vs S JointFitter.step calls.  The points
+BatchedJointFitter.step on S subjects (3 observations each, 5 x 1000 sampled points) vs S JointFitter.step calls.
+--decoder npm: the NPM baseline's DeepSDF decoders (515 -> 1024 x 8 -> 1 and 715 -> 1024 x 8 -> 3, tests/npm_fit_common.py)
+with BatchedNpmIdentityFitter / BatchedNpmJointFitter against NpmIdentityFitter / NpmJointFitter; its JSON lines carry
+"decoder": "npm".  The points
 are sampled once per configuration (host sampling is the same for both paths and not timed).  Batched and sequential runs of
 `--iters` iterations alternate `--reps` times; CUDA events, median.  Prints one JSON line per (mode, S): scan-iterations/s of
 both paths, peak device memory of the batched run, the card and its power limit.  --profile DIR: a torch.profiler kernel table
@@ -45,17 +48,27 @@ def timed(fn, iters):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--decoder', choices=['nphm', 'npm'], default='nphm')
     ap.add_argument('--scans', type=int, nargs='+', default=[1, 2, 4, 8, 16])
     ap.add_argument('--iters', type=int, default=50)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--profile', default=None)
     args = ap.parse_args()
     from conftest import make_deformation, make_ensemble
-    from nphm_b200.models.fitting import (BatchedIdentityFitter, BatchedJointFitter, IdentityFitter, JointFitter,
+    from nphm_b200.models.fitting import (BatchedIdentityFitter, BatchedJointFitter, BatchedNpmIdentityFitter,
+                                          BatchedNpmJointFitter, IdentityFitter, JointFitter, NpmIdentityFitter, NpmJointFitter,
                                           _sample_observations)
     dev = torch.device('cuda:0')
-    dec = make_ensemble(0, device=dev).train()
-    dfn = make_deformation(dev)
+    if args.decoder == 'npm':
+        import npm_fit_common
+        from nphm_b200.models.deepSDF import DeepSDF
+        dec, dfn = npm_fit_common.make_decoders(DeepSDF, dev)
+        BId, Id, BJoint, Joint = BatchedNpmIdentityFitter, NpmIdentityFitter, BatchedNpmJointFitter, NpmJointFitter
+    else:
+        dec = make_ensemble(0, device=dev).train()
+        dfn = make_deformation(dev)
+        BId, Id, BJoint, Joint = BatchedIdentityFitter, IdentityFitter, BatchedJointFitter, JointFitter
+    tag = {'decoder': 'npm'} if args.decoder == 'npm' else {}
     name = card()
 
     def setups(S):
@@ -64,10 +77,10 @@ def main():
         samples = [_sample_observations(s) for s in subs]
         obs = [o for o, _ in samples]
         idx = [i.long().to(dev) for _, i in samples]
-        bf = BatchedIdentityFitter(dec, S, dev)
-        singles = [IdentityFitter(dec, dev) for _ in range(S)]
-        bj = BatchedJointFitter(dec, dfn, [3] * S, dev)
-        jsingles = [JointFitter(dec, dfn, 3, dev) for _ in range(S)]
+        bf = BId(dec, S, dev)
+        singles = [Id(dec, dev) for _ in range(S)]
+        bj = BJoint(dec, dfn, [3] * S, dev)
+        jsingles = [Joint(dec, dfn, 3, dev) for _ in range(S)]
         return {
             'identity': (lambda: bf.step(obs, LAMBDAS, 0.1, 0.01),
                          lambda: [f.step(o, LAMBDAS, 0.1, 0.01) for f, o in zip(singles, obs)]),
@@ -87,7 +100,7 @@ def main():
                 ts.append(timed(sequential, args.iters))
             peak_b = torch.cuda.max_memory_allocated(dev)
             mb, ms = float(np.median(tb)), float(np.median(ts))
-            print(json.dumps({'mode': mode, 'scans': S, 'batched_ms_per_iter': round(mb, 4),
+            print(json.dumps({**tag, 'mode': mode, 'scans': S, 'batched_ms_per_iter': round(mb, 4),
                               'sequential_ms_per_iter': round(ms, 4),
                               'batched_scan_it_per_s': round(1000.0 * S / mb, 1),
                               'sequential_scan_it_per_s': round(1000.0 * S / ms, 1),
@@ -106,8 +119,9 @@ def main():
                 for _ in range(10):
                     batched()
                 torch.cuda.synchronize()
-            with open(os.path.join(args.profile, 'fit_batched_%s_S4.txt' % mode), 'w') as f:
-                f.write('%s, 10 batched iterations at S = 4\n' % name)
+            prefix = 'fit_batched_npm' if args.decoder == 'npm' else 'fit_batched'
+            with open(os.path.join(args.profile, '%s_%s_S4.txt' % (prefix, mode)), 'w') as f:
+                f.write('%s, 10 batched iterations at S = 4\n' % ', '.join([name] + list(tag.values())))
                 f.write(prof.key_averages().table(sort_by='cuda_time_total', row_limit=30))
 
 
