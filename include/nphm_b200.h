@@ -409,6 +409,45 @@ int nphm_render_depth_normals(const float *verts_dev, long long n_verts, const i
                               double zfar, int height, int width, float *depth_dev, unsigned char *normals_dev, int *tri_dev,
                               void *workspace_dev, long long workspace_bytes, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Narrow-band mesh extraction: the steps of extract_mesh_narrowband (nphm_b200/utils/reconstruction.py, DESIGN §4.13), which
+ * gives the mesh of `mesh_from_logits(get_logits(...))` on a res^3 grid while evaluating the decoder only near the surface.
+ * The (res-1)^3 cells are split into blocks of block^3 cells (the last block of an axis may be partial); block b covers the
+ * voxels [b*block, min(b*block + block, res-1)] of every axis.  The decoder is evaluated by the caller, through the existing
+ * query entry points, on coordinates these calls gather; the band state lives in the caller's workspace:
+ *   nphm_band_begin      resets the state; quirk_period > 0: lists the eval-mode quirk voxels (g % p == p-1 or g == res^3-1,
+ *                        which the caller evaluates in a query of period 1) and activates every block owning a cell that touches one
+ *   nphm_band_corners    lists the block corners not evaluated yet (fine indices 0, block, 2 block, ..., res-1)
+ *   nphm_band_classify   activates the blocks with a corner |sdf| <= tau (or NaN) or corners on both sides of the marching-cubes
+ *                        test (-sdf <= 0), then lists the voxels of all newly activated blocks not evaluated yet
+ *   nphm_band_grow       activates every inactive block with an evaluated face voxel on the other side of the test from its
+ *                        corner 0, then lists as classify does (0 listed: the band is closed)
+ *   nphm_band_fill       gives every voxel not evaluated the value of corner 0 of an (inactive) block containing it
+ * A listing call writes its list, ascending in the flat index z + res (y + res x), to the workspace and, when counts_host is not
+ * NULL, {voxels listed, blocks active so far} to counts_host[0..1] (synchronises the stream).  nphm_band_gather writes the
+ * float32(linspace_f64(min, max, res)) coordinates of the first n listed voxels to xyz_dev (n x 3; those of
+ * create_grid_points_from_bounds and nphm_ensemble_query_grid); nphm_band_scatter writes values_dev[i] to vol_dev[list[i]]
+ * (i < n), and every listed voxel counts as evaluated.  vol_dev: res^3 floats, x slowest.
+ * Needs 2 <= res <= 1024, 1 <= block <= 64, tau >= 0 (else NPHM_ERR_INVALID); workspace_bytes (checked, NPHM_ERR_CAPACITY when
+ * short) >= nphm_band_workspace_bytes(res, block). */
+/* bytes of the band workspace (-1: bad arguments) */
+long long nphm_band_workspace_bytes(int res, int block);
+int nphm_band_begin(int res, int block, long long quirk_period, void *workspace_dev, long long workspace_bytes,
+                    long long *counts_host, void *stream);
+int nphm_band_corners(int res, int block, void *workspace_dev, long long workspace_bytes, long long *counts_host, void *stream);
+int nphm_band_gather(int res, int block, const double grid_min[3], const double grid_max[3], long long n, float *xyz_dev,
+                     void *workspace_dev, long long workspace_bytes, void *stream);
+int nphm_band_scatter(int res, int block, long long n, const float *values_dev, float *vol_dev, void *workspace_dev,
+                      long long workspace_bytes, void *stream);
+int nphm_band_classify(int res, int block, float tau, const float *vol_dev, void *workspace_dev, long long workspace_bytes,
+                       long long *counts_host, void *stream);
+int nphm_band_grow(int res, int block, const float *vol_dev, void *workspace_dev, long long workspace_bytes, long long *counts_host,
+                   void *stream);
+int nphm_band_fill(int res, int block, float *vol_dev, void *workspace_dev, long long workspace_bytes, void *stream);
+/* states_dev (blocks^3 bytes, blocks = ceil((res-1)/block), x slowest): 0 inactive, 1 or 2 active */
+int nphm_band_block_states(int res, int block, const void *workspace_dev, long long workspace_bytes, unsigned char *states_dev,
+                           void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -40,6 +40,8 @@ EXPORTED_SYMBOLS = (
     'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad', 'nphm_mlp_fit_surface_grad_batched',
     'nphm_ensemble_sdfgrad_workspace_bytes', 'nphm_ensemble_sdfgrad_forward', 'nphm_ensemble_sdfgrad_backward',
     'nphm_render_workspace_bytes', 'nphm_render_depth_normals',
+    'nphm_band_workspace_bytes', 'nphm_band_begin', 'nphm_band_corners', 'nphm_band_gather', 'nphm_band_scatter',
+    'nphm_band_classify', 'nphm_band_grow', 'nphm_band_fill', 'nphm_band_block_states',
 )
 
 
@@ -192,6 +194,17 @@ def lib() -> ctypes.CDLL:
     L.nphm_render_workspace_bytes.restype = c_longlong
     L.nphm_render_depth_normals.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_double,
                                             c_double, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_workspace_bytes.argtypes = [c_int, c_int]
+    L.nphm_band_workspace_bytes.restype = c_longlong
+    L.nphm_band_begin.argtypes = [c_int, c_int, c_longlong, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_corners.argtypes = [c_int, c_int, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_gather.argtypes = [c_int, c_int, POINTER(c_double), POINTER(c_double), c_longlong, c_void_p, c_void_p, c_longlong,
+                                   c_void_p]
+    L.nphm_band_scatter.argtypes = [c_int, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_classify.argtypes = [c_int, c_int, c_float, c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_grow.argtypes = [c_int, c_int, c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_fill.argtypes = [c_int, c_int, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_block_states.argtypes = [c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -804,3 +817,69 @@ def render_depth_normals(verts: torch.Tensor, faces: torch.Tensor, world_to_eye:
                                           float(znear), float(zfar), H, W, depth.data_ptr(), normals.data_ptr(), _ptr(tri),
                                           ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'nphm_render_depth_normals')
     return (depth.view(V, H, W), normals.view(V, H, W, 3), None if tri is None else tri.view(V, H, W))
+
+
+# ------------------------------------------------------------------------------------------ narrow-band extraction
+class NarrowBand:
+    """Band state of one ``res^3`` grid in blocks of ``block^3`` cells (``nphm_band_*``, DESIGN §4.13) in a workspace this object
+    owns.  The listing steps return the number of voxels they listed; :meth:`gather` / :meth:`scatter` move the listed voxels'
+    coordinates out and their values into a ``res^3`` float32 CUDA volume."""
+
+    def __init__(self, res: int, block: int, device):
+        self.res, self.block = int(res), int(block)
+        self.device = torch.device(device)
+        with torch.cuda.device(self.device):
+            self.ws = _workspace(lib().nphm_band_workspace_bytes(self.res, self.block), 'nphm_band_workspace_bytes', self.device)
+        self.blocks_per_axis = -(-(self.res - 1) // self.block)
+        self.active_blocks = 0
+
+    def _call_listing(self, name, *before_ws):
+        counts = (c_longlong * 2)()
+        with torch.cuda.device(self.device):
+            check(getattr(lib(), name)(self.res, self.block, *before_ws, self.ws.data_ptr(), self.ws.numel(), counts,
+                                       _stream_ptr(self.device)), name)
+        self.active_blocks = counts[1]
+        return counts[0]
+
+    def begin(self, quirk_period: int = 0) -> int:
+        """Reset; with ``quirk_period > 0`` list the eval-mode quirk voxels and activate the blocks around them."""
+        return self._call_listing('nphm_band_begin', int(quirk_period))
+
+    def corners(self) -> int:
+        return self._call_listing('nphm_band_corners')
+
+    def classify(self, tau: float, vol: torch.Tensor) -> int:
+        return self._call_listing('nphm_band_classify', float(tau), vol.data_ptr())
+
+    def grow(self, vol: torch.Tensor) -> int:
+        return self._call_listing('nphm_band_grow', vol.data_ptr())
+
+    def gather(self, n: int, mini, maxi) -> torch.Tensor:
+        """(n, 3) float32 coordinates of the first ``n`` listed voxels."""
+        xyz = torch.empty(int(n), 3, device=self.device, dtype=torch.float32)
+        gmin = (c_double * 3)(*[float(v) for v in mini])
+        gmax = (c_double * 3)(*[float(v) for v in maxi])
+        with torch.cuda.device(self.device):
+            check(lib().nphm_band_gather(self.res, self.block, gmin, gmax, int(n), _ptr(xyz) if n else None, self.ws.data_ptr(),
+                                         self.ws.numel(), _stream_ptr(self.device)), 'nphm_band_gather')
+        return xyz
+
+    def scatter(self, values: torch.Tensor, vol: torch.Tensor):
+        v = _f32c(values).reshape(-1)
+        with torch.cuda.device(self.device):
+            check(lib().nphm_band_scatter(self.res, self.block, v.numel(), v.data_ptr() if v.numel() else None, vol.data_ptr(),
+                                          self.ws.data_ptr(), self.ws.numel(), _stream_ptr(self.device)), 'nphm_band_scatter')
+
+    def fill(self, vol: torch.Tensor):
+        with torch.cuda.device(self.device):
+            check(lib().nphm_band_fill(self.res, self.block, vol.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
+                                       _stream_ptr(self.device)), 'nphm_band_fill')
+
+    def block_states(self) -> torch.Tensor:
+        """(blocks, blocks, blocks) bool: which blocks are active."""
+        nb = self.blocks_per_axis
+        out = torch.empty(nb, nb, nb, device=self.device, dtype=torch.uint8)
+        with torch.cuda.device(self.device):
+            check(lib().nphm_band_block_states(self.res, self.block, self.ws.data_ptr(), self.ws.numel(), out.data_ptr(),
+                                               _stream_ptr(self.device)), 'nphm_band_block_states')
+        return out != 0
