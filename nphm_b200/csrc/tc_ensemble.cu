@@ -5,9 +5,9 @@
 //
 // Math (SURVEY.md 8a'): per member, per point
 //   h0 = sp(W0x c + v0)            K=3   -> CUDA cores (v0 = latent part + bias, per query/member)
-//   h1 = sp(W1 h0 + b1)            64x112x208 wgmma per warpgroup   (N 101 -> 112, K 200 -> 208)
-//   h2 = sp(W2a h1/r2 + W2x c/r2 + v2)   64x208x112 wgmma   (K = 101 + 3 -> 112)
-//   h3 = sp(W3 h2 + b3)            64x208x208 wgmma
+//   h1 = sp(W1 h0 + b1)            64x104x208 wgmma per warpgroup   (N 101 -> 104, K 200 -> 208)
+//   h2 = sp(W2a h1/r2 + W2x c/r2 + v2)   64x200x112 wgmma   (K = 101 + 3 -> 112)
+//   h3 = sp(W3 h2 + b3)            64x200x208 wgmma
 //   s  = w4 . h3 + b4              CUDA cores, on the layer-3 accumulators; Gaussian anchor blend in registers.
 // Precision: tensor cores run fp16 MMAs with fp32 accumulation; every operand is split in two fp16 terms
 // (x = hi + lo, 22 significant bits) and each product is evaluated as hi*hi + hi*lo + lo*hi (3 MMAs), which
@@ -21,33 +21,26 @@ namespace nphm {
 namespace tc {
 
 // ------------------------------------------------------------------------------------------------ packing
-// Weight slabs: for weight set s, tensor layer L (1..3), k-step j: N x 16 fp16 hi then N x 16 fp16 lo, each in
-// no-swizzle K-major core-matrix order: byte offset of (n, kk) = (n/8)*256 + (kk/8)*128 + (n%8)*16 + (kk%8)*2.
+// Weight units (tc_ensemble.cuh): for weight set s, unit u, k-step j of the unit: nw x 16 fp16 hi then nw x 16 fp16 lo, each in
+// no-swizzle K-major core-matrix order: byte offset of (n, kk) = (n/8)*256 + (kk/8)*128 + (n%8)*16 + (kk%8)*2, n counted from
+// the unit's first column.
 // Bias rows: the K padding of layers 1 and 3 (k = 200) carries S * b_l (per weight set, no latent part); the A operand has
 // the constant 1.0 at that k, so the MMAs add the bias and the epilogues do not (layer 2's constant depends on the latent:
-// its k-step-6 slab is re-built per (query, member), see l2_slab_kernel).
+// its k-step-6 slabs are re-built per (query, member), see l2_slab_kernel).
 __global__ void pack_slabs_kernel(const float *__restrict__ W1, const float *__restrict__ W2, const float *__restrict__ W3,
                                   const float *__restrict__ b1, const float *__restrict__ b3,
                                   int n_sets, uint8_t *__restrict__ out)
 {
-    const int total_per_set = (kKS1 * kNP1 + (kKS2 + kKS3) * kNP2) * 16;       // (slab, n, kk) triples
+    const int total_per_set = kSetBytes / 4;       // (unit, k-step, n, kk) quadruples: 4 bytes (hi + lo) each
     const float inv_sqrt2 = 0.70710678118654752440f;
     for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < (size_t)n_sets * total_per_set;
          t += (size_t)gridDim.x * blockDim.x) {
         const int s = (int)(t / total_per_set);
-        int r = (int)(t % total_per_set);
-        int layer, j, n, kk, np;
-        size_t slab_off;
-        if (r < kKS1 * kNP1 * 16) {
-            layer = 1; np = kNP1; j = r / (np * 16); r -= j * np * 16; slab_off = (size_t)j * kSlab1Bytes;
-        } else if ((r -= kKS1 * kNP1 * 16) < kKS2 * kNP2 * 16) {
-            layer = 2; np = kNP2; j = r / (np * 16); r -= j * np * 16; slab_off = kL1Bytes + (size_t)j * kSlabBytes;
-        } else {
-            r -= kKS2 * kNP2 * 16;
-            layer = 3; np = kNP3; j = r / (np * 16); r -= j * np * 16; slab_off = kL1Bytes + kL2Bytes + (size_t)j * kSlabBytes;
-        }
-        n = r / 16; kk = r % 16;
-        const int k = j * 16 + kk;
+        int r = (int)(t % total_per_set), u = 0;
+        while (r >= unit_bytes(u) / 4) { r -= unit_bytes(u) / 4; ++u; }
+        const int layer = unit_layer(u), nw = unit_nw(u);
+        const int j = r / (nw * 16), nl = (r / 16) % nw, kk = r % 16;
+        const int n = unit_n0(u) + nl, k = (unit_k0(u) + j) * 16 + kk;
         float v = 0.f;
         if (layer == 1) {
             if (n < kN1 && k < kH) v = W1[((size_t)s * kN1 + n) * kH + k];
@@ -61,10 +54,10 @@ __global__ void pack_slabs_kernel(const float *__restrict__ W1, const float *__r
         }
         const __half hi = __float2half_rn(v);
         const __half lo = __float2half_rn(v - __half2float(hi));
-        const size_t off = (size_t)(n >> 3) * 256 + (size_t)(kk >> 3) * 128 + (size_t)(n & 7) * 16 + (size_t)(kk & 7) * 2;
-        uint8_t *base = out + (size_t)s * kSetBytes + slab_off;
+        const size_t off = (size_t)(nl >> 3) * 256 + (size_t)(kk >> 3) * 128 + (size_t)(nl & 7) * 16 + (size_t)(kk & 7) * 2;
+        uint8_t *base = out + (size_t)s * kSetBytes + unit_off(u) + (size_t)j * nw * 64;
         *reinterpret_cast<__half *>(base + off) = hi;
-        *reinterpret_cast<__half *>(base + (size_t)np * 32 + off) = lo;
+        *reinterpret_cast<__half *>(base + (size_t)nw * 32 + off) = lo;
     }
 }
 
@@ -78,7 +71,7 @@ __global__ void records_kernel(const float *__restrict__ cvec, int cvec_stride, 
     const float *cv = cvec + ((size_t)qi * n_members + m) * cvec_stride;
     float *rec = recs + ((size_t)qi * n_members + m) * kRecFloats;
     const int d_in = 3 + kCond;
-    for (int n = threadIdx.x; n < kNP2; n += blockDim.x) {
+    for (int n = threadIdx.x; n < 208; n += blockDim.x) {
         const float *w = W0 + ((size_t)set * kH + (n < kH ? n : 0)) * d_in;
         const bool real = n < kH;
         rec[kRecL0 + 4 * n + 0] = real ? w[0] : 0.f;
@@ -86,8 +79,8 @@ __global__ void records_kernel(const float *__restrict__ cvec, int cvec_stride, 
         rec[kRecL0 + 4 * n + 2] = real ? w[2] : 0.f;
         rec[kRecL0 + 4 * n + 3] = real ? kS * cv[coff[0] + n] : 0.f;
     }
-    for (int n = threadIdx.x; n < kNP1; n += blockDim.x) rec[kRecB1 + n] = n < kN1 ? kS * cv[coff[1] + n] : 0.f;
-    for (int n = threadIdx.x; n < kNP2; n += blockDim.x) {
+    for (int n = threadIdx.x; n < 112; n += blockDim.x) rec[kRecB1 + n] = n < kN1 ? kS * cv[coff[1] + n] : 0.f;
+    for (int n = threadIdx.x; n < 208; n += blockDim.x) {
         rec[kRecB2 + n] = n < kH ? kS * cv[coff[2] + n] : 0.f;
         rec[kRecB3 + n] = n < kH ? kS * cv[coff[3] + n] : 0.f;
         rec[kRecW4 + n] = n < kH ? W4[(size_t)set * kH + n] / kS : 0.f;
@@ -106,26 +99,33 @@ __global__ void records_kernel(const float *__restrict__ cvec, int cvec_stride, 
 }
 
 // Layer 2's per-column constant v2 = S * (b2 + W2u u / sqrt(2)) depends on the latent, i.e. on (query, member): the last
-// k-step slab of layer 2 (k 96..111, of which 96..103 are real inputs) is copied per (query, member) and its K-padding row
-// k = 104 filled with v2 (fp16 hi | lo); the A operand carries 1.0 there.  13 KB per (query, member).
+// k-step slabs of layer 2 (k 96..111, of which 96..103 are real inputs; column half a then half b) are copied per (query,
+// member) and their K-padding row k = 104 filled with v2 (fp16 hi | lo); the A operand carries 1.0 there.  12.5 KB per
+// (query, member).
 __global__ void l2_slab_kernel(const uint8_t *__restrict__ weights, const float *__restrict__ cvec, int cvec_stride,
                                const int *__restrict__ coff, int n_members, int n_symm, uint8_t *__restrict__ out)
 {
     const int m = blockIdx.x, qi = blockIdx.y;
     const int set = member_set(m, n_symm);
-    const uint4 *src = reinterpret_cast<const uint4 *>(weights + (size_t)set * kSetBytes + kL1Bytes + (size_t)(kKS2 - 1) * kSlabBytes);
-    uint8_t *dst = out + ((size_t)qi * n_members + m) * kSlabBytes;
-    for (int i = threadIdx.x; i < kSlabBytes / 16; i += blockDim.x) reinterpret_cast<uint4 *>(dst)[i] = src[i];
+    const uint8_t *w = weights + (size_t)set * kSetBytes;
+    uint8_t *dst = out + ((size_t)qi * n_members + m) * kL2SlabBytes;
+    for (int i = threadIdx.x; i < kL2SlabBytes / 16; i += blockDim.x) {
+        const bool half_b = i >= kL2SlabABytes / 16;
+        const uint8_t *src = half_b ? w + unit_off(3) + (kKS2 - 1) * kNB * 64 - kL2SlabABytes : w + unit_off(2) + (kKS2 - 1) * kNA * 64;
+        reinterpret_cast<uint4 *>(dst)[i] = reinterpret_cast<const uint4 *>(src)[i];
+    }
     __syncthreads();
     const float *cv = cvec + ((size_t)qi * n_members + m) * cvec_stride;
     const int kk = (kN1 + 3) - (kKS2 - 1) * 16;          // 104 - 96 = 8
-    for (int n = threadIdx.x; n < kNP2; n += blockDim.x) {
+    for (int n = threadIdx.x; n < kNA + kNB; n += blockDim.x) {
         const float v = n < kH ? kS * cv[coff[2] + n] : 0.f;
         const __half hi = __float2half_rn(v);
         const __half lo = __float2half_rn(v - __half2float(hi));
-        const size_t off = (size_t)(n >> 3) * 256 + (size_t)(kk >> 3) * 128 + (size_t)(n & 7) * 16 + (size_t)(kk & 7) * 2;
-        *reinterpret_cast<__half *>(dst + off) = hi;
-        *reinterpret_cast<__half *>(dst + (size_t)kNP2 * 32 + off) = lo;
+        const int nw = n < kNA ? kNA : kNB, nl = n < kNA ? n : n - kNA;
+        uint8_t *slab = dst + (n < kNA ? 0 : kL2SlabABytes);
+        const size_t off = (size_t)(nl >> 3) * 256 + (size_t)(kk >> 3) * 128 + (size_t)(nl & 7) * 16 + (size_t)(kk & 7) * 2;
+        *reinterpret_cast<__half *>(slab + off) = hi;
+        *reinterpret_cast<__half *>(slab + (size_t)nw * 32 + off) = lo;
     }
 }
 
@@ -223,7 +223,7 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
                                                  h->weights.W[4].as<float>(), q.anchors, h->n_members, h->cfg.n_symm_pairs,
                                                  h->tc_consts.as<float>());
     NPHM_CUDA_CHECK(cudaGetLastError());
-    if ((rc = h->tc_l2slabs.reserve((size_t)q.n_queries * h->n_members * tc::kSlabBytes))) return rc;
+    if ((rc = h->tc_l2slabs.reserve((size_t)q.n_queries * h->n_members * tc::kL2SlabBytes))) return rc;
     tc::l2_slab_kernel<<<grid, 256, 0, stream>>>(h->tc_weights.as<uint8_t>(), q.cvec, h->dims.cvec_stride, h->tc_coff.as<int>(),
                                                  h->n_members, h->cfg.n_symm_pairs, h->tc_l2slabs.as<uint8_t>());
     NPHM_CUDA_CHECK(cudaGetLastError());

@@ -10,13 +10,29 @@ namespace tc {
 constexpr int kH = 200;            // hidden width
 constexpr int kN1 = 101;           // layer-1 width (hidden - d_in)
 constexpr int kCond = 96;
-constexpr int kNP1 = 112, kNP2 = 208, kNP3 = 208;
+constexpr int kNP1 = 104;                            // layer-1 MMA width (101 -> 104)
+constexpr int kNA = 112, kNB = 88;                   // column halves of the 200-wide layers 2 and 3 (200 = 112 + 88)
 constexpr int kKS1 = 13, kKS2 = 7, kKS3 = 13;       // k-steps of 16
-constexpr int kSlab1Bytes = kNP1 * 64;               // hi + lo, 16 K-columns
-constexpr int kSlabBytes = kNP2 * 64;
-constexpr int kGroupBytes = 7 * kSlabBytes;             // weight groups: L1 | L2 | L3 k-steps 0-6 | L3 k-steps 7-12
-constexpr int kL1Bytes = kKS1 * kSlab1Bytes, kL2Bytes = kKS2 * kSlabBytes, kL3Bytes = kKS3 * kSlabBytes;
-constexpr int kSetBytes = kL1Bytes + kL2Bytes + kL3Bytes;     // 359424 per weight set
+// Weight units: each weight set is packed in the order the kernel consumes it, as 8 units of at most kUnitMaxBytes that one
+// bulk copy each fills: L1 k-steps 0-6 | 7-12, L2 half a | half b, L3 half a k-steps 0-6 | 7-12, L3 half b k-steps 0-6 | 7-12.
+// A unit holds consecutive k-step slabs of one column range: per k-step nw x 16 fp16 hi then nw x 16 fp16 lo (nw x 64 bytes).
+constexpr int kUnits = 8;
+__host__ __device__ constexpr int unit_layer(int u) { return u < 2 ? 1 : (u < 4 ? 2 : 3); }
+__host__ __device__ constexpr int unit_n0(int u) { return (u == 3 || u >= 6) ? kNA : 0; }            // first column
+__host__ __device__ constexpr int unit_nw(int u) { return u < 2 ? kNP1 : ((u == 3 || u >= 6) ? kNB : kNA); }
+__host__ __device__ constexpr int unit_k0(int u) { return (u == 1 || u == 5 || u == 7) ? 7 : 0; }    // first k-step
+__host__ __device__ constexpr int unit_nk(int u) { return (u == 1 || u == 5 || u == 7) ? 6 : 7; }
+__host__ __device__ constexpr int unit_bytes(int u) { return unit_nk(u) * unit_nw(u) * 64; }
+__host__ __device__ constexpr int unit_off(int u)
+{
+    int off = 0;
+    for (int i = 0; i < u; ++i) off += unit_bytes(i);
+    return off;
+}
+constexpr int kUnitMaxBytes = 7 * kNA * 64;                 // 50176
+constexpr int kSetBytes = unit_off(kUnits);                // 342528 per weight set
+// the last k-step slab of layer 2 of both column halves, re-built per (query, member) with the latent-dependent bias row
+constexpr int kL2SlabABytes = kNA * 64, kL2SlabBytes = (kNA + kNB) * 64;
 constexpr int kRecSlots = 3;
 // activation derivatives saved per (member, point) for the fitting backward: sigma'0 [208] | sigma'1 [112] | sigma'2 [208] | sigma'3 [208]
 constexpr int kActOff0 = 0, kActOff1 = 208, kActOff2 = 320, kActLd = 528;
@@ -33,7 +49,7 @@ constexpr int kRecFloats = 1576;
 struct Params {
     const uint8_t *weights;     // [n_sets][kSetBytes]
     const float *recs;          // [n_queries][n_members][kRecFloats]
-    const uint8_t *l2_slabs;    // [n_queries][n_members][kSlabBytes]: last k-step slab of layer 2 with the latent-dependent bias row
+    const uint8_t *l2_slabs;    // [n_queries][n_members][kL2SlabBytes]: last k-step slabs of layer 2 (half a | half b) with the latent-dependent bias row
     const float *xyz;
     const float *axes;
     int res;

@@ -5,34 +5,61 @@
 //
 // A CTA is persistent over 128-point tiles: two consumer warpgroups of 64 points each and one producer warpgroup, which
 // hands most of its registers to the consumers (setmaxnreg: 24 / 240 per thread).
-//   producer (warp 8, one lane): bulk async copies of the record of every member and of its weight groups
-//       L1 | L2 | L3 k-steps 0-6 | L3 k-steps 7-12 into two shared-memory buffers (one mbarrier pair each).
+//   producer (warp 8, one lane): bulk async copies of the record of every member and of its 8 weight units (tc_ensemble.cuh)
+//       into a ring of 4 shared-memory slots (one mbarrier pair each), up to 4 units ahead of the consumers.  A slot is
+//       released when the MMAs of both warpgroups on it have retired.
 //   consumers (warps 0-7): per member, layer 0 on CUDA cores straight into registers; layers 1-3 as 64 x N x 16 wgmmas with
 //       A in REGISTERS and B (weights) in shared memory.  The accumulator layout of a 64 x N wgmma is the register layout of
 //       its A operand (tc_common.cuh), so the epilogue of a layer (softplus, fp16 hi/lo split) produces the next layer's A
 //       operand in place, without a round trip through memory.  The output layer (dot with w4) and the anchor blend run on
 //       the accumulator registers of layer 3.
-// Wide layers are issued in two column halves (112 + 96) so that the accumulators and the A operand of a layer fit the
-// register file together: the first half of layer 2 is converted while the MMAs of the second half run.
+// Wide layers are issued in two column halves (112 + 88) so that the accumulators and the A operand of a layer fit the
+// register file together: the first half of layer 2 is converted while the MMAs of the second half run.  MMA issue
+// alternates between the two warpgroups phase by phase (layer 1, layer 2, layer 3 half a, layer 3 half b), so that one
+// warpgroup's epilogue (and its next member's layer 0) runs while the other one's MMAs occupy the tensor cores.  The
+// accumulation order of every output is that of a single warpgroup running alone: the results do not depend on the offset.
 #include "tc_ensemble.cuh"
 
 namespace nphm {
 namespace tc {
 namespace wg {
 
+#ifdef NPHM_ENS_TRACE
+// Timeline of CTA 0 (tools/ens_trace.py): clock64 stamps of kTraceMembers consecutive members, from the kTraceFirst-th member
+// the CTA evaluates.  [0] = CTA start, then per member kTraceStride stamps: consumer warpgroup 0 | warpgroup 1 (kTraceWg each:
+// phase p (L1, L2, L3 half a, L3 half b) event e at 6 p + e, e = weight wait start, weights ready, MMA issue start, MMAs
+// issued, MMAs retired, epilogue done; member start at 24, layer 0 done at 25) | producer (unit u issued at u, slot wait
+// start at 8 + u).
+constexpr int kTraceFirst = 4, kTraceMembers = 4, kTraceWg = 32, kTraceStride = 2 * kTraceWg + 16;
+__device__ long long g_ens_trace[1 + kTraceMembers * kTraceStride];
+#define ENS_STAMP(member, off) do { const int mi_ = (int)(member) - kTraceFirst;                                           \
+        if (blockIdx.x == 0 && mi_ >= 0 && mi_ < kTraceMembers) g_ens_trace[1 + mi_ * kTraceStride + (off)] = clock64(); } while (0)
+#define ENS_CEVT(member, phase, e) do { if ((threadIdx.x & 127) == 0)                                                       \
+        ENS_STAMP(member, (threadIdx.x >> 7) * kTraceWg + 6 * (phase) + (e)); } while (0)
+#define ENS_CMARK(member, off) do { if ((threadIdx.x & 127) == 0) ENS_STAMP(member, (threadIdx.x >> 7) * kTraceWg + (off)); } while (0)
+#define ENS_PEVT(member, off) ENS_STAMP(member, 2 * kTraceWg + (off))
+#else
+#define ENS_CEVT(member, phase, e) do { } while (0)
+#define ENS_CMARK(member, off) do { } while (0)
+#define ENS_PEVT(member, off) do { } while (0)
+#endif
+
 constexpr int kConsumerWarps = 8;
 constexpr int kThreads = 32 * (kConsumerWarps + 4);
 constexpr int kUnits208 = 13, kUnits112 = 7;
-constexpr uint32_t kHalfRows = 14 * 256;       // byte offset of slab row 112 (the second column half of a 208-wide layer)
+constexpr int kSlots = 4;                      // weight ring: unit u of every member lands in slot u % 4
+constexpr int kTurnBar = 1;                    // named barriers kTurnBar + w: "warpgroup w may issue its MMAs"
+static_assert(kUnits == 2 * kSlots, "unit u uses slot u % 4 on its (u / 4)-th use per member");
 
 struct __align__(128) Smem {
-    uint8_t wbuf[2][kGroupBytes];            // weight groups (one bulk copy + one barrier each)
+    uint8_t wbuf[kSlots][kUnitMaxBytes];     // weight units (one bulk copy + one barrier each)
     float rec[kRecSlots][kRecFloats];
-    uint64_t w_full[2], w_empty[2];
+    uint64_t w_full[kSlots], w_empty[kSlots];
     uint64_t rec_full[kRecSlots], rec_empty[kRecSlots];
     uint64_t mask_ready;
     unsigned long long maskq[2][kConsumerWarps];
 };
+static_assert(sizeof(Smem) <= 227 * 1024, "shared memory of the ensemble kernel exceeds the 227 KB of an H100 block");
 
 // 3 MMAs of one k-step (hi*hi + hi*lo + lo*hi): `b` = shared address of the slab's hi half, its lo half lies lo_off further
 template <int N, typename F>
@@ -45,7 +72,8 @@ __device__ __forceinline__ void kstep(F &&mma, float (&d)[N / 2], const uint32_t
     mma(d, al, bh, 1);
 }
 
-// k-step j of an accumulator -> A registers of the next layer.  f(value, column, row 0/1, element) returns the activation.
+// k-step j of an accumulator -> A registers of the next layer.  f(value, column, row 0/1, element) returns the activation;
+// columns beyond the accumulator (the constant columns of the next layer's operand) pass 0 as the value.
 template <int N, typename F>
 __device__ __forceinline__ void to_operand(const float (&d)[N], int j, int col0, int q4, uint32_t (&ah)[4], uint32_t (&al)[4], F &&f)
 {
@@ -57,7 +85,7 @@ __device__ __forceinline__ void to_operand(const float (&d)[N], int j, int col0,
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 const int col = col0 + 16 * j + 8 * hh + 2 * q4 + e;
-                v[r][2 * hh + e] = f(d[4 * (2 * j + hh) + 2 * r + e], col, r, 2 * hh + e);
+                v[r][2 * hh + e] = f(4 * (2 * j + hh) < N ? d[4 * (2 * j + hh) + 2 * r + e] : 0.f, col, r, 2 * hh + e);
             }
     split2(v[0][0], v[0][1], ah[0], al[0]);
     split2(v[1][0], v[1][1], ah[1], al[1]);
@@ -86,19 +114,21 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     };
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) { mbar_init(&sm.w_full[i], 1); mbar_init(&sm.w_empty[i], kConsumerWarps); }
+        for (int i = 0; i < kSlots; ++i) { mbar_init(&sm.w_full[i], 1); mbar_init(&sm.w_empty[i], kConsumerWarps); }
         for (int i = 0; i < kRecSlots; ++i) { mbar_init(&sm.rec_full[i], 1); mbar_init(&sm.rec_empty[i], kConsumerWarps); }
         mbar_init(&sm.mask_ready, kConsumerWarps);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
+#ifdef NPHM_ENS_TRACE
+    if (blockIdx.x == 0 && threadIdx.x == 0) g_ens_trace[0] = clock64();
+#endif
 
     if (warp >= kConsumerWarps) {
         // =========================================================================== producer (bulk async copies)
         asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
         if (warp == kConsumerWarps && lane == 0) {
-            int wb = 0;
-            uint32_t wph = 0, tcount = 0, rcount = 0;
+            uint32_t tcount = 0, rcount = 0;
             for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
                 const long long tile = ACTS ? item / n_groups : item;
                 const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
@@ -117,21 +147,24 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                     ++rcount;
                     const int set = m < 2 * p.n_symm ? (m >> 1) : m - p.n_symm;
                     const uint8_t *w = p.weights + (size_t)set * kSetBytes;
+                    const uint8_t *l2 = p.l2_slabs + ((size_t)qi * p.n_members + m) * kL2SlabBytes;
 #pragma unroll 1
-                    for (int g = 0; g < 4; ++g) {
-                        const uint32_t bytes = g == 0 ? kL1Bytes : (g == 1 ? kL2Bytes : (g == 2 ? 7 * kSlabBytes : 6 * kSlabBytes));
-                        mbar_wait(&sm.w_empty[wb], wph ^ 1);
-                        mbar_expect_tx(&sm.w_full[wb], bytes);
-                        if (g == 1) {
+                    for (int u = 0; u < kUnits; ++u) {
+                        // every member has 8 units, so unit u always goes to slot u % 4, on its (u / 4)-th use per member
+                        const int slot = u & 3;
+                        const uint32_t bytes = unit_bytes(u);
+                        ENS_PEVT(rcount - 1, 8 + u);
+                        mbar_wait(&sm.w_empty[slot], ((u >> 2) & 1) ^ 1);
+                        ENS_PEVT(rcount - 1, u);
+                        mbar_expect_tx(&sm.w_full[slot], bytes);
+                        if (u == 2 || u == 3) {
                             // layer 2: the last k-step slab carries this (query, member)'s bias row (l2_slab_kernel)
-                            bulk_g2s(sm.wbuf[wb], w, bytes - kSlabBytes, &sm.w_full[wb]);
-                            bulk_g2s(sm.wbuf[wb] + (bytes - kSlabBytes), p.l2_slabs + ((size_t)qi * p.n_members + m) * kSlabBytes,
-                                     kSlabBytes, &sm.w_full[wb]);
+                            const uint32_t last = unit_nw(u) * 64;
+                            bulk_g2s(sm.wbuf[slot], w + unit_off(u), bytes - last, &sm.w_full[slot]);
+                            bulk_g2s(sm.wbuf[slot] + (bytes - last), l2 + (u == 3 ? kL2SlabABytes : 0), last, &sm.w_full[slot]);
                         } else {
-                            bulk_g2s(sm.wbuf[wb], w, bytes, &sm.w_full[wb]);
+                            bulk_g2s(sm.wbuf[slot], w + unit_off(u), bytes, &sm.w_full[slot]);
                         }
-                        w += bytes;
-                        if (++wb == 2) { wb = 0; wph ^= 1; }
                     }
                 }
             }
@@ -141,14 +174,26 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
 
     // =========================================================================== consumer warpgroups
     asm volatile("setmaxnreg.inc.sync.aligned.u32 240;" ::: "memory");
-    const int q4 = lane & 3;
+    const int q4 = lane & 3, wgi = warp >> 2;
     int rl[2];                                   // tile rows (points) of this thread's accumulator rows
-    rl[0] = 64 * (warp >> 2) + 16 * (warp & 3) + (lane >> 2);
+    rl[0] = 64 * wgi + 16 * (warp & 3) + (lane >> 2);
     rl[1] = rl[0] + 8;
-    int wb = 0;
-    uint32_t wph = 0, tcount = 0, rcount = 0;
-    auto release = [&](uint64_t *bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
-    auto next_buf = [&]() { if (++wb == 2) { wb = 0; wph ^= 1; } };
+    uint32_t tcount = 0, rcount = 0;
+    auto release = [&](int u) { __syncwarp(); if (lane == 0) mbar_arrive(&sm.w_empty[u & 3]); };
+    auto release_rec = [&](uint64_t *bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+    auto wait_unit = [&](int u) { mbar_wait(&sm.w_full[u & 3], (u >> 2) & 1); };
+    auto unit_addr = [&](int u) { return smem_u32(sm.wbuf[u & 3]); };
+    // MMA issue alternates between the warpgroups, phase by phase (named barriers kTurnBar + warpgroup): a warpgroup
+    // issues, hands the turn to the other one and runs its epilogue while the other warpgroup's MMAs occupy the tensor cores.
+    auto take_turn = [&]() {
+        if (wgi == 0) asm volatile("bar.sync %0, 256;" ::"n"(kTurnBar) : "memory");
+        else asm volatile("bar.sync %0, 256;" ::"n"(kTurnBar + 1) : "memory");
+    };
+    auto pass_turn = [&]() {
+        if (wgi == 0) asm volatile("bar.arrive %0, 256;" ::"n"(kTurnBar + 1) : "memory");
+        else asm volatile("bar.arrive %0, 256;" ::"n"(kTurnBar) : "memory");
+    };
+    if (wgi == 1) pass_turn();                   // warpgroup 0 issues first
 
     for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
         const long long tile = ACTS ? item / n_groups : item;
@@ -226,6 +271,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
         for (int m = 0; m < p.n_members; ++m) {
             if (!((mask >> m) & 1)) continue;
             const uint32_t rslot = rcount % kRecSlots;
+            ENS_CMARK(rcount, 24);
             mbar_wait(&sm.rec_full[rslot], (rcount / kRecSlots) & 1);
             const float *rec = sm.rec[rslot];
             float cx[2], cy[2], cz[2];
@@ -270,24 +316,33 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 split2(v[0][2], v[0][3], a0h[j][2], a0l[j][2]);
                 split2(v[1][2], v[1][3], a0h[j][3], a0l[j][3]);
             }
+            ENS_CMARK(rcount, 25);
 
-            // ---------------- layer 1 (N 112, K 208)
-            float acc1[56];
+            // ---------------- layer 1 (N 104, K 208: units 0 | 1)
+            float acc1[kNP1 / 2];
 #pragma unroll
-            for (int i = 0; i < 56; ++i) acc1[i] = 0.f;
-            mbar_wait(&sm.w_full[wb], wph);
+            for (int i = 0; i < kNP1 / 2; ++i) acc1[i] = 0.f;
+            ENS_CEVT(rcount, 0, 0);
+            wait_unit(0);
+            wait_unit(1);
+            ENS_CEVT(rcount, 0, 1);
+            take_turn();
+            ENS_CEVT(rcount, 0, 2);
             {
-                const uint32_t b0 = smem_u32(sm.wbuf[wb]);
                 wg_fence();
 #pragma unroll
-                for (int j = 0; j < kUnits208; ++j)
-                    kstep<112>(wgmma_rs_n112, acc1, a0h[j], a0l[j], b0 + j * kSlab1Bytes, kNP1 * 32);
+                for (int j = 0; j < kUnits208; ++j) {
+                    kstep<kNP1>(wgmma_rs_n104, acc1, a0h[j], a0l[j], unit_addr(j < 7 ? 0 : 1) + (j % 7) * kNP1 * 64, kNP1 * 32);
+                }
                 wg_commit();
+                pass_turn();
+                ENS_CEVT(rcount, 0, 3);
                 wg_wait<0>();
                 wg_reg_fence(acc1);
+                ENS_CEVT(rcount, 0, 4);
             }
-            release(&sm.w_empty[wb]);
-            next_buf();
+            release(0);
+            release(1);
 
             // ---------------- epilogue of layer 1 -> A operand of layer 2 (K 112: h1 (101) | c (3) | 1.0 (bias row) | zeros)
             uint32_t a1h[kUnits112][4], a1l[kUnits112][4];
@@ -301,14 +356,21 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                     save_act(kActOff1, col, r, a);
                     return a;
                 });
+            ENS_CEVT(rcount, 0, 5);
 
-            // ---------------- layer 2 (N 208 = 112 + 96, K 112): the first half is converted while the second one runs
-            float acc2a[56], acc2b[48];
+            // ---------------- layer 2 (N 200 = 112 (unit 2) + 88 (unit 3), K 112): the first half is converted while the
+            // second one runs
+            float acc2a[kNA / 2], acc2b[kNB / 2];
 #pragma unroll
-            for (int i = 0; i < 56; ++i) acc2a[i] = 0.f;
+            for (int i = 0; i < kNA / 2; ++i) acc2a[i] = 0.f;
 #pragma unroll
-            for (int i = 0; i < 48; ++i) acc2b[i] = 0.f;
-            mbar_wait(&sm.w_full[wb], wph);
+            for (int i = 0; i < kNB / 2; ++i) acc2b[i] = 0.f;
+            ENS_CEVT(rcount, 1, 0);
+            wait_unit(2);
+            wait_unit(3);
+            ENS_CEVT(rcount, 1, 1);
+            take_turn();
+            ENS_CEVT(rcount, 1, 2);
             uint32_t a2h[kUnits208][4], a2l[kUnits208][4];
             auto e2 = [&](float t, int col, int r, int e) {
                 const float a = col < kH ? sp_sel(t, e) : (col == kH ? 1.0f : 0.0f);     // k = 200: bias row of layer 3
@@ -316,60 +378,57 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 return a;
             };
             {
-                const uint32_t b0 = smem_u32(sm.wbuf[wb]);
                 wg_fence();
 #pragma unroll
                 for (int j = 0; j < kUnits112; ++j)
-                    kstep<112>(wgmma_rs_n112, acc2a, a1h[j], a1l[j], b0 + j * kSlabBytes, kNP2 * 32);
+                    kstep<kNA>(wgmma_rs_n112, acc2a, a1h[j], a1l[j], unit_addr(2) + j * kNA * 64, kNA * 32);
                 wg_commit();
 #pragma unroll
                 for (int j = 0; j < kUnits112; ++j)
-                    kstep<96>(wgmma_rs_n96, acc2b, a1h[j], a1l[j], b0 + j * kSlabBytes + kHalfRows, kNP2 * 32);
+                    kstep<kNB>(wgmma_rs_n88, acc2b, a1h[j], a1l[j], unit_addr(3) + j * kNB * 64, kNB * 32);
                 wg_commit();
+                pass_turn();
+                ENS_CEVT(rcount, 1, 3);
                 wg_wait<1>();
                 wg_reg_fence(acc2a);
+                release(2);
 #pragma unroll
                 for (int j = 0; j < 7; ++j) to_operand(acc2a, j, 0, q4, a2h[j], a2l[j], e2);
                 wg_wait<0>();
                 wg_reg_fence(acc2b);
+                ENS_CEVT(rcount, 1, 4);
             }
-            release(&sm.w_empty[wb]);
-            next_buf();
+            release(3);
 #pragma unroll
-            for (int j = 0; j < 6; ++j) to_operand(acc2b, j, 112, q4, a2h[7 + j], a2l[7 + j], e2);
+            for (int j = 0; j < 6; ++j) to_operand(acc2b, j, kNA, q4, a2h[7 + j], a2l[7 + j], e2);
+            ENS_CEVT(rcount, 1, 5);
 
-            // ---------------- layer 3 (N 208 = 112 + 96, K 208 in two weight groups) and the output layer w4 . h3 + b4
-            const int wbA = wb;
-            const uint32_t phA = wph;
-            next_buf();
-            const int wbB = wb;
-            const uint32_t phB = wph;
-            next_buf();
-            mbar_wait(&sm.w_full[wbA], phA);
-            mbar_wait(&sm.w_full[wbB], phB);
-            const uint32_t bA = smem_u32(sm.wbuf[wbA]), bB = smem_u32(sm.wbuf[wbB]);
+            // ---------------- layer 3 (N 200 = 112 (units 4, 5) + 88 (units 6, 7), K 208) and the output layer w4 . h3 + b4
             float part[2] = {0.f, 0.f};
             // sigma'3 is the A operand of the first backward GEMM: saved operand-ready (tc_linear.cuh "packed": per k-step = unit
             // of 16 features [128 x 16 fp16 hi | 128 x 16 fp16 lo], core-matrix order), zeros in the K padding
             uint8_t *const pk = ACTS ? p.acts_packed_out + ((size_t)m * n_tiles + tile) * p.acts_packed_tile_steps * 8192
                                      : nullptr;
             auto out_layer = [&](const auto &acc, int col0, int units) {
+                constexpr int kAcc = sizeof(acc) / sizeof(float);
 #pragma unroll
                 for (int j = 0; j < units; ++j)
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
                         for (int r = 0; r < 2; ++r) {
-                            float v[2];
+                            float v[2] = {0.f, 0.f};
+                            if (4 * (2 * j + hh) < kAcc) {          // columns 200-207 have no accumulator (w4 is zero there)
 #pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int col = col0 + 16 * j + 8 * hh + 2 * q4 + e;
-                                v[e] = sp_sel(acc[4 * (2 * j + hh) + 2 * r + e], e);
-                                part[r] = fmaf(v[e], rec[kRecW4 + col], part[r]);          // w4 is zero in the padding
-                                if (ACTS) {
-                                    float ex;
-                                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(-v[e]));
-                                    v[e] = col < kH ? 1.0f - ex : 0.f;
+                                for (int e = 0; e < 2; ++e) {
+                                    const int col = col0 + 16 * j + 8 * hh + 2 * q4 + e;
+                                    v[e] = sp_sel(acc[4 * (2 * j + hh) + 2 * r + e], e);
+                                    part[r] = fmaf(v[e], rec[kRecW4 + col], part[r]);
+                                    if (ACTS) {
+                                        float ex;
+                                        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(-v[e]));
+                                        v[e] = 1.0f - ex;
+                                    }
                                 }
                             }
                             if (ACTS) {
@@ -383,33 +442,56 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                         }
             };
             {
-                float acc3[56];
+                float acc3[kNA / 2];
 #pragma unroll
-                for (int i = 0; i < 56; ++i) acc3[i] = 0.f;
+                for (int i = 0; i < kNA / 2; ++i) acc3[i] = 0.f;
+                ENS_CEVT(rcount, 2, 0);
+                wait_unit(4);
+                wait_unit(5);
+                ENS_CEVT(rcount, 2, 1);
+                take_turn();
+                ENS_CEVT(rcount, 2, 2);
                 wg_fence();
 #pragma unroll
-                for (int j = 0; j < kUnits208; ++j)
-                    kstep<112>(wgmma_rs_n112, acc3, a2h[j], a2l[j], (j < 7 ? bA + j * kSlabBytes : bB + (j - 7) * kSlabBytes), kNP3 * 32);
+                for (int j = 0; j < kUnits208; ++j) {
+                    kstep<kNA>(wgmma_rs_n112, acc3, a2h[j], a2l[j], unit_addr(j < 7 ? 4 : 5) + (j % 7) * kNA * 64, kNA * 32);
+                }
                 wg_commit();
+                pass_turn();
+                ENS_CEVT(rcount, 2, 3);
                 wg_wait<0>();
                 wg_reg_fence(acc3);
+                ENS_CEVT(rcount, 2, 4);
+                release(4);
+                release(5);
                 out_layer(acc3, 0, 7);
+                ENS_CEVT(rcount, 2, 5);
             }
             {
-                float acc3[48];
+                float acc3[kNB / 2];
 #pragma unroll
-                for (int i = 0; i < 48; ++i) acc3[i] = 0.f;
+                for (int i = 0; i < kNB / 2; ++i) acc3[i] = 0.f;
+                ENS_CEVT(rcount, 3, 0);
+                wait_unit(6);
+                wait_unit(7);
+                ENS_CEVT(rcount, 3, 1);
+                take_turn();
+                ENS_CEVT(rcount, 3, 2);
                 wg_fence();
 #pragma unroll
-                for (int j = 0; j < kUnits208; ++j)
-                    kstep<96>(wgmma_rs_n96, acc3, a2h[j], a2l[j], (j < 7 ? bA + j * kSlabBytes : bB + (j - 7) * kSlabBytes) + kHalfRows,
-                              kNP3 * 32);
+                for (int j = 0; j < kUnits208; ++j) {
+                    kstep<kNB>(wgmma_rs_n88, acc3, a2h[j], a2l[j], unit_addr(j < 7 ? 6 : 7) + (j % 7) * kNB * 64, kNB * 32);
+                }
                 wg_commit();
+                pass_turn();
+                ENS_CEVT(rcount, 3, 3);
                 wg_wait<0>();
                 wg_reg_fence(acc3);
-                release(&sm.w_empty[wbA]);
-                release(&sm.w_empty[wbB]);
-                out_layer(acc3, 112, 6);
+                ENS_CEVT(rcount, 3, 4);
+                release(6);
+                release(7);
+                out_layer(acc3, kNA, 6);
+                ENS_CEVT(rcount, 3, 5);
             }
 
             // ---------------- member output (reduced over the 4 lanes of a row) and the anchor blend
@@ -432,13 +514,14 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 num[r] = fmaf(w, quirk[r] ? 1.0f : s, num[r]);
                 if (!PRUNE) den[r] += w;
             }
-            release(&sm.rec_empty[rslot]);
+            release_rec(&sm.rec_empty[rslot]);
             ++rcount;
         }
 #pragma unroll
         for (int r = 0; r < 2; ++r)
             if (q4 == 0 && valid[r] && n_groups == 1) p.out[(size_t)qi * p.n_points + idx[r]] = __fdiv_rn(num[r], den[r] + 1e-6f);
     }
+    if (wgi == 0) take_turn();                   // the turn warpgroup 1 passed after its last phase
 }
 
 }  // namespace wg
@@ -456,3 +539,15 @@ int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cu
 
 }  // namespace tc
 }  // namespace nphm
+
+#ifdef NPHM_ENS_TRACE
+// Debug entry of the timeline build (tools/ens_trace.py): copies the stamps of the last ensemble launch to host memory.
+extern "C" int nphm_debug_ens_trace(long long *host, int n_ll)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(n_ll >= 1 && n_ll <= 1 + tc::wg::kTraceMembers * tc::wg::kTraceStride, "nphm_debug_ens_trace: bad length");
+    NPHM_CUDA_CHECK(cudaDeviceSynchronize());
+    NPHM_CUDA_CHECK(cudaMemcpyFromSymbol(host, tc::wg::g_ens_trace, (size_t)n_ll * 8));
+    return NPHM_OK;
+}
+#endif
