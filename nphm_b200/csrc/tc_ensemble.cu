@@ -238,16 +238,25 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     NPHM_REQUIRE(!q.acts_out || (q.exact && q.acts_packed_out && q.acts_packed_tile_steps >= tc::kActPackedSteps),
                  "activation dump needs an exact query");
     p.anchors = q.anchors; p.prune_tau = h->tc_prune_tau;
-    p.blocked = 0; p.px0 = p.px1 = 0; p.by = p.bz = 1;
+    // dense queries skip the members whose blend weight is exactly zero on a whole tile; fitting needs every member's output
+    p.zero_skip = !prune && !q.members_out && !q.acts_out;
+    p.blocked = 0; p.px0 = p.px1 = 0; p.by = p.bz = 1; p.tbx = p.tby = p.tbz = 1;
     long long n_tiles = ceil_div(q.n_points, 128) * q.n_queries;
-    if (prune && !q.xyz && q.n_points > 0) {
-        // compact blocks over the x-plane range that contains [first, first + n_points)
+    if ((prune || p.zero_skip) && !q.xyz && q.n_points > 0) {
+        // compact blocks over the x-plane range that contains [first, first + n_points), so that a tile is near few anchors:
+        // 8 x 4 x 4 for the pruned rule (its mask depends on the composition of a tile), 1 x 16 x 8 for the dense rule - it
+        // never crosses an x-plane, so plane-aligned ranges (the whole grid, x-slabs) tile without wasted rows
         const long long rr = (long long)q.res * q.res;
-        p.px0 = (int)(q.first / rr);
-        p.px1 = (int)((q.first + q.n_points - 1) / rr);
-        p.by = (q.res + 3) / 4; p.bz = (q.res + 3) / 4;
-        n_tiles = (long long)((p.px1 - p.px0 + 8) / 8) * p.by * p.bz;
-        p.blocked = 1;
+        const int tbx = prune ? 8 : 1, tby = prune ? 4 : 16, tbz = prune ? 4 : 8;
+        const int px0 = (int)(q.first / rr), px1 = (int)((q.first + q.n_points - 1) / rr);
+        const int by = (q.res + tby - 1) / tby, bz = (q.res + tbz - 1) / tbz;
+        const long long blocked_tiles = (long long)((px1 - px0 + tbx) / tbx) * by * bz;
+        // dense rule: keep linear tiles where blocks would add more than 3 % tiles (partial planes, small or odd grids)
+        if (prune || blocked_tiles * 100 <= n_tiles * 103) {
+            p.blocked = 1;
+            p.px0 = px0; p.px1 = px1; p.by = by; p.bz = bz; p.tbx = tbx; p.tby = tby; p.tbz = tbz;
+            n_tiles = blocked_tiles;
+        }
     }
     p.n_tiles = n_tiles;
     p.member_groups = 1;

@@ -63,12 +63,32 @@ struct Params {
     int acts_packed_tile_steps; // packed GEMM operand in the first kActPackedSteps k-steps of every (member, tile) block
     int n_members, n_symm;
     // pruned mode (opt-in): members whose normalised blend weight is < prune_tau for every point of a tile are skipped
-    const float *anchors;       // [n_queries][n_members-1][3]
+    const float *anchors;       // [n_queries][n_members-1][3] (bit for bit the anchors of the records)
     float prune_tau;
     int member_groups;          // activation-dump variant: CTAs per tile (each evaluates a range of members), >= 1
-    long long n_tiles;          // tiles to process (grid mode + pruning uses compact 8x4x4 blocks)
-    int blocked, px0, px1, by, bz;
+    // dense variant: a tile skips the members whose blend weight is exactly +0 at all of its points (bit-identical result)
+    int zero_skip;
+    long long n_tiles;          // tiles to process
+    // grid mode with compact tiles: blocks of tbx x tby x tbz grid points (tbx tby tbz = 128) over the x-planes px0..px1,
+    // by x bz blocks per plane
+    int blocked, px0, px1, by, bz, tbx, tby, tbz;
 };
+
+// Blend weight of a member at (x, y, z): exp(-(|a - x| + 1e-5)^2 / 0.01) for a member with anchor a, exp(-20) for the
+// global member.  The tile masks and the blend call this one function with the same inputs, so that a member skipped for
+// an exactly zero weight is one whose blend term would have been exactly zero.  The squared distance is spelled out as
+// fma(dz, dz, fma(dx, dx, dy * dy)), the contraction the compiler chose for dx * dx + dy * dy + dz * dz in the kernel before
+// this function existed, so that no inlining context can contract it another way.
+__device__ __forceinline__ float blend_weight(bool has_anchor, float ax, float ay, float az, float x, float y, float z)
+{
+    float d = -0.2f;
+    if (has_anchor) {
+        const float dx = ax - x, dy = ay - y, dz = az - z;
+        const float nrm = sqrtf(__fmaf_rn(dz, dz, __fmaf_rn(dx, dx, __fmul_rn(dy, dy)))) + 10e-6f;
+        d = -(nrm * nrm);
+    }
+    return expf(__fdiv_rn(d, 0.01f));
+}
 
 int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream);
 

@@ -18,6 +18,9 @@
 // alternates between the two warpgroups phase by phase (layer 1, layer 2, layer 3 half a, layer 3 half b), so that one
 // warpgroup's epilogue (and its next member's layer 0) runs while the other one's MMAs occupy the tensor cores.  The
 // accumulation order of every output is that of a single warpgroup running alone: the results do not depend on the offset.
+// At the start of a tile the consumers vote on which members the tile needs (dense: a blend weight that is not exactly zero
+// at some valid point; pruned: the tau rule) and the producer streams only those; grid queries use compact tiles
+// (Params::tbx, tby, tbz) so that a tile lies far from many anchors.
 #include "tc_ensemble.cuh"
 
 namespace nphm {
@@ -32,16 +35,26 @@ namespace wg {
 // start at 8 + u).
 constexpr int kTraceFirst = 4, kTraceMembers = 4, kTraceWg = 32, kTraceStride = 2 * kTraceWg + 16;
 __device__ long long g_ens_trace[1 + kTraceMembers * kTraceStride];
+// Tile boundaries of CTA 0, for its first kTraceTiles tiles: warpgroup 0 starts the tile, has the tile's member mask, has the
+// layer-1 weights of the tile's first member.
+constexpr int kTraceTiles = 4;
+__device__ long long g_ens_tiles[3 * kTraceTiles];
+// Work of every CTA: [0] = CTAs of the last launch, then per CTA the member-tiles it evaluated and its cycles.
+constexpr int kTraceMaxCtas = 1024;
+__device__ long long g_ens_ctas[1 + 2 * kTraceMaxCtas];
 #define ENS_STAMP(member, off) do { const int mi_ = (int)(member) - kTraceFirst;                                           \
         if (blockIdx.x == 0 && mi_ >= 0 && mi_ < kTraceMembers) g_ens_trace[1 + mi_ * kTraceStride + (off)] = clock64(); } while (0)
 #define ENS_CEVT(member, phase, e) do { if ((threadIdx.x & 127) == 0)                                                       \
         ENS_STAMP(member, (threadIdx.x >> 7) * kTraceWg + 6 * (phase) + (e)); } while (0)
 #define ENS_CMARK(member, off) do { if ((threadIdx.x & 127) == 0) ENS_STAMP(member, (threadIdx.x >> 7) * kTraceWg + (off)); } while (0)
 #define ENS_PEVT(member, off) ENS_STAMP(member, 2 * kTraceWg + (off))
+#define ENS_TILE(t, e) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (t) < kTraceTiles)                                   \
+        g_ens_tiles[3 * (t) + (e)] = clock64(); } while (0)
 #else
 #define ENS_CEVT(member, phase, e) do { } while (0)
 #define ENS_CMARK(member, off) do { } while (0)
 #define ENS_PEVT(member, off) do { } while (0)
+#define ENS_TILE(t, e) do { } while (0)
 #endif
 
 constexpr int kConsumerWarps = 8;
@@ -121,8 +134,11 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     }
     __syncthreads();
 #ifdef NPHM_ENS_TRACE
-    if (blockIdx.x == 0 && threadIdx.x == 0) g_ens_trace[0] = clock64();
+    const long long cta_start = clock64();
+    if (blockIdx.x == 0 && threadIdx.x == 0) { g_ens_trace[0] = cta_start; g_ens_ctas[0] = gridDim.x; }
 #endif
+    // the consumers vote on the members of every tile: the pruned rule, or (dense variant) exactly zero blend weights
+    const bool vote = PRUNE || (!ACTS && p.zero_skip);
 
     if (warp >= kConsumerWarps) {
         // =========================================================================== producer (bulk async copies)
@@ -133,7 +149,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 const long long tile = ACTS ? item / n_groups : item;
                 const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
                 unsigned long long mask = group_mask(item);
-                if (PRUNE) {
+                if (vote) {
                     mbar_wait(&sm.mask_ready, tcount & 1);
                     mask = 0;
                     for (int w = 0; w < kConsumerWarps; ++w) mask |= sm.maskq[tcount & 1][w];
@@ -198,17 +214,19 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
         const long long tile = ACTS ? item / n_groups : item;
         const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
+        ENS_TILE(tcount, 0);
         long long idx[2], g[2];
         bool valid[2], quirk[2];
         float x[2], y[2], z[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const int row = rl[i];
-            if (p.blocked) {
-                // compact 8 x 4 x 4 block of grid points (z fastest inside the block)
+            if (!ACTS && p.blocked) {             // (the fitting variant only runs linear tiles)
+                // compact tbx x tby x tbz block of grid points (z fastest inside the block)
                 const long long tz = tile % p.bz, txy = tile / p.bz;
                 const int ty = (int)(txy % p.by), tx = (int)(txy / p.by);
-                const int ix = p.px0 + tx * 8 + (row >> 4), iy = ty * 4 + ((row >> 2) & 3), iz = (int)tz * 4 + (row & 3);
+                const int ix = p.px0 + tx * p.tbx + row / (p.tby * p.tbz), iy = ty * p.tby + (row / p.tbz) % p.tby,
+                          iz = (int)tz * p.tbz + row % p.tbz;
                 g[i] = ((long long)ix * p.res + iy) * p.res + iz;
                 valid[i] = ix <= p.px1 && iy < p.res && iz < p.res && g[i] >= p.first && g[i] < p.first + p.n_points;
                 idx[i] = g[i] - p.first;
@@ -232,33 +250,33 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
         }
         float num[2] = {0.f, 0.f}, den[2] = {0.f, 0.f};
         unsigned long long mask = group_mask(item);
-        if (PRUNE) {
-            // blend weights of all members for this thread's points: S = sum_k w_k; a member is needed by the tile if
-            // w_k >= tau * (S + 1e-6) for at least one of its points (dropped mass per point < n_members * tau).
+        if (vote) {
+            // blend weights of the members for this thread's points (the last, global member is always needed: every tile
+            // evaluates >= 1 member).  Pruned rule: S = sum_k w_k; a member is needed if w_k >= tau * (S + 1e-6) for at least
+            // one valid point of the tile (dropped mass per point < n_members * tau).  Dense rule: a member is needed if
+            // w_k != 0 for at least one valid point - a member with w_k = +0 everywhere adds exactly nothing to num and den.
             const float *anc = p.anchors + (size_t)qi * (p.n_members - 1) * 3;
             auto weight = [&](int k, int i) {
-                float d = -0.2f;
-                if (k < p.n_members - 1) {
-                    const float dx = __ldg(anc + 3 * k) - x[i], dy = __ldg(anc + 3 * k + 1) - y[i], dz = __ldg(anc + 3 * k + 2) - z[i];
-                    const float nrm = sqrtf(dx * dx + dy * dy + dz * dz) + 10e-6f;
-                    d = -(nrm * nrm);
-                }
-                return expf(__fdiv_rn(d, 0.01f));
+                if (k == p.n_members - 1) return blend_weight(false, 0.f, 0.f, 0.f, x[i], y[i], z[i]);
+                return blend_weight(true, __ldg(anc + 3 * k), __ldg(anc + 3 * k + 1), __ldg(anc + 3 * k + 2), x[i], y[i], z[i]);
             };
-            float thr[2];
+            float thr[2] = {0.f, 0.f};
+            if (PRUNE) {
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                float S = 0.f;
-                for (int k = 0; k < p.n_members; ++k) S += weight(k, i);
-                den[i] = S;
-                thr[i] = p.prune_tau * (S + 1e-6f);
+                for (int i = 0; i < 2; ++i) {
+                    float S = 0.f;
+                    for (int k = 0; k < p.n_members; ++k) S += weight(k, i);
+                    den[i] = S;
+                    thr[i] = p.prune_tau * (S + 1e-6f);
+                }
             }
-            unsigned long long wm = 0;
-            for (int k = 0; k < p.n_members; ++k) {
-                const bool need = (valid[0] && weight(k, 0) >= thr[0]) || (valid[1] && weight(k, 1) >= thr[1]);
+            unsigned long long wm = 1ull << (p.n_members - 1);
+            for (int k = 0; k < p.n_members - 1; ++k) {
+                bool need;
+                if (PRUNE) need = (valid[0] && weight(k, 0) >= thr[0]) || (valid[1] && weight(k, 1) >= thr[1]);
+                else need = (valid[0] && weight(k, 0) != 0.f) || (valid[1] && weight(k, 1) != 0.f);
                 if (__any_sync(0xffffffffu, need)) wm |= 1ull << k;
             }
-            wm |= 1ull << (p.n_members - 1);      // every tile evaluates >= 1 member
             if (lane == 0) {
                 sm.maskq[tcount & 1][warp] = wm;
                 mbar_arrive(&sm.mask_ready);
@@ -267,6 +285,8 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
             mask = 0;
             for (int w = 0; w < kConsumerWarps; ++w) mask |= sm.maskq[tcount & 1][w];
         }
+        ENS_TILE(tcount, 1);
+        const uint32_t tile_rc0 = rcount;        // the tile's first member (timeline build)
 
         for (int m = 0; m < p.n_members; ++m) {
             if (!((mask >> m) & 1)) continue;
@@ -326,6 +346,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
             wait_unit(0);
             wait_unit(1);
             ENS_CEVT(rcount, 0, 1);
+            if (rcount == tile_rc0) ENS_TILE(tcount, 2);
             take_turn();
             ENS_CEVT(rcount, 0, 2);
             {
@@ -502,15 +523,8 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 s += __shfl_xor_sync(0xffffffffu, s, 2);
                 s += rec[kRecMisc + 0];
                 if (q4 == 0 && p.members_out && valid[r]) p.members_out[((size_t)qi * p.n_points + idx[r]) * p.n_members + m] = s;
-                float d;
-                if (rec[kRecMisc + 4] != 0.f) {
-                    const float dx = rec[kRecMisc + 1] - x[r], dy = rec[kRecMisc + 2] - y[r], dz = rec[kRecMisc + 3] - z[r];
-                    const float nrm = sqrtf(dx * dx + dy * dy + dz * dz) + 10e-6f;
-                    d = -(nrm * nrm);
-                } else {
-                    d = -0.2f;
-                }
-                const float w = expf(__fdiv_rn(d, 0.01f));
+                const float w = blend_weight(rec[kRecMisc + 4] != 0.f, rec[kRecMisc + 1], rec[kRecMisc + 2], rec[kRecMisc + 3],
+                                             x[r], y[r], z[r]);
                 num[r] = fmaf(w, quirk[r] ? 1.0f : s, num[r]);
                 if (!PRUNE) den[r] += w;
             }
@@ -522,6 +536,12 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
             if (q4 == 0 && valid[r] && n_groups == 1) p.out[(size_t)qi * p.n_points + idx[r]] = __fdiv_rn(num[r], den[r] + 1e-6f);
     }
     if (wgi == 0) take_turn();                   // the turn warpgroup 1 passed after its last phase
+#ifdef NPHM_ENS_TRACE
+    if (threadIdx.x == 0 && blockIdx.x < kTraceMaxCtas) {
+        g_ens_ctas[1 + 2 * blockIdx.x] = rcount;
+        g_ens_ctas[2 + 2 * blockIdx.x] = clock64() - cta_start;
+    }
+#endif
 }
 
 }  // namespace wg
@@ -548,6 +568,19 @@ extern "C" int nphm_debug_ens_trace(long long *host, int n_ll)
     NPHM_REQUIRE(n_ll >= 1 && n_ll <= 1 + tc::wg::kTraceMembers * tc::wg::kTraceStride, "nphm_debug_ens_trace: bad length");
     NPHM_CUDA_CHECK(cudaDeviceSynchronize());
     NPHM_CUDA_CHECK(cudaMemcpyFromSymbol(host, tc::wg::g_ens_trace, (size_t)n_ll * 8));
+    return NPHM_OK;
+}
+
+// Tile boundaries of CTA 0 (3 stamps per tile, kTraceTiles tiles) followed by the work of every CTA ([0] = CTAs, then per
+// CTA member-tiles and cycles) of the last ensemble launch.
+extern "C" int nphm_debug_ens_work(long long *host, int n_ll)
+{
+    using namespace nphm;
+    constexpr int nt = 3 * tc::wg::kTraceTiles, nc = 1 + 2 * tc::wg::kTraceMaxCtas;
+    NPHM_REQUIRE(n_ll == nt + nc, "nphm_debug_ens_work: bad length");
+    NPHM_CUDA_CHECK(cudaDeviceSynchronize());
+    NPHM_CUDA_CHECK(cudaMemcpyFromSymbol(host, tc::wg::g_ens_tiles, (size_t)nt * 8));
+    NPHM_CUDA_CHECK(cudaMemcpyFromSymbol(host + nt, tc::wg::g_ens_ctas, (size_t)nc * 8));
     return NPHM_OK;
 }
 #endif

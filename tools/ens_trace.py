@@ -2,7 +2,9 @@
 """Timeline of one CTA of the dense ensemble kernel (build with -DNPHM_ENS_TRACE: tools/build_variant.sh): runs one grid query
 of the seeded head of bench.py and prints, for four consecutive members of CTA 0, when each consumer warpgroup waited for its
 weights, issued and retired its MMAs and finished its epilogues, when the producer issued each weight unit, and per member:
-cycles waiting for weights, cycles in which neither warpgroup had MMAs in flight, epilogue cycles.
+cycles waiting for weights, cycles in which neither warpgroup had MMAs in flight, epilogue cycles.  Then, per tile of CTA 0,
+the cycles until the tile's member mask and its first member's weights were ready, and over all CTAs the member-tiles the
+kernel evaluated (to set against tools/zero_member_tiles.py) and the cycles per evaluated member-tile.
 
     bash tools/build_variant.sh /tmp/ens -DNPHM_ENS_TRACE && NPHM_B200_LIB=/tmp/ens/libnphm_b200.so python tools/ens_trace.py [res]"""
 import ctypes, os, sys
@@ -11,8 +13,9 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import numpy as np
 import torch
 
-# layout of g_ens_trace (csrc/tc_ensemble_wgmma.cu)
+# layout of g_ens_trace, g_ens_tiles and g_ens_ctas (csrc/tc_ensemble_wgmma.cu)
 MEMBERS, WG, STRIDE = 4, 32, 2 * 32 + 16
+TILES, MAX_CTAS = 4, 1024
 PHASES = ['L1', 'L2', 'L3a', 'L3b']
 EVENTS = ['wait', 'ready', 'turn', 'issued', 'retired', 'epi']
 
@@ -80,6 +83,21 @@ def main():
               % (span, wait, idle, epi))
     tt = np.array(totals, dtype=np.float64).mean(axis=0)
     print('mean per member: span %.0f, weight waits %.0f, no MMA in flight %.0f, epilogues %.0f' % tuple(tt))
+    if not hasattr(lib, 'nphm_debug_ens_work'):
+        return
+    buf = (ctypes.c_longlong * (3 * TILES + 1 + 2 * MAX_CTAS))()
+    _native.check(lib.nphm_debug_ens_work(buf, len(buf)), 'nphm_debug_ens_work')
+    w = np.array(buf[:], dtype=np.int64)
+    tiles = w[:3 * TILES].reshape(TILES, 3) - t0
+    for i in range(TILES):
+        length = ' (%d cycles to the next tile)' % (tiles[i + 1, 0] - tiles[i, 0]) if i + 1 < TILES else ''
+        print('tile %d of CTA 0: start %d, mask ready +%d, first member\'s layer-1 weights ready +%d%s'
+              % (i, tiles[i, 0], tiles[i, 1] - tiles[i, 0], tiles[i, 2] - tiles[i, 0], length))
+    n_ctas = int(w[3 * TILES])
+    ctas = w[3 * TILES + 1:3 * TILES + 1 + 2 * n_ctas].reshape(n_ctas, 2)
+    mt, cyc = int(ctas[:, 0].sum()), int(ctas[:, 1].sum())
+    print('all %d CTAs: %d member-tiles evaluated, %.0f cycles per evaluated member-tile (CTA cycles summed / member-tiles)'
+          % (n_ctas, mt, cyc / max(mt, 1)))
 
 
 if __name__ == '__main__':
