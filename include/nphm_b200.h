@@ -331,6 +331,29 @@ int nphm_ensemble_backward_inputs(nphm_ensemble *h, const float *points_dev, lon
                                   const float *grad_sdf_dev, float *sdf_out_dev, float *grad_latent_dev,
                                   float *grad_points_dev, void *workspace_dev, void *stream);
 
+/* ---- the same in eval mode: FastEnsembleDeepSDFMirrored.forward after decoder.eval() overwrites every member's output at the
+ * last point of each decoder call with 1 (reference src/NPHM/models/EnsembledDeepSDF.py:260-261, `sdf_pred[:, :, -1, 0] = 1`).
+ * Row i (0-based, within a scan) is such a quirk row when quirk_period p > 0 and i % p == p - 1; p = 0 is the training-mode
+ * forward and gives the results of the calls above bit for bit.  At a quirk row s_k = 1 and grad s_k = 0 for all members k, so
+ *   sdf = sum_k wt_k (the normalised blend weights, background included),   d sdf / d xyz = sum_k d wt_k / d xyz,
+ * the member inputs get no gradient from the row, the anchors / mlp_pos / z_glob do, through the weights.  Only the
+ * tensor-core configuration (hidden 200, 4 hidden layers, condition 96) takes p > 0 (else NPHM_ERR_UNSUPPORTED).
+ * == nphm_fit_identity_step for one iteration of inference_identity_space with the decoder in eval mode (fitting.py:229-236:
+ *    one call on the 5 sampled rows of n points each, so p = n) */
+int nphm_fit_identity_step_quirk(nphm_ensemble *h, const float *points_dev, long long n_points, long long quirk_period,
+                                 float *latent_dev, float *adam_m_dev, float *adam_v_dev, const nphm_fit_params *fp,
+                                 int apply_update, float *loss_terms_dev, float *grad_out_dev, void *workspace_dev, void *stream);
+/* == nphm_fit_surface_grad for the joint fitter in eval mode (fitting.py:111-125: `decoder(xc, ...)` on the 5 sampled rows of n
+ *    points, p = n) */
+int nphm_fit_surface_grad_quirk(nphm_ensemble *h, const float *points_dev, long long n_points, long long quirk_period,
+                                const float *latent_dev, const unsigned char *mask_dev, float clamp, float *loss_terms_dev,
+                                float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, void *stream);
+/* == nphm_ensemble_backward_inputs for `decoder.eval(); decoder(xyz, lat)[0].backward(grad_sdf)`: p = n_points is one call
+ *    (the stage-1 losses, loss_functions.py:36-42, make one call per point set) */
+int nphm_ensemble_backward_inputs_quirk(nphm_ensemble *h, const float *points_dev, long long n_points, long long quirk_period,
+                                        const float *latent_dev, const float *grad_sdf_dev, float *sdf_out_dev,
+                                        float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, void *stream);
+
 /* Second half of a fitting iteration (regularisers of fitting.py:252-268 + torch.optim.Adam, :278-279) for a surface
  * gradient that was evaluated elsewhere: the point-sharded fit of one head over several GPUs (north_star / SURVEY.md 8e)
  * evaluates nphm_fit_surface_grad on every rank's share of the sampled points, combines [n_r * grad_r, n_r * loss_r, n_r]
@@ -367,6 +390,17 @@ int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *points_dev, con
                                   long long n_points, const float *latents_dev, float clamp, float *loss_terms_dev,
                                   float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, long long workspace_bytes,
                                   void *stream);
+/* The same two in eval mode (see nphm_fit_identity_step_quirk): quirk_periods_dev [S] int32 on the device (may be NULL = all 0)
+ * holds each scan's period, the points per sampled observation row of that scan (n_k = min(1000, |obs|), fitting.py:111/114,
+ * :234/236); a scan's rows are numbered from 0 within the scan, so the padding after its last row is never a quirk row of it. */
+int nphm_fit_identity_step_batched_quirk(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
+                                         long long n_points, const int *quirk_periods_dev, float *latents_dev, float *adam_m_dev,
+                                         float *adam_v_dev, const nphm_fit_params *fp, int apply_update, float *loss_terms_dev,
+                                         float *grad_out_dev, void *workspace_dev, long long workspace_bytes, void *stream);
+int nphm_fit_surface_grad_batched_quirk(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
+                                        long long n_points, const int *quirk_periods_dev, const float *latents_dev, float clamp,
+                                        float *loss_terms_dev, float *grad_latent_dev, float *grad_points_dev,
+                                        void *workspace_dev, long long workspace_bytes, void *stream);
 /* == nphm_fit_apply_gradient per scan: surface_grad_dev [S][lat_dim], surface_stats_dev [S][2], grad_anchors_dev
  * [S][n_loc*3] (may be NULL), loss_terms_dev [S][8] and grad_out_dev [S][lat_dim] (may be NULL).  Any ensemble configuration;
  * the scratch is the handle's. */

@@ -33,6 +33,8 @@ EXPORTED_SYMBOLS = (
     'nphm_fit_workspace_bytes', 'nphm_fit_identity_step', 'nphm_fit_surface_grad', 'nphm_fit_apply_gradient',
     'nphm_fit_batch_workspace_bytes', 'nphm_fit_identity_step_batched', 'nphm_fit_surface_grad_batched',
     'nphm_fit_apply_gradient_batched',
+    'nphm_fit_identity_step_quirk', 'nphm_fit_surface_grad_quirk', 'nphm_fit_identity_step_batched_quirk',
+    'nphm_fit_surface_grad_batched_quirk', 'nphm_ensemble_backward_inputs_quirk',
     'nphm_ensemble_backward_inputs', 'nphm_ensemble_anchors',
     'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
@@ -159,6 +161,17 @@ def lib() -> ctypes.CDLL:
                                                 c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
     L.nphm_fit_apply_gradient_batched.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, POINTER(FitParams), c_void_p,
                                                   c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
+    L.nphm_fit_identity_step_quirk.argtypes = [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,
+                                               POINTER(FitParams), c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.nphm_fit_surface_grad_quirk.argtypes = [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_float, c_void_p,
+                                              c_void_p, c_void_p, c_void_p, c_void_p]
+    L.nphm_ensemble_backward_inputs_quirk.argtypes = [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,
+                                                      c_void_p, c_void_p, c_void_p, c_void_p]
+    L.nphm_fit_identity_step_batched_quirk.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p,
+                                                       c_void_p, c_void_p, POINTER(FitParams), c_int, c_void_p, c_void_p, c_void_p,
+                                                       c_longlong, c_void_p]
+    L.nphm_fit_surface_grad_batched_quirk.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_float,
+                                                      c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
     L.nphm_adam_step.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_float, c_int, c_void_p]
     L.nphm_mlp_inverse_jacobian.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p]
     L.nphm_broyden_workspace_bytes.argtypes = [c_longlong]
@@ -360,10 +373,12 @@ class EnsembleEngine(_Versioned):
                   'nphm_ensemble_anchors')
         return out
 
-    def backward_inputs(self, xyz: torch.Tensor, latent: torch.Tensor, grad_sdf: torch.Tensor):
+    def backward_inputs(self, xyz: torch.Tensor, latent: torch.Tensor, grad_sdf: torch.Tensor, quirk_period: int = 0):
         """Vector-Jacobian product of the training-mode forward (``nphm_ensemble_backward_inputs``): xyz (N,3), latent
         (lat_dim,), grad_sdf (N,) -> (sdf (N,), d/d latent (lat_dim,), d/d xyz (N,3)) - what autograd gives for
-        ``decoder(xyz, latent)[0].backward(grad_sdf)``, without building a graph."""
+        ``decoder(xyz, latent)[0].backward(grad_sdf)``, without building a graph.  ``quirk_period > 0``: the eval-mode forward
+        (``nphm_ensemble_backward_inputs_quirk``), every member's output is 1 at the rows with ``i % p == p - 1``; ``p = N`` is
+        one eval-mode decoder call."""
         dev = xyz.device
         pts = _f32c(xyz).reshape(-1, 3)
         lat = _f32c(latent).reshape(-1).to(dev)
@@ -373,9 +388,16 @@ class EnsembleEngine(_Versioned):
         g_lat = torch.empty(self.lat_dim, device=dev, dtype=torch.float32)
         g_pts = torch.empty(n, 3, device=dev, dtype=torch.float32)
         with torch.cuda.device(dev):
-            check(lib().nphm_ensemble_backward_inputs(self._h, pts.data_ptr(), n, lat.data_ptr(), g.data_ptr(), sdf.data_ptr(),
-                                                      g_lat.data_ptr(), g_pts.data_ptr(), None, _stream_ptr(dev)),
-                  'nphm_ensemble_backward_inputs')
+            if quirk_period:
+                check(lib().nphm_ensemble_backward_inputs_quirk(self._h, pts.data_ptr(), n, int(quirk_period), lat.data_ptr(),
+                                                                g.data_ptr(), sdf.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(),
+                                                                None, _stream_ptr(dev)),
+                      'nphm_ensemble_backward_inputs_quirk')
+            else:
+                check(lib().nphm_ensemble_backward_inputs(self._h, pts.data_ptr(), n, lat.data_ptr(), g.data_ptr(),
+                                                          sdf.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(), None,
+                                                          _stream_ptr(dev)),
+                      'nphm_ensemble_backward_inputs')
         return sdf, g_lat, g_pts
 
     # ---------------------------------------------------------------- training through grad_x sdf (second order)

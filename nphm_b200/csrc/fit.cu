@@ -76,7 +76,19 @@ struct Buffers {
     const float *upstream;          // optional n: d L / d sdf_p given by the caller (nphm_ensemble_backward_inputs) instead of the
                                     // clamped-|sdf| loss of the fitters
     float *sdf_out;                 // optional n: copy of the blended forward output
+    // eval-mode quirk of FastEnsembleDeepSDFMirrored (EnsembledDeepSDF.py:260-261: every member's output at the last point of
+    // each decoder call is overwritten with 1): row i of a scan with period p > 0 is a quirk row when i % p == p - 1.  The
+    // period is quirk_periods[scan] when that (device, one per scan) array is given, else quirk_period; 0 = training mode.
+    long long quirk_period;
+    const int *quirk_periods;
 };
+
+// whether row i_scan of scan `scan` carries the eval-mode quirk (s_k := 1, grad s_k := 0 for every member k)
+__device__ __forceinline__ bool quirk_row(const Buffers &b, int scan, long long i_scan)
+{
+    const long long p = b.quirk_periods ? (long long)b.quirk_periods[scan] : b.quirk_period;
+    return p > 0 && i_scan % p == p - 1;
+}
 
 template <bool BWD>
 __global__ void __launch_bounds__(kThreads, 1) fit_member_kernel(const Dims d, const Weights w, const Buffers b,
@@ -243,6 +255,7 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
     const long long idx = scan * b.n + i_scan;                                     // row of the point arrays
     const bool ok = i_scan < b.n;
     float x = 0.f, y = 0.f, z = 0.f, g_out = 0.f, Sp = 1.f, outv = 0.f;
+    const bool quirk = ok && quirk_row(b, scan, i_scan);     // members' outputs are the constant 1: no member upstream
     if (ok) {
         const float *stats = b.stats + (size_t)scan * 8;
         const float inv_count = stats[0] > 0.f ? 1.0f / stats[0] : 0.f;
@@ -266,9 +279,9 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
                 dd = -0.2f;
             }
             const float wk = expf(__fdiv_rn(dd, 0.01f));
-            gsv = g_out * wk / Sp;
+            gsv = quirk ? 0.f : g_out * wk / Sp;
             if (has_anchor && r > 0.f) {
-                const float s_k = b.member_s[idx * d.n_members + m];
+                const float s_k = quirk ? 1.0f : b.member_s[idx * d.n_members + m];
                 const float g_w = g_out * (s_k - outv) / Sp;
                 const float coef = g_w * wk * (1.0f / 0.01f) * (-2.0f) * (r + 10e-6f) / r;
                 c[0] = coef * dx; c[1] = coef * dy; c[2] = coef * dz;
@@ -406,7 +419,7 @@ __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d
     }
 }
 
-// sdf = sum_k w_k s_k / (sum_k w_k + 1e-6); kept = |sdf| < clamp   (fitting.py:234-246)
+// sdf = sum_k w_k s_k / (sum_k w_k + 1e-6); kept = |sdf| < clamp   (fitting.py:234-246); s_k = 1 at the eval-mode quirk rows
 __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
 {
     const int scan = blockIdx.y;
@@ -416,6 +429,7 @@ __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
     float cnt = 0.f, sum = 0.f;
     if (i_scan < b.n) {
         const float x = b.points[idx * 3], y = b.points[idx * 3 + 1], z = b.points[idx * 3 + 2];
+        const bool quirk = quirk_row(b, scan, i_scan);
         float num = 0.f, den = 0.f;
         for (int k = 0; k < d.n_members; ++k) {
             float dd;
@@ -427,7 +441,7 @@ __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
                 dd = -0.2f;
             }
             const float wk = expf(__fdiv_rn(dd, 0.01f));
-            num = fmaf(wk, b.member_s[idx * d.n_members + k], num);
+            num = fmaf(wk, quirk ? 1.0f : b.member_s[idx * d.n_members + k], num);
             den += wk;
         }
         const float out = __fdiv_rn(num, den + 1e-6f);
@@ -704,7 +718,7 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
                          float *adam_m_dev, float *adam_v_dev, const nphm_fit_params *fp, int apply_update,
                          float *loss_terms_dev, float *grad_out_dev, const unsigned char *mask_dev, float *grad_points_dev,
                          void *workspace_dev, long long workspace_bytes, void *stream_, const float *upstream_dev = nullptr,
-                         float *sdf_out_dev = nullptr)
+                         float *sdf_out_dev = nullptr, long long quirk_period = 0, const int *quirk_periods_dev = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     NPHM_REQUIRE(h && h->loaded, "nphm_fit_identity_step: weights not loaded");
@@ -715,6 +729,11 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
         return NPHM_ERR_UNSUPPORTED;
     }
     const bool tc_path = tc_ensemble_supported(h) && h->tc_ready;
+    NPHM_REQUIRE(quirk_period >= 0, "nphm_fit: quirk_period < 0");
+    if ((quirk_period > 0 || quirk_periods_dev) && !tc_path) {
+        set_error("the eval-mode quirk in fitting needs the tensor-core configuration (hidden 200, 4 layers, condition 96)");
+        return NPHM_ERR_UNSUPPORTED;
+    }
     if (n_scans > 1 && !tc_path) {
         set_error("scan-batched fitting needs the tensor-core configuration (hidden 200, 4 layers, condition 96)");
         return NPHM_ERR_UNSUPPORTED;
@@ -773,6 +792,8 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
     b.upstream = upstream_dev;
     b.sdf_out = sdf_out_dev;
     b.grad_points = grad_points_dev;
+    b.quirk_period = quirk_period;
+    b.quirk_periods = quirk_periods_dev;
 
     const int tiles = (int)ceil_div(n_points, fit::P);
     dim3 grid(tiles, h->n_members);
@@ -851,6 +872,15 @@ extern "C" int nphm_fit_identity_step(nphm_ensemble *h, const float *points_dev,
                          grad_out_dev, nullptr, nullptr, workspace_dev, -1, stream);
 }
 
+extern "C" int nphm_fit_identity_step_quirk(nphm_ensemble *h, const float *points_dev, long long n_points, long long quirk_period,
+                                            float *latent_dev, float *adam_m_dev, float *adam_v_dev, const nphm_fit_params *fp,
+                                            int apply_update, float *loss_terms_dev, float *grad_out_dev, void *workspace_dev,
+                                            void *stream)
+{
+    return fit_step_impl(h, points_dev, 1, n_points, latent_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
+                         grad_out_dev, nullptr, nullptr, workspace_dev, -1, stream, nullptr, nullptr, quirk_period);
+}
+
 static nphm_fit_params surface_params(float clamp)
 {
     nphm_fit_params fp{};
@@ -869,6 +899,17 @@ extern "C" int nphm_fit_surface_grad(nphm_ensemble *h, const float *points_dev, 
     const nphm_fit_params fp = surface_params(clamp);
     return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, loss_terms_dev,
                          grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream);
+}
+
+extern "C" int nphm_fit_surface_grad_quirk(nphm_ensemble *h, const float *points_dev, long long n_points, long long quirk_period,
+                                           const float *latent_dev, const unsigned char *mask_dev, float clamp,
+                                           float *loss_terms_dev, float *grad_latent_dev, float *grad_points_dev,
+                                           void *workspace_dev, void *stream)
+{
+    NPHM_REQUIRE(grad_latent_dev, "nphm_fit_surface_grad_quirk: grad_latent_dev is NULL");
+    const nphm_fit_params fp = surface_params(clamp);
+    return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, loss_terms_dev,
+                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream, nullptr, nullptr, quirk_period);
 }
 
 // the scan-batched entry points run only on the tensor-core path (no batched FFMA fallback)
@@ -894,6 +935,19 @@ extern "C" int nphm_fit_identity_step_batched(nphm_ensemble *h, const float *poi
                          grad_out_dev, mask_dev, nullptr, workspace_dev, workspace_bytes, stream);
 }
 
+extern "C" int nphm_fit_identity_step_batched_quirk(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev,
+                                                    int n_scans, long long n_points, const int *quirk_periods_dev,
+                                                    float *latents_dev, float *adam_m_dev, float *adam_v_dev,
+                                                    const nphm_fit_params *fp, int apply_update, float *loss_terms_dev,
+                                                    float *grad_out_dev, void *workspace_dev, long long workspace_bytes, void *stream)
+{
+    int rc;
+    if ((rc = require_batched(h, "nphm_fit_identity_step_batched_quirk", n_scans, workspace_dev))) return rc;
+    return fit_step_impl(h, points_dev, n_scans, n_points, latents_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
+                         grad_out_dev, mask_dev, nullptr, workspace_dev, workspace_bytes, stream, nullptr, nullptr, 0,
+                         quirk_periods_dev);
+}
+
 extern "C" int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
                                              long long n_points, const float *latents_dev, float clamp, float *loss_terms_dev,
                                              float *grad_latent_dev, float *grad_points_dev, void *workspace_dev,
@@ -907,11 +961,27 @@ extern "C" int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *poin
                          loss_terms_dev, grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, workspace_bytes, stream);
 }
 
+extern "C" int nphm_fit_surface_grad_batched_quirk(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev,
+                                                   int n_scans, long long n_points, const int *quirk_periods_dev,
+                                                   const float *latents_dev, float clamp, float *loss_terms_dev,
+                                                   float *grad_latent_dev, float *grad_points_dev, void *workspace_dev,
+                                                   long long workspace_bytes, void *stream)
+{
+    int rc;
+    if ((rc = require_batched(h, "nphm_fit_surface_grad_batched_quirk", n_scans, workspace_dev))) return rc;
+    NPHM_REQUIRE(loss_terms_dev && grad_latent_dev, "nphm_fit_surface_grad_batched_quirk: NULL loss terms or gradient");
+    const nphm_fit_params fp = surface_params(clamp);
+    return fit_step_impl(h, points_dev, n_scans, n_points, const_cast<float *>(latents_dev), nullptr, nullptr, &fp, 0,
+                         loss_terms_dev, grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, workspace_bytes, stream,
+                         nullptr, nullptr, 0, quirk_periods_dev);
+}
+
 // Vector-Jacobian product of the ensemble forward w.r.t. its inputs (SURVEY.md 8b: nphm_ensemble_backward_inputs):
 //   grad_points[p]  = grad_sdf[p] * d sdf_p / d xyz_p           (local coordinates of every member + blend weights)
 //   grad_latent     = sum_p grad_sdf[p] * d sdf_p / d latent     (member inputs + anchors/mlp_pos + blend weights)
 // for the training-mode forward (no eval quirk) of FastEnsembleDeepSDFMirrored (EnsembledDeepSDF.py:203-267) - what
-// torch.autograd computes for `decoder(xyz, lat)[0].backward(grad_sdf)`.  Same kernels as the fitting step.
+// torch.autograd computes for `decoder(xyz, lat)[0].backward(grad_sdf)`.  Same kernels as the fitting step.  The _quirk form
+// takes the eval-mode forward: quirk_period = n_points is one decoder call.
 extern "C" int nphm_ensemble_backward_inputs(nphm_ensemble *h, const float *points_dev, long long n_points, const float *latent_dev,
                                              const float *grad_sdf_dev, float *sdf_out_dev, float *grad_latent_dev,
                                              float *grad_points_dev, void *workspace_dev, void *stream)
@@ -920,6 +990,18 @@ extern "C" int nphm_ensemble_backward_inputs(nphm_ensemble *h, const float *poin
     const nphm_fit_params fp = surface_params(0.f);
     return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, nullptr,
                          grad_latent_dev, nullptr, grad_points_dev, workspace_dev, -1, stream, grad_sdf_dev, sdf_out_dev);
+}
+
+extern "C" int nphm_ensemble_backward_inputs_quirk(nphm_ensemble *h, const float *points_dev, long long n_points,
+                                                   long long quirk_period, const float *latent_dev, const float *grad_sdf_dev,
+                                                   float *sdf_out_dev, float *grad_latent_dev, float *grad_points_dev,
+                                                   void *workspace_dev, void *stream)
+{
+    NPHM_REQUIRE(grad_sdf_dev && grad_latent_dev, "nphm_ensemble_backward_inputs_quirk: NULL gradient pointer");
+    const nphm_fit_params fp = surface_params(0.f);
+    return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, nullptr,
+                         grad_latent_dev, nullptr, grad_points_dev, workspace_dev, -1, stream, grad_sdf_dev, sdf_out_dev,
+                         quirk_period);
 }
 
 // ------------------------------------------------------------------------------------------------ sharded fitting

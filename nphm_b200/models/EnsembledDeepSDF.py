@@ -192,13 +192,16 @@ class FastEnsembleDeepSDFMirrored(nn.Module):
             return False             # depth / width the native stack builder rejects: composite path
         return (xyz.dtype == torch.float32 and self.out_dim == 1 and self.input_dim == 3)
 
-    def _sdfgrad_unsupported(self, xyz: torch.Tensor, lat_rep: torch.Tensor) -> Optional[str]:
+    def _sdfgrad_unsupported(self, xyz: torch.Tensor, lat_rep: torch.Tensor, call_sizes=None) -> Optional[str]:
         if not (xyz.is_cuda and lat_rep.is_cuda):
             return 'needs CUDA points and codes'
         if xyz.dtype != torch.float32 or any(p.dtype != torch.float32 for p in self.parameters()):
             return 'needs fp32 points and parameters'
-        if not self.training:
-            return 'needs training mode (the eval-mode quirk stays on the composite path)'
+        if not self.training and call_sizes is None:
+            return ('needs training mode, or call_sizes in eval mode (the eval-mode forward overwrites the last point of '
+                    'every decoder call, so its result depends on where the calls end)')
+        if call_sizes is not None and (any(int(n) < 1 for n in call_sizes) or sum(int(n) for n in call_sizes) != xyz.shape[-2]):
+            return 'needs call_sizes of at least one point each that add up to the points of a batch element'
         e = self.ensembled_deep_sdf
         n_lin = e.num_layers - 1
         if not (self.out_dim == 1 and self.input_dim == 3 and
@@ -210,17 +213,23 @@ class FastEnsembleDeepSDFMirrored(nn.Module):
             return 'needs one code per batch element (B x 1 x lat_dim)'
         return None
 
-    def sdfgrad_supported(self, xyz: torch.Tensor, lat_rep: torch.Tensor) -> bool:
+    def sdfgrad_supported(self, xyz: torch.Tensor, lat_rep: torch.Tensor, call_sizes=None) -> bool:
         """Whether :meth:`forward_with_gradient_native` takes these inputs."""
-        return self._sdfgrad_unsupported(xyz, lat_rep) is None
+        return self._sdfgrad_unsupported(xyz, lat_rep, call_sizes) is None
 
-    def forward_with_gradient_native(self, xyz: torch.Tensor, lat_rep: torch.Tensor):
-        """``(sdf B x N x 1, d sdf / d xyz B x N x 3, anchors B x n_loc x 3)``: the training-mode forward followed by
+    def forward_with_gradient_native(self, xyz: torch.Tensor, lat_rep: torch.Tensor, call_sizes=None):
+        """``(sdf B x N x 1, d sdf / d xyz B x N x 3, anchors B x n_loc x 3)``: the forward followed by
         ``gradient(sdf, xyz)``, with the members' values, gradients and second-order backward on the native kernels (one
         launch per pass for all members) and the anchors, frames and Gaussian blend in autograd
         (``_composite.ensemble_blend_with_gradient``).  Differentiable to first order in the parameters and ``lat_rep``; the
-        points get no gradient.  Raises ``ValueError`` naming what it does not support."""
-        reason = self._sdfgrad_unsupported(xyz, lat_rep)
+        points get no gradient.  Raises ``ValueError`` naming what it does not support.
+
+        In eval mode ``call_sizes`` is required: the points of each batch element stand for consecutive decoder calls of
+        ``call_sizes[i]`` points each (they add up to N), and the reference's eval-mode forward sets every member's output to 1
+        at the last point of each call (EnsembledDeepSDF.py:260-261).  There s_k = 1 and grad s_k = 0 before the blend, so
+        the members' native passes see a zero upstream gradient at those rows.  In training mode ``call_sizes`` only
+        has to be consistent; it changes nothing."""
+        reason = self._sdfgrad_unsupported(xyz, lat_rep, call_sizes)
         if reason is not None:
             raise ValueError('forward_with_gradient_native: ' + reason)
         lat = lat_rep[:, :1]
@@ -231,6 +240,8 @@ class FastEnsembleDeepSDFMirrored(nn.Module):
             lin = getattr(e, 'lin%d' % i)
             params += [lin.weight, lin.bias]
         s, g = _NativeEnsembleSdfGradFn.apply(self.engine(), local, cond[:, :, 0], *params)
+        if not self.training:
+            s, g = _composite.apply_eval_quirk(s, g, call_sizes)
         sdf, grad = _composite.ensemble_blend_with_gradient(self, xyz.detach(), anchors, s, g)
         return sdf, grad, anchors
 

@@ -86,6 +86,26 @@ def ensemble_sdf(module, xyz, lat_rep):
     return gaussian_blend(xyz[..., :3], anchors, s.permute(1, 2, 0, 3), var=BLEND_VAR, background=True), anchors
 
 
+def call_ends(call_sizes):
+    """Indices along the point axis of the last point of each of consecutive decoder calls of ``call_sizes`` points: the rows
+    the eval-mode forward overwrites (EnsembledDeepSDF.py:260-261)."""
+    ends, end = [], 0
+    for n in call_sizes:
+        end += int(n)
+        ends.append(end - 1)
+    return ends
+
+
+def apply_eval_quirk(s, g, call_sizes):
+    """The eval-mode quirk on the members' values s (members x B x N (x 1)) and local gradients g (members x B x N x 3):
+    s_k = 1 and grad s_k = 0 at the last point of every call, as a differentiable select (those rows get no upstream)."""
+    s, g = s.clone(), g.clone()
+    for e in call_ends(call_sizes):
+        s[:, :, e] = 1
+        g[:, :, e] = 0
+    return s, g
+
+
 def ensemble_blend_with_gradient(module, xyz, anchors, s, g):
     """The blend of ``ensemble_sdf`` and its spatial gradient from the members' values and local-frame gradients.
 

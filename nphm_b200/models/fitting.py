@@ -83,12 +83,20 @@ def _current_anchors(decoder, lat_rep_shape, device):
 
 
 def _fused_identity(decoder) -> bool:
-    """The fused step implements the training-mode forward, which is how the reference runs its fitters
-    (scripts/fitting/fitting_pointclouds.py:268 calls ``decoder_shape.train()`` first).  In eval mode the reference's
-    forward overwrites the last point of every row (EnsembledDeepSDF.py:257-259): that case takes the autograd path."""
+    """Whether the fused fitting kernels take this decoder.  The reference runs its fitters in training mode
+    (scripts/fitting/fitting_pointclouds.py:268 calls ``decoder_shape.train()`` first).  In eval mode its forward overwrites
+    every member's output at the last point of each decoder call (EnsembledDeepSDF.py:260-261); the fused kernels reproduce
+    that through the quirk period of their ``_quirk`` entry points, which need the tensor-core configuration
+    (:func:`_tc_ensemble`).  Other eval-mode ensembles take the autograd path."""
     p = next(decoder.parameters())
-    return (isinstance(decoder, FastEnsembleDeepSDFMirrored) and p.is_cuda and decoder.training
-            and decoder.ensembled_deep_sdf.num_layers == 6)
+    if not (isinstance(decoder, FastEnsembleDeepSDFMirrored) and p.is_cuda and decoder.ensembled_deep_sdf.num_layers == 6):
+        return False
+    return decoder.training or _tc_ensemble(decoder)
+
+
+def _quirk_period(decoder, points_per_call: int) -> int:
+    """The quirk period of the fused calls: 0 in training mode, else the points of one reference decoder call."""
+    return 0 if decoder.training else int(points_per_call)
 
 
 class IdentityFitter:
@@ -106,25 +114,36 @@ class IdentityFitter:
         self.t = 0
 
     def step(self, points: torch.Tensor, lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
+        """One iteration on ``points`` (rows x n x 3: the reference's one decoder call on its sampled rows).  In eval mode the
+        last point of every row carries the quirk (``nphm_fit_identity_step_quirk`` with period n)."""
         pts = points.reshape(-1, 3).to(dtype=torch.float32).contiguous()
+        period = _quirk_period(self.decoder, points.shape[-2] if points.dim() > 1 else 1)
         if apply_update:
             self.t += 1
         fp = _native.FitParams(float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0)),
                                float(lambdas.get('reg_loc', 0.0)), float(lambdas.get('reg_unobserved', 0.0)),
                                float(lambdas.get('symm_dist', 0.0)), float(clamp), float(lr), max(self.t, 1))
+        stream = torch.cuda.current_stream(self.device).cuda_stream
         with torch.cuda.device(self.device):
-            _native.check(_native.lib().nphm_fit_identity_step(
-                self.engine.handle, pts.data_ptr(), pts.shape[0], self.latent.data_ptr(), self.m.data_ptr(),
-                self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(),
-                self.grad.data_ptr(), None, torch.cuda.current_stream(self.device).cuda_stream),
-                'nphm_fit_identity_step')
+            if period:
+                _native.check(_native.lib().nphm_fit_identity_step_quirk(
+                    self.engine.handle, pts.data_ptr(), pts.shape[0], period, self.latent.data_ptr(), self.m.data_ptr(),
+                    self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
+                    None, stream), 'nphm_fit_identity_step_quirk')
+            else:
+                _native.check(_native.lib().nphm_fit_identity_step(
+                    self.engine.handle, pts.data_ptr(), pts.shape[0], self.latent.data_ptr(), self.m.data_ptr(),
+                    self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(),
+                    self.grad.data_ptr(), None, stream),
+                    'nphm_fit_identity_step')
 
 
 class _FusedSurfaceLoss(torch.autograd.Function):
     """``sdf = decoder(xc, z_id); sdf[valid].abs()[< clamp].mean()`` of the joint fitter (reference fitting.py:114-125) as
     one native call (`nphm_fit_surface_grad`): tensor-core forward, analytic backward w.r.t. the identity code (member
     inputs, anchors, blend weights) and w.r.t. the query points.  Autograd continues from the point gradient into the
-    implicit-differentiation correction and the deformation network."""
+    implicit-differentiation correction and the deformation network.  In eval mode the last point of every row of ``xc``
+    (rows x n x 3, one decoder call in the reference) carries the quirk (``nphm_fit_surface_grad_quirk``, period n)."""
 
     @staticmethod
     def forward(ctx, xc, lat_rep_shape, valid, clamp, decoder):
@@ -136,11 +155,8 @@ class _FusedSurfaceLoss(torch.autograd.Function):
         terms = torch.empty(8, device=dev, dtype=torch.float32)
         g_lat = torch.empty_like(lat)
         g_pts = torch.empty_like(pts)
-        with torch.cuda.device(dev):
-            _native.check(_native.lib().nphm_fit_surface_grad(
-                eng.handle, pts.data_ptr(), pts.shape[0], lat.data_ptr(), mask.data_ptr(), float(clamp), terms.data_ptr(),
-                g_lat.data_ptr(), g_pts.data_ptr(), None, torch.cuda.current_stream(dev).cuda_stream),
-                'nphm_fit_surface_grad')
+        period = _quirk_period(decoder, xc.shape[-2])
+        _surface_grad(eng, pts, period, lat, mask, clamp, terms, g_lat, g_pts, torch.cuda.current_stream(dev).cuda_stream)
         ctx.save_for_backward(g_lat, g_pts)
         ctx.shapes = (xc.shape, lat_rep_shape.shape)
         return terms[0].clone()
@@ -149,6 +165,20 @@ class _FusedSurfaceLoss(torch.autograd.Function):
     def backward(ctx, grad_out):
         g_lat, g_pts = ctx.saved_tensors
         return grad_out * g_pts.reshape(ctx.shapes[0]), grad_out * g_lat.reshape(ctx.shapes[1]), None, None, None
+
+
+def _surface_grad(eng, pts, period, lat, mask, clamp, terms, g_lat, g_pts, stream):
+    """``nphm_fit_surface_grad`` on ``pts`` (n x 3), or its eval-mode form with quirk period ``period`` > 0."""
+    lib = _native.lib()
+    with torch.cuda.device(pts.device):
+        if period:
+            _native.check(lib.nphm_fit_surface_grad_quirk(eng.handle, pts.data_ptr(), pts.shape[0], period, lat.data_ptr(),
+                                                          mask.data_ptr(), float(clamp), terms.data_ptr(), g_lat.data_ptr(),
+                                                          g_pts.data_ptr(), None, stream), 'nphm_fit_surface_grad_quirk')
+        else:
+            _native.check(lib.nphm_fit_surface_grad(eng.handle, pts.data_ptr(), pts.shape[0], lat.data_ptr(), mask.data_ptr(),
+                                                    float(clamp), terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(), None,
+                                                    stream), 'nphm_fit_surface_grad')
 
 
 def inference_identity_space(decoder,
@@ -241,8 +271,8 @@ def _latent_regularisers(decoder, lat_rep_shape):
 
 
 def _native_joint(decoder, decoder_expr, device) -> bool:
-    """The autograd-free joint fitter applies to the shipped configuration: fused identity ensemble (training mode) and a
-    'compress' DeformationNetwork in eval mode on the same CUDA device."""
+    """The autograd-free joint fitter applies to the shipped configuration: a fused identity ensemble (see
+    :func:`_fused_identity`) and a 'compress' DeformationNetwork in eval mode on the same CUDA device."""
     from .deepSDF import DeformationNetwork
     if device.type != 'cuda' or not _fused_identity(decoder) or not isinstance(decoder_expr, DeformationNetwork):
         return False
@@ -311,9 +341,8 @@ class JointFitter:
             mask = valid.reshape(-1).to(torch.uint8).contiguous()
             g_lat = torch.empty(D, device=dev)
             g_pts = torch.empty_like(pts)
-            nat.check(nat.lib().nphm_fit_surface_grad(self.eng.handle, pts.data_ptr(), pts.shape[0], self.z_id.data_ptr(),
-                                                      mask.data_ptr(), float(clamp), self.terms.data_ptr(), g_lat.data_ptr(),
-                                                      g_pts.data_ptr(), None, stream), 'nphm_fit_surface_grad')
+            _surface_grad(self.eng, pts, _quirk_period(self.dec, n_point), self.z_id, mask, clamp, self.terms, g_lat, g_pts,
+                          stream)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                       # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # nb x (32 + E); same points as j_inv
             g_first = (Wc * g_cond[:, :32].sum(0)[:, None]).sum(0)                       # compressor^T -> [z_id | anchors]
@@ -625,11 +654,27 @@ def _tc_ensemble(decoder) -> bool:
     return _native.hidden_width(e, e.num_layers - 1) == 200 and decoder.lat_dim_glob + decoder.lat_dim_loc == 96
 
 
+class _QuirkPeriods:
+    """The per-scan quirk periods of the batched eval-mode calls as an int32 device tensor, uploaded when they change."""
+
+    def __init__(self):
+        self._key, self._dev = None, None
+
+    def __call__(self, periods: List[int], device) -> torch.Tensor:
+        key = tuple(int(p) for p in periods)
+        if key != self._key:
+            self._key, self._dev = key, torch.tensor(key, dtype=torch.int32).to(device)
+        return self._dev
+
+
 class BatchedIdentityFitter:
     """:class:`IdentityFitter` for S scans at once (``nphm_fit_identity_step_batched``): latents and Adam moments S x D on the
-    device, one launch sequence per iteration for all scans."""
+    device, one launch sequence per iteration for all scans.  In eval mode (``nphm_fit_identity_step_batched_quirk``) scan
+    k's period is the points per row of its sample, so each scan gets the quirk rows of its own single-scan call."""
 
     def __init__(self, decoder: FastEnsembleDeepSDFMirrored, n_scans: int, device):
+        self.decoder = decoder
+        self._periods = _QuirkPeriods()
         self.device = device
         self.engine = decoder.engine()
         self.latents = torch.zeros(n_scans, decoder.lat_dim, device=device, dtype=torch.float32)
@@ -644,6 +689,7 @@ class BatchedIdentityFitter:
         """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ)."""
         pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in points])
         S, n = pts.shape[0], pts.shape[1]
+        eval_mode = not self.decoder.training
         if apply_update:
             self.t += 1
         fp = _native.FitParams(float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0)),
@@ -655,11 +701,19 @@ class BatchedIdentityFitter:
                 self._ws = ((S, n), _native._workspace(lib.nphm_fit_batch_workspace_bytes(self.engine.handle, S, n),
                                                        'nphm_fit_batch_workspace_bytes', self.device))
             ws = self._ws[1]
-            _native.check(lib.nphm_fit_identity_step_batched(
-                self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, self.latents.data_ptr(), self.m.data_ptr(),
-                self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
-                ws.data_ptr(), ws.numel(), torch.cuda.current_stream(self.device).cuda_stream),
-                'nphm_fit_identity_step_batched')
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            if eval_mode:
+                periods = self._periods([p.shape[-2] if p.dim() > 1 else 1 for p in points], self.device)
+                _native.check(lib.nphm_fit_identity_step_batched_quirk(
+                    self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, periods.data_ptr(), self.latents.data_ptr(),
+                    self.m.data_ptr(), self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(),
+                    self.grad.data_ptr(), ws.data_ptr(), ws.numel(), stream), 'nphm_fit_identity_step_batched_quirk')
+            else:
+                _native.check(lib.nphm_fit_identity_step_batched(
+                    self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, self.latents.data_ptr(), self.m.data_ptr(),
+                    self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
+                    ws.data_ptr(), ws.numel(), stream),
+                    'nphm_fit_identity_step_batched')
 
 
 def _scans_device(scans):
@@ -677,7 +731,8 @@ def inference_identity_space_batched(decoder,
     """:func:`inference_identity_space` for several scans (``scans[k]``: the observations of scan k) at once.  Returns
     ``[(lat_rep_shape, anchors)]`` in scan order - what the single-scan function gives when called on each scan in turn, each
     call with a fresh copy of ``lambdas``; the global CPU generator and ``lambdas`` end as those calls leave them.  Runs all
-    scans in one launch sequence per iteration for the fused ensemble in training mode on CUDA (:class:`BatchedIdentityFitter`)
+    scans in one launch sequence per iteration for the fused ensemble on CUDA (:class:`BatchedIdentityFitter`, training or eval
+    mode, see :func:`_fused_identity`)
     and for the NPM baseline's ``DeepSDF`` on CUDA (:class:`BatchedNpmIdentityFitter`); any other configuration calls the
     single-scan function scan by scan."""
     if not scans:
@@ -712,6 +767,28 @@ def inference_identity_space_batched(decoder,
     return out
 
 
+def _pad_rows(obs: List[torch.Tensor], n_point: int, front: bool = False):
+    """Subjects' samples (``obs[k]``: rows x n_k x 3) -> (all rows padded to n_point points, S rows n_point float32; the
+    kept-point mask S x rows x n_point, or None when nothing is padded).  The padding repeats the row's first point, behind
+    the row or, with ``front``, in front of it (then every row ends with its own last point)."""
+    nb = obs[0].shape[0]
+    keep = None
+    if any(o.shape[1] != n_point for o in obs):
+        keep = torch.ones(len(obs), nb, n_point, dtype=torch.bool, device=obs[0].device)
+        for k, o in enumerate(obs):
+            if front:
+                keep[k, :, :n_point - o.shape[1]] = False
+            else:
+                keep[k, :, o.shape[1]:] = False
+
+    def padded(o):
+        if o.shape[1] == n_point:
+            return o
+        pad = o[:, :1].expand(nb, n_point - o.shape[1], 3)
+        return torch.cat([pad, o] if front else [o, pad], dim=1)
+    return torch.cat([padded(o) for o in obs]).to(torch.float32).contiguous(), keep
+
+
 class BatchedJointFitter:
     """:class:`JointFitter` for S subjects at once.  Per iteration, for the 5 sampled observations of every subject:
         anchors of the S identity codes (nphm_ensemble_anchors), condition rows [compressor([z_id | anchors])[subject] | z_ex[row]]
@@ -720,7 +797,10 @@ class BatchedJointFitter:
         u = -J^-T g_x, one adjoint pass, the compressor adjoint summed per subject
         nphm_fit_apply_gradient_batched (regularisers, mlp_pos backward, Adam per subject)
         one nphm_adam_step over the expression codes of all subjects (element-wise, shared step and lr: the same as per subject).
-    The expression codes are one (sum n_obs) x E tensor; subject k's rows start at ``offsets[k]``."""
+    The expression codes are one (sum n_obs) x E tensor; subject k's rows start at ``offsets[k]``.  In eval mode a shorter
+    subject's rows are padded in front instead of behind, so that every row ends with its subject's last sampled point - the
+    quirk row of that subject's single-subject call - and one period, n_point, serves all subjects
+    (``nphm_fit_surface_grad_batched_quirk``)."""
 
     def __init__(self, decoder, decoder_expr, num_observations: List[int], device):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
@@ -759,14 +839,10 @@ class BatchedJointFitter:
             c32 = (Wc[None] * first[:, None, :]).sum(2) + bc                             # S x 32
             rows = torch.cat([idx + off for idx, off in zip(obs_idx, self.offsets)])    # rows of z_ex, 5 S
             cond = torch.cat([c32.repeat_interleave(nb, dim=0), self.z_ex[rows]], dim=1).contiguous()
-            # every subject padded to n_point points per observation (the padding repeats a point and is masked below)
-            keep = None
-            if any(o.shape[1] != n_point for o in obs):
-                keep = torch.ones(S, nb, n_point, dtype=torch.bool, device=dev)
-                for k, o in enumerate(obs):
-                    keep[k, :, o.shape[1]:] = False
-            obs_all = torch.cat([o if o.shape[1] == n_point else torch.cat([o, o[:, :1].expand(nb, n_point - o.shape[1], 3)], dim=1)
-                                 for o in obs]).to(torch.float32).contiguous()                 # 5 S x n_point x 3
+            # every subject padded to n_point points per observation (the padding repeats a point and is masked below); in eval
+            # mode in front of the row, so that its last point stays last
+            front = not self.dec.training
+            obs_all, keep = _pad_rows(obs, n_point, front)                                # 5 S x n_point x 3
             _, j0_inv = self.mlp.inverse_jacobian(obs_all, cond)
             p, _, valid, _ = self.mlp.broyden_search(obs_all, cond, obs_all, j0_inv, max_steps=15, cvg_thresh=1e-6,
                                                      dvg_thresh=0.2, early_exit=self.early_exit)
@@ -782,9 +858,18 @@ class BatchedJointFitter:
             terms = torch.empty(S, 8, device=dev)
             g_lat = torch.empty(S, D, device=dev)
             g_pts = torch.empty_like(pts)
-            nat.check(lib.nphm_fit_surface_grad_batched(self.eng.handle, pts.data_ptr(), mask.data_ptr(), S, n, self.z_id.data_ptr(),
-                                                        float(clamp), terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(),
-                                                        ws.data_ptr(), ws.numel(), stream), 'nphm_fit_surface_grad_batched')
+            if front:
+                periods = torch.full((S,), n_point, dtype=torch.int32, device=dev)
+                nat.check(lib.nphm_fit_surface_grad_batched_quirk(self.eng.handle, pts.data_ptr(), mask.data_ptr(), S, n,
+                                                                  periods.data_ptr(), self.z_id.data_ptr(), float(clamp),
+                                                                  terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(),
+                                                                  ws.data_ptr(), ws.numel(), stream),
+                          'nphm_fit_surface_grad_batched_quirk')
+            else:
+                nat.check(lib.nphm_fit_surface_grad_batched(self.eng.handle, pts.data_ptr(), mask.data_ptr(), S, n,
+                                                            self.z_id.data_ptr(), float(clamp), terms.data_ptr(),
+                                                            g_lat.data_ptr(), g_pts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
+                          'nphm_fit_surface_grad_batched')
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # 5 S x (32 + E)
             g_c32 = g_cond[:, :32].reshape(S, nb, 32).sum(1)

@@ -12,7 +12,9 @@ ensemble - ``anchors``, ``symm_dist``, ``middle_dist``).  Two ways to get the SD
     point set into ``nphm_ensemble_backward_inputs`` with an upstream gradient of ones - a point's SDF depends on its own
     coordinates only, so that vector-Jacobian product IS the per-point spatial gradient (tensor-core forward and backward,
     ``csrc/fit.cu``).  Used when autograd is not recording (the reference cannot evaluate these losses at all under
-    ``torch.no_grad()``: its ``gradient`` needs a graph) or with ``native=True``; training-mode forward only.
+    ``torch.no_grad()``: its ``gradient`` needs a graph) or with ``native=True``.  In eval mode the call is
+    ``nphm_ensemble_backward_inputs_quirk`` with the period of one reference call (its last point gets the eval-mode quirk,
+    EnsembledDeepSDF.py:260-261); that form needs the tensor-core configuration, other eval-mode ensembles stay composite.
   * **composite** (training): the decoder's autograd path and ``diff_operators.gradient`` with ``create_graph=True`` -
     weight gradients of the normal / eikonal terms need the double backward, which stays in PyTorch.
 
@@ -22,7 +24,9 @@ query) and differentiates the SDF and its spatial gradient natively, second-orde
 composite path for it.  With ``native=True``, the ensemble in training mode on CUDA and autograd recording, the ensemble takes
 the same way: ``FastEnsembleDeepSDFMirrored.forward_with_gradient_native`` runs the members' passes natively (one launch per
 pass for all members) and the anchors and blend in autograd.  Under ``torch.no_grad()`` ``native=True`` keeps the evaluation
-path above.
+path above.  Both take the ensemble in eval mode too - the validation step of the reference's stage 1
+(``TrainerAutoDecoder.compute_val_loss``, training.py:250-268, calls ``decoder.eval()`` and then differentiates this loss): the
+four point sets are the reference's four decoder calls, so the last point of each set, per batch element, gets the quirk.
 
 ``compute_loss_corresp_forward`` is first order (no gradient with respect to the points is used), so its decoder calls run
 natively to the weights: ``DeformationNetwork.forward_native_grad`` (forward and backward on the tensor cores, the compressor
@@ -52,13 +56,15 @@ def compute_loss(batch, decoder, latent_codes, device, native=None):
 
 
 def _native_values_and_gradients(decoder, points, glob_cond):
-    """points B x N x 3, glob_cond B x 1 x lat_dim -> (sdf B x N x 1, d sdf / d x  B x N x 3), no graph."""
+    """points B x N x 3, glob_cond B x 1 x lat_dim -> (sdf B x N x 1, d sdf / d x  B x N x 3), no graph.  Each batch element
+    is one decoder call, as in the reference (its last point carries the eval-mode quirk)."""
     engine = decoder.engine()
+    period = 0 if decoder.training else points.shape[1]
     sdf, grad = [], []
     for b in range(points.shape[0]):
         pts = points[b].contiguous()
         ones = torch.ones(pts.shape[0], device=pts.device, dtype=torch.float32)
-        s, _, g = engine.backward_inputs(pts, glob_cond[b].reshape(-1), ones)
+        s, _, g = engine.backward_inputs(pts, glob_cond[b].reshape(-1), ones, quirk_period=period)
         sdf.append(s)
         grad.append(g)
     return torch.stack(sdf)[..., None], torch.stack(grad)
@@ -93,8 +99,8 @@ def _ensemble_sdfgrad_native(decoder, batch_cuda, glob_cond):
     {name: d sdf / d x}, anchors)."""
     sets = [batch_cuda[name] for name in _POINT_SETS]
     pts = torch.cat(sets, dim=1)
-    sdf, g, anchors = decoder.forward_with_gradient_native(pts, glob_cond)
     sizes = [p.shape[1] for p in sets]
+    sdf, g, anchors = decoder.forward_with_gradient_native(pts, glob_cond, call_sizes=sizes)
     return dict(zip(_POINT_SETS, sdf.split(sizes, dim=1))), dict(zip(_POINT_SETS, g.split(sizes, dim=1))), anchors
 
 
@@ -105,8 +111,11 @@ def actual_compute_loss(batch_cuda, decoder, glob_cond, native=None):
     explicit = native is not None and bool(native)
     if native is None:
         native = not torch.is_grad_enabled()
-    native = bool(native) and is_ensemble and decoder.training and batch_cuda['points_face'].is_cuda
+    native = bool(native) and is_ensemble and batch_cuda['points_face'].is_cuda
     ensemble_sdfgrad = native and explicit and torch.is_grad_enabled()
+    if native and not ensemble_sdfgrad and not decoder.training:
+        from .fitting import _fused_identity
+        native = _fused_identity(decoder)          # the eval-mode vector-Jacobian product needs the tensor-core configuration
 
     pred, grad, anchors = {}, {}, None
     if sdfgrad:

@@ -33,7 +33,13 @@ Embedding(., 1344, max_norm 1, sparse) codes, clip_grad_norm_ 0.1 on both.  Nati
 members' passes on the tensor cores, one launch per pass for all 40 members, anchors and blend in autograd) and composite
 steps alternate, with peak memory and the first step's gradient difference as above.  If the batch does not fit, the line
 says so and both are measured at the largest halved batch that does.  --profile --stage 1 --decoder nphm: the kernel
-breakdown of native ensemble steps."""
+breakdown of native ensemble steps.
+
+    python tools/bench_train.py --stage 1 --decoder nphm --eval --steps 10 --warmup 2
+
+The reference's stage-1 validation step (TrainerAutoDecoder.compute_val_loss, src/NPHM/models/training.py:250-268) on the same
+batches: the ensemble in eval mode, the loss and its backward, the codes' gradient clipped and a SparseAdam step on them.
+Native (the members' passes with the eval-mode quirk applied before the blend) against composite, as above."""
 import argparse, gc, json, os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
@@ -188,6 +194,33 @@ def train_step_shape(state, b, native, ev, keep=None, lambdas=LAMBDAS_SHAPE):
     return values['loss']
 
 
+def val_step_nphm(state, b, native, ev, keep=None):
+    """One step of the reference's stage-1 validation (TrainerAutoDecoder.compute_val_loss, training.py:250-268): the decoder in
+    eval mode, the loss and its backward, the codes' gradient clipped and one SparseAdam step on them.  The decoder's own
+    gradients accumulate unused there, as in the reference."""
+    from nphm_b200.models.loss_functions import compute_loss
+    dec, codes, _, opt_lat = state
+    dec.eval()
+    ev[0].record()
+    opt_lat.zero_grad()
+    losses = compute_loss(dict(b), dec, codes, 'cuda', native=native)
+    tot = 0
+    for k, lam in LAMBDAS_NPHM.items():
+        tot = tot + lam * losses[k]
+    ev[1].record()
+    tot.backward()
+    ev[2].record()
+    if keep is not None:
+        keep['codes'] = codes.weight.grad.coalesce().to_dense()
+    ev[4].record()
+    clip_sparse_grad_norm_(codes.weight, max_norm=0.1)
+    opt_lat.step()
+    ev[3].record()
+    values = {k: v.item() for k, v in losses.items()}                # the reference's per-step read-backs
+    values['loss'] = tot.item()
+    return values['loss']
+
+
 def outside_torch_bytes():
     """Device memory in use that torch's caching allocator does not hold (native handles' buffers, CUDA context); read from
     the driver's free count, so other processes on the same GPU would show up here too."""
@@ -243,16 +276,18 @@ def run_mode(mode, args, dev):
     return run(lambda: setup(mode, dev), lambda step: batch(32, 1000, dev, step), train_step, args)
 
 
-def run_nphm(args, dev, name, power):
-    """Native and composite ensemble steps at B = 32, halving B after an out-of-memory error."""
-    out = {'metric': 'stage1_nphm_train_step', 'gpu': name, 'power_limit': power, 'steps': args.steps,
-           'timing': 'median of CUDA-event times per step, native and composite alternated'}
+def run_nphm(args, dev, name, power, eval_mode=False):
+    """Native and composite ensemble steps at B = 32, halving B after an out-of-memory error.  eval_mode: the validation step
+    (:func:`val_step_nphm`) instead of the training step."""
+    out = {'metric': 'stage1_nphm_val_step' if eval_mode else 'stage1_nphm_train_step', 'gpu': name, 'power_limit': power,
+           'steps': args.steps, 'timing': 'median of CUDA-event times per step, native and composite alternated'}
+    step_fn = val_step_nphm if eval_mode else (lambda *a: train_step_shape(*a, lambdas=LAMBDAS_NPHM))
     B = 32
     while B >= 1:
         oom = False
         try:
-            out['nphm'] = run(lambda: setup_nphm(dev), lambda step: batch_shape(B, dev, step, anchors=True),
-                              lambda *a: train_step_shape(*a, lambdas=LAMBDAS_NPHM), args, compare_first=True)
+            out['nphm'] = run(lambda: setup_nphm(dev), lambda step: batch_shape(B, dev, step, anchors=True), step_fn, args,
+                              compare_first=True)
             out['batch'] = '%d x (750 + 50 + 800 + 93) points' % B
             return out
         except torch.cuda.OutOfMemoryError:
@@ -304,6 +339,8 @@ def main():
                     help='2: expression space (train_corresp.py), 1: NPM shape space (train.py without -local)')
     ap.add_argument('--decoder', choices=('npm', 'nphm'), default='npm',
                     help='stage 1: npm (DeepSDF, train.py) or nphm (the ensemble, train.py -local)')
+    ap.add_argument('--eval', action='store_true',
+                    help='--stage 1 --decoder nphm: time the eval-mode validation step (compute_val_loss) instead')
     ap.add_argument('--profile', action='store_true',
                     help='instead: torch.profiler over 5 native steps of the stage, CUDA time per kernel of the step (JSON)')
     args = ap.parse_args()
@@ -311,6 +348,8 @@ def main():
         ap.error('--steps must be >= 1')
     if args.decoder == 'nphm' and args.stage != 1:
         ap.error('--decoder nphm: stage 1 only')
+    if args.eval and (args.decoder != 'nphm' or args.profile):
+        ap.error('--eval: --stage 1 --decoder nphm only, without --profile')
     dev = torch.device('cuda', torch.cuda.current_device())
     name, power = gpu_info()
     if args.profile:
@@ -318,7 +357,7 @@ def main():
                           **profile_native(dev, args.stage, decoder=args.decoder)}))
         return
     if args.stage == 1 and args.decoder == 'nphm':
-        print(json.dumps(run_nphm(args, dev, name, power)))
+        print(json.dumps(run_nphm(args, dev, name, power, eval_mode=args.eval)))
         return
     if args.stage == 1:
         out = {'metric': 'stage1_train_step', 'gpu': name, 'power_limit': power,
