@@ -247,7 +247,7 @@ __global__ void __launch_bounds__(kThreads, 1) fit_member_kernel(const Dims d, c
 __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const Buffers b, float lambda_surface, float *__restrict__ gs,
                                                            long long gs_stride)
 {
-    __shared__ float s_anch[64 * 3], s_acc[64 * 3];
+    __shared__ float s_anch[tc::kMaxMembers * 3], s_acc[tc::kMaxMembers * 3];     // n_loc < kMaxMembers (tc_ensemble_supported)
     const int lane = threadIdx.x & 31, scan = blockIdx.y;
     for (int i = threadIdx.x; i < d.n_loc * 3; i += blockDim.x) { s_anch[i] = b.anchors[(size_t)scan * d.n_loc * 3 + i]; s_acc[i] = 0.f; }
     __syncthreads();
@@ -738,6 +738,10 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
         set_error("scan-batched fitting needs the tensor-core configuration (hidden 200, 4 layers, condition 96)");
         return NPHM_ERR_UNSUPPORTED;
     }
+    if (grad_points_dev && !tc_path) {
+        set_error("gradient w.r.t. the points needs the tensor-core configuration (hidden 200, 4 layers, condition 96)");
+        return NPHM_ERR_UNSUPPORTED;
+    }
     fit::Dims d{};
     d.n_members = h->n_members; d.n_symm = h->cfg.n_symm_pairs; d.n_loc = h->cfg.n_loc;
     d.H = h->cfg.hidden_dim; d.N1 = h->dims.N[1]; d.C = h->dims.cond_dim; d.G = h->cfg.lat_dim_glob; d.Lc = h->cfg.lat_dim_loc;
@@ -745,6 +749,8 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
     for (int l = 0; l < 5; ++l) d.coff[l] = h->dims.coff[l];
     d.r_c = 0; d.r_h0 = 3; d.r_h1 = d.r_h0 + d.H; d.r_h2 = d.r_h1 + d.N1 + 3; d.r_h3 = d.r_h2 + d.H; d.r_s = d.r_h3 + d.H;
     d.rows = d.r_s + 8 + 8 * (fit::kThreads / 32);
+    // nphm_b200/models/fitting.py restates this bound (ffma_fit_rows, FFMA_FIT_MAX_ROWS) to choose the autograd path for
+    // the ensembles it rejects; keep the two in step (tests/test_gpu_ensemble_f64.py checks them against each other)
     const size_t smem = (size_t)d.rows * fit::P * sizeof(float);
     if (smem > 227 * 1024) {
         set_error("nphm_fit_identity_step: hidden width %d too large for the fitting kernel", d.H);
@@ -851,10 +857,6 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
         if (grad_points_dev) fit::fit_reduce_kernel<true><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
         else fit::fit_reduce_kernel<false><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
     } else {
-        if (grad_points_dev) {
-            set_error("gradient w.r.t. the points needs the tensor-core configuration (hidden 200, 4 layers, condition 96)");
-            return NPHM_ERR_UNSUPPORTED;
-        }
         fit::fit_member_kernel<true><<<grid, fit::kThreads, smem, stream>>>(d, w, b, fp->lambda_surface);
     }
     NPHM_CUDA_CHECK(cudaGetLastError());

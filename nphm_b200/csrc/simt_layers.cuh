@@ -136,6 +136,8 @@ __device__ __forceinline__ void dense_layer_bwd(const float *__restrict__ W, int
                                                 const float *delta_s, float *rows_s, int warp, int lane, int nwarps)
 {
     constexpr int P = 32 * TM;
+    // the rows of W are 16-byte aligned only when W is and ldw is a multiple of 4 (a hidden width such as 77 is not)
+    const bool vec = (reinterpret_cast<uintptr_t>(W) & 15) == 0 && (ldw & 3) == 0;
     for (int j0 = warp * 8; j0 < J; j0 += nwarps * 8) {
         float acc[TM][8];
 #pragma unroll
@@ -144,7 +146,7 @@ __device__ __forceinline__ void dense_layer_bwd(const float *__restrict__ W, int
             for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
         const float *w = W + j0;
         const float *d_ptr = delta_s + lane * TM;
-        const bool full = j0 + 8 <= J;
+        const bool full = vec && j0 + 8 <= J;
 #pragma unroll 4
         for (int n = 0; n < n_out; ++n) {
             float a[TM];

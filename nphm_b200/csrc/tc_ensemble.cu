@@ -193,7 +193,7 @@ __global__ void pack_test_slabs_kernel(const float *__restrict__ B, int n, int k
 bool tc_ensemble_supported(const nphm_ensemble *h)
 {
     return h->cfg.hidden_dim == tc::kH && h->cfg.n_layers == 4 && h->cfg.lat_dim_glob + h->cfg.lat_dim_loc == tc::kCond &&
-           h->dims.N[1] == tc::kN1;
+           h->dims.N[1] == tc::kN1 && h->n_members <= tc::kMaxMembers;
 }
 
 int tc_ensemble_pack(nphm_ensemble *h, cudaStream_t stream)

@@ -10,6 +10,9 @@ namespace tc {
 constexpr int kH = 200;            // hidden width
 constexpr int kN1 = 101;           // layer-1 width (hidden - d_in)
 constexpr int kCond = 96;
+// members of one ensemble: the dense kernel keeps member sets in 64-bit masks and fit_upstream_kernel stages the anchors of
+// at most 64 members in shared memory; a larger ensemble runs on the FFMA kernels
+constexpr int kMaxMembers = 64;
 constexpr int kNP1 = 104;                            // layer-1 MMA width (101 -> 104)
 constexpr int kNA = 112, kNB = 88;                   // column halves of the 200-wide layers 2 and 3 (200 = 112 + 88)
 constexpr int kKS1 = 13, kKS2 = 7, kKS3 = 13;       // k-steps of 16

@@ -82,16 +82,37 @@ def _current_anchors(decoder, lat_rep_shape, device):
     return decoder(torch.zeros([1, 1, 3], device=device), lat_rep_shape, None)[1]
 
 
-def _fused_identity(decoder) -> bool:
-    """Whether the fused fitting kernels take this decoder.  The reference runs its fitters in training mode
-    (scripts/fitting/fitting_pointclouds.py:268 calls ``decoder_shape.train()`` first).  In eval mode its forward overwrites
-    every member's output at the last point of each decoder call (EnsembledDeepSDF.py:260-261); the fused kernels reproduce
-    that through the quirk period of their ``_quirk`` entry points, which need the tensor-core configuration
-    (:func:`_tc_ensemble`).  Other eval-mode ensembles take the autograd path."""
-    p = next(decoder.parameters())
-    if not (isinstance(decoder, FastEnsembleDeepSDFMirrored) and p.is_cuda and decoder.ensembled_deep_sdf.num_layers == 6):
+def _fused_identity(decoder, grad_points: bool = False) -> bool:
+    """Whether the fused fitting kernels take this decoder on CUDA (see :func:`fused_fit_config`)."""
+    return (isinstance(decoder, FastEnsembleDeepSDFMirrored) and next(decoder.parameters()).is_cuda
+            and fused_fit_config(decoder, grad_points))
+
+
+# The FFMA fitting step (csrc/fit.cu fit_step_impl) keeps 3 + H + (N1 + 3) + 3 H + 8 + 8 * 16 = 139 + 4 H - C rows of 64 fp32
+# points (N1 = H - C - 3, C = lat_dim_glob + lat_dim_loc) in at most 227 KiB of shared memory.
+FFMA_FIT_MAX_ROWS = 227 * 1024 // (64 * 4)
+
+
+def ffma_fit_rows(hidden: int, cond: int) -> int:
+    return 139 + 4 * hidden - cond
+
+
+def fused_fit_config(decoder, grad_points: bool = False) -> bool:
+    """Whether the fused fitting kernels take an ensemble of this configuration, in its current mode: exactly what the C
+    entry points accept.  They need 4 hidden layers.  The tensor-core configuration (:func:`_tc_ensemble`) serves every entry
+    point.  Any other width runs the FFMA step, which serves only the single-scan training-mode step without point gradients
+    (``nphm_fit_identity_step``) and only within its shared memory (:data:`FFMA_FIT_MAX_ROWS`).  So the eval-mode quirk (the
+    reference's forward overwrites every member's output at the last point of each decoder call, EnsembledDeepSDF.py:260-261)
+    and ``grad_points`` (the joint fitter's surface term, ``nphm_ensemble_backward_inputs``) need the tensor-core
+    configuration; anything the kernels do not take goes to the autograd path.  The reference runs its fitters in training
+    mode (scripts/fitting/fitting_pointclouds.py:268 calls ``decoder_shape.train()`` first)."""
+    if decoder.ensembled_deep_sdf.num_layers != 6:
         return False
-    return decoder.training or _tc_ensemble(decoder)
+    if _tc_ensemble(decoder):
+        return True
+    hidden = _native.hidden_width(decoder.ensembled_deep_sdf, 5)
+    return (decoder.training and not grad_points
+            and ffma_fit_rows(hidden, decoder.lat_dim_glob + decoder.lat_dim_loc) <= FFMA_FIT_MAX_ROWS)
 
 
 def _quirk_period(decoder, points_per_call: int) -> int:
@@ -274,7 +295,7 @@ def _native_joint(decoder, decoder_expr, device) -> bool:
     """The autograd-free joint fitter applies to the shipped configuration: a fused identity ensemble (see
     :func:`_fused_identity`) and a 'compress' DeformationNetwork in eval mode on the same CUDA device."""
     from .deepSDF import DeformationNetwork
-    if device.type != 'cuda' or not _fused_identity(decoder) or not isinstance(decoder_expr, DeformationNetwork):
+    if device.type != 'cuda' or not _fused_identity(decoder, grad_points=True) or not isinstance(decoder_expr, DeformationNetwork):
         return False
     if decoder_expr.training or decoder_expr.mode != 'compress':
         return False
@@ -580,7 +601,7 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
         correction = preds_posed - preds_posed.detach()
         correction = torch.einsum('bnij,bnj->bni', -grad_inv.detach(), correction)
         xc = p_corresp + correction
-        if has_local and _fused_identity(decoder) and xc.is_cuda:
+        if has_local and _fused_identity(decoder, grad_points=True) and xc.is_cuda:
             surface = _FusedSurfaceLoss.apply(xc, lat_rep_shape, search_result['valid_ids'],
                                               _clamp_for_iteration(j, step_scale), decoder)
         else:
@@ -647,11 +668,16 @@ def _sequential(fit_one, scans, lambdas, *args):
     return out
 
 
+TC_MAX_MEMBERS = 64         # the tensor-core kernels keep member sets in 64-bit masks (csrc tc_ensemble.cuh kMaxMembers)
+
+
 def _tc_ensemble(decoder) -> bool:
-    """The scan-batched kernels need the tensor-core configuration (csrc tc_ensemble_supported): hidden width 200 and a
-    condition of 96 (lat_dim_glob + lat_dim_loc); the 4 hidden layers are checked by :func:`_fused_identity`."""
+    """The tensor-core configuration (csrc tc_ensemble_supported): 4 hidden layers of width 200, a condition of 96
+    (lat_dim_glob + lat_dim_loc) and at most 64 members (n_loc + 1).  The scan-batched kernels, the eval-mode quirk and the
+    point gradients need it."""
     e = decoder.ensembled_deep_sdf
-    return _native.hidden_width(e, e.num_layers - 1) == 200 and decoder.lat_dim_glob + decoder.lat_dim_loc == 96
+    return (e.num_layers == 6 and _native.hidden_width(e, e.num_layers - 1) == 200
+            and decoder.lat_dim_glob + decoder.lat_dim_loc == 96 and decoder.num_kps + 1 <= TC_MAX_MEMBERS)
 
 
 class _QuirkPeriods:

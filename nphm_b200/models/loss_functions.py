@@ -113,9 +113,9 @@ def actual_compute_loss(batch_cuda, decoder, glob_cond, native=None):
         native = not torch.is_grad_enabled()
     native = bool(native) and is_ensemble and batch_cuda['points_face'].is_cuda
     ensemble_sdfgrad = native and explicit and torch.is_grad_enabled()
-    if native and not ensemble_sdfgrad and not decoder.training:
+    if native and not ensemble_sdfgrad:
         from .fitting import _fused_identity
-        native = _fused_identity(decoder)          # the eval-mode vector-Jacobian product needs the tensor-core configuration
+        native = _fused_identity(decoder, grad_points=True)      # the vector-Jacobian product needs the tensor-core configuration
 
     pred, grad, anchors = {}, {}, None
     if sdfgrad:

@@ -11,13 +11,13 @@ the rows of the last 128-row tile, to the last 16-column unit (rows and columns)
 each query's condition gradient, each with its own err_fp32 and max|ref64|: a wrong value confined to one tile or unit is
 not hidden by larger values elsewhere.  The kernels multiply in three fp16 passes (hi*hi + hi*lo + lo*hi, ~2^-22 per
 product); a kernel that lost the lo terms would be ~2^11 times worse than fp32.  `-s` prints err_native, err_fp32 and their
-ratio per configuration and tensor."""
-import math
-
+ratio per configuration and tensor (the criterion: tests/f64_check.py)."""
 import pytest
 import torch
 
 import chain_shapes_common as C
+import f64_check
+from f64_check import top_scale
 
 pytestmark = pytest.mark.gpu
 
@@ -25,7 +25,7 @@ pytestmark = pytest.mark.gpu
 # - values, Jacobians, inverse Jacobians, point and condition gradients: worst err_native / err_fp32 123 on a whole tensor
 #   (512-1024x8-1 forward, 1 x 257 rows); where the fp32 error happens to be small (a few rows), err_native / max|ref| up to
 #   2.2e-5 (train out, 40-881x4-1);
-# - weight and bias gradients whose adjoint stays in the range it is stored in (see LO_NORMAL below): worst err_native
+# - weight and bias gradients whose adjoint stays in the range it is stored in (see f64_check.LO_NORMAL): worst err_native
 #   beyond 64 * err_fp32, over the whole tensor and its last units, 5.0e-5 of the whole tensor's max|ref| (512-1024x8-1
 #   lin7.bias, 1 x 257 rows; 8.5e-6 on the smaller stacks).  A unit of a gradient is a sum over the rows of d_l h_{l-1}
 #   whose terms can cancel far below the tensor's largest entry, so its floor is relative to the whole tensor; the
@@ -35,9 +35,6 @@ pytestmark = pytest.mark.gpu
 K = 64.0
 FLOOR = 3e-5
 FLOOR_GRAD = 6e-5
-# a part is also allowed an error below the fp32 resolution of the whole tensor (the parts of a weight gradient behind rows
-# whose softplus derivative is ~exp(-200) are ~1e-30 and come out as 0)
-ULP = 2.0 ** -24
 
 
 @pytest.fixture(autouse=True)
@@ -49,105 +46,9 @@ def _fp32_without_tf32():
     torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = saved
 
 
-class Check:
-    """Collects err_native / err_fp32 of the tensors of one test; ``done()`` fails with every violation."""
-
-    def __init__(self, cfg):
-        self.tag = C.config_id(cfg)
-        self.bad = []
-        self.known = []                  # violations inside the adjoint's fp16 subnormal range (see LO_NORMAL)
-        self.n_known = 0
-
-    def _one(self, what, got, r64, r32, floor, scale=None, whole=0.0, known=False):
-        en = float((got.double() - r64).abs().max())
-        ef = float((r32.double() - r64).abs().max())
-        sc = float(r64.abs().max()) if scale is None else scale
-        bound = K * ef + floor * sc + ULP * whole
-        self.n_known += known
-        if not en <= bound:
-            msg = '%s: err_native %.3e > %.3e (err_fp32 %.3e, max|ref| %.3e)' % (what, en, bound, ef, sc)
-            # inside the known range defect the error stays below a few fp16 ulps of the part; more is another bug
-            (self.known if known and en <= KNOWN_MAX * sc + bound else self.bad).append(msg)
-        return en, ef, sc
-
-    def __call__(self, what, got, r64, r32, kind='rows', scale=None, known=(False, False)):
-        """kind: 'rows' (leading dims are rows: also the last 128-row tile), 'weight' (N x K: also the last 16 rows and the
-        last 16 columns), 'bias' (also the last 16), 'cond' (B x D: also each query's row), 'scalar'.  scale: the magnitude
-        the floor is relative to (default max|ref64|)."""
-        assert got.shape == r64.shape, (what, tuple(got.shape), tuple(r64.shape))
-        floor = FLOOR_GRAD if kind in ('weight', 'bias') else FLOOR
-        en, ef, sc = self._one(what, got, r64, r32, floor, scale, known=known[0])
-        parts = []
-        if kind == 'rows':
-            M = got.shape[0] * got.shape[1] if got.dim() >= 2 else got.shape[0]
-            m0 = (M - 1) // 128 * 128
-            flat = lambda t: t.reshape(M, -1)[m0:]
-            parts.append(('last tile', flat(got), flat(r64), flat(r32), False))
-        elif kind == 'weight':
-            n0, k0 = (got.shape[0] - 1) // 16 * 16, (got.shape[1] - 1) // 16 * 16
-            parts += [('last rows', got[n0:], r64[n0:], r32[n0:], known[1]),
-                      ('last cols', got[:, k0:], r64[:, k0:], r32[:, k0:], known[0])]
-        elif kind == 'bias':
-            n0 = (got.shape[0] - 1) // 16 * 16
-            parts.append(('last unit', got[n0:], r64[n0:], r32[n0:], known[1]))
-        elif kind == 'cond':
-            parts += [('query %d' % q, got[q], r64[q], r32[q], False) for q in range(got.shape[0])]
-        worst = en / ef if ef > 0 else (0.0 if en == 0 else float('inf'))
-        for name, g, a, b, kn in parts:
-            pn, pf, _ = self._one('%s [%s]' % (what, name), g, a, b, floor, scale=sc if kind in ('weight', 'bias') else None,
-                                  whole=sc, known=kn)
-            worst = max(worst, pn / pf if pf > 0 else (0.0 if pn == 0 else float('inf')))
-        print('CHAIN %-16s %-44s err_native %.3e err_fp32 %.3e ratio %7.3f worst-part ratio %7.3f native/max|ref| %.2e'
-              % (self.tag, what, en, ef, en / ef if ef > 0 else float('nan'), worst, en / sc if sc > 0 else 0.0))
-
-    def grads(self, what, gw, gb, r64, r32, chains):
-        """Weight and bias gradients of every layer; chains: [(adjoints d_l of the hidden layers, the device's scale of
-        that adjoint chain)], whose range decides which checks fall under the known defect (adjoint_range)."""
-        known = adjoint_range(chains, len(gw))
-        for l, (a, b) in enumerate(zip(gw, gb)):
-            self('%s lin%d.weight' % (what, l), a, r64[0][l], r32[0][l], 'weight', known=known[l])
-            self('%s lin%d.bias' % (what, l), b, r64[1][l], r32[1][l], 'bias', known=known[l])
-
-    def done(self):
-        print('CHAIN %-16s %d of the checks fall in the adjoint range defect, %d of them beyond the bound'
-              % (self.tag, self.n_known, len(self.known)))
-        assert not self.bad, '%s: %d violations:\n%s' % (self.tag, len(self.bad), '\n'.join(self.bad[:40]))
-        if self.known:
-            pytest.xfail('%s: %d weight / bias gradient checks whose adjoint left its fp16 range exceed the bound (every other '
-                         'check passed):\n%s' % (self.tag, len(self.known), '\n'.join(self.known[:20])))
-
-
-# Known defect: the backward scales the adjoint once, at the top of the chain (its largest magnitude to 2^10, mlp_chain.cu
-# kGradExp), and stores every d_l below as an fp16 hi | lo pair.  Where the values of d_l stay below 2^-3 after that scale,
-# the lo part is subnormal and the weight and bias gradients built from them lose bits (measured: up to 1.5e-3 of max|ref| on
-# lin0 of 4-8x2-1 at one row behind saturated softplus units).  Those checks, and only those, are told apart from the float64
-# adjoints: a check of layer l is in the range defect when d_l (over the part's output features) or any adjoint above it
-# stays below LO_NORMAL after the device's scale.  If one of them fails and nothing else does, the test is reported as an
-# expected failure; an error beyond KNOWN_MAX of the part's max|ref| fails it like any other violation.
-LO_NORMAL = 2.0 ** -3
-KNOWN_MAX = 1e-2
-
-
-def top_scale(*upstream):
-    """The power of two the device scales an upstream gradient by: largest magnitude to [2^10, 2^11)."""
-    m = max(float(g.abs().max()) for g in upstream)
-    return 2.0 ** (10 - math.floor(math.log2(m))) if m > 0 else 1.0
-
-
-def adjoint_range(chains, n_lin):
-    """Per layer l: (whole layer in the range defect, its last 16-feature unit in it)."""
-    known = [(False, False)] * n_lin
-    below = False                          # an adjoint above this layer left the range: its error reaches every layer below
-    for l in range(n_lin - 2, -1, -1):
-        lay = unit = False
-        for ds, scale in chains:
-            d = ds[l].abs().reshape(-1, ds[l].shape[-1]) * scale
-            n0 = (d.shape[1] - 1) // 16 * 16
-            lay |= float(d.max()) < LO_NORMAL
-            unit |= float(d[:, n0:].max()) < LO_NORMAL
-        below |= lay
-        known[l] = (below, below or unit)
-    return known
+def Check(cfg):
+    """The criterion of tests/f64_check.py with this file's constants."""
+    return f64_check.Check(C.config_id(cfg), K, FLOOR, FLOOR_GRAD)
 
 
 def _setup(cfg, device):
