@@ -56,8 +56,8 @@ MC_LAUNCHES = 3                      # classify rows, scan rows, emit rows
 
 
 def launches_per_grid_query(impl='auto') -> int:
-    """grid axes, anchors, folded constants, [tensor-core records], ensemble kernel."""
-    return 4 + (1 if impl in ('auto', 'tc', 'tc_pruned') else 0)
+    """grid axes, anchors, folded constants, [tensor-core records, tile member masks], ensemble kernel."""
+    return 4 + (2 if impl in ('auto', 'tc', 'tc_pruned') else 0)
 
 
 class EnsembleConfig(Structure):

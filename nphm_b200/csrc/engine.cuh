@@ -50,6 +50,8 @@ struct nphm_ensemble {
     nphm::DeviceBuffer anchors, cvec, axes, host_latent, host_volume;
     // tensor-core path (tc_ensemble.cu)
     nphm::DeviceBuffer tc_weights, tc_consts, tc_coff, tc_l2slabs;
+    nphm::DeviceBuffer tc_masks, tc_sched;     // member mask per tile (pre-pass), work counter of the tile schedule
+    long long tc_mask_tiles = 0;               // tiles whose masks the last launch computed (0: it computed none)
     bool tc_ready = false;
     bool tc_prune = false;          // opt-in member pruning (NPHM_IMPL_TC_PRUNED)
     float tc_prune_tau = 1e-8f;

@@ -272,13 +272,41 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
             if (cost < best - 1e-9) { best = cost; p.member_groups = g; }
         }
     }
+    h->tc_mask_tiles = 0;
+    if (prune || p.zero_skip) {
+        if ((rc = h->tc_masks.reserve((size_t)n_tiles * sizeof(unsigned long long)))) return rc;
+        p.tile_masks = h->tc_masks.as<unsigned long long>();
+        h->tc_mask_tiles = n_tiles;
+    }
+    // the kernel leaves the counter at zero when it ends; it starts at zero when allocated
+    if (!h->tc_sched.ptr) {
+        if ((rc = h->tc_sched.reserve(2 * sizeof(unsigned int)))) return rc;
+        NPHM_CUDA_CHECK(cudaMemsetAsync(h->tc_sched.ptr, 0, 2 * sizeof(unsigned int), stream));
+    }
+    p.sched = h->tc_sched.as<unsigned int>();
     const long long n_items = n_tiles * p.member_groups;
+    // 32-bit counter: the counter passes n_items by at most one per CTA
+    NPHM_REQUIRE(n_items + sm_count() < (1ll << 32), "tensor-core ensemble kernel: %lld work items", n_items);
     const int grid_x = (int)(n_items < sm_count() ? n_items : sm_count());
     if ((rc = tc::launch_ensemble_wgmma(p, prune, q.acts_out != nullptr, grid_x, stream))) return rc;
     return NPHM_OK;
 }
 
 }  // namespace nphm
+
+// Debug entry (not part of the public ABI): the member masks the pre-pass computed for the tiles of the handle's last
+// tensor-core launch.  *n_tiles receives their number (0 when that launch evaluated every member); up to `cap` masks are
+// copied to `host`.
+extern "C" int nphm_debug_ens_tile_masks(nphm_ensemble *h, unsigned long long *host, long long cap, long long *n_tiles)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h && n_tiles, "nphm_debug_ens_tile_masks: null argument");
+    *n_tiles = h->tc_mask_tiles;
+    const long long n = std::min(cap, h->tc_mask_tiles);
+    NPHM_CUDA_CHECK(cudaDeviceSynchronize());
+    if (n > 0) NPHM_CUDA_CHECK(cudaMemcpy(host, h->tc_masks.ptr, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    return NPHM_OK;
+}
 
 // Debug entry (not part of the public ABI): D = A * B^T through the tensor-core operand path.
 extern "C" int nphm_debug_tc_mma(const float *a_dev, const float *b_dev, int n, int ks, int variant, float *d_dev,

@@ -75,7 +75,52 @@ struct Params {
     // grid mode with compact tiles: blocks of tbx x tby x tbz grid points (tbx tby tbz = 128) over the x-planes px0..px1,
     // by x bz blocks per plane
     int blocked, px0, px1, by, bz, tbx, tby, tbz;
+    // pruned and zero-skipping queries: the member mask of every tile, written by the mask pre-pass (tile_mask_kernel)
+    unsigned long long *tile_masks;
+    // work counter of the on-demand tile schedule: [0] next work item, [1] CTAs finished; zero between launches
+    unsigned int *sched;
 };
+
+// One row (point) of a tile: its index in the query, its global point index, whether the tile covers a real point with
+// this row, and its coordinates.  The ensemble kernel and the mask pre-pass both call this function, so that they cannot
+// disagree about a point.  `blocked`: compact grid blocks (Params::tbx, tby, tbz); otherwise 128 consecutive points of
+// query qi (from p.xyz, or grid points from p.axes).
+struct TilePoint {
+    long long idx, g;
+    bool valid;
+    float x, y, z;
+};
+__device__ __forceinline__ TilePoint tile_point(const Params &p, bool blocked, long long tile, int qi,
+                                                long long tiles_per_query, int row)
+{
+    TilePoint t;
+    if (blocked) {
+        // compact tbx x tby x tbz block of grid points (z fastest inside the block)
+        const long long tz = tile % p.bz, txy = tile / p.bz;
+        const int ty = (int)(txy % p.by), tx = (int)(txy / p.by);
+        const int ix = p.px0 + tx * p.tbx + row / (p.tby * p.tbz), iy = ty * p.tby + (row / p.tbz) % p.tby,
+                  iz = (int)tz * p.tbz + row % p.tbz;
+        t.g = ((long long)ix * p.res + iy) * p.res + iz;
+        t.valid = ix <= p.px1 && iy < p.res && iz < p.res && t.g >= p.first && t.g < p.first + p.n_points;
+        t.idx = t.g - p.first;
+        const int cx_ = min(ix, p.res - 1), cy_ = min(iy, p.res - 1), cz_ = min(iz, p.res - 1);
+        t.x = __ldg(p.axes + cx_); t.y = __ldg(p.axes + p.res + cy_); t.z = __ldg(p.axes + 2 * p.res + cz_);
+        if (!t.valid) t.g = p.first;
+    } else {
+        t.idx = (tile - (long long)qi * tiles_per_query) * 128 + row;
+        t.valid = t.idx < p.n_points;
+        t.g = p.first + (t.valid ? t.idx : 0);
+        if (p.xyz) {
+            const float *pp = p.xyz + ((size_t)qi * p.n_points + (t.valid ? t.idx : 0)) * 3;
+            t.x = pp[0]; t.y = pp[1]; t.z = pp[2];
+        } else {
+            const long long rr = (long long)p.res * p.res;
+            const int ix = (int)(t.g / rr), iy = (int)((t.g - ix * rr) / p.res), iz = (int)(t.g % p.res);
+            t.x = __ldg(p.axes + ix); t.y = __ldg(p.axes + p.res + iy); t.z = __ldg(p.axes + 2 * p.res + iz);
+        }
+    }
+    return t;
+}
 
 // Blend weight of a member at (x, y, z): exp(-(|a - x| + 1e-5)^2 / 0.01) for a member with anchor a, exp(-20) for the
 // global member.  The tile masks and the blend call this one function with the same inputs, so that a member skipped for
@@ -91,6 +136,21 @@ __device__ __forceinline__ float blend_weight(bool has_anchor, float ax, float a
         d = -(nrm * nrm);
     }
     return expf(__fdiv_rn(d, 0.01f));
+}
+
+// Blend weight of member k of query qi (anchors `anc` = p.anchors of that query; the last member is the global one)
+__device__ __forceinline__ float member_weight(const float *anc, int k, int n_members, float x, float y, float z)
+{
+    if (k == n_members - 1) return blend_weight(false, 0.f, 0.f, 0.f, x, y, z);
+    return blend_weight(true, __ldg(anc + 3 * k), __ldg(anc + 3 * k + 1), __ldg(anc + 3 * k + 2), x, y, z);
+}
+
+// The pruned rule's normaliser at a point: S = sum_k w_k, summed in member order
+__device__ __forceinline__ float weight_sum(const float *anc, int n_members, float x, float y, float z)
+{
+    float S = 0.f;
+    for (int k = 0; k < n_members; ++k) S += member_weight(anc, k, n_members, x, y, z);
+    return S;
 }
 
 int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream);

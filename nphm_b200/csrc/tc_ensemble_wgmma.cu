@@ -18,8 +18,11 @@
 // alternates between the two warpgroups phase by phase (layer 1, layer 2, layer 3 half a, layer 3 half b), so that one
 // warpgroup's epilogue (and its next member's layer 0) runs while the other one's MMAs occupy the tensor cores.  The
 // accumulation order of every output is that of a single warpgroup running alone: the results do not depend on the offset.
-// At the start of a tile the consumers vote on which members the tile needs (dense: a blend weight that is not exactly zero
-// at some valid point; pruned: the tau rule) and the producer streams only those; grid queries use compact tiles
+// Tiles are handed out on demand: the producer lane takes the next work item from a device counter, reads the item's member
+// mask and passes (item, mask) to the consumers through a two-deep queue in shared memory, so that no SM idles while others
+// still have tiles, and the producer streams the next tile's weights while the consumers finish the current one.  A mask
+// pre-pass (tile_mask_kernel) computes which members each tile needs (dense: a blend weight that is not exactly zero at
+// some valid point; pruned: the tau rule) and the producer streams only those; grid queries use compact tiles
 // (Params::tbx, tby, tbz) so that a tile lies far from many anchors.
 #include "tc_ensemble.cuh"
 
@@ -35,8 +38,8 @@ namespace wg {
 // start at 8 + u).
 constexpr int kTraceFirst = 4, kTraceMembers = 4, kTraceWg = 32, kTraceStride = 2 * kTraceWg + 16;
 __device__ long long g_ens_trace[1 + kTraceMembers * kTraceStride];
-// Tile boundaries of CTA 0, for its first kTraceTiles tiles: warpgroup 0 starts the tile, has the tile's member mask, has the
-// layer-1 weights of the tile's first member.
+// Tile boundaries of CTA 0, for its first kTraceTiles tiles: warpgroup 0 takes the tile (and its member mask) from the queue,
+// the producer knows the tile's mask, warpgroup 0 has the layer-1 weights of the tile's first member.
 constexpr int kTraceTiles = 4;
 __device__ long long g_ens_tiles[3 * kTraceTiles];
 // Work of every CTA: [0] = CTAs of the last launch, then per CTA the member-tiles it evaluated and its cycles.
@@ -48,8 +51,7 @@ __device__ long long g_ens_ctas[1 + 2 * kTraceMaxCtas];
         ENS_STAMP(member, (threadIdx.x >> 7) * kTraceWg + 6 * (phase) + (e)); } while (0)
 #define ENS_CMARK(member, off) do { if ((threadIdx.x & 127) == 0) ENS_STAMP(member, (threadIdx.x >> 7) * kTraceWg + (off)); } while (0)
 #define ENS_PEVT(member, off) ENS_STAMP(member, 2 * kTraceWg + (off))
-#define ENS_TILE(t, e) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (t) < kTraceTiles)                                   \
-        g_ens_tiles[3 * (t) + (e)] = clock64(); } while (0)
+#define ENS_TILE(t, e) do { if (blockIdx.x == 0 && (t) < kTraceTiles) g_ens_tiles[3 * (t) + (e)] = clock64(); } while (0)
 #else
 #define ENS_CEVT(member, phase, e) do { } while (0)
 #define ENS_CMARK(member, off) do { } while (0)
@@ -69,8 +71,10 @@ struct __align__(128) Smem {
     float rec[kRecSlots][kRecFloats];
     uint64_t w_full[kSlots], w_empty[kSlots];
     uint64_t rec_full[kRecSlots], rec_empty[kRecSlots];
-    uint64_t mask_ready;
-    unsigned long long maskq[2][kConsumerWarps];
+    // tile queue (producer -> consumers): work item (-1 = no more work) and member mask of the next two tiles
+    uint64_t q_full[2], q_empty[2];
+    long long q_item[2];
+    unsigned long long q_mask[2];
 };
 static_assert(sizeof(Smem) <= 227 * 1024, "shared memory of the ensemble kernel exceeds the 227 KB of an H100 block");
 
@@ -106,6 +110,42 @@ __device__ __forceinline__ void to_operand(const float (&d)[N], int j, int col0,
     split2(v[1][2], v[1][3], ah[3], al[3]);
 }
 
+// Mask pre-pass: one warp per tile, 4 rows per lane; bit k of p.tile_masks[tile] is set when the tile needs member k.  The
+// last, global member is always needed: every tile evaluates >= 1 member.  Dense rule: a member is needed if w_k != 0 at some
+// valid point - a member with w_k = +0 everywhere adds exactly nothing to num and den (denormal weights count as nonzero).
+// Pruned rule: S = sum_k w_k; a member is needed if w_k >= tau * (S + 1e-6) at some valid point (dropped mass per point
+// < n_members * tau).  Points and weights come from tile_point and member_weight, as in the ensemble kernel.
+constexpr int kMaskWarps = 8;
+template <bool PRUNE>
+__global__ void __launch_bounds__(32 * kMaskWarps) tile_mask_kernel(const Params p)
+{
+    const long long tile = (long long)blockIdx.x * kMaskWarps + (threadIdx.x >> 5);
+    if (tile >= p.n_tiles) return;
+    const int lane = threadIdx.x & 31;
+    const long long tiles_per_query = p.blocked ? p.n_tiles : (p.n_points + 127) / 128;
+    const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
+    const float *anc = p.anchors + (size_t)qi * (p.n_members - 1) * 3;
+    TilePoint pt[4];
+    float thr[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        pt[i] = tile_point(p, p.blocked, tile, qi, tiles_per_query, lane + 32 * i);
+        thr[i] = PRUNE ? p.prune_tau * (weight_sum(anc, p.n_members, pt[i].x, pt[i].y, pt[i].z) + 1e-6f) : 0.f;
+    }
+    unsigned long long mask = 1ull << (p.n_members - 1);
+    for (int k = 0; k < p.n_members - 1; ++k) {
+        bool need = false;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            if (!pt[i].valid) continue;
+            const float w = member_weight(anc, k, p.n_members, pt[i].x, pt[i].y, pt[i].z);
+            need |= PRUNE ? w >= thr[i] : w != 0.f;
+        }
+        if (__any_sync(0xffffffffu, need)) mask |= 1ull << k;
+    }
+    if (lane == 0) p.tile_masks[tile] = mask;
+}
+
 template <bool PRUNE, bool ACTS>
 __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Params p)
 {
@@ -129,7 +169,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     if (threadIdx.x == 0) {
         for (int i = 0; i < kSlots; ++i) { mbar_init(&sm.w_full[i], 1); mbar_init(&sm.w_empty[i], kConsumerWarps); }
         for (int i = 0; i < kRecSlots; ++i) { mbar_init(&sm.rec_full[i], 1); mbar_init(&sm.rec_empty[i], kConsumerWarps); }
-        mbar_init(&sm.mask_ready, kConsumerWarps);
+        for (int i = 0; i < 2; ++i) { mbar_init(&sm.q_full[i], 1); mbar_init(&sm.q_empty[i], kConsumerWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -137,25 +177,30 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     const long long cta_start = clock64();
     if (blockIdx.x == 0 && threadIdx.x == 0) { g_ens_trace[0] = cta_start; g_ens_ctas[0] = gridDim.x; }
 #endif
-    // the consumers vote on the members of every tile: the pruned rule, or (dense variant) exactly zero blend weights
-    const bool vote = PRUNE || (!ACTS && p.zero_skip);
+    // tile masks from the pre-pass: the pruned rule, or (dense variant) exactly zero blend weights
+    const bool premask = PRUNE || (!ACTS && p.zero_skip);
 
     if (warp >= kConsumerWarps) {
-        // =========================================================================== producer (bulk async copies)
+        // =========================================================================== producer (tiles, bulk async copies)
         asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
         if (warp == kConsumerWarps && lane == 0) {
-            uint32_t tcount = 0, rcount = 0;
-            for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
-                const long long tile = ACTS ? item / n_groups : item;
-                const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
-                unsigned long long mask = group_mask(item);
-                if (vote) {
-                    mbar_wait(&sm.mask_ready, tcount & 1);
-                    mask = 0;
-                    for (int w = 0; w < kConsumerWarps; ++w) mask |= sm.maskq[tcount & 1][w];
-                }
-                for (int m = 0; m < p.n_members; ++m) {
-                    if (!((mask >> m) & 1)) continue;
+            uint32_t rcount = 0;
+            for (uint32_t tcount = 0;; ++tcount) {
+                // take the next work item and pass it on with its member mask (the end of the work as item -1)
+                const unsigned int item = atomicAdd(p.sched, 1u);
+                const bool more = item < n_items;
+                const unsigned int tile = ACTS ? item / n_groups : item;
+                const int qi = p.blocked ? 0 : (int)(tile / (unsigned int)tiles_per_query);
+                unsigned long long mask = !more ? 0ull : (premask ? p.tile_masks[tile] : group_mask(item));
+                ENS_TILE(tcount, 1);
+                const int qs = tcount & 1;
+                mbar_wait(&sm.q_empty[qs], ((tcount >> 1) & 1) ^ 1);
+                sm.q_item[qs] = more ? (long long)item : -1;
+                sm.q_mask[qs] = mask;
+                mbar_arrive(&sm.q_full[qs]);
+                if (!more) break;
+                for (; mask; mask &= mask - 1) {         // the tile's members in ascending order
+                    const int m = __ffsll((long long)mask) - 1;
                     const int rslot = rcount % kRecSlots;
                     mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
                     mbar_expect_tx(&sm.rec_full[rslot], kRecFloats * 4);
@@ -184,6 +229,13 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                     }
                 }
             }
+            // every CTA has taken its last item once all have counted themselves finished: the last one resets the counter
+            // for the next launch on the stream
+            __threadfence();
+            if (atomicAdd(p.sched + 1, 1u) == gridDim.x - 1) {
+                atomicExch(p.sched, 0u);
+                atomicExch(p.sched + 1, 0u);
+            }
         }
         return;
     }
@@ -194,7 +246,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     int rl[2];                                   // tile rows (points) of this thread's accumulator rows
     rl[0] = 64 * wgi + 16 * (warp & 3) + (lane >> 2);
     rl[1] = rl[0] + 8;
-    uint32_t tcount = 0, rcount = 0;
+    uint32_t rcount = 0;
     auto release = [&](int u) { __syncwarp(); if (lane == 0) mbar_arrive(&sm.w_empty[u & 3]); };
     auto release_rec = [&](uint64_t *bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
     auto wait_unit = [&](int u) { mbar_wait(&sm.w_full[u & 3], (u >> 2) & 1); };
@@ -211,81 +263,32 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     };
     if (wgi == 1) pass_turn();                   // warpgroup 0 issues first
 
-    for (long long item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
+    for (uint32_t tcount = 0;; ++tcount) {
+        // the next tile and its member mask from the producer's queue: no vote and no wait for the other warpgroup, so the
+        // phase offset of the warpgroups carries over from one tile to the next
+        const int qs = tcount & 1;
+        mbar_wait(&sm.q_full[qs], (tcount >> 1) & 1);
+        const long long item = sm.q_item[qs];
+        const unsigned long long mask = sm.q_mask[qs];
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sm.q_empty[qs]);
+        if (item < 0) break;
+        if (threadIdx.x == 0) ENS_TILE(tcount, 0);
         const long long tile = ACTS ? item / n_groups : item;
         const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
-        ENS_TILE(tcount, 0);
         long long idx[2], g[2];
         bool valid[2], quirk[2];
         float x[2], y[2], z[2];
+        float num[2] = {0.f, 0.f}, den[2] = {0.f, 0.f};
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            const int row = rl[i];
-            if (!ACTS && p.blocked) {             // (the fitting variant only runs linear tiles)
-                // compact tbx x tby x tbz block of grid points (z fastest inside the block)
-                const long long tz = tile % p.bz, txy = tile / p.bz;
-                const int ty = (int)(txy % p.by), tx = (int)(txy / p.by);
-                const int ix = p.px0 + tx * p.tbx + row / (p.tby * p.tbz), iy = ty * p.tby + (row / p.tbz) % p.tby,
-                          iz = (int)tz * p.tbz + row % p.tbz;
-                g[i] = ((long long)ix * p.res + iy) * p.res + iz;
-                valid[i] = ix <= p.px1 && iy < p.res && iz < p.res && g[i] >= p.first && g[i] < p.first + p.n_points;
-                idx[i] = g[i] - p.first;
-                const int cx_ = min(ix, p.res - 1), cy_ = min(iy, p.res - 1), cz_ = min(iz, p.res - 1);
-                x[i] = __ldg(p.axes + cx_); y[i] = __ldg(p.axes + p.res + cy_); z[i] = __ldg(p.axes + 2 * p.res + cz_);
-                if (!valid[i]) g[i] = p.first;
-            } else {
-                idx[i] = (tile - (long long)qi * tiles_per_query) * 128 + row;
-                valid[i] = idx[i] < p.n_points;
-                g[i] = p.first + (valid[i] ? idx[i] : 0);
-                if (p.xyz) {
-                    const float *pp = p.xyz + ((size_t)qi * p.n_points + (valid[i] ? idx[i] : 0)) * 3;
-                    x[i] = pp[0]; y[i] = pp[1]; z[i] = pp[2];
-                } else {
-                    const long long rr = (long long)p.res * p.res;
-                    const int ix = (int)(g[i] / rr), iy = (int)((g[i] - ix * rr) / p.res), iz = (int)(g[i] % p.res);
-                    x[i] = __ldg(p.axes + ix); y[i] = __ldg(p.axes + p.res + iy); z[i] = __ldg(p.axes + 2 * p.res + iz);
-                }
-            }
+            // (the fitting variant only runs linear tiles)
+            const TilePoint t = tile_point(p, !ACTS && p.blocked, tile, qi, tiles_per_query, rl[i]);
+            idx[i] = t.idx; g[i] = t.g; valid[i] = t.valid; x[i] = t.x; y[i] = t.y; z[i] = t.z;
             quirk[i] = p.quirk_period > 0 && ((g[i] % p.quirk_period) == p.quirk_period - 1 || g[i] == p.total - 1);
+            // pruned rule: the blend divides by S = sum_k w_k over all members, evaluated or not
+            if (PRUNE) den[i] = weight_sum(p.anchors + (size_t)qi * (p.n_members - 1) * 3, p.n_members, x[i], y[i], z[i]);
         }
-        float num[2] = {0.f, 0.f}, den[2] = {0.f, 0.f};
-        unsigned long long mask = group_mask(item);
-        if (vote) {
-            // blend weights of the members for this thread's points (the last, global member is always needed: every tile
-            // evaluates >= 1 member).  Pruned rule: S = sum_k w_k; a member is needed if w_k >= tau * (S + 1e-6) for at least
-            // one valid point of the tile (dropped mass per point < n_members * tau).  Dense rule: a member is needed if
-            // w_k != 0 for at least one valid point - a member with w_k = +0 everywhere adds exactly nothing to num and den.
-            const float *anc = p.anchors + (size_t)qi * (p.n_members - 1) * 3;
-            auto weight = [&](int k, int i) {
-                if (k == p.n_members - 1) return blend_weight(false, 0.f, 0.f, 0.f, x[i], y[i], z[i]);
-                return blend_weight(true, __ldg(anc + 3 * k), __ldg(anc + 3 * k + 1), __ldg(anc + 3 * k + 2), x[i], y[i], z[i]);
-            };
-            float thr[2] = {0.f, 0.f};
-            if (PRUNE) {
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    float S = 0.f;
-                    for (int k = 0; k < p.n_members; ++k) S += weight(k, i);
-                    den[i] = S;
-                    thr[i] = p.prune_tau * (S + 1e-6f);
-                }
-            }
-            unsigned long long wm = 1ull << (p.n_members - 1);
-            for (int k = 0; k < p.n_members - 1; ++k) {
-                bool need;
-                if (PRUNE) need = (valid[0] && weight(k, 0) >= thr[0]) || (valid[1] && weight(k, 1) >= thr[1]);
-                else need = (valid[0] && weight(k, 0) != 0.f) || (valid[1] && weight(k, 1) != 0.f);
-                if (__any_sync(0xffffffffu, need)) wm |= 1ull << k;
-            }
-            if (lane == 0) {
-                sm.maskq[tcount & 1][warp] = wm;
-                mbar_arrive(&sm.mask_ready);
-            }
-            mbar_wait(&sm.mask_ready, tcount & 1);
-            mask = 0;
-            for (int w = 0; w < kConsumerWarps; ++w) mask |= sm.maskq[tcount & 1][w];
-        }
-        ENS_TILE(tcount, 1);
         const uint32_t tile_rc0 = rcount;        // the tile's first member (timeline build)
 
         for (int m = 0; m < p.n_members; ++m) {
@@ -346,7 +349,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
             wait_unit(0);
             wait_unit(1);
             ENS_CEVT(rcount, 0, 1);
-            if (rcount == tile_rc0) ENS_TILE(tcount, 2);
+            if (threadIdx.x == 0 && rcount == tile_rc0) ENS_TILE(tcount, 2);
             take_turn();
             ENS_CEVT(rcount, 0, 2);
             {
@@ -548,6 +551,12 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
 
 int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream)
 {
+    if (prune || (!acts && p.zero_skip)) {
+        const unsigned blocks = (unsigned)ceil_div(p.n_tiles, (long long)wg::kMaskWarps);
+        if (prune) wg::tile_mask_kernel<true><<<blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
+        else wg::tile_mask_kernel<false><<<blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
     const int smem = (int)sizeof(wg::Smem);
     auto kern = acts ? wg::ensemble_wgmma_kernel<false, true>
                      : (prune ? wg::ensemble_wgmma_kernel<true, false> : wg::ensemble_wgmma_kernel<false, false>);

@@ -3,8 +3,9 @@
 of the seeded head of bench.py and prints, for four consecutive members of CTA 0, when each consumer warpgroup waited for its
 weights, issued and retired its MMAs and finished its epilogues, when the producer issued each weight unit, and per member:
 cycles waiting for weights, cycles in which neither warpgroup had MMAs in flight, epilogue cycles.  Then, per tile of CTA 0,
-the cycles until the tile's member mask and its first member's weights were ready, and over all CTAs the member-tiles the
-kernel evaluated (to set against tools/zero_member_tiles.py) and the cycles per evaluated member-tile.
+when warpgroup 0 took it from the producer's queue, when the producer knew its member mask (before that, when negative) and
+when the first member's layer-1 weights were ready; over all CTAs the member-tiles the kernel evaluated (to set against
+tools/zero_member_tiles.py), the cycles per evaluated member-tile, and the spread of member-tiles and cycles per CTA.
 
     bash tools/build_variant.sh /tmp/ens -DNPHM_ENS_TRACE && NPHM_B200_LIB=/tmp/ens/libnphm_b200.so python tools/ens_trace.py [res]"""
 import ctypes, os, sys
@@ -91,13 +92,16 @@ def main():
     tiles = w[:3 * TILES].reshape(TILES, 3) - t0
     for i in range(TILES):
         length = ' (%d cycles to the next tile)' % (tiles[i + 1, 0] - tiles[i, 0]) if i + 1 < TILES else ''
-        print('tile %d of CTA 0: start %d, mask ready +%d, first member\'s layer-1 weights ready +%d%s'
-              % (i, tiles[i, 0], tiles[i, 1] - tiles[i, 0], tiles[i, 2] - tiles[i, 0], length))
+        print('tile %d of CTA 0: taken from the queue at %d, mask known to the producer %+d, first member\'s layer-1 '
+              'weights ready %+d%s' % (i, tiles[i, 0], tiles[i, 1] - tiles[i, 0], tiles[i, 2] - tiles[i, 0], length))
     n_ctas = int(w[3 * TILES])
     ctas = w[3 * TILES + 1:3 * TILES + 1 + 2 * n_ctas].reshape(n_ctas, 2)
     mt, cyc = int(ctas[:, 0].sum()), int(ctas[:, 1].sum())
     print('all %d CTAs: %d member-tiles evaluated, %.0f cycles per evaluated member-tile (CTA cycles summed / member-tiles)'
           % (n_ctas, mt, cyc / max(mt, 1)))
+    for col, name in ((0, 'member-tiles'), (1, 'cycles')):
+        v = ctas[:, col].astype(np.float64)
+        print('per CTA %s: min %.0f, mean %.0f, max %.0f, max / mean %.4f' % (name, v.min(), v.mean(), v.max(), v.max() / v.mean()))
 
 
 if __name__ == '__main__':
