@@ -224,7 +224,8 @@ int nphm_mlp_jacobian(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, 
  * network:  grad_cond_dev [q][lat_dim] = sum_n (d out_n / d cond_q)^T grad_out_n  (may be NULL),
  *           grad_xyz_dev [q][n][3]    = (d out_n / d xyz_n)^T grad_out_n            (may be NULL).   grad_out_dev: [q][n][out_dim].
  * xyz_dev == NULL: reuse the activations of the preceding nphm_mlp_jacobian / nphm_mlp_inverse_jacobian call on this handle
- * (same points, same condition) instead of recomputing the value pass. */
+ * (same points, same condition) instead of recomputing the value pass.  grad_out may have any magnitude: each query's
+ * upstream is scaled on the device by a power of two into the range of the fp16 adjoint, and the gradients scaled back. */
 int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
                              const float *grad_out_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream);
 /* (I + d out / d xyz)^-1 per point for a 3-output stack == `jac(decoder_expr, x, ...).inverse()` of the reference

@@ -129,6 +129,15 @@ __global__ void xyz_grad_kernel(const float *__restrict__ a, const float *__rest
     out[idx] = (a[r * 4 + i] + b[r * 4 + i]) * (scale ? scale[sstride * member_set(m, n_symm) + 1] : 1.0f);
 }
 
+// dst[i] = src[i] * scale[2 q + which], q = i / per_query: one scale pair per query (grad_scale_kernel); in place is fine
+__global__ void query_scale_kernel(const float *src, long long per_query, long long n, const float *__restrict__ scale, int which,
+                                   float *dst)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n) return;
+    dst[idx] = src[idx] * scale[2 * (idx / per_query) + which];
+}
+
 }  // namespace chain
 
 // ------------------------------------------------------------------------------------------------ members and packed stack
@@ -162,9 +171,9 @@ struct MlpChain : PackedChain {
     // appends them); packed on first use after every weight load.
     tcl::PackedLinear tfwd[kMaxLayers];
     int train_nd = -1;
-    // scratch of the first-order backwards: the packed top adjoint, its scale pair, the two [M][4] point-gradient parts (d_0
-    // and d_skip times their layer's xyz columns)
-    DeviceBuffer Dl, gscale, xtmp, xs_tmp;
+    // scratch of the first-order backwards: the packed top adjoint, its scale pairs, the two [M][4] point-gradient parts (d_0
+    // and d_skip times their layer's xyz columns), the scaled upstream of the adjoint pass
+    DeviceBuffer Dl, gscale, xtmp, xs_tmp, gup;
 };
 
 // the stack a pass runs on
@@ -519,7 +528,18 @@ extern "C" int nphm_mlp_jacobian(nphm_mlp *h, const float *xyz_dev, const float 
     return NPHM_OK;
 }
 
+namespace nphm {
+namespace train {
+__global__ void grad_scale_kernel(const float *__restrict__ g, long long n, const float *__restrict__ g2, long long n2, int n_symm,
+                                  float *__restrict__ scale);
+}  // namespace train
+}  // namespace nphm
+
 // adjoint pass: grad_cond [q][cond_dim] = sum_n (d out_n / d cond)^T grad_out_n ; grad_xyz [q][n][3] optional
+// fp16 range: every d_l is stored as an fp16 hi | lo pair, which keeps its bits only while |d_l| >= 2^-3 (see kGradExp), and
+// the joint fitters' upstream u = -J^-T g_x is ~1e-4.  So the upstream is scaled on the device by one power of two per query,
+// its largest magnitude to 2^kGradExp (grad_scale_kernel; an all-zero or non-finite query keeps scale 1), and the gradients
+// are multiplied back in fp32 (exact).  Per query: a query's gradients do not depend on the other queries of the call.
 extern "C" int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const float *cond_dev, int n_queries, long long n_points,
                                         const float *grad_out_dev, float *grad_cond_dev, float *grad_xyz_dev, void *stream_)
 {
@@ -553,9 +573,17 @@ extern "C" int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const
         return rc;
     NPHM_CUDA_CHECK(cudaMemsetAsync(c.sums0.ptr, 0, (size_t)n_queries * s.N[0] * sizeof(float), stream));
     NPHM_CUDA_CHECK(cudaMemsetAsync(c.sumss.ptr, 0, (size_t)n_queries * s.N[s.skip] * sizeof(float), stream));
-    // the output layer's adjoint is the caller's grad_out as it is; d_l lives in Dp[l & 1]
+    // the output layer's adjoint is the caller's grad_out times its query's scale; d_l lives in Dp[l & 1]
+    if ((rc = c.gscale.reserve((size_t)2 * n_queries * sizeof(float))) || (rc = c.gup.reserve((size_t)M * out_dim * sizeof(float))))
+        return rc;
+    float *gs = c.gscale.as<float>(), *gup = c.gup.as<float>();
+    train::grad_scale_kernel<<<n_queries, 1024, 0, stream>>>(grad_out_dev, n_points * out_dim, nullptr, 0, 0, gs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    chain::query_scale_kernel<<<(unsigned)ceil_div(M * out_dim, 256), 256, 0, stream>>>(grad_out_dev, n_points * out_dim,
+                                                                                       M * out_dim, gs, 0, gup);
+    NPHM_CUDA_CHECK(cudaGetLastError());
     AdjointWalk w;
-    w.top = Adjoint{grad_out_dev, out_dim, nullptr, 0, 0};
+    w.top = Adjoint{gup, out_dim, nullptr, 0, 0};
     for (int l = 0; l < L; ++l) { w.S[l] = c.S[l].as<float>(); w.D[l] = c.Dp[l & 1].as<uint8_t>(); }
     w.xs = grad_xyz_dev ? c.xs_tmp.as<float>() : nullptr;
     // the column sums of d_0 and d_skip feed the condition gradient
@@ -568,8 +596,19 @@ extern "C" int nphm_mlp_backward_inputs(nphm_mlp *h, const float *xyz_dev, const
     };
     const Stack k = stack(h);
     if ((rc = adjoint_walk(k, M, w, col_sums, stream))) return rc;
-    if (grad_cond_dev && (rc = cond_grad(k, n_queries, 16, grad_cond_dev, stream))) return rc;
-    if (grad_xyz_dev && (rc = xyz_grad(k, M, w.D[0], 0, c.xtmp.as<float>(), w.xs, nullptr, 0, grad_xyz_dev, stream))) return rc;
+    // undo the scale: grad_cond rows per query, grad_xyz rows per query's points
+    if (grad_cond_dev) {
+        if ((rc = cond_grad(k, n_queries, 16, grad_cond_dev, stream))) return rc;
+        chain::query_scale_kernel<<<(unsigned)ceil_div((long long)n_queries * s.cond_dim, 256), 256, 0, stream>>>(
+            grad_cond_dev, s.cond_dim, (long long)n_queries * s.cond_dim, gs, 1, grad_cond_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    if (grad_xyz_dev) {
+        if ((rc = xyz_grad(k, M, w.D[0], 0, c.xtmp.as<float>(), w.xs, nullptr, 0, grad_xyz_dev, stream))) return rc;
+        chain::query_scale_kernel<<<(unsigned)ceil_div(M * 3, 256), 256, 0, stream>>>(grad_xyz_dev, n_points * 3, M * 3, gs, 1,
+                                                                                     grad_xyz_dev);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
     return NPHM_OK;
 }
 

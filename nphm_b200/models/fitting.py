@@ -416,16 +416,6 @@ def _native_npm_joint(decoder, decoder_expr, device) -> bool:
     return next(decoder.parameters()).device == device and next(decoder_expr.parameters()).device == device
 
 
-def _pow2_scale(x: torch.Tensor, groups: int = 0) -> torch.Tensor:
-    """A power of two (0-dim tensor, computed on the device) that brings the largest magnitude of ``x`` to [2^9, 2^10); with
-    ``groups``, one such power per group (a ``groups`` tensor) of ``x`` split into ``groups`` equal parts along its first axis."""
-    if groups:
-        _, e = torch.frexp(x.reshape(groups, -1).abs().amax(1))
-        return torch.ldexp(torch.ones(groups, device=x.device), 10 - e)
-    _, e = torch.frexp(x.abs().amax())
-    return torch.ldexp(torch.ones((), device=x.device), 10 - e)
-
-
 class NpmIdentityFitter:
     """``inference_identity_space`` for a one-output ``DeepSDF`` (reference fitting.py:180-285) without an autograd graph.
     Per iteration: the surface term with its code gradient (``nphm_mlp_fit_surface_grad``, all sampled points as one query
@@ -471,8 +461,8 @@ class NpmJointFitter:
         d surface / d z_id, g_x = d surface / d xc  (mask = valid)                          nphm_mlp_fit_surface_grad
         u = -J^-T g_x,  g_cond = sum_n (dF/d cond)^T u_n                                      nphm_mlp_backward_inputs (value pass reused)
         z_id += g_cond[:, :D] summed over the scans,  z_ex[idx_b] += g_cond[b, D:] + reg_expr,  two Adam steps.
-    u is of order 1e-4 and the adjoint pass works on fp16 hi | lo operands, so u is scaled by a power of two (largest magnitude
-    to 2^10, chosen on the device) before the call and g_cond is divided by it afterwards; the adjoint is linear in u."""
+    u is of order 1e-4; the adjoint pass, which works on fp16 hi | lo operands, scales each query's upstream into their range
+    itself."""
 
     def __init__(self, decoder, decoder_expr, num_observations: int, device):
         self.device = device
@@ -513,9 +503,7 @@ class NpmJointFitter:
                                                             workspace=self._ws[1])
             self.loss_terms.copy_(terms)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                     # -J^-T g_x
-            sc = _pow2_scale(u)
-            g_cond, _ = self.mlp.backward_inputs(p, cond, u * sc, reuse_value_pass=True)
-            g_cond = g_cond / sc
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)
             g_zid = lam_s * (g_lat[0] + g_cond[:, :D].sum(0)) + (2.0 * lam_g) * self.z_id
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
@@ -964,9 +952,8 @@ class BatchedNpmJointFitter:
     iteration, for the 5 sampled observations of every subject:
         condition rows [z_id[subject] | z_ex[row]]; J0^-1, sync-free Broyden and J^-1 on all 5 S rows
         nphm_mlp_fit_surface_grad_batched (mask = valid and not padding): per-subject surface term, d/d z_id and d/d point
-        u = -J^-T g_x, scaled by one power of two per subject (its largest magnitude to 2^10 over that subject's rows, so that
-        each subject feeds the fp16 adjoint what its single-subject call would); one adjoint pass with the value pass reused,
-        the g_cond rows divided by their subject's scale
+        u = -J^-T g_x; one adjoint pass with the value pass reused (it scales every row's upstream on its own, so each subject's
+        rows get what its single-subject call gives them)
         z_id: g_cond[:, :D] summed per subject; z_ex rows: g_cond[:, D:] + reg_expr; two nphm_adam_step calls.
     The expression codes are one (sum n_obs) x 200 tensor; subject k's rows start at ``offsets[k]``.  Memory grows linearly with
     S: the Jacobian, Broyden and adjoint buffers of 5 S n_point rows through the expression stack, about 1.4 GB per subject of
@@ -1025,9 +1012,7 @@ class BatchedNpmJointFitter:
                                                                     workspace=self._ws[1])
             self.loss_terms.copy_(terms)
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
-            sc = _pow2_scale(u, S).repeat_interleave(nb)                                 # per subject, one entry per row
-            g_cond, _ = self.mlp.backward_inputs(p, cond, u * sc[:, None, None], reuse_value_pass=True)
-            g_cond = g_cond / sc[:, None]
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)
             g_zid = lam_s * (g_lat + g_cond[:, :D].reshape(S, nb, D).sum(1)) + (2.0 * lam_g) * self.z_id
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, rows, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[rows])

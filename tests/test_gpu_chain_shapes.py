@@ -112,6 +112,39 @@ def test_jacobian_and_adjoint(cuda_device, cfg):
     chk.done()
 
 
+# Upstream magnitudes of the adjoint pass: randn, the joint fitters' u = -J^-T g_x (d surface / d xc over a few thousand
+# kept points, 1e-4 and below) and smaller still.  The pass holds every adjoint as an fp16 hi | lo pair, whose lo part is
+# subnormal below 2^-3 and whose hi part is below 2^-14; it has to scale the upstream into that range itself.
+UPSTREAM_SCALES = [1.0, 2.0 ** -12, 1e-4, 1e-6]
+
+
+@pytest.mark.parametrize('cfg', C.PRODUCTION, ids=C.config_id)
+def test_adjoint_upstream_range(cuda_device, cfg):
+    """backward_inputs (condition and point gradients, fresh points and reusing the value pass of inverse_jacobian /
+    jacobian) on the production stacks with upstreams of every magnitude in UPSTREAM_SCALES; no range-defect exemption."""
+    net, eng, P64, P32 = _setup(cfg, cuda_device)
+    chk = Check(cfg)
+    for B, N in ((1, 129), (9, 37), (5, 1000)):
+        x, c, x64, c64 = _inputs(cfg, B, N, cuda_device)
+        base = torch.randn(B, N, cfg[3], device=cuda_device, generator=torch.Generator(cuda_device).manual_seed(3 * B + N))
+        for sc in UPSTREAM_SCALES:
+            up = base * sc
+            _, gc64, gx64, _, _ = C.ref_vjp(P64, x64, c64, up.double())
+            _, gc32, gx32, _, _ = C.ref_vjp(P32, x, c, up)
+            what = 'backward_inputs up %.0e %dx%d' % (sc, B, N)
+            g_c, g_x = eng.backward_inputs(x, c, up, want_xyz=True)
+            chk(what + ' cond', g_c, gc64, gc32, 'cond')
+            chk(what + ' xyz', g_x, gx64, gx32)
+            if cfg[3] == 3:
+                eng.inverse_jacobian(x, c)
+            else:
+                eng.jacobian(x, c)
+            g_c, g_x = eng.backward_inputs(x, c, up, want_xyz=True, reuse_value_pass=True)
+            chk(what + ' reuse cond', g_c, gc64, gc32, 'cond')
+            chk(what + ' reuse xyz', g_x, gx64, gx32)
+    chk.done()
+
+
 # ------------------------------------------------------------------------------------------------ first-order training
 TRAIN = [(cfg, nd) for cfg in C.CONFIGS for nd in C.noise_dims(cfg)]
 
