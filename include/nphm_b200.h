@@ -482,6 +482,43 @@ int nphm_band_fill(int res, int block, float *vol_dev, void *workspace_dev, long
 /* states_dev (blocks^3 bytes, blocks = ceil((res-1)/block), x slowest): 0 inactive, 1 or 2 active */
 int nphm_band_block_states(int res, int block, const void *workspace_dev, long long workspace_bytes, unsigned char *states_dev,
                            void *stream);
+/* The same steps on an x-slab of the grid, for extracting one mesh on several GPUs (nphm_b200/distributed.py:
+ * extract_mesh_narrowband_sharded, DESIGN §4.16): the slab owns the block layers [l0, l1) along x (0 <= l0 < l1 <= blocks) and
+ * holds the voxel planes [X0, X1] = [l0*block, min(l1*block, res-1)]; a plane X0 > 0 or X1 < res-1 is shared with the neighbouring
+ * slab.  Its workspace (nphm_band_slab_workspace_bytes, -1: bad arguments) covers those planes only, and every vol_dev is the slab
+ * volume of planes X0-1 .. X1, res^2 floats each, where plane X0-1 (the ghost plane the slab marching cubes reads with
+ * x_global0 = X0-1, ghost_lo = 1) is present only when l0 > 0.  List indices are local to the slab; nphm_band_slab_gather writes
+ * the global grid coordinates.  nphm_band_slab_begin lists the quirk voxels of global flat index in the slab's planes and
+ * activates the slab's blocks around them; nphm_band_slab_corners lists the corners on the slab's planes; the block states are
+ * (l1-l0) x blocks x blocks.  Together with a neighbour, after each round of evaluation:
+ *   nphm_band_slab_export  writes plane `plane` of [X0, X1] to buf_dev: res^2 floats of the volume, then res^2 bytes (1: the voxel
+ *                          is evaluated on this slab)
+ *   nphm_band_slab_import  merges a buffer the neighbour exported of the plane both hold (X0 from below, X1 from above): every
+ *                          voxel the neighbour evaluated and this slab did not takes its value and counts as evaluated, so that
+ *                          nphm_band_slab_grow sees it as nphm_band_grow does on the whole grid.  After nphm_band_slab_fill,
+ *                          plane X0-1 imports the filled values of the lower neighbour's plane X1-1 into the ghost plane.
+ * Any other plane is NPHM_ERR_INVALID, as is an empty or out-of-range slab.  Export and import enqueue kernels only. */
+long long nphm_band_slab_workspace_bytes(int res, int block, int l0, int l1);
+int nphm_band_slab_begin(int res, int block, int l0, int l1, long long quirk_period, void *workspace_dev, long long workspace_bytes,
+                         long long *counts_host, void *stream);
+int nphm_band_slab_corners(int res, int block, int l0, int l1, void *workspace_dev, long long workspace_bytes,
+                           long long *counts_host, void *stream);
+int nphm_band_slab_gather(int res, int block, int l0, int l1, const double grid_min[3], const double grid_max[3], long long n,
+                          float *xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream);
+int nphm_band_slab_scatter(int res, int block, int l0, int l1, long long n, const float *values_dev, float *vol_dev,
+                           void *workspace_dev, long long workspace_bytes, void *stream);
+int nphm_band_slab_classify(int res, int block, int l0, int l1, float tau, const float *vol_dev, void *workspace_dev,
+                            long long workspace_bytes, long long *counts_host, void *stream);
+int nphm_band_slab_grow(int res, int block, int l0, int l1, const float *vol_dev, void *workspace_dev, long long workspace_bytes,
+                        long long *counts_host, void *stream);
+int nphm_band_slab_fill(int res, int block, int l0, int l1, float *vol_dev, void *workspace_dev, long long workspace_bytes,
+                        void *stream);
+int nphm_band_slab_block_states(int res, int block, int l0, int l1, const void *workspace_dev, long long workspace_bytes,
+                                unsigned char *states_dev, void *stream);
+int nphm_band_slab_export(int res, int block, int l0, int l1, int plane, const float *vol_dev, const void *workspace_dev,
+                          long long workspace_bytes, unsigned char *buf_dev, void *stream);
+int nphm_band_slab_import(int res, int block, int l0, int l1, int plane, const unsigned char *buf_dev, float *vol_dev,
+                          void *workspace_dev, long long workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Training supervision (DESIGN §4.15): the sampling steps of scripts/data_processing/sample_surface.py:32-135 (stage 1) and

@@ -44,6 +44,9 @@ EXPORTED_SYMBOLS = (
     'nphm_render_workspace_bytes', 'nphm_render_depth_normals',
     'nphm_band_workspace_bytes', 'nphm_band_begin', 'nphm_band_corners', 'nphm_band_gather', 'nphm_band_scatter',
     'nphm_band_classify', 'nphm_band_grow', 'nphm_band_fill', 'nphm_band_block_states',
+    'nphm_band_slab_workspace_bytes', 'nphm_band_slab_begin', 'nphm_band_slab_corners', 'nphm_band_slab_gather',
+    'nphm_band_slab_scatter', 'nphm_band_slab_classify', 'nphm_band_slab_grow', 'nphm_band_slab_fill', 'nphm_band_slab_block_states',
+    'nphm_band_slab_export', 'nphm_band_slab_import',
     'nphm_face_cdf_workspace_bytes', 'nphm_face_cdf', 'nphm_sample_faces', 'nphm_vertex_normals_workspace_bytes',
     'nphm_vertex_normals', 'nphm_interpolate_barycentric', 'nphm_transfer_correspondences',
 )
@@ -220,6 +223,13 @@ def lib() -> ctypes.CDLL:
     L.nphm_band_grow.argtypes = [c_int, c_int, c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
     L.nphm_band_fill.argtypes = [c_int, c_int, c_void_p, c_void_p, c_longlong, c_void_p]
     L.nphm_band_block_states.argtypes = [c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p]
+    slab = [c_int, c_int, c_int, c_int]                 # res, block, l0, l1: the same steps on an x-slab
+    L.nphm_band_slab_workspace_bytes.argtypes = slab
+    L.nphm_band_slab_workspace_bytes.restype = c_longlong
+    for name in ('begin', 'corners', 'gather', 'scatter', 'classify', 'grow', 'fill', 'block_states'):
+        getattr(L, 'nphm_band_slab_' + name).argtypes = slab + getattr(L, 'nphm_band_' + name).argtypes[2:]
+    L.nphm_band_slab_export.argtypes = slab + [c_int, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_band_slab_import.argtypes = slab + [c_int, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
     L.nphm_face_cdf_workspace_bytes.argtypes = [c_longlong]
     L.nphm_face_cdf_workspace_bytes.restype = c_longlong
     L.nphm_face_cdf.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, POINTER(c_double), c_void_p, c_longlong, c_void_p]
@@ -957,61 +967,109 @@ class NarrowBand:
     owns.  The listing steps return the number of voxels they listed; :meth:`gather` / :meth:`scatter` move the listed voxels'
     coordinates out and their values into a ``res^3`` float32 CUDA volume."""
 
+    _prefix = 'nphm_band_'
+
     def __init__(self, res: int, block: int, device):
         self.res, self.block = int(res), int(block)
         self.device = torch.device(device)
+        self._geo = self._geometry()
         with torch.cuda.device(self.device):
-            self.ws = _workspace(lib().nphm_band_workspace_bytes(self.res, self.block), 'nphm_band_workspace_bytes', self.device)
+            self.ws = _workspace(self._fn('workspace_bytes')(*self._geo), self._prefix + 'workspace_bytes', self.device)
         self.blocks_per_axis = -(-(self.res - 1) // self.block)
         self.active_blocks = 0
 
-    def _call_listing(self, name, *before_ws):
-        counts = (c_longlong * 2)()
+    def _geometry(self):
+        return self.res, self.block
+
+    def _fn(self, step):
+        return getattr(lib(), self._prefix + step)
+
+    def _call(self, step, *args):
         with torch.cuda.device(self.device):
-            check(getattr(lib(), name)(self.res, self.block, *before_ws, self.ws.data_ptr(), self.ws.numel(), counts,
-                                       _stream_ptr(self.device)), name)
+            check(self._fn(step)(*self._geo, *args, _stream_ptr(self.device)), self._prefix + step)
+
+    def _call_listing(self, step, *before_ws):
+        counts = (c_longlong * 2)()
+        self._call(step, *before_ws, self.ws.data_ptr(), self.ws.numel(), counts)
         self.active_blocks = counts[1]
         return counts[0]
 
     def begin(self, quirk_period: int = 0) -> int:
         """Reset; with ``quirk_period > 0`` list the eval-mode quirk voxels and activate the blocks around them."""
-        return self._call_listing('nphm_band_begin', int(quirk_period))
+        return self._call_listing('begin', int(quirk_period))
 
     def corners(self) -> int:
-        return self._call_listing('nphm_band_corners')
+        return self._call_listing('corners')
 
     def classify(self, tau: float, vol: torch.Tensor) -> int:
-        return self._call_listing('nphm_band_classify', float(tau), vol.data_ptr())
+        return self._call_listing('classify', float(tau), vol.data_ptr())
 
     def grow(self, vol: torch.Tensor) -> int:
-        return self._call_listing('nphm_band_grow', vol.data_ptr())
+        return self._call_listing('grow', vol.data_ptr())
 
     def gather(self, n: int, mini, maxi) -> torch.Tensor:
         """(n, 3) float32 coordinates of the first ``n`` listed voxels."""
         xyz = torch.empty(int(n), 3, device=self.device, dtype=torch.float32)
         gmin = (c_double * 3)(*[float(v) for v in mini])
         gmax = (c_double * 3)(*[float(v) for v in maxi])
-        with torch.cuda.device(self.device):
-            check(lib().nphm_band_gather(self.res, self.block, gmin, gmax, int(n), _ptr(xyz) if n else None, self.ws.data_ptr(),
-                                         self.ws.numel(), _stream_ptr(self.device)), 'nphm_band_gather')
+        self._call('gather', gmin, gmax, int(n), _ptr(xyz) if n else None, self.ws.data_ptr(), self.ws.numel())
         return xyz
 
     def scatter(self, values: torch.Tensor, vol: torch.Tensor):
         v = _f32c(values).reshape(-1)
-        with torch.cuda.device(self.device):
-            check(lib().nphm_band_scatter(self.res, self.block, v.numel(), v.data_ptr() if v.numel() else None, vol.data_ptr(),
-                                          self.ws.data_ptr(), self.ws.numel(), _stream_ptr(self.device)), 'nphm_band_scatter')
+        self._call('scatter', v.numel(), v.data_ptr() if v.numel() else None, vol.data_ptr(), self.ws.data_ptr(), self.ws.numel())
 
     def fill(self, vol: torch.Tensor):
-        with torch.cuda.device(self.device):
-            check(lib().nphm_band_fill(self.res, self.block, vol.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
-                                       _stream_ptr(self.device)), 'nphm_band_fill')
+        self._call('fill', vol.data_ptr(), self.ws.data_ptr(), self.ws.numel())
+
+    def _states_shape(self):
+        nb = self.blocks_per_axis
+        return nb, nb, nb
 
     def block_states(self) -> torch.Tensor:
-        """(blocks, blocks, blocks) bool: which blocks are active."""
-        nb = self.blocks_per_axis
-        out = torch.empty(nb, nb, nb, device=self.device, dtype=torch.uint8)
-        with torch.cuda.device(self.device):
-            check(lib().nphm_band_block_states(self.res, self.block, self.ws.data_ptr(), self.ws.numel(), out.data_ptr(),
-                                               _stream_ptr(self.device)), 'nphm_band_block_states')
+        """(blocks, blocks, blocks) bool: which blocks are active (a slab: its block layers along x)."""
+        out = torch.empty(self._states_shape(), device=self.device, dtype=torch.uint8)
+        self._call('block_states', self.ws.data_ptr(), self.ws.numel(), out.data_ptr())
         return out != 0
+
+
+class NarrowBandSlab(NarrowBand):
+    """The band of the x-slab of block layers ``[l0, l1)`` of a ``res^3`` grid (``nphm_band_slab_*``, DESIGN §4.16): the same steps
+    as :class:`NarrowBand` on the slab's voxel planes ``[x0, x1]``, with a volume of :attr:`n_planes` planes from :attr:`first_plane`
+    (``x0 - 1``, the ghost plane, when ``l0 > 0``), and :meth:`export` / :meth:`import_` to merge a plane shared with a neighbour."""
+
+    _prefix = 'nphm_band_slab_'
+
+    def __init__(self, res: int, block: int, l0: int, l1: int, device):
+        self.l0, self.l1 = int(l0), int(l1)
+        super().__init__(res, block, device)
+        self.x0 = self.l0 * self.block
+        self.x1 = min(self.l1 * self.block, self.res - 1)
+        self.ghost = self.l0 > 0
+        self.first_plane = self.x0 - int(self.ghost)
+        self.n_planes = self.x1 + 1 - self.first_plane
+        self.plane_bytes = 5 * self.res * self.res          # res^2 float32 values, then res^2 evaluated flags
+
+    def _geometry(self):
+        return self.res, self.block, self.l0, self.l1
+
+    def _states_shape(self):
+        nb = self.blocks_per_axis
+        return self.l1 - self.l0, nb, nb
+
+    def volume(self) -> torch.Tensor:
+        """An uninitialised (n_planes, res, res) float32 slab volume on the band's device."""
+        return torch.empty(self.n_planes, self.res, self.res, device=self.device, dtype=torch.float32)
+
+    def export(self, plane: int, vol: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """uint8 buffer of :attr:`plane_bytes`: the values of global ``plane`` and which of its voxels this slab evaluated."""
+        buf = torch.empty(self.plane_bytes, device=self.device, dtype=torch.uint8) if out is None else out
+        self._call('export', int(plane), vol.data_ptr(), self.ws.data_ptr(), self.ws.numel(), buf.data_ptr())
+        return buf
+
+    def import_(self, plane: int, buf: torch.Tensor, vol: torch.Tensor):
+        """Merge a neighbour's :meth:`export` of the shared ``plane`` (x0 or x1), or copy its filled plane x0 - 1 into the ghost
+        plane."""
+        if buf.device != self.device or buf.dtype != torch.uint8 or buf.numel() != self.plane_bytes:
+            raise ValueError('NarrowBandSlab.import_: need a uint8 buffer of %d bytes on %s' % (self.plane_bytes, self.device))
+        self._call('import', int(plane), buf.data_ptr(), vol.data_ptr(), self.ws.data_ptr(), self.ws.numel())

@@ -1,13 +1,14 @@
 // Narrow-band mesh extraction on sm_90a: the steps that decide WHICH voxels of a res^3 grid the decoder has to evaluate so that
 // marching cubes on the filled volume gives the dense mesh, and that move values between the grid and compact point lists.
-// The decoder itself runs through the existing query entry points on the gathered coordinates (see DESIGN §4.13).
+// The decoder itself runs through the existing query entry points on the gathered coordinates (see DESIGN §4.13, §4.16).
 //
 // The grid's (res - 1)^3 cells are split into blocks of B^3 cells (the last block of an axis may be partial); block b covers the
-// voxels [bB, min(bB + B, res - 1)] of each axis, so neighbouring blocks share a face of voxels.  State lives in a caller-owned
-// workspace:
+// voxels [bB, min(bB + B, res - 1)] of each axis, so neighbouring blocks share a face of voxels.  Every step works on an x-slab:
+// the block layers [L0, L1) and their voxel planes [X0, X1] = [L0 B, min(L1 B, res - 1)]; the whole grid is the slab [0, nb).
+// State lives in a caller-owned workspace, indexed from plane X0:
 //   marks   1 byte per voxel: 0 not evaluated, 1 wanted (set by a marking kernel), 2 listed / evaluated
 //   states  1 byte per block: 0 inactive, 1 activated (its voxels not yet marked), 2 active (marked)
-//   list    u32 flat voxel indices of the last compaction, ascending
+//   list    u32 slab-local flat voxel indices of the last compaction, ascending
 // Marching cubes runs on -sdf at 0, so a voxel is "inside" when -v <= 0, i.e. v >= 0 (NaN: outside) - `side()` below.
 #include "common.cuh"
 #include "simt.cuh"
@@ -27,20 +28,29 @@ enum : unsigned char { kInactive = 0, kActivated = 1, kMarked = 2 };        // b
 
 struct Geo {
     int res, B, C, nb;            // grid points per axis, block edge in cells, cells per axis (res - 1), blocks per axis
-    long long n_vox, n_blocks, n_chunks;
+    int L0, L1, X0, X1;           // block layers [L0, L1) along x and their voxel planes [X0, X1]
+    int ghost;                    // planes the caller's volume holds below X0 (1: a slab's ghost plane X0 - 1)
+    long long rr, n_vox, n_blocks, n_chunks;    // voxels per plane; voxels, blocks and compaction chunks of the slab
 };
 
 struct Layout {
     long long hdr, axes, states, chunk_cnt, chunk_off, marks, list, bytes;
 };
 
-inline Geo make_geo(int res, int block)
+inline int blocks_per_axis(int res, int block) { return (int)ceil_div(res - 1, block); }
+
+// l1 < 0: the whole grid
+inline Geo make_geo(int res, int block, int l0 = 0, int l1 = -1)
 {
     Geo g;
     g.res = res; g.B = block; g.C = res - 1;
-    g.nb = (int)ceil_div(g.C, block);
-    g.n_vox = (long long)res * res * res;
-    g.n_blocks = (long long)g.nb * g.nb * g.nb;
+    g.nb = blocks_per_axis(res, block);
+    g.L0 = l0; g.L1 = l1 < 0 ? g.nb : l1;
+    g.X0 = g.L0 * block; g.X1 = std::min(g.L1 * block, g.C);
+    g.ghost = g.L0 > 0 ? 1 : 0;
+    g.rr = (long long)res * res;
+    g.n_vox = (long long)(g.X1 - g.X0 + 1) * g.rr;
+    g.n_blocks = (long long)(g.L1 - g.L0) * g.nb * g.nb;
     g.n_chunks = ceil_div(g.n_vox, kChunk);
     return g;
 }
@@ -79,9 +89,10 @@ inline Ws carve(void *ws, const Layout &l)
 
 __device__ __forceinline__ bool side(float v) { return v >= 0.f; }
 
+// slab-local flat index of the voxel at global plane x
 __device__ __forceinline__ long long vox(const Geo &g, int x, int y, int z)
 {
-    return ((long long)x * g.res + y) * g.res + z;
+    return ((long long)(x - g.X0) * g.res + y) * g.res + z;
 }
 
 // voxel box of block b along one axis
@@ -93,36 +104,37 @@ __device__ __forceinline__ void unblock(const Geo &g, long long b, int &bx, int 
     bz = (int)(b % g.nb);
     const long long t = b / g.nb;
     by = (int)(t % g.nb);
-    bx = (int)(t / g.nb);
+    bx = g.L0 + (int)(t / g.nb);
 }
 
 // ---------------------------------------------------------------------------------------------- marking
-// eval-mode quirk voxels g = (k + 1) p - 1 and g = res^3 - 1: wanted, and every block owning a cell that touches one is forced
-__global__ void quirk_kernel(const Geo g, long long period, long long n_quirk, unsigned char *__restrict__ marks,
+// eval-mode quirk voxels g = (k + 1) p - 1 and g = res^3 - 1 (k in [k0, k1): those of the slab's planes): wanted, and every block
+// of the slab owning a cell that touches one is forced
+__global__ void quirk_kernel(const Geo g, long long period, long long k0, long long k1, unsigned char *__restrict__ marks,
                              unsigned char *__restrict__ states)
 {
-    const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (k >= n_quirk) return;
-    const long long v = k < g.n_vox / period ? (k + 1) * period - 1 : g.n_vox - 1;
-    const long long rr = (long long)g.res * g.res;
-    const int x = (int)(v / rr), y = (int)((v / g.res) % g.res), z = (int)(v % g.res);
-    marks[v] = kWanted;
-    // cells touching voxel x along an axis: [max(x - 1, 0), min(x, C - 1)]
-    const int bx0 = max(x - 1, 0) / g.B, bx1 = min(x, g.C - 1) / g.B;
+    const long long k = k0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (k >= k1) return;
+    const long long n_all = g.rr * g.res;
+    const long long v = k < n_all / period ? (k + 1) * period - 1 : n_all - 1;
+    const int x = (int)(v / g.rr), y = (int)((v / g.res) % g.res), z = (int)(v % g.res);
+    marks[v - g.X0 * g.rr] = kWanted;
+    // cells touching voxel x along an axis: [max(x - 1, 0), min(x, C - 1)]; along x only the slab's block layers
+    const int bx0 = max(max(x - 1, 0) / g.B, g.L0), bx1 = min(min(x, g.C - 1) / g.B, g.L1 - 1);
     const int by0 = max(y - 1, 0) / g.B, by1 = min(y, g.C - 1) / g.B;
     const int bz0 = max(z - 1, 0) / g.B, bz1 = min(z, g.C - 1) / g.B;
     for (int bx = bx0; bx <= bx1; ++bx)
         for (int by = by0; by <= by1; ++by)
-            for (int bz = bz0; bz <= bz1; ++bz) states[((long long)bx * g.nb + by) * g.nb + bz] = kActivated;
+            for (int bz = bz0; bz <= bz1; ++bz) states[((long long)(bx - g.L0) * g.nb + by) * g.nb + bz] = kActivated;
 }
 
-// block corners (fine indices 0, B, 2B, ..., res - 1 on every axis)
+// block corners (fine indices 0, B, 2B, ..., res - 1 on every axis; along x those of the slab's planes, L0 B ... X1)
 __global__ void corners_kernel(const Geo g, unsigned char *__restrict__ marks)
 {
     const long long n1 = g.nb + 1;
     const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (t >= n1 * n1 * n1) return;
-    const int cz = (int)(t % n1), cy = (int)((t / n1) % n1), cx = (int)(t / (n1 * n1));
+    if (t >= (g.L1 - g.L0 + 1) * n1 * n1) return;
+    const int cz = (int)(t % n1), cy = (int)((t / n1) % n1), cx = g.L0 + (int)(t / (n1 * n1));
     const long long v = vox(g, min(cx * g.B, g.C), min(cy * g.B, g.C), min(cz * g.B, g.C));
     if (marks[v] == kIdle) marks[v] = kWanted;
 }
@@ -194,12 +206,12 @@ __global__ void __launch_bounds__(kThreads) grow_kernel(const Geo g, const float
 }
 
 // every voxel not evaluated takes the value of corner 0 of a block containing it (all such blocks are inactive and on one side)
+// (on a slab the corner lies on the slab's planes too: plane X1 < res - 1 takes corner 0 of block L1, which is on plane X1)
 __global__ void fill_kernel(const Geo g, const unsigned char *__restrict__ marks, float *__restrict__ vol)
 {
-    const long long rr = (long long)g.res * g.res;
     for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < g.n_vox; v += (long long)gridDim.x * blockDim.x) {
         if (marks[v] == kDone) continue;
-        const int x = (int)(v / rr), y = (int)((v / g.res) % g.res), z = (int)(v % g.res);
+        const int x = g.X0 + (int)(v / g.rr), y = (int)((v / g.res) % g.res), z = (int)(v % g.res);
         const int cx = min(x / g.B, g.nb - 1) * g.B, cy = min(y / g.B, g.nb - 1) * g.B, cz = min(z / g.B, g.nb - 1) * g.B;
         vol[v] = vol[vox(g, cx, cy, cz)];
     }
@@ -289,8 +301,8 @@ __global__ void gather_kernel(const Geo g, const unsigned *__restrict__ list, co
 {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (i >= n || i >= (long long)hdr[0]) return;
-    const long long v = list[i], rr = (long long)g.res * g.res;
-    xyz[3 * i] = __ldg(axes + v / rr);
+    const long long v = list[i];
+    xyz[3 * i] = __ldg(axes + g.X0 + v / g.rr);
     xyz[3 * i + 1] = __ldg(axes + g.res + (v / g.res) % g.res);
     xyz[3 * i + 2] = __ldg(axes + 2 * g.res + v % g.res);
 }
@@ -303,6 +315,31 @@ __global__ void scatter_kernel(const unsigned *__restrict__ list, const unsigned
     vol[list[i]] = values[i];
 }
 
+// ---------------------------------------------------------------------------------------------- boundary planes between slabs
+// buffer of plane p: res^2 floats (the volume), then res^2 bytes (1: evaluated)
+__global__ void export_kernel(const Geo g, int plane, const float *__restrict__ vol, const unsigned char *__restrict__ marks,
+                              float *__restrict__ vals, unsigned char *__restrict__ done)
+{
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= g.rr) return;
+    const long long v = (plane - g.X0) * g.rr + i;
+    vals[i] = vol[v];
+    done[i] = marks[v] == kDone ? 1 : 0;
+}
+
+// a voxel the neighbour evaluated and this slab did not takes the neighbour's value and counts as evaluated
+__global__ void import_kernel(const Geo g, int plane, const float *__restrict__ vals, const unsigned char *__restrict__ done,
+                              float *__restrict__ vol, unsigned char *__restrict__ marks)
+{
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= g.rr) return;
+    const long long v = (plane - g.X0) * g.rr + i;
+    if (done[i] && marks[v] != kDone) {
+        marks[v] = kDone;
+        vol[v] = vals[i];
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- host side
 int check_args(int res, int block, const char *who)
 {
@@ -311,16 +348,33 @@ int check_args(int res, int block, const char *who)
     return NPHM_OK;
 }
 
+int check_slab(int res, int block, int l0, int l1, const char *who)
+{
+    int rc = check_args(res, block, who);
+    if (rc) return rc;
+    const int nb = blocks_per_axis(res, block);
+    NPHM_REQUIRE(l0 >= 0 && l0 < l1 && l1 <= nb, "%s: block layers [%d, %d) not a non-empty range of [0, %d)", who, l0, l1, nb);
+    return NPHM_OK;
+}
+
 int check_ws(const Geo &g, const void *ws, long long ws_bytes, const char *who)
 {
     NPHM_REQUIRE(ws, "%s: NULL workspace", who);
     const long long need = layout(g).bytes;
     if (ws_bytes < need) {
-        set_error("%s: band workspace too small: %lld bytes for res %d, block %d, %lld needed", who, ws_bytes, g.res, g.B, need);
+        if (g.L0 == 0 && g.L1 == g.nb)
+            set_error("%s: band workspace too small: %lld bytes for res %d, block %d, %lld needed", who, ws_bytes, g.res, g.B, need);
+        else
+            set_error("%s: band workspace too small: %lld bytes for res %d, block %d, block layers [%d, %d), %lld needed", who,
+                      ws_bytes, g.res, g.B, g.L0, g.L1, need);
         return NPHM_ERR_CAPACITY;
     }
     return NPHM_OK;
 }
+
+// the slab's own planes in a caller volume that starts at plane X0 - ghost
+inline float *own(const Geo &g, float *vol) { return vol + g.ghost * g.rr; }
+inline const float *own(const Geo &g, const float *vol) { return vol + g.ghost * g.rr; }
 
 // wanted voxels -> ascending list (and kDone); counts_host (may be NULL: no read-back) = {listed, active blocks}
 int compact(const Geo &g, const Ws &w, long long *counts_host, cudaStream_t stream)
@@ -349,6 +403,85 @@ int mark_and_compact(const Geo &g, const Ws &w, long long *counts_host, cudaStre
     return compact(g, w, counts_host, stream);
 }
 
+// ---- the steps, on the whole grid or a slab (the entry points below check the arguments)
+int begin(const Geo &g, const Ws &w, long long quirk_period, long long *counts_host, cudaStream_t stream)
+{
+    const Layout l = layout(g);
+    NPHM_CUDA_CHECK(cudaMemsetAsync(w.hdr, 0, 256, stream));
+    NPHM_CUDA_CHECK(cudaMemsetAsync(w.states, 0, g.n_blocks, stream));
+    NPHM_CUDA_CHECK(cudaMemsetAsync(w.marks, 0, l.list - l.marks, stream));
+    if (quirk_period > 0) {
+        // the quirk voxels of global flat indices [X0 res^2, (X1 + 1) res^2): k0 = the first with (k + 1) p - 1 >= X0 res^2; the
+        // last voxel of the grid (k = n_all / p when p does not divide n_all) only on the slab that holds it
+        const long long n_all = g.rr * g.res, g1 = (g.X1 + 1) * g.rr;
+        const long long k0 = g.X0 * g.rr / quirk_period;
+        const long long k1 = g1 == n_all ? ceil_div(n_all, quirk_period) : g1 / quirk_period;
+        if (k1 > k0) {
+            quirk_kernel<<<(unsigned)ceil_div(k1 - k0, kThreads), kThreads, 0, stream>>>(g, quirk_period, k0, k1, w.marks, w.states);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+        }
+    }
+    // compaction only: the forced blocks' other voxels are listed with the first band pass
+    return compact(g, w, counts_host, stream);
+}
+
+int corners(const Geo &g, const Ws &w, long long *counts_host, cudaStream_t stream)
+{
+    const long long n1 = g.nb + 1;
+    corners_kernel<<<(unsigned)ceil_div((g.L1 - g.L0 + 1) * n1 * n1, kThreads), kThreads, 0, stream>>>(g, w.marks);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    // the forced blocks stay activated until classify marks them with the blocks it activates
+    return compact(g, w, counts_host, stream);
+}
+
+int gather(const Geo &g, const Ws &w, const double grid_min[3], const double grid_max[3], long long n, float *xyz_dev,
+           cudaStream_t stream)
+{
+    if (n == 0) return NPHM_OK;
+    int rc = launch_grid_axes(grid_min, grid_max, g.res, w.axes, stream);
+    if (rc) return rc;
+    gather_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, stream>>>(g, w.list, w.hdr, n, w.axes, xyz_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int scatter(const Geo &g, const Ws &w, long long n, const float *values_dev, float *vol_dev, cudaStream_t stream)
+{
+    if (n == 0) return NPHM_OK;
+    scatter_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, stream>>>(w.list, w.hdr, n, values_dev, own(g, vol_dev));
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int classify(const Geo &g, const Ws &w, float tau, const float *vol_dev, long long *counts_host, cudaStream_t stream)
+{
+    classify_kernel<<<(unsigned)ceil_div(g.n_blocks, kThreads), kThreads, 0, stream>>>(g, tau, own(g, vol_dev), w.states);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return mark_and_compact(g, w, counts_host, stream);
+}
+
+int grow(const Geo &g, const Ws &w, const float *vol_dev, long long *counts_host, cudaStream_t stream)
+{
+    grow_kernel<<<(unsigned)ceil_div(g.n_blocks, kWarpsPerCta), kThreads, 0, stream>>>(g, own(g, vol_dev), w.marks, w.states);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return mark_and_compact(g, w, counts_host, stream);
+}
+
+int fill(const Geo &g, const Ws &w, float *vol_dev, cudaStream_t stream)
+{
+    const long long ctas = std::min(ceil_div(g.n_vox, kThreads), 64LL * sm_count());
+    fill_kernel<<<(unsigned)ctas, kThreads, 0, stream>>>(g, w.marks, own(g, vol_dev));
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int block_states(const Geo &g, const void *ws, unsigned char *states_dev, cudaStream_t stream)
+{
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(states_dev, static_cast<const char *>(ws) + layout(g).states, g.n_blocks, cudaMemcpyDeviceToDevice,
+                                    stream));
+    return NPHM_OK;
+}
+
 }  // namespace band
 }  // namespace nphm
 
@@ -359,7 +492,17 @@ using namespace nphm;
     if (rc) return rc;                                                      \
     const band::Geo g = band::make_geo(res, block);                         \
     if ((rc = band::check_ws(g, ws, ws_bytes, who))) return rc;             \
-    const band::Ws w = band::carve(ws, band::layout(g));                    \
+    const band::Ws w = band::carve(const_cast<void *>(static_cast<const void *>(ws)), band::layout(g)); \
+    (void)w;                                                                \
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+
+#define SLAB_PROLOGUE(who)                                                  \
+    int rc = band::check_slab(res, block, l0, l1, who);                    \
+    if (rc) return rc;                                                      \
+    const band::Geo g = band::make_geo(res, block, l0, l1);                 \
+    if ((rc = band::check_ws(g, ws, ws_bytes, who))) return rc;             \
+    const band::Ws w = band::carve(const_cast<void *>(static_cast<const void *>(ws)), band::layout(g)); \
+    (void)w;                                                                \
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
 
 extern "C" long long nphm_band_workspace_bytes(int res, int block)
@@ -373,28 +516,13 @@ extern "C" int nphm_band_begin(int res, int block, long long quirk_period, void 
 {
     BAND_PROLOGUE("nphm_band_begin")
     NPHM_REQUIRE(quirk_period >= 0, "nphm_band_begin: negative quirk period %lld", quirk_period);
-    const band::Layout l = band::layout(g);
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.hdr, 0, 256, stream));
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.states, 0, g.n_blocks, stream));
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.marks, 0, l.list - l.marks, stream));
-    if (quirk_period > 0) {
-        const long long n_quirk = ceil_div(g.n_vox, quirk_period);
-        band::quirk_kernel<<<(unsigned)ceil_div(n_quirk, band::kThreads), band::kThreads, 0, stream>>>(g, quirk_period, n_quirk, w.marks,
-                                                                                                      w.states);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-    }
-    // compaction only: the forced blocks' other voxels are listed with the first band pass
-    return band::compact(g, w, counts_host, stream);
+    return band::begin(g, w, quirk_period, counts_host, stream);
 }
 
 extern "C" int nphm_band_corners(int res, int block, void *ws, long long ws_bytes, long long *counts_host, void *stream_)
 {
     BAND_PROLOGUE("nphm_band_corners")
-    const long long n1 = g.nb + 1;
-    band::corners_kernel<<<(unsigned)ceil_div(n1 * n1 * n1, band::kThreads), band::kThreads, 0, stream>>>(g, w.marks);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    // the forced blocks stay activated until nphm_band_classify marks them with the blocks it activates
-    return band::compact(g, w, counts_host, stream);
+    return band::corners(g, w, counts_host, stream);
 }
 
 extern "C" int nphm_band_gather(int res, int block, const double grid_min[3], const double grid_max[3], long long n, float *xyz_dev,
@@ -402,11 +530,7 @@ extern "C" int nphm_band_gather(int res, int block, const double grid_min[3], co
 {
     BAND_PROLOGUE("nphm_band_gather")
     NPHM_REQUIRE(grid_min && grid_max && n >= 0 && n <= g.n_vox && (n == 0 || xyz_dev), "nphm_band_gather: bad arguments");
-    if (n == 0) return NPHM_OK;
-    if ((rc = launch_grid_axes(grid_min, grid_max, res, w.axes, stream))) return rc;
-    band::gather_kernel<<<(unsigned)ceil_div(n, band::kThreads), band::kThreads, 0, stream>>>(g, w.list, w.hdr, n, w.axes, xyz_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return NPHM_OK;
+    return band::gather(g, w, grid_min, grid_max, n, xyz_dev, stream);
 }
 
 extern "C" int nphm_band_scatter(int res, int block, long long n, const float *values_dev, float *vol_dev, void *ws, long long ws_bytes,
@@ -414,10 +538,7 @@ extern "C" int nphm_band_scatter(int res, int block, long long n, const float *v
 {
     BAND_PROLOGUE("nphm_band_scatter")
     NPHM_REQUIRE(n >= 0 && n <= g.n_vox && vol_dev && (n == 0 || values_dev), "nphm_band_scatter: bad arguments");
-    if (n == 0) return NPHM_OK;
-    band::scatter_kernel<<<(unsigned)ceil_div(n, band::kThreads), band::kThreads, 0, stream>>>(w.list, w.hdr, n, values_dev, vol_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return NPHM_OK;
+    return band::scatter(g, w, n, values_dev, vol_dev, stream);
 }
 
 extern "C" int nphm_band_classify(int res, int block, float tau, const float *vol_dev, void *ws, long long ws_bytes,
@@ -425,9 +546,7 @@ extern "C" int nphm_band_classify(int res, int block, float tau, const float *vo
 {
     BAND_PROLOGUE("nphm_band_classify")
     NPHM_REQUIRE(tau >= 0.f && vol_dev, "nphm_band_classify: need tau >= 0 (got %g) and a volume", (double)tau);
-    band::classify_kernel<<<(unsigned)ceil_div(g.n_blocks, band::kThreads), band::kThreads, 0, stream>>>(g, tau, vol_dev, w.states);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return band::mark_and_compact(g, w, counts_host, stream);
+    return band::classify(g, w, tau, vol_dev, counts_host, stream);
 }
 
 extern "C" int nphm_band_grow(int res, int block, const float *vol_dev, void *ws, long long ws_bytes, long long *counts_host,
@@ -435,30 +554,122 @@ extern "C" int nphm_band_grow(int res, int block, const float *vol_dev, void *ws
 {
     BAND_PROLOGUE("nphm_band_grow")
     NPHM_REQUIRE(vol_dev, "nphm_band_grow: NULL volume");
-    band::grow_kernel<<<(unsigned)ceil_div(g.n_blocks, band::kWarpsPerCta), band::kThreads, 0, stream>>>(g, vol_dev, w.marks, w.states);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return band::mark_and_compact(g, w, counts_host, stream);
+    return band::grow(g, w, vol_dev, counts_host, stream);
 }
 
 extern "C" int nphm_band_fill(int res, int block, float *vol_dev, void *ws, long long ws_bytes, void *stream_)
 {
     BAND_PROLOGUE("nphm_band_fill")
     NPHM_REQUIRE(vol_dev, "nphm_band_fill: NULL volume");
-    const long long ctas = std::min(ceil_div(g.n_vox, band::kThreads), 64LL * sm_count());
-    band::fill_kernel<<<(unsigned)ctas, band::kThreads, 0, stream>>>(g, w.marks, vol_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return NPHM_OK;
+    return band::fill(g, w, vol_dev, stream);
 }
 
 extern "C" int nphm_band_block_states(int res, int block, const void *ws, long long ws_bytes, unsigned char *states_dev, void *stream_)
 {
-    int rc = band::check_args(res, block, "nphm_band_block_states");
-    if (rc) return rc;
-    const band::Geo g = band::make_geo(res, block);
-    if ((rc = band::check_ws(g, ws, ws_bytes, "nphm_band_block_states"))) return rc;
+    BAND_PROLOGUE("nphm_band_block_states")
     NPHM_REQUIRE(states_dev, "nphm_band_block_states: NULL output");
-    const band::Layout l = band::layout(g);
-    NPHM_CUDA_CHECK(cudaMemcpyAsync(states_dev, static_cast<const char *>(ws) + l.states, g.n_blocks, cudaMemcpyDeviceToDevice,
-                                    static_cast<cudaStream_t>(stream_)));
+    return band::block_states(g, ws, states_dev, stream);
+}
+
+// ---------------------------------------------------------------------------------------------- x-slabs of the grid
+extern "C" long long nphm_band_slab_workspace_bytes(int res, int block, int l0, int l1)
+{
+    if (band::check_slab(res, block, l0, l1, "nphm_band_slab_workspace_bytes")) return -1;
+    return band::layout(band::make_geo(res, block, l0, l1)).bytes;
+}
+
+extern "C" int nphm_band_slab_begin(int res, int block, int l0, int l1, long long quirk_period, void *ws, long long ws_bytes,
+                                    long long *counts_host, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_begin")
+    NPHM_REQUIRE(quirk_period >= 0, "nphm_band_slab_begin: negative quirk period %lld", quirk_period);
+    return band::begin(g, w, quirk_period, counts_host, stream);
+}
+
+extern "C" int nphm_band_slab_corners(int res, int block, int l0, int l1, void *ws, long long ws_bytes, long long *counts_host,
+                                      void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_corners")
+    return band::corners(g, w, counts_host, stream);
+}
+
+extern "C" int nphm_band_slab_gather(int res, int block, int l0, int l1, const double grid_min[3], const double grid_max[3],
+                                     long long n, float *xyz_dev, void *ws, long long ws_bytes, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_gather")
+    NPHM_REQUIRE(grid_min && grid_max && n >= 0 && n <= g.n_vox && (n == 0 || xyz_dev), "nphm_band_slab_gather: bad arguments");
+    return band::gather(g, w, grid_min, grid_max, n, xyz_dev, stream);
+}
+
+extern "C" int nphm_band_slab_scatter(int res, int block, int l0, int l1, long long n, const float *values_dev, float *vol_dev,
+                                      void *ws, long long ws_bytes, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_scatter")
+    NPHM_REQUIRE(n >= 0 && n <= g.n_vox && vol_dev && (n == 0 || values_dev), "nphm_band_slab_scatter: bad arguments");
+    return band::scatter(g, w, n, values_dev, vol_dev, stream);
+}
+
+extern "C" int nphm_band_slab_classify(int res, int block, int l0, int l1, float tau, const float *vol_dev, void *ws,
+                                       long long ws_bytes, long long *counts_host, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_classify")
+    NPHM_REQUIRE(tau >= 0.f && vol_dev, "nphm_band_slab_classify: need tau >= 0 (got %g) and a volume", (double)tau);
+    return band::classify(g, w, tau, vol_dev, counts_host, stream);
+}
+
+extern "C" int nphm_band_slab_grow(int res, int block, int l0, int l1, const float *vol_dev, void *ws, long long ws_bytes,
+                                   long long *counts_host, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_grow")
+    NPHM_REQUIRE(vol_dev, "nphm_band_slab_grow: NULL volume");
+    return band::grow(g, w, vol_dev, counts_host, stream);
+}
+
+extern "C" int nphm_band_slab_fill(int res, int block, int l0, int l1, float *vol_dev, void *ws, long long ws_bytes, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_fill")
+    NPHM_REQUIRE(vol_dev, "nphm_band_slab_fill: NULL volume");
+    return band::fill(g, w, vol_dev, stream);
+}
+
+extern "C" int nphm_band_slab_block_states(int res, int block, int l0, int l1, const void *ws, long long ws_bytes,
+                                           unsigned char *states_dev, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_block_states")
+    NPHM_REQUIRE(states_dev, "nphm_band_slab_block_states: NULL output");
+    return band::block_states(g, ws, states_dev, stream);
+}
+
+extern "C" int nphm_band_slab_export(int res, int block, int l0, int l1, int plane, const float *vol_dev, const void *ws,
+                                     long long ws_bytes, unsigned char *buf_dev, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_export")
+    NPHM_REQUIRE(vol_dev && buf_dev, "nphm_band_slab_export: NULL volume or buffer");
+    NPHM_REQUIRE(plane >= g.X0 && plane <= g.X1, "nphm_band_slab_export: plane %d outside the slab's planes [%d, %d]", plane, g.X0,
+                 g.X1);
+    float *vals = reinterpret_cast<float *>(buf_dev);
+    band::export_kernel<<<(unsigned)ceil_div(g.rr, band::kThreads), band::kThreads, 0, stream>>>(
+        g, plane, band::own(g, vol_dev), w.marks, vals, buf_dev + 4 * g.rr);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+extern "C" int nphm_band_slab_import(int res, int block, int l0, int l1, int plane, const unsigned char *buf_dev, float *vol_dev,
+                                     void *ws, long long ws_bytes, void *stream_)
+{
+    SLAB_PROLOGUE("nphm_band_slab_import")
+    NPHM_REQUIRE(vol_dev && buf_dev, "nphm_band_slab_import: NULL volume or buffer");
+    const bool lower = plane == g.X0 && g.L0 > 0, upper = plane == g.X1 && g.X1 < g.C, ghost = plane == g.X0 - 1 && g.ghost;
+    NPHM_REQUIRE(lower || upper || ghost,
+                 "nphm_band_slab_import: plane %d is neither a plane shared with a neighbour nor the ghost plane of the slab of "
+                 "block layers [%d, %d) (planes [%d, %d] of %d)", plane, l0, l1, g.X0, g.X1, g.res);
+    const float *vals = reinterpret_cast<const float *>(buf_dev);
+    if (ghost) {
+        NPHM_CUDA_CHECK(cudaMemcpyAsync(vol_dev, vals, g.rr * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return NPHM_OK;
+    }
+    band::import_kernel<<<(unsigned)ceil_div(g.rr, band::kThreads), band::kThreads, 0, stream>>>(
+        g, plane, vals, buf_dev + 4 * g.rr, band::own(g, vol_dev), w.marks);
+    NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
