@@ -532,3 +532,8 @@ def _dense_sharded(decoder, encoding, mini, maxi, res, nbatch_points, group, dev
     stats = None if mesh is None else {'blocks_active': None, 'blocks_total': None, 'voxels_evaluated': n, 'voxels_total': n,
                                        'growth_rounds': 0, 'margin': None}
     return (mesh, stats) if return_stats else mesh
+
+
+# Data-parallel training steps (DESIGN §6): defined in training_sharded.py, which uses shard_rows above
+from .training_sharded import (LocalTrainGroup, clip_sparse_grad_norm_, shard_trainer, train_step_sharded,  # noqa: E402,F401
+                               val_step_sharded)

@@ -32,6 +32,16 @@ from .EnsembledDeepSDF import sample_point_feature  # same function in the refer
 _SQRT2 = math.sqrt(2.0)
 
 
+def _condition_noise(shape, device, batch_rows=None):
+    """The training-mode condition noise of the ``compress`` mode, ``torch.randn(shape) / 200`` (reference deepSDF.py:220-221).
+    ``batch_rows=(r0, B)``: the ``shape[0]`` queries are rows ``r0 ..`` of a ``B``-row batch; the noise is drawn for all ``B``
+    rows and these rows are kept, so each row gets the noise of a whole-batch call and the generator ends where it would."""
+    if batch_rows is None:
+        return torch.randn(shape, device=device) / 200
+    r0, n_rows = batch_rows
+    return (torch.randn((n_rows,) + tuple(shape[1:]), device=device) / 200)[r0:r0 + shape[0]]
+
+
 @once_differentiable
 def _native_backward(ctx, engine_backward, p0, *upstream):
     """Backward of the native Functions below: ``engine_backward(workspace, *upstream, ...)`` computes what
@@ -313,9 +323,9 @@ class DeformationNetwork(nn.Module):
         self.anchors = anchors
 
     # ------------------------------------------------------------------
-    def _condition(self, xyz, lat_rep, anchors, per_point: bool):
+    def _condition(self, xyz, lat_rep, anchors, per_point: bool, batch_rows=None):
         """Condition vector of the backbone.  ``per_point=False`` returns ``B x 1 x C`` when the
-        mode allows a per-query constant (used by the fused path)."""
+        mode allows a per-query constant (used by the fused path).  ``batch_rows``: see :func:`_condition_noise`."""
         B, N, _ = xyz.shape
         E = self.lat_dim_expr
         if self.mode == 'glob_only':
@@ -337,7 +347,7 @@ class DeformationNetwork(nn.Module):
             if per_point or self.training:
                 compressed = compressed.expand(B, N, compressed.shape[-1])
                 if self.training:
-                    compressed = compressed + torch.randn(compressed.shape, device=compressed.device) / 200
+                    compressed = compressed + _condition_noise(compressed.shape, compressed.device, batch_rows)
                 return torch.cat([compressed, lat_rep[..., -E:].expand(B, N, E)], dim=-1)
             return torch.cat([compressed, lat_rep[:, :1, -E:]], dim=-1)           # B x 1 x 232
         if self.mode == 'GNN':
@@ -370,11 +380,13 @@ class DeformationNetwork(nn.Module):
         return (self.mode in ('compress', 'expr_only', 'glob_only') and self.defDeepSDF.native_grad_supported(xyz)
                 and (lat_rep.dim() == 2 or lat_rep.shape[1] == 1 or lat_rep.stride(1) == 0))
 
-    def forward_native_grad(self, xyz, lat_rep, anchors):
+    def forward_native_grad(self, xyz, lat_rep, anchors, batch_rows=None):
         """:meth:`forward` on the native training kernels, differentiable to first order.  ``lat_rep``: B x 1 x D (or B x D,
         or B x N x D equal over the points; see :meth:`DeepSDF.forward_native_grad` for its gradient).  In ``compress`` mode
         ``compressor([z_id | anchors])`` stays in autograd, and in train mode the noise is drawn by the reference's own call
-        (``torch.randn(B, N, 32) / 200``, deepSDF.py:220-221), so a seeded run sees the same noise as :meth:`forward`."""
+        (``torch.randn(B, N, 32) / 200``, deepSDF.py:220-221), so a seeded run sees the same noise as :meth:`forward`.
+        ``batch_rows=(r0, n)``: the B queries are rows r0 .. r0 + B of an n-row batch, whose noise is drawn whole
+        (:func:`_condition_noise`; a data-parallel step evaluates a slice of the batch this way)."""
         if xyz.dim() < 3:
             xyz = xyz.unsqueeze(0)
         if self.mode not in ('compress', 'expr_only', 'glob_only'):
@@ -389,7 +401,7 @@ class DeformationNetwork(nn.Module):
             a0 = anchors[:, 0] if anchors.dim() == 4 else anchors
             compressed = self.compressor(torch.cat([lat[:, :-E], a0.reshape(B, -1)], dim=-1))          # B x 32
             if self.training:
-                noise = torch.randn((B, N, compressed.shape[-1]), device=compressed.device) / 200
+                noise = _condition_noise((B, N, compressed.shape[-1]), compressed.device, batch_rows)
             cond = torch.cat([compressed, lat[:, -E:]], dim=-1)
         elif self.mode == 'glob_only':
             cond = torch.cat([lat[:, :self.lat_dim_glob_shape], lat[:, -E:]], dim=-1)
@@ -401,9 +413,11 @@ class DeformationNetwork(nn.Module):
     def forward(self,
                 xyz: torch.Tensor,
                 lat_rep: torch.Tensor,
-                anchors: Optional[torch.Tensor]) -> (torch.Tensor, torch.Tensor):
+                anchors: Optional[torch.Tensor],
+                batch_rows=None) -> (torch.Tensor, torch.Tensor):
         """xyz: B x N x 3; lat_rep: B x N|1 x (lat_id + lat_expr) = ``[z_id | z_ex]``;
-        anchors: B x N x K x 3 or B x K x 3.  Returns ``(offsets B x N x 3, last channel B x N x 1)``."""
+        anchors: B x N x K x 3 or B x K x 3.  Returns ``(offsets B x N x 3, last channel B x N x 1)``.
+        ``batch_rows``: as in :meth:`forward_native_grad`."""
         if xyz.dim() < 3:
             xyz = xyz.unsqueeze(0)
         backbone = self.defDeepSDF
@@ -416,6 +430,6 @@ class DeformationNetwork(nn.Module):
                 cond = self._condition(xyz, lat.unsqueeze(1), anchors, per_point=False)   # B x 1 x C
                 pred = backbone.engine().query(xyz, cond[:, 0])
                 return pred[..., :3], pred[..., -1:]
-        cond = self._condition(xyz, lat_rep, anchors, per_point=True)
+        cond = self._condition(xyz, lat_rep, anchors, per_point=True, batch_rows=batch_rows)
         pred = backbone._forward_composite(xyz, cond)
         return pred[..., :3], pred[..., -1:]

@@ -41,7 +41,7 @@ from __future__ import annotations
 import torch
 
 from .EnsembledDeepSDF import FastEnsembleDeepSDFMirrored
-from .deepSDF import DeepSDF
+from .deepSDF import DeepSDF, DeformationNetwork
 from .diff_operators import gradient
 
 _POINT_SETS = ('points_face', 'points_non_face', 'sup_grad_near', 'sup_grad_far')
@@ -170,13 +170,35 @@ def _corresp_native_ok(decoder, points, glob_cond) -> bool:
             and glob_cond.dim() == 3 and glob_cond.shape[1] == 1 and decoder.native_grad_supported(points, glob_cond))
 
 
+def corresp_forward_draws(decoder, n_rows, n_points, device, dtype):
+    """The random draws of :func:`compute_loss_corresp_forward` on a batch of ``n_rows`` x ``n_points`` points, in its order,
+    without evaluating anything: a rank of a data-parallel step that holds no rows keeps its generators in step this way."""
+    noisy = isinstance(decoder, DeformationNetwork) and decoder.mode == 'compress' and decoder.training
+    width = decoder.compressor[0].out_features if noisy else 0
+    if noisy:
+        torch.randn((n_rows, n_points, width), device=device)
+    torch.rand(n_rows, 100, 3, device=device, dtype=dtype)
+    if noisy:
+        torch.randn((n_rows, 100, width), device=device)
+
+
 def compute_loss_corresp_forward(batch, decoder, decoder_shape, latent_codes, latent_codes_shape, device, epoch=-1,
-                                 exp_path=None, native=None):
+                                 exp_path=None, native=None, rows=None):
     """Stage-2 loss of the reference (same arguments, same random draws in the same order, same returned dict:
     ``corresp``, ``lat_reg``, ``loss_reg_zero``).  ``native``: None = the native first-order decoder path when it supports
-    the call, False = the composite path, True = the native path (raises if unsupported)."""
+    the call, False = the composite path, True = the native path (raises if unsupported).
+
+    ``rows=(r0, r1)``: the losses of batch rows [r0, r1) only, each a mean over those rows.  Every random draw is made for the
+    whole batch and these rows are kept, so the rows see the draws of a whole-batch call and the generators end in its state
+    (the data-parallel step, :mod:`nphm_b200.training_sharded`)."""
     if 'path' in batch:
         del batch['path']
+    batch_rows = None
+    if rows is not None:
+        r0, r1 = rows
+        batch_rows = (r0, batch['idx'].shape[0])
+        batch = {k: v[r0:r1] for k, v in batch.items()}
+    noise_rows = {} if batch_rows is None or not isinstance(decoder, DeformationNetwork) else {'batch_rows': batch_rows}
     batch_cuda = {k: v.to(device).float() for (k, v) in zip(batch.keys(), batch.values())}
     glob_cond_shape = latent_codes_shape(batch['subj_ind'].to(device))
     glob_cond_pose = latent_codes(batch['idx'].to(device))
@@ -198,10 +220,10 @@ def compute_loss_corresp_forward(batch, decoder, decoder_shape, latent_codes, la
 
     if native:
         # B x 1 x D condition: its gradient is the sum over the points, which is what the reference's repeat() passes on
-        decoder_call = lambda x, n: decoder.forward_native_grad(x, glob_cond, gt_anchors)     # noqa: E731
+        decoder_call = lambda x, n: decoder.forward_native_grad(x, glob_cond, gt_anchors, **noise_rows)     # noqa: E731
     else:
         cond = glob_cond.repeat(1, points_neutral.shape[1], 1)
-        decoder_call = lambda x, n: decoder(x, cond[:, :n, :], gt_anchors)                    # noqa: E731
+        decoder_call = lambda x, n: decoder(x, cond[:, :n, :], gt_anchors, **noise_rows)                    # noqa: E731
 
     delta, _ = decoder_call(points_neutral, points_neutral.shape[1])
     pred_posed = points_neutral + delta.squeeze()
@@ -211,7 +233,11 @@ def compute_loss_corresp_forward(batch, decoder, decoder_shape, latent_codes, la
     lat_mag = torch.norm(glob_cond_pose, dim=-1) ** 2
 
     # enforce deformation field to be zero elsewhere
-    samps = (torch.rand(glob_cond.shape[0], 100, 3, device=glob_cond.device, dtype=glob_cond.dtype) - 0.5) * 2.5
+    if batch_rows is None:
+        samps = (torch.rand(glob_cond.shape[0], 100, 3, device=glob_cond.device, dtype=glob_cond.dtype) - 0.5) * 2.5
+    else:
+        whole = torch.rand(batch_rows[1], 100, 3, device=glob_cond.device, dtype=glob_cond.dtype)
+        samps = (whole[batch_rows[0]:batch_rows[0] + glob_cond.shape[0]] - 0.5) * 2.5
     delta, _ = decoder_call(samps, 100)
     loss_reg_zero = (delta ** 2).mean()
 
