@@ -537,3 +537,6 @@ def _dense_sharded(decoder, encoding, mini, maxi, res, nbatch_points, group, dev
 # Data-parallel training steps (DESIGN §6): defined in training_sharded.py, which uses shard_rows above
 from .training_sharded import (LocalTrainGroup, clip_sparse_grad_norm_, shard_trainer, train_step_sharded,  # noqa: E402,F401
                                val_step_sharded)
+# Many scans fitted over the ranks (DESIGN §6): defined in fitting_sharded.py
+from .fitting_sharded import (FitPlan, fit_owner, inference_identity_space_batched_sharded,  # noqa: E402,F401
+                              inference_iterative_root_finding_joint_batched_sharded, plan_fit_chunks)

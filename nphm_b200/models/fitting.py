@@ -751,13 +751,26 @@ def inference_identity_space_batched(decoder,
     single-scan function scan by scan."""
     if not scans:
         return []
+    fit = _identity_batch_fit(decoder, scans, n_steps, schedule_cfg, step_scale, lr_scale)
+    if fit is None:
+        return _sequential(lambda obs, lam: inference_identity_space(decoder, obs, lam, n_steps, schedule_cfg, step_scale,
+                                                                     lr_scale), scans, lambdas)
+    return fit(scans, _sampling_plan(scans, int(n_steps * step_scale)), lambdas)
+
+
+def _identity_batch_fit(decoder, scans, n_steps, schedule_cfg, step_scale, lr_scale):
+    """``fit(scans, gens, lambdas)``: the scan-batched identity fit with scan k drawing from ``gens[k]``, when a batched
+    fitter takes this decoder on the scans' device; None when the scans are fitted one by one."""
     device = _scans_device(scans)
     npm = device is not None and device.type == 'cuda' and _native_npm_decoder(decoder, 1)
     if not npm and (device is None or device.type != 'cuda' or not (_fused_identity(decoder) and _tc_ensemble(decoder))):
-        return _sequential(lambda obs, lam: inference_identity_space(decoder, obs, lam, n_steps, schedule_cfg, step_scale,
-                                                                     lr_scale), scans, lambdas)
+        return None
+    return lambda chunk, gens, lambdas: _fit_identity_batch(decoder, chunk, gens, lambdas, n_steps, schedule_cfg, step_scale,
+                                                            lr_scale, device, npm)
+
+
+def _fit_identity_batch(decoder, scans, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale, device, npm):
     n_iters = int(n_steps * step_scale)
-    gens = _sampling_plan(scans, n_iters)
     lr = 0.01 * lr_scale
     if npm:
         fitter = BatchedNpmIdentityFitter(decoder, len(scans), device)
@@ -1041,6 +1054,17 @@ def inference_iterative_root_finding_joint_batched(decoder,
     must fit on the device at once (nothing is split into smaller batches)."""
     if not subjects:
         return []
+    fit = _joint_batch_fit(decoder, decoder_expr, subjects, n_steps, schedule_cfg, step_scale, lr_scale)
+    if fit is None:
+        return _sequential(lambda obs, lam: inference_iterative_root_finding_joint(decoder, decoder_expr, obs, lam, n_steps,
+                                                                                   schedule_cfg, step_scale, lr_scale),
+                           subjects, lambdas)
+    return fit(subjects, _sampling_plan(subjects, int(n_steps * step_scale)), lambdas)
+
+
+def _joint_batch_fit(decoder, decoder_expr, subjects, n_steps, schedule_cfg, step_scale, lr_scale):
+    """``fit(subjects, gens, lambdas)``: the subject-batched joint fit with subject k drawing from ``gens[k]``, when a batched
+    fitter takes these decoders on the subjects' device; None when the subjects are fitted one by one."""
     device = _scans_device(subjects)
     batched = None
     if device is not None and not os.environ.get('NPHM_JOINT_AUTOGRAD'):
@@ -1049,11 +1073,14 @@ def inference_iterative_root_finding_joint_batched(decoder,
         elif _native_joint(decoder, decoder_expr, device) and _tc_ensemble(decoder):
             batched = BatchedJointFitter
     if batched is None:
-        return _sequential(lambda obs, lam: inference_iterative_root_finding_joint(decoder, decoder_expr, obs, lam, n_steps,
-                                                                                   schedule_cfg, step_scale, lr_scale),
-                           subjects, lambdas)
+        return None
+    return lambda chunk, gens, lambdas: _fit_joint_batch(batched, decoder, decoder_expr, chunk, gens, lambdas, n_steps,
+                                                         schedule_cfg, step_scale, lr_scale, device)
+
+
+def _fit_joint_batch(batched, decoder, decoder_expr, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale,
+                     device):
     n_iters = int(n_steps * step_scale)
-    gens = _sampling_plan(subjects, n_iters)
     fitter = batched(decoder, decoder_expr, [len(s) for s in subjects], device)
     lr = 0.01 * lr_scale
     for j in range(n_iters):
