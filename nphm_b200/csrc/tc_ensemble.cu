@@ -129,6 +129,76 @@ __global__ void l2_slab_kernel(const uint8_t *__restrict__ weights, const float 
     }
 }
 
+// B >= |s_k| over the box of a grid query, per (query, member), as the ensemble kernel computes s_k: float64 interval
+// propagation (centre / radius) through layer 0 with the latent folded, the softplus (beta = 100) layers 1-3 with the
+// latent-dependent constants and the skip input of layer 2, and the output layer.  Every pre-activation interval grows by
+// kBoundRel * (|W| |h| + |b|) + kBoundAbs, which covers the kernel's 3-pass fp16 products, fp32 sums and approximate
+// softplus with a wide margin.  At least 1 (quirk points blend 1.0); +inf when the bound is not finite.
+constexpr double kBoundRel = 0x1p-10, kBoundAbs = 0x1p-10;
+__device__ __forceinline__ double softplus64(double x) { return fmax(x, 0.0) + log1p(exp(-100.0 * fabs(x))) / 100.0; }
+__global__ void __launch_bounds__(256) member_bound_kernel(const float *__restrict__ W0, const float *__restrict__ W1,
+                                                           const float *__restrict__ W2, const float *__restrict__ W3,
+                                                           const float *__restrict__ W4, const float *__restrict__ cvec,
+                                                           int cvec_stride, const int *__restrict__ coff,
+                                                           const float *__restrict__ anchors, const float *__restrict__ axes,
+                                                           int res, int n_members, int n_symm, float *__restrict__ bounds)
+{
+    const int m = blockIdx.x, qi = blockIdx.y, set = member_set(m, n_symm);
+    const float *cv = cvec + ((size_t)qi * n_members + m) * cvec_stride;
+    __shared__ double hc[kH + 3], hr[kH + 3], oc[kH], orad[kH], xc[3], xr[3];
+    if (threadIdx.x < 3) {
+        const int d = threadIdx.x;
+        float lo = axes[d * res], hi = lo;
+        for (int i = 1; i < res; ++i) { lo = fminf(lo, axes[d * res + i]); hi = fmaxf(hi, axes[d * res + i]); }
+        const double a = m < n_members - 1 ? (double)anchors[((size_t)qi * (n_members - 1) + m) * 3 + d] : 0.0;
+        double l = lo - a, h = hi - a;
+        if (d == 0 && (m & 1) && m < 2 * n_symm) { const double t = l; l = -h; h = -t; }    // mirrored member
+        xc[d] = 0.5 * (l + h);
+        xr[d] = 0.5 * (h - l);
+    }
+    __syncthreads();
+    // one layer: outputs n < N from inputs k < K (row stride ld, scale sc) plus the constant cv[coff[l] + n]
+    auto layer = [&](const float *W, int N, int K, int ld, double sc, int l, bool act) {
+        for (int n = threadIdx.x; n < N; n += blockDim.x) {
+            const double b = cv[coff[l] + n];
+            double c = b, r = 0.0, mag = fabs(b);
+            for (int k = 0; k < K; ++k) {
+                const double w = sc * (double)W[(size_t)n * ld + k];
+                c += w * hc[k];
+                r += fabs(w) * hr[k];
+                mag += fabs(w) * (fabs(hc[k]) + hr[k]);
+            }
+            r += kBoundRel * mag + kBoundAbs;
+            if (act) {
+                const double lo = softplus64(c - r), hi = softplus64(c + r);
+                oc[n] = 0.5 * (lo + hi);
+                orad[n] = 0.5 * (hi - lo);
+            } else {
+                oc[n] = c;
+                orad[n] = r;
+            }
+        }
+        __syncthreads();
+        for (int n = threadIdx.x; n < N; n += blockDim.x) { hc[n] = oc[n]; hr[n] = orad[n]; }
+        __syncthreads();
+    };
+    const int d_in = 3 + kCond;
+    for (int k = threadIdx.x; k < 3; k += blockDim.x) { hc[k] = xc[k]; hr[k] = xr[k]; }
+    __syncthreads();
+    layer(W0 + (size_t)set * kH * d_in, kH, 3, d_in, 1.0, 0, true);
+    layer(W1 + (size_t)set * kN1 * kH, kN1, kH, kH, 1.0, 1, true);
+    // layer 2: [h1 | local xyz] / sqrt(2), the latent part folded into its constant
+    for (int k = threadIdx.x; k < 3; k += blockDim.x) { hc[kN1 + k] = xc[k]; hr[kN1 + k] = xr[k]; }
+    __syncthreads();
+    layer(W2 + (size_t)set * kH * kH, kH, kN1 + 3, kH, 0.70710678118654752440, 2, true);
+    layer(W3 + (size_t)set * kH * kH, kH, kH, kH, 1.0, 3, true);
+    layer(W4 + (size_t)set * kH, 1, kH, kH, 1.0, 4, false);
+    if (threadIdx.x == 0) {
+        const double B = fmax(fabs(hc[0]) + hr[0], 1.0);
+        bounds[(size_t)qi * n_members + m] = isfinite(B) ? __double2float_ru(B) : INFINITY;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ MMA self test
 // One warpgroup: D[64 x n] = A[64 x 16*ks] * B[n x 16*ks]^T with the operand plumbing of the ensemble kernel (fp16 hi/lo split,
 // A in registers, B slabs in shared memory, 16-column wgmmas).  Rows 64 .. 127 of a 128-row test run in a second CTA.
@@ -277,6 +347,22 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
         if ((rc = h->tc_masks.reserve((size_t)n_tiles * sizeof(unsigned long long)))) return rc;
         p.tile_masks = h->tc_masks.as<unsigned long long>();
         h->tc_mask_tiles = n_tiles;
+    }
+    // dense grid queries also skip the members whose blend terms fp32 rounding absorbs (bit-identical result);
+    // NPHM_ENS_ABSORB=0 turns it off (the same outputs, every non-zero member evaluated)
+    const char *absorb_env = std::getenv("NPHM_ENS_ABSORB");
+    p.absorb = p.zero_skip && !q.xyz && q.n_points > 0 && !(absorb_env && absorb_env[0] == '0');
+    if (p.absorb) {
+        if ((rc = h->tc_absorb.reserve((size_t)n_tiles * (sizeof(unsigned long long) + tc::kMaxMembers)))) return rc;
+        p.absorb_masks = h->tc_absorb.as<unsigned long long>();
+        p.wexp = reinterpret_cast<uint8_t *>(p.absorb_masks + n_tiles);
+        if ((rc = h->tc_bounds.reserve((size_t)q.n_queries * h->n_members * sizeof(float)))) return rc;
+        tc::member_bound_kernel<<<grid, 256, 0, stream>>>(
+            h->weights.W[0].as<float>(), h->weights.W[1].as<float>(), h->weights.W[2].as<float>(), h->weights.W[3].as<float>(),
+            h->weights.W[4].as<float>(), q.cvec, h->dims.cvec_stride, h->tc_coff.as<int>(), q.anchors, q.axes, q.res,
+            h->n_members, h->cfg.n_symm_pairs, h->tc_bounds.as<float>());
+        NPHM_CUDA_CHECK(cudaGetLastError());
+        p.bounds = h->tc_bounds.as<float>();
     }
     // the kernel leaves the counter at zero when it ends; it starts at zero when allocated
     if (!h->tc_sched.ptr) {

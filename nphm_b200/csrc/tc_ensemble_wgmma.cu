@@ -19,11 +19,13 @@
 // warpgroup's epilogue (and its next member's layer 0) runs while the other one's MMAs occupy the tensor cores.  The
 // accumulation order of every output is that of a single warpgroup running alone: the results do not depend on the offset.
 // Tiles are handed out on demand: the producer lane takes the next work item from a device counter, reads the item's member
-// mask and passes (item, mask) to the consumers through a two-deep queue in shared memory, so that no SM idles while others
+// mask and passes the item to the consumers through a two-deep queue in shared memory, so that no SM idles while others
 // still have tiles, and the producer streams the next tile's weights while the consumers finish the current one.  A mask
 // pre-pass (tile_mask_kernel) computes which members each tile needs (dense: a blend weight that is not exactly zero at
 // some valid point; pruned: the tau rule) and the producer streams only those; grid queries use compact tiles
-// (Params::tbx, tby, tbz) so that a tile lies far from many anchors.
+// (Params::tbx, tby, tbz) so that a tile lies far from many anchors.  Dense grid queries also skip the members whose blend
+// terms fp32 rounding absorbs (the producer decides, see there); the producer tells the consumers which member each record
+// slot holds and ends a tile with a record slot without a copy.
 #include "tc_ensemble.cuh"
 
 namespace nphm {
@@ -71,10 +73,15 @@ struct __align__(128) Smem {
     float rec[kRecSlots][kRecFloats];
     uint64_t w_full[kSlots], w_empty[kSlots];
     uint64_t rec_full[kRecSlots], rec_empty[kRecSlots];
-    // tile queue (producer -> consumers): work item (-1 = no more work) and member mask of the next two tiles
+    // tile queue (producer -> consumers): work item of the next two tiles (-1 = no more work)
     uint64_t q_full[2], q_empty[2];
     long long q_item[2];
-    unsigned long long q_mask[2];
+    // producer -> consumers: the member whose record a record slot holds, -1 = the tile has no more members
+    int rec_member[kRecSlots];
+    // consumers -> producer (absorption): per consumer warp, min |num| over its valid points after the member of record
+    // position r (in pub_min[r % 4]), then pub_seq = r + 1
+    float pub_min[4][kConsumerWarps];
+    unsigned int pub_seq[kConsumerWarps];
 };
 static_assert(sizeof(Smem) <= 227 * 1024, "shared memory of the ensemble kernel exceeds the 227 KB of an H100 block");
 
@@ -110,6 +117,9 @@ __device__ __forceinline__ void to_operand(const float (&d)[N], int j, int col0,
     split2(v[1][2], v[1][3], ah[3], al[3]);
 }
 
+__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t *a) { return *reinterpret_cast<const volatile uint32_t *>(a); }
+__device__ __forceinline__ float ld_volatile_f32(const float *a) { return *reinterpret_cast<const volatile float *>(a); }
+
 // Mask pre-pass: one warp per tile, 4 rows per lane; bit k of p.tile_masks[tile] is set when the tile needs member k.  The
 // last, global member is always needed: every tile evaluates >= 1 member.  Dense rule: a member is needed if w_k != 0 at some
 // valid point - a member with w_k = +0 everywhere adds exactly nothing to num and den (denormal weights count as nonzero).
@@ -132,18 +142,36 @@ __global__ void __launch_bounds__(32 * kMaskWarps) tile_mask_kernel(const Params
         pt[i] = tile_point(p, p.blocked, tile, qi, tiles_per_query, lane + 32 * i);
         thr[i] = PRUNE ? p.prune_tau * (weight_sum(anc, p.n_members, pt[i].x, pt[i].y, pt[i].z) + 1e-6f) : 0.f;
     }
-    unsigned long long mask = 1ull << (p.n_members - 1);
-    for (int k = 0; k < p.n_members - 1; ++k) {
-        bool need = false;
+    unsigned long long mask = 1ull << (p.n_members - 1), absorbed = 0;
+    // absorption (dense rule): the in-order partial sums den of the kernel's blend.  A member the kernel skips leaves den as
+    // it was, so these are the sums the kernel sees whichever members it skips.
+    const bool absorb = !PRUNE && p.absorb;
+    float den[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int k = 0; k < p.n_members; ++k) {
+        bool need = false, kept = false;
+        uint32_t wmax = 0;                       // bits of the largest valid weight (non-negative floats order as integers)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             if (!pt[i].valid) continue;
             const float w = member_weight(anc, k, p.n_members, pt[i].x, pt[i].y, pt[i].z);
             need |= PRUNE ? w >= thr[i] : w != 0.f;
+            if (absorb) {
+                kept |= den[i] + w != den[i];
+                den[i] += w;
+                wmax = max(wmax, __float_as_uint(w));
+            }
         }
-        if (__any_sync(0xffffffffu, need)) mask |= 1ull << k;
+        if (k < p.n_members - 1 && __any_sync(0xffffffffu, need)) mask |= 1ull << k;
+        if (absorb) {
+            if (!__any_sync(0xffffffffu, kept)) absorbed |= 1ull << k;
+            wmax = __reduce_max_sync(0xffffffffu, wmax);
+            if (lane == 0) p.wexp[tile * kMaxMembers + k] = wmax ? (uint8_t)((wmax >> 23) + 1) : 0;
+        }
     }
-    if (lane == 0) p.tile_masks[tile] = mask;
+    if (lane == 0) {
+        p.tile_masks[tile] = mask;
+        if (absorb) p.absorb_masks[tile] = absorbed & mask;
+    }
 }
 
 template <bool PRUNE, bool ACTS>
@@ -170,6 +198,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
         for (int i = 0; i < kSlots; ++i) { mbar_init(&sm.w_full[i], 1); mbar_init(&sm.w_empty[i], kConsumerWarps); }
         for (int i = 0; i < kRecSlots; ++i) { mbar_init(&sm.rec_full[i], 1); mbar_init(&sm.rec_empty[i], kConsumerWarps); }
         for (int i = 0; i < 2; ++i) { mbar_init(&sm.q_full[i], 1); mbar_init(&sm.q_empty[i], kConsumerWarps); }
+        for (int i = 0; i < kConsumerWarps; ++i) sm.pub_seq[i] = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -179,6 +208,8 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
 #endif
     // tile masks from the pre-pass: the pruned rule, or (dense variant) exactly zero blend weights
     const bool premask = PRUNE || (!ACTS && p.zero_skip);
+    // members absorbed by fp32 rounding (dense variant with the zero-weight masks only)
+    const bool absorb = !PRUNE && !ACTS && p.zero_skip && p.absorb;
 
     if (warp >= kConsumerWarps) {
         // =========================================================================== producer (tiles, bulk async copies)
@@ -196,13 +227,36 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 const int qs = tcount & 1;
                 mbar_wait(&sm.q_empty[qs], ((tcount >> 1) & 1) ^ 1);
                 sm.q_item[qs] = more ? (long long)item : -1;
-                sm.q_mask[qs] = mask;
                 mbar_arrive(&sm.q_full[qs]);
                 if (!more) break;
+                // absorption: skip member m when den + w == den at every valid point (pre-pass) and w * |s| < ulp(|num|) / 4
+                // there, so that fmaf(w, s, num) returns num: max w <= wb (pre-pass), |s| <= B (member_bound_kernel) and
+                // |num| >= L = min |num| after the member two record positions back (published by the consumer warps before
+                // they retire that member's successor's layer 2, i.e. before this lane could issue the previous member's
+                // last unit) - wb * B of the member in between, rounded down.  Deterministic: the lane waits for that state.
+                const unsigned long long amask = absorb ? p.absorb_masks[tile] : 0ull;
+                const uint32_t rc0 = rcount;
+                float last_bound = 0.f;                  // wb * B of the member at record position rcount - 1, rounded up
                 for (; mask; mask &= mask - 1) {         // the tile's members in ascending order
                     const int m = __ffsll((long long)mask) - 1;
+                    const float bound = absorb ? __fmul_ru(weight_bound(p.wexp[(size_t)tile * kMaxMembers + m]),
+                                                           p.bounds[(size_t)qi * p.n_members + m]) : 0.f;
+                    if (((amask >> m) & 1) && rcount >= rc0 + 2) {
+                        const int ps = (rcount - 2) & 3;
+                        float mn = INFINITY;
+                        for (int w = 0; w < kConsumerWarps; ++w) {
+                            while (ld_volatile_u32(&sm.pub_seq[w]) < rcount - 1) { }
+                            __threadfence_block();
+                            mn = fminf(mn, ld_volatile_f32(&sm.pub_min[ps][w]));
+                        }
+                        const float L = __fsub_rd(mn, last_bound);
+                        // ulp(L) / 4 = 2^(e(L) - 25), exact for L >= 2^-100; NaN and smaller L never certify
+                        if (L >= 0x1p-100f && bound < __uint_as_float(((__float_as_uint(L) >> 23) - 25) << 23)) continue;
+                    }
+                    last_bound = bound;
                     const int rslot = rcount % kRecSlots;
                     mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
+                    sm.rec_member[rslot] = m;
                     mbar_expect_tx(&sm.rec_full[rslot], kRecFloats * 4);
                     bulk_g2s(sm.rec[rslot], p.recs + ((size_t)qi * p.n_members + m) * kRecFloats, kRecFloats * 4, &sm.rec_full[rslot]);
                     ++rcount;
@@ -228,6 +282,12 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                         }
                     }
                 }
+                // the end of the tile's members: a record slot without a copy
+                const int rslot = rcount % kRecSlots;
+                mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
+                sm.rec_member[rslot] = -1;
+                mbar_arrive(&sm.rec_full[rslot]);
+                ++rcount;
             }
             // every CTA has taken its last item once all have counted themselves finished: the last one resets the counter
             // for the next launch on the stream
@@ -246,7 +306,10 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     int rl[2];                                   // tile rows (points) of this thread's accumulator rows
     rl[0] = 64 * wgi + 16 * (warp & 3) + (lane >> 2);
     rl[1] = rl[0] + 8;
-    uint32_t rcount = 0;
+    uint32_t rcount = 0;                         // record positions: the members evaluated and one end marker per tile
+#ifdef NPHM_ENS_TRACE
+    uint32_t n_eval = 0;                         // member-tiles evaluated
+#endif
     auto release = [&](int u) { __syncwarp(); if (lane == 0) mbar_arrive(&sm.w_empty[u & 3]); };
     auto release_rec = [&](uint64_t *bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
     auto wait_unit = [&](int u) { mbar_wait(&sm.w_full[u & 3], (u >> 2) & 1); };
@@ -269,7 +332,6 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
         const int qs = tcount & 1;
         mbar_wait(&sm.q_full[qs], (tcount >> 1) & 1);
         const long long item = sm.q_item[qs];
-        const unsigned long long mask = sm.q_mask[qs];
         __syncwarp();
         if (lane == 0) mbar_arrive(&sm.q_empty[qs]);
         if (item < 0) break;
@@ -291,11 +353,20 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
         }
         const uint32_t tile_rc0 = rcount;        // the tile's first member (timeline build)
 
-        for (int m = 0; m < p.n_members; ++m) {
-            if (!((mask >> m) & 1)) continue;
+        for (;;) {
+            // the tile's next member, as the producer hands it out (-1: no more)
             const uint32_t rslot = rcount % kRecSlots;
             ENS_CMARK(rcount, 24);
             mbar_wait(&sm.rec_full[rslot], (rcount / kRecSlots) & 1);
+            const int m = sm.rec_member[rslot];
+            if (m < 0) {
+                release_rec(&sm.rec_empty[rslot]);
+                ++rcount;
+                break;
+            }
+#ifdef NPHM_ENS_TRACE
+            ++n_eval;
+#endif
             const float *rec = sm.rec[rslot];
             float cx[2], cy[2], cz[2];
 #pragma unroll
@@ -531,6 +602,17 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 num[r] = fmaf(w, quirk[r] ? 1.0f : s, num[r]);
                 if (!PRUNE) den[r] += w;
             }
+            if (absorb) {
+                // publish min |num| over the warp's valid points for the producer's absorption decisions
+                float mn = fminf(valid[0] ? fabsf(num[0]) : INFINITY, valid[1] ? fabsf(num[1]) : INFINITY);
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+                if (lane == 0) {
+                    *reinterpret_cast<volatile float *>(&sm.pub_min[rcount & 3][warp]) = mn;
+                    __threadfence_block();
+                    *reinterpret_cast<volatile unsigned int *>(&sm.pub_seq[warp]) = rcount + 1;
+                }
+            }
             release_rec(&sm.rec_empty[rslot]);
             ++rcount;
         }
@@ -541,7 +623,7 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     if (wgi == 0) take_turn();                   // the turn warpgroup 1 passed after its last phase
 #ifdef NPHM_ENS_TRACE
     if (threadIdx.x == 0 && blockIdx.x < kTraceMaxCtas) {
-        g_ens_ctas[1 + 2 * blockIdx.x] = rcount;
+        g_ens_ctas[1 + 2 * blockIdx.x] = n_eval;
         g_ens_ctas[2 + 2 * blockIdx.x] = clock64() - cta_start;
     }
 #endif

@@ -1,0 +1,230 @@
+#!/usr/bin/env python
+"""How many member-tiles of a dense grid query an fp32 absorption certificate could skip, predicted on the CPU.
+
+The ensemble kernel blends in member order, num = fmaf(w_k, s_k, num) and den += w_k (DESIGN 4.1).  A member whose weight
+is tiny but not zero leaves both sums bit for bit unchanged when, at every valid point of a tile,
+  den_{k-1} + w_k == den_{k-1} in fp32                       (den half), and
+  w_k * B_k < ulp(L) / 4,  L <= |num_{k-1}|,  B_k >= |s_k|   (num half: fmaf returns num_{k-1}).
+Skipping such a member is exact.  This tool counts, for the seeded head of bench.py, the member-tiles that survive the
+zero-weight skip and the ones the certificate would remove on top:
+  * den half: the in-order fp32 partial sums of the weights (absorbed members do not change them);
+  * B_k: a float64 interval bound of member k's output over the grid box (layer 0 with the latent folded, softplus with
+    beta = 100, the latent-dependent layer-2 constant, the output layer), every pre-activation widened by a relative and an
+    absolute slack, and at least 1 (quirk points blend 1.0);
+  * L: what a kernel can know when it decides on member k - the minimum of |num| over the tile after the member two
+    evaluated positions earlier, minus max_w * B of the member evaluated in between (max_w rounded up to a power of two).
+num and den come from the fp32 member outputs of the CPU reference (tests/ensemble_f64_common.py).
+
+    python tools/absorbed_member_tiles.py [--latent 1] [--res 64] [--scale 1] [--plane-stride 1]
+
+Every certified member is checked against the fp32 blend: the tool stops if one would change a bit of num or den.  It also
+prints what better-informed inputs would certify: L without the lag, with the tile's own max |s_k| for B_k, and the members that change
+no bit at all (what no tile-wide certificate can exceed).
+"""
+import argparse
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'tests'))
+sys.path.insert(0, os.path.join(ROOT, 'tools'))
+
+# slack of the member-output bound against what the kernel computes (3-pass fp16 products with fp32 accumulation, softplus
+# in log2 units with a polynomial lg2): every pre-activation interval grows by REL_SLACK * (|W| |h| + |b|) + ABS_SLACK
+REL_SLACK = 2.0 ** -10
+ABS_SLACK = 2.0 ** -10
+
+
+def softplus64(x):
+    """Softplus(beta=100, threshold=20) in float64, monotone."""
+    bx = 100.0 * x
+    return np.where(bx > 20.0, x, np.log1p(np.exp(np.minimum(bx, 20.0))) / 100.0)
+
+
+def member_bound(P, m, z, anc, lo, hi):
+    """B >= |s_m(x)| for every x in the box [lo, hi] (3,), as the kernel computes s_m: float64 interval propagation in
+    centre / radius form with REL_SLACK and ABS_SLACK per layer, at least 1.  inf when the bound is not finite."""
+    from ensemble_f64_common import SQRT2
+    s = P.weight_set(m)
+    layers = [(W[s].double().numpy(), b[s].double().numpy()) for W, b in P.layers]
+    z = z.double().numpy()
+    cond = np.concatenate([z[:P.G], z[P.G + m * P.L:P.G + (m + 1) * P.L]])
+    a = anc[m] if m < P.n_loc else np.zeros(3)
+    xl, xh = np.asarray(lo, np.float64) - a, np.asarray(hi, np.float64) - a
+    if P.mirrored(m):
+        xl, xh = xl.copy(), xh.copy()
+        xl[0], xh[0] = -xh[0], -xl[0]
+    xc, xr = (xl + xh) / 2, (xh - xl) / 2
+    skip = P.n_layers // 2
+    hc, hr = xc, xr
+    with np.errstate(over='ignore', invalid='ignore'):
+        for l, (W, b) in enumerate(layers):
+            if l == 0:
+                Wx, bias = W[:, :3], W[:, 3:] @ cond + b
+            elif l == skip:
+                n_h = hc.shape[0]
+                Wx = W[:, :n_h + 3] / SQRT2
+                bias = W[:, n_h + 3:] @ cond / SQRT2 + b
+                hc, hr = np.concatenate([hc, xc]), np.concatenate([hr, xr])
+            else:
+                Wx, bias = W, b
+            c = Wx @ hc + bias
+            r = np.abs(Wx) @ hr + REL_SLACK * (np.abs(Wx) @ (np.abs(hc) + hr) + np.abs(bias)) + ABS_SLACK
+            if l + 1 < len(layers):
+                lo_, hi_ = softplus64(c - r), softplus64(c + r)
+                hc, hr = (lo_ + hi_) / 2, (hi_ - lo_) / 2
+            else:
+                B = float(np.abs(c[0]) + r[0])
+    return max(B, 1.0) if np.isfinite(B) else float('inf')
+
+
+def pow2_above(x):
+    """The smallest power of two strictly above x > 0 (float32 exponent field + 1), as the kernel stores a weight bound."""
+    e = np.floor(np.log2(x.astype(np.float64)))
+    return np.exp2(e + 1)
+
+
+def ulp32(x):
+    """ulp of positive normal float32 values x (float64 result)."""
+    x = np.asarray(x, np.float32)
+    return (np.nextafter(x, np.float32(np.inf)) - x).astype(np.float64)
+
+
+def absorbable(den, w, num_lo, wmax_bound, B):
+    """The certificate (vectorised): den + w == den in float32, and wmax_bound * B < ulp(num_lo) / 4 with num_lo a lower
+    bound of |num| (float64), wmax_bound >= w and B >= |s|.  When it holds, fmaf(w, s, num) == num and den + w == den."""
+    den, w = np.asarray(den, np.float32), np.asarray(w, np.float32)
+    return ((den + w) == den) & num_half(np.asarray(num_lo, np.float64), np.float64(wmax_bound), B)
+
+
+def grid_setup(latent_seed, scale=1.0):
+    import torch
+    from conftest import make_ensemble, sample_latent
+    from ensemble_f64_common import Params, anchors
+    dec = make_ensemble(0, scale=scale).eval()
+    z = sample_latent(latent_seed).reshape(-1)
+    P32, P64 = Params(dec, torch.float32), Params(dec, torch.float64)
+    with torch.no_grad():
+        anc32 = anchors(P32, z)
+    return P32, P64, z, anc32
+
+
+def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride=1, chunk_tiles=1024):
+    """dict of member-tile counts on the res^3 grid with the kernel's dense tiles (with plane_stride > 1: on the tiles of
+    every plane_stride-th x-plane)."""
+    import torch
+    from conftest import MAXI, MINI
+    from ensemble_f64_common import members
+    from zero_member_tiles import tile_layout, tile_points
+    mini = MINI if mini is None else mini
+    maxi = MAXI if maxi is None else maxi
+    P32, P64, z, anc32 = grid_setup(latent_seed, scale)
+    M = P32.M
+    anc_np = anc32.numpy().astype(np.float32)
+    axes = [np.linspace(mini[a], maxi[a], res).astype(np.float32) for a in range(3)]
+    lo = np.array([axes[a].min() for a in range(3)], np.float64)
+    hi = np.array([axes[a].max() for a in range(3)], np.float64)
+    B = np.array([member_bound(P64, m, z, anc_np.astype(np.float64), lo, hi) for m in range(M)])
+    count = res ** 3
+    kind, block = tile_layout(res, 0, count, 'auto')
+    ix, iy, iz, valid = tile_points(res, 0, count, kind, block)
+    if plane_stride > 1:
+        # a sample of the grid: the tiles of every plane_stride-th x-plane (a dense tile never crosses a plane)
+        keep = ix[:, 0] % plane_stride == 0
+        ix, iy, iz, valid = ix[keep], iy[keep], iz[keep], valid[keep]
+    n_tiles = ix.shape[0]
+    stats = {'tiles': int(n_tiles), 'member_tiles': int(n_tiles * M), 'zero': 0, 'den_absorbed': 0, 'absorbed': 0,
+             'absorbed_no_lag': 0, 'absorbed_tile_max': 0, 'unchanged': 0, 'B': B}
+    gw = np.float32(np.exp(np.float32(-0.2) / np.float32(0.01)))
+    for t0 in range(0, n_tiles, chunk_tiles):
+        sl = slice(t0, min(n_tiles, t0 + chunk_tiles))
+        X = np.stack([axes[0][ix[sl]], axes[1][iy[sl]], axes[2][iz[sl]]], axis=-1)       # T x 128 x 3
+        V = valid[sl]
+        T = X.shape[0]
+        pts = torch.from_numpy(X.reshape(-1, 3))
+        with torch.no_grad():
+            S = members(P32, pts, z, anc32).numpy().reshape(T, 128, M)
+        with np.errstate(under='ignore'):
+            d = anc_np[None, None] - X[:, :, None, :]                                       # T x 128 x 39 x 3
+            d2 = np.float32(d[..., 2] * d[..., 2] + (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]))
+            nrm = np.sqrt(d2) + np.float32(10e-6)
+            Wt = np.exp(-(nrm * nrm) / np.float32(0.01)).astype(np.float32)
+        Wt = np.concatenate([Wt, np.full((T, 128, 1), gw, np.float32)], axis=2)
+        # skipped members leave num and den as they were, so the state is that of the full sequence
+        num = np.zeros((T, 128), np.float32)
+        den = np.zeros((T, 128), np.float32)
+        pub = [np.full(T, -np.inf), np.full(T, -np.inf)]      # min |num| after the last two evaluated members (none: -inf)
+        last_bound = np.zeros(T)                             # max_w * B of the last evaluated member
+        inf32 = np.float32(np.inf)
+        for k in range(M):
+            w = Wt[:, :, k]
+            zero = ~np.any(V & (w != 0), axis=1)
+            den_abs = np.all(~V | ((den + w) == den), axis=1)
+            wmax = np.where(V, w, 0).max(axis=1)
+            wb = np.where(wmax > 0, pow2_above(np.maximum(wmax, np.float32(1e-45))), 0.0)
+            mn_before = np.where(V, np.abs(num), inf32).min(axis=1).astype(np.float64)
+            cert = den_abs & num_half(pub[0] - last_bound, wb, B[k]) & ~zero
+            no_lag = den_abs & num_half(mn_before, wb, B[k]) & ~zero
+            s = np.where(V, S[:, :, k], 0).astype(np.float64)
+            # the same without lag, with the tile's own max |s_k| (at least 1) in place of B_k: what a per-tile bound could reach
+            tile_b = np.maximum(np.abs(s).max(axis=1), 1.0)
+            oracle = den_abs & num_half(mn_before, wb, tile_b) & ~zero
+            new_num = (w.astype(np.float64) * s + num.astype(np.float64)).astype(np.float32)
+            unchanged = den_abs & np.all(~V | (new_num == num), axis=1) & ~zero
+            assert not np.any(cert & ~unchanged), 'the certificate passed a member that changes num'
+            stats['zero'] += int(zero.sum())
+            stats['den_absorbed'] += int((den_abs & ~zero).sum())
+            stats['absorbed'] += int(cert.sum())
+            stats['absorbed_no_lag'] += int(no_lag.sum())
+            stats['absorbed_tile_max'] += int(oracle.sum())
+            stats['unchanged'] += int(unchanged.sum())
+            ev = ~(zero | cert)
+            num = new_num
+            den = den + w
+            mn = np.where(V, np.abs(num), inf32).min(axis=1).astype(np.float64)
+            pub = [np.where(ev, pub[1], pub[0]), np.where(ev, mn, pub[1])]
+            last_bound = np.where(ev, wb * B[k], last_bound)
+    n = stats['member_tiles']
+    stats['evaluated_now'] = n - stats['zero']
+    stats['evaluated_absorb'] = stats['evaluated_now'] - stats['absorbed']
+    return stats
+
+
+def num_half(L, wmax_bound, B):
+    """Per tile: wmax_bound * B < ulp(L) / 4 with L (float64) rounded down to float32; False where L is not a positive
+    normal float32 or B is not finite."""
+    ok = (L > np.finfo(np.float32).tiny) & np.isfinite(B)
+    B = np.where(ok, B, 0.0)
+    L = np.where(ok, L, 1.0)
+    Lc = L.astype(np.float32)
+    Lc = np.where(Lc.astype(np.float64) > L, np.nextafter(Lc, np.float32(0)), Lc)
+    return ok & (wmax_bound * B < ulp32(Lc) / 4)
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument('--latent', type=int, default=1)
+    ap.add_argument('--res', type=int, default=64)
+    ap.add_argument('--scale', type=float, default=1.0)
+    ap.add_argument('--plane-stride', type=int, default=1, help='count the tiles of every n-th x-plane only (dense tiles)')
+    args = ap.parse_args()
+    r = predict(args.latent, args.res, args.scale, plane_stride=args.plane_stride)
+    ev = r['evaluated_now']
+    if args.plane_stride > 1:
+        print('tiles of every %d-th x-plane' % args.plane_stride)
+    print('latent %d, %d^3 grid: %d tiles, %d member-tiles, %d evaluated with the zero-weight skip; den half holds on %d '
+          '(%.1f %%), the full certificate on %d (%.1f %%) -> %d evaluated'
+          % (args.latent, args.res, r['tiles'], r['member_tiles'], ev, r['den_absorbed'], 100 * r['den_absorbed'] / ev,
+             r['absorbed'], 100 * r['absorbed'] / ev, r['evaluated_absorb']))
+    print('with L = min |num_{k-1}| (no lag): %d (%.1f %%); no lag and the tile max of |s_k| for B_k: %d (%.1f %%); '
+          'members that change no bit of num and den: %d (%.1f %%)'
+          % (r['absorbed_no_lag'], 100 * r['absorbed_no_lag'] / ev, r['absorbed_tile_max'],
+             100 * r['absorbed_tile_max'] / ev, r['unchanged'], 100 * r['unchanged'] / ev))
+    print('B_k: min %.3g, median %.3g, max %.3g' % (r['B'].min(), np.median(r['B']), r['B'].max()))
+
+
+if __name__ == '__main__':
+    main()
