@@ -35,7 +35,7 @@ extern "C" {
                                 reference computation: |error| <= n_members * tau * max_k |s_k| (tau default 1e-8). */
 
 const char *nphm_last_error(void);
-int nphm_abi_version(void);
+int nphm_abi_version(void);      /* 2: the narrow-band steps are the nphm_band_slab_* family only */
 /* sm count and compute capability of the current device */
 int nphm_device_info(int *sm_count, int *cc_major, int *cc_minor);
 
@@ -445,59 +445,44 @@ int nphm_render_depth_normals(const float *verts_dev, long long n_verts, const i
                               void *workspace_dev, long long workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Narrow-band mesh extraction: the steps of extract_mesh_narrowband (nphm_b200/utils/reconstruction.py, DESIGN §4.13), which
- * gives the mesh of `mesh_from_logits(get_logits(...))` on a res^3 grid while evaluating the decoder only near the surface.
+ * Narrow-band mesh extraction: the steps of extract_mesh_narrowband (nphm_b200/utils/reconstruction.py, DESIGN §4.13, §4.16),
+ * which gives the mesh of `mesh_from_logits(get_logits(...))` on a res^3 grid while evaluating the decoder only near the surface.
  * The (res-1)^3 cells are split into blocks of block^3 cells (the last block of an axis may be partial); block b covers the
- * voxels [b*block, min(b*block + block, res-1)] of every axis.  The decoder is evaluated by the caller, through the existing
- * query entry points, on coordinates these calls gather; the band state lives in the caller's workspace:
- *   nphm_band_begin      resets the state; quirk_period > 0: lists the eval-mode quirk voxels (g % p == p-1 or g == res^3-1,
- *                        which the caller evaluates in a query of period 1) and activates every block owning a cell that touches one
- *   nphm_band_corners    lists the block corners not evaluated yet (fine indices 0, block, 2 block, ..., res-1)
- *   nphm_band_classify   activates the blocks with a corner |sdf| <= tau (or NaN) or corners on both sides of the marching-cubes
- *                        test (-sdf <= 0), then lists the voxels of all newly activated blocks not evaluated yet
- *   nphm_band_grow       activates every inactive block with an evaluated face voxel on the other side of the test from its
- *                        corner 0, then lists as classify does (0 listed: the band is closed)
- *   nphm_band_fill       gives every voxel not evaluated the value of corner 0 of an (inactive) block containing it
- * A listing call writes its list, ascending in the flat index z + res (y + res x), to the workspace and, when counts_host is not
- * NULL, {voxels listed, blocks active so far} to counts_host[0..1] (synchronises the stream).  nphm_band_gather writes the
- * float32(linspace_f64(min, max, res)) coordinates of the first n listed voxels to xyz_dev (n x 3; those of
- * create_grid_points_from_bounds and nphm_ensemble_query_grid); nphm_band_scatter writes values_dev[i] to vol_dev[list[i]]
- * (i < n), and every listed voxel counts as evaluated.  vol_dev: res^3 floats, x slowest.
- * Needs 2 <= res <= 1024, 1 <= block <= 64, tau >= 0 (else NPHM_ERR_INVALID); workspace_bytes (checked, NPHM_ERR_CAPACITY when
- * short) >= nphm_band_workspace_bytes(res, block). */
-/* bytes of the band workspace (-1: bad arguments) */
-long long nphm_band_workspace_bytes(int res, int block);
-int nphm_band_begin(int res, int block, long long quirk_period, void *workspace_dev, long long workspace_bytes,
-                    long long *counts_host, void *stream);
-int nphm_band_corners(int res, int block, void *workspace_dev, long long workspace_bytes, long long *counts_host, void *stream);
-int nphm_band_gather(int res, int block, const double grid_min[3], const double grid_max[3], long long n, float *xyz_dev,
-                     void *workspace_dev, long long workspace_bytes, void *stream);
-int nphm_band_scatter(int res, int block, long long n, const float *values_dev, float *vol_dev, void *workspace_dev,
-                      long long workspace_bytes, void *stream);
-int nphm_band_classify(int res, int block, float tau, const float *vol_dev, void *workspace_dev, long long workspace_bytes,
-                       long long *counts_host, void *stream);
-int nphm_band_grow(int res, int block, const float *vol_dev, void *workspace_dev, long long workspace_bytes, long long *counts_host,
-                   void *stream);
-int nphm_band_fill(int res, int block, float *vol_dev, void *workspace_dev, long long workspace_bytes, void *stream);
-/* states_dev (blocks^3 bytes, blocks = ceil((res-1)/block), x slowest): 0 inactive, 1 or 2 active */
-int nphm_band_block_states(int res, int block, const void *workspace_dev, long long workspace_bytes, unsigned char *states_dev,
-                           void *stream);
-/* The same steps on an x-slab of the grid, for extracting one mesh on several GPUs (nphm_b200/distributed.py:
- * extract_mesh_narrowband_sharded, DESIGN §4.16): the slab owns the block layers [l0, l1) along x (0 <= l0 < l1 <= blocks) and
- * holds the voxel planes [X0, X1] = [l0*block, min(l1*block, res-1)]; a plane X0 > 0 or X1 < res-1 is shared with the neighbouring
- * slab.  Its workspace (nphm_band_slab_workspace_bytes, -1: bad arguments) covers those planes only, and every vol_dev is the slab
- * volume of planes X0-1 .. X1, res^2 floats each, where plane X0-1 (the ghost plane the slab marching cubes reads with
- * x_global0 = X0-1, ghost_lo = 1) is present only when l0 > 0.  List indices are local to the slab; nphm_band_slab_gather writes
- * the global grid coordinates.  nphm_band_slab_begin lists the quirk voxels of global flat index in the slab's planes and
- * activates the slab's blocks around them; nphm_band_slab_corners lists the corners on the slab's planes; the block states are
- * (l1-l0) x blocks x blocks.  Together with a neighbour, after each round of evaluation:
+ * voxels [b*block, min(b*block + block, res-1)] of every axis.  Every step works on an x-slab: the block layers [l0, l1) along x
+ * (0 <= l0 < l1 <= blocks, blocks = ceil((res-1)/block)) and their voxel planes [X0, X1] = [l0*block, min(l1*block, res-1)].
+ * The whole grid is the slab [0, blocks); several slabs extract one mesh on several GPUs (extract_mesh_narrowband_sharded), and
+ * a plane X0 > 0 or X1 < res-1 is shared with the neighbouring slab.  The decoder is evaluated by the caller, through the
+ * existing query entry points, on coordinates these calls gather; the band state lives in the caller's workspace, which covers
+ * the slab's planes only:
+ *   nphm_band_slab_begin      resets the state; quirk_period > 0: lists the eval-mode quirk voxels of global flat index in the
+ *                             slab's planes (g % p == p-1 or g == res^3-1, which the caller evaluates in a query of period 1) and
+ *                             activates every block of the slab owning a cell that touches one
+ *   nphm_band_slab_corners    lists the block corners on the slab's planes not evaluated yet (fine indices 0, block, 2 block,
+ *                             ..., res-1)
+ *   nphm_band_slab_classify   activates the blocks with a corner |sdf| <= tau (or NaN) or corners on both sides of the
+ *                             marching-cubes test (-sdf <= 0), then lists the voxels of all newly activated blocks not evaluated
+ *                             yet
+ *   nphm_band_slab_grow       activates every inactive block with an evaluated face voxel on the other side of the test from its
+ *                             corner 0, then lists as classify does (0 listed: the band is closed)
+ *   nphm_band_slab_fill       gives every voxel not evaluated the value of corner 0 of an (inactive) block containing it
+ * A listing call writes its list, ascending in the slab-local flat index z + res (y + res (x - X0)), to the workspace and, when
+ * counts_host is not NULL, {voxels listed, blocks active so far} to counts_host[0..1] (synchronises the stream).
+ * nphm_band_slab_gather writes the float32(linspace_f64(min, max, res)) global grid coordinates of the first n listed voxels to
+ * xyz_dev (n x 3; those of create_grid_points_from_bounds and nphm_ensemble_query_grid); nphm_band_slab_scatter writes
+ * values_dev[i] to the listed voxel list[i] of vol_dev (i < n), and every listed voxel counts as evaluated.  vol_dev is the slab
+ * volume of planes X0-1 .. X1, res^2 floats each, x slowest, where plane X0-1 (the ghost plane the slab marching cubes reads
+ * with x_global0 = X0-1, ghost_lo = 1) is present only when l0 > 0: res^3 floats for the whole grid.  Together with a
+ * neighbour, after each round of evaluation:
  *   nphm_band_slab_export  writes plane `plane` of [X0, X1] to buf_dev: res^2 floats of the volume, then res^2 bytes (1: the voxel
  *                          is evaluated on this slab)
  *   nphm_band_slab_import  merges a buffer the neighbour exported of the plane both hold (X0 from below, X1 from above): every
  *                          voxel the neighbour evaluated and this slab did not takes its value and counts as evaluated, so that
- *                          nphm_band_slab_grow sees it as nphm_band_grow does on the whole grid.  After nphm_band_slab_fill,
- *                          plane X0-1 imports the filled values of the lower neighbour's plane X1-1 into the ghost plane.
- * Any other plane is NPHM_ERR_INVALID, as is an empty or out-of-range slab.  Export and import enqueue kernels only. */
+ *                          nphm_band_slab_grow sees it as it would on the whole grid.  After nphm_band_slab_fill, plane X0-1
+ *                          imports the filled values of the lower neighbour's plane X1-1 into the ghost plane.
+ * Any other plane is NPHM_ERR_INVALID; export and import enqueue kernels only.  Needs 2 <= res <= 1024, 1 <= block <= 64, a
+ * non-empty slab within the grid and tau >= 0 (else NPHM_ERR_INVALID); workspace_bytes (checked, NPHM_ERR_CAPACITY when short)
+ * >= nphm_band_slab_workspace_bytes(res, block, l0, l1). */
+/* bytes of the band workspace of the slab (-1: bad arguments) */
 long long nphm_band_slab_workspace_bytes(int res, int block, int l0, int l1);
 int nphm_band_slab_begin(int res, int block, int l0, int l1, long long quirk_period, void *workspace_dev, long long workspace_bytes,
                          long long *counts_host, void *stream);
@@ -513,6 +498,7 @@ int nphm_band_slab_grow(int res, int block, int l0, int l1, const float *vol_dev
                         long long *counts_host, void *stream);
 int nphm_band_slab_fill(int res, int block, int l0, int l1, float *vol_dev, void *workspace_dev, long long workspace_bytes,
                         void *stream);
+/* states_dev ((l1-l0) x blocks x blocks bytes, x slowest): 0 inactive, 1 or 2 active */
 int nphm_band_slab_block_states(int res, int block, int l0, int l1, const void *workspace_dev, long long workspace_bytes,
                                 unsigned char *states_dev, void *stream);
 int nphm_band_slab_export(int res, int block, int l0, int l1, int plane, const float *vol_dev, const void *workspace_dev,

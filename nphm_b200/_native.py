@@ -42,8 +42,6 @@ EXPORTED_SYMBOLS = (
     'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad', 'nphm_mlp_fit_surface_grad_batched',
     'nphm_ensemble_sdfgrad_workspace_bytes', 'nphm_ensemble_sdfgrad_forward', 'nphm_ensemble_sdfgrad_backward',
     'nphm_render_workspace_bytes', 'nphm_render_depth_normals',
-    'nphm_band_workspace_bytes', 'nphm_band_begin', 'nphm_band_corners', 'nphm_band_gather', 'nphm_band_scatter',
-    'nphm_band_classify', 'nphm_band_grow', 'nphm_band_fill', 'nphm_band_block_states',
     'nphm_band_slab_workspace_bytes', 'nphm_band_slab_begin', 'nphm_band_slab_corners', 'nphm_band_slab_gather',
     'nphm_band_slab_scatter', 'nphm_band_slab_classify', 'nphm_band_slab_grow', 'nphm_band_slab_fill', 'nphm_band_slab_block_states',
     'nphm_band_slab_export', 'nphm_band_slab_import',
@@ -212,22 +210,18 @@ def lib() -> ctypes.CDLL:
     L.nphm_render_workspace_bytes.restype = c_longlong
     L.nphm_render_depth_normals.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_double,
                                             c_double, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
-    L.nphm_band_workspace_bytes.argtypes = [c_int, c_int]
-    L.nphm_band_workspace_bytes.restype = c_longlong
-    L.nphm_band_begin.argtypes = [c_int, c_int, c_longlong, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
-    L.nphm_band_corners.argtypes = [c_int, c_int, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
-    L.nphm_band_gather.argtypes = [c_int, c_int, POINTER(c_double), POINTER(c_double), c_longlong, c_void_p, c_void_p, c_longlong,
-                                   c_void_p]
-    L.nphm_band_scatter.argtypes = [c_int, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
-    L.nphm_band_classify.argtypes = [c_int, c_int, c_float, c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
-    L.nphm_band_grow.argtypes = [c_int, c_int, c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
-    L.nphm_band_fill.argtypes = [c_int, c_int, c_void_p, c_void_p, c_longlong, c_void_p]
-    L.nphm_band_block_states.argtypes = [c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p]
-    slab = [c_int, c_int, c_int, c_int]                 # res, block, l0, l1: the same steps on an x-slab
+    slab = [c_int, c_int, c_int, c_int]                 # res, block, l0, l1: the x-slab every step works on
     L.nphm_band_slab_workspace_bytes.argtypes = slab
     L.nphm_band_slab_workspace_bytes.restype = c_longlong
-    for name in ('begin', 'corners', 'gather', 'scatter', 'classify', 'grow', 'fill', 'block_states'):
-        getattr(L, 'nphm_band_slab_' + name).argtypes = slab + getattr(L, 'nphm_band_' + name).argtypes[2:]
+    L.nphm_band_slab_begin.argtypes = slab + [c_longlong, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_slab_corners.argtypes = slab + [c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_slab_gather.argtypes = slab + [POINTER(c_double), POINTER(c_double), c_longlong, c_void_p, c_void_p, c_longlong,
+                                              c_void_p]
+    L.nphm_band_slab_scatter.argtypes = slab + [c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_slab_classify.argtypes = slab + [c_float, c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_slab_grow.argtypes = slab + [c_void_p, c_void_p, c_longlong, POINTER(c_longlong), c_void_p]
+    L.nphm_band_slab_fill.argtypes = slab + [c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_slab_block_states.argtypes = slab + [c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_band_slab_export.argtypes = slab + [c_int, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_band_slab_import.argtypes = slab + [c_int, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
     L.nphm_face_cdf_workspace_bytes.argtypes = [c_longlong]
@@ -963,30 +957,34 @@ def transfer_correspondences(src_verts, src_faces, dst_verts, dst_faces, face_id
 
 # ------------------------------------------------------------------------------------------ narrow-band extraction
 class NarrowBand:
-    """Band state of one ``res^3`` grid in blocks of ``block^3`` cells (``nphm_band_*``, DESIGN §4.13) in a workspace this object
-    owns.  The listing steps return the number of voxels they listed; :meth:`gather` / :meth:`scatter` move the listed voxels'
-    coordinates out and their values into a ``res^3`` float32 CUDA volume."""
+    """Band state of the x-slab of block layers ``[l0, l1)`` of a ``res^3`` grid in blocks of ``block^3`` cells
+    (``nphm_band_slab_*``, DESIGN §4.13, §4.16) in a workspace this object owns; ``l1=None`` takes every block layer, so the
+    default slab is the whole grid.  The slab holds the voxel planes ``[x0, x1]``, with a volume of :attr:`n_planes` planes from
+    :attr:`first_plane` (``x0 - 1``, the ghost plane, when ``l0 > 0``).  The listing steps return the number of voxels they listed;
+    :meth:`gather` / :meth:`scatter` move the listed voxels' coordinates out and their values into the volume, and :meth:`export` /
+    :meth:`import_` merge a plane shared with a neighbour."""
 
-    _prefix = 'nphm_band_'
-
-    def __init__(self, res: int, block: int, device):
+    def __init__(self, res: int, block: int, device, l0: int = 0, l1: Optional[int] = None):
         self.res, self.block = int(res), int(block)
         self.device = torch.device(device)
-        self._geo = self._geometry()
+        # max(): block 0 must reach the native argument check, which rejects it, rather than fail in this division
+        self.blocks_per_axis = -(-(self.res - 1) // max(self.block, 1))
+        self.l0 = int(l0)
+        self.l1 = self.blocks_per_axis if l1 is None else int(l1)
+        self._geo = (self.res, self.block, self.l0, self.l1)
         with torch.cuda.device(self.device):
-            self.ws = _workspace(self._fn('workspace_bytes')(*self._geo), self._prefix + 'workspace_bytes', self.device)
-        self.blocks_per_axis = -(-(self.res - 1) // self.block)
+            self.ws = _workspace(lib().nphm_band_slab_workspace_bytes(*self._geo), 'nphm_band_slab_workspace_bytes', self.device)
         self.active_blocks = 0
-
-    def _geometry(self):
-        return self.res, self.block
-
-    def _fn(self, step):
-        return getattr(lib(), self._prefix + step)
+        self.x0 = self.l0 * self.block
+        self.x1 = min(self.l1 * self.block, self.res - 1)
+        self.ghost = self.l0 > 0
+        self.first_plane = self.x0 - int(self.ghost)
+        self.n_planes = self.x1 + 1 - self.first_plane
+        self.plane_bytes = 5 * self.res * self.res          # res^2 float32 values, then res^2 evaluated flags
 
     def _call(self, step, *args):
         with torch.cuda.device(self.device):
-            check(self._fn(step)(*self._geo, *args, _stream_ptr(self.device)), self._prefix + step)
+            check(getattr(lib(), 'nphm_band_slab_' + step)(*self._geo, *args, _stream_ptr(self.device)), 'nphm_band_slab_' + step)
 
     def _call_listing(self, step, *before_ws):
         counts = (c_longlong * 2)()
@@ -1022,40 +1020,12 @@ class NarrowBand:
     def fill(self, vol: torch.Tensor):
         self._call('fill', vol.data_ptr(), self.ws.data_ptr(), self.ws.numel())
 
-    def _states_shape(self):
-        nb = self.blocks_per_axis
-        return nb, nb, nb
-
     def block_states(self) -> torch.Tensor:
-        """(blocks, blocks, blocks) bool: which blocks are active (a slab: its block layers along x)."""
-        out = torch.empty(self._states_shape(), device=self.device, dtype=torch.uint8)
+        """(l1 - l0, blocks, blocks) bool: which blocks of the slab are active."""
+        nb = self.blocks_per_axis
+        out = torch.empty(self.l1 - self.l0, nb, nb, device=self.device, dtype=torch.uint8)
         self._call('block_states', self.ws.data_ptr(), self.ws.numel(), out.data_ptr())
         return out != 0
-
-
-class NarrowBandSlab(NarrowBand):
-    """The band of the x-slab of block layers ``[l0, l1)`` of a ``res^3`` grid (``nphm_band_slab_*``, DESIGN §4.16): the same steps
-    as :class:`NarrowBand` on the slab's voxel planes ``[x0, x1]``, with a volume of :attr:`n_planes` planes from :attr:`first_plane`
-    (``x0 - 1``, the ghost plane, when ``l0 > 0``), and :meth:`export` / :meth:`import_` to merge a plane shared with a neighbour."""
-
-    _prefix = 'nphm_band_slab_'
-
-    def __init__(self, res: int, block: int, l0: int, l1: int, device):
-        self.l0, self.l1 = int(l0), int(l1)
-        super().__init__(res, block, device)
-        self.x0 = self.l0 * self.block
-        self.x1 = min(self.l1 * self.block, self.res - 1)
-        self.ghost = self.l0 > 0
-        self.first_plane = self.x0 - int(self.ghost)
-        self.n_planes = self.x1 + 1 - self.first_plane
-        self.plane_bytes = 5 * self.res * self.res          # res^2 float32 values, then res^2 evaluated flags
-
-    def _geometry(self):
-        return self.res, self.block, self.l0, self.l1
-
-    def _states_shape(self):
-        nb = self.blocks_per_axis
-        return self.l1 - self.l0, nb, nb
 
     def volume(self) -> torch.Tensor:
         """An uninitialised (n_planes, res, res) float32 slab volume on the band's device."""
@@ -1071,5 +1041,11 @@ class NarrowBandSlab(NarrowBand):
         """Merge a neighbour's :meth:`export` of the shared ``plane`` (x0 or x1), or copy its filled plane x0 - 1 into the ghost
         plane."""
         if buf.device != self.device or buf.dtype != torch.uint8 or buf.numel() != self.plane_bytes:
-            raise ValueError('NarrowBandSlab.import_: need a uint8 buffer of %d bytes on %s' % (self.plane_bytes, self.device))
+            raise ValueError('NarrowBand.import_: need a uint8 buffer of %d bytes on %s' % (self.plane_bytes, self.device))
         self._call('import', int(plane), buf.data_ptr(), vol.data_ptr(), self.ws.data_ptr(), self.ws.numel())
+
+
+def NarrowBandSlab(res: int, block: int, l0: int, l1: int, device) -> NarrowBand:
+    """The :class:`NarrowBand` of the x-slab of block layers ``[l0, l1)``, in the argument order the callers of the multi-GPU band
+    use."""
+    return NarrowBand(res, block, device, l0, l1)

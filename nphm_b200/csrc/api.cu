@@ -110,7 +110,7 @@ void fill_descriptors(const StackDims &s, const NetWeights &w, int n_members, in
 using namespace nphm;
 
 extern "C" const char *nphm_last_error(void) { return g_error; }
-extern "C" int nphm_abi_version(void) { return 1; }
+extern "C" int nphm_abi_version(void) { return 2; }
 
 extern "C" int nphm_device_info(int *sms, int *major, int *minor)
 {

@@ -39,13 +39,12 @@ struct Layout {
 
 inline int blocks_per_axis(int res, int block) { return (int)ceil_div(res - 1, block); }
 
-// l1 < 0: the whole grid
-inline Geo make_geo(int res, int block, int l0 = 0, int l1 = -1)
+inline Geo make_geo(int res, int block, int l0, int l1)
 {
     Geo g;
     g.res = res; g.B = block; g.C = res - 1;
     g.nb = blocks_per_axis(res, block);
-    g.L0 = l0; g.L1 = l1 < 0 ? g.nb : l1;
+    g.L0 = l0; g.L1 = l1;
     g.X0 = g.L0 * block; g.X1 = std::min(g.L1 * block, g.C);
     g.ghost = g.L0 > 0 ? 1 : 0;
     g.rr = (long long)res * res;
@@ -341,17 +340,10 @@ __global__ void import_kernel(const Geo g, int plane, const float *__restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-int check_args(int res, int block, const char *who)
+int check_args(int res, int block, int l0, int l1, const char *who)
 {
     NPHM_REQUIRE(res >= 2 && res <= 1024, "%s: res %d outside [2, 1024]", who, res);
     NPHM_REQUIRE(block >= 1 && block <= 64, "%s: block %d outside [1, 64]", who, block);
-    return NPHM_OK;
-}
-
-int check_slab(int res, int block, int l0, int l1, const char *who)
-{
-    int rc = check_args(res, block, who);
-    if (rc) return rc;
     const int nb = blocks_per_axis(res, block);
     NPHM_REQUIRE(l0 >= 0 && l0 < l1 && l1 <= nb, "%s: block layers [%d, %d) not a non-empty range of [0, %d)", who, l0, l1, nb);
     return NPHM_OK;
@@ -362,11 +354,8 @@ int check_ws(const Geo &g, const void *ws, long long ws_bytes, const char *who)
     NPHM_REQUIRE(ws, "%s: NULL workspace", who);
     const long long need = layout(g).bytes;
     if (ws_bytes < need) {
-        if (g.L0 == 0 && g.L1 == g.nb)
-            set_error("%s: band workspace too small: %lld bytes for res %d, block %d, %lld needed", who, ws_bytes, g.res, g.B, need);
-        else
-            set_error("%s: band workspace too small: %lld bytes for res %d, block %d, block layers [%d, %d), %lld needed", who,
-                      ws_bytes, g.res, g.B, g.L0, g.L1, need);
+        set_error("%s: band workspace too small: %lld bytes for res %d, block %d, block layers [%d, %d), %lld needed", who, ws_bytes,
+                  g.res, g.B, g.L0, g.L1, need);
         return NPHM_ERR_CAPACITY;
     }
     return NPHM_OK;
@@ -403,7 +392,7 @@ int mark_and_compact(const Geo &g, const Ws &w, long long *counts_host, cudaStre
     return compact(g, w, counts_host, stream);
 }
 
-// ---- the steps, on the whole grid or a slab (the entry points below check the arguments)
+// ---- the steps on a slab (the entry points below check the arguments)
 int begin(const Geo &g, const Ws &w, long long quirk_period, long long *counts_host, cudaStream_t stream)
 {
     const Layout l = layout(g);
@@ -487,17 +476,8 @@ int block_states(const Geo &g, const void *ws, unsigned char *states_dev, cudaSt
 
 using namespace nphm;
 
-#define BAND_PROLOGUE(who)                                                  \
-    int rc = band::check_args(res, block, who);                            \
-    if (rc) return rc;                                                      \
-    const band::Geo g = band::make_geo(res, block);                         \
-    if ((rc = band::check_ws(g, ws, ws_bytes, who))) return rc;             \
-    const band::Ws w = band::carve(const_cast<void *>(static_cast<const void *>(ws)), band::layout(g)); \
-    (void)w;                                                                \
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-
 #define SLAB_PROLOGUE(who)                                                  \
-    int rc = band::check_slab(res, block, l0, l1, who);                    \
+    int rc = band::check_args(res, block, l0, l1, who);                     \
     if (rc) return rc;                                                      \
     const band::Geo g = band::make_geo(res, block, l0, l1);                 \
     if ((rc = band::check_ws(g, ws, ws_bytes, who))) return rc;             \
@@ -505,76 +485,10 @@ using namespace nphm;
     (void)w;                                                                \
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
 
-extern "C" long long nphm_band_workspace_bytes(int res, int block)
-{
-    if (band::check_args(res, block, "nphm_band_workspace_bytes")) return -1;
-    return band::layout(band::make_geo(res, block)).bytes;
-}
-
-extern "C" int nphm_band_begin(int res, int block, long long quirk_period, void *ws, long long ws_bytes, long long *counts_host,
-                               void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_begin")
-    NPHM_REQUIRE(quirk_period >= 0, "nphm_band_begin: negative quirk period %lld", quirk_period);
-    return band::begin(g, w, quirk_period, counts_host, stream);
-}
-
-extern "C" int nphm_band_corners(int res, int block, void *ws, long long ws_bytes, long long *counts_host, void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_corners")
-    return band::corners(g, w, counts_host, stream);
-}
-
-extern "C" int nphm_band_gather(int res, int block, const double grid_min[3], const double grid_max[3], long long n, float *xyz_dev,
-                                void *ws, long long ws_bytes, void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_gather")
-    NPHM_REQUIRE(grid_min && grid_max && n >= 0 && n <= g.n_vox && (n == 0 || xyz_dev), "nphm_band_gather: bad arguments");
-    return band::gather(g, w, grid_min, grid_max, n, xyz_dev, stream);
-}
-
-extern "C" int nphm_band_scatter(int res, int block, long long n, const float *values_dev, float *vol_dev, void *ws, long long ws_bytes,
-                                 void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_scatter")
-    NPHM_REQUIRE(n >= 0 && n <= g.n_vox && vol_dev && (n == 0 || values_dev), "nphm_band_scatter: bad arguments");
-    return band::scatter(g, w, n, values_dev, vol_dev, stream);
-}
-
-extern "C" int nphm_band_classify(int res, int block, float tau, const float *vol_dev, void *ws, long long ws_bytes,
-                                  long long *counts_host, void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_classify")
-    NPHM_REQUIRE(tau >= 0.f && vol_dev, "nphm_band_classify: need tau >= 0 (got %g) and a volume", (double)tau);
-    return band::classify(g, w, tau, vol_dev, counts_host, stream);
-}
-
-extern "C" int nphm_band_grow(int res, int block, const float *vol_dev, void *ws, long long ws_bytes, long long *counts_host,
-                              void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_grow")
-    NPHM_REQUIRE(vol_dev, "nphm_band_grow: NULL volume");
-    return band::grow(g, w, vol_dev, counts_host, stream);
-}
-
-extern "C" int nphm_band_fill(int res, int block, float *vol_dev, void *ws, long long ws_bytes, void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_fill")
-    NPHM_REQUIRE(vol_dev, "nphm_band_fill: NULL volume");
-    return band::fill(g, w, vol_dev, stream);
-}
-
-extern "C" int nphm_band_block_states(int res, int block, const void *ws, long long ws_bytes, unsigned char *states_dev, void *stream_)
-{
-    BAND_PROLOGUE("nphm_band_block_states")
-    NPHM_REQUIRE(states_dev, "nphm_band_block_states: NULL output");
-    return band::block_states(g, ws, states_dev, stream);
-}
-
-// ---------------------------------------------------------------------------------------------- x-slabs of the grid
+// ---------------------------------------------------------------------------------------------- entry points
 extern "C" long long nphm_band_slab_workspace_bytes(int res, int block, int l0, int l1)
 {
-    if (band::check_slab(res, block, l0, l1, "nphm_band_slab_workspace_bytes")) return -1;
+    if (band::check_args(res, block, l0, l1, "nphm_band_slab_workspace_bytes")) return -1;
     return band::layout(band::make_geo(res, block, l0, l1)).bytes;
 }
 

@@ -12,7 +12,9 @@ One process per GPU, ``torch.distributed`` (NCCL on GPUs; the host logic is exer
 tests/test_distributed_cpu.py).
 
 The narrow band (``extract_mesh_narrowband_sharded``, DESIGN §4.16) is sharded in x-slabs of whole block layers instead:
-the ranks swap the planes they share after every round of evaluation, and the ghost plane after the fill.
+the ranks swap the planes they share after every round of evaluation, and the ghost plane after the fill.  Its host driver
+(slab plan, round loop, per-slab marching cubes) is the one of the one-GPU band in ``utils/reconstruction.py``, where the
+one-GPU extraction is the one-slab case; this module adds the exchange between ranks (:class:`GroupExchange`).
 """
 from __future__ import annotations
 
@@ -20,6 +22,11 @@ from typing import Callable, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
+
+from .utils.reconstruction import _band_setup, _run_band, plan_block_slabs
+# the band's host driver stays importable from here, where the callers of the multi-GPU band find it next to GroupExchange
+from .utils.reconstruction import (LocalExchange, extract_mesh_narrowband_slabs, narrowband_slab_volumes,  # noqa: F401
+                                   narrowband_slabs_mesh)
 
 
 def plan_slabs(res: int, world: int) -> List[Tuple[int, int]]:
@@ -274,43 +281,6 @@ def inference_identity_space_sharded(decoder, all_obs, lambdas, n_steps, schedul
 # ------------------------------------------------------------------------------------------------------------------
 # Narrow-band extraction sharded in x-slabs of block layers (DESIGN §4.16)
 # ------------------------------------------------------------------------------------------------------------------
-def plan_block_slabs(res: int, block: int, world: int) -> List[Tuple[int, int]]:
-    """Block layers [l0, l1) of each rank: the ceil((res-1)/block) layers split as evenly as possible (first ranks get the extra),
-    so that every slab boundary is a block face; ranks past the number of layers get an empty range."""
-    n_layers = -(-(int(res) - 1) // int(block))
-    base, extra = divmod(n_layers, world)
-    out, c = [], 0
-    for r in range(world):
-        n = base + (1 if r < extra else 0)
-        out.append((c, c + n))
-        c += n
-    return out
-
-
-class LocalExchange:
-    """Every slab of one grid, driven by this process in rank order: planes move between the entries of the slab list and the
-    collectives reduce over it.  Lets one process (one device, or the CPU oracle) run the protocol of every rank in lockstep."""
-
-    def __init__(self, n_slabs: int):
-        self.ranks = list(range(n_slabs))
-
-    def swap(self, sends, expects, nbytes):
-        """sends[i] = (buffer to the lower, to the upper neighbour) of slab i; expects[i] = (from the lower, from the upper)."""
-        return [(sends[i - 1][1] if lo else None, sends[i + 1][0] if hi else None) for i, (lo, hi) in enumerate(expects)]
-
-    def any(self, counts) -> bool:
-        return any(c > 0 for c in counts)
-
-    def rows(self, rows):
-        return [list(r) for r in rows]
-
-    def counts(self, counts):
-        return list(counts)
-
-    def gather(self, parts, counts):
-        return torch.cat([v for v, _ in parts]), torch.cat([t for _, t in parts])
-
-
 class GroupExchange:
     """This rank's slab in a ``torch.distributed`` group: planes go to the neighbouring ranks in one batched point-to-point
     exchange, "anything listed" is an all-reduce, the mesh is assembled by :func:`exchange_counts` and :func:`gather_mesh`.
@@ -357,135 +327,6 @@ class GroupExchange:
         return (None, None) if verts is None else (verts.to(self.device), tris.to(self.device))
 
 
-def narrowband_slab_volumes(slabs, evaluate, mini, maxi, tau: float, exchange, quirk_period: int = 0, evaluate_quirk=None):
-    """The band of :func:`nphm_b200.utils.reconstruction.narrowband_volume` on x-slabs.  ``slabs``: the slabs this process drives
-    (:class:`nphm_b200._native.NarrowBandSlab`, or None for a rank without block layers), in the order of ``exchange.ranks``.
-    Every round: list, gather / evaluate / scatter, swap the planes shared with the neighbours, growth check, and ask the exchange
-    whether any slab listed anything.  After the last round: fill, then hand each slab its neighbour's filled ghost plane.
-    Returns ``(volumes, stats)``: one ``(n_planes, res, res)`` volume per slab (None for None), ``stats`` with ``growth_rounds``
-    and, per slab, ``blocks_active``, ``voxels_evaluated`` and ``bytes_sent`` (one entry per plane exchange)."""
-    vols = [None if s is None else s.volume() for s in slabs]
-    evaluated = [0] * len(slabs)
-    sent = [[] for _ in slabs]
-    nbytes = next((s.plane_bytes for s in slabs if s is not None), 0)
-
-    def run(ns, fn):
-        for i, (s, n) in enumerate(zip(slabs, ns)):
-            if n:
-                s.scatter(fn(s.gather(n, mini, maxi)).reshape(-1), vols[i])
-                evaluated[i] += n
-
-    def swap(plane_lo, plane_hi, ghost):
-        sends, expects = [], []
-        for s, v in zip(slabs, vols):
-            if s is None:
-                sends.append((None, None))
-                expects.append((False, False))
-                continue
-            lo, hi = s.l0 > 0, s.x1 < s.res - 1
-            sends.append((s.export(plane_lo(s), v) if lo and not ghost else None, s.export(plane_hi(s), v) if hi else None))
-            expects.append((lo, hi and not ghost))
-        got = exchange.swap(sends, expects, nbytes)
-        for i, (s, v) in enumerate(zip(slabs, vols)):
-            sent[i].append(sum(nbytes for b in sends[i] if b is not None))
-            if s is None:
-                continue
-            if got[i][0] is not None:
-                s.import_(s.x0 - 1 if ghost else s.x0, got[i][0], v)
-            if got[i][1] is not None:
-                s.import_(s.x1, got[i][1], v)
-
-    ns = [0 if s is None else s.begin(quirk_period) for s in slabs]
-    if quirk_period:
-        run(ns, evaluate_quirk)
-    run([0 if s is None else s.corners() for s in slabs], evaluate)
-    run([0 if s is None else s.classify(tau, v) for s, v in zip(slabs, vols)], evaluate)
-    swap(lambda s: s.x0, lambda s: s.x1, ghost=False)
-    rounds = 0
-    while True:
-        ns = [0 if s is None else s.grow(v) for s, v in zip(slabs, vols)]
-        if not exchange.any(ns):
-            break
-        rounds += 1
-        run(ns, evaluate)
-        swap(lambda s: s.x0, lambda s: s.x1, ghost=False)
-    for s, v in zip(slabs, vols):
-        if s is not None:
-            s.fill(v)
-    swap(None, lambda s: s.x1 - 1, ghost=True)
-    stats = {'growth_rounds': rounds, 'blocks_active': [0 if s is None else int(s.active_blocks) for s in slabs],
-             'voxels_evaluated': evaluated, 'bytes_sent': sent}
-    return vols, stats
-
-
-def _slab_mesh(slabs, vols, exchange, mc_count, mc_emit, device):
-    """mc_count -> exchange_counts -> mc_emit -> gather_mesh over the filled slab volumes: (verts, tris) in global index units,
-    ids as on one GPU, on rank 0 (None, None elsewhere)."""
-    local, params = [], []
-    for s, v in zip(slabs, vols):
-        if s is None:
-            local.append((0, 0))
-            params.append(None)
-            continue
-        nv, nt, p, ws = mc_count(v, 0.0, True, x_global0=s.first_plane, ghost_lo=s.ghost)
-        local.append((nv, nt))
-        params.append((p, ws))
-    counts = exchange.counts(local)
-    parts = []
-    for i, (s, v) in enumerate(zip(slabs, vols)):
-        if s is None:
-            parts.append((torch.empty(0, 3, dtype=torch.float64, device=device), torch.empty(0, 3, dtype=torch.int64, device=device)))
-            continue
-        base = sum(c[0] for c in counts[:exchange.ranks[i]])
-        parts.append(mc_emit(v, params[i][0], params[i][1], local[i][0], local[i][1], base))
-    return exchange.gather(parts, counts)
-
-
-def narrowband_slabs_mesh(slabs, evaluate, mini, maxi, res: int, block: int, tau: float, exchange, quirk_period: int = 0,
-                          evaluate_quirk=None, mc_count: Optional[Callable] = None, mc_emit: Optional[Callable] = None,
-                          device='cpu'):
-    """:func:`narrowband_slab_volumes` + the sharded marching cubes.  Returns ``(verts, tris, stats)`` with the mesh in global
-    index units on the process that holds rank 0 (None elsewhere) and ``stats`` for every rank of the grid.  ``mc_count`` /
-    ``mc_emit`` default to the CUDA kernels; tests inject CPU stand-ins, as for :func:`extract_mesh_sharded`."""
-    if mc_count is None or mc_emit is None:
-        from . import _native
-        mc_count, mc_emit = _native.marching_cubes_count, _native.marching_cubes_emit
-    vols, st = narrowband_slab_volumes(slabs, evaluate, mini, maxi, tau, exchange, quirk_period, evaluate_quirk)
-    verts, tris = _slab_mesh(slabs, vols, exchange, mc_count, mc_emit, device)
-    rows = exchange.rows([[a, e] + b for a, e, b in zip(st['blocks_active'], st['voxels_evaluated'], st['bytes_sent'])])
-    nb = -(-(res - 1) // block)
-    stats = {'blocks_active': [r[0] for r in rows], 'blocks_total': nb ** 3, 'voxels_evaluated': [r[1] for r in rows],
-             'voxels_total': res ** 3, 'growth_rounds': st['growth_rounds'], 'bytes_exchanged': [r[2:] for r in rows],
-             'margin': tau}
-    return verts, tris, stats
-
-
-def _band_setup(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin):
-    """(device, evaluators | None, quirk period, tau) of extract_mesh_narrowband for this decoder."""
-    from .utils.reconstruction import _band_evaluators, default_margin
-    device = next(decoder.parameters()).device
-    fns = _band_evaluators(decoder, encoding, device)
-    quirk_period = 0 if (fns is None or decoder.training or fns[1] is None) else int(nbatch_points)
-    tau = default_margin(mini, maxi, resolution, block) if margin is None else float(margin)
-    return device, fns, quirk_period, tau
-
-
-def _run_band(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin, slab_plan, pick, exchange, return_stats):
-    from . import _native
-    from .utils.reconstruction import _device_mesh
-    res = int(resolution)
-    device, fns, quirk_period, tau = _band_setup(decoder, encoding, mini, maxi, res, nbatch_points, block, margin)
-    if fns is None:
-        raise ValueError('extract_mesh_narrowband_slabs: the decoder has no native band query on %s' % device)
-    with torch.no_grad(), torch.cuda.device(device):
-        slabs = [None if l1 <= l0 else _native.NarrowBandSlab(res, block, l0, l1, device) for l0, l1 in pick(slab_plan)]
-        verts, tris, stats = narrowband_slabs_mesh(slabs, fns[0], mini, maxi, res, block, tau, exchange, quirk_period, fns[1],
-                                                   device=device)
-        mesh = None if verts is None else _device_mesh(verts, tris, mini, maxi, res)
-    stats['slabs'] = slab_plan
-    return (mesh, stats) if return_stats else mesh
-
-
 def extract_mesh_narrowband_sharded(decoder, encoding, mini, maxi, resolution, nbatch_points=100000, block=4, margin=None, group=None,
                                     return_stats=False):
     """:func:`nphm_b200.utils.reconstruction.extract_mesh_narrowband` over the ranks of ``group``, one x-slab of block layers
@@ -503,15 +344,6 @@ def extract_mesh_narrowband_sharded(decoder, encoding, mini, maxi, resolution, n
                     lambda plan: [plan[rank]], GroupExchange(device, group), True)
     mesh, stats = out if rank == 0 else (None, None)
     return (mesh, stats) if return_stats else mesh
-
-
-def extract_mesh_narrowband_slabs(decoder, encoding, mini, maxi, resolution, world: int, nbatch_points=100000, block=4, margin=None,
-                                  return_stats=False):
-    """What :func:`extract_mesh_narrowband_sharded` computes on ``world`` ranks, with every slab on the decoder's device in this
-    process (:class:`LocalExchange`): the protocol of every rank in lockstep, on one GPU."""
-    res = int(resolution)
-    return _run_band(decoder, encoding, mini, maxi, res, nbatch_points, block, margin, plan_block_slabs(res, block, world),
-                     lambda plan: plan, LocalExchange(world), return_stats)
 
 
 def _dense_sharded(decoder, encoding, mini, maxi, res, nbatch_points, group, device, return_stats):

@@ -6,6 +6,8 @@
 """
 from __future__ import annotations
 
+from typing import Callable, List, Optional, Tuple
+
 import numpy as np
 import torch
 
@@ -97,39 +99,168 @@ def default_margin(mini, maxi, resolution, block=4):
     return float(block * np.linalg.norm(h))
 
 
-def narrowband_volume(evaluate, mini, maxi, resolution, device, block=4, margin=None, quirk_period=0, evaluate_quirk=None):
-    """The band of :func:`extract_mesh_narrowband` for any ``evaluate(points (n, 3) float32 CUDA) -> values (n,)``.
+def plan_block_slabs(res: int, block: int, world: int) -> List[Tuple[int, int]]:
+    """Block layers [l0, l1) of each rank: the ceil((res-1)/block) layers split as evenly as possible (first ranks get the extra),
+    so that every slab boundary is a block face; ranks past the number of layers get an empty range."""
+    n_layers = -(-(int(res) - 1) // int(block))
+    base, extra = divmod(n_layers, world)
+    out, c = [], 0
+    for r in range(world):
+        n = base + (1 if r < extra else 0)
+        out.append((c, c + n))
+        c += n
+    return out
 
-    Evaluates the block corners, then every voxel of the blocks with a corner ``|sdf| <= margin`` or a sign change, grows the band
+
+class LocalExchange:
+    """Every slab of one grid, driven by this process in rank order: planes move between the entries of the slab list and the
+    collectives reduce over it.  Lets one process (one device, or the CPU oracle) run the protocol of every rank in lockstep;
+    with one slab it is the one-GPU band, and nothing moves."""
+
+    def __init__(self, n_slabs: int):
+        self.ranks = list(range(n_slabs))
+
+    def swap(self, sends, expects, nbytes):
+        """sends[i] = (buffer to the lower, to the upper neighbour) of slab i; expects[i] = (from the lower, from the upper)."""
+        return [(sends[i - 1][1] if lo else None, sends[i + 1][0] if hi else None) for i, (lo, hi) in enumerate(expects)]
+
+    def any(self, counts) -> bool:
+        return any(c > 0 for c in counts)
+
+    def rows(self, rows):
+        return [list(r) for r in rows]
+
+    def counts(self, counts):
+        return list(counts)
+
+    def gather(self, parts, counts):
+        if len(parts) == 1:                            # one slab: its mesh as it is, without a device copy
+            return parts[0]
+        return torch.cat([v for v, _ in parts]), torch.cat([t for _, t in parts])
+
+
+def narrowband_slab_volumes(slabs, evaluate, mini, maxi, tau: float, exchange, quirk_period: int = 0, evaluate_quirk=None):
+    """The band of :func:`extract_mesh_narrowband` on x-slabs for any ``evaluate(points (n, 3) float32 CUDA) -> values (n,)``.
+    ``slabs``: the slabs this process drives (:class:`_native.NarrowBand`, or None for a rank without block layers), in the order
+    of ``exchange.ranks``.
+
+    Evaluates the block corners, then every voxel of the blocks with a corner ``|sdf| <= tau`` or a sign change, grows the band
     until no evaluated face voxel of an inactive block disagrees with that block's fill, and fills the rest.  ``quirk_period > 0``:
     the voxels ``g % p == p - 1`` and ``g == res^3 - 1`` go to ``evaluate_quirk`` instead, and the blocks around them are active.
-    Returns ``(volume (res, res, res) float32 CUDA, stats, band)`` with ``band`` the :class:`_native.NarrowBand` (block states)."""
+    Every round: list, gather / evaluate / scatter, swap the planes shared with the neighbours, growth check, and ask the exchange
+    whether any slab listed anything.  After the last round: fill, then hand each slab its neighbour's filled ghost plane.
+    Returns ``(volumes, stats)``: one ``(n_planes, res, res)`` volume per slab (None for None), ``stats`` with ``growth_rounds``
+    and, per slab, ``blocks_active``, ``voxels_evaluated`` and ``bytes_sent`` (one entry per plane exchange)."""
     if quirk_period and evaluate_quirk is None:
-        raise ValueError('narrowband_volume: quirk_period > 0 needs evaluate_quirk')
+        raise ValueError('narrowband_slab_volumes: quirk_period > 0 needs evaluate_quirk')
+    vols = [None if s is None else s.volume() for s in slabs]
+    evaluated = [0] * len(slabs)
+    sent = [[] for _ in slabs]
+    nbytes = next((s.plane_bytes for s in slabs if s is not None), 0)
+
+    def run(ns, fn):
+        for i, (s, n) in enumerate(zip(slabs, ns)):
+            if n:
+                s.scatter(fn(s.gather(n, mini, maxi)).reshape(-1), vols[i])
+                evaluated[i] += n
+
+    def swap(plane_lo, plane_hi, ghost):
+        sends, expects = [], []
+        for s, v in zip(slabs, vols):
+            if s is None:
+                sends.append((None, None))
+                expects.append((False, False))
+                continue
+            lo, hi = s.l0 > 0, s.x1 < s.res - 1
+            sends.append((s.export(plane_lo(s), v) if lo and not ghost else None, s.export(plane_hi(s), v) if hi else None))
+            expects.append((lo, hi and not ghost))
+        got = exchange.swap(sends, expects, nbytes)
+        for i, (s, v) in enumerate(zip(slabs, vols)):
+            sent[i].append(sum(nbytes for b in sends[i] if b is not None))
+            if s is None:
+                continue
+            if got[i][0] is not None:
+                s.import_(s.x0 - 1 if ghost else s.x0, got[i][0], v)
+            if got[i][1] is not None:
+                s.import_(s.x1, got[i][1], v)
+
+    ns = [0 if s is None else s.begin(quirk_period) for s in slabs]
+    if quirk_period:
+        run(ns, evaluate_quirk)
+    run([0 if s is None else s.corners() for s in slabs], evaluate)
+    run([0 if s is None else s.classify(tau, v) for s, v in zip(slabs, vols)], evaluate)
+    swap(lambda s: s.x0, lambda s: s.x1, ghost=False)
+    rounds = 0
+    while True:
+        ns = [0 if s is None else s.grow(v) for s, v in zip(slabs, vols)]
+        if not exchange.any(ns):
+            break
+        rounds += 1
+        run(ns, evaluate)
+        swap(lambda s: s.x0, lambda s: s.x1, ghost=False)
+    for s, v in zip(slabs, vols):
+        if s is not None:
+            s.fill(v)
+    swap(None, lambda s: s.x1 - 1, ghost=True)
+    stats = {'growth_rounds': rounds, 'blocks_active': [0 if s is None else int(s.active_blocks) for s in slabs],
+             'voxels_evaluated': evaluated, 'bytes_sent': sent}
+    return vols, stats
+
+
+def _slab_mesh(slabs, vols, exchange, mc_count, mc_emit, device):
+    """mc_count -> exchange.counts -> mc_emit -> exchange.gather over the filled slab volumes: (verts, tris) in global index units,
+    ids as on one GPU, on rank 0 (None, None elsewhere)."""
+    local, params = [], []
+    for s, v in zip(slabs, vols):
+        if s is None:
+            local.append((0, 0))
+            params.append(None)
+            continue
+        nv, nt, p, ws = mc_count(v, 0.0, True, x_global0=s.first_plane, ghost_lo=s.ghost)
+        local.append((nv, nt))
+        params.append((p, ws))
+    counts = exchange.counts(local)
+    parts = []
+    for i, (s, v) in enumerate(zip(slabs, vols)):
+        if s is None:
+            parts.append((torch.empty(0, 3, dtype=torch.float64, device=device), torch.empty(0, 3, dtype=torch.int64, device=device)))
+            continue
+        base = sum(c[0] for c in counts[:exchange.ranks[i]])
+        parts.append(mc_emit(v, params[i][0], params[i][1], local[i][0], local[i][1], base))
+    return exchange.gather(parts, counts)
+
+
+def narrowband_slabs_mesh(slabs, evaluate, mini, maxi, res: int, block: int, tau: float, exchange, quirk_period: int = 0,
+                          evaluate_quirk=None, mc_count: Optional[Callable] = None, mc_emit: Optional[Callable] = None,
+                          device='cpu'):
+    """:func:`narrowband_slab_volumes` + the sharded marching cubes.  Returns ``(verts, tris, stats)`` with the mesh in global
+    index units on the process that holds rank 0 (None elsewhere) and ``stats`` for every rank of the grid.  ``mc_count`` /
+    ``mc_emit`` default to the CUDA kernels; tests inject CPU stand-ins, as for
+    :func:`nphm_b200.distributed.extract_mesh_sharded`."""
+    if mc_count is None or mc_emit is None:
+        mc_count, mc_emit = _native.marching_cubes_count, _native.marching_cubes_emit
+    vols, st = narrowband_slab_volumes(slabs, evaluate, mini, maxi, tau, exchange, quirk_period, evaluate_quirk)
+    verts, tris = _slab_mesh(slabs, vols, exchange, mc_count, mc_emit, device)
+    rows = exchange.rows([[a, e] + b for a, e, b in zip(st['blocks_active'], st['voxels_evaluated'], st['bytes_sent'])])
+    nb = -(-(res - 1) // block)
+    stats = {'blocks_active': [r[0] for r in rows], 'blocks_total': nb ** 3, 'voxels_evaluated': [r[1] for r in rows],
+             'voxels_total': res ** 3, 'growth_rounds': st['growth_rounds'], 'bytes_exchanged': [r[2:] for r in rows],
+             'margin': tau}
+    return verts, tris, stats
+
+
+def narrowband_volume(evaluate, mini, maxi, resolution, device, block=4, margin=None, quirk_period=0, evaluate_quirk=None):
+    """:func:`narrowband_slab_volumes` on the whole grid, one slab, for any ``evaluate(points (n, 3) float32 CUDA) -> values (n,)``
+    with ``tau = margin`` (default :func:`default_margin`).  Returns ``(volume (res, res, res) float32 CUDA, stats, band)`` with
+    ``band`` the :class:`_native.NarrowBand` (block states)."""
     res = int(resolution)
     tau = default_margin(mini, maxi, res, block) if margin is None else float(margin)
     band = _native.NarrowBand(res, block, device)
-    vol = torch.empty(res ** 3, device=device, dtype=torch.float32)
-
-    def run(n, fn):
-        if n:
-            band.scatter(fn(band.gather(n, mini, maxi)).reshape(-1), vol)
-        return n
-
-    evaluated = run(band.begin(int(quirk_period)), evaluate_quirk)
-    evaluated += run(band.corners(), evaluate)
-    evaluated += run(band.classify(tau, vol), evaluate)
-    rounds = 0
-    while True:
-        n = band.grow(vol)
-        if not n:
-            break
-        rounds += 1
-        evaluated += run(n, evaluate)
-    band.fill(vol)
-    stats = {'blocks_active': int(band.active_blocks), 'blocks_total': band.blocks_per_axis ** 3,
-             'voxels_evaluated': int(evaluated), 'voxels_total': res ** 3, 'growth_rounds': rounds, 'margin': tau}
-    return vol.view(res, res, res), stats, band
+    (vol,), st = narrowband_slab_volumes([band], evaluate, mini, maxi, tau, LocalExchange(1), quirk_period, evaluate_quirk)
+    stats = {'blocks_active': st['blocks_active'][0], 'blocks_total': band.blocks_per_axis ** 3,
+             'voxels_evaluated': st['voxels_evaluated'][0], 'voxels_total': res ** 3, 'growth_rounds': st['growth_rounds'],
+             'margin': tau}
+    return vol, stats, band
 
 
 def _band_evaluators(decoder, encoding, device):
@@ -172,8 +303,7 @@ def extract_mesh_narrowband(decoder, encoding, mini, maxi, resolution, nbatch_po
     other decoders and CPU devices take ``get_logits`` + ``mesh_from_logits``.  ``return_stats``: also return a dict with
     ``blocks_active``, ``voxels_evaluated`` and ``growth_rounds`` (and the totals and the margin used)."""
     from ..models.reconstruction import get_logits
-    device = next(decoder.parameters()).device
-    fns = _band_evaluators(decoder, encoding, device)
+    device, fns, quirk_period, tau = _band_setup(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin)
     if fns is None:
         grid = torch.from_numpy(create_grid_points_from_bounds(mini, maxi, resolution)).to(device, dtype=torch.float32)
         mesh = mesh_from_logits(get_logits(decoder, encoding, grid[None], nbatch_points=nbatch_points), mini, maxi, resolution)
@@ -181,11 +311,41 @@ def extract_mesh_narrowband(decoder, encoding, mini, maxi, resolution, nbatch_po
         stats = {'blocks_active': None, 'blocks_total': None, 'voxels_evaluated': n, 'voxels_total': n, 'growth_rounds': 0,
                  'margin': None}
         return (mesh, stats) if return_stats else mesh
-    evaluate, evaluate_quirk = fns
-    quirk_period = 0 if (decoder.training or evaluate_quirk is None) else int(nbatch_points)
     with torch.no_grad(), torch.cuda.device(device):
-        vol, stats, _ = narrowband_volume(evaluate, mini, maxi, resolution, device, block=block, margin=margin,
-                                          quirk_period=quirk_period, evaluate_quirk=evaluate_quirk)
-        v_dev, t_dev = _native.marching_cubes_device(vol, 0.0, negate=True)     # == mesh_from_logits' negation, bit for bit
-        mesh = _device_mesh(v_dev, t_dev, mini, maxi, resolution)
+        vol, stats, band = narrowband_volume(fns[0], mini, maxi, resolution, device, block=block, margin=tau,
+                                             quirk_period=quirk_period, evaluate_quirk=fns[1])
+        verts, tris = _slab_mesh([band], [vol], LocalExchange(1), _native.marching_cubes_count, _native.marching_cubes_emit, device)
+        mesh = _device_mesh(verts, tris, mini, maxi, resolution)
     return (mesh, stats) if return_stats else mesh
+
+
+def _band_setup(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin):
+    """(device, evaluators | None, quirk period, tau) of extract_mesh_narrowband for this decoder."""
+    device = next(decoder.parameters()).device
+    fns = _band_evaluators(decoder, encoding, device)
+    quirk_period = 0 if (fns is None or decoder.training or fns[1] is None) else int(nbatch_points)
+    tau = default_margin(mini, maxi, resolution, block) if margin is None else float(margin)
+    return device, fns, quirk_period, tau
+
+
+def _run_band(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin, slab_plan, pick, exchange, return_stats):
+    res = int(resolution)
+    device, fns, quirk_period, tau = _band_setup(decoder, encoding, mini, maxi, res, nbatch_points, block, margin)
+    if fns is None:
+        raise ValueError('extract_mesh_narrowband_slabs: the decoder has no native band query on %s' % device)
+    with torch.no_grad(), torch.cuda.device(device):
+        slabs = [None if l1 <= l0 else _native.NarrowBandSlab(res, block, l0, l1, device) for l0, l1 in pick(slab_plan)]
+        verts, tris, stats = narrowband_slabs_mesh(slabs, fns[0], mini, maxi, res, block, tau, exchange, quirk_period, fns[1],
+                                                   device=device)
+        mesh = None if verts is None else _device_mesh(verts, tris, mini, maxi, res)
+    stats['slabs'] = slab_plan
+    return (mesh, stats) if return_stats else mesh
+
+
+def extract_mesh_narrowband_slabs(decoder, encoding, mini, maxi, resolution, world: int, nbatch_points=100000, block=4, margin=None,
+                                  return_stats=False):
+    """What :func:`nphm_b200.distributed.extract_mesh_narrowband_sharded` computes on ``world`` ranks, with every slab on the
+    decoder's device in this process (:class:`LocalExchange`): the protocol of every rank in lockstep, on one GPU."""
+    res = int(resolution)
+    return _run_band(decoder, encoding, mini, maxi, res, nbatch_points, block, margin, plan_block_slabs(res, block, world),
+                     lambda plan: plan, LocalExchange(world), return_stats)

@@ -1,6 +1,6 @@
 """Numpy restatement of one x-slab of the narrow band (``nphm_band_slab_*`` in csrc/narrowband.cu, DESIGN §4.16), with the
-interface of ``nphm_b200._native.NarrowBandSlab``, so that the real host driver (``nphm_b200.distributed``) runs on it without a
-GPU.  "Gathering" a voxel yields its global flat index; the tests evaluate it by reading a dense volume, as oracle/band_oracle.py
+interface of ``nphm_b200._native.NarrowBand``, so that the real host driver (``nphm_b200.utils.reconstruction``) runs on it
+without a GPU.  "Gathering" a voxel yields its global flat index; the tests evaluate it by reading a dense volume, as oracle/band_oracle.py
 does for the whole grid."""
 import numpy as np
 import torch
@@ -155,7 +155,7 @@ class OracleSlab:
 
 
 def oracle_slabs(res, block, world):
-    from nphm_b200.distributed import plan_block_slabs
+    from nphm_b200.utils.reconstruction import plan_block_slabs
     return [None if l1 <= l0 else OracleSlab(res, block, l0, l1) for l0, l1 in plan_block_slabs(res, block, world)]
 
 

@@ -181,8 +181,8 @@ def test_error_paths(cuda_device, head):
     from nphm_b200.utils.reconstruction import extract_mesh_narrowband, narrowband_volume
     dec, lat = head
     L = _native.lib()
-    assert L.nphm_band_workspace_bytes(1, 4) == -1 and L.nphm_band_workspace_bytes(64, 0) == -1
-    assert L.nphm_band_workspace_bytes(1025, 4) == -1 and L.nphm_band_workspace_bytes(64, 65) == -1
+    assert L.nphm_band_slab_workspace_bytes(1, 4, 0, 1) == -1 and L.nphm_band_slab_workspace_bytes(64, 0, 0, 16) == -1
+    assert L.nphm_band_slab_workspace_bytes(1025, 4, 0, 256) == -1 and L.nphm_band_slab_workspace_bytes(64, 65, 0, 1) == -1
     with pytest.raises(_native.NativeError):
         extract_mesh_narrowband(dec, lat, MINI, MAXI, 32, margin=-1.0)
     with pytest.raises(_native.NativeError):
@@ -191,10 +191,10 @@ def test_error_paths(cuda_device, head):
         extract_mesh_narrowband(dec, lat, MINI, MAXI, 32, block=0)
     with pytest.raises(ValueError):
         narrowband_volume(lambda p: p[:, 0], MINI, MAXI, 32, cuda_device, quirk_period=10)
-    need = L.nphm_band_workspace_bytes(32, 4)
+    need = L.nphm_band_slab_workspace_bytes(32, 4, 0, 8)
     ws = torch.empty(need - 1, device=cuda_device, dtype=torch.uint8)
     counts = (c_longlong * 2)()
     stream = torch.cuda.current_stream(cuda_device).cuda_stream
-    assert L.nphm_band_begin(32, 4, 0, ws.data_ptr(), ws.numel(), counts, stream) == -4          # NPHM_ERR_CAPACITY
-    assert L.nphm_band_begin(32, 4, -1, ws.data_ptr(), need, counts, stream) == -1               # negative quirk period
-    assert L.nphm_band_begin(32, 4, 0, None, need, counts, stream) == -1                         # no workspace
+    assert L.nphm_band_slab_begin(32, 4, 0, 8, 0, ws.data_ptr(), ws.numel(), counts, stream) == -4     # NPHM_ERR_CAPACITY
+    assert L.nphm_band_slab_begin(32, 4, 0, 8, -1, ws.data_ptr(), need, counts, stream) == -1          # negative quirk period
+    assert L.nphm_band_slab_begin(32, 4, 0, 8, 0, None, need, counts, stream) == -1                    # no workspace

@@ -87,7 +87,7 @@ def test_npm_deepsdf_slabs_equal_single_gpu_band(cuda_device, world):
 
 def _slab_run(evaluate, res, block, tau, world, dev, quirk_period=0, evaluate_quirk=None, lo=MINI, hi=MAXI):
     from nphm_b200 import _native
-    from nphm_b200.distributed import LocalExchange, narrowband_slab_volumes, plan_block_slabs
+    from nphm_b200.utils.reconstruction import LocalExchange, narrowband_slab_volumes, plan_block_slabs
     slabs = [None if l1 <= l0 else _native.NarrowBandSlab(res, block, l0, l1, dev) for l0, l1 in plan_block_slabs(res, block, world)]
     vols, stats = narrowband_slab_volumes(slabs, evaluate, lo, hi, tau, LocalExchange(world), quirk_period, evaluate_quirk)
     return slabs, vols, stats
@@ -98,8 +98,8 @@ def test_thin_plate_across_slabs(cuda_device, world):
     """The analytic plate spanning the x axis: the band grows along it through the slab boundaries, and every slab's filled
     volume (ghost plane included) and block states are the single-grid band's."""
     from nphm_b200 import _native
-    from nphm_b200.distributed import LocalExchange, narrowband_slabs_mesh, plan_block_slabs
-    from nphm_b200.utils.reconstruction import create_grid_points_from_bounds, narrowband_volume
+    from nphm_b200.utils.reconstruction import (LocalExchange, create_grid_points_from_bounds, narrowband_slabs_mesh,
+                                                narrowband_volume, plan_block_slabs)
     res, block = 65, 4
     lo, hi = [-1.0] * 3, [1.0] * 3
     h = 2.0 / (res - 1)
@@ -173,13 +173,12 @@ def test_error_paths(cuda_device):
     from ctypes import c_longlong
     from nphm_b200 import _native
     L = _native.lib()
-    assert L.nphm_band_slab_workspace_bytes(65, 4, 0, 16) == L.nphm_band_workspace_bytes(65, 4)
     for l0, l1 in ((3, 3), (5, 4), (-1, 2), (0, 17)):
         assert L.nphm_band_slab_workspace_bytes(65, 4, l0, l1) == -1
         with pytest.raises(_native.NativeError):
             _native.NarrowBandSlab(65, 4, l0, l1, cuda_device)
     need = L.nphm_band_slab_workspace_bytes(65, 4, 4, 8)
-    assert 0 < need < L.nphm_band_workspace_bytes(65, 4)
+    assert 0 < need < L.nphm_band_slab_workspace_bytes(65, 4, 0, 16)
     ws = torch.empty(need, device=cuda_device, dtype=torch.uint8)
     counts = (c_longlong * 2)()
     stream = torch.cuda.current_stream(cuda_device).cuda_stream

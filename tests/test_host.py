@@ -200,7 +200,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), name
     lib.nphm_abi_version.restype = ctypes.c_int
-    assert lib.nphm_abi_version() == 1
+    assert lib.nphm_abi_version() == 2
 
 
 def test_stack_supported_agrees_with_nphm_mlp_create():

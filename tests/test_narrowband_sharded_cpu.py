@@ -1,4 +1,4 @@
-"""The narrow band on x-slabs (nphm_b200.distributed.narrowband_slabs_mesh) with the numpy restatement of the slab steps
+"""The narrow band on x-slabs (nphm_b200.utils.reconstruction.narrowband_slabs_mesh) with the numpy restatement of the slab steps
 (narrowband_slab_common.OracleSlab): for every world size, the mesh, the block states, the evaluated voxels and the filled
 volume are the single-grid oracle's (oracle/band_oracle.py), in process and through gloo."""
 import os
@@ -21,7 +21,7 @@ def _tau(h, block=4):
 
 
 def _run(dense, block, tau, world, quirk_period=0, exchange=None, slabs=None):
-    from nphm_b200.distributed import LocalExchange, narrowband_slabs_mesh
+    from nphm_b200.utils.reconstruction import LocalExchange, narrowband_slabs_mesh
     res = dense.shape[0]
     flat = dense.reshape(-1)
     ref = BO.band_volume(dense, block=block, tau=tau, quirk_period=quirk_period)
@@ -72,7 +72,7 @@ class _NoBoundaryExchange:
     neighbour evaluated."""
 
     def __init__(self, world):
-        from nphm_b200.distributed import LocalExchange
+        from nphm_b200.utils.reconstruction import LocalExchange
         self.inner = LocalExchange(world)
         self.ranks = self.inner.ranks
 
@@ -101,7 +101,7 @@ def test_growth_crosses_slab_boundaries():
     _check_against_oracle(dense, ref, slabs, verts, tris, stats)
     # without the boundary exchange the slabs miss blocks the single grid activates: growth did cross a boundary
     slabs2 = oracle_slabs(65, 4, 5)
-    from nphm_b200.distributed import narrowband_slab_volumes
+    from nphm_b200.utils.reconstruction import narrowband_slab_volumes
     flat = dense.reshape(-1)
     ev = lambda idx: torch.from_numpy(flat[idx.numpy()])               # noqa: E731
     narrowband_slab_volumes(slabs2, ev, None, None, _tau(h), _NoBoundaryExchange(5))
@@ -130,7 +130,7 @@ def test_world_larger_than_block_layers():
 
 
 @pytest.mark.parametrize('period', [33 * 33, 8 * 33 * 33 + 1, 97])
-@pytest.mark.parametrize('world', [2, 3, 5])
+@pytest.mark.parametrize('world', [1, 2, 3, 5])
 def test_quirk_voxels_on_boundary_planes(period, world):
     """period res^2: the quirk voxels are the last voxel of every plane, so every shared plane holds one; period 8 res^2 + 1: the
     k-th lies on plane 8k, a block face; both ranks around a boundary list it and activate their blocks around it."""
@@ -164,7 +164,8 @@ def _gloo_worker(rank, world, port, q):
     os.environ['MASTER_PORT'] = str(port)
     dist.init_process_group('gloo', rank=rank, world_size=world)
     try:
-        from nphm_b200.distributed import GroupExchange, narrowband_slabs_mesh, plan_block_slabs
+        from nphm_b200.distributed import GroupExchange
+        from nphm_b200.utils.reconstruction import narrowband_slabs_mesh, plan_block_slabs
         dense, h = _plate_along_x(49)
         period = 49 * 49
         g = np.union1d(np.arange(period - 1, 49 ** 3, period), [49 ** 3 - 1])

@@ -60,8 +60,8 @@ def main():
 def run(args, dev, rank, world):
     from conftest import MAXI, MINI, make_ensemble, sample_latent
     from narrowband_common import make_npm_head
-    from nphm_b200.distributed import extract_mesh_narrowband_sharded, extract_mesh_narrowband_slabs
-    from nphm_b200.utils.reconstruction import extract_mesh_narrowband
+    from nphm_b200.distributed import extract_mesh_narrowband_sharded
+    from nphm_b200.utils.reconstruction import extract_mesh_narrowband, extract_mesh_narrowband_slabs
     for name in args.decoders:
         if name == 'nphm':
             dec, lat = make_ensemble(0, device=dev).eval(), sample_latent(1).to(dev)
