@@ -507,6 +507,66 @@ int nphm_band_slab_import(int res, int block, int l0, int l1, int plane, const u
                           void *workspace_dev, long long workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The same steps with block-sparse storage (DESIGN §4.17): nothing is stored per grid voxel.  The workspace
+ * (>= nphm_band_sparse_workspace_bytes) holds a state byte and a u32 brick slot per block, a value and a mark per block corner,
+ * the two planes shared with neighbours and the ghost plane; the pool holds, for each of `slots` bricks, the (block+1)^3 values
+ * (vals, floats) and marks (marks) of one active block's voxels and that block (blocks, u32), plus the list and compaction scratch.
+ * nphm_band_sparse_pool_sizes gives, for `slots` bricks, {mark bytes, list entries, compaction chunks} (vals: slots (block+1)^3
+ * floats, blocks: slots u32); marks beyond the used bricks must be 0, and a grown pool keeps the used bricks' contents.
+ * The steps, gather / scatter and export / import behave as the nphm_band_slab_* steps of the same slab with the volume replaced by
+ * the workspace and pool: begin, corners, classify and grow write {voxels listed, blocks active so far, bricks used, bricks needed}
+ * to counts_host[0..3] (synchronises the stream).  When the pool is short, a listing step writes nothing past it and returns
+ * NPHM_ERR_CAPACITY with counts_host[3] the bricks needed; the caller grows the pool and repeats the same call.  fill writes
+ * nothing: a voxel not evaluated reads as corner 0 of its block wherever it is read.  nphm_band_sparse_volume writes the filled
+ * planes [x_first, x_first + n_planes) of [X0-1 (with a ghost plane) or X0, X1] to out_dev.  Needs 2 <= res <= 8192,
+ * 1 <= block <= 64, (blocks+1)^3 < 2^32 and slots (block+1)^3 < 2^32: corner, block and list indices are u32. */
+typedef struct {
+    float *vals;
+    unsigned char *marks;
+    unsigned *blocks, *list, *chunk_cnt, *chunk_off;
+    long long slots, marks_bytes, list_len, n_chunks;
+} nphm_band_pool;
+/* bytes of the sparse band workspace of the slab (-1: bad arguments) */
+long long nphm_band_sparse_workspace_bytes(int res, int block, int l0, int l1);
+int nphm_band_sparse_pool_sizes(int res, int block, int l0, int l1, long long slots, long long *sizes_host);
+int nphm_band_sparse_begin(int res, int block, int l0, int l1, long long quirk_period, void *workspace_dev, long long workspace_bytes,
+                           const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_corners(int res, int block, int l0, int l1, void *workspace_dev, long long workspace_bytes,
+                             const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_classify(int res, int block, int l0, int l1, float tau, void *workspace_dev, long long workspace_bytes,
+                              const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_grow(int res, int block, int l0, int l1, void *workspace_dev, long long workspace_bytes,
+                          const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_gather(int res, int block, int l0, int l1, const double grid_min[3], const double grid_max[3], long long n,
+                            float *xyz_dev, void *workspace_dev, long long workspace_bytes, const nphm_band_pool *pool, void *stream);
+int nphm_band_sparse_scatter(int res, int block, int l0, int l1, long long n, const float *values_dev, void *workspace_dev,
+                             long long workspace_bytes, const nphm_band_pool *pool, void *stream);
+int nphm_band_sparse_fill(int res, int block, int l0, int l1, void *workspace_dev, long long workspace_bytes,
+                          const nphm_band_pool *pool, void *stream);
+int nphm_band_sparse_block_states(int res, int block, int l0, int l1, const void *workspace_dev, long long workspace_bytes,
+                                  const nphm_band_pool *pool, unsigned char *states_dev, void *stream);
+int nphm_band_sparse_export(int res, int block, int l0, int l1, int plane, const void *workspace_dev, long long workspace_bytes,
+                            const nphm_band_pool *pool, unsigned char *buf_dev, void *stream);
+int nphm_band_sparse_import(int res, int block, int l0, int l1, int plane, const unsigned char *buf_dev, void *workspace_dev,
+                            long long workspace_bytes, const nphm_band_pool *pool, void *stream);
+int nphm_band_sparse_volume(int res, int block, int l0, int l1, int x_first, int n_planes, float *out_dev, const void *workspace_dev,
+                            long long workspace_bytes, const nphm_band_pool *pool, void *stream);
+/* Marching cubes on the bricks: the mesh nphm_mc_count / nphm_mc_emit give on the filled slab volume of planes X0-1 (with a ghost
+ * plane) or X0 .. X1 with x_global0 = that first plane, ghost_lo = (l0 > 0), negate = 1 and iso = 0 - the same counts, vertex ids,
+ * float64 positions and triangle order - reading only the bricks (and, with a ghost plane, it and plane X0).  Ids come from exclusive
+ * scans over the active blocks' cell rows in sweep order (DESIGN §4.17).  After the band's last step; mc_count reads back the
+ * counts (synchronises the stream), mc_emit (same workspace, after mc_count) writes n_verts x 3 doubles and n_tris x 3 ids
+ * (vert_id_base + the id within the slab; ids below vert_id_base belong to the ghost layer's vertices).  The workspace needs
+ * nphm_band_sparse_mc_workspace_bytes(res, block, l0, l1, pool->slots) bytes (NPHM_ERR_CAPACITY when short). */
+long long nphm_band_sparse_mc_workspace_bytes(int res, int block, int l0, int l1, long long slots);
+int nphm_band_sparse_mc_count(int res, int block, int l0, int l1, const void *workspace_dev, long long workspace_bytes,
+                              const nphm_band_pool *pool, void *mc_workspace_dev, long long mc_workspace_bytes, long long *n_verts_host,
+                              long long *n_tris_host, void *stream);
+int nphm_band_sparse_mc_emit(int res, int block, int l0, int l1, const void *workspace_dev, long long workspace_bytes,
+                             const nphm_band_pool *pool, void *mc_workspace_dev, long long mc_workspace_bytes, long long vert_id_base,
+                             double *verts_dev, long long *tris_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Training supervision (DESIGN §4.15): the sampling steps of scripts/data_processing/sample_surface.py:32-135 (stage 1) and
  * scripts/data_processing/sample_deformation_field.py:14-35 (stage 2).  Meshes are n_verts x 3 fp64 vertices and n_faces x 3 int32
  * faces, every index in [0, n_verts) - a PRECONDITION, not checked here (the Python layer checks it).  Samples are n x 3 fp64

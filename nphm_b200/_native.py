@@ -45,6 +45,10 @@ EXPORTED_SYMBOLS = (
     'nphm_band_slab_workspace_bytes', 'nphm_band_slab_begin', 'nphm_band_slab_corners', 'nphm_band_slab_gather',
     'nphm_band_slab_scatter', 'nphm_band_slab_classify', 'nphm_band_slab_grow', 'nphm_band_slab_fill', 'nphm_band_slab_block_states',
     'nphm_band_slab_export', 'nphm_band_slab_import',
+    'nphm_band_sparse_workspace_bytes', 'nphm_band_sparse_pool_sizes', 'nphm_band_sparse_begin', 'nphm_band_sparse_corners',
+    'nphm_band_sparse_classify', 'nphm_band_sparse_grow', 'nphm_band_sparse_gather', 'nphm_band_sparse_scatter',
+    'nphm_band_sparse_fill', 'nphm_band_sparse_block_states', 'nphm_band_sparse_export', 'nphm_band_sparse_import',
+    'nphm_band_sparse_volume', 'nphm_band_sparse_mc_workspace_bytes', 'nphm_band_sparse_mc_count', 'nphm_band_sparse_mc_emit',
     'nphm_face_cdf_workspace_bytes', 'nphm_face_cdf', 'nphm_sample_faces', 'nphm_vertex_normals_workspace_bytes',
     'nphm_vertex_normals', 'nphm_interpolate_barycentric', 'nphm_transfer_correspondences',
 )
@@ -75,6 +79,12 @@ class MlpConfig(Structure):
 class McParams(Structure):
     _fields_ = [('nx', c_int), ('ny', c_int), ('nz', c_int), ('x_global0', c_int), ('ghost_lo', c_int),
                 ('negate', c_int), ('iso', c_double)]
+
+
+class BandPool(Structure):
+    _fields_ = [('vals', c_void_p), ('marks', c_void_p), ('blocks', c_void_p), ('list', c_void_p), ('chunk_cnt', c_void_p),
+                ('chunk_off', c_void_p), ('slots', c_longlong), ('marks_bytes', c_longlong), ('list_len', c_longlong),
+                ('n_chunks', c_longlong)]
 
 
 class FitParams(Structure):
@@ -224,6 +234,26 @@ def lib() -> ctypes.CDLL:
     L.nphm_band_slab_block_states.argtypes = slab + [c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_band_slab_export.argtypes = slab + [c_int, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_band_slab_import.argtypes = slab + [c_int, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_sparse_workspace_bytes.argtypes = slab
+    L.nphm_band_sparse_workspace_bytes.restype = c_longlong
+    L.nphm_band_sparse_pool_sizes.argtypes = slab + [c_longlong, POINTER(c_longlong)]
+    mem = [c_void_p, c_longlong, POINTER(BandPool)]     # workspace, its bytes, the brick pool
+    listing = mem + [POINTER(c_longlong), c_void_p]
+    L.nphm_band_sparse_begin.argtypes = slab + [c_longlong] + listing
+    L.nphm_band_sparse_corners.argtypes = slab + listing
+    L.nphm_band_sparse_classify.argtypes = slab + [c_float] + listing
+    L.nphm_band_sparse_grow.argtypes = slab + listing
+    L.nphm_band_sparse_gather.argtypes = slab + [POINTER(c_double), POINTER(c_double), c_longlong, c_void_p] + mem + [c_void_p]
+    L.nphm_band_sparse_scatter.argtypes = slab + [c_longlong, c_void_p] + mem + [c_void_p]
+    L.nphm_band_sparse_fill.argtypes = slab + mem + [c_void_p]
+    L.nphm_band_sparse_block_states.argtypes = slab + mem + [c_void_p, c_void_p]
+    L.nphm_band_sparse_export.argtypes = slab + [c_int] + mem + [c_void_p, c_void_p]
+    L.nphm_band_sparse_import.argtypes = slab + [c_int, c_void_p] + mem + [c_void_p]
+    L.nphm_band_sparse_volume.argtypes = slab + [c_int, c_int, c_void_p] + mem + [c_void_p]
+    L.nphm_band_sparse_mc_workspace_bytes.argtypes = slab + [c_longlong]
+    L.nphm_band_sparse_mc_workspace_bytes.restype = c_longlong
+    L.nphm_band_sparse_mc_count.argtypes = slab + mem + [c_void_p, c_longlong, POINTER(c_longlong), POINTER(c_longlong), c_void_p]
+    L.nphm_band_sparse_mc_emit.argtypes = slab + mem + [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p]
     L.nphm_face_cdf_workspace_bytes.argtypes = [c_longlong]
     L.nphm_face_cdf_workspace_bytes.restype = c_longlong
     L.nphm_face_cdf.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, POINTER(c_double), c_void_p, c_longlong, c_void_p]
@@ -1049,3 +1079,192 @@ def NarrowBandSlab(res: int, block: int, l0: int, l1: int, device) -> NarrowBand
     """The :class:`NarrowBand` of the x-slab of block layers ``[l0, l1)``, in the argument order the callers of the multi-GPU band
     use."""
     return NarrowBand(res, block, device, l0, l1)
+
+
+NPHM_ERR_CAPACITY = -4
+
+
+class SparseNarrowBand:
+    """The band of :class:`NarrowBand` with block-sparse storage (``nphm_band_sparse_*``, DESIGN §4.17): per block a state byte and
+    a brick slot, per block corner a value, and a brick of ``(block+1)^3`` voxels for each active block only, in a pool that grows
+    between rounds.  Same steps and attributes as :class:`NarrowBand`; :meth:`volume` returns the band itself, the store every step
+    and :func:`sparse_marching_cubes_count` take, and :meth:`dense_volume` materialises the filled slab volume (small grids)."""
+
+    def __init__(self, res: int, block: int, device, l0: int = 0, l1: Optional[int] = None, slots: Optional[int] = None):
+        self.res, self.block = int(res), int(block)
+        self.device = torch.device(device)
+        self.blocks_per_axis = -(-(self.res - 1) // max(self.block, 1))
+        self.l0 = int(l0)
+        self.l1 = self.blocks_per_axis if l1 is None else int(l1)
+        self._geo = (self.res, self.block, self.l0, self.l1)
+        with torch.cuda.device(self.device):
+            self.ws = _workspace(lib().nphm_band_sparse_workspace_bytes(*self._geo), 'nphm_band_sparse_workspace_bytes', self.device)
+        self.active_blocks = 0
+        self.x0 = self.l0 * self.block
+        self.x1 = min(self.l1 * self.block, self.res - 1)
+        self.ghost = self.l0 > 0
+        self.first_plane = self.x0 - int(self.ghost)
+        self.n_planes = self.x1 + 1 - self.first_plane
+        self.plane_bytes = 5 * self.res * self.res
+        self.brick_voxels = (self.block + 1) ** 3
+        self.n_blocks = (self.l1 - self.l0) * self.blocks_per_axis ** 2
+        self.slots_used = 0
+        self.mc_bytes = 0                 # marching-cubes workspace of the last mesh
+        self.native_syncs = 0             # count read-backs (stream synchronisations) of the native calls so far
+        # list entries slot (block+1)^3 + local are u32: the pool never holds more bricks than that allows
+        self.max_slots = min(self.n_blocks, ((1 << 32) - 1) // self.brick_voxels)
+        # a surface crosses about as many blocks per layer as a layer has rows; the pool grows when the band needs more
+        self._pool_tensors = None
+        self._set_pool(min(self.max_slots, max(64, 4 * (self.l1 - self.l0) * self.blocks_per_axis)) if slots is None else int(slots))
+
+    def _set_pool(self, slots: int, keep: int = 0):
+        sizes = (c_longlong * 3)()
+        check(lib().nphm_band_sparse_pool_sizes(*self._geo, int(slots), sizes), 'nphm_band_sparse_pool_sizes')
+        marks_bytes, list_len, n_chunks = sizes[0], sizes[1], sizes[2]
+        V, dev = self.brick_voxels, self.device
+        old = self._pool_tensors
+        if old is not None:                # release the scratch of the old pool before allocating the new one
+            old = old[:3]
+            self._pool_tensors = None
+        vals = torch.empty(slots * V, device=dev, dtype=torch.float32)
+        marks = torch.zeros(marks_bytes, device=dev, dtype=torch.uint8)
+        blocks = torch.empty(max(slots, 1), device=dev, dtype=torch.int32)
+        if old is not None and keep:
+            vals[:keep * V].copy_(old[0][:keep * V])
+            marks[:keep * V].copy_(old[1][:keep * V])
+            blocks[:keep].copy_(old[2][:keep])
+        del old
+        lst = torch.empty(max(list_len, 1), device=dev, dtype=torch.int32)
+        cnt = torch.empty(n_chunks, device=dev, dtype=torch.int32)
+        off = torch.empty(n_chunks, device=dev, dtype=torch.int32)
+        self._pool_tensors = (vals, marks, blocks, lst, cnt, off)
+        self.pool = BandPool(vals.data_ptr() if slots else blocks.data_ptr(), marks.data_ptr(), blocks.data_ptr(), lst.data_ptr(),
+                             cnt.data_ptr(), off.data_ptr(), int(slots), marks_bytes, list_len, n_chunks)
+        self.slots = int(slots)
+
+    def device_bytes(self) -> int:
+        """Bytes the band holds on the device: workspace (block states and slots, corners, shared planes) and brick pool."""
+        return self.ws.numel() + sum(t.numel() * t.element_size() for t in self._pool_tensors)
+
+    def _mem(self):
+        return self.ws.data_ptr(), self.ws.numel(), byref(self.pool)
+
+    def _call(self, step, *args):
+        with torch.cuda.device(self.device):
+            check(getattr(lib(), 'nphm_band_sparse_' + step)(*self._geo, *args, _stream_ptr(self.device)), 'nphm_band_sparse_' + step)
+
+    def _call_listing(self, step, *before):
+        fn = getattr(lib(), 'nphm_band_sparse_' + step)
+        counts = (c_longlong * 4)()
+        with torch.cuda.device(self.device):
+            while True:
+                rc = fn(*self._geo, *before, *self._mem(), counts, _stream_ptr(self.device))
+                self.native_syncs += 1
+                if rc != NPHM_ERR_CAPACITY or counts[3] <= self.slots or counts[3] > self.max_slots:
+                    break
+                # the step wrote nothing past the pool and left the band as it was: grow the pool, keep the bricks, repeat
+                self._set_pool(min(self.max_slots, max(int(counts[3]), 2 * self.slots)), keep=int(counts[2]))
+            if rc == NPHM_ERR_CAPACITY and counts[3] > self.max_slots:
+                raise NativeError('nphm_band_sparse_%s: the band needs %d bricks of %d voxels; list entries are u32, so a pool holds at '
+                                  'most %d' % (step, counts[3], self.brick_voxels, self.max_slots))
+            check(rc, 'nphm_band_sparse_' + step)
+        self.active_blocks = counts[1]
+        self.slots_used = counts[2]
+        return counts[0]
+
+    def _own(self, vol):
+        if vol is not self:
+            raise ValueError('SparseNarrowBand: the volume of a sparse band is the band itself (volume())')
+
+    def begin(self, quirk_period: int = 0) -> int:
+        return self._call_listing('begin', int(quirk_period))
+
+    def corners(self) -> int:
+        return self._call_listing('corners')
+
+    def classify(self, tau: float, vol) -> int:
+        self._own(vol)
+        return self._call_listing('classify', float(tau))
+
+    def grow(self, vol) -> int:
+        self._own(vol)
+        return self._call_listing('grow')
+
+    def gather(self, n: int, mini, maxi) -> torch.Tensor:
+        xyz = torch.empty(int(n), 3, device=self.device, dtype=torch.float32)
+        gmin = (c_double * 3)(*[float(v) for v in mini])
+        gmax = (c_double * 3)(*[float(v) for v in maxi])
+        self._call('gather', gmin, gmax, int(n), _ptr(xyz) if n else None, *self._mem())
+        return xyz
+
+    def scatter(self, values: torch.Tensor, vol):
+        self._own(vol)
+        v = _f32c(values).reshape(-1)
+        self._call('scatter', v.numel(), v.data_ptr() if v.numel() else None, *self._mem())
+
+    def fill(self, vol):
+        self._own(vol)
+        self._call('fill', *self._mem())
+
+    def block_states(self) -> torch.Tensor:
+        nb = self.blocks_per_axis
+        out = torch.empty(self.l1 - self.l0, nb, nb, device=self.device, dtype=torch.uint8)
+        self._call('block_states', *self._mem(), out.data_ptr())
+        return out != 0
+
+    def volume(self):
+        return self
+
+    def planes(self, x_first: int, n_planes: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Filled planes ``[x_first, x_first + n_planes)`` of the slab (ghost plane included) as an (n, res, res) float32 tensor."""
+        if out is None:
+            out = torch.empty(int(n_planes), self.res, self.res, device=self.device, dtype=torch.float32)
+        self._call('volume', int(x_first), int(n_planes), out.data_ptr(), *self._mem())
+        return out
+
+    def dense_volume(self) -> torch.Tensor:
+        """The filled (n_planes, res, res) slab volume the dense band holds: res^3 floats for the whole grid (small grids only)."""
+        return self.planes(self.first_plane, self.n_planes)
+
+    def export(self, plane: int, vol, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        self._own(vol)
+        buf = torch.empty(self.plane_bytes, device=self.device, dtype=torch.uint8) if out is None else out
+        self._call('export', int(plane), *self._mem(), buf.data_ptr())
+        return buf
+
+    def import_(self, plane: int, buf: torch.Tensor, vol):
+        self._own(vol)
+        if buf.device != self.device or buf.dtype != torch.uint8 or buf.numel() != self.plane_bytes:
+            raise ValueError('SparseNarrowBand.import_: need a uint8 buffer of %d bytes on %s' % (self.plane_bytes, self.device))
+        self._call('import', int(plane), buf.data_ptr(), *self._mem())
+
+
+def sparse_marching_cubes_count(band: SparseNarrowBand, iso=0.0, negate=False, x_global0=0, ghost_lo=False):
+    """:func:`marching_cubes_count` of the filled slab volume of a sparse band (``nphm_band_sparse_mc_count``), reading only its
+    bricks: ``(n_verts, n_tris, None, workspace)`` for :func:`sparse_marching_cubes_emit`.  The band's volume is ``-sdf`` at 0, as
+    the narrow band extracts it: ``negate`` must be true and ``iso`` 0."""
+    if x_global0 != band.first_plane or bool(ghost_lo) != band.ghost:
+        raise ValueError('sparse_marching_cubes_count: the slab starts at plane %d (ghost plane: %s)' % (band.first_plane, band.ghost))
+    if not negate or float(iso) != 0.0:
+        raise ValueError('sparse_marching_cubes_count: the band extracts the 0 level set of -sdf (negate=True, iso=0)')
+    with torch.cuda.device(band.device):
+        ws = _workspace(lib().nphm_band_sparse_mc_workspace_bytes(*band._geo, band.slots), 'nphm_band_sparse_mc_workspace_bytes',
+                        band.device)
+        band.mc_bytes = ws.numel()
+        nv, nt = c_longlong(0), c_longlong(0)
+        band.native_syncs += 1
+        check(lib().nphm_band_sparse_mc_count(*band._geo, *band._mem(), ws.data_ptr(), ws.numel(), byref(nv), byref(nt),
+                                              _stream_ptr(band.device)), 'nphm_band_sparse_mc_count')
+    return nv.value, nt.value, None, ws
+
+
+def sparse_marching_cubes_emit(band: SparseNarrowBand, params, ws, n_verts: int, n_tris: int, vert_id_base: int):
+    """:func:`marching_cubes_emit` for :func:`sparse_marching_cubes_count`: (verts, tris) with the ids the whole volume gives."""
+    dev = band.device
+    verts = torch.empty(n_verts, 3, device=dev, dtype=torch.float64)
+    tris = torch.empty(n_tris, 3, device=dev, dtype=torch.int64)
+    if n_verts or n_tris:
+        with torch.cuda.device(dev):
+            check(lib().nphm_band_sparse_mc_emit(*band._geo, *band._mem(), ws.data_ptr(), ws.numel(), int(vert_id_base), verts.data_ptr(),
+                                                 tris.data_ptr(), _stream_ptr(dev)), 'nphm_band_sparse_mc_emit')
+    return verts, tris

@@ -328,20 +328,21 @@ class GroupExchange:
 
 
 def extract_mesh_narrowband_sharded(decoder, encoding, mini, maxi, resolution, nbatch_points=100000, block=4, margin=None, group=None,
-                                    return_stats=False):
+                                    return_stats=False, sparse=False):
     """:func:`nphm_b200.utils.reconstruction.extract_mesh_narrowband` over the ranks of ``group``, one x-slab of block layers
     each (:func:`plan_block_slabs`); every rank holds only its slab's planes.  Rank 0 returns the mesh, bit for bit the one
     ``extract_mesh_narrowband`` gives with the same arguments for any world size; the other ranks return None.  Decoders
     without a native band query take the dense sharded path (:func:`extract_mesh_sharded`, NCCL).  ``return_stats``: also a
     dict with the per-rank ``blocks_active``, ``voxels_evaluated`` and ``bytes_exchanged`` (bytes each rank sent per plane
-    exchange), ``growth_rounds``, the totals, the margin and the slab plan (rank 0; None elsewhere)."""
+    exchange), ``growth_rounds``, the totals, the margin and the slab plan (rank 0; None elsewhere).  ``sparse``: every rank keeps its
+    slab in block-sparse storage (DESIGN §4.17); the stats then give that rank's ``device_bytes``."""
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     res = int(resolution)
     device, fns, _, _ = _band_setup(decoder, encoding, mini, maxi, res, nbatch_points, block, margin)
     if fns is None:
         return _dense_sharded(decoder, encoding, mini, maxi, res, nbatch_points, group, device, return_stats)
     out = _run_band(decoder, encoding, mini, maxi, res, nbatch_points, block, margin, plan_block_slabs(res, block, world),
-                    lambda plan: [plan[rank]], GroupExchange(device, group), True)
+                    lambda plan: [plan[rank]], GroupExchange(device, group), True, sparse)
     mesh, stats = out if rank == 0 else (None, None)
     return (mesh, stats) if return_stats else mesh
 

@@ -249,13 +249,26 @@ def narrowband_slabs_mesh(slabs, evaluate, mini, maxi, res: int, block: int, tau
     return verts, tris, stats
 
 
-def narrowband_volume(evaluate, mini, maxi, resolution, device, block=4, margin=None, quirk_period=0, evaluate_quirk=None):
+def _band_class(sparse: bool):
+    return _native.SparseNarrowBand if sparse else _native.NarrowBand
+
+
+def _mc_pair(sparse: bool):
+    """(mc_count, mc_emit) of :func:`_slab_mesh` for the band's storage."""
+    if sparse:
+        return _native.sparse_marching_cubes_count, _native.sparse_marching_cubes_emit
+    return _native.marching_cubes_count, _native.marching_cubes_emit
+
+
+def narrowband_volume(evaluate, mini, maxi, resolution, device, block=4, margin=None, quirk_period=0, evaluate_quirk=None,
+                      sparse=False):
     """:func:`narrowband_slab_volumes` on the whole grid, one slab, for any ``evaluate(points (n, 3) float32 CUDA) -> values (n,)``
     with ``tau = margin`` (default :func:`default_margin`).  Returns ``(volume (res, res, res) float32 CUDA, stats, band)`` with
-    ``band`` the :class:`_native.NarrowBand` (block states)."""
+    ``band`` the :class:`_native.NarrowBand` (block states).  ``sparse``: the band is a :class:`_native.SparseNarrowBand` and
+    ``volume`` is the band's brick store (``band.dense_volume()`` materialises it)."""
     res = int(resolution)
     tau = default_margin(mini, maxi, res, block) if margin is None else float(margin)
-    band = _native.NarrowBand(res, block, device)
+    band = _band_class(sparse)(res, block, device)
     (vol,), st = narrowband_slab_volumes([band], evaluate, mini, maxi, tau, LocalExchange(1), quirk_period, evaluate_quirk)
     stats = {'blocks_active': st['blocks_active'][0], 'blocks_total': band.blocks_per_axis ** 3,
              'voxels_evaluated': st['voxels_evaluated'][0], 'voxels_total': res ** 3, 'growth_rounds': st['growth_rounds'],
@@ -291,7 +304,7 @@ def _band_evaluators(decoder, encoding, device):
 
 
 def extract_mesh_narrowband(decoder, encoding, mini, maxi, resolution, nbatch_points=100000, block=4, margin=None,
-                            return_stats=False):
+                            return_stats=False, sparse=False):
     """The mesh of ``mesh_from_logits(get_logits(decoder, encoding, grid, nbatch_points), mini, maxi, resolution)`` for the grid
     of ``create_grid_points_from_bounds(mini, maxi, resolution)``, with the decoder evaluated only in a band of ``block^3``-cell
     blocks around the surface (DESIGN §4.13): the same vertex ids, float64 positions and triangles whenever every piece of the
@@ -301,7 +314,11 @@ def extract_mesh_narrowband(decoder, encoding, mini, maxi, resolution, nbatch_po
     Takes ``FastEnsembleDeepSDFMirrored`` (honouring ``decoder.training`` like ``get_logits``: in eval mode the voxels of
     ``get_logits``' last-point-of-chunk quirk are evaluated with it) and one-output ``DeepSDF`` stacks on the native query;
     other decoders and CPU devices take ``get_logits`` + ``mesh_from_logits``.  ``return_stats``: also return a dict with
-    ``blocks_active``, ``voxels_evaluated`` and ``growth_rounds`` (and the totals and the margin used)."""
+    ``blocks_active``, ``voxels_evaluated`` and ``growth_rounds`` (and the totals and the margin used).
+
+    ``sparse=True`` keeps the band in block-sparse storage (DESIGN §4.17): device memory follows the active blocks instead of the
+    grid, for grids up to 6497 points per axis with 4^3-cell blocks (8192 with larger blocks), and the mesh and stats are the same; the stats then also give
+    ``device_bytes``, the band's workspace and brick pool and the largest marching-cubes chunk."""
     from ..models.reconstruction import get_logits
     device, fns, quirk_period, tau = _band_setup(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin)
     if fns is None:
@@ -313,9 +330,11 @@ def extract_mesh_narrowband(decoder, encoding, mini, maxi, resolution, nbatch_po
         return (mesh, stats) if return_stats else mesh
     with torch.no_grad(), torch.cuda.device(device):
         vol, stats, band = narrowband_volume(fns[0], mini, maxi, resolution, device, block=block, margin=tau,
-                                             quirk_period=quirk_period, evaluate_quirk=fns[1])
-        verts, tris = _slab_mesh([band], [vol], LocalExchange(1), _native.marching_cubes_count, _native.marching_cubes_emit, device)
+                                             quirk_period=quirk_period, evaluate_quirk=fns[1], sparse=sparse)
+        verts, tris = _slab_mesh([band], [vol], LocalExchange(1), *_mc_pair(sparse), device)
         mesh = _device_mesh(verts, tris, mini, maxi, resolution)
+    if sparse:
+        stats['device_bytes'] = _sparse_bytes(band)
     return (mesh, stats) if return_stats else mesh
 
 
@@ -328,24 +347,34 @@ def _band_setup(decoder, encoding, mini, maxi, resolution, nbatch_points, block,
     return device, fns, quirk_period, tau
 
 
-def _run_band(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin, slab_plan, pick, exchange, return_stats):
+def _sparse_bytes(band):
+    """Device bytes of a sparse band: {'band': workspace and brick pool, 'mc': the largest marching-cubes chunk}."""
+    return {'band': band.device_bytes(), 'mc': band.mc_bytes}
+
+
+def _run_band(decoder, encoding, mini, maxi, resolution, nbatch_points, block, margin, slab_plan, pick, exchange, return_stats,
+              sparse=False):
     res = int(resolution)
     device, fns, quirk_period, tau = _band_setup(decoder, encoding, mini, maxi, res, nbatch_points, block, margin)
     if fns is None:
         raise ValueError('extract_mesh_narrowband_slabs: the decoder has no native band query on %s' % device)
     with torch.no_grad(), torch.cuda.device(device):
-        slabs = [None if l1 <= l0 else _native.NarrowBandSlab(res, block, l0, l1, device) for l0, l1 in pick(slab_plan)]
+        slabs = [None if l1 <= l0 else _band_class(sparse)(res, block, device, l0, l1) for l0, l1 in pick(slab_plan)]
+        mc_count, mc_emit = _mc_pair(sparse)
         verts, tris, stats = narrowband_slabs_mesh(slabs, fns[0], mini, maxi, res, block, tau, exchange, quirk_period, fns[1],
-                                                   device=device)
+                                                   mc_count=mc_count, mc_emit=mc_emit, device=device)
         mesh = None if verts is None else _device_mesh(verts, tris, mini, maxi, res)
     stats['slabs'] = slab_plan
+    if sparse:
+        stats['device_bytes'] = [None if s is None else _sparse_bytes(s) for s in slabs]
     return (mesh, stats) if return_stats else mesh
 
 
 def extract_mesh_narrowband_slabs(decoder, encoding, mini, maxi, resolution, world: int, nbatch_points=100000, block=4, margin=None,
-                                  return_stats=False):
+                                  return_stats=False, sparse=False):
     """What :func:`nphm_b200.distributed.extract_mesh_narrowband_sharded` computes on ``world`` ranks, with every slab on the
-    decoder's device in this process (:class:`LocalExchange`): the protocol of every rank in lockstep, on one GPU."""
+    decoder's device in this process (:class:`LocalExchange`): the protocol of every rank in lockstep, on one GPU.  ``sparse``: each
+    slab in block-sparse storage, as in :func:`extract_mesh_narrowband` (``device_bytes`` per slab in the stats)."""
     res = int(resolution)
     return _run_band(decoder, encoding, mini, maxi, res, nbatch_points, block, margin, plan_block_slabs(res, block, world),
-                     lambda plan: plan, LocalExchange(world), return_stats)
+                     lambda plan: plan, LocalExchange(world), return_stats, sparse)
