@@ -51,7 +51,7 @@ struct nphm_ensemble {
     // tensor-core path (tc_ensemble.cu)
     nphm::DeviceBuffer tc_weights, tc_consts, tc_coff, tc_l2slabs;
     nphm::DeviceBuffer tc_masks, tc_sched;     // member mask per tile (pre-pass), work counter of the tile schedule
-    nphm::DeviceBuffer tc_absorb, tc_bounds;   // absorption: masks and weight exponents per tile, member bounds per query
+    nphm::DeviceBuffer tc_absorb, tc_bounds;   // absorption: masks per tile, member bounds per query
     long long tc_mask_tiles = 0;               // tiles whose masks the last launch computed (0: it computed none)
     bool tc_ready = false;
     bool tc_prune = false;          // opt-in member pruning (NPHM_IMPL_TC_PRUNED)

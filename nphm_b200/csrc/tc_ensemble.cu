@@ -353,9 +353,8 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     const char *absorb_env = std::getenv("NPHM_ENS_ABSORB");
     p.absorb = p.zero_skip && !q.xyz && q.n_points > 0 && !(absorb_env && absorb_env[0] == '0');
     if (p.absorb) {
-        if ((rc = h->tc_absorb.reserve((size_t)n_tiles * (sizeof(unsigned long long) + tc::kMaxMembers)))) return rc;
+        if ((rc = h->tc_absorb.reserve((size_t)n_tiles * sizeof(unsigned long long)))) return rc;
         p.absorb_masks = h->tc_absorb.as<unsigned long long>();
-        p.wexp = reinterpret_cast<uint8_t *>(p.absorb_masks + n_tiles);
         if ((rc = h->tc_bounds.reserve((size_t)q.n_queries * h->n_members * sizeof(float)))) return rc;
         tc::member_bound_kernel<<<grid, 256, 0, stream>>>(
             h->weights.W[0].as<float>(), h->weights.W[1].as<float>(), h->weights.W[2].as<float>(), h->weights.W[3].as<float>(),

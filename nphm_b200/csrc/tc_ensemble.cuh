@@ -80,12 +80,10 @@ struct Params {
     // work counter of the on-demand tile schedule: [0] next work item, [1] CTAs finished; zero between launches
     unsigned int *sched;
     // dense grid queries: also skip the members whose blend terms fp32 rounding absorbs (tc_ensemble_wgmma.cu).  The pre-pass
-    // writes per tile the members with den + w == den at every valid point (absorb_masks) and per member a power-of-two bound
-    // of the tile's largest weight (wexp[tile][kMaxMembers]: exponent field, 0 = all weights zero); member_bound_kernel writes
+    // writes per tile the members with den + w == den at every valid point (absorb_masks); member_bound_kernel writes
     // B >= |s_k| per (query, member) (bounds, +inf: never skipped)
     int absorb;
     unsigned long long *absorb_masks;
-    uint8_t *wexp;
     const float *bounds;
 };
 
@@ -160,9 +158,6 @@ __device__ __forceinline__ float weight_sum(const float *anc, int n_members, flo
     for (int k = 0; k < n_members; ++k) S += member_weight(anc, k, n_members, x, y, z);
     return S;
 }
-
-// A power of two above the tile's largest weight, from its Params::wexp byte (the exponent field + 1; 0: all weights +0)
-__device__ __forceinline__ float weight_bound(uint32_t e) { return e ? __uint_as_float(e << 23) : 0.f; }
 
 int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream);
 

@@ -5,7 +5,7 @@
 //
 // A CTA is persistent over 128-point tiles: two consumer warpgroups of 64 points each and one producer warpgroup, which
 // hands most of its registers to the consumers (setmaxnreg: 24 / 240 per thread).
-//   producer (warp 8, one lane): bulk async copies of the record of every member and of its 8 weight units (tc_ensemble.cuh)
+//   producer (warps 8-11; one thread unless the warpgroup decides an absorption): bulk async copies of the record of every member and of its 8 weight units (tc_ensemble.cuh)
 //       into a ring of 4 shared-memory slots (one mbarrier pair each), up to 4 units ahead of the consumers.  A slot is
 //       released when the MMAs of both warpgroups on it have retired.
 //   consumers (warps 0-7): per member, layer 0 on CUDA cores straight into registers; layers 1-3 as 64 x N x 16 wgmmas with
@@ -24,8 +24,8 @@
 // pre-pass (tile_mask_kernel) computes which members each tile needs (dense: a blend weight that is not exactly zero at
 // some valid point; pruned: the tau rule) and the producer streams only those; grid queries use compact tiles
 // (Params::tbx, tby, tbz) so that a tile lies far from many anchors.  Dense grid queries also skip the members whose blend
-// terms fp32 rounding absorbs (the producer decides, see there); the producer tells the consumers which member each record
-// slot holds and ends a tile with a record slot without a copy.
+// terms fp32 rounding absorbs (the producer warpgroup decides per point, see there); the producer tells the consumers which member
+// each record slot holds and ends a tile with a record slot without a copy.
 #include "tc_ensemble.cuh"
 
 namespace nphm {
@@ -44,9 +44,11 @@ __device__ long long g_ens_trace[1 + kTraceMembers * kTraceStride];
 // the producer knows the tile's mask, warpgroup 0 has the layer-1 weights of the tile's first member.
 constexpr int kTraceTiles = 4;
 __device__ long long g_ens_tiles[3 * kTraceTiles];
-// Work of every CTA: [0] = CTAs of the last launch, then per CTA the member-tiles it evaluated and its cycles.
-constexpr int kTraceMaxCtas = 1024;
-__device__ long long g_ens_ctas[1 + 2 * kTraceMaxCtas];
+// Work of every CTA: [0] = CTAs of the last launch, then per CTA the member-tiles it evaluated, its cycles, its tiles, the
+// producer's cycles from the first wait of an absorption candidate to its decision (summed) and the part of them spent
+// waiting for the consumers' |num|.
+constexpr int kTraceMaxCtas = 1024, kTraceCtaWords = 5;
+__device__ long long g_ens_ctas[1 + kTraceCtaWords * kTraceMaxCtas];
 #define ENS_STAMP(member, off) do { const int mi_ = (int)(member) - kTraceFirst;                                           \
         if (blockIdx.x == 0 && mi_ >= 0 && mi_ < kTraceMembers) g_ens_trace[1 + mi_ * kTraceStride + (off)] = clock64(); } while (0)
 #define ENS_CEVT(member, phase, e) do { if ((threadIdx.x & 127) == 0)                                                       \
@@ -78,9 +80,9 @@ struct __align__(128) Smem {
     long long q_item[2];
     // producer -> consumers: the member whose record a record slot holds, -1 = the tile has no more members
     int rec_member[kRecSlots];
-    // consumers -> producer (absorption): per consumer warp, min |num| over its valid points after the member of record
-    // position r (in pub_min[r % 4]), then pub_seq = r + 1
-    float pub_min[4][kConsumerWarps];
+    // consumers -> producer (absorption): per tile row, |num| after the member of record position r in pub_num[r % 4][row];
+    // then the consumer warp that owns the row (rows 16 warp .. 16 warp + 15) sets pub_seq[warp] = r + 1
+    float pub_num[4][128];
     unsigned int pub_seq[kConsumerWarps];
 };
 static_assert(sizeof(Smem) <= 227 * 1024, "shared memory of the ensemble kernel exceeds the 227 KB of an H100 block");
@@ -120,6 +122,19 @@ __device__ __forceinline__ void to_operand(const float (&d)[N], int j, int col0,
 __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t *a) { return *reinterpret_cast<const volatile uint32_t *>(a); }
 __device__ __forceinline__ float ld_volatile_f32(const float *a) { return *reinterpret_cast<const volatile float *>(a); }
 
+// Named barrier of the 128 producer threads (warps 8-11).  The non-aligned barrier.cta forms: the lead thread of warp 8 may
+// reach them after the rest of its warp.
+constexpr int kProducerBar = 3;
+__device__ __forceinline__ void producer_sync() { asm volatile("barrier.cta.sync %0, 128;" ::"n"(kProducerBar) : "memory"); }
+// true when v holds on every producer thread
+__device__ __forceinline__ bool producer_all(bool v)
+{
+    uint32_t r;
+    asm volatile("{\n\t.reg .pred pv, pr;\n\tsetp.ne.u32 pv, %1, 0;\n\tbarrier.cta.red.and.pred pr, %2, 128, pv;\n\t"
+                 "selp.u32 %0, 1, 0, pr;\n}" : "=r"(r) : "r"((uint32_t)v), "n"(kProducerBar) : "memory");
+    return r != 0;
+}
+
 // Mask pre-pass: one warp per tile, 4 rows per lane; bit k of p.tile_masks[tile] is set when the tile needs member k.  The
 // last, global member is always needed: every tile evaluates >= 1 member.  Dense rule: a member is needed if w_k != 0 at some
 // valid point - a member with w_k = +0 everywhere adds exactly nothing to num and den (denormal weights count as nonzero).
@@ -149,7 +164,6 @@ __global__ void __launch_bounds__(32 * kMaskWarps) tile_mask_kernel(const Params
     float den[4] = {0.f, 0.f, 0.f, 0.f};
     for (int k = 0; k < p.n_members; ++k) {
         bool need = false, kept = false;
-        uint32_t wmax = 0;                       // bits of the largest valid weight (non-negative floats order as integers)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             if (!pt[i].valid) continue;
@@ -158,15 +172,10 @@ __global__ void __launch_bounds__(32 * kMaskWarps) tile_mask_kernel(const Params
             if (absorb) {
                 kept |= den[i] + w != den[i];
                 den[i] += w;
-                wmax = max(wmax, __float_as_uint(w));
             }
         }
         if (k < p.n_members - 1 && __any_sync(0xffffffffu, need)) mask |= 1ull << k;
-        if (absorb) {
-            if (!__any_sync(0xffffffffu, kept)) absorbed |= 1ull << k;
-            wmax = __reduce_max_sync(0xffffffffu, wmax);
-            if (lane == 0) p.wexp[tile * kMaxMembers + k] = wmax ? (uint8_t)((wmax >> 23) + 1) : 0;
-        }
+        if (absorb && !__any_sync(0xffffffffu, kept)) absorbed |= 1ull << k;
     }
     if (lane == 0) {
         p.tile_masks[tile] = mask;
@@ -214,87 +223,137 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     if (warp >= kConsumerWarps) {
         // =========================================================================== producer (tiles, bulk async copies)
         asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
-        if (warp == kConsumerWarps && lane == 0) {
+        {
+            // thread 0 of the producer warpgroup (lead) takes the tiles, waits on the barriers and issues the copies; the
+            // whole warpgroup decides absorption, thread `prow` for tile row prow, as in tile_mask_kernel
+            const int prow = threadIdx.x - 32 * kConsumerWarps;
+            const bool lead = prow == 0;
             uint32_t rcount = 0;
+#ifdef NPHM_ENS_TRACE
+            long long t_decide = 0, t_wait = 0;  // cycles from a candidate's first wait to its decision, of them waiting
+#endif
             for (uint32_t tcount = 0;; ++tcount) {
-                // take the next work item and pass it on with its member mask (the end of the work as item -1)
-                const unsigned int item = atomicAdd(p.sched, 1u);
-                const bool more = item < n_items;
+                // take the next work item and pass it on (the end of the work as item -1), also to the other producer threads
+                const int qs = tcount & 1;
+                if (lead) {
+                    const unsigned int item = atomicAdd(p.sched, 1u);
+                    ENS_TILE(tcount, 1);
+                    mbar_wait(&sm.q_empty[qs], ((tcount >> 1) & 1) ^ 1);
+                    sm.q_item[qs] = item < n_items ? (long long)item : -1;
+                    mbar_arrive(&sm.q_full[qs]);
+                }
+                __syncwarp();
+                producer_sync();
+                // q_item[qs] is rewritten two tiles later, after every producer thread has passed the next tile's sync
+                const long long qitem = sm.q_item[qs];
+                if (qitem < 0) {
+#ifdef NPHM_ENS_TRACE
+                    if (lead && blockIdx.x < kTraceMaxCtas) {
+                        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x + 2] = tcount;
+                        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x + 3] = t_decide;
+                        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x + 4] = t_wait;
+                    }
+#endif
+                    break;
+                }
+                const unsigned int item = (unsigned int)qitem;
                 const unsigned int tile = ACTS ? item / n_groups : item;
                 const int qi = p.blocked ? 0 : (int)(tile / (unsigned int)tiles_per_query);
-                unsigned long long mask = !more ? 0ull : (premask ? p.tile_masks[tile] : group_mask(item));
-                ENS_TILE(tcount, 1);
-                const int qs = tcount & 1;
-                mbar_wait(&sm.q_empty[qs], ((tcount >> 1) & 1) ^ 1);
-                sm.q_item[qs] = more ? (long long)item : -1;
-                mbar_arrive(&sm.q_full[qs]);
-                if (!more) break;
-                // absorption: skip member m when den + w == den at every valid point (pre-pass) and w * |s| < ulp(|num|) / 4
-                // there, so that fmaf(w, s, num) returns num: max w <= wb (pre-pass), |s| <= B (member_bound_kernel) and
-                // |num| >= L = min |num| after the member two record positions back (published by the consumer warps before
-                // they retire that member's successor's layer 2, i.e. before this lane could issue the previous member's
-                // last unit) - wb * B of the member in between, rounded down.  Deterministic: the lane waits for that state.
+                unsigned long long mask = premask ? p.tile_masks[tile] : group_mask(item);
+                // absorption: skip member m when den + w == den at every valid point (pre-pass) and, at every valid point p
+                // with w_m(p) != 0, w_m(p) * B_m < ulp(L(p)) / 4 (so that fmaf(w, s, num) returns num), with |s_m| <= B_m
+                // (member_bound_kernel) and |num(p)| >= L(p) = |num(p)| after the member two record positions back
+                // (published by the consumer warps before they retire that member's successor's layer 2, i.e. before the
+                // lead could issue the previous member's last unit) - w(p) * B of the member in between, rounded down.
+                // Deterministic: each thread waits for that state of its row.  w_m(p) is member_weight(), bit for bit the
+                // blend's weight.  The decision is a barrier reduction over the 128 producer threads.
                 const unsigned long long amask = absorb ? p.absorb_masks[tile] : 0ull;
+                const float *anc = p.anchors + (size_t)qi * (p.n_members - 1) * 3;
+                float px = 0.f, py = 0.f, pz = 0.f;
+                float lag = 0.f;                         // w * B of the member at record position rcount - 1, rounded up
+                bool pvalid = false;
+                if (amask) {
+                    const TilePoint t = tile_point(p, p.blocked, tile, qi, tiles_per_query, prow);
+                    px = t.x; py = t.y; pz = t.z; pvalid = t.valid;
+                }
                 const uint32_t rc0 = rcount;
-                float last_bound = 0.f;                  // wb * B of the member at record position rcount - 1, rounded up
                 for (; mask; mask &= mask - 1) {         // the tile's members in ascending order
                     const int m = __ffsll((long long)mask) - 1;
-                    const float bound = absorb ? __fmul_ru(weight_bound(p.wexp[(size_t)tile * kMaxMembers + m]),
-                                                           p.bounds[(size_t)qi * p.n_members + m]) : 0.f;
-                    if (((amask >> m) & 1) && rcount >= rc0 + 2) {
-                        const int ps = (rcount - 2) & 3;
-                        float mn = INFINITY;
-                        for (int w = 0; w < kConsumerWarps; ++w) {
-                            while (ld_volatile_u32(&sm.pub_seq[w]) < rcount - 1) { }
-                            __threadfence_block();
-                            mn = fminf(mn, ld_volatile_f32(&sm.pub_min[ps][w]));
-                        }
-                        const float L = __fsub_rd(mn, last_bound);
+                    const float bm = amask ? p.bounds[(size_t)qi * p.n_members + m] : 0.f;
+                    float wb = -1.f;                     // w_m * B_m of this row, rounded up, once computed
+                    if (((amask >> m) & 1) && rcount >= rc0 + 2 && bm < INFINITY) {
+#ifdef NPHM_ENS_TRACE
+                        const long long t0 = clock64();
+#endif
+                        // the consumer warp of row prow: rows 16 w .. 16 w + 15
+                        while (ld_volatile_u32(&sm.pub_seq[prow >> 4]) < rcount - 1) { }
+                        __threadfence_block();
+#ifdef NPHM_ENS_TRACE
+                        const long long t1 = clock64();
+#endif
+                        const float w = member_weight(anc, m, p.n_members, px, py, pz);
+                        wb = __fmul_ru(w, bm);
+                        const float L = __fsub_rd(ld_volatile_f32(&sm.pub_num[(rcount - 2) & 3][prow]), lag);
                         // ulp(L) / 4 = 2^(e(L) - 25), exact for L >= 2^-100; NaN and smaller L never certify
-                        if (L >= 0x1p-100f && bound < __uint_as_float(((__float_as_uint(L) >> 23) - 25) << 23)) continue;
+                        const bool ok = !pvalid || w == 0.f ||
+                                        (L >= 0x1p-100f && wb < __uint_as_float(((__float_as_uint(L) >> 23) - 25) << 23));
+                        const bool skip = producer_all(ok);
+#ifdef NPHM_ENS_TRACE
+                        if (lead) { const long long t2 = clock64(); t_decide += t2 - t0; t_wait += t1 - t0; }
+#endif
+                        if (skip) continue;
                     }
-                    last_bound = bound;
-                    const int rslot = rcount % kRecSlots;
-                    mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
-                    sm.rec_member[rslot] = m;
-                    mbar_expect_tx(&sm.rec_full[rslot], kRecFloats * 4);
-                    bulk_g2s(sm.rec[rslot], p.recs + ((size_t)qi * p.n_members + m) * kRecFloats, kRecFloats * 4, &sm.rec_full[rslot]);
-                    ++rcount;
-                    const int set = m < 2 * p.n_symm ? (m >> 1) : m - p.n_symm;
-                    const uint8_t *w = p.weights + (size_t)set * kSetBytes;
-                    const uint8_t *l2 = p.l2_slabs + ((size_t)qi * p.n_members + m) * kL2SlabBytes;
+                    // a later member is a candidate: the lag term of this one
+                    if ((amask >> m) >> 1) lag = wb >= 0.f ? wb : __fmul_ru(member_weight(anc, m, p.n_members, px, py, pz), bm);
+                    if (lead) {
+                        const int rslot = rcount % kRecSlots;
+                        mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
+                        sm.rec_member[rslot] = m;
+                        mbar_expect_tx(&sm.rec_full[rslot], kRecFloats * 4);
+                        bulk_g2s(sm.rec[rslot], p.recs + ((size_t)qi * p.n_members + m) * kRecFloats, kRecFloats * 4, &sm.rec_full[rslot]);
+                        const int set = m < 2 * p.n_symm ? (m >> 1) : m - p.n_symm;
+                        const uint8_t *w = p.weights + (size_t)set * kSetBytes;
+                        const uint8_t *l2 = p.l2_slabs + ((size_t)qi * p.n_members + m) * kL2SlabBytes;
 #pragma unroll 1
-                    for (int u = 0; u < kUnits; ++u) {
-                        // every member has 8 units, so unit u always goes to slot u % 4, on its (u / 4)-th use per member
-                        const int slot = u & 3;
-                        const uint32_t bytes = unit_bytes(u);
-                        ENS_PEVT(rcount - 1, 8 + u);
-                        mbar_wait(&sm.w_empty[slot], ((u >> 2) & 1) ^ 1);
-                        ENS_PEVT(rcount - 1, u);
-                        mbar_expect_tx(&sm.w_full[slot], bytes);
-                        if (u == 2 || u == 3) {
-                            // layer 2: the last k-step slab carries this (query, member)'s bias row (l2_slab_kernel)
-                            const uint32_t last = unit_nw(u) * 64;
-                            bulk_g2s(sm.wbuf[slot], w + unit_off(u), bytes - last, &sm.w_full[slot]);
-                            bulk_g2s(sm.wbuf[slot] + (bytes - last), l2 + (u == 3 ? kL2SlabABytes : 0), last, &sm.w_full[slot]);
-                        } else {
-                            bulk_g2s(sm.wbuf[slot], w + unit_off(u), bytes, &sm.w_full[slot]);
+                        for (int u = 0; u < kUnits; ++u) {
+                            // every member has 8 units, so unit u always goes to slot u % 4, on its (u / 4)-th use per member
+                            const int slot = u & 3;
+                            const uint32_t bytes = unit_bytes(u);
+                            ENS_PEVT(rcount, 8 + u);
+                            mbar_wait(&sm.w_empty[slot], ((u >> 2) & 1) ^ 1);
+                            ENS_PEVT(rcount, u);
+                            mbar_expect_tx(&sm.w_full[slot], bytes);
+                            if (u == 2 || u == 3) {
+                                // layer 2: the last k-step slab carries this (query, member)'s bias row (l2_slab_kernel)
+                                const uint32_t last = unit_nw(u) * 64;
+                                bulk_g2s(sm.wbuf[slot], w + unit_off(u), bytes - last, &sm.w_full[slot]);
+                                bulk_g2s(sm.wbuf[slot] + (bytes - last), l2 + (u == 3 ? kL2SlabABytes : 0), last, &sm.w_full[slot]);
+                            } else {
+                                bulk_g2s(sm.wbuf[slot], w + unit_off(u), bytes, &sm.w_full[slot]);
+                            }
                         }
                     }
+                    __syncwarp();
+                    ++rcount;
                 }
                 // the end of the tile's members: a record slot without a copy
-                const int rslot = rcount % kRecSlots;
-                mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
-                sm.rec_member[rslot] = -1;
-                mbar_arrive(&sm.rec_full[rslot]);
+                if (lead) {
+                    const int rslot = rcount % kRecSlots;
+                    mbar_wait(&sm.rec_empty[rslot], ((rcount / kRecSlots) & 1) ^ 1);
+                    sm.rec_member[rslot] = -1;
+                    mbar_arrive(&sm.rec_full[rslot]);
+                }
+                __syncwarp();
                 ++rcount;
             }
             // every CTA has taken its last item once all have counted themselves finished: the last one resets the counter
             // for the next launch on the stream
-            __threadfence();
-            if (atomicAdd(p.sched + 1, 1u) == gridDim.x - 1) {
-                atomicExch(p.sched, 0u);
-                atomicExch(p.sched + 1, 0u);
+            if (lead) {
+                __threadfence();
+                if (atomicAdd(p.sched + 1, 1u) == gridDim.x - 1) {
+                    atomicExch(p.sched, 0u);
+                    atomicExch(p.sched + 1, 0u);
+                }
             }
         }
         return;
@@ -603,12 +662,16 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                 if (!PRUNE) den[r] += w;
             }
             if (absorb) {
-                // publish min |num| over the warp's valid points for the producer's absorption decisions
-                float mn = fminf(valid[0] ? fabsf(num[0]) : INFINITY, valid[1] ? fabsf(num[1]) : INFINITY);
+                // publish |num| of the warp's rows for the producer's absorption decisions (rows without a valid point
+                // too: the producer passes them by itself); the rows are rl[0] and rl[1], recomputed from the warp
+                if (q4 == 0) {
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+                    for (int r = 0; r < 2; ++r)
+                        *reinterpret_cast<volatile float *>(&sm.pub_num[rcount & 3][16 * warp + (lane >> 2) + 8 * r]) = fabsf(num[r]);
+                    __threadfence_block();
+                }
+                __syncwarp();
                 if (lane == 0) {
-                    *reinterpret_cast<volatile float *>(&sm.pub_min[rcount & 3][warp]) = mn;
                     __threadfence_block();
                     *reinterpret_cast<volatile unsigned int *>(&sm.pub_seq[warp]) = rcount + 1;
                 }
@@ -623,8 +686,8 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     if (wgi == 0) take_turn();                   // the turn warpgroup 1 passed after its last phase
 #ifdef NPHM_ENS_TRACE
     if (threadIdx.x == 0 && blockIdx.x < kTraceMaxCtas) {
-        g_ens_ctas[1 + 2 * blockIdx.x] = n_eval;
-        g_ens_ctas[2 + 2 * blockIdx.x] = clock64() - cta_start;
+        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x] = n_eval;
+        g_ens_ctas[2 + kTraceCtaWords * blockIdx.x] = clock64() - cta_start;
     }
 #endif
 }
@@ -663,11 +726,11 @@ extern "C" int nphm_debug_ens_trace(long long *host, int n_ll)
 }
 
 // Tile boundaries of CTA 0 (3 stamps per tile, kTraceTiles tiles) followed by the work of every CTA ([0] = CTAs, then per
-// CTA member-tiles and cycles) of the last ensemble launch.
+// CTA member-tiles, cycles, tiles, decision cycles, decision wait cycles) of the last ensemble launch.
 extern "C" int nphm_debug_ens_work(long long *host, int n_ll)
 {
     using namespace nphm;
-    constexpr int nt = 3 * tc::wg::kTraceTiles, nc = 1 + 2 * tc::wg::kTraceMaxCtas;
+    constexpr int nt = 3 * tc::wg::kTraceTiles, nc = 1 + tc::wg::kTraceCtaWords * tc::wg::kTraceMaxCtas;
     NPHM_REQUIRE(n_ll == nt + nc, "nphm_debug_ens_work: bad length");
     NPHM_CUDA_CHECK(cudaDeviceSynchronize());
     NPHM_CUDA_CHECK(cudaMemcpyFromSymbol(host, tc::wg::g_ens_tiles, (size_t)nt * 8));

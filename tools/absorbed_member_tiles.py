@@ -11,15 +11,21 @@ zero-weight skip and the ones the certificate would remove on top:
   * B_k: a float64 interval bound of member k's output over the grid box (layer 0 with the latent folded, softplus with
     beta = 100, the latent-dependent layer-2 constant, the output layer), every pre-activation widened by a relative and an
     absolute slack, and at least 1 (quirk points blend 1.0);
-  * L: what a kernel can know when it decides on member k - the minimum of |num| over the tile after the member two
-    evaluated positions earlier, minus max_w * B of the member evaluated in between (max_w rounded up to a power of two).
+  * L: what a kernel can know when it decides on member k.  Two rules:
+    - per point (the kernel): at every valid point p with w_k(p) != +0, w_k(p) * B_k < ulp(L(p)) / 4 with
+      L(p) = |num(p)| after the member two evaluated positions earlier minus w(p) * B of the member evaluated in between,
+      rounded down (fp32 with directed rounding, as the kernel computes it); B_k finite; the first two evaluated members of
+      a tile are never certified (keys absorbed_point, evaluated_point);
+    - tile-wide (the kernel before per-point): the minimum of |num| over the tile after the member two evaluated positions
+      earlier, minus max_w * B of the member evaluated in between (max_w rounded up to a power of two), paired with the
+      tile's largest weight (keys absorbed, evaluated_absorb).
 num and den come from the fp32 member outputs of the CPU reference (tests/ensemble_f64_common.py).
 
     python tools/absorbed_member_tiles.py [--latent 1] [--res 64] [--scale 1] [--plane-stride 1]
 
 Every certified member is checked against the fp32 blend: the tool stops if one would change a bit of num or den.  It also
-prints what better-informed inputs would certify: L without the lag, with the tile's own max |s_k| for B_k, and the members that change
-no bit at all (what no tile-wide certificate can exceed).
+prints what better-informed inputs would certify: L without the lag (tile-wide and per point), with the tile's own max |s_k|
+for B_k, and the members that change no bit at all (what no certificate can exceed).
 """
 import argparse
 import os
@@ -93,6 +99,53 @@ def ulp32(x):
     return (np.nextafter(x, np.float32(np.inf)) - x).astype(np.float64)
 
 
+def f32_up(x):
+    """float64 -> the smallest float32 >= x."""
+    x = np.asarray(x, np.float64)
+    f = x.astype(np.float32)
+    return np.where(f.astype(np.float64) < x, np.nextafter(f, np.float32(np.inf)), f)
+
+
+def f32_down(x):
+    """float64 -> the largest float32 <= x."""
+    x = np.asarray(x, np.float64)
+    f = x.astype(np.float32)
+    return np.where(f.astype(np.float64) > x, np.nextafter(f, np.float32(-np.inf)), f)
+
+
+def fmul_ru(a, b):
+    """__fmul_ru of float32 operands: the product is exact in float64 (24 + 24 significant bits, no float64 underflow)."""
+    with np.errstate(invalid='ignore', over='ignore'):
+        return f32_up(np.asarray(a, np.float32).astype(np.float64) * np.asarray(b, np.float32).astype(np.float64))
+
+
+def fsub_rd(a, b):
+    """__fsub_rd of float32 operands: the float64 difference plus its exact error (TwoSum) gives the float64 round-down,
+    and rounding that down to float32 is the float32 round-down of the exact difference."""
+    a = np.asarray(a, np.float32).astype(np.float64)
+    b = -np.asarray(b, np.float32).astype(np.float64)
+    with np.errstate(invalid='ignore', over='ignore'):
+        s = a + b
+        bb = s - a
+        err = (a - (s - bb)) + (b - bb)
+        s = np.where(np.isfinite(s) & (err < 0), np.nextafter(s, -np.inf), s)
+    return f32_down(s)
+
+
+def point_pass(w, B, pub, lag, valid):
+    """The per-point rule of the kernel at each point (vectorised, float32 inputs): invalid points and w = +0 pass;
+    otherwise L = pub - lag rounded down must be >= 2^-100 and w * B rounded up < 2^(e(L) - 25) = ulp(L) / 4 (2^103 for
+    L = +inf).  pub = |num| two evaluated positions back, lag = w * B of the member in between rounded up, B = B_k as
+    float32."""
+    w = np.asarray(w, np.float32)
+    L = fsub_rd(pub, lag)
+    e = (L.view(np.uint32) >> 23).astype(np.int64) & 0xff
+    thr = np.ldexp(1.0, e - 152)
+    with np.errstate(invalid='ignore'):
+        ok = (L >= np.float32(2.0 ** -100)) & (fmul_ru(w, B).astype(np.float64) < thr)
+    return ~np.asarray(valid, bool) | (w == 0) | ok
+
+
 def absorbable(den, w, num_lo, wmax_bound, B):
     """The certificate (vectorised): den + w == den in float32, and wmax_bound * B < ulp(num_lo) / 4 with num_lo a lower
     bound of |num| (float64), wmax_bound >= w and B >= |s|.  When it holds, fmaf(w, s, num) == num and den + w == den."""
@@ -137,7 +190,9 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
         ix, iy, iz, valid = ix[keep], iy[keep], iz[keep], valid[keep]
     n_tiles = ix.shape[0]
     stats = {'tiles': int(n_tiles), 'member_tiles': int(n_tiles * M), 'zero': 0, 'den_absorbed': 0, 'absorbed': 0,
-             'absorbed_no_lag': 0, 'absorbed_tile_max': 0, 'unchanged': 0, 'B': B}
+             'absorbed_no_lag': 0, 'absorbed_tile_max': 0, 'unchanged': 0, 'B': B,
+             'absorbed_point': 0, 'absorbed_point_no_lag': 0}
+    B32 = f32_up(B)                                     # the kernel's B_k (member_bound_kernel rounds up; inf stays inf)
     gw = np.float32(np.exp(np.float32(-0.2) / np.float32(0.01)))
     for t0 in range(0, n_tiles, chunk_tiles):
         sl = slice(t0, min(n_tiles, t0 + chunk_tiles))
@@ -158,6 +213,10 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
         den = np.zeros((T, 128), np.float32)
         pub = [np.full(T, -np.inf), np.full(T, -np.inf)]      # min |num| after the last two evaluated members (none: -inf)
         last_bound = np.zeros(T)                             # max_w * B of the last evaluated member
+        # per-point rule: |num| after the last two evaluated members, w * B of the last one (rounded up), members evaluated
+        pp = [np.zeros((T, 128), np.float32), np.zeros((T, 128), np.float32)]
+        lag = np.zeros((T, 128), np.float32)
+        npos = np.zeros(T, np.int64)
         inf32 = np.float32(np.inf)
         for k in range(M):
             w = Wt[:, :, k]
@@ -175,6 +234,13 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
             new_num = (w.astype(np.float64) * s + num.astype(np.float64)).astype(np.float32)
             unchanged = den_abs & np.all(~V | (new_num == num), axis=1) & ~zero
             assert not np.any(cert & ~unchanged), 'the certificate passed a member that changes num'
+            cand = den_abs & ~zero & np.isfinite(B32[k])
+            cert_p = cand & (npos >= 2) & np.all(point_pass(w, B32[k], pp[0], lag, V), axis=1)
+            no_lag_p = cand & np.all(point_pass(w, B32[k], np.abs(num), np.float32(0), V), axis=1)
+            assert not np.any(cert_p & ~unchanged), 'the per-point rule passed a member that changes num'
+            stats['absorbed_point'] += int(cert_p.sum())
+            stats['absorbed_point_no_lag'] += int(no_lag_p.sum())
+            ev_p = ~(zero | cert_p)
             stats['zero'] += int(zero.sum())
             stats['den_absorbed'] += int((den_abs & ~zero).sum())
             stats['absorbed'] += int(cert.sum())
@@ -187,9 +253,14 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
             mn = np.where(V, np.abs(num), inf32).min(axis=1).astype(np.float64)
             pub = [np.where(ev, pub[1], pub[0]), np.where(ev, mn, pub[1])]
             last_bound = np.where(ev, wb * B[k], last_bound)
+            e2 = ev_p[:, None]
+            pp = [np.where(e2, pp[1], pp[0]), np.where(e2, np.abs(num), pp[1])]
+            lag = np.where(e2, fmul_ru(w, B32[k]), lag)
+            npos += ev_p
     n = stats['member_tiles']
     stats['evaluated_now'] = n - stats['zero']
     stats['evaluated_absorb'] = stats['evaluated_now'] - stats['absorbed']
+    stats['evaluated_point'] = stats['evaluated_now'] - stats['absorbed_point']
     return stats
 
 
@@ -216,13 +287,16 @@ def main():
     if args.plane_stride > 1:
         print('tiles of every %d-th x-plane' % args.plane_stride)
     print('latent %d, %d^3 grid: %d tiles, %d member-tiles, %d evaluated with the zero-weight skip; den half holds on %d '
-          '(%.1f %%), the full certificate on %d (%.1f %%) -> %d evaluated'
+          '(%.1f %%), the tile-wide rule (the kernel before per-point) on %d (%.1f %%) -> %d evaluated'
           % (args.latent, args.res, r['tiles'], r['member_tiles'], ev, r['den_absorbed'], 100 * r['den_absorbed'] / ev,
              r['absorbed'], 100 * r['absorbed'] / ev, r['evaluated_absorb']))
     print('with L = min |num_{k-1}| (no lag): %d (%.1f %%); no lag and the tile max of |s_k| for B_k: %d (%.1f %%); '
           'members that change no bit of num and den: %d (%.1f %%)'
           % (r['absorbed_no_lag'], 100 * r['absorbed_no_lag'] / ev, r['absorbed_tile_max'],
              100 * r['absorbed_tile_max'] / ev, r['unchanged'], 100 * r['unchanged'] / ev))
+    print('per point (the kernel): %d (%.1f %%) -> %d evaluated; per point without the lag: %d (%.1f %%)'
+          % (r['absorbed_point'], 100 * r['absorbed_point'] / ev, r['evaluated_point'], r['absorbed_point_no_lag'],
+             100 * r['absorbed_point_no_lag'] / ev))
     print('B_k: min %.3g, median %.3g, max %.3g' % (r['B'].min(), np.median(r['B']), r['B'].max()))
 
 

@@ -5,7 +5,8 @@ weights, issued and retired its MMAs and finished its epilogues, when the produc
 cycles waiting for weights, cycles in which neither warpgroup had MMAs in flight, epilogue cycles.  Then, per tile of CTA 0,
 when warpgroup 0 took it from the producer's queue, when the producer knew its member mask (before that, when negative) and
 when the first member's layer-1 weights were ready; over all CTAs the member-tiles the kernel evaluated (to set against
-tools/zero_member_tiles.py), the cycles per evaluated member-tile, and the spread of member-tiles and cycles per CTA.
+tools/zero_member_tiles.py and tools/absorbed_member_tiles.py), the cycles per evaluated member-tile, the spread of
+member-tiles and cycles per CTA, and the producer's cycles per tile from an absorption candidate's first wait to its decision.
 
     bash tools/build_variant.sh /tmp/ens -DNPHM_ENS_TRACE && NPHM_B200_LIB=/tmp/ens/libnphm_b200.so python tools/ens_trace.py [res]"""
 import ctypes, os, sys
@@ -16,7 +17,7 @@ import torch
 
 # layout of g_ens_trace, g_ens_tiles and g_ens_ctas (csrc/tc_ensemble_wgmma.cu)
 MEMBERS, WG, STRIDE = 4, 32, 2 * 32 + 16
-TILES, MAX_CTAS = 4, 1024
+TILES, MAX_CTAS, CTA_WORDS = 4, 1024, 5
 PHASES = ['L1', 'L2', 'L3a', 'L3b']
 EVENTS = ['wait', 'ready', 'turn', 'issued', 'retired', 'epi']
 
@@ -86,7 +87,7 @@ def main():
     print('mean per member: span %.0f, weight waits %.0f, no MMA in flight %.0f, epilogues %.0f' % tuple(tt))
     if not hasattr(lib, 'nphm_debug_ens_work'):
         return
-    buf = (ctypes.c_longlong * (3 * TILES + 1 + 2 * MAX_CTAS))()
+    buf = (ctypes.c_longlong * (3 * TILES + 1 + CTA_WORDS * MAX_CTAS))()
     _native.check(lib.nphm_debug_ens_work(buf, len(buf)), 'nphm_debug_ens_work')
     w = np.array(buf[:], dtype=np.int64)
     tiles = w[:3 * TILES].reshape(TILES, 3) - t0
@@ -95,13 +96,17 @@ def main():
         print('tile %d of CTA 0: taken from the queue at %d, mask known to the producer %+d, first member\'s layer-1 '
               'weights ready %+d%s' % (i, tiles[i, 0], tiles[i, 1] - tiles[i, 0], tiles[i, 2] - tiles[i, 0], length))
     n_ctas = int(w[3 * TILES])
-    ctas = w[3 * TILES + 1:3 * TILES + 1 + 2 * n_ctas].reshape(n_ctas, 2)
+    ctas = w[3 * TILES + 1:3 * TILES + 1 + CTA_WORDS * n_ctas].reshape(n_ctas, CTA_WORDS)
     mt, cyc = int(ctas[:, 0].sum()), int(ctas[:, 1].sum())
     print('all %d CTAs: %d member-tiles evaluated, %.0f cycles per evaluated member-tile (CTA cycles summed / member-tiles)'
           % (n_ctas, mt, cyc / max(mt, 1)))
     for col, name in ((0, 'member-tiles'), (1, 'cycles')):
         v = ctas[:, col].astype(np.float64)
         print('per CTA %s: min %.0f, mean %.0f, max %.0f, max / mean %.4f' % (name, v.min(), v.mean(), v.max(), v.max() / v.mean()))
+    # the producer's absorption decisions: from a candidate's first wait for the consumers' |num| to the warp's vote
+    tiles, decide, wait = int(ctas[:, 2].sum()), int(ctas[:, 3].sum()), int(ctas[:, 4].sum())
+    print('producer absorption decisions: %.0f cycles per tile (%.0f of them waiting for |num|), %.2f %% of the CTA cycles'
+          % (decide / max(tiles, 1), wait / max(tiles, 1), 100.0 * decide / max(cyc, 1)))
 
 
 if __name__ == '__main__':
