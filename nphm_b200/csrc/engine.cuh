@@ -53,6 +53,12 @@ struct nphm_ensemble {
     nphm::DeviceBuffer tc_masks, tc_sched;     // member mask per tile (pre-pass), work counter of the tile schedule
     nphm::DeviceBuffer tc_absorb, tc_bounds;   // absorption: masks per tile, member bounds per query
     long long tc_mask_tiles = 0;               // tiles whose masks the last launch computed (0: it computed none)
+    // debug view of the absorption decisions of the last launch (nphm_debug_ens_*): tiles with absorb masks (0: absorption
+    // was off), bounds written, tiles with a skip log; the skip log (members skipped by vote, per tile) only when enabled
+    long long tc_absorb_tiles = 0, tc_bound_count = 0, tc_skip_tiles = 0;
+    nphm::DeviceBuffer tc_skip_log;
+    bool tc_skip_log_on = false;
+    double tc_bound_scale = 1.0;               // factor on every member bound (1; a debug entry sets it for a negative control)
     bool tc_ready = false;
     bool tc_prune = false;          // opt-in member pruning (NPHM_IMPL_TC_PRUNED)
     float tc_prune_tau = 1e-8f;

@@ -133,7 +133,8 @@ __global__ void l2_slab_kernel(const uint8_t *__restrict__ weights, const float 
 // propagation (centre / radius) through layer 0 with the latent folded, the softplus (beta = 100) layers 1-3 with the
 // latent-dependent constants and the skip input of layer 2, and the output layer.  Every pre-activation interval grows by
 // kBoundRel * (|W| |h| + |b|) + kBoundAbs, which covers the kernel's 3-pass fp16 products, fp32 sums and approximate
-// softplus with a wide margin.  At least 1 (quirk points blend 1.0); +inf when the bound is not finite.
+// softplus with a wide margin.  At least 1 (quirk points blend 1.0); +inf when the bound is not finite.  `scale` multiplies
+// the bound (1 except for the negative control of nphm_debug_ens_bound_scale).
 constexpr double kBoundRel = 0x1p-10, kBoundAbs = 0x1p-10;
 __device__ __forceinline__ double softplus64(double x) { return fmax(x, 0.0) + log1p(exp(-100.0 * fabs(x))) / 100.0; }
 __global__ void __launch_bounds__(256) member_bound_kernel(const float *__restrict__ W0, const float *__restrict__ W1,
@@ -141,7 +142,8 @@ __global__ void __launch_bounds__(256) member_bound_kernel(const float *__restri
                                                            const float *__restrict__ W4, const float *__restrict__ cvec,
                                                            int cvec_stride, const int *__restrict__ coff,
                                                            const float *__restrict__ anchors, const float *__restrict__ axes,
-                                                           int res, int n_members, int n_symm, float *__restrict__ bounds)
+                                                           int res, int n_members, int n_symm, double scale,
+                                                           float *__restrict__ bounds)
 {
     const int m = blockIdx.x, qi = blockIdx.y, set = member_set(m, n_symm);
     const float *cv = cvec + ((size_t)qi * n_members + m) * cvec_stride;
@@ -194,7 +196,7 @@ __global__ void __launch_bounds__(256) member_bound_kernel(const float *__restri
     layer(W3 + (size_t)set * kH * kH, kH, kH, kH, 1.0, 3, true);
     layer(W4 + (size_t)set * kH, 1, kH, kH, 1.0, 4, false);
     if (threadIdx.x == 0) {
-        const double B = fmax(fabs(hc[0]) + hr[0], 1.0);
+        const double B = fmax(fabs(hc[0]) + hr[0], 1.0) * scale;
         bounds[(size_t)qi * n_members + m] = isfinite(B) ? __double2float_ru(B) : INFINITY;
     }
 }
@@ -343,6 +345,7 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
         }
     }
     h->tc_mask_tiles = 0;
+    h->tc_absorb_tiles = h->tc_bound_count = h->tc_skip_tiles = 0;
     if (prune || p.zero_skip) {
         if ((rc = h->tc_masks.reserve((size_t)n_tiles * sizeof(unsigned long long)))) return rc;
         p.tile_masks = h->tc_masks.as<unsigned long long>();
@@ -359,9 +362,17 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
         tc::member_bound_kernel<<<grid, 256, 0, stream>>>(
             h->weights.W[0].as<float>(), h->weights.W[1].as<float>(), h->weights.W[2].as<float>(), h->weights.W[3].as<float>(),
             h->weights.W[4].as<float>(), q.cvec, h->dims.cvec_stride, h->tc_coff.as<int>(), q.anchors, q.axes, q.res,
-            h->n_members, h->cfg.n_symm_pairs, h->tc_bounds.as<float>());
+            h->n_members, h->cfg.n_symm_pairs, h->tc_bound_scale, h->tc_bounds.as<float>());
         NPHM_CUDA_CHECK(cudaGetLastError());
         p.bounds = h->tc_bounds.as<float>();
+        h->tc_absorb_tiles = n_tiles;
+        h->tc_bound_count = (long long)q.n_queries * h->n_members;
+        if (h->tc_skip_log_on) {
+            if ((rc = h->tc_skip_log.reserve((size_t)n_tiles * sizeof(unsigned long long)))) return rc;
+            NPHM_CUDA_CHECK(cudaMemsetAsync(h->tc_skip_log.ptr, 0, (size_t)n_tiles * sizeof(unsigned long long), stream));
+            p.skip_log = h->tc_skip_log.as<unsigned long long>();
+            h->tc_skip_tiles = n_tiles;
+        }
     }
     // the kernel leaves the counter at zero when it ends; it starts at zero when allocated
     if (!h->tc_sched.ptr) {
@@ -390,6 +401,62 @@ extern "C" int nphm_debug_ens_tile_masks(nphm_ensemble *h, unsigned long long *h
     const long long n = std::min(cap, h->tc_mask_tiles);
     NPHM_CUDA_CHECK(cudaDeviceSynchronize());
     if (n > 0) NPHM_CUDA_CHECK(cudaMemcpy(host, h->tc_masks.ptr, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    return NPHM_OK;
+}
+
+// Debug entries (not part of the public ABI) on the absorption decisions of the handle's last tensor-core launch, in the
+// shape of nphm_debug_ens_tile_masks (*n receives the count, up to `cap` values are copied to `host`; 0 when that launch did
+// not skip absorbed members):
+//   nphm_debug_ens_bounds: the member bounds B, per query and member (float);
+//   nphm_debug_ens_absorb_masks: per tile, the members the pre-pass found den-absorbed at every valid point;
+//   nphm_debug_ens_skipped: per tile, the members the producer skipped by vote (launches made with the skip log enabled).
+// nphm_debug_ens_skip_log(h, 1) enables the skip log for the handle's later launches; nphm_debug_ens_bound_scale(h, f)
+// multiplies every later bound by f (1 by default; anything else may change the outputs: a negative control only).
+static int copy_debug(const nphm::DeviceBuffer &buf, size_t elem, long long count, void *host, long long cap, long long *n)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(n && cap >= 0 && (cap == 0 || host), "nphm_debug_ens_*: bad argument");
+    *n = count;
+    const long long k = std::min(cap, count);
+    NPHM_CUDA_CHECK(cudaDeviceSynchronize());
+    if (k > 0) NPHM_CUDA_CHECK(cudaMemcpy(host, buf.ptr, (size_t)k * elem, cudaMemcpyDeviceToHost));
+    return NPHM_OK;
+}
+
+extern "C" int nphm_debug_ens_bounds(nphm_ensemble *h, float *host, long long cap, long long *n)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h, "nphm_debug_ens_bounds: null handle");
+    return copy_debug(h->tc_bounds, sizeof(float), h->tc_bound_count, host, cap, n);
+}
+
+extern "C" int nphm_debug_ens_absorb_masks(nphm_ensemble *h, unsigned long long *host, long long cap, long long *n)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h, "nphm_debug_ens_absorb_masks: null handle");
+    return copy_debug(h->tc_absorb, sizeof(unsigned long long), h->tc_absorb_tiles, host, cap, n);
+}
+
+extern "C" int nphm_debug_ens_skipped(nphm_ensemble *h, unsigned long long *host, long long cap, long long *n)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h, "nphm_debug_ens_skipped: null handle");
+    return copy_debug(h->tc_skip_log, sizeof(unsigned long long), h->tc_skip_tiles, host, cap, n);
+}
+
+extern "C" int nphm_debug_ens_skip_log(nphm_ensemble *h, int enable)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h, "nphm_debug_ens_skip_log: null handle");
+    h->tc_skip_log_on = enable != 0;
+    return NPHM_OK;
+}
+
+extern "C" int nphm_debug_ens_bound_scale(nphm_ensemble *h, double factor)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h && factor > 0.0, "nphm_debug_ens_bound_scale: bad argument");
+    h->tc_bound_scale = factor;
     return NPHM_OK;
 }
 

@@ -85,6 +85,8 @@ struct Params {
     int absorb;
     unsigned long long *absorb_masks;
     const float *bounds;
+    // debug (nphm_debug_ens_skip_log): per tile, bit m set when the producer skipped member m by vote; nullptr unless enabled
+    unsigned long long *skip_log;
 };
 
 // One row (point) of a tile: its index in the query, its global point index, whether the tile covers a real point with

@@ -183,7 +183,8 @@ __global__ void __launch_bounds__(32 * kMaskWarps) tile_mask_kernel(const Params
     }
 }
 
-template <bool PRUNE, bool ACTS>
+// LOG: the debug skip log (Params::skip_log) - a variant of its own, so that the kernel without it is not slowed by it
+template <bool PRUNE, bool ACTS, bool LOG = false>
 __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Params p)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -301,7 +302,10 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
 #ifdef NPHM_ENS_TRACE
                         if (lead) { const long long t2 = clock64(); t_decide += t2 - t0; t_wait += t1 - t0; }
 #endif
-                        if (skip) continue;
+                        if (skip) {
+                            if (LOG && lead) atomicOr(p.skip_log + tile, 1ull << m);
+                            continue;
+                        }
                     }
                     // a later member is a candidate: the lag term of this one
                     if ((amask >> m) >> 1) lag = wb >= 0.f ? wb : __fmul_ru(member_weight(anc, m, p.n_members, px, py, pz), bm);
@@ -704,7 +708,8 @@ int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cu
     }
     const int smem = (int)sizeof(wg::Smem);
     auto kern = acts ? wg::ensemble_wgmma_kernel<false, true>
-                     : (prune ? wg::ensemble_wgmma_kernel<true, false> : wg::ensemble_wgmma_kernel<false, false>);
+                     : (prune ? wg::ensemble_wgmma_kernel<true, false>
+                              : (p.skip_log ? wg::ensemble_wgmma_kernel<false, false, true> : wg::ensemble_wgmma_kernel<false, false>));
     NPHM_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     kern<<<grid_x, wg::kThreads, smem, stream>>>(p);
     NPHM_CUDA_CHECK(cudaGetLastError());

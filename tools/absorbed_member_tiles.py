@@ -21,7 +21,12 @@ zero-weight skip and the ones the certificate would remove on top:
       tile's largest weight (keys absorbed, evaluated_absorb).
 num and den come from the fp32 member outputs of the CPU reference (tests/ensemble_f64_common.py).
 
-    python tools/absorbed_member_tiles.py [--latent 1] [--res 64] [--scale 1] [--plane-stride 1]
+    python tools/absorbed_member_tiles.py [--latent 1] [--res 64] [--scale 1] [--plane-stride 1] [--quirk-period 0]
+
+replay() is the per-point rule over a batch of tiles in torch (any device): predict() runs it on its own decisions, and
+tests/test_gpu_ensemble_absorb_replay.py on the decisions the kernel logged, with the kernel's weights, bounds and masks.
+fold_consts() restates how the GPU folds the latent into the layer constants, so that member_bound can take the inputs the
+kernel's bound has.
 
 Every certified member is checked against the fp32 blend: the tool stops if one would change a bit of num or den.  It also
 prints what better-informed inputs would certify: L without the lag (tile-wide and per point), with the tile's own max |s_k|
@@ -50,9 +55,10 @@ def softplus64(x):
     return np.where(bx > 20.0, x, np.log1p(np.exp(np.minimum(bx, 20.0))) / 100.0)
 
 
-def member_bound(P, m, z, anc, lo, hi):
+def member_bound(P, m, z, anc, lo, hi, consts=None):
     """B >= |s_m(x)| for every x in the box [lo, hi] (3,), as the kernel computes s_m: float64 interval propagation in
-    centre / radius form with REL_SLACK and ABS_SLACK per layer, at least 1.  inf when the bound is not finite."""
+    centre / radius form with REL_SLACK and ABS_SLACK per layer, at least 1.  inf when the bound is not finite.  consts: the
+    per-layer constants (latent folded, fold_consts) in place of the float64 fold - the inputs member_bound_kernel has."""
     from ensemble_f64_common import SQRT2
     s = P.weight_set(m)
     layers = [(W[s].double().numpy(), b[s].double().numpy()) for W, b in P.layers]
@@ -77,6 +83,8 @@ def member_bound(P, m, z, anc, lo, hi):
                 hc, hr = np.concatenate([hc, xc]), np.concatenate([hr, xr])
             else:
                 Wx, bias = W, b
+            if consts is not None:
+                bias = np.asarray(consts[l], np.float64)
             c = Wx @ hc + bias
             r = np.abs(Wx) @ hr + REL_SLACK * (np.abs(Wx) @ (np.abs(hc) + hr) + np.abs(bias)) + ABS_SLACK
             if l + 1 < len(layers):
@@ -146,6 +154,162 @@ def point_pass(w, B, pub, lag, valid):
     return ~np.asarray(valid, bool) | (w == 0) | ok
 
 
+def fmaf32(a, b, c):
+    """fp32 fmaf(a, b, c), correctly rounded: a * b is exact in float64 and TwoSum gives the error e of s = a * b + c, which
+    decides the one case where rounding s to float32 differs from rounding the exact sum (s halfway between two float32)."""
+    a, b, c = (np.asarray(t, np.float32).astype(np.float64) for t in (a, b, c))
+    p = a * b
+    s = p + c
+    bb = s - p
+    e = (p - (s - bb)) + (c - bb)
+    f = s.astype(np.float32)
+    fd = f.astype(np.float64)
+    up = np.nextafter(f, np.float32(np.inf))
+    dn = np.nextafter(f, np.float32(-np.inf))
+    f = np.where((s == (fd + up.astype(np.float64)) / 2) & (e > 0), up, f)
+    return np.where((s == (fd + dn.astype(np.float64)) / 2) & (e < 0), dn, f)
+
+
+def fold_consts(P32, z, m):
+    """The per-layer constants of member m as the GPU folds the latent into them (csrc/simt.cu cvec_kernel, fp32): for
+    layer 0 and the skip layer, fmaf(scale, sum_j W[n, K + j] u_j, b[n]) with the sum taken per lane of a warp (j = lane,
+    lane + 32, ... by fmaf) and reduced by the xor butterfly; the other layers' biases.  float32 arrays, one per layer."""
+    s_ = P32.weight_set(m)
+    zz = z.float().numpy()
+    u = np.concatenate([zz[:P32.G], zz[P32.G + m * P32.L:P32.G + (m + 1) * P32.L]]).astype(np.float32)
+    C = u.shape[0]
+    skip = P32.n_layers // 2
+    out = []
+    for l, (W, b) in enumerate(P32.layers):
+        W, b = W[s_].float().numpy(), b[s_].float().numpy()
+        if l not in (0, skip):
+            out.append(b)
+            continue
+        Wc = W[:, W.shape[1] - C:]
+        lanes = np.zeros((W.shape[0], 32), np.float32)
+        for j0 in range(0, C, 32):
+            n = min(32, C - j0)
+            lanes[:, :n] = fmaf32(Wc[:, j0:j0 + n], u[None, j0:j0 + n], lanes[:, :n])
+        for o in (16, 8, 4, 2, 1):
+            lanes = lanes + lanes[:, np.arange(32) ^ o]
+        scale = np.float32(1.0) if l == 0 else np.float32(1.0 / np.sqrt(2.0))
+        out.append(fmaf32(lanes[:, 0], scale, b))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ replay of the per-point rule
+# The producer's decisions, tile by tile, as torch tensors on any device (float64 arithmetic for the directed roundings).
+def _t_f32_up(x):
+    f = x.float()
+    return torch_mod().where(f.double() < x, torch_mod().nextafter(f, f.new_tensor(float('inf'))), f)
+
+
+def _t_f32_down(x):
+    f = x.float()
+    return torch_mod().where(f.double() > x, torch_mod().nextafter(f, f.new_tensor(float('-inf'))), f)
+
+
+def torch_mod():
+    import torch
+    return torch
+
+
+def t_fmul_ru(a, b):
+    """__fmul_ru of float32 tensors (the product is exact in float64)."""
+    return _t_f32_up(a.double() * b.double())
+
+
+def t_fsub_rd(a, b):
+    """__fsub_rd of float32 tensors (TwoSum in float64, then the float32 round-down), as fsub_rd."""
+    torch = torch_mod()
+    a, b = a.double(), -b.double()
+    s = a + b
+    bb = s - a
+    err = (a - (s - bb)) + (b - bb)
+    s = torch.where(torch.isfinite(s) & (err < 0), torch.nextafter(s, s.new_tensor(float('-inf'))), s)
+    return _t_f32_down(s)
+
+
+def t_point_pass(w, B, pub, lag, valid):
+    """point_pass on float32 tensors: invalid points and w = +0 pass; else L = pub - lag (rounded down) >= 2^-100 and
+    w * B (rounded up) < ulp(L) / 4 = 2^(e(L) - 25)."""
+    torch = torch_mod()
+    L = t_fsub_rd(pub, lag)
+    e = (L.view(torch.int32) >> 23) & 0xff
+    thr = torch.ldexp(torch.ones_like(L, dtype=torch.float64), (e - 152).double())
+    ok = (L >= 2.0 ** -100) & (t_fmul_ru(w, B).double() < thr)
+    return ~valid | (w == 0) | ok
+
+
+# relative error of the kernel's blend weight against the replay's (expf: 2 ulp; the squared distance, its root and the
+# quotient each round with 2^-24 relative and may contract differently; the exponent's absolute error is |ln w| times that)
+W_REL = 2.0 ** -20
+
+
+def replay(W, S, V, mask, amask, B32, follow=None, s_err=None):
+    """The producer warpgroup's per-point decisions over a batch of tiles (DESIGN 4.1), replayed in torch.
+
+    W, S: T x 128 x M float32 blend weights and member outputs (1.0 at quirk rows); V: T x 128 valid rows; mask: T x M the
+    tile's members (pre-pass); amask: T x M its den-absorbed members; B32: M float32 bounds (+inf: never a candidate).
+    follow: T x M members the kernel skipped; when given, they (not the replay's own verdicts) drive num, the two published
+    |num| and the lag, so that every verdict is the rule applied to the state the kernel had.  s_err: T x 128 x M bound on
+    |s_kernel - S| (default 0).  Returns dict of T x M bool: cand (a candidate: in both masks, finite B, two members of the
+    tile evaluated before it), skip (the rule on the replay's state), sure_skip / sure_keep (the verdict under every w, s and
+    num within the rounding differences between the replay and the kernel: w within W_REL (1 + |ln w|) relative, num within
+    the accumulated sum of w |ds| + ulp(|num|) per member evaluated), and margin: T x M float64, the smallest
+    (ulp(L) / 4 - w B) / (ulp(L) / 4) over the tile's deciding points (nan where no point decides)."""
+    torch = torch_mod()
+    T, R, M = W.shape
+    dev = W.device
+    f32 = torch.float32
+    num = torch.zeros(T, R, dtype=f32, device=dev)
+    dn = torch.zeros(T, R, dtype=torch.float64, device=dev)            # bound on |num_kernel - num|
+    pp = [torch.zeros(T, R, dtype=f32, device=dev)] * 2
+    pd = [torch.zeros(T, R, dtype=torch.float64, device=dev)] * 2
+    lag = torch.zeros(T, R, dtype=f32, device=dev)
+    lag_w = torch.zeros(T, R, dtype=torch.float64, device=dev)        # relative error bound of the lag's weight
+    npos = torch.zeros(T, dtype=torch.int64, device=dev)
+    out = {k: torch.zeros(T, M, dtype=torch.bool, device=dev) for k in ('cand', 'skip', 'sure_skip', 'sure_keep')}
+    out['margin'] = torch.full((T, M), float('nan'), dtype=torch.float64, device=dev)
+    inf = float('inf')
+    for k in range(M):
+        w, s = W[:, :, k], S[:, :, k]
+        Bk = B32[k].reshape(1, 1).expand(T, R).float()
+        ew = torch.where(w > 0, W_REL * (1.0 - torch.log(w.double().clamp_min(1e-45))), torch.zeros_like(dn))
+        cand = mask[:, k] & amask[:, k] & bool(torch.isfinite(B32[k])) & (npos >= 2)
+        ok = t_point_pass(w, Bk, pp[0], lag, V)
+        w_hi, w_lo = _t_f32_up(w.double() * (1 + ew)), _t_f32_down(w.double() * (1 - ew))
+        lag_hi, lag_lo = _t_f32_up(lag.double() * (1 + lag_w)), _t_f32_down(lag.double() * (1 - lag_w))
+        pub_lo = _t_f32_down((pp[0].double() - pd[0]).clamp_min(0.0))
+        pub_hi = _t_f32_up(pp[0].double() + pd[0])
+        ok_pes = t_point_pass(w_hi, Bk, pub_lo, lag_hi, V)
+        ok_opt = t_point_pass(w_lo, Bk, pub_hi, lag_lo, V)
+        out['cand'][:, k] = cand
+        out['skip'][:, k] = cand & ok.all(dim=1)
+        out['sure_skip'][:, k] = cand & ok_pes.all(dim=1)
+        out['sure_keep'][:, k] = ~cand | ~ok_opt.all(dim=1)
+        L = t_fsub_rd(pp[0], lag)
+        e = (L.view(torch.int32) >> 23) & 0xff
+        thr = torch.ldexp(torch.ones_like(L, dtype=torch.float64), (e - 152).double())
+        rel = (thr - t_fmul_ru(w, Bk).double()) / thr
+        rel = torch.where(V & (w != 0) & (L >= 2.0 ** -100), rel, torch.full_like(rel, inf))
+        mn = rel.min(dim=1).values
+        out['margin'][:, k] = torch.where(cand & torch.isfinite(mn), mn, out['margin'][:, k])
+        skipped = out['skip'][:, k] if follow is None else follow[:, k]
+        ev = (mask[:, k] & ~skipped)[:, None]
+        new = (w.double() * s.double() + num.double()).float()
+        err = w.double() * (s_err[:, :, k].double() if s_err is not None else 0.0)
+        dn_new = dn + err + (torch.nextafter(new.abs(), new.new_tensor(inf)) - new.abs()).double()
+        num = torch.where(ev, new, num)
+        dn = torch.where(ev, dn_new, dn)
+        pp = [torch.where(ev, pp[1], pp[0]), torch.where(ev, num.abs(), pp[1])]
+        pd = [torch.where(ev, pd[1], pd[0]), torch.where(ev, dn, pd[1])]
+        lag = torch.where(ev, t_fmul_ru(w, Bk), lag)
+        lag_w = torch.where(ev, ew, lag_w)
+        npos += ev[:, 0].long()
+    return out
+
+
 def absorbable(den, w, num_lo, wmax_bound, B):
     """The certificate (vectorised): den + w == den in float32, and wmax_bound * B < ulp(num_lo) / 4 with num_lo a lower
     bound of |num| (float64), wmax_bound >= w and B >= |s|.  When it holds, fmaf(w, s, num) == num and den + w == den."""
@@ -165,9 +329,10 @@ def grid_setup(latent_seed, scale=1.0):
     return P32, P64, z, anc32
 
 
-def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride=1, chunk_tiles=1024):
+def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride=1, chunk_tiles=1024, quirk_period=0):
     """dict of member-tile counts on the res^3 grid with the kernel's dense tiles (with plane_stride > 1: on the tiles of
-    every plane_stride-th x-plane)."""
+    every plane_stride-th x-plane).  quirk_period > 0: the eval-mode query's quirk rows (grid index g % period == period - 1
+    and the last point) blend 1.0 for every member, as in the kernel."""
     import torch
     from conftest import MAXI, MINI
     from ensemble_f64_common import members
@@ -202,6 +367,9 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
         pts = torch.from_numpy(X.reshape(-1, 3))
         with torch.no_grad():
             S = members(P32, pts, z, anc32).numpy().reshape(T, 128, M)
+        if quirk_period > 0:
+            g = (ix[sl] * res + iy[sl]) * res + iz[sl]
+            S[(g % quirk_period == quirk_period - 1) | (g == count - 1)] = 1.0
         with np.errstate(under='ignore'):
             d = anc_np[None, None] - X[:, :, None, :]                                       # T x 128 x 39 x 3
             d2 = np.float32(d[..., 2] * d[..., 2] + (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]))
@@ -213,11 +381,8 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
         den = np.zeros((T, 128), np.float32)
         pub = [np.full(T, -np.inf), np.full(T, -np.inf)]      # min |num| after the last two evaluated members (none: -inf)
         last_bound = np.zeros(T)                             # max_w * B of the last evaluated member
-        # per-point rule: |num| after the last two evaluated members, w * B of the last one (rounded up), members evaluated
-        pp = [np.zeros((T, 128), np.float32), np.zeros((T, 128), np.float32)]
-        lag = np.zeros((T, 128), np.float32)
-        npos = np.zeros(T, np.int64)
         inf32 = np.float32(np.inf)
+        zero_all, den_all, unchanged_all = (np.zeros((T, M), bool) for _ in range(3))
         for k in range(M):
             w = Wt[:, :, k]
             zero = ~np.any(V & (w != 0), axis=1)
@@ -235,12 +400,9 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
             unchanged = den_abs & np.all(~V | (new_num == num), axis=1) & ~zero
             assert not np.any(cert & ~unchanged), 'the certificate passed a member that changes num'
             cand = den_abs & ~zero & np.isfinite(B32[k])
-            cert_p = cand & (npos >= 2) & np.all(point_pass(w, B32[k], pp[0], lag, V), axis=1)
             no_lag_p = cand & np.all(point_pass(w, B32[k], np.abs(num), np.float32(0), V), axis=1)
-            assert not np.any(cert_p & ~unchanged), 'the per-point rule passed a member that changes num'
-            stats['absorbed_point'] += int(cert_p.sum())
             stats['absorbed_point_no_lag'] += int(no_lag_p.sum())
-            ev_p = ~(zero | cert_p)
+            zero_all[:, k], den_all[:, k], unchanged_all[:, k] = zero, den_abs, unchanged
             stats['zero'] += int(zero.sum())
             stats['den_absorbed'] += int((den_abs & ~zero).sum())
             stats['absorbed'] += int(cert.sum())
@@ -253,10 +415,12 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
             mn = np.where(V, np.abs(num), inf32).min(axis=1).astype(np.float64)
             pub = [np.where(ev, pub[1], pub[0]), np.where(ev, mn, pub[1])]
             last_bound = np.where(ev, wb * B[k], last_bound)
-            e2 = ev_p[:, None]
-            pp = [np.where(e2, pp[1], pp[0]), np.where(e2, np.abs(num), pp[1])]
-            lag = np.where(e2, fmul_ru(w, B32[k]), lag)
-            npos += ev_p
+        # the per-point rule (the kernel's): its own decisions drive the state
+        r = replay(torch.from_numpy(Wt), torch.from_numpy(S), torch.from_numpy(V), torch.from_numpy(~zero_all),
+                   torch.from_numpy(den_all), torch.from_numpy(B32.astype(np.float32)))
+        cert_p = r['skip'].numpy()
+        assert not np.any(cert_p & ~unchanged_all), 'the per-point rule passed a member that changes num'
+        stats['absorbed_point'] += int(cert_p.sum())
     n = stats['member_tiles']
     stats['evaluated_now'] = n - stats['zero']
     stats['evaluated_absorb'] = stats['evaluated_now'] - stats['absorbed']
@@ -281,8 +445,9 @@ def main():
     ap.add_argument('--res', type=int, default=64)
     ap.add_argument('--scale', type=float, default=1.0)
     ap.add_argument('--plane-stride', type=int, default=1, help='count the tiles of every n-th x-plane only (dense tiles)')
+    ap.add_argument('--quirk-period', type=int, default=0, help='quirk period of the query (bench.py and ens_trace.py: 25000)')
     args = ap.parse_args()
-    r = predict(args.latent, args.res, args.scale, plane_stride=args.plane_stride)
+    r = predict(args.latent, args.res, args.scale, plane_stride=args.plane_stride, quirk_period=args.quirk_period)
     ev = r['evaluated_now']
     if args.plane_stride > 1:
         print('tiles of every %d-th x-plane' % args.plane_stride)
