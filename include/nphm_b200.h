@@ -35,7 +35,7 @@ extern "C" {
                                 reference computation: |error| <= n_members * tau * max_k |s_k| (tau default 1e-8). */
 
 const char *nphm_last_error(void);
-int nphm_abi_version(void);      /* 2: the narrow-band steps are the nphm_band_slab_* family only */
+int nphm_abi_version(void);      /* 2: the narrow-band steps are the nphm_band_slab_* family, with nphm_band_heads_* added */
 /* sm count and compute capability of the current device */
 int nphm_device_info(int *sm_count, int *cc_major, int *cc_minor);
 
@@ -163,6 +163,18 @@ int nphm_mc_count(const float *vol_dev, const nphm_mc_params *p, void *workspace
  * shards; 0 for a whole volume). */
 int nphm_mc_emit(const float *vol_dev, const nphm_mc_params *p, void *workspace_dev,
                  long long vert_id_base, double *verts_dev, long long *tris_dev, void *stream);
+/* The same two passes over S volumes of p's shape (n_heads = S, whole volumes: ghost_lo = 0), vols_dev holding them one after
+ * the other (nx*ny*nz floats each), each kernel launched once for all S (DESIGN §4.18).  The workspace (>=
+ * nphm_mc_heads_workspace_bytes, NPHM_ERR_CAPACITY when short) holds the S totals and one nphm_mc_workspace_bytes(p) scratch per
+ * volume.  nphm_mc_heads_count writes {n_verts, n_tris} of every volume to counts_host[2h..2h+1] (one read-back, synchronises the
+ * stream); nphm_mc_heads_emit writes volume h's vertices and triangles after those of volumes 0..h-1 in verts_dev / tris_dev, with
+ * ids local to the volume (from 0): for every h, exactly what nphm_mc_count / nphm_mc_emit (vert_id_base 0) give on volume h.
+ * Needs 1 <= n_heads <= 65535 (else NPHM_ERR_INVALID, and -1 from nphm_mc_heads_workspace_bytes). */
+long long nphm_mc_heads_workspace_bytes(const nphm_mc_params *p, int n_heads);
+int nphm_mc_heads_count(const float *vols_dev, const nphm_mc_params *p, int n_heads, void *workspace_dev, long long workspace_bytes,
+                        long long *counts_host, void *stream);
+int nphm_mc_heads_emit(const float *vols_dev, const nphm_mc_params *p, int n_heads, void *workspace_dev, long long workspace_bytes,
+                       double *verts_dev, long long *tris_dev, void *stream);
 /* Host-buffer convenience == mcubes.marching_cubes on a host volume: two-call protocol, call with
  * verts_host == NULL to get the counts. Synchronous. */
 int nphm_marching_cubes_host(const float *vol_host, int nx, int ny, int nz, double iso, int negate,
@@ -505,6 +517,40 @@ int nphm_band_slab_export(int res, int block, int l0, int l1, int plane, const f
                           long long workspace_bytes, unsigned char *buf_dev, void *stream);
 int nphm_band_slab_import(int res, int block, int l0, int l1, int plane, const unsigned char *buf_dev, float *vol_dev,
                           void *workspace_dev, long long workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * The band of S heads in lockstep (n_heads = S latent codes of one decoder, DESIGN §4.18): the nphm_band_slab_* steps of the whole
+ * grid (the slab [0, blocks)) for S bands at once, each step one launch sequence for all S heads.  vols_dev holds the S res^3
+ * volumes one after the other; the workspace (>= nphm_band_heads_workspace_bytes, NPHM_ERR_CAPACITY when short) holds the S
+ * {voxels listed, blocks active} pairs and S slab workspaces.  Every head's state, lists and volume evolve exactly as those of a
+ * single band driven through the same steps.
+ *   begin, corners, classify, grow   as the slab steps, for every head; counts_host (2 S long longs, may be NULL) receives head h's
+ *                                    pair at [2h..2h+1], read back with one copy (one synchronisation whatever S is).  The quirk
+ *                                    voxels depend only on res and quirk_period, so every head lists the same ones.
+ *   gather                           n_pad rows per head, head-major (xyz_dev: S x n_pad x 3): head h's listed voxels first, then
+ *                                    rows that repeat its last listed voxel (voxel 0 when it listed nothing); n_pad >= the
+ *                                    largest count is the caller's choice
+ *   scatter                          values_dev (S x n_pad) in the same layout: head h's first (listed) rows into its volume,
+ *                                    the padding dropped
+ *   fill, block_states               as the slab steps; states_dev: S x blocks^3 bytes
+ * Needs 1 <= n_heads <= 65535 and what the slab steps need (else NPHM_ERR_INVALID; -1 from nphm_band_heads_workspace_bytes). */
+long long nphm_band_heads_workspace_bytes(int res, int block, int n_heads);
+int nphm_band_heads_begin(int res, int block, int n_heads, long long quirk_period, void *workspace_dev, long long workspace_bytes,
+                          long long *counts_host, void *stream);
+int nphm_band_heads_corners(int res, int block, int n_heads, void *workspace_dev, long long workspace_bytes, long long *counts_host,
+                            void *stream);
+int nphm_band_heads_classify(int res, int block, int n_heads, float tau, const float *vols_dev, void *workspace_dev,
+                             long long workspace_bytes, long long *counts_host, void *stream);
+int nphm_band_heads_grow(int res, int block, int n_heads, const float *vols_dev, void *workspace_dev, long long workspace_bytes,
+                         long long *counts_host, void *stream);
+int nphm_band_heads_gather(int res, int block, int n_heads, const double grid_min[3], const double grid_max[3], long long n_pad,
+                           float *xyz_dev, void *workspace_dev, long long workspace_bytes, void *stream);
+int nphm_band_heads_scatter(int res, int block, int n_heads, long long n_pad, const float *values_dev, float *vols_dev,
+                            void *workspace_dev, long long workspace_bytes, void *stream);
+int nphm_band_heads_fill(int res, int block, int n_heads, float *vols_dev, void *workspace_dev, long long workspace_bytes,
+                         void *stream);
+int nphm_band_heads_block_states(int res, int block, int n_heads, const void *workspace_dev, long long workspace_bytes,
+                                 unsigned char *states_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * The same steps with block-sparse storage (DESIGN §4.17): nothing is stored per grid voxel.  The workspace

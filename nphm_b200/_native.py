@@ -45,6 +45,9 @@ EXPORTED_SYMBOLS = (
     'nphm_band_slab_workspace_bytes', 'nphm_band_slab_begin', 'nphm_band_slab_corners', 'nphm_band_slab_gather',
     'nphm_band_slab_scatter', 'nphm_band_slab_classify', 'nphm_band_slab_grow', 'nphm_band_slab_fill', 'nphm_band_slab_block_states',
     'nphm_band_slab_export', 'nphm_band_slab_import',
+    'nphm_band_heads_workspace_bytes', 'nphm_band_heads_begin', 'nphm_band_heads_corners', 'nphm_band_heads_classify',
+    'nphm_band_heads_grow', 'nphm_band_heads_gather', 'nphm_band_heads_scatter', 'nphm_band_heads_fill',
+    'nphm_band_heads_block_states', 'nphm_mc_heads_workspace_bytes', 'nphm_mc_heads_count', 'nphm_mc_heads_emit',
     'nphm_band_sparse_workspace_bytes', 'nphm_band_sparse_pool_sizes', 'nphm_band_sparse_begin', 'nphm_band_sparse_corners',
     'nphm_band_sparse_classify', 'nphm_band_sparse_grow', 'nphm_band_sparse_gather', 'nphm_band_sparse_scatter',
     'nphm_band_sparse_fill', 'nphm_band_sparse_block_states', 'nphm_band_sparse_export', 'nphm_band_sparse_import',
@@ -234,6 +237,22 @@ def lib() -> ctypes.CDLL:
     L.nphm_band_slab_block_states.argtypes = slab + [c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_band_slab_export.argtypes = slab + [c_int, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_band_slab_import.argtypes = slab + [c_int, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    heads = [c_int, c_int, c_int]                      # res, block, n_heads: S bands of the whole grid
+    L.nphm_band_heads_workspace_bytes.argtypes = heads
+    L.nphm_band_heads_workspace_bytes.restype = c_longlong
+    L.nphm_band_heads_begin.argtypes = heads + [c_longlong, c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_band_heads_corners.argtypes = heads + [c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_band_heads_classify.argtypes = heads + [c_float, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_band_heads_grow.argtypes = heads + [c_void_p, c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_band_heads_gather.argtypes = heads + [POINTER(c_double), POINTER(c_double), c_longlong, c_void_p, c_void_p, c_longlong,
+                                                 c_void_p]
+    L.nphm_band_heads_scatter.argtypes = heads + [c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_heads_fill.argtypes = heads + [c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_band_heads_block_states.argtypes = heads + [c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_mc_heads_workspace_bytes.argtypes = [POINTER(McParams), c_int]
+    L.nphm_mc_heads_workspace_bytes.restype = c_longlong
+    L.nphm_mc_heads_count.argtypes = [c_void_p, POINTER(McParams), c_int, c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_mc_heads_emit.argtypes = [c_void_p, POINTER(McParams), c_int, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p]
     L.nphm_band_sparse_workspace_bytes.argtypes = slab
     L.nphm_band_sparse_workspace_bytes.restype = c_longlong
     L.nphm_band_sparse_pool_sizes.argtypes = slab + [c_longlong, POINTER(c_longlong)]
@@ -1079,6 +1098,111 @@ def NarrowBandSlab(res: int, block: int, l0: int, l1: int, device) -> NarrowBand
     """The :class:`NarrowBand` of the x-slab of block layers ``[l0, l1)``, in the argument order the callers of the multi-GPU band
     use."""
     return NarrowBand(res, block, device, l0, l1)
+
+
+class NarrowBandHeads:
+    """The band of :class:`NarrowBand` on the whole ``res^3`` grid for ``n_heads`` heads in lockstep (``nphm_band_heads_*``,
+    DESIGN §4.18): S latent codes of one decoder, each step one launch sequence for all of them.  The listing steps return the S
+    counts (read back with one copy; :attr:`readbacks` counts the synchronising calls), :meth:`gather` / :meth:`scatter` move
+    ``S x n_pad`` head-major rows, and :meth:`marching_cubes` meshes the S filled volumes with one count read-back.  Every head's
+    state evolves exactly as a :class:`NarrowBand` driven through the same steps."""
+
+    def __init__(self, res: int, block: int, device, n_heads: int):
+        self.res, self.block, self.n_heads = int(res), int(block), int(n_heads)
+        self.device = torch.device(device)
+        self.blocks_per_axis = -(-(self.res - 1) // max(self.block, 1))
+        self._geo = (self.res, self.block, self.n_heads)
+        with torch.cuda.device(self.device):
+            self.ws = _workspace(lib().nphm_band_heads_workspace_bytes(*self._geo), 'nphm_band_heads_workspace_bytes', self.device)
+        self.active_blocks = [0] * self.n_heads
+        self.readbacks = 0                  # stream synchronisations of the listing steps and marching cubes so far
+        self.mc_bytes = 0                   # marching-cubes workspace of the last mesh
+
+    @staticmethod
+    def device_bytes_per_head(res: int, block: int) -> int:
+        """Device bytes one head holds: its band workspace, volume and marching-cubes scratch."""
+        L = lib()
+        band = L.nphm_band_heads_workspace_bytes(int(res), int(block), 2) - L.nphm_band_heads_workspace_bytes(int(res), int(block), 1)
+        p = McParams(int(res), int(res), int(res), 0, 0, 1, 0.0)
+        mc = L.nphm_mc_heads_workspace_bytes(byref(p), 2) - L.nphm_mc_heads_workspace_bytes(byref(p), 1)
+        if band < 0 or mc < 0:
+            check(-1, 'nphm_band_heads_workspace_bytes')
+        return int(band + mc + 4 * int(res) ** 3)
+
+    def _call(self, step, *args):
+        with torch.cuda.device(self.device):
+            check(getattr(lib(), 'nphm_band_heads_' + step)(*self._geo, *args, _stream_ptr(self.device)), 'nphm_band_heads_' + step)
+
+    def _call_listing(self, step, *before_ws):
+        counts = (c_longlong * (2 * self.n_heads))()
+        self._call(step, *before_ws, self.ws.data_ptr(), self.ws.numel(), counts)
+        self.readbacks += 1
+        self.active_blocks = list(counts[1::2])
+        return list(counts[0::2])
+
+    def begin(self, quirk_period: int = 0):
+        """Reset every head; with ``quirk_period > 0`` list the eval-mode quirk voxels (the same for every head)."""
+        return self._call_listing('begin', int(quirk_period))
+
+    def corners(self):
+        return self._call_listing('corners')
+
+    def classify(self, tau: float, vols: torch.Tensor):
+        return self._call_listing('classify', float(tau), vols.data_ptr())
+
+    def grow(self, vols: torch.Tensor):
+        return self._call_listing('grow', vols.data_ptr())
+
+    def gather(self, n_pad: int, mini, maxi) -> torch.Tensor:
+        """(S, n_pad, 3) float32 coordinates: each head's listed voxels, then padding rows that repeat one of them."""
+        xyz = torch.empty(self.n_heads, int(n_pad), 3, device=self.device, dtype=torch.float32)
+        gmin = (c_double * 3)(*[float(v) for v in mini])
+        gmax = (c_double * 3)(*[float(v) for v in maxi])
+        self._call('gather', gmin, gmax, int(n_pad), _ptr(xyz) if n_pad else None, self.ws.data_ptr(), self.ws.numel())
+        return xyz
+
+    def scatter(self, values: torch.Tensor, vols: torch.Tensor):
+        """values (S, n_pad) in the layout of :meth:`gather`: each head's listed rows into its volume, the padding dropped."""
+        v = _f32c(values).reshape(self.n_heads, -1)
+        n_pad = v.shape[1]
+        self._call('scatter', n_pad, v.data_ptr() if n_pad else None, vols.data_ptr(), self.ws.data_ptr(), self.ws.numel())
+
+    def fill(self, vols: torch.Tensor):
+        self._call('fill', vols.data_ptr(), self.ws.data_ptr(), self.ws.numel())
+
+    def block_states(self) -> torch.Tensor:
+        """(S, blocks, blocks, blocks) bool: which blocks of each head are active."""
+        nb = self.blocks_per_axis
+        out = torch.empty(self.n_heads, nb, nb, nb, device=self.device, dtype=torch.uint8)
+        self._call('block_states', self.ws.data_ptr(), self.ws.numel(), out.data_ptr())
+        return out != 0
+
+    def volumes(self) -> torch.Tensor:
+        """Uninitialised (S, res, res, res) float32 volumes on the band's device."""
+        return torch.empty(self.n_heads, self.res, self.res, self.res, device=self.device, dtype=torch.float32)
+
+    def marching_cubes(self, vols: torch.Tensor):
+        """Marching cubes on ``-vols`` at 0 for every head (``nphm_mc_heads_count`` / ``_emit``): ``(verts (V, 3) float64, tris
+        (T, 3) int64, counts)`` with the S meshes one after the other in index units, ids local to each head, and ``counts`` the
+        S ``(n_verts, n_tris)``; head h's part is what :func:`marching_cubes_device` ``(vols[h], 0, negate=True)`` gives."""
+        v = vols.contiguous()
+        assert v.shape == (self.n_heads, self.res, self.res, self.res) and v.dtype == torch.float32 and v.device == self.device
+        p = McParams(self.res, self.res, self.res, 0, 0, 1, 0.0)
+        L = lib()
+        with torch.cuda.device(self.device):
+            ws = _workspace(L.nphm_mc_heads_workspace_bytes(byref(p), self.n_heads), 'nphm_mc_heads_workspace_bytes', self.device)
+            self.mc_bytes = ws.numel()
+            counts = (c_longlong * (2 * self.n_heads))()
+            check(L.nphm_mc_heads_count(v.data_ptr(), byref(p), self.n_heads, ws.data_ptr(), ws.numel(), counts,
+                                        _stream_ptr(self.device)), 'nphm_mc_heads_count')
+            self.readbacks += 1
+            pairs = [(counts[2 * h], counts[2 * h + 1]) for h in range(self.n_heads)]
+            verts = torch.empty(sum(c[0] for c in pairs), 3, device=self.device, dtype=torch.float64)
+            tris = torch.empty(sum(c[1] for c in pairs), 3, device=self.device, dtype=torch.int64)
+            if verts.shape[0] or tris.shape[0]:
+                check(L.nphm_mc_heads_emit(v.data_ptr(), byref(p), self.n_heads, ws.data_ptr(), ws.numel(), verts.data_ptr(),
+                                           tris.data_ptr(), _stream_ptr(self.device)), 'nphm_mc_heads_emit')
+        return verts, tris, pairs
 
 
 NPHM_ERR_CAPACITY = -4

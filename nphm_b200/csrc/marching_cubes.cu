@@ -19,9 +19,14 @@
 //                 owner-cell lookup of a triangle corner costs one 8-byte load instead of a per-cell u32 array.
 // Algorithmic HBM traffic: 4 B/voxel read + 24 B/vertex + 24 B/triangle written; scratch: 1 B/cell (case index) +
 // 2 B per 8 cells (group prefix) written once, read once by K3 (rows with a crossing and their neighbours only).
+//
+// Heads (DESIGN §4.18): S volumes of the same shape in one launch of each kernel, the head in blockIdx.y; head h's volume and
+// workspace lie h * Heads::vol floats and h * Heads::ws bytes past head 0's.  nphm_mc_count / nphm_mc_emit are the S = 1 call.
 #include "common.cuh"
 #include "mc_tables.h"
 #include <cstring>
+#include <type_traits>
+#include <vector>
 
 namespace nphm {
 
@@ -52,6 +57,17 @@ __constant__ unsigned char c_edge_b[12] = {1, 2, 3, 0, 5, 6, 7, 4, 4, 5, 6, 7};
 // edge id from (axis, offset of its low end point along the two other axes): [axis][d_first][d_second]
 // x edges: (dj,dk); y edges: (di,dk); z edges: (di,dj)
 __constant__ unsigned char c_edge_of[3][2][2] = {{{0, 4}, {2, 6}}, {{3, 7}, {1, 5}}, {{8, 11}, {9, 10}}};
+
+struct Heads {
+    long long ws, vol;       // strides between heads: workspace bytes, volume floats
+};
+
+template <class T>
+__device__ __forceinline__ T *head_at(T *p, long long stride_bytes)
+{
+    using B = typename std::conditional<std::is_const<T>::value, const char, char>::type;
+    return reinterpret_cast<T *>(reinterpret_cast<B *>(p) + blockIdx.y * stride_bytes);
+}
 
 struct Dims {
     int nx, ny, nz;          // planes
@@ -129,9 +145,15 @@ template <bool ALIGNED>
 __global__ void __launch_bounds__(kRowThreads) mc_classify_rows_kernel(const float *__restrict__ vol, const Dims d,
                                                                        unsigned char *__restrict__ cube_out,
                                                                        unsigned short *__restrict__ grp_prefix,
-                                                                       unsigned *__restrict__ row_nv, unsigned *__restrict__ row_nt)
+                                                                       unsigned *__restrict__ row_nv, unsigned *__restrict__ row_nt,
+                                                                       const Heads H)
 {
     __shared__ uint4 s_tab[kTabTri / 16];
+    vol += blockIdx.y * H.vol;
+    cube_out = head_at(cube_out, H.ws);
+    grp_prefix = head_at(grp_prefix, H.ws);
+    row_nv = head_at(row_nv, H.ws);
+    row_nt = head_at(row_nt, H.ws);
     for (int i = threadIdx.x; i < kTabTri / 16; i += kRowThreads) s_tab[i] = __ldg(g_tables + i);
     __syncthreads();
     const unsigned short *s_edge = reinterpret_cast<const unsigned short *>(s_tab);
@@ -180,12 +202,21 @@ __global__ void __launch_bounds__(kRowThreads) mc_classify_rows_kernel(const flo
 
 // K2: exclusive scan of the row counts.  row_v/row_t receive the exclusive prefix INSIDE their chunk of kRowChunk rows,
 // chunk_v/chunk_t the exclusive prefix of the chunk sums (written by the last CTA to finish), totals[0..1] the grand
-// totals and totals[2..3] what the ghost layer (cell layer 0 of a slab with ghost_lo) creates.
+// totals and totals[2..3] what the ghost layer (cell layer 0 of a slab with ghost_lo) creates; the last CTA also copies them to
+// pairs[4h..4h+3] (the S heads' totals side by side, read back with one copy).
 __global__ void __launch_bounds__(256) mc_scan_rows_kernel(const unsigned *__restrict__ row_nv, const unsigned *__restrict__ row_nt,
                                                            unsigned *__restrict__ row_v, unsigned *__restrict__ row_t,
                                                            unsigned *__restrict__ chunk_v, unsigned *__restrict__ chunk_t,
-                                                           int n_rows, int ghost_rows, unsigned long long *__restrict__ totals)
+                                                           int n_rows, int ghost_rows, unsigned long long *__restrict__ totals,
+                                                           const Heads H, unsigned long long *pairs)     // one volume: == totals
 {
+    row_nv = head_at(row_nv, H.ws);
+    row_nt = head_at(row_nt, H.ws);
+    row_v = head_at(row_v, H.ws);
+    row_t = head_at(row_t, H.ws);
+    chunk_v = head_at(chunk_v, H.ws);
+    chunk_t = head_at(chunk_t, H.ws);
+    totals = head_at(totals, H.ws);
     __shared__ unsigned wsum[2][8];
     __shared__ bool last;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -237,6 +268,7 @@ __global__ void __launch_bounds__(256) mc_scan_rows_kernel(const unsigned *__res
             } else if (ghost_rows > 0) {
                 totals[2] = cv; totals[3] = ct;
             }
+            for (int i = 0; i < 4; ++i) pairs[4 * blockIdx.y + i] = totals[i];
         }
     }
 }
@@ -257,15 +289,27 @@ struct Scratch {
     const unsigned long long *totals;
 };
 
+__device__ __forceinline__ Scratch head_at(const Scratch &w, long long stride_bytes)
+{
+    return Scratch{head_at(w.cube, stride_bytes), head_at(w.grp_prefix, stride_bytes), head_at(w.row_nv, stride_bytes),
+                   head_at(w.row_nt, stride_bytes), head_at(w.row_v, stride_bytes), head_at(w.row_t, stride_bytes),
+                   head_at(w.chunk_v, stride_bytes), head_at(w.chunk_t, stride_bytes), head_at(w.totals, stride_bytes)};
+}
+
 // One warp per cell row.  The active cells of the row (a handful out of 255 for a head) are processed ONE AT A TIME BY THE
 // WHOLE WARP: lane e < 12 resolves the vertex id of cube edge e (owner cell lookup), lane o < 12 creates the o-th vertex
 // of the cell's creation order, lane m < 3 * n_triangles writes one triangle index (ids travel by shuffle).  The per-edge
 // constants (end corners, axis, creation rank mask) are therefore per-LANE constants held in registers.
-__global__ void __launch_bounds__(kRowThreads) mc_emit_rows_kernel(const float *__restrict__ vol, const Dims d, const Scratch w,
+// Heads: head h writes its vertices and triangles after those of heads 0 .. h-1 (their totals, summed here), with ids from
+// vert_id_base as a single volume numbers them.  HEADS = false (one volume) keeps the scratch pointers in the parameter bank.
+template <bool HEADS>
+__global__ void __launch_bounds__(kRowThreads) mc_emit_rows_kernel(const float *__restrict__ vol, const Dims d, const Scratch w0,
                                                                    long long vert_id_base, double *__restrict__ verts,
-                                                                   long long *__restrict__ tris)
+                                                                   long long *__restrict__ tris, const Heads H)
 {
     __shared__ uint4 s_tab[kTabBytes / 16];
+    if (HEADS) vol += blockIdx.y * H.vol;
+    const Scratch w = HEADS ? head_at(w0, H.ws) : w0;
     const int lane = threadIdx.x & 31;
     const int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
     const int ci = r < d.n_rows ? r / d.cy : 0, cj = r < d.n_rows ? r - ci * d.cy : 0;
@@ -279,6 +323,17 @@ __global__ void __launch_bounds__(kRowThreads) mc_emit_rows_kernel(const float *
     const unsigned char *s_ntri = reinterpret_cast<const unsigned char *>(s_tab) + kTabNtri;
     const signed char (*s_tri)[16] = reinterpret_cast<const signed char (*)[16]>(reinterpret_cast<const unsigned char *>(s_tab) + kTabTri);
     const int gi = d.x_global0 + ci;
+    if (HEADS) {
+        unsigned long long v_off = 0, t_off = 0;
+        for (unsigned h = 0; h < blockIdx.y; ++h) {
+            const unsigned long long *t = reinterpret_cast<const unsigned long long *>(reinterpret_cast<const char *>(w0.totals) +
+                                                                                         h * H.ws);
+            v_off += t[0];
+            t_off += t[1];
+        }
+        verts += 3 * v_off;
+        tris += 3 * t_off;
+    }
     const unsigned ghost_v = d.ghost_lo ? (unsigned)w.totals[2] : 0u;
     const unsigned ghost_t = d.ghost_lo ? (unsigned)w.totals[3] : 0u;
     auto base_v = [&](int row) { return w.chunk_v[row / kRowChunk] + w.row_v[row]; };
@@ -492,6 +547,73 @@ extern "C" long long nphm_mc_workspace_bytes(const nphm_mc_params *p)
     return carve(nullptr, d).bytes;
 }
 
+namespace nphm {
+namespace {
+
+// S volumes at a stride of n_vox floats, head 0's workspace at ws0 and the others at a stride of ws_stride bytes; counts_host:
+// {n_verts, n_tris} of every head (one read-back of the S totals in `pairs`, one synchronisation)
+int count_heads(const float *vol_dev, const Dims &d, int S, void *ws0, long long ws_stride, unsigned long long *pairs,
+                long long *counts_host, cudaStream_t stream)
+{
+    int rc = load_tables();
+    if (rc) return rc;
+    Workspace w = carve(ws0, d);
+    for (int h = 0; h < S; ++h)
+        NPHM_CUDA_CHECK(cudaMemsetAsync(reinterpret_cast<char *>(w.totals) + h * ws_stride, 0, 256, stream));
+    const Heads H{ws_stride, (long long)d.nx * d.ny * d.nz};
+    const dim3 grid((unsigned)ceil_div(d.n_rows, kWarpsPerCta), (unsigned)S);
+    const bool aligned = (d.nz % 4 == 0) && ((reinterpret_cast<uintptr_t>(vol_dev) & 15) == 0);
+    if (aligned)
+        mc_classify_rows_kernel<true><<<grid, kRowThreads, 0, stream>>>(vol_dev, d, w.cube, w.grp_prefix, w.row_nv, w.row_nt, H);
+    else
+        mc_classify_rows_kernel<false><<<grid, kRowThreads, 0, stream>>>(vol_dev, d, w.cube, w.grp_prefix, w.row_nv, w.row_nt, H);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    mc_scan_rows_kernel<<<dim3((unsigned)w.n_chunks, (unsigned)S), 256, 0, stream>>>(w.row_nv, w.row_nt, w.row_v, w.row_t, w.chunk_v,
+                                                                                     w.chunk_t, d.n_rows, d.ghost_lo ? d.cy : 0,
+                                                                                     w.totals, H, pairs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    std::vector<unsigned long long> totals(4 * (size_t)S);
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(totals.data(), pairs, totals.size() * sizeof(totals[0]), cudaMemcpyDeviceToHost, stream));
+    NPHM_CUDA_CHECK(cudaStreamSynchronize(stream));
+    for (int h = 0; h < S; ++h) {
+        const unsigned long long *t = totals.data() + 4 * h;
+        NPHM_REQUIRE(t[0] < 0xffffffffull && t[1] < 0xffffffffull, "nphm_mc_count: mesh too large for 32-bit scratch");
+        counts_host[2 * h] = (long long)(t[0] - (d.ghost_lo ? t[2] : 0));
+        counts_host[2 * h + 1] = (long long)(t[1] - (d.ghost_lo ? t[3] : 0));
+    }
+    return NPHM_OK;
+}
+
+int emit_heads(const float *vol_dev, const Dims &d, int S, void *ws0, long long ws_stride, long long vert_id_base, double *verts_dev,
+               long long *tris_dev, cudaStream_t stream)
+{
+    Workspace w = carve(ws0, d);
+    Scratch s{w.cube, w.grp_prefix, w.row_nv, w.row_nt, w.row_v, w.row_t, w.chunk_v, w.chunk_t, w.totals};
+    const Heads H{ws_stride, (long long)d.nx * d.ny * d.nz};
+    const dim3 grid((unsigned)ceil_div(d.n_rows, kWarpsPerCta), (unsigned)S);
+    if (S > 1)
+        mc_emit_rows_kernel<true><<<grid, kRowThreads, 0, stream>>>(vol_dev, d, s, vert_id_base, verts_dev, tris_dev, H);
+    else
+        mc_emit_rows_kernel<false><<<grid, kRowThreads, 0, stream>>>(vol_dev, d, s, vert_id_base, verts_dev, tris_dev, H);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+// workspace of S heads: their totals side by side, then S single-volume workspaces
+long long pairs_bytes(int S) { return (32LL * S + 255) / 256 * 256; }
+
+int heads_dims(const nphm_mc_params *p, int S, Dims &d, const char *who)
+{
+    int rc = make_dims(p, d);
+    if (rc) return rc;
+    NPHM_REQUIRE(S >= 1 && S <= 65535, "%s: %d heads outside [1, 65535]", who, S);
+    NPHM_REQUIRE(!d.ghost_lo, "%s: the heads are whole volumes (ghost_lo = 0)", who);
+    return NPHM_OK;
+}
+
+}  // namespace
+}  // namespace nphm
+
 extern "C" int nphm_mc_count(const float *vol_dev, const nphm_mc_params *p, void *workspace_dev,
                              long long *n_verts_host, long long *n_tris_host, void *stream_)
 {
@@ -503,26 +625,11 @@ extern "C" int nphm_mc_count(const float *vol_dev, const nphm_mc_params *p, void
     *n_verts_host = 0; *n_tris_host = 0;
     if (d.ncells == 0) return NPHM_OK;
     NPHM_REQUIRE(vol_dev && workspace_dev, "nphm_mc_count: NULL volume / workspace");
-    rc = load_tables();
+    long long counts[2];
+    rc = count_heads(vol_dev, d, 1, workspace_dev, 0, carve(workspace_dev, d).totals, counts, stream);
     if (rc) return rc;
-    Workspace w = carve(workspace_dev, d);
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.totals, 0, 256, stream));
-    const int grid = (int)ceil_div(d.n_rows, kWarpsPerCta);
-    const bool aligned = (d.nz % 4 == 0) && ((reinterpret_cast<uintptr_t>(vol_dev) & 15) == 0);
-    if (aligned)
-        mc_classify_rows_kernel<true><<<grid, kRowThreads, 0, stream>>>(vol_dev, d, w.cube, w.grp_prefix, w.row_nv, w.row_nt);
-    else
-        mc_classify_rows_kernel<false><<<grid, kRowThreads, 0, stream>>>(vol_dev, d, w.cube, w.grp_prefix, w.row_nv, w.row_nt);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    mc_scan_rows_kernel<<<w.n_chunks, 256, 0, stream>>>(w.row_nv, w.row_nt, w.row_v, w.row_t, w.chunk_v, w.chunk_t, d.n_rows,
-                                                        d.ghost_lo ? d.cy : 0, w.totals);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    unsigned long long totals[4];
-    NPHM_CUDA_CHECK(cudaMemcpyAsync(totals, w.totals, sizeof(totals), cudaMemcpyDeviceToHost, stream));
-    NPHM_CUDA_CHECK(cudaStreamSynchronize(stream));
-    NPHM_REQUIRE(totals[0] < 0xffffffffull && totals[1] < 0xffffffffull, "nphm_mc_count: mesh too large for 32-bit scratch");
-    *n_verts_host = (long long)(totals[0] - (d.ghost_lo ? totals[2] : 0));
-    *n_tris_host = (long long)(totals[1] - (d.ghost_lo ? totals[3] : 0));
+    *n_verts_host = counts[0];
+    *n_tris_host = counts[1];
     return NPHM_OK;
 }
 
@@ -535,12 +642,53 @@ extern "C" int nphm_mc_emit(const float *vol_dev, const nphm_mc_params *p, void 
     if (rc) return rc;
     if (d.ncells == 0) return NPHM_OK;
     NPHM_REQUIRE(vol_dev && workspace_dev, "nphm_mc_emit: NULL volume / workspace");
-    Workspace w = carve(workspace_dev, d);
-    Scratch s{w.cube, w.grp_prefix, w.row_nv, w.row_nt, w.row_v, w.row_t, w.chunk_v, w.chunk_t, w.totals};
-    mc_emit_rows_kernel<<<(int)ceil_div(d.n_rows, kWarpsPerCta), kRowThreads, 0, stream>>>(vol_dev, d, s, vert_id_base, verts_dev,
-                                                                                          tris_dev);
-    NPHM_CUDA_CHECK(cudaGetLastError());
-    return NPHM_OK;
+    return emit_heads(vol_dev, d, 1, workspace_dev, 0, vert_id_base, verts_dev, tris_dev, stream);
+}
+
+extern "C" long long nphm_mc_heads_workspace_bytes(const nphm_mc_params *p, int n_heads)
+{
+    Dims d;
+    if (heads_dims(p, n_heads, d, "nphm_mc_heads_workspace_bytes") != NPHM_OK) return -1;
+    return pairs_bytes(n_heads) + n_heads * carve(nullptr, d).bytes;
+}
+
+extern "C" int nphm_mc_heads_count(const float *vols_dev, const nphm_mc_params *p, int n_heads, void *workspace_dev,
+                                   long long workspace_bytes, long long *counts_host, void *stream_)
+{
+    Dims d;
+    int rc = heads_dims(p, n_heads, d, "nphm_mc_heads_count");
+    if (rc) return rc;
+    NPHM_REQUIRE(counts_host, "nphm_mc_heads_count: NULL counts");
+    for (int i = 0; i < 2 * n_heads; ++i) counts_host[i] = 0;
+    if (d.ncells == 0) return NPHM_OK;
+    const long long stride = carve(nullptr, d).bytes;
+    NPHM_REQUIRE(vols_dev && workspace_dev, "nphm_mc_heads_count: NULL volumes / workspace");
+    if (workspace_bytes < pairs_bytes(n_heads) + n_heads * stride) {
+        set_error("nphm_mc_heads_count: workspace too small: %lld bytes, %lld needed", workspace_bytes,
+                  pairs_bytes(n_heads) + n_heads * stride);
+        return NPHM_ERR_CAPACITY;
+    }
+    char *ws = static_cast<char *>(workspace_dev);
+    return count_heads(vols_dev, d, n_heads, ws + pairs_bytes(n_heads), stride, reinterpret_cast<unsigned long long *>(ws), counts_host,
+                       static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int nphm_mc_heads_emit(const float *vols_dev, const nphm_mc_params *p, int n_heads, void *workspace_dev,
+                                  long long workspace_bytes, double *verts_dev, long long *tris_dev, void *stream_)
+{
+    Dims d;
+    int rc = heads_dims(p, n_heads, d, "nphm_mc_heads_emit");
+    if (rc) return rc;
+    if (d.ncells == 0) return NPHM_OK;
+    const long long stride = carve(nullptr, d).bytes;
+    NPHM_REQUIRE(vols_dev && workspace_dev, "nphm_mc_heads_emit: NULL volumes / workspace");
+    if (workspace_bytes < pairs_bytes(n_heads) + n_heads * stride) {
+        set_error("nphm_mc_heads_emit: workspace too small: %lld bytes, %lld needed", workspace_bytes,
+                  pairs_bytes(n_heads) + n_heads * stride);
+        return NPHM_ERR_CAPACITY;
+    }
+    return emit_heads(vols_dev, d, n_heads, static_cast<char *>(workspace_dev) + pairs_bytes(n_heads), stride, 0, verts_dev, tris_dev,
+                      static_cast<cudaStream_t>(stream_));
 }
 
 // Host-buffer convenience (== mcubes.marching_cubes on a host array).  The device staging buffers are kept between calls

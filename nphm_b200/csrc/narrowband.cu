@@ -10,9 +10,15 @@
 //   states  1 byte per block: 0 inactive, 1 activated (its voxels not yet marked), 2 active (marked)
 //   list    u32 slab-local flat voxel indices of the last compaction, ascending
 // Marching cubes runs on -sdf at 0, so a voxel is "inside" when -v <= 0, i.e. v >= 0 (NaN: outside) - `side()` below.
+//
+// Heads: S bands of the same slab (S latent codes of one decoder, DESIGN §4.18) step together.  Head h's workspace and volume lie
+// h * Heads::ws bytes and h * Heads::vol floats past head 0's; every kernel takes its head from blockIdx.y, so one launch serves
+// all S heads, and the single-band entry points are the S = 1 call of the same kernels.
 #include "common.cuh"
 #include "simt.cuh"
 #include <algorithm>
+#include <type_traits>
+#include <vector>
 
 namespace nphm {
 namespace band {
@@ -70,6 +76,20 @@ inline Layout layout(const Geo &g)
     return l;
 }
 
+struct Heads {
+    long long ws, vol;            // strides between heads: workspace bytes, volume floats (0, 0 for one band)
+};
+
+template <class T>
+__device__ __forceinline__ T *head_at(T *p, long long stride_bytes)
+{
+    using B = typename std::conditional<std::is_const<T>::value, const char, char>::type;
+    return reinterpret_cast<T *>(reinterpret_cast<B *>(p) + blockIdx.y * stride_bytes);
+}
+
+template <class T>
+__device__ __forceinline__ T *head_vol(T *vol, const Heads &H) { return vol + blockIdx.y * H.vol; }
+
 struct Ws {
     unsigned long long *hdr;
     float *axes;
@@ -110,10 +130,12 @@ __device__ __forceinline__ void unblock(const Geo &g, long long b, int &bx, int 
 // eval-mode quirk voxels g = (k + 1) p - 1 and g = res^3 - 1 (k in [k0, k1): those of the slab's planes): wanted, and every block
 // of the slab owning a cell that touches one is forced
 __global__ void quirk_kernel(const Geo g, long long period, long long k0, long long k1, unsigned char *__restrict__ marks,
-                             unsigned char *__restrict__ states)
+                             unsigned char *__restrict__ states, const Heads H)
 {
     const long long k = k0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (k >= k1) return;
+    marks = head_at(marks, H.ws);
+    states = head_at(states, H.ws);
     const long long n_all = g.rr * g.res;
     const long long v = k < n_all / period ? (k + 1) * period - 1 : n_all - 1;
     const int x = (int)(v / g.rr), y = (int)((v / g.res) % g.res), z = (int)(v % g.res);
@@ -128,20 +150,24 @@ __global__ void quirk_kernel(const Geo g, long long period, long long k0, long l
 }
 
 // block corners (fine indices 0, B, 2B, ..., res - 1 on every axis; along x those of the slab's planes, L0 B ... X1)
-__global__ void corners_kernel(const Geo g, unsigned char *__restrict__ marks)
+__global__ void corners_kernel(const Geo g, unsigned char *__restrict__ marks, const Heads H)
 {
     const long long n1 = g.nb + 1;
     const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (t >= (g.L1 - g.L0 + 1) * n1 * n1) return;
+    marks = head_at(marks, H.ws);
     const int cz = (int)(t % n1), cy = (int)((t / n1) % n1), cx = g.L0 + (int)(t / (n1 * n1));
     const long long v = vox(g, min(cx * g.B, g.C), min(cy * g.B, g.C), min(cz * g.B, g.C));
     if (marks[v] == kIdle) marks[v] = kWanted;
 }
 
 // an inactive block becomes active when a corner has |sdf| <= tau (or is NaN) or its corners lie on both sides of the test
-__global__ void classify_kernel(const Geo g, float tau, const float *__restrict__ vol, unsigned char *__restrict__ states)
+__global__ void classify_kernel(const Geo g, float tau, const float *__restrict__ vol, unsigned char *__restrict__ states,
+                                const Heads H)
 {
     const long long b = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    states = head_at(states, H.ws);
+    vol = head_vol(vol, H);
     if (b >= g.n_blocks || states[b] != kInactive) return;
     int bx, by, bz;
     unblock(g, b, bx, by, bz);
@@ -159,10 +185,14 @@ __global__ void classify_kernel(const Geo g, float tau, const float *__restrict_
 
 // one warp per block: the voxels of every activated block are wanted (those not evaluated yet); the block becomes active
 __global__ void __launch_bounds__(kThreads) mark_blocks_kernel(const Geo g, unsigned char *__restrict__ states,
-                                                               unsigned char *__restrict__ marks, unsigned long long *__restrict__ hdr)
+                                                               unsigned char *__restrict__ marks, unsigned long long *__restrict__ hdr,
+                                                               const Heads H)
 {
     const long long b = blockIdx.x * (long long)kWarpsPerCta + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
+    states = head_at(states, H.ws);
+    marks = head_at(marks, H.ws);
+    hdr = head_at(hdr, H.ws);
     if (b >= g.n_blocks || states[b] != kActivated) return;
     int bx, by, bz;
     unblock(g, b, bx, by, bz);
@@ -183,10 +213,13 @@ __global__ void __launch_bounds__(kThreads) mark_blocks_kernel(const Geo g, unsi
 // one warp per inactive block: an evaluated voxel on its faces on the other side of the test from its corner 0 (the value its
 // unevaluated voxels get) means the surface leaves the band there - the block is activated
 __global__ void __launch_bounds__(kThreads) grow_kernel(const Geo g, const float *__restrict__ vol, const unsigned char *__restrict__ marks,
-                                                        unsigned char *__restrict__ states)
+                                                        unsigned char *__restrict__ states, const Heads H)
 {
     const long long b = blockIdx.x * (long long)kWarpsPerCta + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
+    states = head_at(states, H.ws);
+    marks = head_at(marks, H.ws);
+    vol = head_vol(vol, H);
     if (b >= g.n_blocks || states[b] != kInactive) return;
     int bx, by, bz;
     unblock(g, b, bx, by, bz);
@@ -206,8 +239,10 @@ __global__ void __launch_bounds__(kThreads) grow_kernel(const Geo g, const float
 
 // every voxel not evaluated takes the value of corner 0 of a block containing it (all such blocks are inactive and on one side)
 // (on a slab the corner lies on the slab's planes too: plane X1 < res - 1 takes corner 0 of block L1, which is on plane X1)
-__global__ void fill_kernel(const Geo g, const unsigned char *__restrict__ marks, float *__restrict__ vol)
+__global__ void fill_kernel(const Geo g, const unsigned char *__restrict__ marks, float *__restrict__ vol, const Heads H)
 {
+    marks = head_at(marks, H.ws);
+    vol = head_vol(vol, H);
     for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < g.n_vox; v += (long long)gridDim.x * blockDim.x) {
         if (marks[v] == kDone) continue;
         const int x = g.X0 + (int)(v / g.rr), y = (int)((v / g.res) % g.res), z = (int)(v % g.res);
@@ -248,8 +283,11 @@ __device__ __forceinline__ unsigned cta_exclusive_scan(unsigned v, unsigned &tot
     return base + inc - v;
 }
 
-__global__ void __launch_bounds__(kThreads) count_kernel(const unsigned char *__restrict__ marks, unsigned *__restrict__ chunk_cnt)
+__global__ void __launch_bounds__(kThreads) count_kernel(const unsigned char *__restrict__ marks, unsigned *__restrict__ chunk_cnt,
+                                                         const Heads H)
 {
+    marks = head_at(marks, H.ws);
+    chunk_cnt = head_at(chunk_cnt, H.ws);
     const uint4 m = __ldg(reinterpret_cast<const uint4 *>(marks + (size_t)blockIdx.x * kChunk) + threadIdx.x);
     uint4 eq;
     unsigned total;
@@ -257,9 +295,14 @@ __global__ void __launch_bounds__(kThreads) count_kernel(const unsigned char *__
     if (threadIdx.x == 0) chunk_cnt[blockIdx.x] = total;
 }
 
+// one CTA per head; {listed, active blocks} also go to pairs[2h..2h+1] (the S heads' counts, read back with one copy)
 __global__ void __launch_bounds__(kScanThreads) scan_kernel(const unsigned *__restrict__ chunk_cnt, unsigned *__restrict__ chunk_off,
-                                                            long long n_chunks, unsigned long long *__restrict__ hdr)
+                                                            long long n_chunks, unsigned long long *__restrict__ hdr, const Heads H,
+                                                            unsigned long long *pairs)      // a single band: pairs == hdr
 {
+    chunk_cnt = head_at(chunk_cnt, H.ws);
+    chunk_off = head_at(chunk_off, H.ws);
+    hdr = head_at(hdr, H.ws);
     const long long per = (n_chunks + kScanThreads - 1) / kScanThreads;
     const long long c0 = threadIdx.x * per, c1 = min(c0 + per, n_chunks);
     unsigned s = 0;
@@ -270,12 +313,21 @@ __global__ void __launch_bounds__(kScanThreads) scan_kernel(const unsigned *__re
         chunk_off[c] = run;
         run += chunk_cnt[c];
     }
-    if (threadIdx.x == 0) hdr[0] = total;
+    if (threadIdx.x == 0) {
+        hdr[0] = total;
+        pairs[2 * blockIdx.y] = total;
+        pairs[2 * blockIdx.y + 1] = hdr[1];
+    }
 }
 
 __global__ void __launch_bounds__(kThreads) emit_kernel(unsigned char *__restrict__ marks, const unsigned *__restrict__ chunk_cnt,
-                                                        const unsigned *__restrict__ chunk_off, unsigned *__restrict__ list)
+                                                        const unsigned *__restrict__ chunk_off, unsigned *__restrict__ list,
+                                                        const Heads H)
 {
+    marks = head_at(marks, H.ws);
+    chunk_cnt = head_at(chunk_cnt, H.ws);
+    chunk_off = head_at(chunk_off, H.ws);
+    list = head_at(list, H.ws);
     if (chunk_cnt[blockIdx.x] == 0) return;
     uint4 *p = reinterpret_cast<uint4 *>(marks + (size_t)blockIdx.x * kChunk) + threadIdx.x;
     uint4 m = *p, eq;
@@ -295,23 +347,30 @@ __global__ void __launch_bounds__(kThreads) emit_kernel(unsigned char *__restric
 }
 
 // ---------------------------------------------------------------------------------------------- lists <-> grid
+// rows of head h: xyz / values rows [h n, h n + n), its listed voxels first.  `pad`: the rows past its count repeat its last listed
+// voxel (voxel 0 of the slab when it listed nothing), so that every row is a grid point of the head; else they are not written.
+// axes: those of head 0's workspace (every head has the same grid).
 __global__ void gather_kernel(const Geo g, const unsigned *__restrict__ list, const unsigned long long *__restrict__ hdr, long long n,
-                              const float *__restrict__ axes, float *__restrict__ xyz)
+                              bool pad, const float *__restrict__ axes, float *__restrict__ xyz, const Heads H)
 {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (i >= n || i >= (long long)hdr[0]) return;
-    const long long v = list[i];
-    xyz[3 * i] = __ldg(axes + g.X0 + v / g.rr);
-    xyz[3 * i + 1] = __ldg(axes + g.res + (v / g.res) % g.res);
-    xyz[3 * i + 2] = __ldg(axes + 2 * g.res + v % g.res);
+    if (i >= n) return;
+    list = head_at(list, H.ws);
+    const long long cnt = (long long)head_at(hdr, H.ws)[0];
+    if (i >= cnt && !pad) return;
+    const long long v = i < cnt ? list[i] : (cnt > 0 ? list[cnt - 1] : 0);
+    float *out = xyz + 3 * (blockIdx.y * n + i);
+    out[0] = __ldg(axes + g.X0 + v / g.rr);
+    out[1] = __ldg(axes + g.res + (v / g.res) % g.res);
+    out[2] = __ldg(axes + 2 * g.res + v % g.res);
 }
 
 __global__ void scatter_kernel(const unsigned *__restrict__ list, const unsigned long long *__restrict__ hdr, long long n,
-                               const float *__restrict__ values, float *__restrict__ vol)
+                               const float *__restrict__ values, float *__restrict__ vol, const Heads H)
 {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (i >= n || i >= (long long)hdr[0]) return;
-    vol[list[i]] = values[i];
+    if (i >= n || i >= (long long)head_at(hdr, H.ws)[0]) return;
+    head_vol(vol, H)[head_at(list, H.ws)[i]] = values[blockIdx.y * n + i];
 }
 
 // ---------------------------------------------------------------------------------------------- boundary planes between slabs
@@ -365,109 +424,138 @@ int check_ws(const Geo &g, const void *ws, long long ws_bytes, const char *who)
 inline float *own(const Geo &g, float *vol) { return vol + g.ghost * g.rr; }
 inline const float *own(const Geo &g, const float *vol) { return vol + g.ghost * g.rr; }
 
-// wanted voxels -> ascending list (and kDone); counts_host (may be NULL: no read-back) = {listed, active blocks}
-int compact(const Geo &g, const Ws &w, long long *counts_host, cudaStream_t stream)
+// S bands of one slab: head 0's geometry and carved workspace, the strides to the others, and where the listing steps put the S
+// {listed, active blocks} pairs (a single band: its own header)
+struct Band {
+    Geo g;
+    Ws w;
+    Heads H;
+    int S;
+    unsigned long long *pairs;
+};
+
+inline dim3 grid2(long long x, int S) { return dim3((unsigned)x, (unsigned)S); }
+
+// wanted voxels -> ascending list (and kDone); counts_host (may be NULL: no read-back) = the S pairs {listed, active blocks}, read
+// back with one copy and one synchronisation whatever S is
+int compact(const Band &b, long long *counts_host, cudaStream_t stream)
 {
-    count_kernel<<<(unsigned)g.n_chunks, kThreads, 0, stream>>>(w.marks, w.chunk_cnt);
+    const Geo &g = b.g;
+    const Ws &w = b.w;
+    count_kernel<<<grid2(g.n_chunks, b.S), kThreads, 0, stream>>>(w.marks, w.chunk_cnt, b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    scan_kernel<<<1, kScanThreads, 0, stream>>>(w.chunk_cnt, w.chunk_off, g.n_chunks, w.hdr);
+    scan_kernel<<<grid2(1, b.S), kScanThreads, 0, stream>>>(w.chunk_cnt, w.chunk_off, g.n_chunks, w.hdr, b.H, b.pairs);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    emit_kernel<<<(unsigned)g.n_chunks, kThreads, 0, stream>>>(w.marks, w.chunk_cnt, w.chunk_off, w.list);
+    emit_kernel<<<grid2(g.n_chunks, b.S), kThreads, 0, stream>>>(w.marks, w.chunk_cnt, w.chunk_off, w.list, b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
     if (counts_host) {
-        unsigned long long h[2];
-        NPHM_CUDA_CHECK(cudaMemcpyAsync(h, w.hdr, sizeof(h), cudaMemcpyDeviceToHost, stream));
+        std::vector<unsigned long long> h(2 * (size_t)b.S);
+        NPHM_CUDA_CHECK(cudaMemcpyAsync(h.data(), b.pairs, h.size() * sizeof(h[0]), cudaMemcpyDeviceToHost, stream));
         NPHM_CUDA_CHECK(cudaStreamSynchronize(stream));
-        counts_host[0] = (long long)h[0];
-        counts_host[1] = (long long)h[1];
+        for (size_t i = 0; i < h.size(); ++i) counts_host[i] = (long long)h[i];
     }
     return NPHM_OK;
 }
 
 // activated blocks -> their voxels not evaluated yet are wanted -> compact
-int mark_and_compact(const Geo &g, const Ws &w, long long *counts_host, cudaStream_t stream)
+int mark_and_compact(const Band &b, long long *counts_host, cudaStream_t stream)
 {
-    mark_blocks_kernel<<<(unsigned)ceil_div(g.n_blocks, kWarpsPerCta), kThreads, 0, stream>>>(g, w.states, w.marks, w.hdr);
+    mark_blocks_kernel<<<grid2(ceil_div(b.g.n_blocks, kWarpsPerCta), b.S), kThreads, 0, stream>>>(b.g, b.w.states, b.w.marks,
+                                                                                                  b.w.hdr, b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    return compact(g, w, counts_host, stream);
+    return compact(b, counts_host, stream);
 }
 
 // ---- the steps on a slab (the entry points below check the arguments)
-int begin(const Geo &g, const Ws &w, long long quirk_period, long long *counts_host, cudaStream_t stream)
+int begin(const Band &b, long long quirk_period, long long *counts_host, cudaStream_t stream)
 {
+    const Geo &g = b.g;
+    const Ws &w = b.w;
     const Layout l = layout(g);
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.hdr, 0, 256, stream));
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.states, 0, g.n_blocks, stream));
-    NPHM_CUDA_CHECK(cudaMemsetAsync(w.marks, 0, l.list - l.marks, stream));
+    for (int h = 0; h < b.S; ++h) {              // one memset per head and region: a 2D memset's pitch is capped below 2^31 bytes
+        char *ws = reinterpret_cast<char *>(w.hdr) + h * b.H.ws;
+        NPHM_CUDA_CHECK(cudaMemsetAsync(ws + l.hdr, 0, 256, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(ws + l.states, 0, g.n_blocks, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(ws + l.marks, 0, l.list - l.marks, stream));
+    }
     if (quirk_period > 0) {
         // the quirk voxels of global flat indices [X0 res^2, (X1 + 1) res^2): k0 = the first with (k + 1) p - 1 >= X0 res^2; the
-        // last voxel of the grid (k = n_all / p when p does not divide n_all) only on the slab that holds it
+        // last voxel of the grid (k = n_all / p when p does not divide n_all) only on the slab that holds it.  They depend only on
+        // res and p, so every head lists the same ones, which the caller evaluates as S queries of period 1.
         const long long n_all = g.rr * g.res, g1 = (g.X1 + 1) * g.rr;
         const long long k0 = g.X0 * g.rr / quirk_period;
         const long long k1 = g1 == n_all ? ceil_div(n_all, quirk_period) : g1 / quirk_period;
         if (k1 > k0) {
-            quirk_kernel<<<(unsigned)ceil_div(k1 - k0, kThreads), kThreads, 0, stream>>>(g, quirk_period, k0, k1, w.marks, w.states);
+            quirk_kernel<<<grid2(ceil_div(k1 - k0, kThreads), b.S), kThreads, 0, stream>>>(g, quirk_period, k0, k1, w.marks, w.states,
+                                                                                           b.H);
             NPHM_CUDA_CHECK(cudaGetLastError());
         }
     }
     // compaction only: the forced blocks' other voxels are listed with the first band pass
-    return compact(g, w, counts_host, stream);
+    return compact(b, counts_host, stream);
 }
 
-int corners(const Geo &g, const Ws &w, long long *counts_host, cudaStream_t stream)
+int corners(const Band &b, long long *counts_host, cudaStream_t stream)
 {
+    const Geo &g = b.g;
     const long long n1 = g.nb + 1;
-    corners_kernel<<<(unsigned)ceil_div((g.L1 - g.L0 + 1) * n1 * n1, kThreads), kThreads, 0, stream>>>(g, w.marks);
+    corners_kernel<<<grid2(ceil_div((g.L1 - g.L0 + 1) * n1 * n1, kThreads), b.S), kThreads, 0, stream>>>(g, b.w.marks, b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
     // the forced blocks stay activated until classify marks them with the blocks it activates
-    return compact(g, w, counts_host, stream);
+    return compact(b, counts_host, stream);
 }
 
-int gather(const Geo &g, const Ws &w, const double grid_min[3], const double grid_max[3], long long n, float *xyz_dev,
+// n: rows per head; pad: see gather_kernel
+int gather(const Band &b, const double grid_min[3], const double grid_max[3], long long n, bool pad, float *xyz_dev,
            cudaStream_t stream)
 {
     if (n == 0) return NPHM_OK;
-    int rc = launch_grid_axes(grid_min, grid_max, g.res, w.axes, stream);
+    int rc = launch_grid_axes(grid_min, grid_max, b.g.res, b.w.axes, stream);
     if (rc) return rc;
-    gather_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, stream>>>(g, w.list, w.hdr, n, w.axes, xyz_dev);
+    gather_kernel<<<grid2(ceil_div(n, kThreads), b.S), kThreads, 0, stream>>>(b.g, b.w.list, b.w.hdr, n, pad, b.w.axes, xyz_dev, b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
 
-int scatter(const Geo &g, const Ws &w, long long n, const float *values_dev, float *vol_dev, cudaStream_t stream)
+int scatter(const Band &b, long long n, const float *values_dev, float *vol_dev, cudaStream_t stream)
 {
     if (n == 0) return NPHM_OK;
-    scatter_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, stream>>>(w.list, w.hdr, n, values_dev, own(g, vol_dev));
+    scatter_kernel<<<grid2(ceil_div(n, kThreads), b.S), kThreads, 0, stream>>>(b.w.list, b.w.hdr, n, values_dev, own(b.g, vol_dev),
+                                                                               b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
 
-int classify(const Geo &g, const Ws &w, float tau, const float *vol_dev, long long *counts_host, cudaStream_t stream)
+int classify(const Band &b, float tau, const float *vol_dev, long long *counts_host, cudaStream_t stream)
 {
-    classify_kernel<<<(unsigned)ceil_div(g.n_blocks, kThreads), kThreads, 0, stream>>>(g, tau, own(g, vol_dev), w.states);
+    classify_kernel<<<grid2(ceil_div(b.g.n_blocks, kThreads), b.S), kThreads, 0, stream>>>(b.g, tau, own(b.g, vol_dev), b.w.states,
+                                                                                           b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    return mark_and_compact(g, w, counts_host, stream);
+    return mark_and_compact(b, counts_host, stream);
 }
 
-int grow(const Geo &g, const Ws &w, const float *vol_dev, long long *counts_host, cudaStream_t stream)
+int grow(const Band &b, const float *vol_dev, long long *counts_host, cudaStream_t stream)
 {
-    grow_kernel<<<(unsigned)ceil_div(g.n_blocks, kWarpsPerCta), kThreads, 0, stream>>>(g, own(g, vol_dev), w.marks, w.states);
+    grow_kernel<<<grid2(ceil_div(b.g.n_blocks, kWarpsPerCta), b.S), kThreads, 0, stream>>>(b.g, own(b.g, vol_dev), b.w.marks,
+                                                                                           b.w.states, b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    return mark_and_compact(g, w, counts_host, stream);
+    return mark_and_compact(b, counts_host, stream);
 }
 
-int fill(const Geo &g, const Ws &w, float *vol_dev, cudaStream_t stream)
+int fill(const Band &b, float *vol_dev, cudaStream_t stream)
 {
-    const long long ctas = std::min(ceil_div(g.n_vox, kThreads), 64LL * sm_count());
-    fill_kernel<<<(unsigned)ctas, kThreads, 0, stream>>>(g, w.marks, own(g, vol_dev));
+    const long long ctas = std::min(ceil_div(b.g.n_vox, kThreads), 64LL * sm_count());
+    fill_kernel<<<grid2(ctas, b.S), kThreads, 0, stream>>>(b.g, b.w.marks, own(b.g, vol_dev), b.H);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }
 
-int block_states(const Geo &g, const void *ws, unsigned char *states_dev, cudaStream_t stream)
+// states_dev: S x n_blocks bytes
+int block_states(const Band &b, unsigned char *states_dev, cudaStream_t stream)
 {
-    NPHM_CUDA_CHECK(cudaMemcpyAsync(states_dev, static_cast<const char *>(ws) + layout(g).states, g.n_blocks, cudaMemcpyDeviceToDevice,
-                                    stream));
+    for (int h = 0; h < b.S; ++h)
+        NPHM_CUDA_CHECK(cudaMemcpyAsync(states_dev + h * b.g.n_blocks, b.w.states + h * b.H.ws, b.g.n_blocks, cudaMemcpyDeviceToDevice,
+                                        stream));
     return NPHM_OK;
 }
 
@@ -482,7 +570,8 @@ using namespace nphm;
     const band::Geo g = band::make_geo(res, block, l0, l1);                 \
     if ((rc = band::check_ws(g, ws, ws_bytes, who))) return rc;             \
     const band::Ws w = band::carve(const_cast<void *>(static_cast<const void *>(ws)), band::layout(g)); \
-    (void)w;                                                                \
+    const band::Band b{g, w, band::Heads{band::layout(g).bytes, 0}, 1, w.hdr}; \
+    (void)b;                                                                \
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
 
 // ---------------------------------------------------------------------------------------------- entry points
@@ -497,14 +586,14 @@ extern "C" int nphm_band_slab_begin(int res, int block, int l0, int l1, long lon
 {
     SLAB_PROLOGUE("nphm_band_slab_begin")
     NPHM_REQUIRE(quirk_period >= 0, "nphm_band_slab_begin: negative quirk period %lld", quirk_period);
-    return band::begin(g, w, quirk_period, counts_host, stream);
+    return band::begin(b, quirk_period, counts_host, stream);
 }
 
 extern "C" int nphm_band_slab_corners(int res, int block, int l0, int l1, void *ws, long long ws_bytes, long long *counts_host,
                                       void *stream_)
 {
     SLAB_PROLOGUE("nphm_band_slab_corners")
-    return band::corners(g, w, counts_host, stream);
+    return band::corners(b, counts_host, stream);
 }
 
 extern "C" int nphm_band_slab_gather(int res, int block, int l0, int l1, const double grid_min[3], const double grid_max[3],
@@ -512,7 +601,7 @@ extern "C" int nphm_band_slab_gather(int res, int block, int l0, int l1, const d
 {
     SLAB_PROLOGUE("nphm_band_slab_gather")
     NPHM_REQUIRE(grid_min && grid_max && n >= 0 && n <= g.n_vox && (n == 0 || xyz_dev), "nphm_band_slab_gather: bad arguments");
-    return band::gather(g, w, grid_min, grid_max, n, xyz_dev, stream);
+    return band::gather(b, grid_min, grid_max, n, false, xyz_dev, stream);
 }
 
 extern "C" int nphm_band_slab_scatter(int res, int block, int l0, int l1, long long n, const float *values_dev, float *vol_dev,
@@ -520,7 +609,7 @@ extern "C" int nphm_band_slab_scatter(int res, int block, int l0, int l1, long l
 {
     SLAB_PROLOGUE("nphm_band_slab_scatter")
     NPHM_REQUIRE(n >= 0 && n <= g.n_vox && vol_dev && (n == 0 || values_dev), "nphm_band_slab_scatter: bad arguments");
-    return band::scatter(g, w, n, values_dev, vol_dev, stream);
+    return band::scatter(b, n, values_dev, vol_dev, stream);
 }
 
 extern "C" int nphm_band_slab_classify(int res, int block, int l0, int l1, float tau, const float *vol_dev, void *ws,
@@ -528,7 +617,7 @@ extern "C" int nphm_band_slab_classify(int res, int block, int l0, int l1, float
 {
     SLAB_PROLOGUE("nphm_band_slab_classify")
     NPHM_REQUIRE(tau >= 0.f && vol_dev, "nphm_band_slab_classify: need tau >= 0 (got %g) and a volume", (double)tau);
-    return band::classify(g, w, tau, vol_dev, counts_host, stream);
+    return band::classify(b, tau, vol_dev, counts_host, stream);
 }
 
 extern "C" int nphm_band_slab_grow(int res, int block, int l0, int l1, const float *vol_dev, void *ws, long long ws_bytes,
@@ -536,14 +625,14 @@ extern "C" int nphm_band_slab_grow(int res, int block, int l0, int l1, const flo
 {
     SLAB_PROLOGUE("nphm_band_slab_grow")
     NPHM_REQUIRE(vol_dev, "nphm_band_slab_grow: NULL volume");
-    return band::grow(g, w, vol_dev, counts_host, stream);
+    return band::grow(b, vol_dev, counts_host, stream);
 }
 
 extern "C" int nphm_band_slab_fill(int res, int block, int l0, int l1, float *vol_dev, void *ws, long long ws_bytes, void *stream_)
 {
     SLAB_PROLOGUE("nphm_band_slab_fill")
     NPHM_REQUIRE(vol_dev, "nphm_band_slab_fill: NULL volume");
-    return band::fill(g, w, vol_dev, stream);
+    return band::fill(b, vol_dev, stream);
 }
 
 extern "C" int nphm_band_slab_block_states(int res, int block, int l0, int l1, const void *ws, long long ws_bytes,
@@ -551,7 +640,7 @@ extern "C" int nphm_band_slab_block_states(int res, int block, int l0, int l1, c
 {
     SLAB_PROLOGUE("nphm_band_slab_block_states")
     NPHM_REQUIRE(states_dev, "nphm_band_slab_block_states: NULL output");
-    return band::block_states(g, ws, states_dev, stream);
+    return band::block_states(b, states_dev, stream);
 }
 
 extern "C" int nphm_band_slab_export(int res, int block, int l0, int l1, int plane, const float *vol_dev, const void *ws,
@@ -586,4 +675,107 @@ extern "C" int nphm_band_slab_import(int res, int block, int l0, int l1, int pla
         g, plane, vals, buf_dev + 4 * g.rr, band::own(g, vol_dev), w.marks);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- S heads of one whole grid
+namespace nphm {
+namespace band {
+
+// workspace of S heads: the S {listed, active blocks} pairs, then S band workspaces of the whole grid at a stride of their bytes
+inline long long pairs_bytes(int S) { return (16LL * S + 255) / 256 * 256; }
+inline long long heads_bytes(const Geo &g, int S) { return pairs_bytes(S) + S * layout(g).bytes; }
+
+int check_heads(int res, int block, int S, const char *who)
+{
+    int rc = check_args(res, block, 0, 1, who);
+    if (rc) return rc;
+    NPHM_REQUIRE(S >= 1 && S <= 65535, "%s: %d heads outside [1, 65535]", who, S);
+    return NPHM_OK;
+}
+
+}  // namespace band
+}  // namespace nphm
+
+#define HEADS_PROLOGUE(who)                                                                                   \
+    int rc = band::check_heads(res, block, n_heads, who);                                                     \
+    if (rc) return rc;                                                                                        \
+    const band::Geo g = band::make_geo(res, block, 0, band::blocks_per_axis(res, block));                     \
+    NPHM_REQUIRE(ws, "%s: NULL workspace", who);                                                              \
+    if (ws_bytes < band::heads_bytes(g, n_heads)) {                                                           \
+        set_error("%s: band workspace too small: %lld bytes for %d heads of res %d, block %d, %lld needed", who, ws_bytes, n_heads, \
+                  res, block, band::heads_bytes(g, n_heads));                                                 \
+        return NPHM_ERR_CAPACITY;                                                                             \
+    }                                                                                                         \
+    char *ws0 = static_cast<char *>(const_cast<void *>(static_cast<const void *>(ws)));                       \
+    const band::Band b{g, band::carve(ws0 + band::pairs_bytes(n_heads), band::layout(g)),                     \
+                       band::Heads{band::layout(g).bytes, g.n_vox}, n_heads, reinterpret_cast<unsigned long long *>(ws0)}; \
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+
+extern "C" long long nphm_band_heads_workspace_bytes(int res, int block, int n_heads)
+{
+    if (band::check_heads(res, block, n_heads, "nphm_band_heads_workspace_bytes")) return -1;
+    return band::heads_bytes(band::make_geo(res, block, 0, band::blocks_per_axis(res, block)), n_heads);
+}
+
+extern "C" int nphm_band_heads_begin(int res, int block, int n_heads, long long quirk_period, void *ws, long long ws_bytes,
+                                     long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_begin")
+    NPHM_REQUIRE(quirk_period >= 0, "nphm_band_heads_begin: negative quirk period %lld", quirk_period);
+    return band::begin(b, quirk_period, counts_host, stream);
+}
+
+extern "C" int nphm_band_heads_corners(int res, int block, int n_heads, void *ws, long long ws_bytes, long long *counts_host,
+                                       void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_corners")
+    return band::corners(b, counts_host, stream);
+}
+
+extern "C" int nphm_band_heads_classify(int res, int block, int n_heads, float tau, const float *vols_dev, void *ws, long long ws_bytes,
+                                        long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_classify")
+    NPHM_REQUIRE(tau >= 0.f && vols_dev, "nphm_band_heads_classify: need tau >= 0 (got %g) and volumes", (double)tau);
+    return band::classify(b, tau, vols_dev, counts_host, stream);
+}
+
+extern "C" int nphm_band_heads_grow(int res, int block, int n_heads, const float *vols_dev, void *ws, long long ws_bytes,
+                                    long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_grow")
+    NPHM_REQUIRE(vols_dev, "nphm_band_heads_grow: NULL volumes");
+    return band::grow(b, vols_dev, counts_host, stream);
+}
+
+extern "C" int nphm_band_heads_gather(int res, int block, int n_heads, const double grid_min[3], const double grid_max[3],
+                                      long long n_pad, float *xyz_dev, void *ws, long long ws_bytes, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_gather")
+    NPHM_REQUIRE(grid_min && grid_max && n_pad >= 0 && n_pad <= g.n_vox && (n_pad == 0 || xyz_dev),
+                 "nphm_band_heads_gather: bad arguments");
+    return band::gather(b, grid_min, grid_max, n_pad, true, xyz_dev, stream);
+}
+
+extern "C" int nphm_band_heads_scatter(int res, int block, int n_heads, long long n_pad, const float *values_dev, float *vols_dev,
+                                       void *ws, long long ws_bytes, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_scatter")
+    NPHM_REQUIRE(n_pad >= 0 && n_pad <= g.n_vox && vols_dev && (n_pad == 0 || values_dev), "nphm_band_heads_scatter: bad arguments");
+    return band::scatter(b, n_pad, values_dev, vols_dev, stream);
+}
+
+extern "C" int nphm_band_heads_fill(int res, int block, int n_heads, float *vols_dev, void *ws, long long ws_bytes, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_fill")
+    NPHM_REQUIRE(vols_dev, "nphm_band_heads_fill: NULL volumes");
+    return band::fill(b, vols_dev, stream);
+}
+
+extern "C" int nphm_band_heads_block_states(int res, int block, int n_heads, const void *ws, long long ws_bytes,
+                                            unsigned char *states_dev, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_heads_block_states")
+    NPHM_REQUIRE(states_dev, "nphm_band_heads_block_states: NULL output");
+    return band::block_states(b, states_dev, stream);
 }

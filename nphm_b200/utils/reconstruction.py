@@ -276,31 +276,42 @@ def narrowband_volume(evaluate, mini, maxi, resolution, device, block=4, margin=
     return vol, stats, band
 
 
-def _band_evaluators(decoder, encoding, device):
-    """(evaluate, evaluate_quirk | None) for the decoders whose native query gives every point a value independent of the other
-    points of its call, or None (then the caller extracts densely)."""
+def _heads_evaluators(decoder, codes, device):
+    """(evaluate, evaluate_quirk | None) on ``S x n x 3`` points -> ``S x n`` values, head h under ``codes[h]`` (``codes`` S x D),
+    for the decoders whose native query gives every point a value independent of the other points and heads of its call: one
+    ``nphm_ensemble_query`` with S latents, or one ``nphm_mlp_query`` with S condition rows.  None for the other decoders (then the
+    caller extracts densely)."""
     from ..models.EnsembledDeepSDF import FastEnsembleDeepSDFMirrored
     from ..models.deepSDF import DeepSDF
     if device.type != 'cuda':
         return None
+    S = codes.shape[0]
     if isinstance(decoder, FastEnsembleDeepSDFMirrored):
         engine = decoder.engine()
-        lat = encoding.reshape(1, -1).to(device)
+        lat = codes.reshape(S, -1).to(device)
 
         def query(pts, quirk):
-            sdf, _ = engine.query(pts[None], lat, eval_quirk=quirk, quirk_period=1 if quirk else None)
-            return sdf.reshape(-1)
+            sdf, _ = engine.query(pts, lat, eval_quirk=quirk, quirk_period=1 if quirk else None)
+            return sdf.reshape(S, -1)
         return (lambda pts: query(pts, False)), (lambda pts: query(pts, True))
     if isinstance(decoder, DeepSDF) and decoder.out_dim_net == 1:
-        code = encoding.reshape(1, 1, -1).to(device)
+        code = codes.reshape(S, 1, -1).to(device)
         with torch.no_grad():
-            if not decoder._fused_ok(torch.zeros(1, 1, 3, device=device), code):
+            if not decoder._fused_ok(torch.zeros(S, 1, 3, device=device), code):
                 return None
 
         def evaluate(pts):
-            return decoder(pts[None], code.expand(1, pts.shape[0], code.shape[-1]), None)[0].reshape(-1)
+            return decoder(pts, code.expand(S, pts.shape[1], code.shape[-1]), None)[0].reshape(S, -1)
         return evaluate, None
     return None
+
+
+def _band_evaluators(decoder, encoding, device):
+    """:func:`_heads_evaluators` of one code, on ``(n, 3)`` points -> ``(n,)`` values."""
+    fns = _heads_evaluators(decoder, encoding.reshape(1, -1), device)
+    if fns is None:
+        return None
+    return tuple(None if f is None else (lambda pts, f=f: f(pts[None]).reshape(-1)) for f in fns)
 
 
 def extract_mesh_narrowband(decoder, encoding, mini, maxi, resolution, nbatch_points=100000, block=4, margin=None,
@@ -378,3 +389,157 @@ def extract_mesh_narrowband_slabs(decoder, encoding, mini, maxi, resolution, wor
     res = int(resolution)
     return _run_band(decoder, encoding, mini, maxi, res, nbatch_points, block, margin, plan_block_slabs(res, block, world),
                      lambda plan: plan, LocalExchange(world), return_stats, sparse)
+
+
+# ------------------------------------------------------------------------------------------ many heads in one band run
+PAD_ROWS = 128                    # the head-major rows of a round are padded to a multiple of one decoder tile
+
+
+def pad_rows(counts, multiple: int = PAD_ROWS) -> int:
+    """Rows per head of a round in which the heads listed ``counts`` voxels: the largest count rounded up to ``multiple``."""
+    m = max(int(c) for c in counts)
+    return -(-m // multiple) * multiple
+
+
+def split_heads(flat: torch.Tensor, counts) -> List[torch.Tensor]:
+    """The parts of ``flat`` (rows one head after the other) with ``counts[h]`` rows each."""
+    out, c = [], 0
+    for n in counts:
+        out.append(flat[c:c + int(n)])
+        c += int(n)
+    return out
+
+
+def plan_head_chunks(n_heads: int, bytes_per_head: int, budget_bytes: int, max_heads: Optional[int] = None) -> List[Tuple[int, int]]:
+    """Heads ``[h0, h1)`` of each chunk, in order: as many heads per chunk as ``budget_bytes`` holds at ``bytes_per_head`` (at least
+    one, at most ``max_heads``), every chunk that size but the last."""
+    per = max(1, int(budget_bytes) // max(int(bytes_per_head), 1))
+    if max_heads is not None:
+        if int(max_heads) < 1:
+            raise ValueError('max_heads must be >= 1 (got %r)' % (max_heads,))
+        per = min(per, int(max_heads))
+    return [(h, min(h + per, n_heads)) for h in range(0, n_heads, per)]
+
+
+def _as_codes(encodings) -> torch.Tensor:
+    """``S x D`` tensor or a list of codes (any shape of D elements each) -> ``S x D``."""
+    if isinstance(encodings, torch.Tensor):
+        if encodings.dim() < 1 or encodings.shape[0] == 0:
+            raise ValueError('extract_meshes_narrowband: no latent codes')
+        return encodings.reshape(encodings.shape[0], -1)
+    codes = [torch.as_tensor(e).reshape(-1) for e in encodings]
+    if not codes:
+        raise ValueError('extract_meshes_narrowband: no latent codes')
+    widths = sorted({c.numel() for c in codes})
+    if len(widths) > 1:
+        raise ValueError('extract_meshes_narrowband: the codes have different widths %s' % widths)
+    return torch.stack([c.to(codes[0].device) for c in codes])
+
+
+def narrowband_heads_volumes(bands, evaluate, mini, maxi, tau: float, quirk_period: int = 0, evaluate_quirk=None):
+    """:func:`narrowband_slab_volumes` on the whole grid for the S heads of ``bands`` (a :class:`_native.NarrowBandHeads`) in
+    lockstep, with ``evaluate(points S x n_pad x 3 float32 CUDA) -> values S x n_pad``: the same steps in the same order, each one
+    launch sequence and one count read-back for all heads, and one evaluation per round for all heads that listed something.  A
+    round's rows are padded to :func:`pad_rows` of its counts.  The band runs until no head's growth step lists anything; a head
+    that has closed lists nothing in the later rounds, so each head's volume is the one its single band gives.  Returns
+    ``(volumes (S, res, res, res), stats)``: per head ``blocks_active``, ``voxels_evaluated``, ``growth_rounds`` (the rounds in
+    which it listed voxels) and ``padded_rows`` (rows evaluated on its behalf beyond its count)."""
+    if quirk_period and evaluate_quirk is None:
+        raise ValueError('narrowband_heads_volumes: quirk_period > 0 needs evaluate_quirk')
+    S = bands.n_heads
+    vols = bands.volumes()
+    evaluated, padded, rounds = [0] * S, [0] * S, [0] * S
+
+    def run(ns, fn):
+        if not any(ns):
+            return
+        n_pad = pad_rows(ns)
+        bands.scatter(fn(bands.gather(n_pad, mini, maxi)), vols)
+        for h, n in enumerate(ns):
+            evaluated[h] += n
+            padded[h] += n_pad - n
+
+    ns = bands.begin(quirk_period)
+    if quirk_period:
+        run(ns, evaluate_quirk)
+    run(bands.corners(), evaluate)
+    run(bands.classify(tau, vols), evaluate)
+    while True:
+        ns = bands.grow(vols)
+        if not any(ns):
+            break
+        for h, n in enumerate(ns):
+            rounds[h] += n > 0
+        run(ns, evaluate)
+    bands.fill(vols)
+    stats = [{'blocks_active': int(bands.active_blocks[h]), 'voxels_evaluated': evaluated[h], 'growth_rounds': rounds[h],
+              'padded_rows': padded[h]} for h in range(S)]
+    return vols, stats
+
+
+def _device_meshes(verts, tris, counts, mini, maxi, resolution):
+    """:func:`_device_mesh` of each head's part of :meth:`_native.NarrowBandHeads.marching_cubes`, with one host copy for all."""
+    dev = verts.device
+    step = (np.array(maxi) - np.array(mini)) / (resolution - 1)
+    v_host, t_host = _to_host(verts), _to_host(tris).view(np.uint64)
+    dev_verts = verts * torch.as_tensor(step, device=dev) + torch.as_tensor(np.asarray(mini, dtype=np.float64), device=dev)
+    nv, nt = [c[0] for c in counts], [c[1] for c in counts]
+    meshes = []
+    for v, t, dv in zip(np.split(v_host, np.cumsum(nv)[:-1]), np.split(t_host, np.cumsum(nt)[:-1]), split_heads(dev_verts, nv)):
+        vertices = v * np.expand_dims(step, axis=0)
+        vertices += [mini[0], mini[1], mini[2]]
+        mesh = make_mesh(vertices, t)
+        if len(mesh.vertices) == dv.shape[0]:
+            try:
+                mesh._nphm_device_vertices = dv.to(torch.float32)
+            except AttributeError:
+                pass
+        meshes.append(mesh)
+    return meshes
+
+
+def extract_meshes_narrowband(decoder, encodings, mini, maxi, resolution, nbatch_points=100000, block=4, margin=None,
+                              return_stats=False, max_heads=None, sparse=False):
+    """The meshes of ``extract_mesh_narrowband(decoder, encodings[h], ...)`` for S latent codes of one decoder in one band run
+    (DESIGN §4.18): every step of the band one launch sequence and one read-back for all heads, each round one decoder query for
+    all heads, and one marching-cubes count and emit for all.  Head h's mesh is bit for bit the single-head one (vertex ids,
+    float64 positions, triangles), and so the dense ``mesh_from_logits(get_logits(...))`` mesh whenever that one is.
+
+    ``encodings``: an ``S x D`` tensor or a list of codes.  ``decoder.training`` is honoured as in :func:`extract_mesh_narrowband`.
+    Heads run in chunks of as many as half the free device memory holds, at :meth:`_native.NarrowBandHeads.device_bytes_per_head`
+    plus 16 bytes of query rows per voxel, and at most ``max_heads``; chunking changes no mesh.
+    Returns the list of S meshes, and with ``return_stats`` also the list of S stats dicts of :func:`extract_mesh_narrowband`, each
+    with ``padded_rows``, the rows evaluated on the head's behalf beyond its voxels (0 when nothing is padded).  Decoders or
+    devices without a native band query, and ``sparse=True`` (not batched: the sparse band runs once per head), extract head by
+    head with :func:`extract_mesh_narrowband`."""
+    codes = _as_codes(encodings)
+    S, res = codes.shape[0], int(resolution)
+    device = next(decoder.parameters()).device
+    fns = _heads_evaluators(decoder, codes[:1], device)
+    if fns is None or sparse:
+        meshes, stats = [], []
+        for h in range(S):
+            m, st = extract_mesh_narrowband(decoder, codes[h:h + 1], mini, maxi, res, nbatch_points=nbatch_points, block=block,
+                                            margin=margin, return_stats=True, sparse=sparse)
+            meshes.append(m)
+            stats.append(dict(st, padded_rows=0))
+        return (meshes, stats) if return_stats else meshes
+    quirk_period = 0 if (decoder.training or fns[1] is None) else int(nbatch_points)
+    tau = default_margin(mini, maxi, res, block) if margin is None else float(margin)
+    per_head = _native.NarrowBandHeads.device_bytes_per_head(res, block) + 16 * res ** 3
+    budget = torch.cuda.mem_get_info(device)[0] // 2
+    meshes, stats = [], []
+    with torch.no_grad(), torch.cuda.device(device):
+        for h0, h1 in plan_head_chunks(S, per_head, budget, max_heads):
+            ev, evq = _heads_evaluators(decoder, codes[h0:h1], device)
+            bands = _native.NarrowBandHeads(res, block, device, h1 - h0)
+            vols, st = narrowband_heads_volumes(bands, ev, mini, maxi, tau, quirk_period, evq)
+            verts, tris, counts = bands.marching_cubes(vols)
+            del vols
+            meshes += _device_meshes(verts, tris, counts, mini, maxi, res)
+            nb = bands.blocks_per_axis
+            stats += [{'blocks_active': s['blocks_active'], 'blocks_total': nb ** 3, 'voxels_evaluated': s['voxels_evaluated'],
+                       'voxels_total': res ** 3, 'growth_rounds': s['growth_rounds'], 'margin': tau, 'padded_rows': s['padded_rows']}
+                      for s in st]
+            del bands
+    return (meshes, stats) if return_stats else meshes
