@@ -315,11 +315,13 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     p.blocked = 0; p.px0 = p.px1 = 0; p.by = p.bz = 1; p.tbx = p.tby = p.tbz = 1;
     long long n_tiles = ceil_div(q.n_points, 128) * q.n_queries;
     if ((prune || p.zero_skip) && !q.xyz && q.n_points > 0) {
-        // compact blocks over the x-plane range that contains [first, first + n_points), so that a tile is near few anchors:
-        // 8 x 4 x 4 for the pruned rule (its mask depends on the composition of a tile), 1 x 16 x 8 for the dense rule - it
-        // never crosses an x-plane, so plane-aligned ranges (the whole grid, x-slabs) tile without wasted rows
+        // compact blocks over the x-plane range that contains [first, first + n_points), so that a tile is near few anchors
+        // and few absorption boundaries: 8 x 4 x 4 for the pruned rule (its mask depends on the composition of a tile) and
+        // for dense ranges of whole 8-plane groups (the whole grid); 1 x 16 x 8 for other dense ranges - it never crosses an
+        // x-plane, so x-slabs with ghost planes tile without wasted rows.  tools/zero_member_tiles.py:tile_layout mirrors this.
         const long long rr = (long long)q.res * q.res;
-        const int tbx = prune ? 8 : 1, tby = prune ? 4 : 16, tbz = prune ? 4 : 8;
+        const bool cube = prune || (q.first % rr == 0 && q.n_points % (8 * rr) == 0);
+        const int tbx = cube ? 8 : 1, tby = cube ? 4 : 16, tbz = cube ? 4 : 8;
         const int px0 = (int)(q.first / rr), px1 = (int)((q.first + q.n_points - 1) / rr);
         const int by = (q.res + tby - 1) / tby, bz = (q.res + tbz - 1) / tbz;
         const long long blocked_tiles = (long long)((px1 - px0 + tbx) / tbx) * by * bz;

@@ -329,10 +329,13 @@ def grid_setup(latent_seed, scale=1.0):
     return P32, P64, z, anc32
 
 
-def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride=1, chunk_tiles=1024, quirk_period=0):
+def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride=1, chunk_tiles=1024, quirk_period=0,
+            tile='auto', planes=None):
     """dict of member-tile counts on the res^3 grid with the kernel's dense tiles (with plane_stride > 1: on the tiles of
     every plane_stride-th x-plane).  quirk_period > 0: the eval-mode query's quirk rows (grid index g % period == period - 1
-    and the last point) blend 1.0 for every member, as in the kernel."""
+    and the last point of the grid) blend 1.0 for every member, as in the kernel.  tile: as in zero_member_tiles.tile_layout
+    for the whole grid.  planes = (x0, x1): only the tiles of x-planes x0 .. x1 - 1 of that layout; a block shape must not
+    cross x0 or x1, so that the counts are those of the whole-grid query on these planes."""
     import torch
     from conftest import MAXI, MINI
     from ensemble_f64_common import members
@@ -347,8 +350,13 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
     hi = np.array([axes[a].max() for a in range(3)], np.float64)
     B = np.array([member_bound(P64, m, z, anc_np.astype(np.float64), lo, hi) for m in range(M)])
     count = res ** 3
-    kind, block = tile_layout(res, 0, count, 'auto')
+    kind, block = tile_layout(res, 0, count, tile)
     ix, iy, iz, valid = tile_points(res, 0, count, kind, block)
+    if planes is not None:
+        x0, x1 = planes
+        assert kind == 'blocked' and x0 % block[0] == 0 and x1 % block[0] == 0, 'planes must be whole blocks deep'
+        keep = (ix[:, 0] >= x0) & (ix[:, 0] < x1)
+        ix, iy, iz, valid = ix[keep], iy[keep], iz[keep], valid[keep]
     if plane_stride > 1:
         # a sample of the grid: the tiles of every plane_stride-th x-plane (a dense tile never crosses a plane)
         keep = ix[:, 0] % plane_stride == 0
@@ -446,11 +454,17 @@ def main():
     ap.add_argument('--scale', type=float, default=1.0)
     ap.add_argument('--plane-stride', type=int, default=1, help='count the tiles of every n-th x-plane only (dense tiles)')
     ap.add_argument('--quirk-period', type=int, default=0, help='quirk period of the query (bench.py and ens_trace.py: 25000)')
+    ap.add_argument('--tile', default='auto', help='auto or a block shape XxYxZ with X*Y*Z = 128 (zero_member_tiles.py)')
+    ap.add_argument('--planes', type=int, nargs=2, metavar=('X0', 'X1'), default=None,
+                    help='count the tiles of x-planes X0 .. X1-1 only (multiples of the block depth): compares layouts fairly')
     args = ap.parse_args()
-    r = predict(args.latent, args.res, args.scale, plane_stride=args.plane_stride, quirk_period=args.quirk_period)
+    r = predict(args.latent, args.res, args.scale, plane_stride=args.plane_stride, quirk_period=args.quirk_period,
+                tile=args.tile, planes=args.planes)
     ev = r['evaluated_now']
     if args.plane_stride > 1:
         print('tiles of every %d-th x-plane' % args.plane_stride)
+    if args.planes:
+        print('tiles of x-planes %d .. %d' % (args.planes[0], args.planes[1] - 1))
     print('latent %d, %d^3 grid: %d tiles, %d member-tiles, %d evaluated with the zero-weight skip; den half holds on %d '
           '(%.1f %%), the tile-wide rule (the kernel before per-point) on %d (%.1f %%) -> %d evaluated'
           % (args.latent, args.res, r['tiles'], r['member_tiles'], ev, r['den_absorbed'], 100 * r['den_absorbed'] / ev,

@@ -11,8 +11,8 @@ a prediction: the -DNPHM_ENS_TRACE build (tools/ens_trace.py) measures the membe
     python tools/zero_member_tiles.py [--latent 1] [--res 256] [--tile auto|linear|XxYxZ] [--first F --count N]
                                       [--mini X Y Z --maxi X Y Z]
 
---tile auto picks the tiles the kernel picks for the dense path: 1 x 16 x 8 blocks, or 128 consecutive points where blocks
-would add more than 3 % tiles."""
+--tile auto picks the tiles the kernel picks for the dense path: 8 x 4 x 4 blocks over a whole number of 8-plane groups (the
+whole grid), 1 x 16 x 8 blocks over other x-plane ranges, or 128 consecutive points where blocks would add more than 3 % tiles."""
 import argparse
 import os
 import sys
@@ -23,7 +23,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
-DENSE_BLOCK = (1, 16, 8)
+DENSE_BLOCK = (8, 4, 4)          # x-ranges of whole 8-plane groups
+SLAB_BLOCK = (1, 16, 8)          # other x-ranges: a block never crosses an x-plane
 
 
 def parse_args(argv=None):
@@ -53,13 +54,13 @@ def tile_layout(res, first, count, tile):
     """(kind, block) as the kernel chooses it: ('linear', None) or ('blocked', (tbx, tby, tbz))."""
     if tile == 'linear':
         return 'linear', None
+    rr = res * res
     if tile == 'auto':
-        block = DENSE_BLOCK
+        block = DENSE_BLOCK if first % rr == 0 and count % (DENSE_BLOCK[0] * rr) == 0 else SLAB_BLOCK
     else:
         block = tuple(int(v) for v in tile.split('x'))
         assert len(block) == 3 and np.prod(block) == 128, 'a block has 128 points'
     tbx, tby, tbz = block
-    rr = res * res
     px0, px1 = first // rr, (first + count - 1) // rr
     blocked = ((px1 - px0 + tbx) // tbx) * ((res + tby - 1) // tby) * ((res + tbz - 1) // tbz)
     if tile == 'auto' and blocked * 100 > -(-count // 128) * 103:
