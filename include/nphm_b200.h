@@ -137,6 +137,18 @@ int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n_queries, l
                             float cvg_thresh, float dvg_thresh, float eps, float *diff_dev,
                             unsigned char *valid_dev, int *steps_done, void *workspace_dev, void *stream);
 
+/* nphm_mlp_broyden_search with the same arguments and bitwise the same x, diff and valid, for large point sets where most
+ * samples freeze early: every step compacts each query's live samples into an ordered row list (per-query prefix of the
+ * active flags), and only those rows go through the network and the 3x3 update.  The launches keep their full grids and
+ * read the per-query live counts on the device; the CTAs beyond a query's count return at once, so the call stays
+ * sync-free (CUDA-graph capturable) when steps_done is NULL.
+ *   workspace_dev: nphm_broyden_compact_workspace_bytes(n_queries, n_points) bytes. */
+long long nphm_broyden_compact_workspace_bytes(int n_queries, long long n_points);
+int nphm_mlp_broyden_search_compact(nphm_mlp *h, const float *cond_dev, int n_queries, long long n_points,
+                                    const float *obs_dev, float *x_dev, const float *jinv_init_dev, int max_steps,
+                                    float cvg_thresh, float dvg_thresh, float eps, float *diff_dev,
+                                    unsigned char *valid_dev, int *steps_done, void *workspace_dev, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Marching cubes == mcubes.marching_cubes(volume, iso) as called at utils/reconstruction.py:30
  * (PyMCubes semantics restated in oracle/mc_oracle.c: x-major cell order, `<=` classification, one vertex per

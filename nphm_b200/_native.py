@@ -36,7 +36,8 @@ EXPORTED_SYMBOLS = (
     'nphm_fit_identity_step_quirk', 'nphm_fit_surface_grad_quirk', 'nphm_fit_identity_step_batched_quirk',
     'nphm_fit_surface_grad_batched_quirk', 'nphm_ensemble_backward_inputs_quirk',
     'nphm_ensemble_backward_inputs', 'nphm_ensemble_anchors',
-    'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_nearest_neighbors',
+    'nphm_broyden_workspace_bytes', 'nphm_mlp_broyden_search', 'nphm_broyden_compact_workspace_bytes',
+    'nphm_mlp_broyden_search_compact', 'nphm_nearest_neighbors',
     'nphm_mlp_train_workspace_bytes', 'nphm_mlp_train_forward', 'nphm_mlp_train_backward',
     'nphm_mlp_sdfgrad_workspace_bytes', 'nphm_mlp_sdfgrad_forward', 'nphm_mlp_sdfgrad_backward',
     'nphm_mlp_fit_workspace_bytes', 'nphm_mlp_fit_surface_grad', 'nphm_mlp_fit_surface_grad_batched',
@@ -195,6 +196,9 @@ def lib() -> ctypes.CDLL:
     L.nphm_mlp_broyden_search.argtypes = [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_int,
                                           c_float, c_float, c_float, c_void_p, c_void_p, POINTER(c_int), c_void_p,
                                           c_void_p]
+    L.nphm_broyden_compact_workspace_bytes.argtypes = [c_int, c_longlong]
+    L.nphm_broyden_compact_workspace_bytes.restype = c_longlong
+    L.nphm_mlp_broyden_search_compact.argtypes = L.nphm_mlp_broyden_search.argtypes
     L.nphm_nearest_neighbors.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p]
     L.nphm_mlp_train_workspace_bytes.argtypes = [c_void_p, c_int, c_longlong, c_int]
     L.nphm_mlp_train_workspace_bytes.restype = c_longlong
@@ -766,9 +770,11 @@ class MlpEngine(_Versioned):
 
     def broyden_search(self, obs: torch.Tensor, cond: torch.Tensor, x_init: torch.Tensor, J_inv_init: torch.Tensor,
                        max_steps: int = 15, cvg_thresh: float = 1e-6, dvg_thresh: float = 0.2, eps: float = 1e-6,
-                       early_exit: bool = True):
+                       early_exit: bool = True, compact: bool = False):
         """Roots of ``x + F(x; cond) - obs`` by the reference's Broyden iteration, entirely on the device.
-        obs, x_init: B x N x 3, cond: B x lat_dim, J_inv_init: B x N x 3 x 3.
+        obs, x_init: B x N x 3, cond: B x lat_dim, J_inv_init: B x N x 3 x 3.  ``compact``: each step runs the network and
+        the update on the still-live samples only (nphm_mlp_broyden_search_compact; bitwise the same result), for point sets
+        large enough that the frozen samples dominate.
         Returns ``(x B x N x 3, diff B x N, valid B x N bool, steps taken)``."""
         B, N, _ = obs.shape
         dev = obs.device
@@ -780,12 +786,16 @@ class MlpEngine(_Versioned):
         valid = torch.empty(B, N, device=dev, dtype=torch.uint8)
         steps = c_int(0)
         with torch.cuda.device(dev):
-            ws = torch.empty(max(int(lib().nphm_broyden_workspace_bytes(B * N)), 256), device=dev, dtype=torch.uint8)
-            check(lib().nphm_mlp_broyden_search(self._h, cond.data_ptr(), B, N, obs.data_ptr(), x.data_ptr(),
-                                                jinv.data_ptr(), int(max_steps), float(cvg_thresh), float(dvg_thresh),
-                                                float(eps), diff.data_ptr(), valid.data_ptr(),
-                                                byref(steps) if early_exit else None,       # None: no host sync, all steps run
-                                                ws.data_ptr(), _stream_ptr(dev)), 'nphm_mlp_broyden_search')
+            if compact:
+                nbytes, fn = lib().nphm_broyden_compact_workspace_bytes(B, N), 'nphm_mlp_broyden_search_compact'
+            else:
+                nbytes, fn = lib().nphm_broyden_workspace_bytes(B * N), 'nphm_mlp_broyden_search'
+            ws = torch.empty(max(int(nbytes), 256), device=dev, dtype=torch.uint8)
+            check(getattr(lib(), fn)(self._h, cond.data_ptr(), B, N, obs.data_ptr(), x.data_ptr(),
+                                     jinv.data_ptr(), int(max_steps), float(cvg_thresh), float(dvg_thresh),
+                                     float(eps), diff.data_ptr(), valid.data_ptr(),
+                                     byref(steps) if early_exit else None,       # None: no host sync, all steps run
+                                     ws.data_ptr(), _stream_ptr(dev)), fn)
         return x, diff, valid.bool(), steps.value
 
 

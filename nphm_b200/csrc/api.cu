@@ -360,7 +360,7 @@ int mlp_run(nphm_mlp *h, const float *xyz_dev, int n_queries, long long n_points
     if (use_tc) return chain_forward(h, xyz_dev, n_queries, n_points, out_dev, stream);
     SimtQuery q{};
     q.xyz = xyz_dev; q.total = n_points; q.n_points = n_points; q.n_queries = n_queries; q.quirk_period = 0;
-    q.cvec = h->cvec.as<float>(); q.anchors = nullptr; q.blend = 0; q.out = out_dev;
+    q.cvec = h->cvec.as<float>(); q.anchors = nullptr; q.blend = 0; q.out = out_dev; q.live_rows = h->live_rows;
     return launch_folded_net(h->net, q, stream);
 }
 }  // namespace nphm

@@ -10,6 +10,9 @@
 // once diff <= cvg or its current norm >= dvg; b = vT.dgx is pushed away from zero by +-eps before the division.
 #include "engine.cuh"
 #include "simt.cuh"
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
+#include <climits>
 
 namespace nphm {
 int mlp_prepare(nphm_mlp *h, const float *cond_dev, int n_queries, cudaStream_t stream);
@@ -59,16 +62,16 @@ __global__ void advance_kernel(State s, long long n)
     for (int c = 0; c < 3; ++c) s.x[i * 3 + c] += s.upd[i * 3 + c];
 }
 
-// after F(x) is available: residual bookkeeping, freeze test, rank-one update of J_inv, next step
-__global__ void update_kernel(State s, const float *__restrict__ obs, long long n, float cvg, float dvg, float eps)
+// after F(x) is available (f: the network output of sample i): residual bookkeeping, freeze test, rank-one update of J_inv,
+// next step
+__device__ __forceinline__ void update_sample(const State &s, long long i, const float *f, const float *__restrict__ obs,
+                                              float cvg, float dvg, float eps)
 {
-    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (i >= n || !s.active[i]) return;
     float dx[3], dg[3], g[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         dx[c] = s.upd[i * 3 + c];
-        const float gnew = (s.f[i * 3 + c] + s.x[i * 3 + c]) - obs[i * 3 + c];
+        const float gnew = (f[c] + s.x[i * 3 + c]) - obs[i * 3 + c];
         const float gold = s.gx[i * 3 + c];
         dg[c] = gnew - gold;
         g[c] = gold + dg[c];                                  // gx[ids] += delta_gx[ids]
@@ -103,6 +106,48 @@ __global__ void update_kernel(State s, const float *__restrict__ obs, long long 
     for (int r = 0; r < 3; ++r) s.upd[i * 3 + r] = -(J[r * 3] * g[0] + J[r * 3 + 1] * g[1] + J[r * 3 + 2] * g[2]);
 }
 
+__global__ void update_kernel(State s, const float *__restrict__ obs, long long n, float cvg, float dvg, float eps)
+{
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= n || !s.active[i]) return;
+    update_sample(s, i, s.f + i * 3, obs, cvg, dvg, eps);
+}
+
+// ---- compacting variant: slot k < cnt[q] of query q (rows q * n_points + k of the row list) holds live sample
+// q * n_points + idx[k]; the network reads xc and writes s.f in slot order
+
+// the sample of slot k, or -1 beyond its query's live count
+__device__ __forceinline__ long long slot_sample(const int *idx, const int *cnt, long long n_points, long long k)
+{
+    const long long q = k / n_points;
+    return k - q * n_points < cnt[q] ? q * n_points + idx[k] : -1;
+}
+
+// x += update of every live sample (advance_kernel), and its copy into slot order
+__global__ void gather_advance_kernel(State s, const int *__restrict__ idx, const int *__restrict__ cnt, long long n_points,
+                                      long long n, float *__restrict__ xc)
+{
+    const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const long long i = slot_sample(idx, cnt, n_points, k);
+    if (i < 0) return;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        s.x[i * 3 + c] += s.upd[i * 3 + c];
+        xc[k * 3 + c] = s.x[i * 3 + c];
+    }
+}
+
+__global__ void update_compact_kernel(State s, const int *__restrict__ idx, const int *__restrict__ cnt, long long n_points,
+                                      const float *__restrict__ obs, long long n, float cvg, float dvg, float eps)
+{
+    const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const long long i = slot_sample(idx, cnt, n_points, k);
+    if (i < 0) return;
+    update_sample(s, i, s.f + k * 3, obs, cvg, dvg, eps);
+}
+
 __global__ void finish_kernel(State s, long long n, float cvg, float *diff, unsigned char *valid)
 {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -126,17 +171,46 @@ extern "C" long long nphm_broyden_workspace_bytes(long long n_total)
     return (long long)(align256(n * 9 * 4) + 3 * align256(n * 3 * 4) + align256(n * 4) + align256(n) + 1024);
 }
 
-extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n_queries, long long n_points,
-                                       const float *obs_dev, float *x_dev, const float *jinv_init_dev, int max_steps,
-                                       float cvg_thresh, float dvg_thresh, float eps, float *diff_dev,
-                                       unsigned char *valid_dev, int *steps_done, void *workspace_dev, void *stream_)
+// the compacting search's buffers (Compact::carve): slot list, live counts, points in slot order, CUB scratch
+struct Compact {
+    int *idx = nullptr, *cnt = nullptr;
+    float *xc = nullptr;
+    void *scratch = nullptr;
+    size_t scratch_bytes = 0;
+};
+
+static size_t select_scratch_bytes(long long n_points)
 {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    NPHM_REQUIRE(h && h->loaded, "nphm_mlp_broyden_search: weights not loaded");
-    NPHM_REQUIRE(h->cfg.out_dim == 3, "nphm_mlp_broyden_search: the field must have 3 outputs (has %d)", h->cfg.out_dim);
-    NPHM_REQUIRE(n_queries >= 1 && n_points >= 0 && max_steps >= 0, "nphm_mlp_broyden_search: bad sizes");
+    size_t bytes = 0;
+    cub::DeviceSelect::Flagged(nullptr, bytes, thrust::counting_iterator<int>(0), (const unsigned char *)nullptr, (int *)nullptr,
+                               (int *)nullptr, (int)n_points);
+    return bytes;
+}
+
+static size_t compact_extra_bytes(int n_queries, long long n_points)
+{
+    const size_t n = (size_t)n_queries * n_points;
+    return align256(n * 4) + align256(n * 12) + align256((size_t)n_queries * 4) + align256(select_scratch_bytes(n_points));
+}
+
+extern "C" long long nphm_broyden_compact_workspace_bytes(int n_queries, long long n_points)
+{
+    if (n_queries < 1 || n_points < 0 || n_points > INT_MAX) return NPHM_ERR_INVALID;
+    return nphm_broyden_workspace_bytes((long long)n_queries * n_points) + (long long)compact_extra_bytes(n_queries, n_points);
+}
+
+// the dense search (every step evaluates all samples, frozen ones are ignored) or the compacting one
+static int broyden_search(const char *who, nphm_mlp *h, const float *cond_dev, int n_queries, long long n_points,
+                          const float *obs_dev, float *x_dev, const float *jinv_init_dev, int max_steps, float cvg_thresh,
+                          float dvg_thresh, float eps, float *diff_dev, unsigned char *valid_dev, int *steps_done,
+                          void *workspace_dev, cudaStream_t stream, bool compact)
+{
+    NPHM_REQUIRE(h && h->loaded, "%s: weights not loaded", who);
+    NPHM_REQUIRE(h->cfg.out_dim == 3, "%s: the field must have 3 outputs (has %d)", who, h->cfg.out_dim);
+    NPHM_REQUIRE(n_queries >= 1 && n_points >= 0 && max_steps >= 0, "%s: bad sizes", who);
+    NPHM_REQUIRE(!compact || n_points <= INT_MAX, "%s: at most 2^31 - 1 points per query", who);
     NPHM_REQUIRE(cond_dev && (n_points == 0 || (obs_dev && x_dev && jinv_init_dev && diff_dev && valid_dev && workspace_dev)),
-                 "nphm_mlp_broyden_search: NULL pointer");
+                 "%s: NULL pointer", who);
     if (steps_done) *steps_done = 0;
     const long long n = n_points * n_queries;
     if (n == 0) return NPHM_OK;
@@ -150,7 +224,16 @@ extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n
     s.best = reinterpret_cast<float *>(p); p += align256((size_t)n * 4);
     s.active = reinterpret_cast<unsigned char *>(p); p += align256((size_t)n);
     int *counters = reinterpret_cast<int *>(p);              // one counter per step (max 255), zeroed once
-    NPHM_REQUIRE(max_steps < 255, "nphm_mlp_broyden_search: max_steps must be < 255");
+    p += 1024;
+    Compact cmp;
+    if (compact) {
+        cmp.idx = reinterpret_cast<int *>(p); p += align256((size_t)n * 4);
+        cmp.xc = reinterpret_cast<float *>(p); p += align256((size_t)n * 12);
+        cmp.cnt = reinterpret_cast<int *>(p); p += align256((size_t)n_queries * 4);
+        cmp.scratch = p;
+        cmp.scratch_bytes = select_scratch_bytes(n_points);
+    }
+    NPHM_REQUIRE(max_steps < 255, "%s: max_steps must be < 255", who);
     NPHM_CUDA_CHECK(cudaMemsetAsync(counters, 0, 1024, stream));
     s.n_active = counters;
     NPHM_CUDA_CHECK(cudaMemcpyAsync(s.jinv, jinv_init_dev, (size_t)n * 36, cudaMemcpyDeviceToDevice, stream));
@@ -163,18 +246,36 @@ extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n
     NPHM_CUDA_CHECK(cudaGetLastError());
     int done = 0;
     for (int step = 0; step < max_steps; ++step) {
-        broyden::advance_kernel<<<blocks, 256, 0, stream>>>(s, n);
-        NPHM_CUDA_CHECK(cudaGetLastError());
-        // once nobody is active (counter of the previous step == 0) the network evaluation returns at once: a device-side
-        // early exit that needs no host synchronisation (the reference leaves its loop at that point)
-        // once nobody is active (counter of the previous step == 0) the network evaluation returns at once: a device-side
-        // early exit that needs no host synchronisation (the reference leaves its loop at that point)
-        h->live = step > 0 ? counters + (step - 1) : nullptr;
-        rc = mlp_run(h, s.x, n_queries, n_points, s.f, NPHM_IMPL_AUTO, stream);
-        h->live = nullptr;
-        if (rc) return rc;
-        s.n_active = counters + step;
-        broyden::update_kernel<<<blocks, 256, 0, stream>>>(s, obs_dev, n, cvg_thresh, dvg_thresh, eps);
+        if (compact) {
+            // ordered per-query compaction of the active flags: slot k of query q <- its k-th live sample; the launches below
+            // keep their full grids and return at once beyond the counts, so no host synchronisation is needed
+            for (int q = 0; q < n_queries; ++q) {
+                size_t bytes = cmp.scratch_bytes;
+                NPHM_CUDA_CHECK(cub::DeviceSelect::Flagged(cmp.scratch, bytes, thrust::counting_iterator<int>(0),
+                                                           s.active + (size_t)q * n_points, cmp.idx + (size_t)q * n_points,
+                                                           cmp.cnt + q, (int)n_points, stream));
+            }
+            broyden::gather_advance_kernel<<<blocks, 256, 0, stream>>>(s, cmp.idx, cmp.cnt, n_points, n, cmp.xc);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+            h->live_rows = cmp.cnt;
+            rc = mlp_run(h, cmp.xc, n_queries, n_points, s.f, NPHM_IMPL_AUTO, stream);
+            h->live_rows = nullptr;
+            if (rc) return rc;
+            s.n_active = counters + step;
+            broyden::update_compact_kernel<<<blocks, 256, 0, stream>>>(s, cmp.idx, cmp.cnt, n_points, obs_dev, n, cvg_thresh,
+                                                                       dvg_thresh, eps);
+        } else {
+            broyden::advance_kernel<<<blocks, 256, 0, stream>>>(s, n);
+            NPHM_CUDA_CHECK(cudaGetLastError());
+            // once nobody is active (counter of the previous step == 0) the network evaluation returns at once: a device-side
+            // early exit that needs no host synchronisation (the reference leaves its loop at that point)
+            h->live = step > 0 ? counters + (step - 1) : nullptr;
+            rc = mlp_run(h, s.x, n_queries, n_points, s.f, NPHM_IMPL_AUTO, stream);
+            h->live = nullptr;
+            if (rc) return rc;
+            s.n_active = counters + step;
+            broyden::update_kernel<<<blocks, 256, 0, stream>>>(s, obs_dev, n, cvg_thresh, dvg_thresh, eps);
+        }
         NPHM_CUDA_CHECK(cudaGetLastError());
         done = step + 1;
         // optional host-side early exit (4-byte read-back + stream sync every kCheckEvery steps); a caller that passes
@@ -191,4 +292,24 @@ extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n
     NPHM_CUDA_CHECK(cudaGetLastError());
     if (steps_done) *steps_done = done;
     return NPHM_OK;
+}
+
+extern "C" int nphm_mlp_broyden_search(nphm_mlp *h, const float *cond_dev, int n_queries, long long n_points,
+                                       const float *obs_dev, float *x_dev, const float *jinv_init_dev, int max_steps,
+                                       float cvg_thresh, float dvg_thresh, float eps, float *diff_dev,
+                                       unsigned char *valid_dev, int *steps_done, void *workspace_dev, void *stream)
+{
+    return broyden_search("nphm_mlp_broyden_search", h, cond_dev, n_queries, n_points, obs_dev, x_dev, jinv_init_dev, max_steps,
+                          cvg_thresh, dvg_thresh, eps, diff_dev, valid_dev, steps_done, workspace_dev,
+                          static_cast<cudaStream_t>(stream), false);
+}
+
+extern "C" int nphm_mlp_broyden_search_compact(nphm_mlp *h, const float *cond_dev, int n_queries, long long n_points,
+                                               const float *obs_dev, float *x_dev, const float *jinv_init_dev, int max_steps,
+                                               float cvg_thresh, float dvg_thresh, float eps, float *diff_dev,
+                                               unsigned char *valid_dev, int *steps_done, void *workspace_dev, void *stream)
+{
+    return broyden_search("nphm_mlp_broyden_search_compact", h, cond_dev, n_queries, n_points, obs_dev, x_dev, jinv_init_dev,
+                          max_steps, cvg_thresh, dvg_thresh, eps, diff_dev, valid_dev, steps_done, workspace_dev,
+                          static_cast<cudaStream_t>(stream), true);
 }

@@ -80,6 +80,7 @@ struct nphm_mlp {
     nphm::PackSpec spec;
     nphm::DeviceBuffer cvec;
     const int *live = nullptr;      // set around an evaluation by the Broyden loop: device counter, 0 = skip the evaluation
+    const int *live_rows = nullptr; // set by the compacting Broyden loop: per-query device counts, rows beyond them are skipped
     // layer-by-layer tensor-core passes: any width, Jacobian, adjoint (mlp_chain.cu)
     nphm::MlpChain *chain = nullptr;
 };

@@ -257,6 +257,7 @@ struct ValueRows {
     float *S[kMaxLayers] = {}; long long sS[kMaxLayers] = {};               // s_l, blocked (optional)
     float *out = nullptr; long long sOut = 0;                                // the output layer, row-major
     const int *live = nullptr;                                               // see forward_pass
+    const int *live_rows = nullptr; long long live_off = 0;                  // see forward_pass
 };
 
 // value pass: softplus layers 0 .. n_lin - 2 and the linear output layer
@@ -268,6 +269,7 @@ static int value_layers(const Stack &k, long long M, const ValueRows &v, cudaStr
         tcl::LinearParams p;
         p.M = M; p.batch = k.m.count; p.w_pairs = k.m.n_symm;
         p.live = v.live;
+        p.live_rows = v.live_rows; p.live_off = v.live_off;
         if (l == 0) { p.A1 = v.X; p.lda1 = v.ldx; p.K1 = 3 + v.nd; p.sA1 = v.sX; }
         else { p.Ap = v.Hp[l - 1]; p.a_ksteps = W.ksteps; p.sAp = v.sHp[l - 1]; }   // at the skip layer: [h | xyz | noise]
         p.bias = v.bias + s.coff[l]; p.ldb = s.cvec_stride; p.rows_per_bias = v.rows_per_bias; p.sBias = v.sBias;
@@ -314,10 +316,11 @@ static int value_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_
 // Forward only (no derivatives kept), in chunks of at most kForwardChunkRows rows through two ping-pong operand buffers: the
 // memory it needs is bounded by the chunk (2 x 128 MB for the deformation backbone), not by the number of points, so a whole
 // 256^3 grid can be queried in one call.  Chunks hold whole queries, or a run of rows of one query.  `live` (optional device
-// counter): every launch returns at once when it reads 0.
+// counter): every launch returns at once when it reads 0.  `live_rows` (optional, per query): only the points below it are
+// computed, the tiles beyond it return at once.
 constexpr long long kForwardChunkRows = 1 << 16;
 static int forward_pass(nphm_mlp *h, const float *xyz, int n_queries, long long n_points, float *out, const int *live,
-                        cudaStream_t stream)
+                        const int *live_rows, cudaStream_t stream)
 {
     if (n_points == 0) return NPHM_OK;
     MlpChain &c = *h->chain;
@@ -341,6 +344,7 @@ static int forward_pass(nphm_mlp *h, const float *xyz, int n_queries, long long 
             v.X = xyz + row0 * 3;
             v.bias = h->cvec.as<float>() + (size_t)q0 * s.cvec_stride; v.rows_per_bias = np;
             v.out = out + row0 * out_dim;
+            if (live_rows) { v.live_rows = live_rows + q0; v.live_off = p0; }
             if ((rc = value_layers(stack(h), nq * np, v, stream))) return rc;
         }
     }
@@ -460,7 +464,7 @@ int chain_forward(nphm_mlp *h, const float *xyz, int n_queries, long long n_poin
 {
     int rc = chain_ready(h, "chain_forward");
     if (rc) return rc;
-    return forward_pass(h, xyz, n_queries, n_points, out, h->live, stream);
+    return forward_pass(h, xyz, n_queries, n_points, out, h->live, h->live_rows, stream);
 }
 }  // namespace nphm
 
@@ -475,7 +479,7 @@ extern "C" int nphm_mlp_query_layers(nphm_mlp *h, const float *xyz_dev, const fl
     if (n_points == 0) return NPHM_OK;
     NPHM_REQUIRE(xyz_dev && out_dev, "nphm_mlp_query_layers: NULL pointer");
     if ((rc = mlp_prepare(h, cond_dev, n_queries, stream))) return rc;
-    return forward_pass(h, xyz_dev, n_queries, n_points, out_dev, nullptr, stream);
+    return forward_pass(h, xyz_dev, n_queries, n_points, out_dev, nullptr, nullptr, stream);
 }
 
 // value + forward-mode tangents: out [q][n][out_dim] (optional), jac [q][n][out_dim][3] = d out / d xyz

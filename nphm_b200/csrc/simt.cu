@@ -31,6 +31,7 @@ __global__ void __launch_bounds__(256) folded_net_kernel(const FoldedNet net, co
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int qi = (int)(tile / tiles_per_query);
         const long long p0 = (tile - (long long)qi * tiles_per_query) * P;
+        if (q.live_rows && p0 >= q.live_rows[qi]) continue;          // uniform over the CTA
 
         float x[TM], y[TM], z[TM];
         bool quirk[TM];

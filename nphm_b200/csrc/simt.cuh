@@ -22,6 +22,7 @@ struct SimtQuery {
     unsigned char *acts_packed_out;   // goes with acts_out, see tc::Params::acts_packed_out
     int acts_packed_tile_steps;
     int exact;                // 1: never use the opt-in pruned mode for this query (fitting needs every member)
+    const int *live_rows;     // optional (plain MLP): query q computes only its points below live_rows[q] (device counts)
 };
 
 // description of the reference-layout parameters, used by the packing / cvec kernels

@@ -79,10 +79,20 @@ __device__ long long g_tcl_trace[16 * 64];
 
 // MODE and PACKED_C (packed output present) are compile-time: the epilogue is the longest part of a latency-bound layer and
 // loses ~a fifth of its instructions when the per-unit mode / layout tests disappear
+// whether any row of the 128-row tile at row0 is inside its query's live prefix (LinearParams::live_rows)
+__device__ __forceinline__ bool tile_live(const LinearParams &p, long long row0)
+{
+    const long long R = p.rows_per_bias, last = min(row0 + 127, p.M - 1);
+    for (long long q = row0 / R; q <= last / R; ++q)
+        if (p.live_rows[q] - p.live_off > max(row0 - q * R, 0LL)) return true;
+    return false;
+}
+
 template <int MODE, bool PACKED_C>
 __global__ void __launch_bounds__(kThreads, 1) linear_tc_kernel(const LinearParams p)
 {
     if (p.live && *p.live == 0) return;                 // uniform over the grid (Broyden: every sample of the search is frozen)
+    if (p.live_rows && !tile_live(p, (long long)blockIdx.x * 128)) return;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     Ctl &sm = *reinterpret_cast<Ctl *>(smem_raw);
     const int kStages = p.stages;

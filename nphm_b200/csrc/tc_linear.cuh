@@ -41,6 +41,9 @@ struct LinearParams {
     // and (strides in floats / bytes) bias + z sBias, Dv + z sDv, app + z sApp, cpl_z + z sCplZ, cpl_a + z sCplA
     long long sBias = 0, sDv = 0, sApp = 0, sCplZ = 0, sCplA = 0;
     const int *live = nullptr;                               // optional device counter: the launch does nothing when *live == 0
+    // optional per-query live prefix (the compacting Broyden search): query q = row / rows_per_bias keeps only its rows below
+    // live_rows[q] - live_off; a CTA none of whose 128 rows is kept returns at once
+    const int *live_rows = nullptr; long long live_off = 0;
     // filled by launch_linear from the packed weights
     const uint8_t *W = nullptr; long long w_stride = 0; int N = 0, Nt = 0, ksteps = 0, stages = 0;
 };

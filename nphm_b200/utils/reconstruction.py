@@ -543,3 +543,55 @@ def extract_meshes_narrowband(decoder, encodings, mini, maxi, resolution, nbatch
                       for s in st]
             del bands
     return (meshes, stats) if return_stats else meshes
+
+
+# ------------------------------------------------------------------------------------------ posed meshes
+def extract_posed_meshes_narrowband(decoder_shape, decoder_expr, lat_rep_shape, lat_reps_expr, mini, maxi, resolution,
+                                    nbatch_points=100000, block=4, margin=None, return_stats=False, max_heads=None):
+    """The posed meshes ``mesh_from_logits(get_logits_posed(decoder_shape, decoder_expr, lat_rep_shape, lat_reps_expr, grid,
+    nbatch_points)[s], mini, maxi, resolution)`` of the S expression codes (``(S, E)``, ``(S, 1, E)`` or ``(E,)``), bit for bit
+    (vertex ids, float64 positions, triangles), from the head-batched narrow band of :func:`extract_meshes_narrowband` with the
+    posed query as its evaluator: the expressions are the heads, and every round runs one native posed query for all of them
+    (:func:`nphm_b200.models.reconstruction.posed_evaluator`).
+
+    The band is exact when every piece of the posed surface inside a block outside the band reaches one of its faces.  The
+    default ``margin`` (:func:`default_margin`) guarantees that for a posed field with ``|grad| <= 2``; the posed field's
+    gradient is ``grad sdf(xc) (I + dF_ex/dx)^-1`` at the root, so a deformation that compresses space raises it above the
+    identity SDF's, and ``margin`` (SDF units) is the override for such fields.  Decoders or devices without the native posed
+    query take the dense ``get_logits_posed`` and ``mesh_from_logits``.  ``return_stats``: also the S stats dicts of
+    :func:`extract_meshes_narrowband`."""
+    from ..models.EnsembledDeepSDF import FastEnsembleDeepSDFMirrored
+    from ..models.reconstruction import _expression_codes, get_logits_posed, posed_evaluator
+    codes, _ = _expression_codes(lat_reps_expr)
+    S, res = codes.shape[0], int(resolution)
+    device = next(decoder_shape.parameters()).device
+    fn = posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes[:1])
+    if fn is None:
+        grid = torch.from_numpy(create_grid_points_from_bounds(mini, maxi, res)).to(device, dtype=torch.float32)
+        logits = get_logits_posed(decoder_shape, decoder_expr, lat_rep_shape, codes, grid[None], nbatch_points=nbatch_points)
+        meshes = [mesh_from_logits(logits[s], mini, maxi, res) for s in range(S)]
+        n = res ** 3
+        stats = [{'blocks_active': None, 'blocks_total': None, 'voxels_evaluated': n, 'voxels_total': n, 'growth_rounds': 0,
+                  'margin': None, 'padded_rows': 0} for _ in range(S)]
+        return (meshes, stats) if return_stats else meshes
+    quirk = not decoder_shape.training and isinstance(decoder_shape, FastEnsembleDeepSDFMirrored)
+    quirk_period = int(nbatch_points) if quirk else 0
+    tau = default_margin(mini, maxi, res, block) if margin is None else float(margin)
+    per_head = _native.NarrowBandHeads.device_bytes_per_head(res, block) + 16 * res ** 3
+    budget = torch.cuda.mem_get_info(device)[0] // 2
+    meshes, stats = [], []
+    with torch.no_grad(), torch.cuda.device(device):
+        for h0, h1 in plan_head_chunks(S, per_head, budget, max_heads):
+            fn = posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes[h0:h1])
+            bands = _native.NarrowBandHeads(res, block, device, h1 - h0)
+            vols, st = narrowband_heads_volumes(bands, lambda pts: fn(pts)[0], mini, maxi, tau, quirk_period,
+                                                (lambda pts: fn(pts, quirk=True)[0]) if quirk else None)
+            verts, tris, counts = bands.marching_cubes(vols)
+            del vols
+            meshes += _device_meshes(verts, tris, counts, mini, maxi, res)
+            nb = bands.blocks_per_axis
+            stats += [{'blocks_active': s['blocks_active'], 'blocks_total': nb ** 3, 'voxels_evaluated': s['voxels_evaluated'],
+                       'voxels_total': res ** 3, 'growth_rounds': s['growth_rounds'], 'margin': tau, 'padded_rows': s['padded_rows']}
+                      for s in st]
+            del bands
+    return (meshes, stats) if return_stats else meshes
