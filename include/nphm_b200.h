@@ -222,9 +222,12 @@ int nphm_fit_identity_step(nphm_ensemble *h, const float *points_dev, long long 
  * (reference src/NPHM/models/fitting.py:114-125: `sdf = decoder(xc, lat_rep_shape)`, `sdf[valid_ids]`, `l[l < clamp].mean()`):
  *   loss = mean over { p : mask[p] != 0 and |sdf_p| < clamp } of |sdf_p|        (training-mode forward, no eval quirk)
  * mask_dev (n_points bytes, may be NULL = all valid).  loss_terms_dev[0] = loss (NaN if nothing is kept, like torch),
- * [5] = number of kept points, [1..4] = the latent regularisers (unweighted).  grad_latent_dev (lat_dim) and
+ * [5] = number of kept points, [1..4] = the latent regularisers (unweighted).  grad_latent_dev (lat_dim, may be NULL) and
  * grad_points_dev (n_points*3, may be NULL) receive d loss / d latent (member inputs + anchors/mlp_pos + blend weights) and
- * d loss / d point (local coordinates of every member + blend weights); both are zero when nothing is kept.
+ * d loss / d point (local coordinates of every member + blend weights); both are zero when nothing is kept.  With
+ * grad_latent_dev NULL (a fit that holds the identity code fixed) the tensor-core path skips the latent-only work - the member
+ * input column sums, the anchor part of the blend path and the mlp_pos backward - and loss_terms_dev / grad_points_dev are
+ * bitwise those of the call with a gradient: every sum they take runs in a fixed order.
  * The latent is not modified.  Same workspace as nphm_fit_identity_step.  Needs the tensor-core configuration when
  * grad_points_dev is given. */
 int nphm_fit_surface_grad(nphm_ensemble *h, const float *points_dev, long long n_points, const float *latent_dev,
@@ -410,7 +413,7 @@ int nphm_fit_identity_step_batched(nphm_ensemble *h, const float *points_dev, co
                                    long long n_points, float *latents_dev, float *adam_m_dev, float *adam_v_dev,
                                    const nphm_fit_params *fp, int apply_update, float *loss_terms_dev, float *grad_out_dev,
                                    void *workspace_dev, long long workspace_bytes, void *stream);
-/* == nphm_fit_surface_grad per scan; loss_terms_dev and grad_latent_dev are required */
+/* == nphm_fit_surface_grad per scan; loss_terms_dev is required, grad_latent_dev may be NULL as there */
 int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev, int n_scans,
                                   long long n_points, const float *latents_dev, float clamp, float *loss_terms_dev,
                                   float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, long long workspace_bytes,

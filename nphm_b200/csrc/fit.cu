@@ -69,8 +69,12 @@ struct Buffers {
                                     // the backward GEMMs overwrite them with the layer deltas
     float *out, *S, *gsign;         // n each
     float *acc;                     // members x 2H   (sum delta0 | sum delta2)
-    float *blend_acc;               // n_loc x 3
+    float *blend_acc;               // n_loc x 3 (NULL: no latent gradient is wanted, the anchor part of the blend path is skipped)
     float *stats;                   // [count, sum |sdf| kept, -, -]
+    float *sum_part;                // optional [scan][warp]: fit_blend_kernel's per-warp sums of |sdf| kept, which
+                                    // fit_finalize_kernel adds in warp order (stats[1] then stays 0): a reproducible loss
+    float *points_part;             // optional: the per-member point gradients of fit_reduce_kernel<true>, [member][tile][3][128]
+                                    // (over the activation blocks, dead by then), added in member order by fit_points_kernel
     float *ganch;                   // n_loc x 3
     float *grad;                    // lat_dim
     const float *upstream;          // optional n: d L / d sdf_p given by the caller (nphm_ensemble_backward_inputs) instead of the
@@ -289,7 +293,7 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
             }
             gs[(size_t)m * gs_stride + scan * b.tiles_per_scan * 128 + i_scan] = gsv;
         }
-        if (has_anchor) {
+        if (has_anchor && b.blend_acc) {
 #pragma unroll
             for (int a = 0; a < 3; ++a) {
                 float v = c[a];
@@ -300,20 +304,21 @@ __global__ void __launch_bounds__(256) fit_upstream_kernel(const Dims d, const B
         }
     }
     if (ok && b.grad_points) { b.grad_points[idx * 3] = gx[0]; b.grad_points[idx * 3 + 1] = gx[1]; b.grad_points[idx * 3 + 2] = gx[2]; }
+    if (!b.blend_acc) return;
     __syncthreads();
     for (int i = threadIdx.x; i < d.n_loc * 3; i += blockDim.x)
         if (s_acc[i] != 0.f) atomicAdd(b.blend_acc + (size_t)scan * d.n_loc * 3 + i, s_acc[i]);
 }
 
-// one CTA per (128-point tile, member): g_s-weighted sums of delta0 / delta2 over the points (-> acc) and (POINTS) the gradient
-// w.r.t. every point through the member's local coordinates.  The deltas come operand-ready from the GEMMs (packed: per k-step
-// of 16 features [128 x 16 fp16 hi | 128 x 16 fp16 lo], value = hi + lo).
+// one CTA per (128-point tile, member): (LATENT) g_s-weighted sums of delta0 / delta2 over the points (-> acc) and (POINTS) the
+// gradient w.r.t. every point through the member's local coordinates (-> points_part).  The deltas come operand-ready from the
+// GEMMs (packed: per k-step of 16 features [128 x 16 fp16 hi | 128 x 16 fp16 lo], value = hi + lo).
 constexpr int kReduceThreads = 256;
 constexpr float kDeltaScale = 64.0f;          // the GEMMs carry the deltas per unit upstream gradient, times this power of two: the
                                               // fp16 hi/lo operand split needs O(1) magnitudes (g_s itself is ~1e-4 / n_points)
 constexpr int kStepsH = 13, kStepsN1 = 7;     // packed k-steps of a hidden-width (200) / layer-1-width (101) block
 constexpr int kPackedPerTile = 2 * kStepsH + kStepsN1;      // [sigma'3 -> delta2 | delta1 | delta0]
-template <bool POINTS>
+template <bool POINTS, bool LATENT>
 __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d, const Weights w, const Buffers b,
                                                                    const uint8_t *__restrict__ packed, long long tiles,
                                                                    const float *__restrict__ gs)
@@ -381,12 +386,14 @@ __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d
                     for (int a = 0; a < 3; ++a) gp[i][a] = fmaf(wa[a], v0, fmaf(wb[a], v1, gp[i][a]));
                 }
             }
-            // sum over the 8 rows of the group (lane bits 2..4), then over the row groups through shared memory
+            if (LATENT) {
+                // sum over the 8 rows of the group (lane bits 2..4), then over the row groups through shared memory
 #pragma unroll
-            for (int o = 4; o < 32; o <<= 1) { c0 += __shfl_xor_sync(0xffffffffu, c0, o); c1 += __shfl_xor_sync(0xffffffffu, c1, o); }
-            if (lane < 4) {
-                if (c0 != 0.f) atomicAdd(&s_sum[which][f], c0);
-                if (c1 != 0.f) atomicAdd(&s_sum[which][f + 1], c1);
+                for (int o = 4; o < 32; o <<= 1) { c0 += __shfl_xor_sync(0xffffffffu, c0, o); c1 += __shfl_xor_sync(0xffffffffu, c1, o); }
+                if (lane < 4) {
+                    if (c0 != 0.f) atomicAdd(&s_sum[which][f], c0);
+                    if (c1 != 0.f) atomicAdd(&s_sum[which][f + 1], c1);
+                }
             }
         }
     }
@@ -403,19 +410,39 @@ __global__ void __launch_bounds__(kReduceThreads) fit_reduce_kernel(const Dims d
             }
         __syncthreads();
         const bool mirror = (m & 1) && m < 2 * d.n_symm;
+        float *part = b.points_part + ((size_t)m * tiles + blockIdx.x) * 3 * 128;
         for (int i = threadIdx.x; i < 128 * 3; i += blockDim.x) {
-            const int pt = i / 3, a = i % 3;
+            const int pt = i % 128, a = i / 128;
             float v = s_g[0][pt][a] + s_g[1][pt][a];
             if (a == 0 && mirror) v = -v;
-            const long long row = row0 + pt;
-            if (row < b.n && v != 0.f) atomicAdd(b.grad_points + (scan * b.n + row) * 3 + a, v);
+            part[i] = v;
         }
     }
+    if (!LATENT) return;
     __syncthreads();
     float *acc = b.acc + ((size_t)scan * d.n_members + m) * 2 * d.H;
     for (int i = threadIdx.x; i < 2 * d.H; i += blockDim.x) {
         const float v = i < d.H ? s_sum[0][i] : s_sum[1][i - d.H];          // acc = [sum delta0 | sum delta2]
         if (v != 0.f) atomicAdd(acc + i, v);
+    }
+}
+
+// grad_points += the members' point gradients in member order (one order the float atomics of a member-parallel sum could
+// take, fixed, so that equal inputs give equal bits); zero terms are skipped like the atomics skip them
+__global__ void __launch_bounds__(128) fit_points_kernel(const Dims d, const Buffers b, long long tiles)
+{
+    const int scan = blockIdx.y;
+    const long long i_scan = (long long)blockIdx.x * 128 + threadIdx.x;
+    if (i_scan >= b.n) return;
+    const long long tile = scan * b.tiles_per_scan + blockIdx.x;
+    float *g = b.grad_points + (scan * b.n + i_scan) * 3;
+    for (int a = 0; a < 3; ++a) {
+        float s = g[a];
+        for (int m = 0; m < d.n_members; ++m) {
+            const float v = b.points_part[(((size_t)m * tiles + tile) * 3 + a) * 128 + threadIdx.x];
+            if (v != 0.f) s += v;
+        }
+        g[a] = s;
     }
 }
 
@@ -465,7 +492,11 @@ __global__ void fit_blend_kernel(const Dims d, const Buffers b, float clamp)
         sum += __shfl_xor_sync(0xffffffffu, sum, o);
     }
     float *stats = b.stats + (size_t)scan * 8;
-    if ((threadIdx.x & 31) == 0 && (cnt != 0.f || sum != 0.f)) { atomicAdd(stats + 0, cnt); atomicAdd(stats + 1, sum); }
+    if ((threadIdx.x & 31) == 0) {
+        // the count is a sum of small integers, exact in any order; the per-warp sums are added in warp order by the finalize
+        if (cnt != 0.f) atomicAdd(stats + 0, cnt);
+        b.sum_part[(size_t)scan * gridDim.x * (blockDim.x / 32) + (blockIdx.x * blockDim.x + threadIdx.x) / 32] = sum;
+    }
 }
 
 // per member: g_u = W0u^T D0 + W2u^T D2 / sqrt2 ; g_c = W0x^T D0 + W2x^T D2 / sqrt2
@@ -524,6 +555,7 @@ struct FinalizeArgs {
     float lambda_surface, lambda_reg_global, lambda_reg_loc, lambda_reg_unobserved, lambda_symm_dist;
     float step_size, bc2_sqrt, one_minus_beta1, beta2, one_minus_beta2, eps;
     int apply_update;
+    int latent_grad;                // 0: only the loss terms are wanted (no mlp_pos backward)
 };
 
 // mlp_pos backward (anchor gradient -> z_glob), regularisers (fitting.py:252-268), loss terms, Adam; one CTA per scan (the
@@ -545,7 +577,7 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
     const int tid = threadIdx.x, nt = blockDim.x;
     const int Hd = d.pos_hid, G = d.G, O = d.n_loc * 3;
     // forward of mlp_pos (ReLU masks): one warp per output row (coalesced weight rows + shuffle reduction)
-    {
+    if (a.latent_grad) {
         const int lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
         for (int n = warp; n < Hd; n += nw) {
             float s = 0.f;
@@ -587,9 +619,11 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
             __syncthreads();
         }
     };
-    matvec_t(w.pos_w[2], Hd, O, Hd, ganch, [&](int j, float t) { g1[j] = h1[j] > 0.f ? t : 0.f; });
-    matvec_t(w.pos_w[1], Hd, Hd, Hd, g1, [&](int j, float t) { g0[j] = h0[j] > 0.f ? t : 0.f; });
-    matvec_t(w.pos_w[0], G, Hd, G, g0, [&](int j, float t) { grad[j] += t; });
+    if (a.latent_grad) {
+        matvec_t(w.pos_w[2], Hd, O, Hd, ganch, [&](int j, float t) { g1[j] = h1[j] > 0.f ? t : 0.f; });
+        matvec_t(w.pos_w[1], Hd, Hd, Hd, g1, [&](int j, float t) { g0[j] = h0[j] > 0.f ? t : 0.f; });
+        matvec_t(w.pos_w[0], G, Hd, G, g0, [&](int j, float t) { grad[j] += t; });
+    }
     // regularisers
     float part[4] = {0.f, 0.f, 0.f, 0.f};        // reg_global, reg_loc, reg_unobserved, (unused)
     const int unobs[3] = {30, 31, 39};
@@ -634,7 +668,13 @@ __global__ void __launch_bounds__(1024) fit_finalize_kernel(const Dims d, const 
     if (tid == 0 && loss_terms) {
         float rg = 0.f, rl = 0.f, ru = 0.f, sy = 0.f;
         for (int wi = 0; wi < nt / 32; ++wi) { rg += red[wi]; rl += red[32 + wi]; ru += red[64 + wi]; sy += red[96 + wi]; }
-        loss_terms[0] = stats[1] / stats[0];      // surface = mean |sdf| over kept points (NaN if none, like torch)
+        float sum = stats[1];
+        if (b.sum_part) {
+            const long long parts = (b.n + 127) / 128 * 4;
+            const float *sp = b.sum_part + (size_t)scan * parts;
+            for (long long i = 0; i < parts; ++i) if (sp[i] != 0.f) sum += sp[i];
+        }
+        loss_terms[0] = sum / stats[0];           // surface = mean |sdf| over kept points (NaN if none, like torch)
         loss_terms[1] = rg; loss_terms[2] = rl; loss_terms[3] = ru;
         loss_terms[4] = d.n_symm ? sy / d.n_symm : 0.f;
         loss_terms[5] = stats[0];
@@ -684,7 +724,7 @@ int backward_packs(nphm_ensemble *h, cudaStream_t stream)
 // fit_finalize_kernel over n_scans scans with the Adam constants of fp
 int launch_finalize(const Dims &d, const Weights &w, const Buffers &b, int n_scans, float *latent_dev, float *adam_m_dev,
                     float *adam_v_dev, const nphm_fit_params *fp, int apply_update, float *loss_terms_dev, float *grad_out_dev,
-                    cudaStream_t stream);
+                    cudaStream_t stream, bool latent_grad = true);
 }}
 namespace nphm {
 void fit_packs_destroy(nphm_ensemble *h)
@@ -699,7 +739,7 @@ extern "C" long long nphm_fit_batch_workspace_bytes(const nphm_ensemble *h, int 
     if (!h || n_scans < 1 || n_points < 0) return -1;
     const long long S = n_scans;
     long long floats = S * (n_points * (h->n_members + 3) + (long long)h->n_members * 2 * h->cfg.hidden_dim +
-                            (long long)h->cfg.n_loc * 6 + 8 + h->lat_dim);
+                            (long long)h->cfg.n_loc * 6 + 8 + h->lat_dim + (n_points + 127) / 128 * 4);
     // activation derivatives handed from the tensor-core forward to the backward GEMMs ([member][tile][kActLd][128], layers 0-2) and the upstream gradient of every member output ([member][rows]); every scan owns whole tiles
     const long long tiles = S * ((n_points + 127) / 128);
     floats += (long long)h->n_members * tiles * 128 * (nphm::tc::kActLd + 1);
@@ -718,7 +758,8 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
                          float *adam_m_dev, float *adam_v_dev, const nphm_fit_params *fp, int apply_update,
                          float *loss_terms_dev, float *grad_out_dev, const unsigned char *mask_dev, float *grad_points_dev,
                          void *workspace_dev, long long workspace_bytes, void *stream_, const float *upstream_dev = nullptr,
-                         float *sdf_out_dev = nullptr, long long quirk_period = 0, const int *quirk_periods_dev = nullptr)
+                         float *sdf_out_dev = nullptr, long long quirk_period = 0, const int *quirk_periods_dev = nullptr,
+                         bool latent_grad = true)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     NPHM_REQUIRE(h && h->loaded, "nphm_fit_identity_step: weights not loaded");
@@ -791,6 +832,7 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
     b.ganch = p; p += S * d.n_loc * 3;
     b.grad = p; p += S * d.lat_dim;
     NPHM_CUDA_CHECK(cudaMemsetAsync(zero_begin, 0, (size_t)(p - zero_begin) * sizeof(float), stream));
+    b.sum_part = p; p += S * b.tiles_per_scan * 4;                  // written whole by fit_blend_kernel
     p += (4 - ((p - ws) & 3)) & 3;                                  // 16-byte alignment of the activation block
     float *acts = p;
     b.acts = nullptr;
@@ -798,6 +840,10 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
     b.upstream = upstream_dev;
     b.sdf_out = sdf_out_dev;
     b.grad_points = grad_points_dev;
+    // without a latent gradient the tensor-core backward keeps only what the point gradients need (the FFMA step computes
+    // both in one kernel and drops the latent part)
+    const bool skip_latent = !latent_grad && tc_path;
+    if (skip_latent) b.blend_acc = nullptr;
     b.quirk_period = quirk_period;
     b.quirk_periods = quirk_periods_dev;
 
@@ -824,7 +870,7 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
     }
     fit::fit_blend_kernel<<<dim3((unsigned)ceil_div(n_points, 128), n_scans), 128, 0, stream>>>(d, b, fp->clamp);
     NPHM_CUDA_CHECK(cudaGetLastError());
-    if (b.acts) {
+    if (b.acts && !(skip_latent && !grad_points_dev)) {
         const long long n_tiles = rows_total / 128;
         float *gs = acts + (size_t)h->n_members * rows_total * tc::kActLd;
         uint8_t *packed = reinterpret_cast<uint8_t *>(gs + (size_t)h->n_members * rows_total);
@@ -854,16 +900,23 @@ static int fit_step_impl(nphm_ensemble *h, const float *points_dev, int n_scans,
         lp.Ap = p1; lp.a_ksteps = fit::kStepsN1; lp.Mul = acts + tc::kActOff0 * 128; lp.Cp = p0; lp.c_ksteps = fit::kStepsH;
         if ((rc = tcl::launch_linear(bp.l1, lp, stream))) return rc;
         dim3 rgrid((unsigned)n_tiles, h->n_members);
-        if (grad_points_dev) fit::fit_reduce_kernel<true><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
-        else fit::fit_reduce_kernel<false><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
-    } else {
+        b.points_part = acts;           // the activation derivatives are dead once the three GEMMs have consumed them
+        if (skip_latent) fit::fit_reduce_kernel<true, false><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
+        else if (grad_points_dev) fit::fit_reduce_kernel<true, true><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
+        else fit::fit_reduce_kernel<false, true><<<rgrid, fit::kReduceThreads, 0, stream>>>(d, w, b, packed, n_tiles, gs);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+        if (grad_points_dev)
+            fit::fit_points_kernel<<<dim3((unsigned)b.tiles_per_scan, n_scans), 128, 0, stream>>>(d, b, n_tiles);
+    } else if (!b.acts) {
         fit::fit_member_kernel<true><<<grid, fit::kThreads, smem, stream>>>(d, w, b, fp->lambda_surface);
     }
     NPHM_CUDA_CHECK(cudaGetLastError());
-    fit::fit_member_grad_kernel<<<dim3(h->n_members, n_scans), 128 * fit::kGradSlices, 0, stream>>>(d, w, b);
-    NPHM_CUDA_CHECK(cudaGetLastError());
+    if (!skip_latent) {
+        fit::fit_member_grad_kernel<<<dim3(h->n_members, n_scans), 128 * fit::kGradSlices, 0, stream>>>(d, w, b);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
     return fit::launch_finalize(d, w, b, n_scans, latent_dev, adam_m_dev, adam_v_dev, fp, apply_update, loss_terms_dev,
-                                grad_out_dev, stream);
+                                grad_out_dev, stream, !skip_latent);
 }
 
 extern "C" int nphm_fit_identity_step(nphm_ensemble *h, const float *points_dev, long long n_points, float *latent_dev,
@@ -897,10 +950,10 @@ extern "C" int nphm_fit_surface_grad(nphm_ensemble *h, const float *points_dev, 
                                      const unsigned char *mask_dev, float clamp, float *loss_terms_dev,
                                      float *grad_latent_dev, float *grad_points_dev, void *workspace_dev, void *stream)
 {
-    NPHM_REQUIRE(grad_latent_dev, "nphm_fit_surface_grad: grad_latent_dev is NULL");
     const nphm_fit_params fp = surface_params(clamp);
     return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, loss_terms_dev,
-                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream);
+                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream, nullptr, nullptr, 0, nullptr,
+                         grad_latent_dev != nullptr);
 }
 
 extern "C" int nphm_fit_surface_grad_quirk(nphm_ensemble *h, const float *points_dev, long long n_points, long long quirk_period,
@@ -908,10 +961,10 @@ extern "C" int nphm_fit_surface_grad_quirk(nphm_ensemble *h, const float *points
                                            float *loss_terms_dev, float *grad_latent_dev, float *grad_points_dev,
                                            void *workspace_dev, void *stream)
 {
-    NPHM_REQUIRE(grad_latent_dev, "nphm_fit_surface_grad_quirk: grad_latent_dev is NULL");
     const nphm_fit_params fp = surface_params(clamp);
     return fit_step_impl(h, points_dev, 1, n_points, const_cast<float *>(latent_dev), nullptr, nullptr, &fp, 0, loss_terms_dev,
-                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream, nullptr, nullptr, quirk_period);
+                         grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, -1, stream, nullptr, nullptr, quirk_period,
+                         nullptr, grad_latent_dev != nullptr);
 }
 
 // the scan-batched entry points run only on the tensor-core path (no batched FFMA fallback)
@@ -957,10 +1010,11 @@ extern "C" int nphm_fit_surface_grad_batched(nphm_ensemble *h, const float *poin
 {
     int rc;
     if ((rc = require_batched(h, "nphm_fit_surface_grad_batched", n_scans, workspace_dev))) return rc;
-    NPHM_REQUIRE(loss_terms_dev && grad_latent_dev, "nphm_fit_surface_grad_batched: NULL loss terms or gradient");
+    NPHM_REQUIRE(loss_terms_dev, "nphm_fit_surface_grad_batched: NULL loss terms");
     const nphm_fit_params fp = surface_params(clamp);
     return fit_step_impl(h, points_dev, n_scans, n_points, const_cast<float *>(latents_dev), nullptr, nullptr, &fp, 0,
-                         loss_terms_dev, grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, workspace_bytes, stream);
+                         loss_terms_dev, grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, workspace_bytes, stream,
+                         nullptr, nullptr, 0, nullptr, grad_latent_dev != nullptr);
 }
 
 extern "C" int nphm_fit_surface_grad_batched_quirk(nphm_ensemble *h, const float *points_dev, const unsigned char *mask_dev,
@@ -971,11 +1025,11 @@ extern "C" int nphm_fit_surface_grad_batched_quirk(nphm_ensemble *h, const float
 {
     int rc;
     if ((rc = require_batched(h, "nphm_fit_surface_grad_batched_quirk", n_scans, workspace_dev))) return rc;
-    NPHM_REQUIRE(loss_terms_dev && grad_latent_dev, "nphm_fit_surface_grad_batched_quirk: NULL loss terms or gradient");
+    NPHM_REQUIRE(loss_terms_dev, "nphm_fit_surface_grad_batched_quirk: NULL loss terms");
     const nphm_fit_params fp = surface_params(clamp);
     return fit_step_impl(h, points_dev, n_scans, n_points, const_cast<float *>(latents_dev), nullptr, nullptr, &fp, 0,
                          loss_terms_dev, grad_latent_dev, mask_dev, grad_points_dev, workspace_dev, workspace_bytes, stream,
-                         nullptr, nullptr, 0, quirk_periods_dev);
+                         nullptr, nullptr, 0, quirk_periods_dev, grad_latent_dev != nullptr);
 }
 
 // Vector-Jacobian product of the ensemble forward w.r.t. its inputs (SURVEY.md 8b: nphm_ensemble_backward_inputs):
@@ -1036,7 +1090,7 @@ __global__ void adam_dense_kernel(float *__restrict__ param, const float *__rest
 
 int launch_finalize(const Dims &d, const Weights &w, const Buffers &b, int n_scans, float *latent_dev, float *adam_m_dev,
                     float *adam_v_dev, const nphm_fit_params *fp, int apply_update, float *loss_terms_dev, float *grad_out_dev,
-                    cudaStream_t stream)
+                    cudaStream_t stream, bool latent_grad)
 {
     FinalizeArgs a{};
     a.lambda_surface = fp->lambda_surface; a.lambda_reg_global = fp->lambda_reg_global; a.lambda_reg_loc = fp->lambda_reg_loc;
@@ -1047,7 +1101,7 @@ int launch_finalize(const Dims &d, const Weights &w, const Buffers &b, int n_sca
     a.step_size = (float)((double)fp->lr / bc1);
     a.bc2_sqrt = (float)std::sqrt(bc2);
     a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
-    a.eps = 1e-8f; a.apply_update = apply_update;
+    a.eps = 1e-8f; a.apply_update = apply_update; a.latent_grad = latent_grad;
     const size_t fsm = (size_t)(4 * d.pos_hid + 128 + 1024) * sizeof(float);
     fit_finalize_kernel<<<n_scans, 1024, fsm, stream>>>(d, w, b, latent_dev, adam_m_dev, adam_v_dev, a, loss_terms_dev, grad_out_dev);
     NPHM_CUDA_CHECK(cudaGetLastError());

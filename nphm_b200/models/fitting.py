@@ -2,6 +2,7 @@
 
   * ``inference_identity_space``                 src/NPHM/models/fitting.py:180-285
   * ``inference_iterative_root_finding_joint``   src/NPHM/models/fitting.py:14-177
+  * ``inference_expression_space``               the same joint loop with the identity code given and held fixed
 
 ``inference_identity_space`` runs on the fused fitting kernels (``nphm_fit_identity_step``: forward, clamped |sdf|
 loss, analytic latent gradient and Adam in five launches, no autograd graph) when the decoder is a
@@ -189,16 +190,17 @@ class _FusedSurfaceLoss(torch.autograd.Function):
 
 
 def _surface_grad(eng, pts, period, lat, mask, clamp, terms, g_lat, g_pts, stream):
-    """``nphm_fit_surface_grad`` on ``pts`` (n x 3), or its eval-mode form with quirk period ``period`` > 0."""
+    """``nphm_fit_surface_grad`` on ``pts`` (n x 3), or its eval-mode form with quirk period ``period`` > 0.  ``g_lat=None``:
+    no identity-code gradient (the kernels skip that work)."""
     lib = _native.lib()
     with torch.cuda.device(pts.device):
         if period:
             _native.check(lib.nphm_fit_surface_grad_quirk(eng.handle, pts.data_ptr(), pts.shape[0], period, lat.data_ptr(),
-                                                          mask.data_ptr(), float(clamp), terms.data_ptr(), g_lat.data_ptr(),
+                                                          mask.data_ptr(), float(clamp), terms.data_ptr(), _native._ptr(g_lat),
                                                           g_pts.data_ptr(), None, stream), 'nphm_fit_surface_grad_quirk')
         else:
             _native.check(lib.nphm_fit_surface_grad(eng.handle, pts.data_ptr(), pts.shape[0], lat.data_ptr(), mask.data_ptr(),
-                                                    float(clamp), terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(), None,
+                                                    float(clamp), terms.data_ptr(), _native._ptr(g_lat), g_pts.data_ptr(), None,
                                                     stream), 'nphm_fit_surface_grad')
 
 
@@ -303,6 +305,14 @@ def _native_joint(decoder, decoder_expr, device) -> bool:
     return next(bb.parameters()).is_cuda and bb.num_freq_bands is None and bb.beta == 100 and bb.out_dim_net == 3
 
 
+def _adam_expressions(fitter, g_zex, lr, stream):
+    """The update of a fixed-identity step: Adam on the expression codes alone."""
+    _native.check(_native.lib().nphm_adam_step(fitter.z_ex.data_ptr(), g_zex.data_ptr(), fitter.m_ex.data_ptr(),
+                                               fitter.v_ex.data_ptr(), fitter.z_ex.numel(), float(lr), fitter.t, stream),
+                  'nphm_adam_step')
+    return None
+
+
 class JointFitter:
     """One iteration of ``inference_iterative_root_finding_joint`` (reference fitting.py:38-175) WITHOUT an autograd graph.
 
@@ -313,10 +323,16 @@ class JointFitter:
         g_c   = sum_n (dF_ex/d cond)^T u_n   per sampled scan       nphm_mlp_backward_inputs (adjoint pass, tensor cores)
         cond  = [compressor([z_id | anchors]) (32) | z_ex (200)]    -> z_ex rows, and through the compressor to z_id and the
                                                                       anchors (mlp_pos backward inside nphm_fit_apply_gradient)
-    followed by the regularisers and the two Adam updates (nphm_fit_apply_gradient, nphm_adam_step)."""
+    followed by the regularisers and the two Adam updates (nphm_fit_apply_gradient, nphm_adam_step).
 
-    def __init__(self, decoder, decoder_expr, num_observations: int, device):
+    ``fixed_identity=True`` holds ``z_id`` (set by the caller before the first step) fixed: the anchors and the compressor row
+    are computed once, the surface term runs without the identity-code gradient, and a step is the z_ex route alone
+    (-J^-T g_x, adjoint pass, reg_expr, Adam).  ``loss_terms`` are then the surface call's (unweighted)."""
+
+    def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
+        self.fixed_identity = fixed_identity
+        self._c32 = None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.defDeepSDF.engine()
         E = decoder_expr.lat_dim_expr
@@ -334,7 +350,8 @@ class JointFitter:
 
     def step(self, obs, obs_idx, lambdas, clamp, lr, apply_update: bool = True):
         """One iteration; with ``apply_update=False`` nothing is modified and ``(d loss / d z_id, d loss / d z_ex)`` - the
-        tensors the reference hands to its two ``Adam.step()`` calls - are returned."""
+        tensors the reference hands to its two ``Adam.step()`` calls - are returned (``d loss / d z_id`` is None with a fixed
+        identity)."""
         nat, dev = _native, self.device
         nb, n_point, _ = obs.shape
         E, D = self.z_ex.shape[1], self.z_id.shape[0]
@@ -342,13 +359,14 @@ class JointFitter:
             self.t += 1
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.no_grad(), torch.cuda.device(dev):
-            anchors = self.eng.anchors(self.z_id[None])                                  # 1 x K x 3, pre-update code (:59)
-            self.anchors = anchors
             # condition of the deformation backbone (deepSDF.py:218-219): compressor([z_id | anchors]) (32) | z_ex (E)
             lin = self.dfn.compressor[0] if isinstance(self.dfn.compressor, torch.nn.Sequential) else self.dfn.compressor
             Wc, bc = lin.weight, lin.bias
-            first = torch.cat([self.z_id, anchors.reshape(-1)])
-            c32 = (Wc * first[None, :]).sum(1) + bc
+            if self._c32 is None or not self.fixed_identity:
+                self.anchors = self.eng.anchors(self.z_id[None])                         # 1 x K x 3, pre-update code (:59)
+                first = torch.cat([self.z_id, self.anchors.reshape(-1)])
+                self._c32 = (Wc * first[None, :]).sum(1) + bc
+            c32 = self._c32
             cond = torch.cat([c32[None, :].expand(nb, -1), self.z_ex[obs_idx]], dim=1).contiguous()
             # correspondence search (iterative_root_finding.py:91-168): J0^-1 at the observed points, Broyden on the device
             obs = obs.to(torch.float32).contiguous()
@@ -360,20 +378,23 @@ class JointFitter:
             # surface term (:111-136): value + d/d z_id + d/d xc
             pts = p.reshape(-1, 3)
             mask = valid.reshape(-1).to(torch.uint8).contiguous()
-            g_lat = torch.empty(D, device=dev)
+            g_lat = None if self.fixed_identity else torch.empty(D, device=dev)
             g_pts = torch.empty_like(pts)
             _surface_grad(self.eng, pts, _quirk_period(self.dec, n_point), self.z_id, mask, clamp, self.terms, g_lat, g_pts,
                           stream)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                       # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # nb x (32 + E); same points as j_inv
-            g_first = (Wc * g_cond[:, :32].sum(0)[:, None]).sum(0)                       # compressor^T -> [z_id | anchors]
-            g_zid = (g_lat + g_first[:D]).contiguous()
-            g_anchors = g_first[D:].contiguous()
-            stats = torch.stack([self.terms[5], self.terms[0] * self.terms[5]]).nan_to_num_(0.0).contiguous()
             # expression codes: surface route + reg_expr = mean_b ||z_ex[idx_b]||^2 (:137), dense Adam over all rows (:169)
             lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, 32:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
+            if self.fixed_identity:
+                self.loss_terms.copy_(self.terms)
+                return _adam_expressions(self, g_zex, lr, stream) if apply_update else (None, g_zex)
+            g_first = (Wc * g_cond[:, :32].sum(0)[:, None]).sum(0)                       # compressor^T -> [z_id | anchors]
+            g_zid = (g_lat + g_first[:D]).contiguous()
+            g_anchors = g_first[D:].contiguous()
+            stats = torch.stack([self.terms[5], self.terms[0] * self.terms[5]]).nan_to_num_(0.0).contiguous()
             fp = nat.FitParams(lam_s, float(lambdas.get('reg_global', 0.0)), float(lambdas.get('reg_loc', 0.0)),
                                float(lambdas.get('reg_unobserved', 0.0)), float(lambdas.get('symm_dist', 0.0)), float(clamp),
                                float(lr), max(self.t, 1))
@@ -462,10 +483,12 @@ class NpmJointFitter:
         u = -J^-T g_x,  g_cond = sum_n (dF/d cond)^T u_n                                      nphm_mlp_backward_inputs (value pass reused)
         z_id += g_cond[:, :D] summed over the scans,  z_ex[idx_b] += g_cond[b, D:] + reg_expr,  two Adam steps.
     u is of order 1e-4; the adjoint pass, which works on fp16 hi | lo operands, scales each query's upstream into their range
-    itself."""
+    itself.  ``fixed_identity=True``: ``z_id`` (set by the caller) is held fixed, a step updates the expression codes alone (see
+    :class:`JointFitter`)."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: int, device):
+    def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False):
         self.device = device
+        self.fixed_identity = fixed_identity
         self.eng = decoder.engine()
         self.mlp = decoder_expr.engine()
         D = decoder.lat_dim
@@ -504,9 +527,11 @@ class NpmJointFitter:
             self.loss_terms.copy_(terms)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                     # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)
-            g_zid = lam_s * (g_lat[0] + g_cond[:, :D].sum(0)) + (2.0 * lam_g) * self.z_id
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
+            if self.fixed_identity:
+                return _adam_expressions(self, g_zex, lr, stream) if apply_update else (None, g_zex)
+            g_zid = lam_s * (g_lat[0] + g_cond[:, :D].sum(0)) + (2.0 * lam_g) * self.z_id
             if not apply_update:
                 return g_zid, g_zex
             for z, g, m, v in ((self.z_id, g_zid, self.m_id, self.v_id), (self.z_ex, g_zex, self.m_ex, self.v_ex)):
@@ -539,39 +564,59 @@ def inference_iterative_root_finding_joint(decoder,
         elif _native_npm_joint(decoder, decoder_expr, device):
             fitter = NpmJointFitter(decoder, decoder_expr, num_observations, device)
         if fitter is not None:
-            lr = 0.01 * lr_scale
-            for j in range(int(n_steps * step_scale)):
-                lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
-                obs, obs_idx = _sample_observations(all_obs)
-                fitter.step(obs, obs_idx.long().to(device), lambdas, _clamp_for_iteration(j, step_scale), lr)
+            _run_joint(fitter, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
             lat_rep = fitter.z_ex.reshape(num_observations, 1, -1).clone().requires_grad_(True)
             lat_rep_shape = fitter.z_id.reshape(1, 1, -1).clone().requires_grad_(True)
             return lat_rep, lat_rep_shape, fitter.anchors
     return _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
 
 
-def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1):
+def _run_joint(fitter, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale):
+    """The reference loop (:38-175) around one native joint or fixed-identity fitter."""
+    device = fitter.device
+    lr = 0.01 * lr_scale
+    for j in range(int(n_steps * step_scale)):
+        lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
+        obs, obs_idx = _sample_observations(all_obs)
+        fitter.step(obs, obs_idx.long().to(device), lambdas, _clamp_for_iteration(j, step_scale), lr)
+
+
+def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1,
+                              lat_rep_shape=None, lat_rep_init=None):
     """The composite path of :func:`inference_iterative_root_finding_joint`: the correspondence search on the device where
-    the search supports the decoder, everything else on autograd through the modules."""
+    the search supports the decoder, everything else on autograd through the modules.  A given ``lat_rep_shape`` is held
+    fixed (the path of :func:`inference_expression_space`): no identity optimizer, the anchors computed once, and ``z_ex``
+    starts at ``lat_rep_init`` when one is given."""
     device = all_obs[0].device
     num_observations = len(all_obs)
     lat_expr_dim = decoder_expr.lat_dim_expr if hasattr(decoder_expr, 'lat_dim_expr') else 200
-    lat_rep = torch.zeros([num_observations, 1, lat_expr_dim], device=device, requires_grad=True)
-    lat_rep_shape = torch.zeros([1, 1, decoder.lat_dim], device=device, requires_grad=True)
+    lat_rep = torch.zeros([num_observations, 1, lat_expr_dim], device=device)
+    if lat_rep_init is not None:
+        lat_rep.copy_(lat_rep_init.detach().reshape(lat_rep.shape))
+    lat_rep.requires_grad_(True)
+    fixed = lat_rep_shape is not None
+    if fixed:
+        lat_rep_shape = lat_rep_shape.detach().reshape(1, 1, decoder.lat_dim).to(device=device, dtype=torch.float32).clone()
+    else:
+        lat_rep_shape = torch.zeros([1, 1, decoder.lat_dim], device=device, requires_grad=True)
     lr = 0.01 * lr_scale
-    opt = optim.Adam(params=[lat_rep_shape], lr=lr)
     opt_expr = optim.Adam(params=[lat_rep], lr=lr)
+    opts = [opt_expr] if fixed else [optim.Adam(params=[lat_rep_shape], lr=lr), opt_expr]
     anchors = None
+    if fixed:
+        with torch.no_grad():
+            anchors = _current_anchors(decoder, lat_rep_shape, device)
     for j in range(int(n_steps * step_scale)):
         new_lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
         if new_lr != lr:
             lr = new_lr
-            for o in (opt, opt_expr):
+            for o in opts:
                 for group in o.param_groups:
                     group['lr'] = lr
-        opt.zero_grad()
-        opt_expr.zero_grad()
-        anchors = _current_anchors(decoder, lat_rep_shape, device)
+        for o in opts:
+            o.zero_grad()
+        if not fixed:
+            anchors = _current_anchors(decoder, lat_rep_shape, device)
         obs, obs_idx = _sample_observations(all_obs)
         obs_idx = obs_idx.long().to(device)
         nb, n_point, _ = obs.shape
@@ -608,8 +653,8 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
         for k in lambdas.keys():
             loss = loss + loss_dict[k] * lambdas[k]
         loss.backward()
-        opt.step()
-        opt_expr.step()
+        for o in opts:                      # the identity's optimizer first, as in the reference (:168-169)
+            o.step()
     return lat_rep, lat_rep_shape, anchors
 
 
@@ -827,10 +872,13 @@ class BatchedJointFitter:
     The expression codes are one (sum n_obs) x E tensor; subject k's rows start at ``offsets[k]``.  In eval mode a shorter
     subject's rows are padded in front instead of behind, so that every row ends with its subject's last sampled point - the
     quirk row of that subject's single-subject call - and one period, n_point, serves all subjects
-    (``nphm_fit_surface_grad_batched_quirk``)."""
+    (``nphm_fit_surface_grad_batched_quirk``).  ``fixed_identity=True``: the S identity codes (set by the caller) are held
+    fixed, as in :class:`JointFitter`."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: List[int], device):
+    def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
+        self.fixed_identity = fixed_identity
+        self._c32 = None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.defDeepSDF.engine()
         E, S = decoder_expr.lat_dim_expr, len(num_observations)
@@ -848,7 +896,8 @@ class BatchedJointFitter:
 
     def step(self, obs: List[torch.Tensor], obs_idx: List[torch.Tensor], lambdas, clamp, lr, apply_update: bool = True):
         """One iteration; ``obs[k]`` (5 x n_k x 3) and ``obs_idx[k]`` (5, on the device) are subject k's sample.  With
-        ``apply_update=False`` nothing is modified and ``(d loss / d z_id (S x D), [d loss / d z_ex of subject k])`` is returned."""
+        ``apply_update=False`` nothing is modified and ``(d loss / d z_id (S x D), [d loss / d z_ex of subject k])`` is returned
+        (``d loss / d z_id`` is None with fixed identities)."""
         nat, dev = _native, self.device
         S, D = self.z_id.shape
         nb = obs[0].shape[0]
@@ -858,12 +907,13 @@ class BatchedJointFitter:
         stream = torch.cuda.current_stream(dev).cuda_stream
         lib = nat.lib()
         with torch.no_grad(), torch.cuda.device(dev):
-            anchors = self.eng.anchors(self.z_id)                                        # S x K x 3, pre-update codes
-            self.anchors = anchors
             lin = self.dfn.compressor[0] if isinstance(self.dfn.compressor, torch.nn.Sequential) else self.dfn.compressor
             Wc, bc = lin.weight, lin.bias
-            first = torch.cat([self.z_id, anchors.reshape(S, -1)], dim=1)
-            c32 = (Wc[None] * first[:, None, :]).sum(2) + bc                             # S x 32
+            if self._c32 is None or not self.fixed_identity:
+                self.anchors = self.eng.anchors(self.z_id)                               # S x K x 3, pre-update codes
+                first = torch.cat([self.z_id, self.anchors.reshape(S, -1)], dim=1)
+                self._c32 = (Wc[None] * first[:, None, :]).sum(2) + bc                   # S x 32
+            c32 = self._c32
             rows = torch.cat([idx + off for idx, off in zip(obs_idx, self.offsets)])    # rows of z_ex, 5 S
             cond = torch.cat([c32.repeat_interleave(nb, dim=0), self.z_ex[rows]], dim=1).contiguous()
             # every subject padded to n_point points per observation (the padding repeats a point and is masked below); in eval
@@ -883,30 +933,35 @@ class BatchedJointFitter:
                                                    'nphm_fit_batch_workspace_bytes', dev))
             ws = self._ws[1]
             terms = torch.empty(S, 8, device=dev)
-            g_lat = torch.empty(S, D, device=dev)
+            g_lat = None if self.fixed_identity else torch.empty(S, D, device=dev)
             g_pts = torch.empty_like(pts)
             if front:
                 periods = torch.full((S,), n_point, dtype=torch.int32, device=dev)
                 nat.check(lib.nphm_fit_surface_grad_batched_quirk(self.eng.handle, pts.data_ptr(), mask.data_ptr(), S, n,
                                                                   periods.data_ptr(), self.z_id.data_ptr(), float(clamp),
-                                                                  terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(),
+                                                                  terms.data_ptr(), nat._ptr(g_lat), g_pts.data_ptr(),
                                                                   ws.data_ptr(), ws.numel(), stream),
                           'nphm_fit_surface_grad_batched_quirk')
             else:
                 nat.check(lib.nphm_fit_surface_grad_batched(self.eng.handle, pts.data_ptr(), mask.data_ptr(), S, n,
                                                             self.z_id.data_ptr(), float(clamp), terms.data_ptr(),
-                                                            g_lat.data_ptr(), g_pts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
+                                                            nat._ptr(g_lat), g_pts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
                           'nphm_fit_surface_grad_batched')
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # 5 S x (32 + E)
+            lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
+            g_zex = torch.zeros_like(self.z_ex)
+            g_zex.index_add_(0, rows, lam_s * g_cond[:, 32:] + (2.0 * lam_e / nb) * self.z_ex[rows])
+            if self.fixed_identity:
+                self.loss_terms.copy_(terms)
+                if not apply_update:
+                    return None, [g_zex[o:o + c] for o, c in zip(self.offsets, self.num_observations)]
+                return _adam_expressions(self, g_zex, lr, stream)
             g_c32 = g_cond[:, :32].reshape(S, nb, 32).sum(1)
             g_first = (Wc[None] * g_c32[:, :, None]).sum(1)                              # compressor^T, S x (D + 3 K)
             g_zid = (g_lat + g_first[:, :D]).contiguous()
             g_anchors = g_first[:, D:].contiguous()
             stats = torch.stack([terms[:, 5], terms[:, 0] * terms[:, 5]], dim=1).nan_to_num_(0.0).contiguous()
-            lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
-            g_zex = torch.zeros_like(self.z_ex)
-            g_zex.index_add_(0, rows, lam_s * g_cond[:, 32:] + (2.0 * lam_e / nb) * self.z_ex[rows])
             fp = nat.FitParams(lam_s, float(lambdas.get('reg_global', 0.0)), float(lambdas.get('reg_loc', 0.0)),
                                float(lambdas.get('reg_unobserved', 0.0)), float(lambdas.get('symm_dist', 0.0)), float(clamp),
                                float(lr), max(self.t, 1))
@@ -971,10 +1026,12 @@ class BatchedNpmJointFitter:
     The expression codes are one (sum n_obs) x 200 tensor; subject k's rows start at ``offsets[k]``.  Memory grows linearly with
     S: the Jacobian, Broyden and adjoint buffers of 5 S n_point rows through the expression stack, about 1.4 GB per subject of
     5 x 1000 points (22.7 GB peak at S = 16, tools/bench_fit_batched.py --decoder npm), so an 80 GB card holds about 50
-    subjects per batch; the caller chooses S, nothing is split."""
+    subjects per batch; the caller chooses S, nothing is split.  ``fixed_identity=True``: the identity codes (set by the caller)
+    are held fixed, as in :class:`JointFitter`."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: List[int], device):
+    def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False):
         self.device = device
+        self.fixed_identity = fixed_identity
         self.eng = decoder.engine()
         self.mlp = decoder_expr.engine()
         D, S = decoder.lat_dim, len(num_observations)
@@ -1026,9 +1083,13 @@ class BatchedNpmJointFitter:
             self.loss_terms.copy_(terms)
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)
-            g_zid = lam_s * (g_lat + g_cond[:, :D].reshape(S, nb, D).sum(1)) + (2.0 * lam_g) * self.z_id
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, rows, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[rows])
+            if self.fixed_identity:
+                if not apply_update:
+                    return None, [g_zex[o:o + c] for o, c in zip(self.offsets, self.num_observations)]
+                return _adam_expressions(self, g_zex, lr, stream)
+            g_zid = lam_s * (g_lat + g_cond[:, :D].reshape(S, nb, D).sum(1)) + (2.0 * lam_g) * self.z_id
             if not apply_update:
                 return g_zid, [g_zex[o:o + c] for o, c in zip(self.offsets, self.num_observations)]
             for z, g, m, v in ((self.z_id, g_zid, self.m_id, self.v_id), (self.z_ex, g_zex, self.m_ex, self.v_ex)):
@@ -1078,19 +1139,119 @@ def _joint_batch_fit(decoder, decoder_expr, subjects, n_steps, schedule_cfg, ste
                                                          schedule_cfg, step_scale, lr_scale, device)
 
 
-def _fit_joint_batch(batched, decoder, decoder_expr, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale,
-                     device):
-    n_iters = int(n_steps * step_scale)
-    fitter = batched(decoder, decoder_expr, [len(s) for s in subjects], device)
+def _run_joint_batch(fitter, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale):
+    """:func:`_run_joint` for a subject-batched fitter, subject k drawing from ``gens[k]``."""
+    device = fitter.device
     lr = 0.01 * lr_scale
-    for j in range(n_iters):
+    for j in range(int(n_steps * step_scale)):
         lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
         sample = [_sample_observations(all_obs, g) for all_obs, g in zip(subjects, gens)]
         fitter.step([o for o, _ in sample], [i.long().to(device) for _, i in sample], lambdas,
                     _clamp_for_iteration(j, step_scale), lr)
+
+
+def _fit_joint_batch(batched, decoder, decoder_expr, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale,
+                     device):
+    fitter = batched(decoder, decoder_expr, [len(s) for s in subjects], device)
+    _run_joint_batch(fitter, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
     out = []
     for k, (off, cnt) in enumerate(zip(fitter.offsets, fitter.num_observations)):
         lat_rep = fitter.z_ex[off:off + cnt].reshape(cnt, 1, -1).clone().requires_grad_(True)
         lat_rep_shape = fitter.z_id[k].reshape(1, 1, -1).clone().requires_grad_(True)
         out.append((lat_rep, lat_rep_shape, None if fitter.anchors is None else fitter.anchors[k:k + 1].clone()))
     return out
+
+
+# ------------------------------------------------------------------------------ expressions of a subject whose identity is known
+def _expression_fitter(decoder, decoder_expr, device, batched: bool):
+    """The native fitter class that fits expressions with a fixed identity on ``device``, or None (the autograd mirror)."""
+    if device is None or os.environ.get('NPHM_JOINT_AUTOGRAD'):
+        return None
+    if _native_npm_joint(decoder, decoder_expr, device):
+        return BatchedNpmJointFitter if batched else NpmJointFitter
+    if _native_joint(decoder, decoder_expr, device) and (not batched or _tc_ensemble(decoder)):
+        return BatchedJointFitter if batched else JointFitter
+    return None
+
+
+def _identity_row(decoder, lat_rep_shape) -> torch.Tensor:
+    z = lat_rep_shape.detach()
+    if z.numel() != decoder.lat_dim:
+        raise ValueError('lat_rep_shape has %d entries, the identity decoder takes %d' % (z.numel(), decoder.lat_dim))
+    return z.reshape(-1)
+
+
+def inference_expression_space(decoder,
+                               decoder_expr,
+                               lat_rep_shape: torch.Tensor,
+                               all_obs: List[torch.Tensor],
+                               lambdas,
+                               n_steps,
+                               schedule_cfg: Dict,
+                               step_scale=1,
+                               lr_scale=1,
+                               lat_reps_expr_init=None):
+    """Fit expression codes to the observations ``all_obs`` of a subject whose identity code ``lat_rep_shape`` (1,1,D) is
+    known, e.g. from :func:`inference_identity_space` on a neutral scan.  The loop is the reference's joint loop (:14-177) with
+    ``lat_rep_shape`` held fixed: the same 5-of-K observation draws from torch's global CPU generator, lr / lambda / clamp
+    schedules (``lambdas`` is mutated as there), surface term at the Broyden roots with the implicit-differentiation correction,
+    and ``reg_expr``; the identity regularisers have no gradient w.r.t. the expression codes.  ``z_ex`` starts at
+    ``lat_reps_expr_init`` (K,1,E) or at zeros.  ``lat_rep_shape`` is not modified.  Returns ``(lat_reps_expr (K,1,E),
+    anchors)``: the anchors of the identity code (None for a ``DeepSDF`` identity decoder).
+
+    Runs natively (:class:`JointFitter` / :class:`NpmJointFitter` with ``fixed_identity=True``) for the configurations of
+    :func:`inference_iterative_root_finding_joint`; anything else - CPU, other decoders, ``NPHM_JOINT_AUTOGRAD=1`` - runs the
+    same loop on autograd."""
+    device = all_obs[0].device
+    K = len(all_obs)
+    z_id = _identity_row(decoder, lat_rep_shape)
+    cls = _expression_fitter(decoder, decoder_expr, device, batched=False)
+    if cls is None:
+        lat_rep, _, anchors = _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg,
+                                                        step_scale, lr_scale, lat_rep_shape=z_id,
+                                                        lat_rep_init=lat_reps_expr_init)
+        return lat_rep, anchors
+    fitter = cls(decoder, decoder_expr, K, device, fixed_identity=True)
+    fitter.z_id.copy_(z_id)
+    if lat_reps_expr_init is not None:
+        fitter.z_ex.copy_(lat_reps_expr_init.detach().reshape(fitter.z_ex.shape))
+    _run_joint(fitter, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
+    return fitter.z_ex.reshape(K, 1, -1).clone().requires_grad_(True), fitter.anchors
+
+
+def inference_expression_space_batched(decoder,
+                                       decoder_expr,
+                                       subjects,
+                                       lambdas,
+                                       n_steps,
+                                       schedule_cfg: Dict,
+                                       step_scale=1,
+                                       lr_scale=1):
+    """:func:`inference_expression_space` for several subjects at once.  ``subjects[k]`` is ``(lat_rep_shape, all_obs)`` or
+    ``(lat_rep_shape, all_obs, lat_reps_expr_init)``; to track the T frames of one person, pass T single-observation entries
+    that share one ``lat_rep_shape``.  Returns ``[(lat_reps_expr, anchors)]`` in subject order under the contract of
+    :func:`inference_identity_space_batched`: what the single-subject function gives when called on each entry in turn, each
+    call with a fresh copy of ``lambdas``, and the global CPU generator and ``lambdas`` end as those calls leave them.  The
+    configurations of :func:`inference_iterative_root_finding_joint_batched` run all subjects in one launch sequence per
+    iteration (:class:`BatchedJointFitter` / :class:`BatchedNpmJointFitter` with ``fixed_identity=True``); anything else calls
+    the single-subject function subject by subject."""
+    if not subjects:
+        return []
+    entries = [(e[0], e[1], e[2] if len(e) > 2 else None) for e in subjects]
+    scans = [e[1] for e in entries]
+    device = _scans_device(scans)
+    cls = _expression_fitter(decoder, decoder_expr, device, batched=True)
+    if cls is None:
+        return _sequential(lambda e, lam: inference_expression_space(decoder, decoder_expr, e[0], e[1], lam, n_steps,
+                                                                     schedule_cfg, step_scale, lr_scale, e[2]),
+                           entries, lambdas)
+    gens = _sampling_plan(scans, int(n_steps * step_scale))
+    fitter = cls(decoder, decoder_expr, [len(o) for o in scans], device, fixed_identity=True)
+    fitter.z_id.copy_(torch.stack([_identity_row(decoder, e[0]) for e in entries]))
+    for (_, _, init), off, cnt in zip(entries, fitter.offsets, fitter.num_observations):
+        if init is not None:
+            fitter.z_ex[off:off + cnt].copy_(init.detach().reshape(cnt, -1))
+    _run_joint_batch(fitter, scans, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
+    return [(fitter.z_ex[off:off + cnt].reshape(cnt, 1, -1).clone().requires_grad_(True),
+             None if fitter.anchors is None else fitter.anchors[k:k + 1].clone())
+            for k, (off, cnt) in enumerate(zip(fitter.offsets, fitter.num_observations))]
