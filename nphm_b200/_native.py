@@ -66,9 +66,34 @@ class NativeError(RuntimeError):
 MC_LAUNCHES = 3                      # classify rows, scan rows, emit rows
 
 
-def launches_per_grid_query(impl='auto') -> int:
-    """grid axes, anchors, folded constants, [tensor-core records, tile member masks], ensemble kernel."""
-    return 4 + (2 if impl in ('auto', 'tc', 'tc_pruned') else 0)
+def dense_grid_tiles(res: int, first: int, count: int) -> int:
+    """Tiles of a dense tensor-core query of grid points [first, first + count) of the res^3 grid, as
+    tc_ensemble_launch lays them out: 8 x 4 x 4 blocks for whole 8-plane groups, 1 x 16 x 8 blocks otherwise, linear
+    128-point tiles where blocks would add more than 3 % tiles."""
+    rr = res * res
+    tbx, tby, tbz = (8, 4, 4) if first % rr == 0 and count % (8 * rr) == 0 else (1, 16, 8)
+    px0, px1 = first // rr, (first + count - 1) // rr
+    blocked = ((px1 - px0 + tbx) // tbx) * (-(-res // tby)) * (-(-res // tbz))
+    linear = -(-count // 128)
+    return blocked if blocked * 100 <= linear * 103 else linear
+
+
+def launches_per_grid_query(impl='auto', n_members=40, res=256, first=0, count=None) -> int:
+    """Kernels of one grid query over points [first, first + count) (default: the whole grid) of the res^3 grid: grid
+    axes, anchors and folded constants, then
+      'simt': the ensemble kernel;
+      'tc_pruned', and 'auto' / 'tc' with NPHM_ENS_ABSORB=0: records, layer-2 slabs, tile member masks, the ensemble
+        kernel;
+      'auto' / 'tc' (absorption on: member by member): records, layer-2 slabs, member bounds over the grid, tile member
+        masks, member bounds per sub-box, and per chunk of at most 2^17 tiles (2^24 rows) a member pass and the ensemble
+        kernel per member and the finalize."""
+    if impl == 'simt':
+        return 4
+    if impl == 'tc_pruned' or os.environ.get('NPHM_ENS_ABSORB', '1')[:1] == '0':
+        return 3 + 4
+    count = res ** 3 - first if count is None else count
+    chunks = -(-dense_grid_tiles(res, first, count) // (1 << 17))
+    return 3 + 5 + chunks * (2 * n_members + 1)
 
 
 class EnsembleConfig(Structure):

@@ -134,7 +134,10 @@ __global__ void l2_slab_kernel(const uint8_t *__restrict__ weights, const float 
 // latent-dependent constants and the skip input of layer 2, and the output layer.  Every pre-activation interval grows by
 // kBoundRel * (|W| |h| + |b|) + kBoundAbs, which covers the kernel's 3-pass fp16 products, fp32 sums and approximate
 // softplus with a wide margin.  At least 1 (quirk points blend 1.0); +inf when the bound is not finite.  `scale` multiplies
-// the bound (1 except for the negative control of nphm_debug_ens_bound_scale).
+// the bound (1 except for the negative control of nphm_debug_ens_bound_scale).  Grid (members, queries), written to
+// bounds[query][member]; sub_n > 0: per 32^3-point sub-box of the grid instead, query 0, one-dimensional grid (sub-boxes x
+// members: a 2048^3 grid has 262 144 sub-boxes, more than gridDim.y allows), block b = sub-box b / n_members ((sx - sub_x0,
+// sy, sz) in x-major order, sub_n per axis), member b % n_members, written to bounds[sub-box][member].
 constexpr double kBoundRel = 0x1p-10, kBoundAbs = 0x1p-10;
 __device__ __forceinline__ double softplus64(double x) { return fmax(x, 0.0) + log1p(exp(-100.0 * fabs(x))) / 100.0; }
 __global__ void __launch_bounds__(256) member_bound_kernel(const float *__restrict__ W0, const float *__restrict__ W1,
@@ -143,15 +146,23 @@ __global__ void __launch_bounds__(256) member_bound_kernel(const float *__restri
                                                            int cvec_stride, const int *__restrict__ coff,
                                                            const float *__restrict__ anchors, const float *__restrict__ axes,
                                                            int res, int n_members, int n_symm, double scale,
-                                                           float *__restrict__ bounds)
+                                                           int sub_x0, int sub_n, float *__restrict__ bounds)
 {
-    const int m = blockIdx.x, qi = blockIdx.y, set = member_set(m, n_symm);
+    const long long blk = sub_n > 0 ? (long long)blockIdx.x : (long long)blockIdx.y * n_members + blockIdx.x;
+    const int m = (int)(blk % n_members), qi = sub_n > 0 ? 0 : blockIdx.y, set = member_set(m, n_symm);
     const float *cv = cvec + ((size_t)qi * n_members + m) * cvec_stride;
     __shared__ double hc[kH + 3], hr[kH + 3], oc[kH], orad[kH], xc[3], xr[3];
     if (threadIdx.x < 3) {
         const int d = threadIdx.x;
-        float lo = axes[d * res], hi = lo;
-        for (int i = 1; i < res; ++i) { lo = fminf(lo, axes[d * res + i]); hi = fmaxf(hi, axes[d * res + i]); }
+        int i0 = 0, i1 = res;                    // the grid indices of the box along axis d
+        if (sub_n > 0) {
+            const int sb = (int)(blk / n_members);
+            const int c = d == 0 ? sub_x0 + sb / (sub_n * sub_n) : (d == 1 ? (sb / sub_n) % sub_n : sb % sub_n);
+            i0 = 32 * c;
+            i1 = min(res, i0 + 32);
+        }
+        float lo = axes[d * res + i0], hi = lo;
+        for (int i = i0 + 1; i < i1; ++i) { lo = fminf(lo, axes[d * res + i]); hi = fmaxf(hi, axes[d * res + i]); }
         const double a = m < n_members - 1 ? (double)anchors[((size_t)qi * (n_members - 1) + m) * 3 + d] : 0.0;
         double l = lo - a, h = hi - a;
         if (d == 0 && (m & 1) && m < 2 * n_symm) { const double t = l; l = -h; h = -t; }    // mirrored member
@@ -197,7 +208,7 @@ __global__ void __launch_bounds__(256) member_bound_kernel(const float *__restri
     layer(W4 + (size_t)set * kH, 1, kH, kH, 1.0, 4, false);
     if (threadIdx.x == 0) {
         const double B = fmax(fabs(hc[0]) + hr[0], 1.0) * scale;
-        bounds[(size_t)qi * n_members + m] = isfinite(B) ? __double2float_ru(B) : INFINITY;
+        bounds[blk] = isfinite(B) ? __double2float_ru(B) : INFINITY;
     }
 }
 
@@ -364,7 +375,7 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
         tc::member_bound_kernel<<<grid, 256, 0, stream>>>(
             h->weights.W[0].as<float>(), h->weights.W[1].as<float>(), h->weights.W[2].as<float>(), h->weights.W[3].as<float>(),
             h->weights.W[4].as<float>(), q.cvec, h->dims.cvec_stride, h->tc_coff.as<int>(), q.anchors, q.axes, q.res,
-            h->n_members, h->cfg.n_symm_pairs, h->tc_bound_scale, h->tc_bounds.as<float>());
+            h->n_members, h->cfg.n_symm_pairs, h->tc_bound_scale, 0, 0, h->tc_bounds.as<float>());
         NPHM_CUDA_CHECK(cudaGetLastError());
         p.bounds = h->tc_bounds.as<float>();
         h->tc_absorb_tiles = n_tiles;
@@ -382,6 +393,52 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
         NPHM_CUDA_CHECK(cudaMemsetAsync(h->tc_sched.ptr, 0, 2 * sizeof(unsigned int), stream));
     }
     p.sched = h->tc_sched.as<unsigned int>();
+    // dense grid queries with absorption run member by member (the skip log records the tile-major kernel's decisions, so
+    // a launch with it on stays tile-major): exact per-row absorption decisions and compact tiles of the rows that remain.
+    // The member-major kernel serves one query, as every grid query is
+    h->tc_mm_counts = 0;
+    if (p.absorb && !p.skip_log && q.n_queries == 1) {
+        const long long chunk = std::min(n_tiles, tc::kMmChunkTiles), n_chunks = ceil_div(n_tiles, chunk);
+        if ((rc = h->tc_mm_num.reserve((size_t)chunk * 128 * sizeof(float)))) return rc;
+        if ((rc = h->tc_mm_den.reserve((size_t)chunk * 128 * sizeof(float)))) return rc;
+        if ((rc = h->tc_mm_list.reserve((size_t)chunk * 128 * sizeof(int)))) return rc;
+        if ((rc = h->tc_mm_count.reserve((size_t)n_chunks * h->n_members * sizeof(unsigned int)))) return rc;
+        NPHM_CUDA_CHECK(cudaMemsetAsync(h->tc_mm_count.ptr, 0, (size_t)n_chunks * h->n_members * sizeof(unsigned int), stream));
+        h->tc_mm_counts = n_chunks * h->n_members;
+        // (the whole-box bounds above and the pre-pass's absorb masks are not read on this path: they stay for the debug
+        // entries nphm_debug_ens_bounds / _absorb_masks and the replay test)
+        if ((rc = tc::launch_ensemble_mask(p, false, stream))) return rc;
+        // member bounds per 32^3-point sub-box of the x-planes of the query: a sub-box lies far from more anchors than the
+        // whole grid, so its bound is smaller and certifies more rows
+        const long long rr = (long long)q.res * q.res;
+        const int sx0 = (int)(q.first / rr) >> 5, sx1 = (int)((q.first + q.n_points - 1) / rr) >> 5;
+        const int sub_n = (q.res + 31) / 32;
+        const long long n_sub = (long long)(sx1 - sx0 + 1) * sub_n * sub_n, n_blocks = n_sub * h->n_members;
+        // at most 64^3 sub-boxes (res <= 2048) of kMaxMembers members: far below the 2^31 - 1 blocks of gridDim.x
+        NPHM_REQUIRE(n_blocks < (1ll << 31), "tensor-core ensemble kernel: %lld sub-box bounds", n_blocks);
+        if ((rc = h->tc_sub_bounds.reserve((size_t)n_blocks * sizeof(float)))) return rc;
+        tc::member_bound_kernel<<<(unsigned)n_blocks, 256, 0, stream>>>(
+            h->weights.W[0].as<float>(), h->weights.W[1].as<float>(), h->weights.W[2].as<float>(), h->weights.W[3].as<float>(),
+            h->weights.W[4].as<float>(), q.cvec, h->dims.cvec_stride, h->tc_coff.as<int>(), q.anchors, q.axes, q.res,
+            h->n_members, h->cfg.n_symm_pairs, h->tc_bound_scale, sx0, sub_n, h->tc_sub_bounds.as<float>());
+        NPHM_CUDA_CHECK(cudaGetLastError());
+        p.sub_bounds = h->tc_sub_bounds.as<float>();
+        p.sub_x0 = sx0;
+        p.sub_n = sub_n;
+        p.mm_num = h->tc_mm_num.as<float>();
+        p.mm_den = h->tc_mm_den.as<float>();
+        p.mm_list = h->tc_mm_list.as<int>();
+        for (long long c = 0; c < n_chunks; ++c) {
+            p.mm_t0 = c * chunk;
+            p.mm_tiles = std::min(chunk, n_tiles - p.mm_t0);
+            p.mm_count = h->tc_mm_count.as<unsigned int>() + c * h->n_members;
+            NPHM_CUDA_CHECK(cudaMemsetAsync(p.mm_num, 0, (size_t)p.mm_tiles * 128 * sizeof(float), stream));
+            NPHM_CUDA_CHECK(cudaMemsetAsync(p.mm_den, 0, (size_t)p.mm_tiles * 128 * sizeof(float), stream));
+            // the item count is on the device: every SM takes part
+            if ((rc = tc::launch_member_major_chunk(p, sm_count(), stream))) return rc;
+        }
+        return NPHM_OK;
+    }
     const long long n_items = n_tiles * p.member_groups;
     // 32-bit counter: the counter passes n_items by at most one per CTA
     NPHM_REQUIRE(n_items + sm_count() < (1ll << 32), "tensor-core ensemble kernel: %lld work items", n_items);
@@ -444,6 +501,15 @@ extern "C" int nphm_debug_ens_skipped(nphm_ensemble *h, unsigned long long *host
     using namespace nphm;
     NPHM_REQUIRE(h, "nphm_debug_ens_skipped: null handle");
     return copy_debug(h->tc_skip_log, sizeof(unsigned long long), h->tc_skip_tiles, host, cap, n);
+}
+
+// Debug entry (not part of the public ABI), in the shape of the ones above: the rows the member passes of the handle's last
+// launch listed, per chunk of tiles and member (uint32, chunk-major); 0 when that launch ran tile-major.
+extern "C" int nphm_debug_ens_pair_counts(nphm_ensemble *h, unsigned int *host, long long cap, long long *n)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h, "nphm_debug_ens_pair_counts: null handle");
+    return copy_debug(h->tc_mm_count, sizeof(unsigned int), h->tc_mm_counts, host, cap, n);
 }
 
 extern "C" int nphm_debug_ens_skip_log(nphm_ensemble *h, int enable)

@@ -87,6 +87,18 @@ struct Params {
     const float *bounds;
     // debug (nphm_debug_ens_skip_log): per tile, bit m set when the producer skipped member m by vote; nullptr unless enabled
     unsigned long long *skip_log;
+    // member-major dense grid queries (tc_ensemble_wgmma.cu, member_pass_kernel): a chunk of whole tiles mm_t0 ..
+    // mm_t0 + mm_tiles - 1 keeps num and den per row (index (tile - mm_t0) * 128 + row); the pass of member mm_member lists
+    // the rows that still need it in mm_list and counts them in mm_count[mm_member]
+    int mm_member;
+    long long mm_t0, mm_tiles;
+    float *mm_num, *mm_den;
+    int *mm_list;
+    unsigned int *mm_count;
+    // member bounds per 32^3-point sub-box of the grid (member_bound_kernel over the sub-box): [sub-box][member], sub-boxes
+    // (sx - sub_x0, sy, sz) in x-major order, sub_n per axis; nullptr: the whole-box bounds
+    const float *sub_bounds;
+    int sub_x0, sub_n;
 };
 
 // One row (point) of a tile: its index in the query, its global point index, whether the tile covers a real point with
@@ -97,6 +109,7 @@ struct TilePoint {
     long long idx, g;
     bool valid;
     float x, y, z;
+    int ix, iy, iz;            // grid coordinates (grid queries), clamped to the grid
 };
 __device__ __forceinline__ TilePoint tile_point(const Params &p, bool blocked, long long tile, int qi,
                                                 long long tiles_per_query, int row)
@@ -113,6 +126,7 @@ __device__ __forceinline__ TilePoint tile_point(const Params &p, bool blocked, l
         t.idx = t.g - p.first;
         const int cx_ = min(ix, p.res - 1), cy_ = min(iy, p.res - 1), cz_ = min(iz, p.res - 1);
         t.x = __ldg(p.axes + cx_); t.y = __ldg(p.axes + p.res + cy_); t.z = __ldg(p.axes + 2 * p.res + cz_);
+        t.ix = cx_; t.iy = cy_; t.iz = cz_;
         if (!t.valid) t.g = p.first;
     } else {
         t.idx = (tile - (long long)qi * tiles_per_query) * 128 + row;
@@ -121,10 +135,12 @@ __device__ __forceinline__ TilePoint tile_point(const Params &p, bool blocked, l
         if (p.xyz) {
             const float *pp = p.xyz + ((size_t)qi * p.n_points + (t.valid ? t.idx : 0)) * 3;
             t.x = pp[0]; t.y = pp[1]; t.z = pp[2];
+            t.ix = t.iy = t.iz = 0;
         } else {
             const long long rr = (long long)p.res * p.res;
             const int ix = (int)(t.g / rr), iy = (int)((t.g - ix * rr) / p.res), iz = (int)(t.g % p.res);
             t.x = __ldg(p.axes + ix); t.y = __ldg(p.axes + p.res + iy); t.z = __ldg(p.axes + 2 * p.res + iz);
+            t.ix = ix; t.iy = iy; t.iz = iz;
         }
     }
     return t;
@@ -162,6 +178,11 @@ __device__ __forceinline__ float weight_sum(const float *anc, int n_members, flo
 }
 
 int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream);
+// member-major order of a dense grid query with absorption (p.mm_* set, chunk of at most kMmChunkTiles tiles): per member,
+// the pass that blends quirk rows, skips absorbed rows and lists the rest, then the ensemble kernel on that list
+constexpr long long kMmChunkTiles = 1ll << 17;     // 2^24 rows: 12 B of state per row
+int launch_member_major_chunk(const Params &p, int grid_x, cudaStream_t stream);
+int launch_ensemble_mask(const Params &p, bool prune, cudaStream_t stream);
 
 }  // namespace tc
 }  // namespace nphm

@@ -26,6 +26,9 @@
 // (Params::tbx, tby, tbz) so that a tile lies far from many anchors.  Dense grid queries also skip the members whose blend
 // terms fp32 rounding absorbs (the producer warpgroup decides per point, see there); the producer tells the consumers which member
 // each record slot holds and ends a tile with a record slot without a copy.
+// Dense grid queries with absorption run member by member instead (MM variant): per member, member_pass_kernel decides
+// every row on the exact state and lists the rows that need the member, and the kernel runs 128-row tiles of that list,
+// whose rows the producer warpgroup gathers into shared memory one work item ahead.
 #include "tc_ensemble.cuh"
 
 namespace nphm {
@@ -84,6 +87,10 @@ struct __align__(128) Smem {
     // then the consumer warp that owns the row (rows 16 warp .. 16 warp + 15) sets pub_seq[warp] = r + 1
     float pub_num[4][128];
     unsigned int pub_seq[kConsumerWarps];
+    // member-major: the rows of the queue's two work items, staged by the producer warpgroup (thread prow: row prow): point,
+    // num, chunk state index (-1: past the end of the member's list)
+    float mm_pt[2][4][128];
+    int mm_pos[2][128];
 };
 static_assert(sizeof(Smem) <= 227 * 1024, "shared memory of the ensemble kernel exceeds the 227 KB of an H100 block");
 
@@ -183,8 +190,78 @@ __global__ void __launch_bounds__(32 * kMaskWarps) tile_mask_kernel(const Params
     }
 }
 
-// LOG: the debug skip log (Params::skip_log) - a variant of its own, so that the kernel without it is not slowed by it
-template <bool PRUNE, bool ACTS, bool LOG = false>
+// Member-major order (dense grid queries with absorption): before member k runs, every row of the chunk holds num and den
+// after members 0 .. k-1 exactly, so the pass of member k decides per row with no lag.  One warp per tile, 4 rows per lane,
+// only tiles whose pre-pass mask has bit k (elsewhere w_k = +0 at every valid point).  At a valid row with w = w_k != +0
+// (member_weight(), bit for bit the blend's weight):
+//   quirk row (every member outputs 1.0): blended here, num = fmaf(w, 1, num), den += w;
+//   absorbed: den + w == den and w * B_k (rounded up) < ulp(|num|) / 4 with |s_k| <= B_k (member_bound_kernel), so that
+//     fmaf(w, s_k, num) == num: nothing changes;
+//   otherwise den += w and the row goes to member k's list (a warp-aggregated append), whose num the ensemble kernel
+//     updates with fmaf(w, s_k, num).
+// Each row's num and den see the same terms in the same order as in the tile-major kernel, whose skips are exact too:
+// the outputs are the same bits.
+__global__ void __launch_bounds__(32 * kMaskWarps) member_pass_kernel(const Params p)
+{
+    const long long lt = (long long)blockIdx.x * kMaskWarps + (threadIdx.x >> 5);
+    if (lt >= p.mm_tiles) return;
+    const long long tile = p.mm_t0 + lt;
+    const int k = p.mm_member, lane = threadIdx.x & 31;
+    if (!((p.tile_masks[tile] >> k) & 1)) return;
+    const long long tiles_per_query = p.blocked ? p.n_tiles : (p.n_points + 127) / 128;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int row = lane + 32 * i;
+        const int s = (int)(lt * 128 + row);
+        const TilePoint t = tile_point(p, p.blocked, tile, 0, tiles_per_query, row);
+        bool listed = false;
+        if (t.valid) {
+            const float B = p.sub_bounds ? p.sub_bounds[((size_t)(((t.ix >> 5) - p.sub_x0) * p.sub_n + (t.iy >> 5)) * p.sub_n +
+                                                          (t.iz >> 5)) * p.n_members + k]
+                                         : p.bounds[k];
+            const float w = member_weight(p.anchors, k, p.n_members, t.x, t.y, t.z);
+            if (w != 0.f) {
+                const bool quirk = p.quirk_period > 0 && ((t.g % p.quirk_period) == p.quirk_period - 1 || t.g == p.total - 1);
+                const float num = p.mm_num[s], den = p.mm_den[s];
+                if (quirk) {
+                    p.mm_num[s] = fmaf(w, 1.0f, num);
+                    p.mm_den[s] = den + w;
+                } else {
+                    const float L = fabsf(num);
+                    // ulp(L) / 4 = 2^(e(L) - 25), exact for L >= 2^-100; NaN, smaller L and B = +inf never certify
+                    const bool absorbed = den + w == den && B < INFINITY && L >= 0x1p-100f &&
+                                          __fmul_ru(w, B) < __uint_as_float(((__float_as_uint(L) >> 23) - 25) << 23);
+                    if (!absorbed) {
+                        p.mm_den[s] = den + w;
+                        listed = true;
+                    }
+                }
+            }
+        }
+        const unsigned int ballot = __ballot_sync(0xffffffffu, listed);
+        if (ballot) {
+            unsigned int base = 0;
+            if (lane == 0) base = atomicAdd(p.mm_count + k, (unsigned int)__popc(ballot));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (listed) p.mm_list[base + __popc(ballot & ((1u << lane) - 1))] = s;
+        }
+    }
+}
+
+// Member-major: the blend of every valid row of the chunk, out = num / (den + 1e-6), the tile-major kernel's expression
+__global__ void __launch_bounds__(256) member_finalize_kernel(const Params p)
+{
+    const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= p.mm_tiles * 128) return;
+    const long long tiles_per_query = p.blocked ? p.n_tiles : (p.n_points + 127) / 128;
+    const TilePoint t = tile_point(p, p.blocked, p.mm_t0 + s / 128, 0, tiles_per_query, (int)(s % 128));
+    if (t.valid) p.out[t.idx] = __fdiv_rn(p.mm_num[s], p.mm_den[s] + 1e-6f);
+}
+
+// LOG: the debug skip log (Params::skip_log) - a variant of its own, so that the kernel without it is not slowed by it.
+// MM: member-major dense grid query - every work item is a tile of 128 listed rows of member p.mm_member (member_pass_kernel),
+// which load num from the chunk's state and store it back after the blend (den and out are the pass's and finalize's)
+template <bool PRUNE, bool ACTS, bool LOG = false, bool MM = false>
 __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Params p)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -195,7 +272,9 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     // ACTS (fitting: few points, so few tiles): the members of a tile are split over `member_groups` CTAs - a work item is
     // (tile, group of consecutive members), the in-kernel blend is meaningless then and `out` is not written
     const int n_groups = ACTS ? p.member_groups : 1;
-    const long long n_items = n_tiles * n_groups;
+    // MM: the items of the member's row list, counted by the pass launched before on the stream
+    const long long mm_rows = MM ? (long long)p.mm_count[p.mm_member] : 0;
+    const long long n_items = MM ? (mm_rows + 127) / 128 : n_tiles * n_groups;
     auto group_mask = [&](long long item) -> unsigned long long {
         const unsigned long long all = p.n_members >= 64 ? ~0ull : (1ull << p.n_members) - 1;
         if (!ACTS || n_groups == 1) return all;
@@ -218,8 +297,8 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
 #endif
     // tile masks from the pre-pass: the pruned rule, or (dense variant) exactly zero blend weights
     const bool premask = PRUNE || (!ACTS && p.zero_skip);
-    // members absorbed by fp32 rounding (dense variant with the zero-weight masks only)
-    const bool absorb = !PRUNE && !ACTS && p.zero_skip && p.absorb;
+    // members absorbed by fp32 rounding (dense variant with the zero-weight masks only; member-major: decided by the pass)
+    const bool absorb = !PRUNE && !ACTS && !MM && p.zero_skip && p.absorb;
 
     if (warp >= kConsumerWarps) {
         // =========================================================================== producer (tiles, bulk async copies)
@@ -241,26 +320,44 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
                     ENS_TILE(tcount, 1);
                     mbar_wait(&sm.q_empty[qs], ((tcount >> 1) & 1) ^ 1);
                     sm.q_item[qs] = item < n_items ? (long long)item : -1;
-                    mbar_arrive(&sm.q_full[qs]);
+                    if (!MM) mbar_arrive(&sm.q_full[qs]);
                 }
                 __syncwarp();
                 producer_sync();
                 // q_item[qs] is rewritten two tiles later, after every producer thread has passed the next tile's sync
                 const long long qitem = sm.q_item[qs];
+                if (MM) {
+                    // the item's listed rows, gathered here while the consumers still run the previous item: thread
+                    // prow stages row prow (listed row qitem * 128 + prow of the member), then the lead publishes the item
+                    if (qitem >= 0) {
+                        const long long s = qitem * 128 + prow;
+                        const int pos = s < mm_rows ? p.mm_list[s] : -1;
+                        const TilePoint t = tile_point(p, p.blocked, p.mm_t0 + max(pos, 0) / 128, 0, tiles_per_query, max(pos, 0) % 128);
+                        sm.mm_pt[qs][0][prow] = t.x;
+                        sm.mm_pt[qs][1][prow] = t.y;
+                        sm.mm_pt[qs][2][prow] = t.z;
+                        sm.mm_pt[qs][3][prow] = pos >= 0 ? p.mm_num[pos] : 0.f;
+                        sm.mm_pos[qs][prow] = pos;
+                    }
+                    producer_sync();
+                    if (lead) mbar_arrive(&sm.q_full[qs]);
+                }
                 if (qitem < 0) {
 #ifdef NPHM_ENS_TRACE
                     if (lead && blockIdx.x < kTraceMaxCtas) {
-                        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x + 2] = tcount;
-                        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x + 3] = t_decide;
-                        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x + 4] = t_wait;
+                        // member-major: every word summed over the member launches of the query (zeroed before the first;
+                        // the decision words stay 0, the producer decides nothing there)
+                        long long *w = g_ens_ctas + 1 + kTraceCtaWords * blockIdx.x;
+                        if (MM) { w[2] += tcount; w[3] += t_decide; w[4] += t_wait; }
+                        else { w[2] = tcount; w[3] = t_decide; w[4] = t_wait; }
                     }
 #endif
                     break;
                 }
                 const unsigned int item = (unsigned int)qitem;
                 const unsigned int tile = ACTS ? item / n_groups : item;
-                const int qi = p.blocked ? 0 : (int)(tile / (unsigned int)tiles_per_query);
-                unsigned long long mask = premask ? p.tile_masks[tile] : group_mask(item);
+                const int qi = (MM || p.blocked) ? 0 : (int)(tile / (unsigned int)tiles_per_query);
+                unsigned long long mask = MM ? 1ull << p.mm_member : (premask ? p.tile_masks[tile] : group_mask(item));
                 // absorption: skip member m when den + w == den at every valid point (pre-pass) and, at every valid point p
                 // with w_m(p) != 0, w_m(p) * B_m < ulp(L(p)) / 4 (so that fmaf(w, s, num) returns num), with |s_m| <= B_m
                 // (member_bound_kernel) and |num(p)| >= L(p) = |num(p)| after the member two record positions back
@@ -395,24 +492,43 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
         const int qs = tcount & 1;
         mbar_wait(&sm.q_full[qs], (tcount >> 1) & 1);
         const long long item = sm.q_item[qs];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm.q_empty[qs]);
+        // (member-major: the slot's staged rows are read below, before the slot is released)
+        if (!MM || item < 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&sm.q_empty[qs]);
+        }
         if (item < 0) break;
         if (threadIdx.x == 0) ENS_TILE(tcount, 0);
         const long long tile = ACTS ? item / n_groups : item;
-        const int qi = p.blocked ? 0 : (int)(tile / tiles_per_query);
+        const int qi = (MM || p.blocked) ? 0 : (int)(tile / tiles_per_query);
         long long idx[2], g[2];
         bool valid[2], quirk[2];
         float x[2], y[2], z[2];
         float num[2] = {0.f, 0.f}, den[2] = {0.f, 0.f};
+        int mpos[2];                             // MM: the rows' chunk state index
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
+            if (MM) {
+                // listed row tile * 128 + rl[i] of the member, as the producer staged it: its point and num after the
+                // members before; rows past the list end run on the chunk's first point and do not store
+                mpos[i] = sm.mm_pos[qs][rl[i]];
+                valid[i] = mpos[i] >= 0;
+                x[i] = sm.mm_pt[qs][0][rl[i]]; y[i] = sm.mm_pt[qs][1][rl[i]]; z[i] = sm.mm_pt[qs][2][rl[i]];
+                num[i] = sm.mm_pt[qs][3][rl[i]];
+                idx[i] = g[i] = 0;
+                quirk[i] = false;                // quirk rows are blended by the pass, never listed
+                continue;
+            }
             // (the fitting variant only runs linear tiles)
             const TilePoint t = tile_point(p, !ACTS && p.blocked, tile, qi, tiles_per_query, rl[i]);
             idx[i] = t.idx; g[i] = t.g; valid[i] = t.valid; x[i] = t.x; y[i] = t.y; z[i] = t.z;
             quirk[i] = p.quirk_period > 0 && ((g[i] % p.quirk_period) == p.quirk_period - 1 || g[i] == p.total - 1);
             // pruned rule: the blend divides by S = sum_k w_k over all members, evaluated or not
             if (PRUNE) den[i] = weight_sum(p.anchors + (size_t)qi * (p.n_members - 1) * 3, p.n_members, x[i], y[i], z[i]);
+        }
+        if (MM) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&sm.q_empty[qs]);
         }
         const uint32_t tile_rc0 = rcount;        // the tile's first member (timeline build)
 
@@ -684,28 +800,69 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
             ++rcount;
         }
 #pragma unroll
-        for (int r = 0; r < 2; ++r)
-            if (q4 == 0 && valid[r] && n_groups == 1) p.out[(size_t)qi * p.n_points + idx[r]] = __fdiv_rn(num[r], den[r] + 1e-6f);
+        for (int r = 0; r < 2; ++r) {
+            if (MM) {
+                if (q4 == 0 && valid[r]) p.mm_num[mpos[r]] = num[r];
+            } else if (q4 == 0 && valid[r] && n_groups == 1) {
+                p.out[(size_t)qi * p.n_points + idx[r]] = __fdiv_rn(num[r], den[r] + 1e-6f);
+            }
+        }
     }
     if (wgi == 0) take_turn();                   // the turn warpgroup 1 passed after its last phase
 #ifdef NPHM_ENS_TRACE
     if (threadIdx.x == 0 && blockIdx.x < kTraceMaxCtas) {
-        g_ens_ctas[1 + kTraceCtaWords * blockIdx.x] = n_eval;
-        g_ens_ctas[2 + kTraceCtaWords * blockIdx.x] = clock64() - cta_start;
+        if (MM) {
+            g_ens_ctas[1 + kTraceCtaWords * blockIdx.x] += n_eval;
+            g_ens_ctas[2 + kTraceCtaWords * blockIdx.x] += clock64() - cta_start;
+        } else {
+            g_ens_ctas[1 + kTraceCtaWords * blockIdx.x] = n_eval;
+            g_ens_ctas[2 + kTraceCtaWords * blockIdx.x] = clock64() - cta_start;
+        }
     }
 #endif
 }
 
 }  // namespace wg
 
-int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream)
+int launch_ensemble_mask(const Params &p, bool prune, cudaStream_t stream)
 {
-    if (prune || (!acts && p.zero_skip)) {
-        const unsigned blocks = (unsigned)ceil_div(p.n_tiles, (long long)wg::kMaskWarps);
-        if (prune) wg::tile_mask_kernel<true><<<blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
-        else wg::tile_mask_kernel<false><<<blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
+    const unsigned blocks = (unsigned)ceil_div(p.n_tiles, (long long)wg::kMaskWarps);
+    if (prune) wg::tile_mask_kernel<true><<<blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
+    else wg::tile_mask_kernel<false><<<blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int launch_member_major_chunk(const Params &p0, int grid_x, cudaStream_t stream)
+{
+    const int smem = (int)sizeof(wg::Smem);
+    auto kern = wg::ensemble_wgmma_kernel<false, false, false, true>;
+    NPHM_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+#ifdef NPHM_ENS_TRACE
+    if (p0.mm_t0 == 0) {                         // the work counts of the trace build sum over the query's member launches
+        void *ctas = nullptr;
+        NPHM_CUDA_CHECK(cudaGetSymbolAddress(&ctas, wg::g_ens_ctas));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(ctas, 0, sizeof(wg::g_ens_ctas), stream));
+    }
+#endif
+    const unsigned pass_blocks = (unsigned)ceil_div(p0.mm_tiles, (long long)wg::kMaskWarps);
+    Params p = p0;
+    for (int k = 0; k < p.n_members; ++k) {
+        p.mm_member = k;
+        wg::member_pass_kernel<<<pass_blocks, 32 * wg::kMaskWarps, 0, stream>>>(p);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+        kern<<<grid_x, wg::kThreads, smem, stream>>>(p);
         NPHM_CUDA_CHECK(cudaGetLastError());
     }
+    wg::member_finalize_kernel<<<(unsigned)ceil_div(p.mm_tiles * 128, 256ll), 256, 0, stream>>>(p);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int launch_ensemble_wgmma(const Params &p, bool prune, bool acts, int grid_x, cudaStream_t stream)
+{
+    int rc;
+    if ((prune || (!acts && p.zero_skip)) && (rc = launch_ensemble_mask(p, prune, stream))) return rc;
     const int smem = (int)sizeof(wg::Smem);
     auto kern = acts ? wg::ensemble_wgmma_kernel<false, true>
                      : (prune ? wg::ensemble_wgmma_kernel<true, false>

@@ -18,10 +18,15 @@ zero-weight skip and the ones the certificate would remove on top:
       a tile are never certified (keys absorbed_point, evaluated_point);
     - tile-wide (the kernel before per-point): the minimum of |num| over the tile after the member two evaluated positions
       earlier, minus max_w * B of the member evaluated in between (max_w rounded up to a power of two), paired with the
-      tile's largest weight (keys absorbed, evaluated_absorb).
+      tile's largest weight (keys absorbed, evaluated_absorb);
+    - member by member (the kernel's dense grid queries): per point with L(p) = |num(p)| after member k - 1, no lag, and
+      B_k of the point's 32^3-point sub-box of the grid (the box of its grid indices 32 c .. 32 c + 31 per axis); a (point,
+      member) pair is evaluated when w != +0, the point is not a quirk row (it blends 1.0 without the network) and the
+      certificate fails; member k's pairs run in ceil(n_k / 128) tiles (keys compact_pairs per member, compact_tiles;
+      compact_pairs_box, compact_tiles_box with the whole-box B_k).
 num and den come from the fp32 member outputs of the CPU reference (tests/ensemble_f64_common.py).
 
-    python tools/absorbed_member_tiles.py [--latent 1] [--res 64] [--scale 1] [--plane-stride 1] [--quirk-period 0]
+    python tools/absorbed_member_tiles.py [--latent 1] [--res 64] [--scale 1] [--plane-stride 1] [--quirk-period 0] [--compact]
 
 replay() is the per-point rule over a batch of tiles in torch (any device): predict() runs it on its own decisions, and
 tests/test_gpu_ensemble_absorb_replay.py on the decisions the kernel logged, with the kernel's weights, bounds and masks.
@@ -364,8 +369,21 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
     n_tiles = ix.shape[0]
     stats = {'tiles': int(n_tiles), 'member_tiles': int(n_tiles * M), 'zero': 0, 'den_absorbed': 0, 'absorbed': 0,
              'absorbed_no_lag': 0, 'absorbed_tile_max': 0, 'unchanged': 0, 'B': B,
-             'absorbed_point': 0, 'absorbed_point_no_lag': 0}
+             'absorbed_point': 0, 'absorbed_point_no_lag': 0, 'compact_pairs': np.zeros(M, np.int64),
+             'compact_pairs_box': np.zeros(M, np.int64)}
     B32 = f32_up(B)                                     # the kernel's B_k (member_bound_kernel rounds up; inf stays inf)
+    # B_k per 32^3-point sub-box (member by member): [member][sx][sy][sz]
+    n_sub = (res + 31) // 32
+    sub_lo = [[axes[a][32 * c:32 * c + 32].min() for c in range(n_sub)] for a in range(3)]
+    sub_hi = [[axes[a][32 * c:32 * c + 32].max() for c in range(n_sub)] for a in range(3)]
+    B32_sub = np.zeros((M, n_sub, n_sub, n_sub), np.float32)
+    for m in range(M):
+        for cx in range(n_sub):
+            for cy in range(n_sub):
+                for cz in range(n_sub):
+                    lo_s = np.array([sub_lo[0][cx], sub_lo[1][cy], sub_lo[2][cz]], np.float64)
+                    hi_s = np.array([sub_hi[0][cx], sub_hi[1][cy], sub_hi[2][cz]], np.float64)
+                    B32_sub[m, cx, cy, cz] = f32_up(member_bound(P64, m, z, anc_np.astype(np.float64), lo_s, hi_s))
     gw = np.float32(np.exp(np.float32(-0.2) / np.float32(0.01)))
     for t0 in range(0, n_tiles, chunk_tiles):
         sl = slice(t0, min(n_tiles, t0 + chunk_tiles))
@@ -375,9 +393,11 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
         pts = torch.from_numpy(X.reshape(-1, 3))
         with torch.no_grad():
             S = members(P32, pts, z, anc32).numpy().reshape(T, 128, M)
+        Q = np.zeros((T, 128), bool)
         if quirk_period > 0:
             g = (ix[sl] * res + iy[sl]) * res + iz[sl]
-            S[(g % quirk_period == quirk_period - 1) | (g == count - 1)] = 1.0
+            Q = (g % quirk_period == quirk_period - 1) | (g == count - 1)
+            S[Q] = 1.0
         with np.errstate(under='ignore'):
             d = anc_np[None, None] - X[:, :, None, :]                                       # T x 128 x 39 x 3
             d2 = np.float32(d[..., 2] * d[..., 2] + (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]))
@@ -410,6 +430,12 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
             cand = den_abs & ~zero & np.isfinite(B32[k])
             no_lag_p = cand & np.all(point_pass(w, B32[k], np.abs(num), np.float32(0), V), axis=1)
             stats['absorbed_point_no_lag'] += int(no_lag_p.sum())
+            # member by member: the exact state after member k - 1 at every point, quirk rows blended without the network
+            need = V & (w != 0) & ~Q & ~(((den + w) == den) & point_pass(w, B32[k], np.abs(num), np.float32(0), V))
+            stats['compact_pairs_box'][k] += int(need.sum())
+            Bp = B32_sub[k][np.minimum(ix[sl], res - 1) >> 5, np.minimum(iy[sl], res - 1) >> 5, np.minimum(iz[sl], res - 1) >> 5]
+            need = V & (w != 0) & ~Q & ~(((den + w) == den) & point_pass(w, Bp, np.abs(num), np.float32(0), V))
+            stats['compact_pairs'][k] += int(need.sum())
             zero_all[:, k], den_all[:, k], unchanged_all[:, k] = zero, den_abs, unchanged
             stats['zero'] += int(zero.sum())
             stats['den_absorbed'] += int((den_abs & ~zero).sum())
@@ -433,6 +459,8 @@ def predict(latent_seed=1, res=64, scale=1.0, mini=None, maxi=None, plane_stride
     stats['evaluated_now'] = n - stats['zero']
     stats['evaluated_absorb'] = stats['evaluated_now'] - stats['absorbed']
     stats['evaluated_point'] = stats['evaluated_now'] - stats['absorbed_point']
+    stats['compact_tiles'] = int(((stats['compact_pairs'] + 127) // 128).sum())
+    stats['compact_tiles_box'] = int(((stats['compact_pairs_box'] + 127) // 128).sum())
     return stats
 
 
@@ -457,6 +485,7 @@ def main():
     ap.add_argument('--tile', default='auto', help='auto or a block shape XxYxZ with X*Y*Z = 128 (zero_member_tiles.py)')
     ap.add_argument('--planes', type=int, nargs=2, metavar=('X0', 'X1'), default=None,
                     help='count the tiles of x-planes X0 .. X1-1 only (multiples of the block depth): compares layouts fairly')
+    ap.add_argument('--compact', action='store_true', help='also print the member-by-member counts: pairs and compact tiles')
     args = ap.parse_args()
     r = predict(args.latent, args.res, args.scale, plane_stride=args.plane_stride, quirk_period=args.quirk_period,
                 tile=args.tile, planes=args.planes)
@@ -476,6 +505,13 @@ def main():
     print('per point (the kernel): %d (%.1f %%) -> %d evaluated; per point without the lag: %d (%.1f %%)'
           % (r['absorbed_point'], 100 * r['absorbed_point'] / ev, r['evaluated_point'], r['absorbed_point_no_lag'],
              100 * r['absorbed_point_no_lag'] / ev))
+    if args.compact:
+        print('member by member (per point, no lag, quirk rows blended directly), whole-box B_k: %d (point, member) pairs '
+              'evaluated in %d compact tiles (x%.3f fewer than per point)'
+              % (r['compact_pairs_box'].sum(), r['compact_tiles_box'], r['evaluated_point'] / max(r['compact_tiles_box'], 1)))
+        print('member by member, B_k per 32^3-point sub-box (the kernel): %d pairs in %d compact tiles (x%.3f fewer than '
+              'per point)' % (r['compact_pairs'].sum(), r['compact_tiles'], r['evaluated_point'] / max(r['compact_tiles'], 1)))
+        print('pairs per member: %s' % ' '.join(str(int(v)) for v in r['compact_pairs']))
     print('B_k: min %.3g, median %.3g, max %.3g' % (r['B'].min(), np.median(r['B']), r['B'].max()))
 
 
