@@ -59,9 +59,11 @@ struct nphm_ensemble {
     nphm::DeviceBuffer tc_skip_log;
     bool tc_skip_log_on = false;
     // member-major dense grid queries: num, den and the row list of one chunk of tiles, and the rows listed per (chunk,
-    // member) by the last launch (tc_mm_counts of them; 0 when it ran tile-major)
+    // member) by the last launch (tc_mm_counts of them; 0 when it ran tile-major); the member bounds per 32^3-point sub-box
+    // of that launch (tc_sub_bound_count of them, sub-boxes from x-slab tc_sub_x0, tc_sub_n per axis; 0 when tile-major)
     nphm::DeviceBuffer tc_mm_num, tc_mm_den, tc_mm_list, tc_mm_count, tc_sub_bounds;
-    long long tc_mm_counts = 0;
+    long long tc_mm_counts = 0, tc_sub_bound_count = 0;
+    int tc_sub_x0 = 0, tc_sub_n = 0;
     double tc_bound_scale = 1.0;               // factor on every member bound (1; a debug entry sets it for a negative control)
     bool tc_ready = false;
     bool tc_prune = false;          // opt-in member pruning (NPHM_IMPL_TC_PRUNED)

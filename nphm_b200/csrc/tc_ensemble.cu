@@ -396,7 +396,8 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
     // dense grid queries with absorption run member by member (the skip log records the tile-major kernel's decisions, so
     // a launch with it on stays tile-major): exact per-row absorption decisions and compact tiles of the rows that remain.
     // The member-major kernel serves one query, as every grid query is
-    h->tc_mm_counts = 0;
+    h->tc_mm_counts = h->tc_sub_bound_count = 0;
+    h->tc_sub_x0 = h->tc_sub_n = 0;
     if (p.absorb && !p.skip_log && q.n_queries == 1) {
         const long long chunk = std::min(n_tiles, tc::kMmChunkTiles), n_chunks = ceil_div(n_tiles, chunk);
         if ((rc = h->tc_mm_num.reserve((size_t)chunk * 128 * sizeof(float)))) return rc;
@@ -425,6 +426,9 @@ int tc_ensemble_launch(nphm_ensemble *h, const SimtQuery &q, cudaStream_t stream
         p.sub_bounds = h->tc_sub_bounds.as<float>();
         p.sub_x0 = sx0;
         p.sub_n = sub_n;
+        h->tc_sub_bound_count = n_blocks;
+        h->tc_sub_x0 = sx0;
+        h->tc_sub_n = sub_n;
         p.mm_num = h->tc_mm_num.as<float>();
         p.mm_den = h->tc_mm_den.as<float>();
         p.mm_list = h->tc_mm_list.as<int>();
@@ -510,6 +514,18 @@ extern "C" int nphm_debug_ens_pair_counts(nphm_ensemble *h, unsigned int *host, 
     using namespace nphm;
     NPHM_REQUIRE(h, "nphm_debug_ens_pair_counts: null handle");
     return copy_debug(h->tc_mm_count, sizeof(unsigned int), h->tc_mm_counts, host, cap, n);
+}
+
+// Debug entry (not part of the public ABI), in the shape of the ones above: the member bounds per 32^3-point sub-box of the
+// handle's last launch, [sub-box][member] (float; sub-box (sx - sub_x0, sy, sz) in x-major order, sub_n per axis); *sub_x0
+// and *sub_n receive the first x-slab and the sub-boxes per axis.  0 when that launch ran tile-major.
+extern "C" int nphm_debug_ens_sub_bounds(nphm_ensemble *h, float *host, long long cap, long long *n, int *sub_x0, int *sub_n)
+{
+    using namespace nphm;
+    NPHM_REQUIRE(h && sub_x0 && sub_n, "nphm_debug_ens_sub_bounds: null argument");
+    *sub_x0 = h->tc_sub_x0;
+    *sub_n = h->tc_sub_n;
+    return copy_debug(h->tc_sub_bounds, sizeof(float), h->tc_sub_bound_count, host, cap, n);
 }
 
 extern "C" int nphm_debug_ens_skip_log(nphm_ensemble *h, int enable)

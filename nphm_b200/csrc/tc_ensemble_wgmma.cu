@@ -275,12 +275,13 @@ __global__ void __launch_bounds__(kThreads, 1) ensemble_wgmma_kernel(const Param
     // MM: the items of the member's row list, counted by the pass launched before on the stream
     const long long mm_rows = MM ? (long long)p.mm_count[p.mm_member] : 0;
     const long long n_items = MM ? (mm_rows + 127) / 128 : n_tiles * n_groups;
+    // members 0 .. n - 1 as a mask, n <= 64 (a shift by 64 is undefined in C++)
+    auto bits_below = [](int n) -> unsigned long long { return n >= 64 ? ~0ull : (1ull << n) - 1; };
     auto group_mask = [&](long long item) -> unsigned long long {
-        const unsigned long long all = p.n_members >= 64 ? ~0ull : (1ull << p.n_members) - 1;
-        if (!ACTS || n_groups == 1) return all;
+        if (!ACTS || n_groups == 1) return bits_below(p.n_members);
         const int per = (p.n_members + n_groups - 1) / n_groups, lo = (int)(item % n_groups) * per;
         const int hi = min(p.n_members, lo + per);
-        return ((1ull << hi) - 1) & ~((1ull << lo) - 1);
+        return bits_below(hi) & ~bits_below(lo);
     };
 
     if (threadIdx.x == 0) {

@@ -26,6 +26,15 @@ CONFIGS = {
     'prod-x2': (39, 16, 64, 32, 200, 4, 'x2'),
     'tc-64m': (63, 16, 64, 32, 200, 4, 'init'),        # 64 members: the most the tensor-core kernel's member masks hold
     'tc-65m': (64, 16, 64, 32, 200, 4, 'init'),        # 65 members at the tensor-core widths: the FFMA kernels
+    # other member structures the tensor-core kernel takes (hidden 200, 4 layers, G + L = 96, at most 64 members)
+    'tc-2m': (1, 0, 64, 32, 200, 4, 'init'),           # fewest members: one local member and the global one
+    'tc-3m-pair': (2, 1, 64, 32, 200, 4, 'stack'),     # one mirrored pair and nothing else
+    'tc-nosymm': (39, 0, 64, 32, 200, 4, 'init'),      # the production anchors without a mirror: 40 weight sets
+    'tc-allpairs': (38, 19, 64, 32, 200, 4, 'init'),   # every local member mirrored or mirroring
+    'tc-33m': (32, 8, 64, 32, 200, 4, 'x2'),           # the global member at mask bit 32, just past a 32-bit word
+    'tc-64m-nosymm': (63, 0, 64, 32, 200, 4, 'init'),  # 64 members and 64 weight sets: mask bit 63, the most sets
+    'tc-split-32-64': (39, 16, 32, 64, 200, 4, 'init'),    # another latent split: wide local codes
+    'tc-split-80-16': (39, 16, 80, 16, 200, 4, 'stack'),   # another latent split: narrow local codes
     'api': (10, 3, 32, 16, 160, 4, 'init'),
     'fit': (39, 16, 16, 8, 128, 4, 'stack'),
     'symm0': (5, 0, 16, 8, 64, 4, 'stack'),

@@ -98,6 +98,9 @@ def test_rescaled_weights_reach_the_softplus_kink_and_its_saturated_end(name):
 @pytest.mark.parametrize('name,training,grad_points,want', [
     ('prod', True, False, True), ('prod', True, True, True), ('prod', False, False, True), ('prod', False, True, True),
     ('tc-64m', False, True, True),
+    ('tc-2m', True, True, True), ('tc-2m', False, True, True),
+    ('tc-64m-nosymm', True, True, True), ('tc-64m-nosymm', False, True, True),
+    ('tc-allpairs', False, True, True), ('tc-split-32-64', False, True, True), ('tc-split-80-16', False, True, True),
     # 65 members at the tensor-core widths: the FFMA step only (training mode, no point gradients)
     ('tc-65m', True, False, True), ('tc-65m', True, True, False), ('tc-65m', False, False, False),
     ('api', True, False, True), ('api', True, True, False), ('api', False, False, False),

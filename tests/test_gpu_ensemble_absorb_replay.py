@@ -73,6 +73,9 @@ def lib():
     L = _native.lib()
     for f in ('nphm_debug_ens_tile_masks', 'nphm_debug_ens_absorb_masks', 'nphm_debug_ens_skipped', 'nphm_debug_ens_bounds'):
         getattr(L, f).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.POINTER(ctypes.c_longlong)]
+    L.nphm_debug_ens_sub_bounds.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong,
+                                            ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_int),
+                                            ctypes.POINTER(ctypes.c_int)]
     L.nphm_debug_ens_skip_log.argtypes = [ctypes.c_void_p, ctypes.c_int]
     L.nphm_debug_ens_bound_scale.argtypes = [ctypes.c_void_p, ctypes.c_double]
     return L

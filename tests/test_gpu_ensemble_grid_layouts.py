@@ -164,18 +164,22 @@ def grid_query(eng, z, res, first, count, period, impl='tc', absorb=True, out=No
 
 class Refs:
     """float64 and fp32 references per x-plane of a res^3 grid, for one head and code: the blended SDF, its value at a quirk
-    row (every s_k = 1: the sum of the normalised weights) and max_k |s_k| (float64)."""
+    row (every s_k = 1: the sum of the normalised weights) and max_k |s_k| (float64).  sub_max: also, per x-plane, the float64
+    max |s_m| of every member over the plane's points in each 32 x 32 (y, z) block of the kernel's 32^3-point sub-boxes."""
 
-    def __init__(self, dec, z):
+    def __init__(self, dec, z, sub_max=False):
         self.P64, self.P32 = E.Params(dec, F64), E.Params(dec, F32)
         self.z = z.reshape(-1).float()
         self.cache = {}
+        self.sub_max = sub_max
+        self.sub_cache = {}
 
     def _compute(self, res, planes):
         ax = _axes(res, self.z.device)
         rr = res * res
         g = torch.cat([torch.arange(p * rr, (p + 1) * rr, device=self.z.device) for p in planes])
         cols = [[] for _ in range(5)]
+        s_abs = []
         with torch.no_grad():
             for c0 in range(0, g.shape[0], 1 << 17):
                 x = _xyz(ax, res, g[c0:c0 + (1 << 17)])
@@ -187,9 +191,28 @@ class Refs:
                     cols[c + 1].append(w.sum(dim=1))
                     if P is self.P64:
                         cols[4].append(s.abs().max(dim=1).values)
+                        if self.sub_max:
+                            s_abs.append(s.abs())
         cols = [torch.cat(c) for c in cols]
         for i, p in enumerate(planes):
             self.cache[(res, p)] = [c[i * rr:(i + 1) * rr] for c in cols]
+        if self.sub_max:
+            n_sub, M = (res + 31) // 32, self.P64.M
+            s = torch.cat(s_abs).reshape(len(planes), res, res, M)
+            s = torch.nn.functional.pad(s, (0, 0, 0, 32 * n_sub - res, 0, 32 * n_sub - res))     # |s| >= 0: pad with 0
+            s = s.reshape(len(planes), n_sub, 32, n_sub, 32, M).amax(dim=(2, 4))
+            for i, p in enumerate(planes):
+                self.sub_cache[(res, p)] = s[i]
+
+    def sub_boxes(self, res, planes):
+        """{sx: n_sub x n_sub x M float64 max |s_m| over the points of ``planes`` in the sub-boxes (sx, sy, sz)}."""
+        todo = [p for p in planes if (res, p) not in self.sub_cache]
+        for i in range(0, len(todo), max(1, (1 << 20) // (res * res))):
+            self._compute(res, todo[i:i + max(1, (1 << 20) // (res * res))])
+        out = {}
+        for p in planes:
+            out[p >> 5] = torch.maximum(out[p >> 5], self.sub_cache[(res, p)]) if (p >> 5) in out else self.sub_cache[(res, p)]
+        return out
 
     def rows(self, res, first, count, planes):
         """(output rows, grid indices, [sdf64, quirk64, sdf32, quirk32, smax64]) over the range's points in ``planes``."""
@@ -303,11 +326,27 @@ def sentinel_out(count, res, dev):
 _state = {}
 
 
-def _head(dev):
-    if 'eng' not in _state:
-        dec = E.make_decoder('prod', dev)
-        z = E.latent('prod', seed=5, device=dev)
-        _state.update(dec=dec, eng=dec.engine(), z=z, refs=Refs(dec, z))
+def make_head(name, dev):
+    """The decoder of a configuration of tests/ensemble_f64_common.py; '<name>:shift': with its anchors moved 0.13 in x, so
+    that a mirrored member's boxes are not those of its unmirrored partner reflected."""
+    base, _, variant = name.partition(':')
+    dec = E.make_decoder(base, dev)
+    if variant == 'shift':
+        with torch.no_grad():
+            dec.anchors = dec.anchors + torch.tensor([0.13, 0.0, 0.0], device=dec.anchors.device)
+    else:
+        assert not variant, name
+    return dec
+
+
+def _head(dev, name='prod', sub_max=False):
+    """(decoder, engine, code, Refs) of one head at a time on the device (latent seed 5 of the configuration)."""
+    if _state.get('name') != name:
+        _state.clear()
+        torch.cuda.empty_cache()
+        dec = make_head(name, dev)
+        z = E.latent(name.partition(':')[0], seed=5, device=dev)
+        _state.update(name=name, dec=dec, eng=dec.engine(), z=z, refs=Refs(dec, z, sub_max))
     return _state['dec'], _state['eng'], _state['z'], _state['refs']
 
 
