@@ -628,6 +628,52 @@ int nphm_band_sparse_mc_emit(int res, int block, int l0, int l1, const void *wor
                              double *verts_dev, long long *tris_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The block-sparse band of S heads in lockstep (n_heads = S, DESIGN §4.21): the nphm_band_sparse_* steps of the whole grid (the slab
+ * [0, blocks)) for S heads at once, as nphm_band_heads_* does for dense storage.  The workspace (>=
+ * nphm_band_sparse_heads_workspace_bytes, NPHM_ERR_CAPACITY when short) holds a record of the heads and each head's block states
+ * and slots and corner values and marks; `pool` describes one head's pool (its sizes are those nphm_band_sparse_pool_sizes gives
+ * for the whole grid), and each of its buffers holds S such pools one after the other.  Every head's state, lists and mesh evolve
+ * exactly as those of a single sparse band of the whole grid driven through the same steps.
+ *   begin, corners, classify, grow   as the sparse steps, for every head; counts_host (4 S long longs, may be NULL) receives head
+ *                                    h's {voxels listed, blocks active, bricks used, bricks needed} at [4h .. 4h+3], read back with
+ *                                    one copy (one synchronisation whatever S is).  When a pool is short, no head takes a brick or
+ *                                    lists anything, NPHM_ERR_CAPACITY is returned and the caller grows every pool and repeats the
+ *                                    same call.  The quirk voxels depend only on res and quirk_period: every head lists the same.
+ *   gather, scatter                  n_pad head-major rows per head, as nphm_band_heads_gather / _scatter
+ *   fill                             writes nothing, as nphm_band_sparse_fill
+ *   block_states                     states_dev: S x blocks^3 bytes
+ * Marching cubes: mc_count writes head h's (n_verts, n_tris) to counts_host[2h .. 2h+1] (one synchronisation); mc_emit (same
+ * workspace, after mc_count) writes the S meshes one after the other, head h at the offsets of heads 0 .. h-1 and with ids local
+ * to the head: head h's part is what nphm_band_sparse_mc_count / _emit give for that head alone.  The marching-cubes workspace
+ * needs nphm_band_sparse_heads_mc_workspace_bytes(res, block, n_heads, pool->slots) bytes.  Needs 1 <= n_heads <= 65535 and what
+ * the sparse steps need (else NPHM_ERR_INVALID; -1 from the byte counts). */
+long long nphm_band_sparse_heads_workspace_bytes(int res, int block, int n_heads);
+int nphm_band_sparse_heads_begin(int res, int block, int n_heads, long long quirk_period, void *workspace_dev, long long workspace_bytes,
+                                 const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_heads_corners(int res, int block, int n_heads, void *workspace_dev, long long workspace_bytes,
+                                   const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_heads_classify(int res, int block, int n_heads, float tau, void *workspace_dev, long long workspace_bytes,
+                                    const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_heads_grow(int res, int block, int n_heads, void *workspace_dev, long long workspace_bytes,
+                                const nphm_band_pool *pool, long long *counts_host, void *stream);
+int nphm_band_sparse_heads_gather(int res, int block, int n_heads, const double grid_min[3], const double grid_max[3], long long n_pad,
+                                  float *xyz_dev, void *workspace_dev, long long workspace_bytes, const nphm_band_pool *pool,
+                                  void *stream);
+int nphm_band_sparse_heads_scatter(int res, int block, int n_heads, long long n_pad, const float *values_dev, void *workspace_dev,
+                                   long long workspace_bytes, const nphm_band_pool *pool, void *stream);
+int nphm_band_sparse_heads_fill(int res, int block, int n_heads, void *workspace_dev, long long workspace_bytes,
+                                const nphm_band_pool *pool, void *stream);
+int nphm_band_sparse_heads_block_states(int res, int block, int n_heads, const void *workspace_dev, long long workspace_bytes,
+                                        const nphm_band_pool *pool, unsigned char *states_dev, void *stream);
+long long nphm_band_sparse_heads_mc_workspace_bytes(int res, int block, int n_heads, long long slots);
+int nphm_band_sparse_heads_mc_count(int res, int block, int n_heads, const void *workspace_dev, long long workspace_bytes,
+                                    const nphm_band_pool *pool, void *mc_workspace_dev, long long mc_workspace_bytes,
+                                    long long *counts_host, void *stream);
+int nphm_band_sparse_heads_mc_emit(int res, int block, int n_heads, const void *workspace_dev, long long workspace_bytes,
+                                   const nphm_band_pool *pool, void *mc_workspace_dev, long long mc_workspace_bytes, double *verts_dev,
+                                   long long *tris_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Training supervision (DESIGN §4.15): the sampling steps of scripts/data_processing/sample_surface.py:32-135 (stage 1) and
  * scripts/data_processing/sample_deformation_field.py:14-35 (stage 2).  Meshes are n_verts x 3 fp64 vertices and n_faces x 3 int32
  * faces, every index in [0, n_verts) - a PRECONDITION, not checked here (the Python layer checks it).  Samples are n x 3 fp64

@@ -53,6 +53,10 @@ EXPORTED_SYMBOLS = (
     'nphm_band_sparse_classify', 'nphm_band_sparse_grow', 'nphm_band_sparse_gather', 'nphm_band_sparse_scatter',
     'nphm_band_sparse_fill', 'nphm_band_sparse_block_states', 'nphm_band_sparse_export', 'nphm_band_sparse_import',
     'nphm_band_sparse_volume', 'nphm_band_sparse_mc_workspace_bytes', 'nphm_band_sparse_mc_count', 'nphm_band_sparse_mc_emit',
+    'nphm_band_sparse_heads_workspace_bytes', 'nphm_band_sparse_heads_begin', 'nphm_band_sparse_heads_corners',
+    'nphm_band_sparse_heads_classify', 'nphm_band_sparse_heads_grow', 'nphm_band_sparse_heads_gather',
+    'nphm_band_sparse_heads_scatter', 'nphm_band_sparse_heads_fill', 'nphm_band_sparse_heads_block_states',
+    'nphm_band_sparse_heads_mc_workspace_bytes', 'nphm_band_sparse_heads_mc_count', 'nphm_band_sparse_heads_mc_emit',
     'nphm_face_cdf_workspace_bytes', 'nphm_face_cdf', 'nphm_sample_faces', 'nphm_vertex_normals_workspace_bytes',
     'nphm_vertex_normals', 'nphm_interpolate_barycentric', 'nphm_transfer_correspondences',
 )
@@ -302,6 +306,21 @@ def lib() -> ctypes.CDLL:
     L.nphm_band_sparse_mc_workspace_bytes.restype = c_longlong
     L.nphm_band_sparse_mc_count.argtypes = slab + mem + [c_void_p, c_longlong, POINTER(c_longlong), POINTER(c_longlong), c_void_p]
     L.nphm_band_sparse_mc_emit.argtypes = slab + mem + [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p]
+    L.nphm_band_sparse_heads_workspace_bytes.argtypes = heads
+    L.nphm_band_sparse_heads_workspace_bytes.restype = c_longlong
+    heads_listing = mem + [c_void_p, c_void_p]           # counts: 4 S long longs
+    L.nphm_band_sparse_heads_begin.argtypes = heads + [c_longlong] + heads_listing
+    L.nphm_band_sparse_heads_corners.argtypes = heads + heads_listing
+    L.nphm_band_sparse_heads_classify.argtypes = heads + [c_float] + heads_listing
+    L.nphm_band_sparse_heads_grow.argtypes = heads + heads_listing
+    L.nphm_band_sparse_heads_gather.argtypes = heads + [POINTER(c_double), POINTER(c_double), c_longlong, c_void_p] + mem + [c_void_p]
+    L.nphm_band_sparse_heads_scatter.argtypes = heads + [c_longlong, c_void_p] + mem + [c_void_p]
+    L.nphm_band_sparse_heads_fill.argtypes = heads + mem + [c_void_p]
+    L.nphm_band_sparse_heads_block_states.argtypes = heads + mem + [c_void_p, c_void_p]
+    L.nphm_band_sparse_heads_mc_workspace_bytes.argtypes = heads + [c_longlong]
+    L.nphm_band_sparse_heads_mc_workspace_bytes.restype = c_longlong
+    L.nphm_band_sparse_heads_mc_count.argtypes = heads + mem + [c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_band_sparse_heads_mc_emit.argtypes = heads + mem + [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p]
     L.nphm_face_cdf_workspace_bytes.argtypes = [c_longlong]
     L.nphm_face_cdf_workspace_bytes.restype = c_longlong
     L.nphm_face_cdf.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, POINTER(c_double), c_void_p, c_longlong, c_void_p]
@@ -1427,3 +1446,186 @@ def sparse_marching_cubes_emit(band: SparseNarrowBand, params, ws, n_verts: int,
             check(lib().nphm_band_sparse_mc_emit(*band._geo, *band._mem(), ws.data_ptr(), ws.numel(), int(vert_id_base), verts.data_ptr(),
                                                  tris.data_ptr(), _stream_ptr(dev)), 'nphm_band_sparse_mc_emit')
     return verts, tris
+
+
+class SparseNarrowBandHeads:
+    """The band of :class:`SparseNarrowBand` on the whole ``res^3`` grid for ``n_heads`` heads in lockstep
+    (``nphm_band_sparse_heads_*``, DESIGN §4.21), with the interface of :class:`NarrowBandHeads`: each listing step is one launch
+    sequence and one count read-back for all heads (:attr:`readbacks` counts the synchronising calls), :meth:`gather` /
+    :meth:`scatter` move ``S x n_pad`` head-major rows, and :meth:`marching_cubes` meshes every head with one count read-back.
+    Each head keeps a frame (block states and slots, corners) and a brick pool; the S pools are of one size, in one allocation per
+    buffer, and grow together: when a step finds a pool short, no head changes, every pool grows (keeping the used bricks) and the
+    step repeats.  :meth:`volumes` returns the band itself, the store every step takes.  Every head's state and mesh are those of a
+    :class:`SparseNarrowBand` of the whole grid driven through the same steps."""
+
+    def __init__(self, res: int, block: int, device, n_heads: int, slots: Optional[int] = None):
+        self.res, self.block, self.n_heads = int(res), int(block), int(n_heads)
+        self.device = torch.device(device)
+        self.blocks_per_axis = -(-(self.res - 1) // max(self.block, 1))
+        self._geo = (self.res, self.block, self.n_heads)
+        self._slab = (self.res, self.block, 0, self.blocks_per_axis)
+        with torch.cuda.device(self.device):
+            self.ws = _workspace(lib().nphm_band_sparse_heads_workspace_bytes(*self._geo), 'nphm_band_sparse_heads_workspace_bytes',
+                                 self.device)
+        self.brick_voxels = (self.block + 1) ** 3
+        self.n_blocks = self.blocks_per_axis ** 3
+        self.active_blocks = [0] * self.n_heads
+        self.slots_used = [0] * self.n_heads
+        self.readbacks = 0                # stream synchronisations of the listing steps and marching cubes so far
+        self.mc_bytes = 0                 # marching-cubes workspace of the last mesh
+        # list entries slot (block+1)^3 + local are u32 within each head's pool
+        self.max_slots = min(self.n_blocks, ((1 << 32) - 1) // self.brick_voxels)
+        self._pool_tensors = None
+        self._set_pool(self.default_slots(self.res, self.block) if slots is None else int(slots))
+
+    @staticmethod
+    def default_slots(res: int, block: int) -> int:
+        """Bricks each head's pool starts with, as :class:`SparseNarrowBand` (a surface crosses about as many blocks per layer as a
+        layer has rows); the pools grow when the band needs more."""
+        nb = -(-(int(res) - 1) // max(int(block), 1))
+        return min(nb ** 3, ((1 << 32) - 1) // (int(block) + 1) ** 3, max(64, 4 * nb * nb))
+
+    @staticmethod
+    def device_bytes_per_head(res: int, block: int, slots: Optional[int] = None) -> int:
+        """Device bytes one head holds at the start: its frame (block states and slots, corner values and marks), its brick pool of
+        ``slots`` bricks (default :meth:`default_slots`) with the list and compaction scratch, and its marching-cubes workspace."""
+        L = lib()
+        res, block = int(res), int(block)
+        slots = SparseNarrowBandHeads.default_slots(res, block) if slots is None else int(slots)
+        frame = L.nphm_band_sparse_heads_workspace_bytes(res, block, 2) - L.nphm_band_sparse_heads_workspace_bytes(res, block, 1)
+        mc = L.nphm_band_sparse_heads_mc_workspace_bytes(res, block, 2, slots) - L.nphm_band_sparse_heads_mc_workspace_bytes(res, block, 1, slots)
+        nb = -(-(res - 1) // max(block, 1))
+        sizes = (c_longlong * 3)()
+        if frame < 0 or mc < 0 or L.nphm_band_sparse_pool_sizes(res, block, 0, nb, slots, sizes) != 0:
+            check(-1, 'nphm_band_sparse_heads_workspace_bytes')
+        pool = slots * (block + 1) ** 3 * 4 + sizes[0] + 4 * max(slots, 1) + 4 * max(sizes[1], 1) + 8 * sizes[2]
+        return int(frame + pool + mc)
+
+    def _set_pool(self, slots: int, keep: int = 0):
+        sizes = (c_longlong * 3)()
+        check(lib().nphm_band_sparse_pool_sizes(*self._slab, int(slots), sizes), 'nphm_band_sparse_pool_sizes')
+        marks_bytes, list_len, n_chunks = sizes[0], sizes[1], sizes[2]
+        S, V, dev = self.n_heads, self.brick_voxels, self.device
+        old = self._pool_tensors
+        if old is not None:                # release the scratch of the old pools before allocating the new ones
+            old = old[:3]
+            self._pool_tensors = None
+        vals = torch.empty(S, slots * V, device=dev, dtype=torch.float32)
+        marks = torch.zeros(S, marks_bytes, device=dev, dtype=torch.uint8)
+        blocks = torch.empty(S, max(slots, 1), device=dev, dtype=torch.int32)
+        if old is not None and keep:       # every head's used bricks, at the same place in its new pool
+            vals[:, :keep * V].copy_(old[0][:, :keep * V])
+            marks[:, :keep * V].copy_(old[1][:, :keep * V])
+            blocks[:, :keep].copy_(old[2][:, :keep])
+        del old
+        lst = torch.empty(S, max(list_len, 1), device=dev, dtype=torch.int32)
+        cnt = torch.empty(S, n_chunks, device=dev, dtype=torch.int32)
+        off = torch.empty(S, n_chunks, device=dev, dtype=torch.int32)
+        self._pool_tensors = (vals, marks, blocks, lst, cnt, off)
+        # the native side steps from one head's pool to the next by these sizes: the rows above
+        self.pool = BandPool(vals.data_ptr() if slots else blocks.data_ptr(), marks.data_ptr(), blocks.data_ptr(), lst.data_ptr(),
+                             cnt.data_ptr(), off.data_ptr(), int(slots), marks_bytes, max(list_len, 1), n_chunks)
+        self.slots = int(slots)
+
+    def device_bytes(self) -> int:
+        """Bytes the band holds on the device: the workspace (record and every head's frame) and the S brick pools."""
+        return self.ws.numel() + sum(t.numel() * t.element_size() for t in self._pool_tensors)
+
+    def _mem(self):
+        return self.ws.data_ptr(), self.ws.numel(), byref(self.pool)
+
+    def _call(self, step, *args):
+        with torch.cuda.device(self.device):
+            check(getattr(lib(), 'nphm_band_sparse_heads_' + step)(*self._geo, *args, _stream_ptr(self.device)),
+                  'nphm_band_sparse_heads_' + step)
+
+    def _call_listing(self, step, *before):
+        fn = getattr(lib(), 'nphm_band_sparse_heads_' + step)
+        S = self.n_heads
+        counts = (c_longlong * (4 * S))()
+        with torch.cuda.device(self.device):
+            while True:
+                rc = fn(*self._geo, *before, *self._mem(), counts, _stream_ptr(self.device))
+                self.readbacks += 1
+                need = max(counts[4 * h + 3] for h in range(S))
+                if rc != NPHM_ERR_CAPACITY or need <= self.slots or need > self.max_slots:
+                    break
+                # no head changed and nothing was listed: grow every pool, keep the used bricks, repeat the same step
+                self._set_pool(min(self.max_slots, max(int(need), 2 * self.slots)), keep=max(counts[4 * h + 2] for h in range(S)))
+            if rc == NPHM_ERR_CAPACITY and need > self.max_slots:
+                raise NativeError('nphm_band_sparse_heads_%s: a head needs %d bricks of %d voxels; list entries are u32, so a pool '
+                                  'holds at most %d' % (step, need, self.brick_voxels, self.max_slots))
+            check(rc, 'nphm_band_sparse_heads_' + step)
+        self.active_blocks = [counts[4 * h + 1] for h in range(S)]
+        self.slots_used = [counts[4 * h + 2] for h in range(S)]
+        return [counts[4 * h] for h in range(S)]
+
+    def _own(self, vols):
+        if vols is not self:
+            raise ValueError('SparseNarrowBandHeads: the volumes of a sparse band are the band itself (volumes())')
+
+    def begin(self, quirk_period: int = 0):
+        """Reset every head; with ``quirk_period > 0`` list the eval-mode quirk voxels (the same for every head)."""
+        return self._call_listing('begin', int(quirk_period))
+
+    def corners(self):
+        return self._call_listing('corners')
+
+    def classify(self, tau: float, vols):
+        self._own(vols)
+        return self._call_listing('classify', float(tau))
+
+    def grow(self, vols):
+        self._own(vols)
+        return self._call_listing('grow')
+
+    def gather(self, n_pad: int, mini, maxi) -> torch.Tensor:
+        """(S, n_pad, 3) float32 coordinates: each head's listed voxels, then padding rows that repeat one of them."""
+        xyz = torch.empty(self.n_heads, int(n_pad), 3, device=self.device, dtype=torch.float32)
+        gmin = (c_double * 3)(*[float(v) for v in mini])
+        gmax = (c_double * 3)(*[float(v) for v in maxi])
+        self._call('gather', gmin, gmax, int(n_pad), _ptr(xyz) if n_pad else None, *self._mem())
+        return xyz
+
+    def scatter(self, values: torch.Tensor, vols):
+        """values (S, n_pad) in the layout of :meth:`gather`: each head's listed rows into its bricks, the padding dropped."""
+        self._own(vols)
+        v = _f32c(values).reshape(self.n_heads, -1)
+        n_pad = v.shape[1]
+        self._call('scatter', n_pad, v.data_ptr() if n_pad else None, *self._mem())
+
+    def fill(self, vols):
+        self._own(vols)
+        self._call('fill', *self._mem())
+
+    def block_states(self) -> torch.Tensor:
+        """(S, blocks, blocks, blocks) bool: which blocks of each head are active."""
+        nb = self.blocks_per_axis
+        out = torch.empty(self.n_heads, nb, nb, nb, device=self.device, dtype=torch.uint8)
+        self._call('block_states', *self._mem(), out.data_ptr())
+        return out != 0
+
+    def volumes(self):
+        return self
+
+    def marching_cubes(self, vols):
+        """Marching cubes on every head's bricks (``nphm_band_sparse_heads_mc_count`` / ``_emit``): ``(verts (V, 3) float64, tris
+        (T, 3) int64, counts)`` as :meth:`NarrowBandHeads.marching_cubes` gives them, head h's part what
+        :func:`sparse_marching_cubes_count` / :func:`sparse_marching_cubes_emit` give for that head alone."""
+        self._own(vols)
+        L = lib()
+        with torch.cuda.device(self.device):
+            ws = _workspace(L.nphm_band_sparse_heads_mc_workspace_bytes(*self._geo, self.slots), 'nphm_band_sparse_heads_mc_workspace_bytes',
+                            self.device)
+            self.mc_bytes = ws.numel()
+            counts = (c_longlong * (2 * self.n_heads))()
+            check(L.nphm_band_sparse_heads_mc_count(*self._geo, *self._mem(), ws.data_ptr(), ws.numel(), counts,
+                                                    _stream_ptr(self.device)), 'nphm_band_sparse_heads_mc_count')
+            self.readbacks += 1
+            pairs = [(counts[2 * h], counts[2 * h + 1]) for h in range(self.n_heads)]
+            verts = torch.empty(sum(c[0] for c in pairs), 3, device=self.device, dtype=torch.float64)
+            tris = torch.empty(sum(c[1] for c in pairs), 3, device=self.device, dtype=torch.int64)
+            if verts.shape[0] or tris.shape[0]:
+                check(L.nphm_band_sparse_heads_mc_emit(*self._geo, *self._mem(), ws.data_ptr(), ws.numel(), verts.data_ptr(),
+                                                       tris.data_ptr(), _stream_ptr(self.device)), 'nphm_band_sparse_heads_mc_emit')
+        return verts, tris, pairs

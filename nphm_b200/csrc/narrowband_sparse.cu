@@ -17,6 +17,7 @@
 #include "simt.cuh"
 #include "mc_tables.h"
 #include <algorithm>
+#include <vector>
 
 namespace nphm {
 namespace sband {
@@ -289,7 +290,7 @@ __device__ __forceinline__ unsigned cta_exclusive_scan(unsigned v, unsigned &tot
     return base + inc - v;
 }
 
-__global__ void __launch_bounds__(kThreads) count_kernel(const unsigned char *__restrict__ bytes, unsigned want4, unsigned *__restrict__ cnt)
+__device__ __forceinline__ void count_body(const unsigned char *__restrict__ bytes, unsigned want4, unsigned *__restrict__ cnt)
 {
     const uint4 m = __ldg(reinterpret_cast<const uint4 *>(bytes + (size_t)blockIdx.x * kChunk) + threadIdx.x);
     uint4 eq;
@@ -298,8 +299,13 @@ __global__ void __launch_bounds__(kThreads) count_kernel(const unsigned char *__
     if (threadIdx.x == 0) cnt[blockIdx.x] = total;
 }
 
-__global__ void __launch_bounds__(kScanThreads) scan_kernel(const unsigned *__restrict__ cnt, unsigned *__restrict__ off, long long n_chunks,
-                                                            unsigned long long *__restrict__ total_out)
+__global__ void __launch_bounds__(kThreads) count_kernel(const unsigned char *__restrict__ bytes, unsigned want4, unsigned *__restrict__ cnt)
+{
+    count_body(bytes, want4, cnt);
+}
+
+__device__ __forceinline__ void scan_body(const unsigned *__restrict__ cnt, unsigned *__restrict__ off, long long n_chunks,
+                                          unsigned long long *__restrict__ total_out)
 {
     const long long per = (n_chunks + kScanThreads - 1) / kScanThreads;
     const long long c0 = threadIdx.x * per, c1 = min(c0 + per, n_chunks);
@@ -314,13 +320,16 @@ __global__ void __launch_bounds__(kScanThreads) scan_kernel(const unsigned *__re
     if (threadIdx.x == 0) *total_out = total;
 }
 
-// list the indices of the bytes == want in ascending order and set them to `set`; nothing is written when *total + *used > cap
-__global__ void __launch_bounds__(kThreads) emit_kernel(unsigned char *__restrict__ bytes, unsigned want4, unsigned set4,
-                                                        const unsigned *__restrict__ cnt, const unsigned *__restrict__ off,
-                                                        unsigned *__restrict__ list, const unsigned long long *__restrict__ total,
-                                                        const unsigned long long *__restrict__ used, unsigned long long cap)
+__global__ void __launch_bounds__(kScanThreads) scan_kernel(const unsigned *__restrict__ cnt, unsigned *__restrict__ off, long long n_chunks,
+                                                            unsigned long long *__restrict__ total_out)
 {
-    if (cnt[blockIdx.x] == 0 || *total + (used ? *used : 0ull) > cap) return;
+    scan_body(cnt, off, n_chunks, total_out);
+}
+
+// chunk blockIdx.x of the compaction: list its bytes == want (from their chunk's offset on) and set them to `set`
+__device__ __forceinline__ void emit_body(unsigned char *__restrict__ bytes, unsigned want4, unsigned set4, const unsigned *__restrict__ off,
+                                          unsigned *__restrict__ list)
+{
     uint4 *p = reinterpret_cast<uint4 *>(bytes + (size_t)blockIdx.x * kChunk) + threadIdx.x;
     uint4 m = *p, eq;
     const unsigned c = match_bytes(m, want4, eq);
@@ -339,8 +348,18 @@ __global__ void __launch_bounds__(kThreads) emit_kernel(unsigned char *__restric
     *p = m;
 }
 
+// list the indices of the bytes == want in ascending order and set them to `set`; nothing is written when *total + *used > cap
+__global__ void __launch_bounds__(kThreads) emit_kernel(unsigned char *__restrict__ bytes, unsigned want4, unsigned set4,
+                                                        const unsigned *__restrict__ cnt, const unsigned *__restrict__ off,
+                                                        unsigned *__restrict__ list, const unsigned long long *__restrict__ total,
+                                                        const unsigned long long *__restrict__ used, unsigned long long cap)
+{
+    if (cnt[blockIdx.x] == 0 || *total + (used ? *used : 0ull) > cap) return;
+    emit_body(bytes, want4, set4, off, list);
+}
+
 // ---------------------------------------------------------------------------------------------- allocation and marking
-__global__ void quirk_states_kernel(const Geo g, long long period, long long k0, long long k1, unsigned char *__restrict__ states)
+__device__ __forceinline__ void quirk_states_body(const Geo g, long long period, long long k0, long long k1, unsigned char *__restrict__ states)
 {
     const long long k = k0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (k >= k1) return;
@@ -355,7 +374,12 @@ __global__ void quirk_states_kernel(const Geo g, long long period, long long k0,
             for (int bz = z0; bz <= z1; ++bz) states[blk(g, bx, by, bz)] = kActivated;
 }
 
-__global__ void quirk_mark_kernel(const Geo g, const Mem m, long long period, long long k0, long long k1)
+__global__ void quirk_states_kernel(const Geo g, long long period, long long k0, long long k1, unsigned char *__restrict__ states)
+{
+    quirk_states_body(g, period, k0, k1, states);
+}
+
+__device__ __forceinline__ void quirk_mark_body(const Geo g, const Mem m, long long period, long long k0, long long k1)
 {
     const long long k = k0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (k >= k1 || m.hdr[H_OVER]) return;
@@ -363,6 +387,11 @@ __global__ void quirk_mark_kernel(const Geo g, const Mem m, long long period, lo
     const long long v = k < n_all / period ? (k + 1) * period - 1 : n_all - 1;
     long long e;
     if (owner(g, m, (int)(v / g.rr), (int)((v / g.res) % g.res), (int)(v % g.res), e) != kNoSlot) m.bmarks[e] = kWanted;
+}
+
+__global__ void quirk_mark_kernel(const Geo g, const Mem m, long long period, long long k0, long long k1)
+{
+    quirk_mark_body(g, m, period, k0, k1);
 }
 
 // after the compaction of the activated blocks into the list: take their slots, or flag that the pool is short
@@ -379,13 +408,18 @@ __global__ void commit_kernel(unsigned long long *hdr, unsigned long long cap)
     hdr[H_OVER] = 0;
 }
 
-__global__ void assign_kernel(const Mem m)
+__device__ __forceinline__ void assign_body(const Mem m)
 {
     const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (m.hdr[H_OVER] || i >= (long long)m.hdr[H_NEW]) return;
     const unsigned b = m.list[i], s = (unsigned)(m.hdr[H_OLD] + i);
     m.slot[b] = s;
     m.sblock[s] = b;
+}
+
+__global__ void assign_kernel(const Mem m)
+{
+    assign_body(m);
 }
 
 __device__ __forceinline__ void box(const Geo &g, long long b, int lo[3], int d[3])
@@ -400,7 +434,7 @@ __device__ __forceinline__ void box(const Geo &g, long long b, int lo[3], int d[
 }
 
 // one warp per new brick: what the older bricks, the corners and the shared planes hold
-__global__ void __launch_bounds__(kThreads) init_kernel(const Geo g, const Mem m)
+__device__ __forceinline__ void init_body(const Geo g, const Mem m)
 {
     const long long s = blockIdx.x * (long long)kWarps + (threadIdx.x >> 5);
     const unsigned long long old = m.hdr[H_OLD];
@@ -417,8 +451,13 @@ __global__ void __launch_bounds__(kThreads) init_kernel(const Geo g, const Mem m
     }
 }
 
+__global__ void __launch_bounds__(kThreads) init_kernel(const Geo g, const Mem m)
+{
+    init_body(g, m);
+}
+
 // one warp per brick of a block being marked: its voxels not evaluated are wanted, by the first marked block that holds them
-__global__ void __launch_bounds__(kThreads) mark_kernel(const Geo g, const Mem m)
+__device__ __forceinline__ void mark_body(const Geo g, const Mem m)
 {
     const long long s = blockIdx.x * (long long)kWarps + (threadIdx.x >> 5);
     if (m.hdr[H_OVER] || s >= (long long)m.hdr[H_USED] || m.states[m.sblock[s]] != kForced) return;
@@ -432,7 +471,12 @@ __global__ void __launch_bounds__(kThreads) mark_kernel(const Geo g, const Mem m
     }
 }
 
-__global__ void promote_kernel(const Mem m)
+__global__ void __launch_bounds__(kThreads) mark_kernel(const Geo g, const Mem m)
+{
+    mark_body(g, m);
+}
+
+__device__ __forceinline__ void promote_body(const Mem m)
 {
     const long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (m.hdr[H_OVER] || s >= (long long)m.hdr[H_USED]) return;
@@ -443,6 +487,11 @@ __global__ void promote_kernel(const Mem m)
     }
 }
 
+__global__ void promote_kernel(const Mem m)
+{
+    promote_body(m);
+}
+
 // ---------------------------------------------------------------------------------------------- the band tests
 __global__ void corners_kernel(long long n, unsigned char *__restrict__ cmarks)
 {
@@ -450,7 +499,7 @@ __global__ void corners_kernel(long long n, unsigned char *__restrict__ cmarks)
     if (c < n && cmarks[c] == kIdle) cmarks[c] = kWanted;
 }
 
-__global__ void classify_kernel(const Geo g, float tau, const float *__restrict__ cvals, unsigned char *__restrict__ states)
+__device__ __forceinline__ void classify_body(const Geo g, float tau, const float *__restrict__ cvals, unsigned char *__restrict__ states)
 {
     const long long b = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (b >= g.n_blocks || states[b] != kInactive) return;
@@ -467,8 +516,13 @@ __global__ void classify_kernel(const Geo g, float tau, const float *__restrict_
     if (near || (n_in != 0 && n_in != 8)) states[b] = kActivated;
 }
 
+__global__ void classify_kernel(const Geo g, float tau, const float *__restrict__ cvals, unsigned char *__restrict__ states)
+{
+    classify_body(g, tau, cvals, states);
+}
+
 // one warp per brick: its face voxels (all evaluated) push growth into the inactive blocks around it
-__global__ void __launch_bounds__(kThreads) grow_bricks_kernel(const Geo g, const Mem m)
+__device__ __forceinline__ void grow_bricks_body(const Geo g, const Mem m)
 {
     const long long s = blockIdx.x * (long long)kWarps + (threadIdx.x >> 5);
     if (s >= (long long)m.hdr[H_USED]) return;
@@ -479,6 +533,11 @@ __global__ void __launch_bounds__(kThreads) grow_bricks_kernel(const Geo g, cons
         if (lx != 0 && lx != d[0] - 1 && ly != 0 && ly != d[1] - 1 && lz != 0 && lz != d[2] - 1) continue;
         push(g, m, lo[0] + lx, lo[1] + ly, lo[2] + lz, m.bvals[s * g.V + ((long long)lx * g.E + ly) * g.E + lz]);
     }
+}
+
+__global__ void __launch_bounds__(kThreads) grow_bricks_kernel(const Geo g, const Mem m)
+{
+    grow_bricks_body(g, m);
 }
 
 // the voxels a neighbour evaluated on a shared plane push growth the same way
@@ -783,7 +842,7 @@ inline McWs mc_carve(void *ws, const Geo &g, long long slots)
 }
 
 // exclusive scan of n u32 in place, total to *total: chunk sums, a one-CTA scan of those, then each chunk rescanned from its offset
-__global__ void __launch_bounds__(kThreads) sum_kernel(const unsigned *__restrict__ v, long long n, unsigned *__restrict__ cnt)
+__device__ __forceinline__ void sum_body(const unsigned *__restrict__ v, long long n, unsigned *__restrict__ cnt)
 {
     const long long i0 = (long long)blockIdx.x * kChunk + threadIdx.x * kPerThread;
     unsigned s = 0, total;
@@ -792,7 +851,12 @@ __global__ void __launch_bounds__(kThreads) sum_kernel(const unsigned *__restric
     if (threadIdx.x == 0) cnt[blockIdx.x] = total;
 }
 
-__global__ void __launch_bounds__(kThreads) rescan_kernel(unsigned *__restrict__ v, long long n, const unsigned *__restrict__ off)
+__global__ void __launch_bounds__(kThreads) sum_kernel(const unsigned *__restrict__ v, long long n, unsigned *__restrict__ cnt)
+{
+    sum_body(v, n, cnt);
+}
+
+__device__ __forceinline__ void rescan_body(unsigned *__restrict__ v, long long n, const unsigned *__restrict__ off)
 {
     const long long i0 = (long long)blockIdx.x * kChunk + threadIdx.x * kPerThread;
     unsigned s = 0, total;
@@ -804,6 +868,11 @@ __global__ void __launch_bounds__(kThreads) rescan_kernel(unsigned *__restrict__
             v[i0 + t] = run;
             run += x;
         }
+}
+
+__global__ void __launch_bounds__(kThreads) rescan_kernel(unsigned *__restrict__ v, long long n, const unsigned *__restrict__ off)
+{
+    rescan_body(v, n, off);
 }
 
 int scan_u32(const McWs &w, unsigned *v, long long n, unsigned long long *total, cudaStream_t stream)
@@ -818,18 +887,28 @@ int scan_u32(const McWs &w, unsigned *v, long long n, unsigned long long *total,
     return NPHM_OK;
 }
 
-__global__ void col_count_kernel(const Geo g, const McWs w)
+__device__ __forceinline__ void col_count_body(const Geo g, const McWs w)
 {
     const long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (p < (long long)w.hdr[0]) atomicAdd(w.colcnt + w.alist[p] / g.nb, 1u);
 }
 
-__global__ void row_count_kernel(const Geo g, const McWs w)
+__global__ void col_count_kernel(const Geo g, const McWs w)
+{
+    col_count_body(g, w);
+}
+
+__device__ __forceinline__ void row_count_body(const Geo g, const McWs w)
 {
     const long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (r >= w.nrows) return;
     const int i = g.X0 + (int)(r / g.C), j = (int)(r % g.C);
     w.rowbase[r] = w.colcnt[(long long)(i / g.B - g.L0) * g.nb + j / g.B];
+}
+
+__global__ void row_count_kernel(const Geo g, const McWs w)
+{
+    row_count_body(g, w);
 }
 
 // case index of cell (i, j, k) of the block at brick slot s whose voxel box starts at lo
@@ -885,7 +964,7 @@ __device__ __forceinline__ bool segment(const Geo &g, const Mem &m, const McWs &
     return true;
 }
 
-__global__ void seg_count_kernel(const Geo g, const Mem m, const McWs w)
+__device__ __forceinline__ void seg_count_body(const Geo g, const Mem m, const McWs w)
 {
     Seg sg;
     if (!segment(g, m, w, blockIdx.x * (long long)blockDim.x + threadIdx.x, sg)) return;
@@ -897,6 +976,11 @@ __global__ void seg_count_kernel(const Geo g, const Mem m, const McWs w)
     }
     w.segv[sg.s] = nv;
     w.segt[sg.s] = nt;
+}
+
+__global__ void seg_count_kernel(const Geo g, const Mem m, const McWs w)
+{
+    seg_count_body(g, m, w);
 }
 
 // one thread per row of the ghost layer: the vertices its cells create, as a running count within the row
@@ -1034,6 +1118,480 @@ int mc_count(const Geo &g, const Mem &m, const McWs &w, long long *n_verts, long
     NPHM_REQUIRE(h[2] < 0xffffffffull && h[3] < 0xffffffffull, "nphm_band_sparse_mc_count: mesh too large for 32-bit ids");
     *n_verts = (long long)h[2];
     *n_tris = (long long)h[3];
+    return NPHM_OK;
+}
+
+
+// ---------------------------------------------------------------------------------------------- S heads of one whole grid
+// The band of S heads in lockstep (DESIGN §4.21): every head runs the steps above on the whole grid (the slab [0, nb): no shared or
+// ghost plane), the head being blockIdx.y of every launch.  Head h's frame (header, block states and slots, corner values and
+// marks) lies h F bytes after head 0's, where F stops before the plane buffers the whole grid never reads; the axes are head 0's.
+// Head h's pool is the h-th of S pools of equal size in the caller's buffers, each of the sizes nphm_band_pool gives, so a list
+// entry slot (B+1)^3 + local stays local to its head and the u32 caps of the single band apply per head.  A step that allocates
+// decides for all heads at once (commit_heads_kernel): when one head's pool is short, no head takes a brick or lists anything, so
+// the caller can grow every pool and repeat the same call.  The heads record (256-byte aligned, before head 0's frame) holds that
+// decision and a copy of each head's header, read back with one copy per listing step.
+struct HeadStrides {
+    long long frame, vals, marks, blocks, list, chunks;     // bytes between two heads' frames and pool buffers
+};
+
+template <class T> __host__ __device__ __forceinline__ T *shift(T *p, long long bytes) { return (T *)((const char *)p + bytes); }
+
+__host__ __device__ __forceinline__ Mem head_mem(const Mem &m0, const HeadStrides &hs, long long h)
+{
+    Mem m = m0;
+    const long long f = h * hs.frame;
+    m.hdr = shift(m0.hdr, f); m.states = shift(m0.states, f); m.slot = shift(m0.slot, f);
+    m.cmarks = shift(m0.cmarks, f); m.cvals = shift(m0.cvals, f);
+    m.bvals = shift(m0.bvals, h * hs.vals); m.bmarks = shift(m0.bmarks, h * hs.marks); m.sblock = shift(m0.sblock, h * hs.blocks);
+    m.list = shift(m0.list, h * hs.list);
+    m.chunk_cnt = shift(m0.chunk_cnt, h * hs.chunks); m.chunk_off = shift(m0.chunk_off, h * hs.chunks);
+    return m;
+}
+
+__host__ __device__ __forceinline__ McWs head_mc(const McWs &w0, long long stride, long long h)
+{
+    McWs w = w0;
+    const long long o = h * stride;
+    w.hdr = shift(w0.hdr, o); w.alist = shift(w0.alist, o); w.colcnt = shift(w0.colcnt, o); w.colstart = shift(w0.colstart, o);
+    w.rowbase = shift(w0.rowbase, o); w.segv = shift(w0.segv, o); w.segt = shift(w0.segt, o); w.gloc = shift(w0.gloc, o);
+    w.growv = shift(w0.growv, o); w.px0 = shift(w0.px0, o); w.cnt = shift(w0.cnt, o); w.off = shift(w0.off, o);
+    return w;
+}
+
+inline long long heads_record_bytes(int S) { return al(64LL * (S + 1)); }     // word 0: pool short; words 8h + 8 ..: head h's header
+inline long long heads_frame_bytes(const Geo &g) { return frame_layout(g).pvals; }
+inline long long heads_bytes(const Geo &g, int S) { return heads_record_bytes(S) + S * heads_frame_bytes(g); }
+inline long long heads_mc_record_bytes(int S) { return al(32LL * S); }         // S (n_verts, n_tris), then their exclusive scans
+
+struct HeadsBand {
+    Geo g;
+    Mem m0;
+    HeadStrides hs;
+    int S;
+    unsigned long long *rec;
+};
+
+__global__ void __launch_bounds__(kThreads) count_heads_kernel(const unsigned char *__restrict__ bytes, long long bstride, unsigned want4,
+                                                               unsigned *__restrict__ cnt, long long cstride)
+{
+    count_body(shift(bytes, blockIdx.y * bstride), want4, shift(cnt, blockIdx.y * cstride));
+}
+
+__global__ void __launch_bounds__(kScanThreads) scan_heads_kernel(const unsigned *__restrict__ cnt, unsigned *__restrict__ off,
+                                                                  long long cstride, long long n_chunks,
+                                                                  unsigned long long *__restrict__ total, long long tstride)
+{
+    scan_body(shift(cnt, blockIdx.y * cstride), shift(off, blockIdx.y * cstride), n_chunks, shift(total, blockIdx.y * tstride));
+}
+
+// `short_flag`: nothing is listed or set when *short_flag (the allocation's decision for all heads)
+__global__ void __launch_bounds__(kThreads) emit_heads_kernel(unsigned char *__restrict__ bytes, long long bstride, unsigned want4,
+                                                              unsigned set4, const unsigned *__restrict__ cnt,
+                                                              const unsigned *__restrict__ off, long long cstride,
+                                                              unsigned *__restrict__ list, long long lstride,
+                                                              const unsigned long long *__restrict__ short_flag)
+{
+    if (shift(cnt, blockIdx.y * cstride)[blockIdx.x] == 0 || (short_flag && *short_flag)) return;
+    emit_body(shift(bytes, blockIdx.y * bstride), want4, set4, shift(off, blockIdx.y * cstride), shift(list, blockIdx.y * lstride));
+}
+
+// after the compaction counts of the activated blocks: every head takes its slots, or - when one head's pool is short - none does
+__global__ void __launch_bounds__(kScanThreads) commit_heads_kernel(const Mem m0, const HeadStrides hs, int S, unsigned long long cap,
+                                                                    unsigned long long *rec)
+{
+    bool over = false;
+    for (int h = threadIdx.x; h < S; h += blockDim.x) {
+        const unsigned long long *hdr = shift(m0.hdr, h * hs.frame);
+        over |= hdr[H_USED] + hdr[H_NEW] > cap;
+    }
+    const int any = __syncthreads_or(over);
+    for (int h = threadIdx.x; h < S; h += blockDim.x) {
+        unsigned long long *hdr = shift(m0.hdr, h * hs.frame);
+        const unsigned long long used = hdr[H_USED], n = hdr[H_NEW];
+        if (any) {
+            hdr[H_NEED] = used + n;
+            hdr[H_OVER] = 1;
+        } else {
+            hdr[H_OLD] = used;
+            hdr[H_USED] = used + n;
+            hdr[H_OVER] = 0;
+        }
+    }
+    if (threadIdx.x == 0) rec[0] = any ? 1ull : 0ull;
+}
+
+__global__ void set_kind_heads_kernel(const Mem m0, const HeadStrides hs, int S, unsigned long long kind)
+{
+    for (int h = blockIdx.x * blockDim.x + threadIdx.x; h < S; h += gridDim.x * blockDim.x) shift(m0.hdr, h * hs.frame)[H_KIND] = kind;
+}
+
+// each head's header words to the record, for the one read-back
+__global__ void record_heads_kernel(const Mem m0, const HeadStrides hs, int S, unsigned long long *rec)
+{
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < 8 * S; t += gridDim.x * blockDim.x) rec[8 + t] = shift(m0.hdr, (t / 8) * hs.frame)[t % 8];
+}
+
+__global__ void quirk_states_heads_kernel(const Geo g, long long period, long long k0, long long k1, unsigned char *__restrict__ states,
+                                          long long fstride)
+{
+    quirk_states_body(g, period, k0, k1, shift(states, blockIdx.y * fstride));
+}
+
+__global__ void quirk_mark_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs, long long period, long long k0, long long k1)
+{
+    quirk_mark_body(g, head_mem(m0, hs, blockIdx.y), period, k0, k1);
+}
+
+__global__ void assign_heads_kernel(const Mem m0, const HeadStrides hs) { assign_body(head_mem(m0, hs, blockIdx.y)); }
+__global__ void __launch_bounds__(kThreads) init_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs) { init_body(g, head_mem(m0, hs, blockIdx.y)); }
+__global__ void __launch_bounds__(kThreads) mark_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs) { mark_body(g, head_mem(m0, hs, blockIdx.y)); }
+__global__ void promote_heads_kernel(const Mem m0, const HeadStrides hs) { promote_body(head_mem(m0, hs, blockIdx.y)); }
+__global__ void __launch_bounds__(kThreads) grow_bricks_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs)
+{
+    grow_bricks_body(g, head_mem(m0, hs, blockIdx.y));
+}
+
+__global__ void corners_heads_kernel(long long n, unsigned char *__restrict__ cmarks, long long fstride)
+{
+    const long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    unsigned char *cm = shift(cmarks, blockIdx.y * fstride);
+    if (c < n && cm[c] == kIdle) cm[c] = kWanted;
+}
+
+__global__ void classify_heads_kernel(const Geo g, float tau, const Mem m0, const HeadStrides hs)
+{
+    const Mem m = head_mem(m0, hs, blockIdx.y);
+    classify_body(g, tau, m.cvals, m.states);
+}
+
+// rows [h n_pad, (h + 1) n_pad) of head h: its listed voxels, then rows that repeat its last listed voxel (voxel 0 when it listed
+// nothing), so that every row is a grid point; the axes are head 0's
+__global__ void gather_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs, long long n_pad, float *__restrict__ xyz)
+{
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= n_pad) return;
+    const Mem m = head_mem(m0, hs, blockIdx.y);
+    const long long cnt = (long long)m.hdr[H_LISTED];
+    int x = 0, y = 0, z = 0;
+    if (cnt > 0) entry_voxel(g, m, m.hdr[H_KIND], m.list[i < cnt ? i : cnt - 1], x, y, z);
+    float *out = xyz + 3 * (blockIdx.y * n_pad + i);
+    out[0] = m0.axes[x];
+    out[1] = m0.axes[g.res + y];
+    out[2] = m0.axes[2 * g.res + z];
+}
+
+__global__ void scatter_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs, long long n_pad, const float *__restrict__ values)
+{
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    const Mem m = head_mem(m0, hs, blockIdx.y);
+    if (i >= n_pad || i >= (long long)m.hdr[H_LISTED]) return;
+    int x, y, z;
+    entry_voxel(g, m, m.hdr[H_KIND], m.list[i], x, y, z);
+    store(g, m, x, y, z, values[blockIdx.y * n_pad + i]);
+}
+
+// ---- compaction, allocation and listing of S heads
+// the bytes == want of every head (at bstride from head 0's) -> the heads' lists (at lstride), totals to each header word `word`
+int compact_heads(const HeadsBand &b, unsigned char *bytes, long long bstride, long long n_padded, unsigned char want, unsigned char set,
+                  int word, unsigned *list, long long lstride, bool allocating, cudaStream_t stream)
+{
+    const long long n_chunks = n_padded / kChunk;
+    const dim3 grid((unsigned)n_chunks, (unsigned)b.S);
+    count_heads_kernel<<<grid, kThreads, 0, stream>>>(bytes, bstride, rep4(want), b.m0.chunk_cnt, b.hs.chunks);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    scan_heads_kernel<<<dim3(1, (unsigned)b.S), kScanThreads, 0, stream>>>(b.m0.chunk_cnt, b.m0.chunk_off, b.hs.chunks, n_chunks,
+                                                                            b.m0.hdr + word, b.hs.frame);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    if (allocating) {
+        commit_heads_kernel<<<1, kScanThreads, 0, stream>>>(b.m0, b.hs, b.S, (unsigned long long)b.m0.slots, b.rec);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    emit_heads_kernel<<<grid, kThreads, 0, stream>>>(bytes, bstride, rep4(want), rep4(set), b.m0.chunk_cnt, b.m0.chunk_off, b.hs.chunks,
+                                                     list, lstride, allocating ? b.rec : nullptr);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int allocate_heads(const HeadsBand &b, cudaStream_t stream)
+{
+    int rc = compact_heads(b, b.m0.states, b.hs.frame, pad(b.g.n_blocks), kActivated, kForced, H_NEW, b.m0.list, b.hs.list, true, stream);
+    if (rc) return rc;
+    const unsigned slot_ctas = (unsigned)std::max(ceil_div(b.m0.slots, kThreads), 1LL);
+    const unsigned warp_ctas = (unsigned)std::max(ceil_div(b.m0.slots, kWarps), 1LL);
+    assign_heads_kernel<<<dim3(slot_ctas, (unsigned)b.S), kThreads, 0, stream>>>(b.m0, b.hs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    init_heads_kernel<<<dim3(warp_ctas, (unsigned)b.S), kThreads, 0, stream>>>(b.g, b.m0, b.hs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+// the wanted marks of every head -> its list; counts_host[4h ..] = {listed, active blocks, bricks used, bricks needed} of head h,
+// read back with one copy; NPHM_ERR_CAPACITY when the pools were short
+int list_and_read_heads(const HeadsBand &b, unsigned char *marks, long long mstride, long long n_padded, unsigned char kind,
+                        long long *counts_host, cudaStream_t stream)
+{
+    set_kind_heads_kernel<<<(unsigned)ceil_div(b.S, kThreads), kThreads, 0, stream>>>(b.m0, b.hs, b.S, kind);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    int rc = compact_heads(b, marks, mstride, n_padded, kWanted, kDone, H_LISTED, b.m0.list, b.hs.list, false, stream);
+    if (rc) return rc;
+    record_heads_kernel<<<(unsigned)ceil_div(8LL * b.S, kThreads), kThreads, 0, stream>>>(b.m0, b.hs, b.S, b.rec);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    std::vector<unsigned long long> h(8 * (size_t)(b.S + 1));
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(h.data(), b.rec, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+    NPHM_CUDA_CHECK(cudaStreamSynchronize(stream));
+    unsigned long long need = 0;
+    for (int i = 0; i < b.S; ++i) {
+        const unsigned long long *r = h.data() + 8 * (i + 1);
+        const unsigned long long ni = r[H_OVER] ? r[H_NEED] : r[H_USED];
+        need = std::max(need, ni);
+        if (counts_host) {
+            counts_host[4 * i] = (long long)r[H_LISTED];
+            counts_host[4 * i + 1] = (long long)r[H_ACTIVE];
+            counts_host[4 * i + 2] = (long long)r[H_USED];
+            counts_host[4 * i + 3] = (long long)ni;
+        }
+    }
+    if (h[0]) {
+        set_error("sparse band of %d heads: each head's brick pool holds %lld bricks, %llu needed", b.S, b.m0.slots, need);
+        return NPHM_ERR_CAPACITY;
+    }
+    return NPHM_OK;
+}
+
+int list_bricks_heads(const HeadsBand &b, long long *counts_host, cudaStream_t stream)
+{
+    long long s[3];
+    pool_sizes(b.g, b.m0.slots, s);
+    return list_and_read_heads(b, b.m0.bmarks, b.hs.marks, s[0], 0, counts_host, stream);
+}
+
+int mark_and_list_heads(const HeadsBand &b, long long *counts_host, cudaStream_t stream)
+{
+    int rc = allocate_heads(b, stream);
+    if (rc) return rc;
+    const unsigned warp_ctas = (unsigned)std::max(ceil_div(b.m0.slots, kWarps), 1LL);
+    mark_heads_kernel<<<dim3(warp_ctas, (unsigned)b.S), kThreads, 0, stream>>>(b.g, b.m0, b.hs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    promote_heads_kernel<<<dim3((unsigned)std::max(ceil_div(b.m0.slots, kThreads), 1LL), (unsigned)b.S), kThreads, 0, stream>>>(b.m0, b.hs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return list_bricks_heads(b, counts_host, stream);
+}
+
+int begin_heads(const HeadsBand &b, long long quirk_period, long long *counts_host, cudaStream_t stream)
+{
+    const Geo &g = b.g;
+    long long s[3];
+    pool_sizes(g, b.m0.slots, s);
+    NPHM_CUDA_CHECK(cudaMemsetAsync(b.rec, 0, heads_record_bytes(b.S), stream));
+    for (int i = 0; i < b.S; ++i) {
+        const Mem m = head_mem(b.m0, b.hs, i);
+        NPHM_CUDA_CHECK(cudaMemsetAsync(m.hdr, 0, 256, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(m.states, 0, pad(g.n_blocks), stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(m.slot, 0xff, g.n_blocks * 4, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(m.cmarks, 0, pad(g.n_corners), stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(m.bmarks, 0, s[0], stream));
+    }
+    if (quirk_period > 0) {
+        // the quirk voxels of the whole grid, the same for every head: their blocks are forced and take bricks now
+        const long long k1 = ceil_div(g.rr * g.res, quirk_period);
+        const dim3 grid((unsigned)ceil_div(k1, kThreads), (unsigned)b.S);
+        quirk_states_heads_kernel<<<grid, kThreads, 0, stream>>>(g, quirk_period, 0, k1, b.m0.states, b.hs.frame);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+        int rc = allocate_heads(b, stream);
+        if (rc) return rc;
+        quirk_mark_heads_kernel<<<grid, kThreads, 0, stream>>>(g, b.m0, b.hs, quirk_period, 0, k1);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    return list_bricks_heads(b, counts_host, stream);
+}
+
+// ---- marching cubes of S heads: the single band's scans per head (blockIdx.y), one read-back of the S counts
+__global__ void __launch_bounds__(kThreads) sum_heads_kernel(const unsigned *__restrict__ v, long long n, unsigned *__restrict__ cnt,
+                                                             long long stride)
+{
+    sum_body(shift(v, blockIdx.y * stride), n, shift(cnt, blockIdx.y * stride));
+}
+
+__global__ void __launch_bounds__(kThreads) rescan_heads_kernel(unsigned *__restrict__ v, long long n, const unsigned *__restrict__ off,
+                                                                long long stride)
+{
+    rescan_body(shift(v, blockIdx.y * stride), n, shift(off, blockIdx.y * stride));
+}
+
+__global__ void col_count_heads_kernel(const Geo g, const McWs w0, long long stride) { col_count_body(g, head_mc(w0, stride, blockIdx.y)); }
+__global__ void row_count_heads_kernel(const Geo g, const McWs w0, long long stride) { row_count_body(g, head_mc(w0, stride, blockIdx.y)); }
+__global__ void seg_count_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs, const McWs w0, long long stride)
+{
+    seg_count_body(g, head_mem(m0, hs, blockIdx.y), head_mc(w0, stride, blockIdx.y));
+}
+
+// S (n_verts, n_tris) from the heads' headers to rec[0 .. 2S), their exclusive scans over the heads to rec[2S .. 4S)
+__global__ void mc_record_heads_kernel(const McWs w0, long long stride, int S, unsigned long long *rec)
+{
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    unsigned long long v = 0, t = 0;
+    for (int h = 0; h < S; ++h) {
+        const unsigned long long *hdr = shift(w0.hdr, h * stride);
+        rec[2 * h] = hdr[2];
+        rec[2 * h + 1] = hdr[3];
+        rec[2 * S + 2 * h] = v;
+        rec[2 * S + 2 * h + 1] = t;
+        v += hdr[2];
+        t += hdr[3];
+    }
+}
+
+// seg_emit_kernel for head blockIdx.y, its vertices and triangles at the offsets of heads 0 .. h-1, ids local to the head.  The
+// single band's kernel keeps its own copy of this body: its restrict-qualified outputs let it read the bricks through the
+// read-only cache, which an inlined body loses.
+__global__ void seg_emit_heads_kernel(const Geo g, const Mem m0, const HeadStrides hs, const McWs w0, long long stride,
+                                      const unsigned long long *__restrict__ rec, int S, double *__restrict__ verts,
+                                      long long *__restrict__ tris)
+{
+    const Mem m = head_mem(m0, hs, blockIdx.y);
+    const McWs w = head_mc(w0, stride, blockIdx.y);
+    Seg sg;
+    if (!segment(g, m, w, blockIdx.x * (long long)blockDim.x + threadIdx.x, sg)) return;
+    verts += 3 * (long long)rec[2 * S + 2 * blockIdx.y];
+    tris += 3 * (long long)rec[2 * S + 2 * blockIdx.y + 1];
+    long long vrun = w.segv[sg.s], trun = w.segt[sg.s];
+    const float *bv = m.bvals + sg.slot * g.V;
+    for (int k = sg.k0; k < sg.k1; ++k) {
+        const unsigned cube = brick_case(g, m, sg.slot, sg.lo, sg.i, sg.j, k);
+        if (cube == 0u || cube == 255u) continue;
+        const unsigned created = c_edge[cube] & own_mask(sg.i, sg.j, k);
+        for (int e = 0; e < 12; ++e) {
+            if (!(created & (1u << e))) continue;
+            const int a = c_edge_a[e], b = c_edge_b[e];
+            const int axis = c_corner[a][0] != c_corner[b][0] ? 0 : (c_corner[a][1] != c_corner[b][1] ? 1 : 2);
+            auto val = [&](int c) {
+                return -(double)bv[((long long)(sg.i + c_corner[c][0] - sg.lo[0]) * g.E + (sg.j + c_corner[c][1] - sg.lo[1])) * g.E +
+                                   (k + c_corner[c][2] - sg.lo[2])];
+            };
+            double pos[3] = {(double)(sg.i + c_corner[a][0]), (double)(sg.j + c_corner[a][1]), (double)(k + c_corner[a][2])};
+            const double qa = pos[axis], qb = qa + (double)(c_corner[b][axis] - c_corner[a][axis]);
+            pos[axis] = mc_interp(val(a), val(b), qa, qb);
+            double *dst = verts + (vrun + __popc(created & c_before[e])) * 3;
+            dst[0] = pos[0]; dst[1] = pos[1]; dst[2] = pos[2];
+        }
+        const int n = c_ntri[cube];
+        for (int q = 0; q < 3 * n; ++q) tris[trun * 3 + q] = vertex_id(g, m, w, sg.i, sg.j, k, cube, vrun, c_tri[cube][q]);
+        vrun += __popc(created);
+        trun += n;
+    }
+}
+
+int scan_u32_heads(const McWs &w0, long long stride, int S, unsigned *v, long long n, unsigned long long *total, cudaStream_t stream)
+{
+    const long long chunks = std::max(ceil_div(n, kChunk), 1LL);
+    sum_heads_kernel<<<dim3((unsigned)chunks, (unsigned)S), kThreads, 0, stream>>>(v, n, w0.cnt, stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    scan_heads_kernel<<<dim3(1, (unsigned)S), kScanThreads, 0, stream>>>(w0.cnt, w0.off, stride, chunks, total, stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    rescan_heads_kernel<<<dim3((unsigned)chunks, (unsigned)S), kThreads, 0, stream>>>(v, n, w0.off, stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+int mc_count_heads(const HeadsBand &b, const McWs &w0, long long stride, unsigned long long *mrec, long long *counts_host,
+                   cudaStream_t stream)
+{
+    const Geo &g = b.g;
+    const int S = b.S;
+    int rc = load_mc_tables();
+    if (rc) return rc;
+    for (int i = 0; i < S; ++i) {
+        const McWs w = head_mc(w0, stride, i);
+        NPHM_CUDA_CHECK(cudaMemsetAsync(w.hdr, 0, 256, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(w.colcnt, 0, w.ncol * 4, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(w.segv, 0, w.nseg * 4, stream));
+        NPHM_CUDA_CHECK(cudaMemsetAsync(w.segt, 0, w.nseg * 4, stream));
+    }
+    // the active blocks of each head in block order (states are only read: kMarked stays kMarked); totals to each w.hdr[0]
+    const long long n_chunks = pad(g.n_blocks) / kChunk;
+    const dim3 grid((unsigned)n_chunks, (unsigned)S);
+    count_heads_kernel<<<grid, kThreads, 0, stream>>>(b.m0.states, b.hs.frame, rep4(kMarked), b.m0.chunk_cnt, b.hs.chunks);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    scan_heads_kernel<<<dim3(1, (unsigned)S), kScanThreads, 0, stream>>>(b.m0.chunk_cnt, b.m0.chunk_off, b.hs.chunks, n_chunks, w0.hdr,
+                                                                          stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    emit_heads_kernel<<<grid, kThreads, 0, stream>>>(b.m0.states, b.hs.frame, rep4(kMarked), rep4(kMarked), b.m0.chunk_cnt,
+                                                     b.m0.chunk_off, b.hs.chunks, w0.alist, stride, nullptr);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    col_count_heads_kernel<<<dim3((unsigned)std::max(ceil_div(b.m0.slots, kThreads), 1LL), (unsigned)S), kThreads, 0, stream>>>(g, w0, stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    for (int i = 0; i < S; ++i) {
+        const McWs w = head_mc(w0, stride, i);
+        NPHM_CUDA_CHECK(cudaMemcpyAsync(w.colstart, w.colcnt, w.ncol * 4, cudaMemcpyDeviceToDevice, stream));
+    }
+    if ((rc = scan_u32_heads(w0, stride, S, w0.colstart, w0.ncol, w0.hdr + 5, stream))) return rc;
+    row_count_heads_kernel<<<dim3((unsigned)ceil_div(w0.nrows, kThreads), (unsigned)S), kThreads, 0, stream>>>(g, w0, stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    if ((rc = scan_u32_heads(w0, stride, S, w0.rowbase, w0.nrows, w0.hdr + 1, stream))) return rc;
+    seg_count_heads_kernel<<<dim3((unsigned)ceil_div(w0.nseg, kThreads), (unsigned)S), kThreads, 0, stream>>>(g, b.m0, b.hs, w0, stride);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    if ((rc = scan_u32_heads(w0, stride, S, w0.segv, w0.nseg, w0.hdr + 2, stream)) ||
+        (rc = scan_u32_heads(w0, stride, S, w0.segt, w0.nseg, w0.hdr + 3, stream)))
+        return rc;
+    mc_record_heads_kernel<<<1, 1, 0, stream>>>(w0, stride, S, mrec);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    std::vector<unsigned long long> h(2 * (size_t)S);
+    NPHM_CUDA_CHECK(cudaMemcpyAsync(h.data(), mrec, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+    NPHM_CUDA_CHECK(cudaStreamSynchronize(stream));
+    for (int i = 0; i < S; ++i) {
+        NPHM_REQUIRE(h[2 * i] < 0xffffffffull && h[2 * i + 1] < 0xffffffffull,
+                     "nphm_band_sparse_heads_mc_count: the mesh of head %d is too large for 32-bit ids", i);
+        counts_host[2 * i] = (long long)h[2 * i];
+        counts_host[2 * i + 1] = (long long)h[2 * i + 1];
+    }
+    return NPHM_OK;
+}
+
+int check_heads(int res, int block, int S, const char *who)
+{
+    int rc = check_args(res, block, 0, std::max((int)ceil_div(res - 1, std::max(block, 1)), 1), who);
+    if (rc) return rc;
+    NPHM_REQUIRE(S >= 1 && S <= 65535, "%s: %d heads outside [1, 65535]", who, S);
+    return NPHM_OK;
+}
+
+// the S heads' band over the caller's workspace and pools (NPHM_ERR_CAPACITY when short, as check_mem)
+int carve_heads(int res, int block, int S, const void *ws, long long ws_bytes, const nphm_band_pool *p, HeadsBand &b, const char *who)
+{
+    int rc = check_heads(res, block, S, who);
+    if (rc) return rc;
+    b.g = make_geo(res, block, 0, (int)ceil_div(res - 1, block));
+    b.S = S;
+    NPHM_REQUIRE(ws && p, "%s: NULL workspace or pool", who);
+    const long long need = heads_bytes(b.g, S);
+    if (ws_bytes < need) {
+        set_error("%s: sparse band workspace too small: %lld bytes for %d heads of res %d, block %d, %lld needed", who, ws_bytes, S, res,
+                  block, need);
+        return NPHM_ERR_CAPACITY;
+    }
+    NPHM_REQUIRE(p->slots >= 0 && p->slots * b.g.V < (1LL << 32), "%s: pools of %lld bricks of %lld voxels: brick indices are u32", who,
+                 p->slots, b.g.V);
+    NPHM_REQUIRE(p->vals && p->marks && p->blocks && p->list && p->chunk_cnt && p->chunk_off, "%s: NULL pool buffer", who);
+    long long s[3];
+    pool_sizes(b.g, p->slots, s);
+    if (p->marks_bytes < s[0] || p->list_len < s[1] || p->n_chunks < s[2]) {
+        set_error("%s: pool buffers too small for %lld bricks: %lld mark bytes, %lld list entries, %lld chunks needed", who, p->slots,
+                  s[0], s[1], s[2]);
+        return NPHM_ERR_CAPACITY;
+    }
+    char *base = static_cast<char *>(const_cast<void *>(ws));
+    b.rec = reinterpret_cast<unsigned long long *>(base);
+    b.m0 = carve(base + heads_record_bytes(S), b.g, p);
+    b.m0.pvals = nullptr;                        // the whole grid has no shared or ghost plane: never read
+    b.m0.pdone = nullptr;
+    b.m0.ghostv = nullptr;
+    b.hs.frame = heads_frame_bytes(b.g);
+    b.hs.vals = p->slots * b.g.V * 4;
+    b.hs.marks = p->marks_bytes;
+    b.hs.blocks = p->slots * 4;
+    b.hs.list = p->list_len * 4;
+    b.hs.chunks = p->n_chunks * 4;
     return NPHM_OK;
 }
 
@@ -1235,6 +1793,147 @@ extern "C" int nphm_band_sparse_mc_emit(int res, int block, int l0, int l1, cons
     NPHM_REQUIRE(verts_dev && tris_dev, "nphm_band_sparse_mc_emit: NULL output");
     sband::seg_emit_kernel<<<(unsigned)ceil_div(w.nseg, sband::kThreads), sband::kThreads, 0, stream>>>(g, m, w, vert_id_base, verts_dev,
                                                                                                       tris_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- entry points: S heads
+#define HEADS_PROLOGUE(who)                                                                                         \
+    sband::HeadsBand b;                                                                                             \
+    int rc = sband::carve_heads(res, block, n_heads, ws, ws_bytes, pool, b, who);                                   \
+    if (rc) return rc;                                                                                              \
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+
+extern "C" long long nphm_band_sparse_heads_workspace_bytes(int res, int block, int n_heads)
+{
+    if (sband::check_heads(res, block, n_heads, "nphm_band_sparse_heads_workspace_bytes")) return -1;
+    return sband::heads_bytes(sband::make_geo(res, block, 0, (int)ceil_div(res - 1, block)), n_heads);
+}
+
+extern "C" int nphm_band_sparse_heads_begin(int res, int block, int n_heads, long long quirk_period, void *ws, long long ws_bytes,
+                                            const nphm_band_pool *pool, long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_begin")
+    NPHM_REQUIRE(quirk_period >= 0, "nphm_band_sparse_heads_begin: negative quirk period %lld", quirk_period);
+    return sband::begin_heads(b, quirk_period, counts_host, stream);
+}
+
+extern "C" int nphm_band_sparse_heads_corners(int res, int block, int n_heads, void *ws, long long ws_bytes, const nphm_band_pool *pool,
+                                              long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_corners")
+    const long long nc = b.g.n_corners;
+    sband::corners_heads_kernel<<<dim3((unsigned)ceil_div(nc, sband::kThreads), (unsigned)n_heads), sband::kThreads, 0, stream>>>(
+        nc, b.m0.cmarks, b.hs.frame);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return sband::list_and_read_heads(b, b.m0.cmarks, b.hs.frame, sband::pad(nc), 1, counts_host, stream);
+}
+
+extern "C" int nphm_band_sparse_heads_classify(int res, int block, int n_heads, float tau, void *ws, long long ws_bytes,
+                                               const nphm_band_pool *pool, long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_classify")
+    NPHM_REQUIRE(tau >= 0.f, "nphm_band_sparse_heads_classify: need tau >= 0 (got %g)", (double)tau);
+    sband::classify_heads_kernel<<<dim3((unsigned)ceil_div(b.g.n_blocks, sband::kThreads), (unsigned)n_heads), sband::kThreads, 0,
+                                   stream>>>(b.g, tau, b.m0, b.hs);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return sband::mark_and_list_heads(b, counts_host, stream);
+}
+
+extern "C" int nphm_band_sparse_heads_grow(int res, int block, int n_heads, void *ws, long long ws_bytes, const nphm_band_pool *pool,
+                                           long long *counts_host, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_grow")
+    if (b.m0.slots > 0) {
+        sband::grow_bricks_heads_kernel<<<dim3((unsigned)ceil_div(b.m0.slots, sband::kWarps), (unsigned)n_heads), sband::kThreads, 0,
+                                          stream>>>(b.g, b.m0, b.hs);
+        NPHM_CUDA_CHECK(cudaGetLastError());
+    }
+    return sband::mark_and_list_heads(b, counts_host, stream);
+}
+
+extern "C" int nphm_band_sparse_heads_gather(int res, int block, int n_heads, const double grid_min[3], const double grid_max[3],
+                                             long long n_pad, float *xyz_dev, void *ws, long long ws_bytes, const nphm_band_pool *pool,
+                                             void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_gather")
+    NPHM_REQUIRE(grid_min && grid_max && n_pad >= 0 && (n_pad == 0 || xyz_dev), "nphm_band_sparse_heads_gather: bad arguments");
+    if (n_pad == 0) return NPHM_OK;
+    if ((rc = launch_grid_axes(grid_min, grid_max, b.g.res, b.m0.axes, stream))) return rc;
+    sband::gather_heads_kernel<<<dim3((unsigned)ceil_div(n_pad, sband::kThreads), (unsigned)n_heads), sband::kThreads, 0, stream>>>(
+        b.g, b.m0, b.hs, n_pad, xyz_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+extern "C" int nphm_band_sparse_heads_scatter(int res, int block, int n_heads, long long n_pad, const float *values_dev, void *ws,
+                                              long long ws_bytes, const nphm_band_pool *pool, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_scatter")
+    NPHM_REQUIRE(n_pad >= 0 && (n_pad == 0 || values_dev), "nphm_band_sparse_heads_scatter: bad arguments");
+    if (n_pad == 0) return NPHM_OK;
+    sband::scatter_heads_kernel<<<dim3((unsigned)ceil_div(n_pad, sband::kThreads), (unsigned)n_heads), sband::kThreads, 0, stream>>>(
+        b.g, b.m0, b.hs, n_pad, values_dev);
+    NPHM_CUDA_CHECK(cudaGetLastError());
+    return NPHM_OK;
+}
+
+extern "C" int nphm_band_sparse_heads_fill(int res, int block, int n_heads, void *ws, long long ws_bytes, const nphm_band_pool *pool,
+                                           void *stream_)
+{
+    (void)stream_;            // a voxel not evaluated reads as its fill value wherever it is read (lookup): nothing to write
+    sband::HeadsBand b;
+    return sband::carve_heads(res, block, n_heads, ws, ws_bytes, pool, b, "nphm_band_sparse_heads_fill");
+}
+
+extern "C" int nphm_band_sparse_heads_block_states(int res, int block, int n_heads, const void *ws, long long ws_bytes,
+                                                   const nphm_band_pool *pool, unsigned char *states_dev, void *stream_)
+{
+    HEADS_PROLOGUE("nphm_band_sparse_heads_block_states")
+    NPHM_REQUIRE(states_dev, "nphm_band_sparse_heads_block_states: NULL output");
+    for (int i = 0; i < n_heads; ++i)
+        NPHM_CUDA_CHECK(cudaMemcpyAsync(states_dev + i * b.g.n_blocks, sband::head_mem(b.m0, b.hs, i).states, b.g.n_blocks,
+                                        cudaMemcpyDeviceToDevice, stream));
+    return NPHM_OK;
+}
+
+extern "C" long long nphm_band_sparse_heads_mc_workspace_bytes(int res, int block, int n_heads, long long slots)
+{
+    if (sband::check_heads(res, block, n_heads, "nphm_band_sparse_heads_mc_workspace_bytes") || slots < 0) return -1;
+    const sband::Geo g = sband::make_geo(res, block, 0, (int)ceil_div(res - 1, block));
+    return sband::heads_mc_record_bytes(n_heads) + n_heads * sband::mc_carve(nullptr, g, slots).bytes;
+}
+
+#define HEADS_MC_PROLOGUE(who)                                                                                      \
+    HEADS_PROLOGUE(who)                                                                                             \
+    NPHM_REQUIRE(mc_ws, "%s: NULL marching-cubes workspace", who);                                                  \
+    char *mc_base = static_cast<char *>(mc_ws);                                                                     \
+    const long long mc_stride = sband::mc_carve(nullptr, b.g, b.m0.slots).bytes;                                    \
+    const sband::McWs w0 = sband::mc_carve(mc_base + sband::heads_mc_record_bytes(n_heads), b.g, b.m0.slots);       \
+    unsigned long long *mrec = reinterpret_cast<unsigned long long *>(mc_base);                                     \
+    if (mc_ws_bytes < sband::heads_mc_record_bytes(n_heads) + n_heads * mc_stride) {                                \
+        set_error("%s: marching-cubes workspace too small: %lld bytes, %lld needed", who, mc_ws_bytes,              \
+                  sband::heads_mc_record_bytes(n_heads) + n_heads * mc_stride);                                      \
+        return NPHM_ERR_CAPACITY;                                                                                   \
+    }
+
+extern "C" int nphm_band_sparse_heads_mc_count(int res, int block, int n_heads, const void *ws, long long ws_bytes,
+                                               const nphm_band_pool *pool, void *mc_ws, long long mc_ws_bytes, long long *counts_host,
+                                               void *stream_)
+{
+    HEADS_MC_PROLOGUE("nphm_band_sparse_heads_mc_count")
+    NPHM_REQUIRE(counts_host, "nphm_band_sparse_heads_mc_count: NULL counts");
+    return sband::mc_count_heads(b, w0, mc_stride, mrec, counts_host, stream);
+}
+
+extern "C" int nphm_band_sparse_heads_mc_emit(int res, int block, int n_heads, const void *ws, long long ws_bytes,
+                                              const nphm_band_pool *pool, void *mc_ws, long long mc_ws_bytes, double *verts_dev,
+                                              long long *tris_dev, void *stream_)
+{
+    HEADS_MC_PROLOGUE("nphm_band_sparse_heads_mc_emit")
+    NPHM_REQUIRE(verts_dev && tris_dev, "nphm_band_sparse_heads_mc_emit: NULL output");
+    sband::seg_emit_heads_kernel<<<dim3((unsigned)ceil_div(w0.nseg, sband::kThreads), (unsigned)n_heads), sband::kThreads, 0, stream>>>(
+        b.g, b.m0, b.hs, w0, mc_stride, mrec, n_heads, verts_dev, tris_dev);
     NPHM_CUDA_CHECK(cudaGetLastError());
     return NPHM_OK;
 }

@@ -510,13 +510,19 @@ def extract_meshes_narrowband(decoder, encodings, mini, maxi, resolution, nbatch
     plus 16 bytes of query rows per voxel, and at most ``max_heads``; chunking changes no mesh.
     Returns the list of S meshes, and with ``return_stats`` also the list of S stats dicts of :func:`extract_mesh_narrowband`, each
     with ``padded_rows``, the rows evaluated on the head's behalf beyond its voxels (0 when nothing is padded).  Decoders or
-    devices without a native band query, and ``sparse=True`` (not batched: the sparse band runs once per head), extract head by
-    head with :func:`extract_mesh_narrowband`."""
+    devices without a native band query extract head by head with :func:`extract_mesh_narrowband`.
+
+    ``sparse=True`` runs the heads in the block-sparse band of S heads (:class:`_native.SparseNarrowBandHeads`, DESIGN §4.21):
+    each head's mesh and band stats are those of ``extract_mesh_narrowband(..., sparse=True)``, and ``device_bytes`` gives the
+    memory of the chunk that ran the head (``'band'``, ``'mc'``, and its number of ``'heads'``).  Chunks are planned at
+    :meth:`_native.SparseNarrowBandHeads.device_bytes_per_head` plus 16 bytes of query rows per voxel of that head's starting pool;
+    a band that outgrows those pools (a field whose band covers much of the grid) may need a smaller ``max_heads``, and a chunk
+    whose pools cannot grow raises."""
     codes = _as_codes(encodings)
     S, res = codes.shape[0], int(resolution)
     device = next(decoder.parameters()).device
     fns = _heads_evaluators(decoder, codes[:1], device)
-    if fns is None or sparse:
+    if fns is None:
         meshes, stats = [], []
         for h in range(S):
             m, st = extract_mesh_narrowband(decoder, codes[h:h + 1], mini, maxi, res, nbatch_points=nbatch_points, block=block,
@@ -526,13 +532,30 @@ def extract_meshes_narrowband(decoder, encodings, mini, maxi, resolution, nbatch
         return (meshes, stats) if return_stats else meshes
     quirk_period = 0 if (decoder.training or fns[1] is None) else int(nbatch_points)
     tau = default_margin(mini, maxi, res, block) if margin is None else float(margin)
-    per_head = _native.NarrowBandHeads.device_bytes_per_head(res, block) + 16 * res ** 3
+    meshes, stats = _heads_meshes(lambda h0, h1: _heads_evaluators(decoder, codes[h0:h1], device), S, mini, maxi, res, block, tau,
+                                  quirk_period, device, max_heads, sparse)
+    return (meshes, stats) if return_stats else meshes
+
+
+def _heads_chunk_bytes(res: int, block: int, sparse: bool) -> int:
+    """Device bytes one head of a chunk is planned at: its band and marching-cubes scratch plus 16 bytes of query rows per voxel it
+    may evaluate (the whole grid for dense storage, the voxels of its starting brick pool for sparse storage)."""
+    if not sparse:
+        return _native.NarrowBandHeads.device_bytes_per_head(res, block) + 16 * res ** 3
+    slots = _native.SparseNarrowBandHeads.default_slots(res, block)
+    return _native.SparseNarrowBandHeads.device_bytes_per_head(res, block, slots) + 16 * slots * block ** 3
+
+
+def _heads_meshes(evaluators, S, mini, maxi, res, block, tau, quirk_period, device, max_heads, sparse):
+    """The S meshes and stats of the head-batched band, in chunks of as many heads as half the free device memory holds at
+    :func:`_heads_chunk_bytes` (at most ``max_heads``); ``evaluators(h0, h1)`` gives (evaluate, evaluate_quirk) of heads
+    [h0, h1)."""
     budget = torch.cuda.mem_get_info(device)[0] // 2
     meshes, stats = [], []
     with torch.no_grad(), torch.cuda.device(device):
-        for h0, h1 in plan_head_chunks(S, per_head, budget, max_heads):
-            ev, evq = _heads_evaluators(decoder, codes[h0:h1], device)
-            bands = _native.NarrowBandHeads(res, block, device, h1 - h0)
+        for h0, h1 in plan_head_chunks(S, _heads_chunk_bytes(res, block, sparse), budget, max_heads):
+            ev, evq = evaluators(h0, h1)
+            bands = (_native.SparseNarrowBandHeads if sparse else _native.NarrowBandHeads)(res, block, device, h1 - h0)
             vols, st = narrowband_heads_volumes(bands, ev, mini, maxi, tau, quirk_period, evq)
             verts, tris, counts = bands.marching_cubes(vols)
             del vols
@@ -541,13 +564,17 @@ def extract_meshes_narrowband(decoder, encodings, mini, maxi, resolution, nbatch
             stats += [{'blocks_active': s['blocks_active'], 'blocks_total': nb ** 3, 'voxels_evaluated': s['voxels_evaluated'],
                        'voxels_total': res ** 3, 'growth_rounds': s['growth_rounds'], 'margin': tau, 'padded_rows': s['padded_rows']}
                       for s in st]
+            if sparse:
+                used = {'band': bands.device_bytes(), 'mc': bands.mc_bytes, 'heads': h1 - h0}
+                for s in stats[h0 - h1:]:
+                    s['device_bytes'] = dict(used)
             del bands
-    return (meshes, stats) if return_stats else meshes
+    return meshes, stats
 
 
 # ------------------------------------------------------------------------------------------ posed meshes
 def extract_posed_meshes_narrowband(decoder_shape, decoder_expr, lat_rep_shape, lat_reps_expr, mini, maxi, resolution,
-                                    nbatch_points=100000, block=4, margin=None, return_stats=False, max_heads=None):
+                                    nbatch_points=100000, block=4, margin=None, return_stats=False, max_heads=None, sparse=False):
     """The posed meshes ``mesh_from_logits(get_logits_posed(decoder_shape, decoder_expr, lat_rep_shape, lat_reps_expr, grid,
     nbatch_points)[s], mini, maxi, resolution)`` of the S expression codes (``(S, E)``, ``(S, 1, E)`` or ``(E,)``), bit for bit
     (vertex ids, float64 positions, triangles), from the head-batched narrow band of :func:`extract_meshes_narrowband` with the
@@ -559,7 +586,8 @@ def extract_posed_meshes_narrowband(decoder_shape, decoder_expr, lat_rep_shape, 
     gradient is ``grad sdf(xc) (I + dF_ex/dx)^-1`` at the root, so a deformation that compresses space raises it above the
     identity SDF's, and ``margin`` (SDF units) is the override for such fields.  Decoders or devices without the native posed
     query take the dense ``get_logits_posed`` and ``mesh_from_logits``.  ``return_stats``: also the S stats dicts of
-    :func:`extract_meshes_narrowband`."""
+    :func:`extract_meshes_narrowband`.  ``sparse=True``: the expressions are the heads of the block-sparse band of S heads (DESIGN
+    §4.21), whose memory follows the band instead of the grid, as in :func:`extract_meshes_narrowband`; the meshes are the same."""
     from ..models.EnsembledDeepSDF import FastEnsembleDeepSDFMirrored
     from ..models.reconstruction import _expression_codes, get_logits_posed, posed_evaluator
     codes, _ = _expression_codes(lat_reps_expr)
@@ -577,21 +605,9 @@ def extract_posed_meshes_narrowband(decoder_shape, decoder_expr, lat_rep_shape, 
     quirk = not decoder_shape.training and isinstance(decoder_shape, FastEnsembleDeepSDFMirrored)
     quirk_period = int(nbatch_points) if quirk else 0
     tau = default_margin(mini, maxi, res, block) if margin is None else float(margin)
-    per_head = _native.NarrowBandHeads.device_bytes_per_head(res, block) + 16 * res ** 3
-    budget = torch.cuda.mem_get_info(device)[0] // 2
-    meshes, stats = [], []
-    with torch.no_grad(), torch.cuda.device(device):
-        for h0, h1 in plan_head_chunks(S, per_head, budget, max_heads):
-            fn = posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes[h0:h1])
-            bands = _native.NarrowBandHeads(res, block, device, h1 - h0)
-            vols, st = narrowband_heads_volumes(bands, lambda pts: fn(pts)[0], mini, maxi, tau, quirk_period,
-                                                (lambda pts: fn(pts, quirk=True)[0]) if quirk else None)
-            verts, tris, counts = bands.marching_cubes(vols)
-            del vols
-            meshes += _device_meshes(verts, tris, counts, mini, maxi, res)
-            nb = bands.blocks_per_axis
-            stats += [{'blocks_active': s['blocks_active'], 'blocks_total': nb ** 3, 'voxels_evaluated': s['voxels_evaluated'],
-                       'voxels_total': res ** 3, 'growth_rounds': s['growth_rounds'], 'margin': tau, 'padded_rows': s['padded_rows']}
-                      for s in st]
-            del bands
+
+    def evaluators(h0, h1):
+        fn = posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes[h0:h1])
+        return (lambda pts: fn(pts)[0]), ((lambda pts: fn(pts, quirk=True)[0]) if quirk else None)
+    meshes, stats = _heads_meshes(evaluators, S, mini, maxi, res, block, tau, quirk_period, device, max_heads, sparse)
     return (meshes, stats) if return_stats else meshes
