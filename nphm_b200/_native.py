@@ -586,9 +586,10 @@ class MlpEngine(_Versioned):
         check(lib().nphm_mlp_create(byref(cfg), byref(self._h)), 'nphm_mlp_create')
         self.out_dim = module.out_dim_net
         # which kernel family AUTO picks (mirrors tc_mlp_supported in csrc/mlp_chain.cu): nphm_mlp_query sends the
-        # forward-deformation backbone to the tensor cores; every other shape runs layer by layer on the generic wgmma linear layer
-        # (csrc/tc_linear.cu, any width - e.g. the NPM baseline 515 -> 1024 x 8); the fp32 FFMA kernel is kept for impl='simt'
-        self.fused_shape = (hidden == 512 and self.n_lin == 7 and module.lat_dim == 232 and module.out_dim_net == 3)
+        # forward-deformation backbone (condition 232 / 200 / 264: modes compress / expr_only / glob_only) to the tensor cores;
+        # every other shape runs layer by layer on the generic wgmma linear layer (csrc/tc_linear.cu, any width - e.g. the NPM
+        # baseline 515 -> 1024 x 8); the fp32 FFMA kernel is kept for impl='simt'
+        self.fused_shape = (hidden == 512 and self.n_lin == 7 and module.lat_dim in (232, 200, 264) and module.out_dim_net == 3)
         self.simt_ok = hidden <= 880
         self.lat_dim = module.lat_dim
         self.layer_shapes = [tuple(getattr(module, 'lin%d' % i).weight.shape) for i in range(self.n_lin)]

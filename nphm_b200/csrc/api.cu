@@ -375,7 +375,7 @@ extern "C" int nphm_mlp_query(nphm_mlp *h, const float *xyz_dev, const float *co
     NPHM_REQUIRE(impl == NPHM_IMPL_AUTO || impl == NPHM_IMPL_SIMT || impl == NPHM_IMPL_TC, "nphm_mlp_query: unknown impl %d", impl);
     const bool tc_ok = tc_mlp_supported(h);
     if (impl == NPHM_IMPL_TC && !tc_ok) {
-        set_error("tensor-core MLP path supports only the deformation backbone (hidden 512, 6 layers, condition 232, 3 outputs)");
+        set_error("tensor-core MLP path supports only the deformation backbone (hidden 512, 6 layers, condition 232 / 200 / 264, 3 outputs)");
         return NPHM_ERR_UNSUPPORTED;
     }
     const bool use_tc = impl == NPHM_IMPL_TC || (impl == NPHM_IMPL_AUTO && tc_ok);

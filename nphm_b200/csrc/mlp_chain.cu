@@ -449,12 +449,15 @@ static int chain_ready(nphm_mlp *h, const char *who)
 }
 
 namespace nphm {
-// the forward-deformation backbone (DeepSDF MLP, hidden 512, 6 hidden layers, condition 232, 3 outputs: the `compress`
-// DeformationNetwork of scripts/configs/nphm_def.yaml) - the shape NPHM_IMPL_AUTO sends to the tensor cores
+// the forward-deformation backbone (DeepSDF MLP, hidden 512, 6 hidden layers, 3 outputs) with the condition of a
+// DeformationNetwork mode whose condition is constant per query: 232 (`compress`, scripts/configs/nphm_def.yaml), 200
+// (`expr_only`) or 264 (`glob_only`) - the shapes NPHM_IMPL_AUTO sends to the tensor cores (the Broyden search's evaluations
+// included, which the FFMA kernel would otherwise run at a sixteenth of the rate)
 bool tc_mlp_supported(const nphm_mlp *h)
 {
-    return h->cfg.hidden_dim == 512 && h->cfg.n_layers == 6 && h->cfg.lat_dim == 232 && h->cfg.out_dim == 3 && h->chain &&
-           h->chain->packed;
+    const int c = h->cfg.lat_dim;
+    return h->cfg.hidden_dim == 512 && h->cfg.n_layers == 6 && (c == 232 || c == 200 || c == 264) && h->cfg.out_dim == 3 &&
+           h->chain && h->chain->packed;
 }
 
 bool chain_packed(const nphm_mlp *h) { return h->chain && h->chain->packed; }

@@ -268,9 +268,9 @@ class DeformationNetwork(nn.Module):
     ``mode='compress'`` (the shipped configuration, ``scripts/configs/nphm_def.yaml``) conditions a
     :class:`DeepSDF` backbone on ``[Linear([z_id | anchors]) (32) | z_ex]``.  ``expr_only`` (``z_ex``) and ``glob_only``
     (``[z_id[:lat_dim_glob_shape] | z_ex]``) condition it on rows that are constant per query as well and take the same native
-    paths in eval mode (``forward``, ``offset_jacobian``, ``forward_native_grad``, the device Broyden search and the posed
-    queries); only the fitters need ``compress``.  ``interpolate`` and ``GNN`` are kept for API completeness (composite path
-    only)."""
+    paths in eval mode (``forward``, ``offset_jacobian``, ``forward_native_grad``, the device Broyden search, the posed
+    queries and the joint, batched and fixed-identity fitters, see ``fitting._IdentityRoute``).  ``interpolate`` and ``GNN``
+    are kept for API completeness (composite path only)."""
 
     def __init__(
             self,

@@ -293,16 +293,76 @@ def _latent_regularisers(decoder, lat_rep_shape):
     return out
 
 
+NATIVE_JOINT_MODES = ('compress', 'glob_only', 'expr_only')
+
+
 def _native_joint(decoder, decoder_expr, device) -> bool:
-    """The autograd-free joint fitter applies to the shipped configuration: a fused identity ensemble (see
-    :func:`_fused_identity`) and a 'compress' DeformationNetwork in eval mode on the same CUDA device."""
+    """The autograd-free joint fitter applies to a fused identity ensemble (see :func:`_fused_identity`) and a
+    DeformationNetwork in eval mode on the same CUDA device whose condition is constant per query (modes compress, glob_only,
+    expr_only; :class:`_IdentityRoute`).  glob_only also needs the identity code's global part to be as wide as the
+    deformation network's ``lat_dim_glob_shape``."""
     from .deepSDF import DeformationNetwork
     if device.type != 'cuda' or not _fused_identity(decoder, grad_points=True) or not isinstance(decoder_expr, DeformationNetwork):
         return False
-    if decoder_expr.training or decoder_expr.mode != 'compress':
+    if decoder_expr.training or decoder_expr.mode not in NATIVE_JOINT_MODES:
+        return False
+    if decoder_expr.mode == 'glob_only' and decoder_expr.lat_dim_glob_shape != decoder.lat_dim_glob:
         return False
     bb = decoder_expr.defDeepSDF
     return next(bb.parameters()).is_cuda and bb.num_freq_bands is None and bb.beta == 100 and bb.out_dim_net == 3
+
+
+class _IdentityRoute:
+    """How the identity code enters the deformation network's condition rows ``[prefix | z_ex]`` (deepSDF.py:203-224), and how
+    the prefix columns of the adjoint pass's condition gradient go back to the identity code:
+
+        mode       prefix (width P)                         d/d prefix goes to
+        compress   compressor([z_id | anchors])  (32)       through the compressor to z_id and the anchors
+        glob_only  z_id[:lat_dim_glob_shape]     (64)       summed over a subject's rows, added to d/d z_id[:P]
+        expr_only  nothing                       (0)        nowhere
+
+    ``z_ex`` takes the columns P: in every mode.  Only compress has an anchor term; the others hand the identity update a zero
+    anchor gradient.  Shapes follow the fitter: one subject (``z_id`` D, anchors 1 x K x 3, rows nb x P) or S subjects
+    (``z_id`` S x D, anchors S x K x 3, rows S nb x P); the compress arithmetic is the fitters' own, in their order."""
+
+    def __init__(self, decoder_expr):
+        self.mode = decoder_expr.mode
+        if self.mode == 'compress':
+            lin = decoder_expr.compressor[0] if isinstance(decoder_expr.compressor, torch.nn.Sequential) else decoder_expr.compressor
+            self.Wc, self.bc = lin.weight, lin.bias
+            self.width = self.Wc.shape[0]
+        else:
+            self.width = decoder_expr.lat_dim_glob_shape if self.mode == 'glob_only' else 0
+        self._zero_anchors = None
+
+    def prefix(self, z_id, anchors):
+        """The condition prefix of each subject: P, or S x P."""
+        if self.mode != 'compress':
+            return z_id[..., :self.width]
+        if z_id.dim() == 1:
+            first = torch.cat([z_id, anchors.reshape(-1)])
+            return (self.Wc * first[None, :]).sum(1) + self.bc
+        first = torch.cat([z_id, anchors.reshape(z_id.shape[0], -1)], dim=1)
+        return (self.Wc[None] * first[:, None, :]).sum(2) + self.bc
+
+    def identity_gradients(self, g_lat, g_rows, anchors):
+        """``(d/d z_id, d/d anchors)`` of the identity update: the surface term's ``g_lat`` (D or S x D) plus the prefix columns
+        ``g_rows`` of the condition gradient (nb x P or S nb x P), and the anchor gradient (3 K or S x 3 K) it passes on."""
+        D = g_lat.shape[-1]
+        if self.mode == 'compress':
+            if g_lat.dim() == 1:
+                g_first = (self.Wc * g_rows.sum(0)[:, None]).sum(0)                    # compressor^T -> [z_id | anchors]
+            else:
+                g_c32 = g_rows.reshape(g_lat.shape[0], -1, self.width).sum(1)
+                g_first = (self.Wc[None] * g_c32[:, :, None]).sum(1)                   # compressor^T, S x (D + 3 K)
+            return (g_lat + g_first[..., :D]).contiguous(), g_first[..., D:].contiguous()
+        if self._zero_anchors is None or self._zero_anchors.shape[:-1] != g_lat.shape[:-1]:
+            self._zero_anchors = g_lat.new_zeros(*g_lat.shape[:-1], anchors[0].numel())
+        if self.width == 0:
+            return g_lat, self._zero_anchors
+        g_zid = g_lat.clone()
+        g_zid[..., :self.width] += g_rows.reshape(*g_lat.shape[:-1], -1, self.width).sum(-2)
+        return g_zid, self._zero_anchors
 
 
 def _adam_expressions(fitter, g_zex, lr, stream):
@@ -321,18 +381,19 @@ class JointFitter:
         g_x   = d surface / d xc                                   nphm_fit_surface_grad (with d surface / d z_id)
         u     = -J^-T g_x            per point, J = I + dF_ex/dx    nphm_mlp_inverse_jacobian (forward-mode, tensor cores)
         g_c   = sum_n (dF_ex/d cond)^T u_n   per sampled scan       nphm_mlp_backward_inputs (adjoint pass, tensor cores)
-        cond  = [compressor([z_id | anchors]) (32) | z_ex (200)]    -> z_ex rows, and through the compressor to z_id and the
-                                                                      anchors (mlp_pos backward inside nphm_fit_apply_gradient)
-    followed by the regularisers and the two Adam updates (nphm_fit_apply_gradient, nphm_adam_step).
+        cond  = [prefix (P) | z_ex (E)]                             -> z_ex rows, and the prefix columns to z_id and the anchors
+    followed by the regularisers and the two Adam updates (nphm_fit_apply_gradient, nphm_adam_step).  The prefix depends on
+    the deformation mode (:class:`_IdentityRoute`): compress [compressor([z_id | anchors]) (32), whose gradient reaches the
+    anchors through mlp_pos inside nphm_fit_apply_gradient], glob_only [z_id[:64]] or expr_only [nothing].
 
-    ``fixed_identity=True`` holds ``z_id`` (set by the caller before the first step) fixed: the anchors and the compressor row
+    ``fixed_identity=True`` holds ``z_id`` (set by the caller before the first step) fixed: the anchors and the condition prefix
     are computed once, the surface term runs without the identity-code gradient, and a step is the z_ex route alone
     (-J^-T g_x, adjoint pass, reg_expr, Adam).  ``loss_terms`` are then the surface call's (unweighted)."""
 
     def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
         self.fixed_identity = fixed_identity
-        self._c32 = None
+        self.route, self._prefix = _IdentityRoute(decoder_expr), None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.defDeepSDF.engine()
         E = decoder_expr.lat_dim_expr
@@ -359,15 +420,12 @@ class JointFitter:
             self.t += 1
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.no_grad(), torch.cuda.device(dev):
-            # condition of the deformation backbone (deepSDF.py:218-219): compressor([z_id | anchors]) (32) | z_ex (E)
-            lin = self.dfn.compressor[0] if isinstance(self.dfn.compressor, torch.nn.Sequential) else self.dfn.compressor
-            Wc, bc = lin.weight, lin.bias
-            if self._c32 is None or not self.fixed_identity:
+            # condition of the deformation backbone (deepSDF.py:203-224): the identity prefix (P) | z_ex (E)
+            if self._prefix is None or not self.fixed_identity:
                 self.anchors = self.eng.anchors(self.z_id[None])                         # 1 x K x 3, pre-update code (:59)
-                first = torch.cat([self.z_id, self.anchors.reshape(-1)])
-                self._c32 = (Wc * first[None, :]).sum(1) + bc
-            c32 = self._c32
-            cond = torch.cat([c32[None, :].expand(nb, -1), self.z_ex[obs_idx]], dim=1).contiguous()
+                self._prefix = self.route.prefix(self.z_id, self.anchors)
+            P = self.route.width
+            cond = torch.cat([self._prefix[None, :].expand(nb, -1), self.z_ex[obs_idx]], dim=1).contiguous()
             # correspondence search (iterative_root_finding.py:91-168): J0^-1 at the observed points, Broyden on the device
             obs = obs.to(torch.float32).contiguous()
             _, j0_inv = self.mlp.inverse_jacobian(obs, cond)
@@ -383,17 +441,15 @@ class JointFitter:
             _surface_grad(self.eng, pts, _quirk_period(self.dec, n_point), self.z_id, mask, clamp, self.terms, g_lat, g_pts,
                           stream)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                       # -J^-T g_x
-            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # nb x (32 + E); same points as j_inv
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # nb x (P + E); same points as j_inv
             # expression codes: surface route + reg_expr = mean_b ||z_ex[idx_b]||^2 (:137), dense Adam over all rows (:169)
             lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
             g_zex = torch.zeros_like(self.z_ex)
-            g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, 32:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
+            g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, P:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
             if self.fixed_identity:
                 self.loss_terms.copy_(self.terms)
                 return _adam_expressions(self, g_zex, lr, stream) if apply_update else (None, g_zex)
-            g_first = (Wc * g_cond[:, :32].sum(0)[:, None]).sum(0)                       # compressor^T -> [z_id | anchors]
-            g_zid = (g_lat + g_first[:D]).contiguous()
-            g_anchors = g_first[D:].contiguous()
+            g_zid, g_anchors = self.route.identity_gradients(g_lat, g_cond[:, :P], self.anchors)
             stats = torch.stack([self.terms[5], self.terms[0] * self.terms[5]]).nan_to_num_(0.0).contiguous()
             fp = nat.FitParams(lam_s, float(lambdas.get('reg_global', 0.0)), float(lambdas.get('reg_loc', 0.0)),
                                float(lambdas.get('reg_unobserved', 0.0)), float(lambdas.get('symm_dist', 0.0)), float(clamp),
@@ -550,8 +606,8 @@ def inference_iterative_root_finding_joint(decoder,
                                            lr_scale=1):
     """Joint identity + expression fitting with Broyden correspondences (reference :14-177).
 
-    Shipped configuration (fused ensemble + 'compress' DeformationNetwork on CUDA): no autograd graph at all, see
-    :class:`JointFitter`; the same for the NPM baseline (``DeepSDF`` decoders on CUDA), see :class:`NpmJointFitter`.
+    Fused ensemble + eval-mode DeformationNetwork in mode compress (the shipped configuration), glob_only or expr_only on
+    CUDA: no autograd graph at all, see :class:`JointFitter`; the same for the NPM baseline (``DeepSDF`` decoders on CUDA), see :class:`NpmJointFitter`.
     ``NPHM_JOINT_AUTOGRAD=1`` keeps both on the composite path.  Anything else: the correspondence search runs on the device (`nphm_mlp_broyden_search`), the
     surface term comes from `nphm_fit_surface_grad`, the deformation network's part of the chain stays on autograd.  Returns
     ``(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)``."""
@@ -863,10 +919,10 @@ def _pad_rows(obs: List[torch.Tensor], n_point: int, front: bool = False):
 
 class BatchedJointFitter:
     """:class:`JointFitter` for S subjects at once.  Per iteration, for the 5 sampled observations of every subject:
-        anchors of the S identity codes (nphm_ensemble_anchors), condition rows [compressor([z_id | anchors])[subject] | z_ex[row]]
+        anchors of the S identity codes (nphm_ensemble_anchors), condition rows [prefix(z_id, anchors)[subject] | z_ex[row]]
         J0^-1, Broyden and J^-1 on all 5 S rows (per-row conditions; shorter subjects padded, the padding masked)
         nphm_fit_surface_grad_batched: per-subject surface term, d/d z_id and d/d point
-        u = -J^-T g_x, one adjoint pass, the compressor adjoint summed per subject
+        u = -J^-T g_x, one adjoint pass, the prefix columns routed to each subject's identity code (:class:`_IdentityRoute`)
         nphm_fit_apply_gradient_batched (regularisers, mlp_pos backward, Adam per subject)
         one nphm_adam_step over the expression codes of all subjects (element-wise, shared step and lr: the same as per subject).
     The expression codes are one (sum n_obs) x E tensor; subject k's rows start at ``offsets[k]``.  In eval mode a shorter
@@ -878,7 +934,7 @@ class BatchedJointFitter:
     def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
         self.fixed_identity = fixed_identity
-        self._c32 = None
+        self.route, self._prefix = _IdentityRoute(decoder_expr), None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.defDeepSDF.engine()
         E, S = decoder_expr.lat_dim_expr, len(num_observations)
@@ -907,15 +963,12 @@ class BatchedJointFitter:
         stream = torch.cuda.current_stream(dev).cuda_stream
         lib = nat.lib()
         with torch.no_grad(), torch.cuda.device(dev):
-            lin = self.dfn.compressor[0] if isinstance(self.dfn.compressor, torch.nn.Sequential) else self.dfn.compressor
-            Wc, bc = lin.weight, lin.bias
-            if self._c32 is None or not self.fixed_identity:
+            if self._prefix is None or not self.fixed_identity:
                 self.anchors = self.eng.anchors(self.z_id)                               # S x K x 3, pre-update codes
-                first = torch.cat([self.z_id, self.anchors.reshape(S, -1)], dim=1)
-                self._c32 = (Wc[None] * first[:, None, :]).sum(2) + bc                   # S x 32
-            c32 = self._c32
+                self._prefix = self.route.prefix(self.z_id, self.anchors)                # S x P
+            P = self.route.width
             rows = torch.cat([idx + off for idx, off in zip(obs_idx, self.offsets)])    # rows of z_ex, 5 S
-            cond = torch.cat([c32.repeat_interleave(nb, dim=0), self.z_ex[rows]], dim=1).contiguous()
+            cond = torch.cat([self._prefix.repeat_interleave(nb, dim=0), self.z_ex[rows]], dim=1).contiguous()
             # every subject padded to n_point points per observation (the padding repeats a point and is masked below); in eval
             # mode in front of the row, so that its last point stays last
             front = not self.dec.training
@@ -948,19 +1001,16 @@ class BatchedJointFitter:
                                                             nat._ptr(g_lat), g_pts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
                           'nphm_fit_surface_grad_batched')
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
-            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # 5 S x (32 + E)
+            g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # 5 S x (P + E)
             lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
             g_zex = torch.zeros_like(self.z_ex)
-            g_zex.index_add_(0, rows, lam_s * g_cond[:, 32:] + (2.0 * lam_e / nb) * self.z_ex[rows])
+            g_zex.index_add_(0, rows, lam_s * g_cond[:, P:] + (2.0 * lam_e / nb) * self.z_ex[rows])
             if self.fixed_identity:
                 self.loss_terms.copy_(terms)
                 if not apply_update:
                     return None, [g_zex[o:o + c] for o, c in zip(self.offsets, self.num_observations)]
                 return _adam_expressions(self, g_zex, lr, stream)
-            g_c32 = g_cond[:, :32].reshape(S, nb, 32).sum(1)
-            g_first = (Wc[None] * g_c32[:, :, None]).sum(1)                              # compressor^T, S x (D + 3 K)
-            g_zid = (g_lat + g_first[:, :D]).contiguous()
-            g_anchors = g_first[:, D:].contiguous()
+            g_zid, g_anchors = self.route.identity_gradients(g_lat, g_cond[:, :P], self.anchors)
             stats = torch.stack([terms[:, 5], terms[:, 0] * terms[:, 5]], dim=1).nan_to_num_(0.0).contiguous()
             fp = nat.FitParams(lam_s, float(lambdas.get('reg_global', 0.0)), float(lambdas.get('reg_loc', 0.0)),
                                float(lambdas.get('reg_unobserved', 0.0)), float(lambdas.get('symm_dist', 0.0)), float(clamp),
@@ -1108,7 +1158,7 @@ def inference_iterative_root_finding_joint_batched(decoder,
                                                    lr_scale=1):
     """:func:`inference_iterative_root_finding_joint` for several subjects (``subjects[k]``: the observations of subject k) at
     once.  Returns ``[(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)]`` in subject order, under the contract of
-    :func:`inference_identity_space_batched`.  The shipped configuration (see :func:`_native_joint`) runs all subjects in one
+    :func:`inference_identity_space_batched`.  The ensemble configurations of :func:`_native_joint` run all subjects in one
     launch sequence per iteration (:class:`BatchedJointFitter`), and so does the NPM baseline (see :func:`_native_npm_joint`,
     :class:`BatchedNpmJointFitter`); anything else - CPU, other decoders or deformation modes, ``NPHM_JOINT_AUTOGRAD=1`` -
     calls the single-subject function subject by subject.  Memory grows linearly with the number of subjects; all subjects
