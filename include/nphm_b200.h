@@ -717,6 +717,60 @@ int nphm_transfer_correspondences(const double *src_verts_dev, long long n_src_v
                                   const long long *face_idx_dev, const double *bary_dev, const double *offsets_dev, long long n,
                                   double *p_src_dev, double *p_dst_dev, double *n_src_dev, double *n_dst_dev, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Sphere tracing of SDF heads into render_views' image format (csrc/sdf_trace.cu, DESIGN.md §4.23).  A chunk is n_rays
+ * consecutive pixels of V views of H x W for each of n_heads heads; the caller evaluates the field between the steps with the
+ * existing query entry points.  Ray of pixel (r, c) of view v: origin = translation of cam_to_world[v], direction =
+ * rotation of cam_to_world[v] applied to ((c + 0.5 - cx)/fx, (cy - r - 0.5)/fy, -1) (render.cu's eye ray), unit u, arc length s.
+ * The field seen along it is f(s) = sdf(scale (o + s u)); the march runs over s in [s_in, s_out], the ray's part inside
+ * {x : scale x in [box_min, box_max]} and eye depth [znear, zfar]; a ray with s_in > s_out is a miss without a query.
+ * A march step on a LIVE ray with f = sigma f(s), sigma = the sign of f at the first sample (-1 when the ray enters inside):
+ *   f < 0 after a positive sample            -> BRACKET [last positive sample, s], s = secant point (fraction clamped to [0.1, 0.9])
+ *   f < hit_eps                              -> HIT at s
+ *   else  s += step_factor max(f / scale, min_step);  s > s_out -> MISS;  else steps == max_steps -> OUT_OF_STEPS
+ *   and, with a valid flag (posed heads), an invalid sample -> INVALID.
+ * A refinement step on a BRACKET ray replaces the end of the bracket whose sign f(s) has, then s = the secant point again.
+ * Status codes: 0 LIVE, 1 BRACKET, 2 HIT, 3 MISS, 4 OUT_OF_STEPS, 5 INVALID.  Nothing here reads back to the host except
+ * nphm_trace_counts. */
+typedef struct {
+    int n_heads;              /* S: heads (or expressions), each with its own ray state                                  */
+    long long n_rays;         /* pixels of the chunk; n_heads * n_rays < 2^31                                             */
+    double box_min[3], box_max[3];  /* the box, in the decoder's coordinates                                              */
+    double scale;             /* query point = scale * world point                                                        */
+    double znear, zfar;       /* eye-depth range                                                                          */
+    float step_factor, min_step, hit_eps;   /* min_step: world units (arc length); hit_eps: SDF units                    */
+    int max_steps;
+} nphm_trace_params;
+
+/* bytes of the state of one chunk (-1: bad sizes) */
+long long nphm_trace_workspace_bytes(int n_heads, long long n_rays);
+/* ray setup of pixels [first_pixel, first_pixel + n_rays) of the views (cam_to_world_dev: V x 12 rows of the camera-to-world
+ * 3 x 4, intrinsics_dev: V x 4 fx fy cx cy, fp64) for every head: state LIVE at s_in, or MISS */
+int nphm_trace_begin(const nphm_trace_params *p, const double *cam_to_world_dev, const double *intrinsics_dev, int n_views,
+                     int height, int width, long long first_pixel, void *workspace_dev, long long workspace_bytes, void *stream);
+/* ordered list of each head's LIVE rays (refine = 0) or BRACKET rays (refine = 1), and the per-head counts, on the device */
+int nphm_trace_compact(const nphm_trace_params *p, int refine, void *workspace_dev, long long workspace_bytes, void *stream);
+/* the per-head counts of the last compaction -> counts_host (n_heads ints); synchronises the stream */
+int nphm_trace_counts(const nphm_trace_params *p, const void *workspace_dev, long long workspace_bytes, int *counts_host, void *stream);
+/* points_dev [n_heads][n_cols][3]: row j < count_h of head h the scaled sample point of its j-th listed ray, the rest (0, 0, 0).
+ * n_cols must be at least every head's count (n_rays always is). */
+int nphm_trace_gather(const nphm_trace_params *p, long long n_cols, void *workspace_dev, long long workspace_bytes, float *points_dev,
+                      void *stream);
+/* one march (refine = 0) or refinement (refine = 1) step of the listed rays from sdf_dev [n_heads][n_cols] at the gathered
+ * points; valid_dev [n_heads][n_cols] bytes (may be NULL = all valid) */
+int nphm_trace_advance(const nphm_trace_params *p, int refine, long long n_cols, const float *sdf_dev, const unsigned char *valid_dev,
+                       void *workspace_dev, long long workspace_bytes, void *stream);
+/* points_dev [n_heads][n_rays][3]: the scaled hit point of every HIT or BRACKET ray, (0, 0, 0) elsewhere */
+int nphm_trace_points(const nphm_trace_params *p, const void *workspace_dev, long long workspace_bytes, float *points_dev, void *stream);
+/* Writes ray i of head h to pixel h * n_pixels + first_pixel + i of the images: BRACKET rays become HITs at their last secant
+ * point; a HIT with valid_dev[h][i] == 0 (may be NULL) becomes INVALID.  depth_dev: eye depth of the hit, 0 elsewhere;
+ * normals_dev (3 bytes per pixel): normalize(grad) - grad_dev [n_heads][n_rays][3], or J^T grad with jinv_dev
+ * [n_heads][n_rays][3][3] (may be NULL) - rounded as render.cu rounds face normals, (0, 0, 0) elsewhere; points_dev (may be
+ * NULL): world point of HIT and INVALID rays, 0 elsewhere; status_dev / steps_dev (may be NULL): status and march steps. */
+int nphm_trace_finish(const nphm_trace_params *p, const void *workspace_dev, long long workspace_bytes, const float *grad_dev,
+                      const float *jinv_dev, const unsigned char *valid_dev, long long n_pixels, long long first_pixel, float *depth_dev,
+                      unsigned char *normals_dev, float *points_dev, unsigned char *status_dev, int *steps_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

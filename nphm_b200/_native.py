@@ -59,6 +59,8 @@ EXPORTED_SYMBOLS = (
     'nphm_band_sparse_heads_mc_workspace_bytes', 'nphm_band_sparse_heads_mc_count', 'nphm_band_sparse_heads_mc_emit',
     'nphm_face_cdf_workspace_bytes', 'nphm_face_cdf', 'nphm_sample_faces', 'nphm_vertex_normals_workspace_bytes',
     'nphm_vertex_normals', 'nphm_interpolate_barycentric', 'nphm_transfer_correspondences',
+    'nphm_trace_workspace_bytes', 'nphm_trace_begin', 'nphm_trace_compact', 'nphm_trace_counts', 'nphm_trace_gather',
+    'nphm_trace_advance', 'nphm_trace_points', 'nphm_trace_finish',
 )
 
 
@@ -118,6 +120,12 @@ class BandPool(Structure):
     _fields_ = [('vals', c_void_p), ('marks', c_void_p), ('blocks', c_void_p), ('list', c_void_p), ('chunk_cnt', c_void_p),
                 ('chunk_off', c_void_p), ('slots', c_longlong), ('marks_bytes', c_longlong), ('list_len', c_longlong),
                 ('n_chunks', c_longlong)]
+
+
+class TraceParams(Structure):
+    _fields_ = [('n_heads', c_int), ('n_rays', c_longlong), ('box_min', c_double * 3), ('box_max', c_double * 3),
+                ('scale', c_double), ('znear', c_double), ('zfar', c_double), ('step_factor', c_float), ('min_step', c_float),
+                ('hit_eps', c_float), ('max_steps', c_int)]
 
 
 class FitParams(Structure):
@@ -332,6 +340,17 @@ def lib() -> ctypes.CDLL:
                                                c_void_p]
     L.nphm_transfer_correspondences.argtypes = [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p,
                                                 c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    tp = [POINTER(TraceParams)]
+    L.nphm_trace_workspace_bytes.argtypes = [c_int, c_longlong]
+    L.nphm_trace_workspace_bytes.restype = c_longlong
+    L.nphm_trace_begin.argtypes = tp + [c_void_p, c_void_p, c_int, c_int, c_int, c_longlong, c_void_p, c_longlong, c_void_p]
+    L.nphm_trace_compact.argtypes = tp + [c_int, c_void_p, c_longlong, c_void_p]
+    L.nphm_trace_counts.argtypes = tp + [c_void_p, c_longlong, POINTER(c_int), c_void_p]
+    L.nphm_trace_gather.argtypes = tp + [c_longlong, c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_trace_advance.argtypes = tp + [c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]
+    L.nphm_trace_points.argtypes = tp + [c_void_p, c_longlong, c_void_p, c_void_p]
+    L.nphm_trace_finish.argtypes = tp + [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p,
+                                         c_void_p, c_void_p, c_void_p, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L
@@ -965,6 +984,74 @@ def render_depth_normals(verts: torch.Tensor, faces: torch.Tensor, world_to_eye:
                                           float(znear), float(zfar), H, W, depth.data_ptr(), normals.data_ptr(), _ptr(tri),
                                           ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'nphm_render_depth_normals')
     return (depth.view(V, H, W), normals.view(V, H, W, 3), None if tri is None else tri.view(V, H, W))
+
+
+# ------------------------------------------------------------------------------------------ sphere tracing
+TRACE_LIVE, TRACE_BRACKET, TRACE_HIT, TRACE_MISS, TRACE_OUT_OF_STEPS, TRACE_INVALID = range(6)
+
+
+class SdfTrace:
+    """The ray state of one chunk of a sphere trace (csrc/sdf_trace.cu): ``n_rays`` consecutive pixels of the views for each of
+    ``n_heads`` heads.  The field is evaluated by the caller between :meth:`gather` and :meth:`advance`; nothing but
+    :meth:`counts` reads back from the device."""
+
+    def __init__(self, n_heads: int, n_rays: int, mini, maxi, scale: float, znear: float, zfar: float, step_factor: float,
+                 min_step: float, hit_eps: float, max_steps: int, device):
+        self.p = TraceParams(int(n_heads), int(n_rays), (c_double * 3)(*[float(v) for v in mini]),
+                             (c_double * 3)(*[float(v) for v in maxi]), float(scale), float(znear), float(zfar), float(step_factor),
+                             float(min_step), float(hit_eps), int(max_steps))
+        self.device = device
+        self.ws = _workspace(lib().nphm_trace_workspace_bytes(int(n_heads), int(n_rays)), 'nphm_trace_workspace_bytes', device)
+
+    def _call(self, fn, *args):
+        with torch.cuda.device(self.device):
+            check(getattr(lib(), fn)(byref(self.p), *args), fn)
+
+    def _mem(self):
+        return self.ws.data_ptr(), self.ws.numel()
+
+    def begin(self, cam_to_world: torch.Tensor, intrinsics: torch.Tensor, height: int, width: int, first_pixel: int):
+        """cam_to_world (V, 12) and intrinsics (V, 4) float64 CUDA tensors."""
+        self._c2w, self._intr = cam_to_world, intrinsics                  # kept alive until the stream has read them
+        self._call('nphm_trace_begin', cam_to_world.data_ptr(), intrinsics.data_ptr(), cam_to_world.shape[0], int(height), int(width),
+                   int(first_pixel), *self._mem(), _stream_ptr(self.device))
+
+    def compact(self, refine: bool):
+        self._call('nphm_trace_compact', int(bool(refine)), *self._mem(), _stream_ptr(self.device))
+
+    def counts(self):
+        """The per-head counts of the last :meth:`compact` (one read-back)."""
+        out = (c_int * self.p.n_heads)()
+        self._call('nphm_trace_counts', *self._mem(), out, _stream_ptr(self.device))
+        return list(out)
+
+    def gather(self, n_cols: int, out: torch.Tensor) -> torch.Tensor:
+        """out: (n_heads, >= n_cols, 3) float32; returns its (n_heads, n_cols, 3) view of the listed rays' sample points."""
+        pts = out.reshape(-1)[:self.p.n_heads * n_cols * 3]
+        self._call('nphm_trace_gather', int(n_cols), *self._mem(), pts.data_ptr(), _stream_ptr(self.device))
+        return pts.view(self.p.n_heads, n_cols, 3)
+
+    def advance(self, refine: bool, sdf: torch.Tensor, valid: Optional[torch.Tensor] = None):
+        """sdf (n_heads, n_cols) float32 at the gathered points, valid the same shape (bool / uint8) or None."""
+        n_cols = sdf.shape[1]
+        sdf = _f32c(sdf)
+        v = None if valid is None else valid.to(torch.uint8).contiguous()
+        self._call('nphm_trace_advance', int(bool(refine)), int(n_cols), sdf.data_ptr(), _ptr(v), *self._mem(), _stream_ptr(self.device))
+        self._keep = (sdf, v)
+
+    def points(self) -> torch.Tensor:
+        out = torch.empty(self.p.n_heads, self.p.n_rays, 3, device=self.device, dtype=torch.float32)
+        self._call('nphm_trace_points', *self._mem(), out.data_ptr(), _stream_ptr(self.device))
+        return out
+
+    def finish(self, grad: torch.Tensor, jinv: Optional[torch.Tensor], valid: Optional[torch.Tensor], first_pixel: int,
+               depth: torch.Tensor, normals: torch.Tensor, points: Optional[torch.Tensor], status: torch.Tensor, steps: torch.Tensor):
+        """Write the chunk into the (S, n_pixels, ...) images."""
+        g = _f32c(grad)
+        j = None if jinv is None else _f32c(jinv)
+        v = None if valid is None else valid.to(torch.uint8).contiguous()
+        self._call('nphm_trace_finish', *self._mem(), g.data_ptr(), _ptr(j), _ptr(v), depth.shape[1], int(first_pixel), depth.data_ptr(),
+                   normals.data_ptr(), _ptr(points), status.data_ptr(), steps.data_ptr(), _stream_ptr(self.device))
 
 
 # ------------------------------------------------------------------------------------------ training supervision

@@ -195,3 +195,6 @@ def gen_render_samples(m, N, scale=4):
     depth, normals = render_views(vertices, mesh.faces, poses, KK, (1280, 960))
     points, nrm = samples_from_images(depth, normals, cams, poses, scale)
     return points.cpu().numpy(), nrm.cpu().numpy()
+
+
+from .sdf_render import render_sdf_views  # noqa: E402,F401  (sphere-traced images of SDF heads in this module's format)

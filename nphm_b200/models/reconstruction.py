@@ -104,13 +104,10 @@ def _expression_codes(lat_reps_expr):
     return codes, single
 
 
-def posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes):
-    """The native posed query of expressions ``codes`` (S x E), or None when the decoders have none (see
-    :func:`get_logits_posed`): a function ``(points S x n x 3 float32 CUDA, quirk) -> (sdf S x n, valid S x n bool)``, row
-    (s, i) the posed SDF of ``points[s, i]`` under expression s.  ``quirk``: every row takes the ensemble's eval-mode
-    last-point-of-call value.  Each row depends on its own point and code only: J0^-1 at the point
-    (``nphm_mlp_inverse_jacobian``), the compacting Broyden search (``nphm_mlp_broyden_search_compact``) and the identity query at
-    the root, in pieces of :data:`POSED_PIECE_ROWS` rows."""
+def posed_parts(decoder_shape, decoder_expr, lat_rep_shape, codes):
+    """The native pieces of the posed query of expressions ``codes`` (S x E), or None when the decoders have none:
+    ``(device, cond S x C, search_engine, identity)`` with ``identity(xc S x n x 3, quirk) -> sdf S x n`` the identity decoder at
+    canonical points.  ``shape_engine`` and ``z_id`` (1 x D) are attributes of ``identity``."""
     from .deepSDF import DeepSDF, DeformationNetwork
     from .fitting import NPM_EXPR_DIM, _native_npm_decoder
     from .iterative_root_finding import _fused_search_condition
@@ -149,6 +146,22 @@ def posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes):
                 return shape_engine.query(xc, lat).reshape(S, -1)
         else:
             return None
+    identity.shape_engine, identity.z_id = shape_engine, z_id
+    return device, cond, search_engine, identity
+
+
+def posed_evaluator(decoder_shape, decoder_expr, lat_rep_shape, codes):
+    """The native posed query of expressions ``codes`` (S x E), or None when the decoders have none (see
+    :func:`get_logits_posed`): a function ``(points S x n x 3 float32 CUDA, quirk) -> (sdf S x n, valid S x n bool)``, row
+    (s, i) the posed SDF of ``points[s, i]`` under expression s.  ``quirk``: every row takes the ensemble's eval-mode
+    last-point-of-call value.  Each row depends on its own point and code only: J0^-1 at the point
+    (``nphm_mlp_inverse_jacobian``), the compacting Broyden search (``nphm_mlp_broyden_search_compact``) and the identity query at
+    the root, in pieces of :data:`POSED_PIECE_ROWS` rows."""
+    parts = posed_parts(decoder_shape, decoder_expr, lat_rep_shape, codes)
+    if parts is None:
+        return None
+    device, cond, search_engine, identity = parts
+    S = codes.shape[0]
 
     def evaluate(points, quirk=False):
         n = points.shape[1]
