@@ -771,6 +771,27 @@ int nphm_trace_finish(const nphm_trace_params *p, const void *workspace_dev, lon
                       const float *jinv_dev, const unsigned char *valid_dev, long long n_pixels, long long first_pixel, float *depth_dev,
                       unsigned char *normals_dev, float *points_dev, unsigned char *status_dev, int *steps_dev, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Observation poses of the fitters (csrc/pose.cu, DESIGN.md §4.24): observation o maps scan-frame points p to the model frame,
+ * q = exp(sigma_o) R_o p + t_o.  table_dev: n_obs x 13 fp64, row o = [R_o row-major | t_o | sigma_o].  Points come in n_rows
+ * rows of n_point, row r drawn from observation row_obs_dev[r] (int32, device); a row whose index lies outside [0, n_obs) is
+ * padding.  All three enqueue on the stream and never synchronise.
+ * ---------------------------------------------------------------------------------------------- */
+/* out_dev [n_rows][n_point][3] = q of points_dev (same layout), evaluated in fp64 and rounded once; padding rows are copied */
+int nphm_pose_apply(const float *points_dev, const int *row_obs_dev, long long n_rows, long long n_point, const double *table_dev,
+                    int n_obs, float *out_dev, void *stream);
+/* grad_dev [n_obs][7] = lam_surface * sum over the rows of o and their points of ((q - t_o) x g, g, g . (q - t_o)) with g =
+ * d loss / d q (grad_q_dev, the layout of q_dev): the gradient w.r.t. (omega, t, sigma) for the left perturbation
+ * R <- Exp(omega) R.  Summed in fp64, within a row and then over the rows in row order: bitwise repeatable.  Padding rows
+ * contribute nothing; an observation without rows gets 0. */
+int nphm_pose_grad(const float *q_dev, const float *grad_q_dev, const int *row_obs_dev, long long n_rows, long long n_point,
+                   const double *table_dev, int n_obs, double lam_surface, double *grad_dev, void *stream);
+/* Adam (betas 0.9 / 0.999, eps 1e-8, 1-based step) on (omega, t, sigma) of every observation with learning rates lr_rot (omega),
+ * lr_trans (t) and lr_scale (sigma); the step delta = -step is applied as R <- Exp(delta_omega) R (Rodrigues, then the rows
+ * re-orthonormalised), t += delta_t and, when fit_scale, sigma += delta_sigma.  adam_m_dev / adam_v_dev: n_obs x 7 fp64. */
+int nphm_pose_adam(double *table_dev, double *adam_m_dev, double *adam_v_dev, const double *grad_dev, int n_obs, double lr_rot,
+                   double lr_trans, double lr_scale, int fit_scale, int step, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

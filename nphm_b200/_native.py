@@ -61,6 +61,7 @@ EXPORTED_SYMBOLS = (
     'nphm_vertex_normals', 'nphm_interpolate_barycentric', 'nphm_transfer_correspondences',
     'nphm_trace_workspace_bytes', 'nphm_trace_begin', 'nphm_trace_compact', 'nphm_trace_counts', 'nphm_trace_gather',
     'nphm_trace_advance', 'nphm_trace_points', 'nphm_trace_finish',
+    'nphm_pose_apply', 'nphm_pose_grad', 'nphm_pose_adam',
 )
 
 
@@ -351,6 +352,11 @@ def lib() -> ctypes.CDLL:
     L.nphm_trace_points.argtypes = tp + [c_void_p, c_longlong, c_void_p, c_void_p]
     L.nphm_trace_finish.argtypes = tp + [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p]
+    L.nphm_pose_apply.argtypes = [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_void_p, c_void_p]
+    L.nphm_pose_grad.argtypes = [c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_double, c_void_p,
+                                 c_void_p]
+    L.nphm_pose_adam.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_int, c_int,
+                                 c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L

@@ -26,6 +26,7 @@ from torch import optim
 from .. import _native
 from .EnsembledDeepSDF import FastEnsembleDeepSDFMirrored
 from .iterative_root_finding import search, nabla          # noqa: F401  (same names as the reference imports)
+from .pose import ObservationPoses, check_poses, compose_f64  # noqa: F401  (ObservationPoses is public here)
 from .diff_operators import gradient, jac                    # noqa: F401
 
 NUM_OBSERVATIONS_PER_BATCH = 5
@@ -121,11 +122,26 @@ def _quirk_period(decoder, points_per_call: int) -> int:
     return 0 if decoder.training else int(points_per_call)
 
 
-class IdentityFitter:
-    """Stateful wrapper around ``nphm_fit_identity_step``: latent + Adam moments live on the device."""
+def _pose_step(fitter, q, g_q, rows, lam_s, lr, apply_update):
+    """The pose's part of a posed step: ``poses.grad`` from ``g_q = d surface / d q`` at the sampled points ``q`` (rows x n x 3,
+    row r from observation ``rows[r]``), then, with ``apply_update``, Adam at the fitter's step count with the pose rates
+    scaled by lr / (the lr of the fitter's first step)."""
+    if fitter.pose_lr0 is None:
+        fitter.pose_lr0 = lr
+    fitter.poses.gradient(q, g_q, rows, lam_s)
+    if apply_update:
+        fitter.poses.update(lr / fitter.pose_lr0, fitter.t)
 
-    def __init__(self, decoder: FastEnsembleDeepSDFMirrored, device):
+
+class IdentityFitter:
+    """Stateful wrapper around ``nphm_fit_identity_step``: latent + Adam moments live on the device.  With ``poses`` (an
+    :class:`ObservationPoses` of the scan's observations) a step moves the sampled rows into the model frame first and fits
+    the poses too; the fused step has no point gradient, so it then runs as ``nphm_fit_surface_grad`` with the point gradient
+    and ``nphm_fit_apply_gradient`` (the joint fitter's route, the same math), which needs the tensor-core configuration."""
+
+    def __init__(self, decoder: FastEnsembleDeepSDFMirrored, device, poses: ObservationPoses = None):
         self.decoder = decoder
+        self.poses, self.pose_lr0, self._ones = poses, None, None
         self.device = device
         self.engine = decoder.engine()
         self.latent = torch.zeros(decoder.lat_dim, device=device, dtype=torch.float32)
@@ -135,9 +151,11 @@ class IdentityFitter:
         self.grad = torch.zeros_like(self.latent)
         self.t = 0
 
-    def step(self, points: torch.Tensor, lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
+    def step(self, points: torch.Tensor, lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True,
+             obs_idx: torch.Tensor = None):
         """One iteration on ``points`` (rows x n x 3: the reference's one decoder call on its sampled rows).  In eval mode the
-        last point of every row carries the quirk (``nphm_fit_identity_step_quirk`` with period n)."""
+        last point of every row carries the quirk (``nphm_fit_identity_step_quirk`` with period n).  With poses, ``obs_idx``
+        (rows, on the device) gives each row's observation."""
         pts = points.reshape(-1, 3).to(dtype=torch.float32).contiguous()
         period = _quirk_period(self.decoder, points.shape[-2] if points.dim() > 1 else 1)
         if apply_update:
@@ -147,7 +165,21 @@ class IdentityFitter:
                                float(lambdas.get('symm_dist', 0.0)), float(clamp), float(lr), max(self.t, 1))
         stream = torch.cuda.current_stream(self.device).cuda_stream
         with torch.cuda.device(self.device):
-            if period:
+            if self.poses is not None:
+                q = self.poses.apply(points, obs_idx)
+                pts = q.reshape(-1, 3)
+                if self._ones is None or self._ones.shape[0] != pts.shape[0]:
+                    self._ones = torch.ones(pts.shape[0], dtype=torch.uint8, device=self.device)
+                terms, g_pts = torch.empty(8, device=self.device), torch.empty_like(pts)
+                g_lat = torch.empty_like(self.latent)
+                _surface_grad(self.engine, pts, period, self.latent, self._ones, clamp, terms, g_lat, g_pts, stream)
+                stats = torch.stack([terms[5], terms[0] * terms[5]]).nan_to_num_(0.0).contiguous()
+                _native.check(_native.lib().nphm_fit_apply_gradient(
+                    self.engine.handle, self.latent.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), ctypes.byref(fp),
+                    g_lat.data_ptr(), stats.data_ptr(), None, int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
+                    stream), 'nphm_fit_apply_gradient')
+                _pose_step(self, q, g_pts.reshape(q.shape), obs_idx, float(lambdas.get('surface', 0.0)), lr, apply_update)
+            elif period:
                 _native.check(_native.lib().nphm_fit_identity_step_quirk(
                     self.engine.handle, pts.data_ptr(), pts.shape[0], period, self.latent.data_ptr(), self.m.data_ptr(),
                     self.v.data_ptr(), ctypes.byref(fp), int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
@@ -210,40 +242,69 @@ def inference_identity_space(decoder,
                              n_steps,
                              schedule_cfg: Dict,
                              step_scale=1,
-                             lr_scale=1):
+                             lr_scale=1,
+                             poses: ObservationPoses = None):
     """Fit the identity code to point-cloud observations.  Returns ``(lat_rep_shape (1,1,D), anchors (1,K,3))``; a
-    ``DeepSDF`` decoder has no anchors (``None``), as in the reference."""
+    ``DeepSDF`` decoder has no anchors (``None``), as in the reference.  ``poses`` (an :class:`ObservationPoses` of
+    ``len(all_obs)`` observations on their device): the observations are in their own frames and their similarity transforms
+    to the model frame are fitted with the code, in place (DESIGN.md §4.24)."""
     device = all_obs[0].device
+    check_poses(poses, len(all_obs), device)
     lr = 0.01 * lr_scale
     if device.type == 'cuda' and _native_npm_decoder(decoder, 1):
-        fitter = NpmIdentityFitter(decoder, device)
+        fitter = NpmIdentityFitter(decoder, device, poses)
         for j in range(int(n_steps * step_scale)):
             lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
-            obs, _ = _sample_observations(all_obs)
-            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+            obs, idx = _sample_observations(all_obs)
+            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr, obs_idx=_pose_rows(poses, idx, device))
         return fitter.latent.reshape(1, 1, -1).clone().requires_grad_(True), None
-    if _fused_identity(decoder) and device.type == 'cuda':
-        fitter = IdentityFitter(decoder, device)
+    if _fused_identity(decoder, grad_points=poses is not None) and device.type == 'cuda':
+        fitter = IdentityFitter(decoder, device, poses)
         z_prev = fitter.latent.clone()
         for j in range(int(n_steps * step_scale)):
             lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
-            obs, _ = _sample_observations(all_obs)
+            obs, idx = _sample_observations(all_obs)
             z_prev.copy_(fitter.latent)
-            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr, obs_idx=_pose_rows(poses, idx, device))
         with torch.no_grad():
             _, anchors = fitter.engine.query(torch.zeros(1, 1, 3, device=device), z_prev.reshape(1, -1), eval_quirk=False)
         lat_rep_shape = fitter.latent.reshape(1, 1, -1).clone().requires_grad_(True)
         return lat_rep_shape, anchors
-    return _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
+    return _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale, poses)
 
 
-def _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1):
+def _pose_rows(poses, idx, device):
+    """The sampled rows' observation indices on the device for a posed fit (None without poses: no upload)."""
+    return None if poses is None else idx.to(device=device, dtype=torch.int32)
+
+
+class _TangentPoses:
+    """The autograd fallback's pose: a zero tangent leaf per observation composed with the current pose (``compose_f64``);
+    after ``backward`` its gradient is the pose gradient, and the update is the float64 Adam and retraction of the kernels."""
+
+    def __init__(self, poses: ObservationPoses):
+        self.poses, self.lr0, self.xi = poses, None, None
+
+    def __call__(self, obs, idx):
+        self.xi = torch.zeros(self.poses.n, 7, dtype=torch.float64, device=self.poses.device, requires_grad=True)
+        return compose_f64(self.poses.table, obs, idx, self.xi)
+
+    def step(self, lr, step):
+        if self.lr0 is None:
+            self.lr0 = lr
+        self.poses.grad.copy_(self.xi.grad)
+        self.poses.update(lr / self.lr0, step, native=False)
+
+
+def _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1,
+                                       poses=None):
     """The composite path of :func:`inference_identity_space`: autograd through the modules (any decoder, CPU or GPU)."""
     device = all_obs[0].device
     lr = 0.01 * lr_scale
     lat_dim = decoder.lat_dim
     lat_rep_shape = torch.zeros([1, 1, lat_dim], device=device, requires_grad=True)
     opt = optim.Adam(params=[lat_rep_shape], lr=lr)
+    tangent = None if poses is None else _TangentPoses(poses)
     anchors = None
     for j in range(int(n_steps * step_scale)):
         new_lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
@@ -253,7 +314,9 @@ def _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, sched
                 group['lr'] = lr
         opt.zero_grad()
         anchors = _current_anchors(decoder, lat_rep_shape, device)
-        obs, _ = _sample_observations(all_obs)
+        obs, idx = _sample_observations(all_obs)
+        if tangent is not None:
+            obs = tangent(obs, idx)
         nb = obs.shape[0]
         if hasattr(decoder, 'lat_dim_loc'):
             sdf, _ = decoder(obs, lat_rep_shape.repeat(nb, 1, 1), None)
@@ -268,6 +331,8 @@ def _inference_identity_space_autograd(decoder, all_obs, lambdas, n_steps, sched
             loss = loss + loss_dict[k] * lambdas[k]
         loss.backward()
         opt.step()
+        if tangent is not None:
+            tangent.step(lr, j + 1)
     return lat_rep_shape, anchors
 
 
@@ -390,9 +455,11 @@ class JointFitter:
     are computed once, the surface term runs without the identity-code gradient, and a step is the z_ex route alone
     (-J^-T g_x, adjoint pass, reg_expr, Adam).  ``loss_terms`` are then the surface call's (unweighted)."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False):
+    def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False,
+                 poses: ObservationPoses = None):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
         self.fixed_identity = fixed_identity
+        self.poses, self.pose_lr0 = poses, None
         self.route, self._prefix = _IdentityRoute(decoder_expr), None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.defDeepSDF.engine()
@@ -428,6 +495,8 @@ class JointFitter:
             cond = torch.cat([self._prefix[None, :].expand(nb, -1), self.z_ex[obs_idx]], dim=1).contiguous()
             # correspondence search (iterative_root_finding.py:91-168): J0^-1 at the observed points, Broyden on the device
             obs = obs.to(torch.float32).contiguous()
+            if self.poses is not None:                                                   # q: the Broyden target and start
+                obs = self.poses.apply(obs, obs_idx)
             _, j0_inv = self.mlp.inverse_jacobian(obs, cond)
             p, _, valid, _ = self.mlp.broyden_search(obs, cond, obs, j0_inv, max_steps=15, cvg_thresh=1e-6, dvg_thresh=0.2,
                                                      early_exit=self.early_exit)
@@ -441,6 +510,8 @@ class JointFitter:
             _surface_grad(self.eng, pts, _quirk_period(self.dec, n_point), self.z_id, mask, clamp, self.terms, g_lat, g_pts,
                           stream)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                       # -J^-T g_x
+            if self.poses is not None:                                                   # d surface / d q = J^-T g_x = -u
+                _pose_step(self, obs, u, obs_idx, -float(lambdas.get('surface', 0.0)), lr, apply_update)
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # nb x (P + E); same points as j_inv
             # expression codes: surface route + reg_expr = mean_b ||z_ex[idx_b]||^2 (:137), dense Adam over all rows (:169)
             lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
@@ -497,10 +568,12 @@ class NpmIdentityFitter:
     """``inference_identity_space`` for a one-output ``DeepSDF`` (reference fitting.py:180-285) without an autograd graph.
     Per iteration: the surface term with its code gradient (``nphm_mlp_fit_surface_grad``, all sampled points as one query
     with condition ``z``), ``reg_global = ||z||^2`` (gradient ``2 z``; the reference sets reg_loc, reg_unobserved and
-    symm_dist to 0 for a DeepSDF), and Adam (``nphm_adam_step``)."""
+    symm_dist to 0 for a DeepSDF), and Adam (``nphm_adam_step``).  With ``poses`` the sampled rows are moved into the model
+    frame first and the surface call also returns the point gradient, from which the poses are fitted."""
 
-    def __init__(self, decoder, device):
+    def __init__(self, decoder, device, poses: ObservationPoses = None):
         self.device = device
+        self.poses, self.pose_lr0 = poses, None
         self.engine = decoder.engine()
         self.latent = torch.zeros(decoder.lat_dim, device=device, dtype=torch.float32)
         self.m = torch.zeros_like(self.latent)
@@ -510,18 +583,23 @@ class NpmIdentityFitter:
         self.t = 0
         self._ws = None
 
-    def step(self, points: torch.Tensor, lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
-        """One iteration on ``points`` (B x N x 3); with ``apply_update=False`` only ``grad`` and ``loss_terms`` are set."""
-        pts = points.reshape(1, -1, 3).to(dtype=torch.float32).contiguous()
+    def step(self, points: torch.Tensor, lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True,
+             obs_idx: torch.Tensor = None):
+        """One iteration on ``points`` (B x N x 3); with ``apply_update=False`` only ``grad`` and ``loss_terms`` (and the poses'
+        ``grad``) are set.  With poses, ``obs_idx`` (B, on the device) gives each row's observation."""
         if apply_update:
             self.t += 1
         lam_s, lam_g = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0))
         with torch.no_grad(), torch.cuda.device(self.device):
+            q = None if self.poses is None else self.poses.apply(points, obs_idx)
+            pts = (points if q is None else q).reshape(1, -1, 3).to(dtype=torch.float32).contiguous()
             if self._ws is None or self._ws[0] != pts.shape[1]:
                 self._ws = (pts.shape[1], self.engine.fit_workspace(1, pts.shape[1], self.device))
-            terms, g_cond, _ = self.engine.fit_surface_grad(pts, self.latent[None], None, clamp, want_xyz=False,
-                                                            workspace=self._ws[1])
+            terms, g_cond, g_xyz = self.engine.fit_surface_grad(pts, self.latent[None], None, clamp, want_xyz=q is not None,
+                                                                workspace=self._ws[1])
             self.loss_terms.copy_(terms)
+            if q is not None:
+                _pose_step(self, q, g_xyz.reshape(q.shape), obs_idx, lam_s, lr, apply_update)
             torch.add(lam_s * g_cond[0], self.latent, alpha=2.0 * lam_g, out=self.grad)
             if apply_update:
                 _native.check(_native.lib().nphm_adam_step(self.latent.data_ptr(), self.grad.data_ptr(), self.m.data_ptr(),
@@ -542,9 +620,11 @@ class NpmJointFitter:
     itself.  ``fixed_identity=True``: ``z_id`` (set by the caller) is held fixed, a step updates the expression codes alone (see
     :class:`JointFitter`)."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False):
+    def __init__(self, decoder, decoder_expr, num_observations: int, device, fixed_identity: bool = False,
+                 poses: ObservationPoses = None):
         self.device = device
         self.fixed_identity = fixed_identity
+        self.poses, self.pose_lr0 = poses, None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.engine()
         D = decoder.lat_dim
@@ -572,6 +652,8 @@ class NpmJointFitter:
         with torch.no_grad(), torch.cuda.device(dev):
             cond = torch.cat([self.z_id[None].expand(nb, D), self.z_ex[obs_idx]], dim=1).contiguous()
             obs = obs.to(torch.float32).contiguous()
+            if self.poses is not None:                                                   # q: the Broyden target and start
+                obs = self.poses.apply(obs, obs_idx)
             _, j0_inv = self.mlp.inverse_jacobian(obs, cond)
             p, _, valid, _ = self.mlp.broyden_search(obs, cond, obs, j0_inv, max_steps=15, cvg_thresh=1e-6, dvg_thresh=0.2,
                                                      early_exit=self.early_exit)
@@ -582,6 +664,8 @@ class NpmJointFitter:
                                                             workspace=self._ws[1])
             self.loss_terms.copy_(terms)
             u = -(j_inv * g_pts.reshape(nb, n_point, 3, 1)).sum(-2)                     # -J^-T g_x
+            if self.poses is not None:                                                   # d surface / d q = J^-T g_x = -u
+                _pose_step(self, obs, u, obs_idx, -lam_s, lr, apply_update)
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, obs_idx, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[obs_idx])
@@ -603,8 +687,10 @@ def inference_iterative_root_finding_joint(decoder,
                                            n_steps,
                                            schedule_cfg: Dict,
                                            step_scale=1,
-                                           lr_scale=1):
-    """Joint identity + expression fitting with Broyden correspondences (reference :14-177).
+                                           lr_scale=1,
+                                           poses: ObservationPoses = None):
+    """Joint identity + expression fitting with Broyden correspondences (reference :14-177).  ``poses``: the observations'
+    similarity transforms to the model frame, fitted with the codes as in :func:`inference_identity_space`.
 
     Fused ensemble + eval-mode DeformationNetwork in mode compress (the shipped configuration), glob_only or expr_only on
     CUDA: no autograd graph at all, see :class:`JointFitter`; the same for the NPM baseline (``DeepSDF`` decoders on CUDA), see :class:`NpmJointFitter`.
@@ -613,18 +699,20 @@ def inference_iterative_root_finding_joint(decoder,
     ``(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)``."""
     device = all_obs[0].device
     num_observations = len(all_obs)
+    check_poses(poses, num_observations, device)
     if not os.environ.get('NPHM_JOINT_AUTOGRAD'):
         fitter = None
         if _native_joint(decoder, decoder_expr, device):
-            fitter = JointFitter(decoder, decoder_expr, num_observations, device)
+            fitter = JointFitter(decoder, decoder_expr, num_observations, device, poses=poses)
         elif _native_npm_joint(decoder, decoder_expr, device):
-            fitter = NpmJointFitter(decoder, decoder_expr, num_observations, device)
+            fitter = NpmJointFitter(decoder, decoder_expr, num_observations, device, poses=poses)
         if fitter is not None:
             _run_joint(fitter, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
             lat_rep = fitter.z_ex.reshape(num_observations, 1, -1).clone().requires_grad_(True)
             lat_rep_shape = fitter.z_id.reshape(1, 1, -1).clone().requires_grad_(True)
             return lat_rep, lat_rep_shape, fitter.anchors
-    return _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
+    return _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale,
+                                     poses=poses)
 
 
 def _run_joint(fitter, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_scale):
@@ -638,7 +726,7 @@ def _run_joint(fitter, all_obs, lambdas, n_steps, schedule_cfg, step_scale, lr_s
 
 
 def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg, step_scale=1, lr_scale=1,
-                              lat_rep_shape=None, lat_rep_init=None):
+                              lat_rep_shape=None, lat_rep_init=None, poses=None):
     """The composite path of :func:`inference_iterative_root_finding_joint`: the correspondence search on the device where
     the search supports the decoder, everything else on autograd through the modules.  A given ``lat_rep_shape`` is held
     fixed (the path of :func:`inference_expression_space`): no identity optimizer, the anchors computed once, and ``z_ex``
@@ -659,6 +747,7 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
     opt_expr = optim.Adam(params=[lat_rep], lr=lr)
     opts = [opt_expr] if fixed else [optim.Adam(params=[lat_rep_shape], lr=lr), opt_expr]
     anchors = None
+    tangent = None if poses is None else _TangentPoses(poses)
     if fixed:
         with torch.no_grad():
             anchors = _current_anchors(decoder, lat_rep_shape, device)
@@ -675,6 +764,10 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
             anchors = _current_anchors(decoder, lat_rep_shape, device)
         obs, obs_idx = _sample_observations(all_obs)
         obs_idx = obs_idx.long().to(device)
+        q = None
+        if tangent is not None:                     # q: the Broyden target, d xc / d q = J^-1
+            q = tangent(obs, obs_idx)
+            obs = q.detach()
         nb, n_point, _ = obs.shape
         glob_cond = torch.cat([lat_rep_shape.repeat(nb, 1, 1), lat_rep[obs_idx, :, :]], dim=-1)
         has_local = hasattr(decoder, 'lat_dim_loc')
@@ -689,6 +782,8 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
         grad_inv = jac(decoder_expr, p_corresp, glob_cond.repeat(1, n_point, 1), _anchors).inverse()
         correction = preds_posed - preds_posed.detach()
         correction = torch.einsum('bnij,bnj->bni', -grad_inv.detach(), correction)
+        if q is not None:
+            correction = correction + torch.einsum('bnij,bnj->bni', grad_inv.detach(), q - q.detach())
         xc = p_corresp + correction
         if has_local and _fused_identity(decoder, grad_points=True) and xc.is_cuda:
             surface = _FusedSurfaceLoss.apply(xc, lat_rep_shape, search_result['valid_ids'],
@@ -711,6 +806,8 @@ def _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, 
         loss.backward()
         for o in opts:                      # the identity's optimizer first, as in the reference (:168-169)
             o.step()
+        if tangent is not None:
+            tangent.step(lr, j + 1)
     return lat_rep, lat_rep_shape, anchors
 
 
@@ -744,6 +841,26 @@ def _pad_scans(points: List[torch.Tensor]):
         m[p.shape[0]:] = 0
         masks.append(m)
     return torch.stack(padded).contiguous(), torch.stack(masks).contiguous()
+
+
+def _batch_poses(poses, scans, device):
+    """Checks one :class:`ObservationPoses` per scan (or ``poses=None``)."""
+    if poses is None:
+        return
+    if len(poses) != len(scans):
+        raise ValueError('%d poses for %d scans' % (len(poses), len(scans)))
+    for p, all_obs in zip(poses, scans):
+        check_poses(p, len(all_obs), device if device is not None else all_obs[0].device)
+
+
+def _fit_posed(fit, scans, gens, lambdas, poses):
+    """``fit(scans, gens, lambdas, shared)`` with the scans' poses in one shared table, written back afterwards."""
+    if poses is None:
+        return fit(scans, gens, lambdas)
+    shared = ObservationPoses.concat(poses)
+    out = fit(scans, gens, lambdas, shared)
+    shared.scatter(poses)
+    return out
 
 
 def _sequential(fit_one, scans, lambdas, *args):
@@ -782,13 +899,39 @@ class _QuirkPeriods:
         return self._dev
 
 
+def _posed_scans(poses, points: List[torch.Tensor], rows: torch.Tensor):
+    """A posed batched identity step's points: the scans' sampled rows (``points[k]``: nb x n_k x 3) padded to one row block
+    (S nb x n_point x 3, row r from observation ``rows[r]`` of the shared table) and moved into the model frame in one launch;
+    returns that block and each scan's rows of it (nb x n_k x 3), the points the unposed step takes."""
+    nb, n_point = points[0].shape[0], max(p.shape[1] for p in points)
+    q, _ = _pad_rows(points, n_point)
+    q = poses.apply(q, rows)
+    return q, [q[k * nb:(k + 1) * nb, :p.shape[1]] for k, p in enumerate(points)]
+
+
+def _rows_of_scans(g_pts: torch.Tensor, q: torch.Tensor, points: List[torch.Tensor]) -> torch.Tensor:
+    """The per-scan point gradients of a batched surface call (S x n x 3, scan k's nb n_k points first) laid out as the row
+    block ``q`` of :func:`_posed_scans`; the padding gets 0."""
+    nb, n_point = points[0].shape[0], q.shape[1]
+    if all(p.shape[1] == n_point for p in points):
+        return g_pts.reshape(q.shape)
+    out = torch.zeros_like(q)
+    for k, p in enumerate(points):
+        out[k * nb:(k + 1) * nb, :p.shape[1]] = g_pts[k, :nb * p.shape[1]].reshape(nb, p.shape[1], 3)
+    return out
+
+
 class BatchedIdentityFitter:
     """:class:`IdentityFitter` for S scans at once (``nphm_fit_identity_step_batched``): latents and Adam moments S x D on the
     device, one launch sequence per iteration for all scans.  In eval mode (``nphm_fit_identity_step_batched_quirk``) scan
-    k's period is the points per row of its sample, so each scan gets the quirk rows of its own single-scan call."""
+    k's period is the points per row of its sample, so each scan gets the quirk rows of its own single-scan call.  With
+    ``poses`` (one :class:`ObservationPoses` over all scans' observations, scan k's first at the sum of the earlier scans'
+    counts) the step runs as :class:`IdentityFitter`'s posed step does: ``nphm_fit_surface_grad_batched`` with the point
+    gradients, then ``nphm_fit_apply_gradient_batched``."""
 
-    def __init__(self, decoder: FastEnsembleDeepSDFMirrored, n_scans: int, device):
+    def __init__(self, decoder: FastEnsembleDeepSDFMirrored, n_scans: int, device, poses: ObservationPoses = None):
         self.decoder = decoder
+        self.poses, self.pose_lr0 = poses, None
         self._periods = _QuirkPeriods()
         self.device = device
         self.engine = decoder.engine()
@@ -800,9 +943,15 @@ class BatchedIdentityFitter:
         self.t = 0
         self._ws = None
 
-    def step(self, points: List[torch.Tensor], lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
-        """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ)."""
-        pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in points])
+    def step(self, points: List[torch.Tensor], lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True,
+             obs_idx: torch.Tensor = None):
+        """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ).  With poses
+        ``points[k]`` are scan k's sampled rows (nb x n_k x 3) and ``obs_idx`` (S nb, on the device) the rows' observations in
+        the shared table."""
+        scan_pts = points
+        if self.poses is not None:
+            q, scan_pts = _posed_scans(self.poses, points, obs_idx)
+        pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in scan_pts])
         S, n = pts.shape[0], pts.shape[1]
         eval_mode = not self.decoder.training
         if apply_update:
@@ -817,7 +966,27 @@ class BatchedIdentityFitter:
                                                        'nphm_fit_batch_workspace_bytes', self.device))
             ws = self._ws[1]
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            if eval_mode:
+            if self.poses is not None:
+                periods = self._periods([p.shape[-2] for p in points], self.device) if eval_mode else None
+                terms, g_lat, g_pts = torch.empty(S, 8, device=self.device), torch.empty_like(self.latents), torch.empty_like(pts)
+                if eval_mode:
+                    _native.check(lib.nphm_fit_surface_grad_batched_quirk(
+                        self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, periods.data_ptr(), self.latents.data_ptr(),
+                        float(clamp), terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
+                        'nphm_fit_surface_grad_batched_quirk')
+                else:
+                    _native.check(lib.nphm_fit_surface_grad_batched(
+                        self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, self.latents.data_ptr(), float(clamp),
+                        terms.data_ptr(), g_lat.data_ptr(), g_pts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
+                        'nphm_fit_surface_grad_batched')
+                stats = torch.stack([terms[:, 5], terms[:, 0] * terms[:, 5]], dim=1).nan_to_num_(0.0).contiguous()
+                _native.check(lib.nphm_fit_apply_gradient_batched(
+                    self.engine.handle, S, self.latents.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), ctypes.byref(fp),
+                    g_lat.data_ptr(), stats.data_ptr(), None, int(apply_update), self.loss_terms.data_ptr(), self.grad.data_ptr(),
+                    stream), 'nphm_fit_apply_gradient_batched')
+                _pose_step(self, q, _rows_of_scans(g_pts, q, points), obs_idx, float(lambdas.get('surface', 0.0)), lr,
+                           apply_update)
+            elif eval_mode:
                 periods = self._periods([p.shape[-2] if p.dim() > 1 else 1 for p in points], self.device)
                 _native.check(lib.nphm_fit_identity_step_batched_quirk(
                     self.engine.handle, pts.data_ptr(), _native._ptr(mask), S, n, periods.data_ptr(), self.latents.data_ptr(),
@@ -842,51 +1011,66 @@ def inference_identity_space_batched(decoder,
                                      n_steps,
                                      schedule_cfg: Dict,
                                      step_scale=1,
-                                     lr_scale=1):
+                                     lr_scale=1,
+                                     poses: List[ObservationPoses] = None):
     """:func:`inference_identity_space` for several scans (``scans[k]``: the observations of scan k) at once.  Returns
     ``[(lat_rep_shape, anchors)]`` in scan order - what the single-scan function gives when called on each scan in turn, each
     call with a fresh copy of ``lambdas``; the global CPU generator and ``lambdas`` end as those calls leave them.  Runs all
     scans in one launch sequence per iteration for the fused ensemble on CUDA (:class:`BatchedIdentityFitter`, training or eval
     mode, see :func:`_fused_identity`)
     and for the NPM baseline's ``DeepSDF`` on CUDA (:class:`BatchedNpmIdentityFitter`); any other configuration calls the
-    single-scan function scan by scan."""
+    single-scan function scan by scan.  ``poses``: one :class:`ObservationPoses` per scan, fitted in place as the single-scan
+    function fits its ``poses``; all must share rates, ``fit_scale`` and ``fit`` (they update as one table)."""
     if not scans:
         return []
-    fit = _identity_batch_fit(decoder, scans, n_steps, schedule_cfg, step_scale, lr_scale)
+    _batch_poses(poses, scans, _scans_device(scans))
+    fit = _identity_batch_fit(decoder, scans, n_steps, schedule_cfg, step_scale, lr_scale, posed=poses is not None)
     if fit is None:
-        return _sequential(lambda obs, lam: inference_identity_space(decoder, obs, lam, n_steps, schedule_cfg, step_scale,
-                                                                     lr_scale), scans, lambdas)
-    return fit(scans, _sampling_plan(scans, int(n_steps * step_scale)), lambdas)
+        return _sequential(lambda e, lam: inference_identity_space(decoder, e[0], lam, n_steps, schedule_cfg, step_scale,
+                                                                   lr_scale, poses=e[1]),
+                           list(zip(scans, poses or [None] * len(scans))), lambdas)
+    return _fit_posed(fit, scans, _sampling_plan(scans, int(n_steps * step_scale)), lambdas, poses)
 
 
-def _identity_batch_fit(decoder, scans, n_steps, schedule_cfg, step_scale, lr_scale):
-    """``fit(scans, gens, lambdas)``: the scan-batched identity fit with scan k drawing from ``gens[k]``, when a batched
-    fitter takes this decoder on the scans' device; None when the scans are fitted one by one."""
+def _identity_batch_fit(decoder, scans, n_steps, schedule_cfg, step_scale, lr_scale, posed: bool = False):
+    """``fit(scans, gens, lambdas[, poses])``: the scan-batched identity fit with scan k drawing from ``gens[k]``, when a
+    batched fitter takes this decoder on the scans' device; None when the scans are fitted one by one."""
     device = _scans_device(scans)
     npm = device is not None and device.type == 'cuda' and _native_npm_decoder(decoder, 1)
-    if not npm and (device is None or device.type != 'cuda' or not (_fused_identity(decoder) and _tc_ensemble(decoder))):
+    if not npm and (device is None or device.type != 'cuda' or not (_fused_identity(decoder, posed) and _tc_ensemble(decoder))):
         return None
-    return lambda chunk, gens, lambdas: _fit_identity_batch(decoder, chunk, gens, lambdas, n_steps, schedule_cfg, step_scale,
-                                                            lr_scale, device, npm)
+    return lambda chunk, gens, lambdas, poses=None: _fit_identity_batch(decoder, chunk, gens, lambdas, n_steps, schedule_cfg,
+                                                                        step_scale, lr_scale, device, npm, poses)
 
 
-def _fit_identity_batch(decoder, scans, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale, device, npm):
+def _sample_batch(scans, gens, offsets, device):
+    """One iteration's samples of every scan, and (with poses, ``offsets`` not None) the rows' observations in the shared
+    table on the device."""
+    sample = [_sample_observations(all_obs, g) for all_obs, g in zip(scans, gens)]
+    rows = None
+    if offsets is not None:
+        rows = torch.cat([i + o for (_, i), o in zip(sample, offsets)]).to(device=device, dtype=torch.int32)
+    return [o for o, _ in sample], rows
+
+
+def _fit_identity_batch(decoder, scans, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale, device, npm, poses=None):
     n_iters = int(n_steps * step_scale)
     lr = 0.01 * lr_scale
+    offsets = None if poses is None else [sum(len(s) for s in scans[:k]) for k in range(len(scans))]
     if npm:
-        fitter = BatchedNpmIdentityFitter(decoder, len(scans), device)
+        fitter = BatchedNpmIdentityFitter(decoder, len(scans), device, poses)
         for j in range(n_iters):
             lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
-            obs = [_sample_observations(all_obs, g)[0] for all_obs, g in zip(scans, gens)]
-            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+            obs, rows = _sample_batch(scans, gens, offsets, device)
+            fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr, obs_idx=rows)
         return [(fitter.latents[k].reshape(1, 1, -1).clone().requires_grad_(True), None) for k in range(len(scans))]
-    fitter = BatchedIdentityFitter(decoder, len(scans), device)
+    fitter = BatchedIdentityFitter(decoder, len(scans), device, poses)
     z_prev = fitter.latents.clone()
     for j in range(n_iters):
         lr = _apply_schedule(j, step_scale, schedule_cfg, lambdas, lr)
-        obs = [_sample_observations(all_obs, g)[0] for all_obs, g in zip(scans, gens)]
+        obs, rows = _sample_batch(scans, gens, offsets, device)
         z_prev.copy_(fitter.latents)
-        fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr)
+        fitter.step(obs, lambdas, _clamp_for_iteration(j, step_scale), lr, obs_idx=rows)
     out = []
     with torch.no_grad():
         for k in range(len(scans)):
@@ -931,9 +1115,11 @@ class BatchedJointFitter:
     (``nphm_fit_surface_grad_batched_quirk``).  ``fixed_identity=True``: the S identity codes (set by the caller) are held
     fixed, as in :class:`JointFitter`."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False):
+    def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False,
+                 poses: ObservationPoses = None):
         self.dec, self.dfn, self.device = decoder, decoder_expr, device
         self.fixed_identity = fixed_identity
+        self.poses, self.pose_lr0 = poses, None
         self.route, self._prefix = _IdentityRoute(decoder_expr), None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.defDeepSDF.engine()
@@ -973,6 +1159,8 @@ class BatchedJointFitter:
             # mode in front of the row, so that its last point stays last
             front = not self.dec.training
             obs_all, keep = _pad_rows(obs, n_point, front)                                # 5 S x n_point x 3
+            if self.poses is not None:                                                   # q: the Broyden target and start
+                obs_all = self.poses.apply(obs_all, rows)
             _, j0_inv = self.mlp.inverse_jacobian(obs_all, cond)
             p, _, valid, _ = self.mlp.broyden_search(obs_all, cond, obs_all, j0_inv, max_steps=15, cvg_thresh=1e-6,
                                                      dvg_thresh=0.2, early_exit=self.early_exit)
@@ -1003,6 +1191,8 @@ class BatchedJointFitter:
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)     # 5 S x (P + E)
             lam_s, lam_e = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_expr', 0.0))
+            if self.poses is not None:                                                   # d surface / d q = J^-T g_x = -u
+                _pose_step(self, obs_all, u, rows, -lam_s, lr, apply_update)
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, rows, lam_s * g_cond[:, P:] + (2.0 * lam_e / nb) * self.z_ex[rows])
             if self.fixed_identity:
@@ -1032,10 +1222,12 @@ class BatchedNpmIdentityFitter:
     """:class:`NpmIdentityFitter` for S scans at once: latents, Adam moments and ``grad`` S x D, ``loss_terms`` S x 8.  Per
     iteration one surface call over all scans (``nphm_mlp_fit_surface_grad_batched``, scan k = query k with condition z_k and
     its own loss), ``grad = lambda_s g_cond + 2 lambda_g z`` and one ``nphm_adam_step`` over the S D elements (Adam is
-    element-wise and the scans share the step and lr)."""
+    element-wise and the scans share the step and lr).  With ``poses`` (over all scans' observations, as for
+    :class:`BatchedIdentityFitter`) the surface call also returns the point gradients, from which the poses are fitted."""
 
-    def __init__(self, decoder, n_scans: int, device):
+    def __init__(self, decoder, n_scans: int, device, poses: ObservationPoses = None):
         self.device = device
+        self.poses, self.pose_lr0 = poses, None
         self.engine = decoder.engine()
         self.latents = torch.zeros(n_scans, decoder.lat_dim, device=device, dtype=torch.float32)
         self.m = torch.zeros_like(self.latents)
@@ -1045,19 +1237,26 @@ class BatchedNpmIdentityFitter:
         self.t = 0
         self._ws = None
 
-    def step(self, points: List[torch.Tensor], lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True):
-        """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ)."""
-        pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in points])
-        S, n = pts.shape[0], pts.shape[1]
+    def step(self, points: List[torch.Tensor], lambdas: Dict[str, float], clamp: float, lr: float, apply_update: bool = True,
+             obs_idx: torch.Tensor = None):
+        """One iteration; ``points[k]`` are scan k's sampled points (any shape ending in 3, lengths may differ); with poses as
+        in :meth:`BatchedIdentityFitter.step`."""
         if apply_update:
             self.t += 1
         lam_s, lam_g = float(lambdas.get('surface', 0.0)), float(lambdas.get('reg_global', 0.0))
         with torch.no_grad(), torch.cuda.device(self.device):
+            scan_pts = points
+            if self.poses is not None:
+                q, scan_pts = _posed_scans(self.poses, points, obs_idx)
+            pts, mask = _pad_scans([p.reshape(-1, 3).to(dtype=torch.float32) for p in scan_pts])
+            S, n = pts.shape[0], pts.shape[1]
             if self._ws is None or self._ws[0] != (S, n):
                 self._ws = ((S, n), self.engine.fit_workspace(S, n, self.device))
-            terms, g_cond, _ = self.engine.fit_surface_grad_batched(pts, self.latents, mask, clamp, want_xyz=False,
-                                                                    workspace=self._ws[1])
+            terms, g_cond, g_xyz = self.engine.fit_surface_grad_batched(pts, self.latents, mask, clamp,
+                                                                        want_xyz=self.poses is not None, workspace=self._ws[1])
             self.loss_terms.copy_(terms)
+            if self.poses is not None:
+                _pose_step(self, q, _rows_of_scans(g_xyz, q, points), obs_idx, lam_s, lr, apply_update)
             torch.add(lam_s * g_cond, self.latents, alpha=2.0 * lam_g, out=self.grad)
             if apply_update:
                 _native.check(_native.lib().nphm_adam_step(self.latents.data_ptr(), self.grad.data_ptr(), self.m.data_ptr(),
@@ -1079,9 +1278,11 @@ class BatchedNpmJointFitter:
     subjects per batch; the caller chooses S, nothing is split.  ``fixed_identity=True``: the identity codes (set by the caller)
     are held fixed, as in :class:`JointFitter`."""
 
-    def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False):
+    def __init__(self, decoder, decoder_expr, num_observations: List[int], device, fixed_identity: bool = False,
+                 poses: ObservationPoses = None):
         self.device = device
         self.fixed_identity = fixed_identity
+        self.poses, self.pose_lr0 = poses, None
         self.eng = decoder.engine()
         self.mlp = decoder_expr.engine()
         D, S = decoder.lat_dim, len(num_observations)
@@ -1119,6 +1320,8 @@ class BatchedNpmJointFitter:
                     keep[k, :, o.shape[1]:] = False
             obs_all = torch.cat([o if o.shape[1] == n_point else torch.cat([o, o[:, :1].expand(nb, n_point - o.shape[1], 3)], dim=1)
                                  for o in obs]).to(torch.float32).contiguous()                 # 5 S x n_point x 3
+            if self.poses is not None:                                                   # q: the Broyden target and start
+                obs_all = self.poses.apply(obs_all, rows)
             _, j0_inv = self.mlp.inverse_jacobian(obs_all, cond)
             p, _, valid, _ = self.mlp.broyden_search(obs_all, cond, obs_all, j0_inv, max_steps=15, cvg_thresh=1e-6,
                                                      dvg_thresh=0.2, early_exit=self.early_exit)
@@ -1132,6 +1335,8 @@ class BatchedNpmJointFitter:
                                                                     workspace=self._ws[1])
             self.loss_terms.copy_(terms)
             u = -(j_inv * g_pts.reshape(S * nb, n_point, 3, 1)).sum(-2)                  # -J^-T g_x
+            if self.poses is not None:                                                   # d surface / d q = J^-T g_x = -u
+                _pose_step(self, obs_all, u, rows, -lam_s, lr, apply_update)
             g_cond, _ = self.mlp.backward_inputs(p, cond, u, reuse_value_pass=True)
             g_zex = torch.zeros_like(self.z_ex)
             g_zex.index_add_(0, rows, lam_s * g_cond[:, D:] + (2.0 * lam_e / nb) * self.z_ex[rows])
@@ -1155,22 +1360,25 @@ def inference_iterative_root_finding_joint_batched(decoder,
                                                    n_steps,
                                                    schedule_cfg: Dict,
                                                    step_scale=1,
-                                                   lr_scale=1):
+                                                   lr_scale=1,
+                                                   poses: List[ObservationPoses] = None):
     """:func:`inference_iterative_root_finding_joint` for several subjects (``subjects[k]``: the observations of subject k) at
     once.  Returns ``[(lat_rep (n_obs,1,E), lat_rep_shape (1,1,D), anchors)]`` in subject order, under the contract of
     :func:`inference_identity_space_batched`.  The ensemble configurations of :func:`_native_joint` run all subjects in one
     launch sequence per iteration (:class:`BatchedJointFitter`), and so does the NPM baseline (see :func:`_native_npm_joint`,
     :class:`BatchedNpmJointFitter`); anything else - CPU, other decoders or deformation modes, ``NPHM_JOINT_AUTOGRAD=1`` -
     calls the single-subject function subject by subject.  Memory grows linearly with the number of subjects; all subjects
-    must fit on the device at once (nothing is split into smaller batches)."""
+    must fit on the device at once (nothing is split into smaller batches).  ``poses``: one :class:`ObservationPoses` per
+    subject, fitted in place; all must share rates, ``fit_scale`` and ``fit`` (they update as one table)."""
     if not subjects:
         return []
+    _batch_poses(poses, subjects, _scans_device(subjects))
     fit = _joint_batch_fit(decoder, decoder_expr, subjects, n_steps, schedule_cfg, step_scale, lr_scale)
     if fit is None:
-        return _sequential(lambda obs, lam: inference_iterative_root_finding_joint(decoder, decoder_expr, obs, lam, n_steps,
-                                                                                   schedule_cfg, step_scale, lr_scale),
-                           subjects, lambdas)
-    return fit(subjects, _sampling_plan(subjects, int(n_steps * step_scale)), lambdas)
+        return _sequential(lambda e, lam: inference_iterative_root_finding_joint(decoder, decoder_expr, e[0], lam, n_steps,
+                                                                                 schedule_cfg, step_scale, lr_scale, poses=e[1]),
+                           list(zip(subjects, poses or [None] * len(subjects))), lambdas)
+    return _fit_posed(fit, subjects, _sampling_plan(subjects, int(n_steps * step_scale)), lambdas, poses)
 
 
 def _joint_batch_fit(decoder, decoder_expr, subjects, n_steps, schedule_cfg, step_scale, lr_scale):
@@ -1185,8 +1393,8 @@ def _joint_batch_fit(decoder, decoder_expr, subjects, n_steps, schedule_cfg, ste
             batched = BatchedJointFitter
     if batched is None:
         return None
-    return lambda chunk, gens, lambdas: _fit_joint_batch(batched, decoder, decoder_expr, chunk, gens, lambdas, n_steps,
-                                                         schedule_cfg, step_scale, lr_scale, device)
+    return lambda chunk, gens, lambdas, poses=None: _fit_joint_batch(batched, decoder, decoder_expr, chunk, gens, lambdas,
+                                                                     n_steps, schedule_cfg, step_scale, lr_scale, device, poses)
 
 
 def _run_joint_batch(fitter, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale):
@@ -1201,8 +1409,8 @@ def _run_joint_batch(fitter, subjects, gens, lambdas, n_steps, schedule_cfg, ste
 
 
 def _fit_joint_batch(batched, decoder, decoder_expr, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale,
-                     device):
-    fitter = batched(decoder, decoder_expr, [len(s) for s in subjects], device)
+                     device, poses=None):
+    fitter = batched(decoder, decoder_expr, [len(s) for s in subjects], device, poses=poses)
     _run_joint_batch(fitter, subjects, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
     out = []
     for k, (off, cnt) in enumerate(zip(fitter.offsets, fitter.num_observations)):
@@ -1240,7 +1448,8 @@ def inference_expression_space(decoder,
                                schedule_cfg: Dict,
                                step_scale=1,
                                lr_scale=1,
-                               lat_reps_expr_init=None):
+                               lat_reps_expr_init=None,
+                               poses: ObservationPoses = None):
     """Fit expression codes to the observations ``all_obs`` of a subject whose identity code ``lat_rep_shape`` (1,1,D) is
     known, e.g. from :func:`inference_identity_space` on a neutral scan.  The loop is the reference's joint loop (:14-177) with
     ``lat_rep_shape`` held fixed: the same 5-of-K observation draws from torch's global CPU generator, lr / lambda / clamp
@@ -1251,17 +1460,19 @@ def inference_expression_space(decoder,
 
     Runs natively (:class:`JointFitter` / :class:`NpmJointFitter` with ``fixed_identity=True``) for the configurations of
     :func:`inference_iterative_root_finding_joint`; anything else - CPU, other decoders, ``NPHM_JOINT_AUTOGRAD=1`` - runs the
-    same loop on autograd."""
+    same loop on autograd.  ``poses``: each observation's similarity transform to the model frame, fitted with the
+    expression codes as in :func:`inference_identity_space` (e.g. the frames of a capture in which the head moves)."""
     device = all_obs[0].device
     K = len(all_obs)
+    check_poses(poses, K, device)
     z_id = _identity_row(decoder, lat_rep_shape)
     cls = _expression_fitter(decoder, decoder_expr, device, batched=False)
     if cls is None:
         lat_rep, _, anchors = _inference_joint_autograd(decoder, decoder_expr, all_obs, lambdas, n_steps, schedule_cfg,
                                                         step_scale, lr_scale, lat_rep_shape=z_id,
-                                                        lat_rep_init=lat_reps_expr_init)
+                                                        lat_rep_init=lat_reps_expr_init, poses=poses)
         return lat_rep, anchors
-    fitter = cls(decoder, decoder_expr, K, device, fixed_identity=True)
+    fitter = cls(decoder, decoder_expr, K, device, fixed_identity=True, poses=poses)
     fitter.z_id.copy_(z_id)
     if lat_reps_expr_init is not None:
         fitter.z_ex.copy_(lat_reps_expr_init.detach().reshape(fitter.z_ex.shape))
@@ -1276,7 +1487,8 @@ def inference_expression_space_batched(decoder,
                                        n_steps,
                                        schedule_cfg: Dict,
                                        step_scale=1,
-                                       lr_scale=1):
+                                       lr_scale=1,
+                                       poses: List[ObservationPoses] = None):
     """:func:`inference_expression_space` for several subjects at once.  ``subjects[k]`` is ``(lat_rep_shape, all_obs)`` or
     ``(lat_rep_shape, all_obs, lat_reps_expr_init)``; to track the T frames of one person, pass T single-observation entries
     that share one ``lat_rep_shape``.  Returns ``[(lat_reps_expr, anchors)]`` in subject order under the contract of
@@ -1284,24 +1496,29 @@ def inference_expression_space_batched(decoder,
     call with a fresh copy of ``lambdas``, and the global CPU generator and ``lambdas`` end as those calls leave them.  The
     configurations of :func:`inference_iterative_root_finding_joint_batched` run all subjects in one launch sequence per
     iteration (:class:`BatchedJointFitter` / :class:`BatchedNpmJointFitter` with ``fixed_identity=True``); anything else calls
-    the single-subject function subject by subject."""
+    the single-subject function subject by subject.  ``poses``: one :class:`ObservationPoses` per entry, fitted in place; all
+    must share rates, ``fit_scale`` and ``fit`` (they update as one table)."""
     if not subjects:
         return []
     entries = [(e[0], e[1], e[2] if len(e) > 2 else None) for e in subjects]
     scans = [e[1] for e in entries]
     device = _scans_device(scans)
+    _batch_poses(poses, scans, device)
     cls = _expression_fitter(decoder, decoder_expr, device, batched=True)
     if cls is None:
         return _sequential(lambda e, lam: inference_expression_space(decoder, decoder_expr, e[0], e[1], lam, n_steps,
-                                                                     schedule_cfg, step_scale, lr_scale, e[2]),
-                           entries, lambdas)
+                                                                     schedule_cfg, step_scale, lr_scale, e[2], poses=e[3]),
+                           [e + (p,) for e, p in zip(entries, poses or [None] * len(entries))], lambdas)
     gens = _sampling_plan(scans, int(n_steps * step_scale))
-    fitter = cls(decoder, decoder_expr, [len(o) for o in scans], device, fixed_identity=True)
+    shared = None if poses is None else ObservationPoses.concat(poses)
+    fitter = cls(decoder, decoder_expr, [len(o) for o in scans], device, fixed_identity=True, poses=shared)
     fitter.z_id.copy_(torch.stack([_identity_row(decoder, e[0]) for e in entries]))
     for (_, _, init), off, cnt in zip(entries, fitter.offsets, fitter.num_observations):
         if init is not None:
             fitter.z_ex[off:off + cnt].copy_(init.detach().reshape(cnt, -1))
     _run_joint_batch(fitter, scans, gens, lambdas, n_steps, schedule_cfg, step_scale, lr_scale)
+    if shared is not None:
+        shared.scatter(poses)
     return [(fitter.z_ex[off:off + cnt].reshape(cnt, 1, -1).clone().requires_grad_(True),
              None if fitter.anchors is None else fitter.anchors[k:k + 1].clone())
             for k, (off, cnt) in enumerate(zip(fitter.offsets, fitter.num_observations))]
