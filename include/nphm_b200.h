@@ -792,6 +792,37 @@ int nphm_pose_grad(const float *q_dev, const float *grad_q_dev, const int *row_o
 int nphm_pose_adam(double *table_dev, double *adam_m_dev, double *adam_v_dev, const double *grad_dev, int n_obs, double lr_rot,
                    double lr_trans, double lr_scale, int fit_scale, int step, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Global registration against an SDF grid (csrc/register.cu, DESIGN.md §4.25).  The grid has res points per axis from mini with
+ * spacing h (get_logits' layout: x slowest, z fastest, end points included).  Both enqueue on the stream and never synchronise.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    int res;              /* grid points per axis, >= 2 */
+    float mini[3];        /* the grid's first point */
+    float h[3];           /* the spacing per axis (fp32, as prepare used it) */
+    int n_obs;            /* observations */
+    int n_use;            /* points per observation this stage uses: the first min(count_o, n_use) */
+    int n_hyp;            /* hypotheses (rows of the table) */
+    int n_iter;           /* Gauss-Newton iterations, followed by one scoring pass */
+    int fit_scale;        /* 1: similarity (7 parameters), 0: rigid (sigma held) */
+    double tau0, tau1;    /* truncation at the first and the last iteration (model units), geometric in between; the score's */
+    double damping;       /* the step solves (A + damping diag(A)) delta = -b */
+} nphm_register_params;
+
+/* field_dev [res^3] float4 = (sdf, d/dx, d/dy, d/dz) of volume_dev [res^3] fp32: central differences (v+ - v-) / (2 h) in fp32,
+ * one-sided (v1 - v0) / h at the faces, each operation rounded once */
+int nphm_register_prepare(const float *volume_dev, int res, float hx, float hy, float hz, void *field_dev, void *stream);
+/* Gauss-Newton on every hypothesis: row k of table_dev (n_hyp x 13 fp64, ObservationPoses' layout) is a pose of observation
+ * hyp_obs_dev[k], whose points are points_dev[offsets_dev[o] ..] (fp32 x 3, counts_dev[o] of them; unit_dev[o] its reference
+ * scale).  Residual r = sdf(q) unit / exp(sigma), truncated at tau (weight 0 beyond it and outside the grid); sigma stays within
+ * log 2 / 8 of sigma_seed_dev[k].  On return table_dev holds the final poses, score_dev [n_hyp] fp64 the mean of min(r^2, tau1^2)
+ * over the points (tau1^2 outside the grid) and inliers_dev [n_hyp] the count with |r| < tau1.  max_points: the largest
+ * min(count_o, n_use), which sizes the shared memory.  Bitwise repeatable, and a row's result does not depend on the others. */
+int nphm_register_search(const nphm_register_params *p, const void *field_dev, const float *points_dev,
+                         const long long *offsets_dev, const int *counts_dev, const double *unit_dev, double *table_dev,
+                         const double *sigma_seed_dev, const int *hyp_obs_dev, int max_points, double *score_dev, int *inliers_dev,
+                         void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -62,6 +62,7 @@ EXPORTED_SYMBOLS = (
     'nphm_trace_workspace_bytes', 'nphm_trace_begin', 'nphm_trace_compact', 'nphm_trace_counts', 'nphm_trace_gather',
     'nphm_trace_advance', 'nphm_trace_points', 'nphm_trace_finish',
     'nphm_pose_apply', 'nphm_pose_grad', 'nphm_pose_adam',
+    'nphm_register_prepare', 'nphm_register_search',
 )
 
 
@@ -127,6 +128,11 @@ class TraceParams(Structure):
     _fields_ = [('n_heads', c_int), ('n_rays', c_longlong), ('box_min', c_double * 3), ('box_max', c_double * 3),
                 ('scale', c_double), ('znear', c_double), ('zfar', c_double), ('step_factor', c_float), ('min_step', c_float),
                 ('hit_eps', c_float), ('max_steps', c_int)]
+
+
+class RegisterParams(Structure):
+    _fields_ = [('res', c_int), ('mini', c_float * 3), ('h', c_float * 3), ('n_obs', c_int), ('n_use', c_int), ('n_hyp', c_int),
+                ('n_iter', c_int), ('fit_scale', c_int), ('tau0', c_double), ('tau1', c_double), ('damping', c_double)]
 
 
 class FitParams(Structure):
@@ -357,6 +363,9 @@ def lib() -> ctypes.CDLL:
                                  c_void_p]
     L.nphm_pose_adam.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_int, c_int,
                                  c_void_p]
+    L.nphm_register_prepare.argtypes = [c_void_p, c_int, c_float, c_float, c_float, c_void_p, c_void_p]
+    L.nphm_register_search.argtypes = [POINTER(RegisterParams), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
     for name in EXPORTED_SYMBOLS:                      # fail at load time, not at first use, if a symbol is missing
         getattr(L, name)
     _lib = L

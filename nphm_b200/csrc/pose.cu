@@ -10,16 +10,13 @@
 // float64 restatement in the same order gives the same bits, and the identity transform maps every point to itself.
 #include <cmath>
 #include "common.cuh"
+#include "pose_math.cuh"
 
 namespace nphm {
 namespace pose {
 
 constexpr int kThreads = 256;
 constexpr int kStride = 13;     // R (9), t (3), sigma
-
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
 
 __global__ void __launch_bounds__(kThreads) apply_kernel(const float *__restrict__ pts, const int *__restrict__ row_obs,
                                                          long long n_rows, long long n_point, const double *__restrict__ table,
@@ -93,29 +90,6 @@ __global__ void __launch_bounds__(kThreads) grad_kernel(const float *__restrict_
     }
 }
 
-// Exp(w): I + A K + B K^2 (Rodrigues), K the cross-product matrix of w; the series near 0 so that Exp(0) is exactly I.
-__device__ void rodrigues(const double w[3], double E[9])
-{
-    const double th2 = add(add(mul(w[0], w[0]), mul(w[1], w[1])), mul(w[2], w[2]));
-    double A, B;
-    if (th2 < 1e-16) {
-        A = sub(1.0, th2 / 6.0);
-        B = sub(0.5, th2 / 24.0);
-    } else {
-        const double th = sqrt(th2);
-        A = sin(th) / th;
-        B = sub(1.0, cos(th)) / th2;
-    }
-    const double K[9] = {0.0, -w[2], w[1], w[2], 0.0, -w[0], -w[1], w[0], 0.0};
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const double k2 = add(add(mul(K[3 * r], K[c]), mul(K[3 * r + 1], K[3 + c])), mul(K[3 * r + 2], K[6 + c]));
-            E[3 * r + c] = add(add(r == c ? 1.0 : 0.0, mul(A, K[3 * r + c])), mul(B, k2));
-        }
-}
-
 __global__ void adam_kernel(double *__restrict__ table, double *__restrict__ m, double *__restrict__ v,
                             const double *__restrict__ grad, int n_obs, double lr_rot, double lr_trans, double lr_scale,
                             int fit_scale, double bc1, double bc2_sqrt)
@@ -137,20 +111,8 @@ __global__ void adam_kernel(double *__restrict__ table, double *__restrict__ m, 
     double E[9], R[9];
     rodrigues(d, E);
 #pragma unroll
-    for (int r = 0; r < 3; ++r)
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-            R[3 * r + c] = add(add(mul(E[3 * r], T[c]), mul(E[3 * r + 1], T[3 + c])), mul(E[3 * r + 2], T[6 + c]));
-    // re-orthonormalise (Gram-Schmidt on the rows, the third row the cross product: det +1)
-    double n0 = sqrt(add(add(mul(R[0], R[0]), mul(R[1], R[1])), mul(R[2], R[2])));
-    R[0] /= n0; R[1] /= n0; R[2] /= n0;
-    const double dp = add(add(mul(R[0], R[3]), mul(R[1], R[4])), mul(R[2], R[5]));
-    R[3] = sub(R[3], mul(dp, R[0])); R[4] = sub(R[4], mul(dp, R[1])); R[5] = sub(R[5], mul(dp, R[2]));
-    const double n1 = sqrt(add(add(mul(R[3], R[3]), mul(R[4], R[4])), mul(R[5], R[5])));
-    R[3] /= n1; R[4] /= n1; R[5] /= n1;
-    R[6] = sub(mul(R[1], R[5]), mul(R[2], R[4]));
-    R[7] = sub(mul(R[2], R[3]), mul(R[0], R[5]));
-    R[8] = sub(mul(R[0], R[4]), mul(R[1], R[3]));
+    for (int k = 0; k < 9; ++k) R[k] = T[k];
+    rotate_left_orthonormal(E, R);
 #pragma unroll
     for (int k = 0; k < 9; ++k) T[k] = R[k];
     T[9] = add(T[9], d[3]); T[10] = add(T[10], d[4]); T[11] = add(T[11], d[5]);

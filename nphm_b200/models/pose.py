@@ -13,7 +13,8 @@ of observation ``o`` (``lam_s = lambdas['surface']``)::
 for the left perturbation ``R <- Exp(omega) R``, and Adam on ``(omega, t, sigma)`` updates the pose in the same step as the
 codes.  On CUDA the three steps are the kernels of csrc/pose.cu; the functions ``*_f64`` below restate them in torch float64
 and are what CPU fits and the tests use.  The fit is local: it corrects errors of degrees and centimetres, not arbitrary
-orientations - initialise far-off poses (landmarks, ICP) before fitting.
+orientations - initialise far-off poses with :func:`nphm_b200.models.registration.register_scans` (DESIGN.md §4.25) before
+fitting.
 """
 from __future__ import annotations
 
